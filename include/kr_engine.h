@@ -384,7 +384,10 @@ typedef struct kr_results_view {
    * complete and bit-identical to what a full pass would return.  n_changed / changed_clusters name the records that were
    * recomputed: n_changed == n_clusters and changed_clusters == NULL after a full pass.  Anything the resident state cannot
    * absorb (a changed table key or CSR offset, wholesale column commits, different flags, an overflowing bucket) silently
-   * takes the full pass.  KR_NO_INCR=1 in the environment turns the incremental path off. */
+   * takes the full pass.  Snapshots with multi-host worker groups (numOfHosts > 1) keep incremental epochs, and so does an edit of
+   * numOfHosts.  Every pass is a full one on the sort pipeline — no resident state — while the caller fetches the full pod lists
+   * (fetch_pod_lists = 1), while some RayCluster lists more than 256 pods or has more than 32 worker groups, or when
+   * KR_NO_INCR=1 is set in the environment. */
   uint32_t n_changed;
   const uint32_t          *changed_clusters; /* [n_changed] cluster rows, unordered */
 } kr_results_view;

@@ -17,8 +17,9 @@
 //              replica indices from the registers and reserves its places in the action list / create arena with one returning
 //              atomic, so nothing follows it: no scan, no creates kernel, no compaction kernel.
 // A bucket stride too small for some cluster voids the attempt (the engine widens the stride or falls back to the sort
-// pipeline); clusters with multi-host groups or more than KR_SMEM_GROUPS worker groups are routed to the sort pipeline by the
-// host before the pass.
+// pipeline); snapshots with a RayCluster of more than KR_SMEM_GROUPS worker groups are routed to the sort pipeline by the host
+// before the pass.  Multi-host worker groups (numOfHosts > 1 under the RayMultiHostIndexing gate) are decided here too, by the
+// k_decide2<K, kInc, true> instantiations the engine launches only when the snapshot has such a group (decide_multihost2).
 #pragma once
 
 #include "kr_decide.cuh"
@@ -180,16 +181,138 @@ struct Decide2Args {
               // 2: only the clusters an incremental epoch marked dirty (kr_incr.cuh) — digests resident, places reused while they suffice
 };
 
+// reconcileMultiHostWorkerGroup (raycluster_controller.go:963-1125) for worker group `gi` of the warp's RayCluster, from the
+// registers of k_decide2 — the decisions of decide_multihost (kr_decide.cuh), which the sort pipeline takes, bit for bit.
+// A replica is the set of the group's pods sharing a ray.io/worker-group-replica-name; it is identified by its smallest pod index,
+// so ascending identity is "first appearance in List order" (the stand-in for the reference's Go-map iteration) although the
+// bucket is in arrival order.  Replicas are peeled off in that order (a warp minimum over the unassigned members, then a compare
+// of its name against the K registers): O(replicas x K) warp steps.  The replica-name id is not in the 16-byte bucket record; it
+// is read from the pod column here, for the group's members only (an incremental epoch patches that column before this kernel).
+// The group's per-pod actions go straight into act[]; mh_head gets bit k for every pod that is the first pod of a healthy
+// replica (its replica index is "in use" for the creates); s_rep (>= 32*K words of the warp's shared memory) holds the
+// per-replica flags.  Returns the KR_ERR_* kind (0 = nil).
+template <int K>
+__device__ __forceinline__ int decide_multihost2(const SnapDev &s, uint32_t gi, int32_t expected, int32_t H, bool delete_allowed, uint32_t wtd_cnt,
+                                                 const uint32_t (&pidx)[K], const uint32_t (&pw)[K], uint32_t (&act)[K], uint32_t &mh_head,
+                                                 uint32_t *s_rep, kr_group_result &gr, int32_t &err_arg, uint32_t lane) {
+  const uint32_t lt = lanemask_lt();
+  uint32_t rep[K];  // the pod's replica-name id until its replica is identified, then the replica's ordinal (identity order)
+  uint32_t todo = 0, noname = 0;  // bit k: member with the label whose replica is not identified yet / member without the label
+#pragma unroll
+  for (int k = 0; k < K; k++) {
+    const bool member = (pw[k] >> 16) == gi;  // (an empty register has no group)
+    rep[k] = member ? __ldg(&s.p_replica_name_id[pidx[k]]) : 0u;
+    if (member) { if (rep[k]) todo |= 1u << k; else noname |= 1u << k; }
+  }
+  const uint32_t labelled = todo;
+  // 1. replicaMap (:967-972); 2. the first incomplete replica in identity order aborts the group (:975-984)
+  uint32_t n_rep = 0, r_empty = KR_MH_NONE, heads = 0;
+  while (__any_sync(0xFFFFFFFFu, todo)) {
+    uint32_t m = 0xFFFFFFFFu, mname = 0;
+#pragma unroll
+    for (int k = 0; k < K; k++) if (((todo >> k) & 1u) && pidx[k] < m) { m = pidx[k]; mname = rep[k]; }
+    const uint32_t wm = __reduce_min_sync(0xFFFFFFFFu, m);
+    const uint32_t name = __shfl_sync(0xFFFFFFFFu, mname, __ffs(__ballot_sync(0xFFFFFFFFu, m == wm)) - 1);
+    uint32_t count = 0, mine = 0;
+#pragma unroll
+    for (int k = 0; k < K; k++) {
+      const bool hit = ((todo >> k) & 1u) && rep[k] == name;
+      if (hit) { rep[k] = n_rep; mine |= 1u << k; if (pidx[k] == wm) heads |= 1u << k; }
+      count += __popc(__ballot_sync(0xFFFFFFFFu, hit));
+    }
+    todo &= ~mine;
+    if ((int64_t)count < (int64_t)H) {
+#pragma unroll
+      for (int k = 0; k < K; k++) if ((mine >> k) & 1u) act[k] = KR_ACT_DELETE_MH_INCOMPLETE;
+      gr.flags |= KR_GR_ABORTED; err_arg = (int32_t)count;
+      return KR_ERR_MH_INCOMPLETE;
+    }
+    if (name == KR_ID_EMPTY_STRING) r_empty = n_rep;
+    n_rep++;
+  }
+  for (uint32_t r = lane; r < n_rep; r += 32) s_rep[r] = 0;
+  __syncwarp();
+  // 3. unhealthy replicas (:987-1007): a pod marks its replica; unlabelled pods resolve to the "" replica if one exists
+#pragma unroll
+  for (int k = 0; k < K; k++) {
+    if ((((labelled | noname) >> k) & 1u) && (pw[k] & KR_ROW_UNHEALTHY)) {
+      const uint32_t r = ((noname >> k) & 1u) ? r_empty : rep[k];
+      if (r != KR_MH_NONE) atomicOr(&s_rep[r], KR_MHF_DELETED);
+    }
+  }
+  __syncwarp();
+  int32_t n_unh = 0;
+#pragma unroll
+  for (int k = 0; k < K; k++) {
+    const bool hit = ((labelled >> k) & 1u) && (s_rep[rep[k]] & KR_MHF_DELETED);
+    if (hit) act[k] = KR_ACT_DELETE_MH_UNHEALTHY;
+    n_unh += __popc(__ballot_sync(0xFFFFFFFFu, hit));
+  }
+  gr.n_unhealthy = n_unh;
+  // 4. explicit deletions from the autoscaler (:1010-1038): whole replicas
+  if (wtd_cnt > 0) {
+#pragma unroll
+    for (int k = 0; k < K; k++) {
+      if ((((labelled | noname) >> k) & 1u) && (pw[k] & KR_ROW_WTD_OWN)) {
+        const uint32_t r = ((noname >> k) & 1u) ? r_empty : rep[k];
+        if (r != KR_MH_NONE) atomicOr(&s_rep[r], KR_MHF_WTD);
+      }
+    }
+    __syncwarp();
+    int32_t n_del = 0;
+#pragma unroll
+    for (int k = 0; k < K; k++) {
+      const bool hit = ((labelled >> k) & 1u) && (s_rep[rep[k]] & KR_MHF_WTD);
+      if (hit && act[k] == KR_ACT_KEEP) act[k] = KR_ACT_DELETE_MH_WTD;
+      n_del += __popc(__ballot_sync(0xFFFFFFFFu, hit));
+    }
+    gr.flags |= KR_GR_WTD_EXECUTED;
+    if (n_del > 0) { gr.flags |= KR_GR_ABORTED; err_arg = n_del; return KR_ERR_MH_WTD; }
+  }
+  // 5. diff by replica (:1042-1064): healthy (complete) replicas are running
+  int32_t running = 0;
+  for (uint32_t r = lane; r < n_rep; r += 32) running += (s_rep[r] & KR_MHF_DELETED) ? 0 : 1;
+  running = __reduce_add_sync(0xFFFFFFFFu, running);
+#pragma unroll
+  for (int k = 0; k < K; k++) if (((heads >> k) & 1u) && !(s_rep[rep[k]] & KR_MHF_DELETED)) mh_head |= 1u << k;
+  gr.n_running = running;
+  if (expected % H != 0) { gr.flags |= KR_GR_ABORTED; err_arg = expected; return KR_ERR_MH_NOT_MULTIPLE; }
+  const int32_t to_create = expected / H - running;
+  gr.diff = to_create;
+  if (to_create > 0) gr.n_create = (uint32_t)to_create;  // replica groups; the creates below allocate one replica index each
+  else if (to_create < 0) {
+    if (delete_allowed) {  // :1104-1118 — the first -to_create healthy replicas in identity order
+      const int32_t remove = -to_create;
+      int32_t seen = 0;
+      for (uint32_t b = 0; b < n_rep && seen < remove; b += 32) {
+        const uint32_t r = b + lane;
+        const bool ok = r < n_rep && !(s_rep[r] & KR_MHF_DELETED);
+        const uint32_t bal = __ballot_sync(0xFFFFFFFFu, ok);
+        if (ok && seen + (int32_t)__popc(bal & lt) < remove) s_rep[r] |= KR_MHF_SCALE;
+        seen += __popc(bal);
+      }
+      __syncwarp();
+#pragma unroll
+      for (int k = 0; k < K; k++) if (((labelled >> k) & 1u) && (s_rep[rep[k]] & KR_MHF_SCALE)) act[k] = KR_ACT_DELETE_MH_SCALE_DOWN;
+    } else gr.flags |= KR_GR_RANDOM_DELETE_OFF;
+  }
+  return KR_ERR_NONE;
+}
+
 // reconcilePods (raycluster_controller.go:619-935) + calculateStatus (:1552-1719) for one RayCluster whose bucket (<= 32*K pods,
-// arrival order) sits in registers.  Multi-host groups never reach this kernel.
+// arrival order) sits in registers.
 // kInc: the instantiation an incremental epoch launches (phase 2 only); the instantiation of the full pass carries none of its code.
-template <int K, bool kInc = false>
-__global__ void __launch_bounds__(kD2Warps * 32, (K <= 4 ? 32 : 16) / kD2Warps) k_decide2(Decide2Args a) {
+// kMH: the snapshot has a multi-host worker group and the RayMultiHostIndexing gate is on — only these instantiations carry the
+// multi-host branch (decide_multihost2), so the common path keeps its register budget.  They run at half the occupancy of the
+// K <= 4 common path: with the replica peel in the 64-register budget the compiler spills.
+template <int K, bool kInc = false, bool kMH = false>
+__global__ void __launch_bounds__(kD2Warps * 32, (K <= 4 && !kMH ? 32 : 16) / kD2Warps) k_decide2(Decide2Args a) {
   const int phase = kInc ? 2 : a.phase;
   KR_TL(phase ? 12 : 3);
   __shared__ int32_t s_acc[kD2Warps][3][KR_SMEM_GROUPS];   // n_list, n_unhealthy, n_wtd_own per group
-  __shared__ int32_t s_mode[kD2Warps][3][KR_SMEM_GROUPS];  // mode, delete-prefix length, n_create
-  __shared__ uint32_t s_list[kD2Warps][32 * K];            // pod indices being ranked (delete candidates / acted pods)
+  __shared__ int32_t s_mode[kD2Warps][kMH ? 4 : 3][KR_SMEM_GROUPS];  // mode, delete-prefix length, n_create (, n_running of a multi-host group)
+  __shared__ uint32_t s_list[kD2Warps][32 * K];            // pod indices being ranked (delete candidates / acted pods); per-replica flags
+                                                           // of the multi-host group being decided
   __shared__ uint32_t s_bits[kD2Warps][32];                // 1024-bit window of replica indices in use
   const SnapDev &s = a.s;
   const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -297,7 +420,8 @@ __global__ void __launch_bounds__(kD2Warps * 32, (K <= 4 ? 32 : 16) / kD2Warps) 
   }
   (void)head_pos;
   int32_t *acc_list = s_acc[warp][0], *acc_unh = s_acc[warp][1], *acc_wtd = s_acc[warp][2];
-  int32_t *g_mode = s_mode[warp][0], *g_prefix = s_mode[warp][1], *g_ncreate = s_mode[warp][2];
+  int32_t *g_mode = s_mode[warp][0], *g_prefix = s_mode[warp][1], *g_ncreate = s_mode[warp][2], *g_mh_running = s_mode[warp][kMH ? 3 : 2];
+  uint32_t mh_head = 0;  // kMH: bit k = this lane's pod of chunk k is the first pod of a healthy replica of a multi-host group
   if (lane < KR_SMEM_GROUPS) { acc_list[lane] = 0; acc_unh[lane] = 0; acc_wtd[lane] = 0; g_mode[lane] = GM_UNPROCESSED; g_prefix[lane] = 0; g_ncreate[lane] = 0; }
   __syncwarp();
 
@@ -433,6 +557,14 @@ __global__ void __launch_bounds__(kD2Warps * 32, (K <= 4 ? 32 : 16) / kD2Warps) 
           const int32_t n_list = acc_list[gi], n_unh = acc_unh[gi], n_wtd = acc_wtd[gi];
           gr.expected = expected; gr.n_list = n_list;
           if (gf & KR_GF_SUSPEND) { gr.flags |= KR_GR_SUSPENDED; mode = GM_SUSPENDED; }
+          else if (kMH && hosts > 1 && a.f.gate_multihost_indexing) {  // :777-784 (numOfHosts from the group row, never from the table's bit)
+            gr.flags |= KR_GR_MULTIHOST; mode = GM_MULTIHOST;
+            int32_t earg = 0;
+            const int ek = decide_multihost2<K>(s, gi, expected, hosts, !autoscaling || a.f.env_random_pod_delete, LDG(s.g_wtd_cnt[g]), pidx, pw, act, mh_head,
+                                                s_list[warp], gr, earg, lane);
+            if (ek != KR_ERR_NONE) { cr.err_kind = (uint8_t)ek; cr.err_arg = earg; abort_here = true; }
+            if (lane == 0) g_mh_running[gi] = gr.n_running;
+          }
           else if (n_unh > 0) {  // :786-812
             gr.n_unhealthy = n_unh; gr.flags |= KR_GR_ABORTED; mode = GM_UNHEALTHY;
             cr.err_kind = KR_ERR_UNHEALTHY_WORKERS; cr.err_arg = n_unh; abort_here = true;
@@ -488,6 +620,7 @@ __global__ void __launch_bounds__(kD2Warps * 32, (K <= 4 ? 32 : 16) / kD2Warps) 
       if (all_action != KR_ACT_KEEP) ac = valid ? all_action : (uint32_t)KR_ACT_KEEP;
       else if (head_delete) { if (valid && pidx[k] == head_pod) ac = KR_ACT_DELETE_HEAD; }
       else if (mode == GM_SUSPENDED) ac = KR_ACT_DELETE_GROUP_SUSPEND;
+      else if (kMH && mode == GM_MULTIHOST) ac = act[k];  // decided with its group (decide_multihost2)
       else if (mode == GM_UNHEALTHY) { if (fl & KR_ROW_UNHEALTHY) ac = KR_ACT_DELETE_UNHEALTHY; }
       else if (mode == GM_NORMAL) {
         if (fl & KR_ROW_WTD_OWN) ac = KR_ACT_DELETE_WTD;
@@ -640,7 +773,9 @@ __global__ void __launch_bounds__(kD2Warps * 32, (K <= 4 ? 32 : 16) / kD2Warps) 
       if (!a.f.gate_multihost_indexing) {  // createWorkerPod without an index (:884-889)
         for (uint32_t k2 = lane; k2 < want; k2 += 32) out[k2] = -1;
       } else {
-        const uint64_t bound = (uint64_t)(acc_list[gi] - acc_wtd[gi]) + want;  // the `want` lowest free indices all lie below n_running + want
+        // multi-host (:1067-1077): in use = the label of the first pod of every healthy replica, and n_create counts replicas
+        const bool mh = kMH && g_mode[gi] == GM_MULTIHOST;
+        const uint64_t bound = (uint64_t)(mh ? g_mh_running[gi] : acc_list[gi] - acc_wtd[gi]) + want;  // the `want` lowest free indices all lie below n_running + want
         uint32_t written = 0;
         for (uint64_t w0 = 0; w0 < bound && written < want; w0 += 1024) {
           s_bits[warp][lane] = 0;
@@ -648,7 +783,7 @@ __global__ void __launch_bounds__(kD2Warps * 32, (K <= 4 ? 32 : 16) / kD2Warps) 
 #pragma unroll
           for (int k = 0; k < K; k++) {
             // runningPods of this group: listed, not deleted by name, label present and numeric
-            if ((pw[k] >> 16) == gi && (pw[k] & KR_PP_HAS_REPLICA_IDX) && act[k] == KR_ACT_KEEP && pidx[k] != 0xFFFFFFFFu) {
+            if ((pw[k] >> 16) == gi && (pw[k] & KR_PP_HAS_REPLICA_IDX) && (mh ? ((mh_head >> k) & 1u) != 0 : (act[k] == KR_ACT_KEEP && pidx[k] != 0xFFFFFFFFu))) {
               const int32_t idx = (int32_t)ridx[k];
               if (idx >= 0 && (uint64_t)idx >= w0 && (uint64_t)idx < w0 + 1024 && (uint64_t)idx < bound)
                 atomicOr(&s_bits[warp][(idx - w0) >> 5], 1u << ((idx - w0) & 31));

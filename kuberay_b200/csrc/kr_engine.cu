@@ -61,11 +61,13 @@ static_assert(sizeof(kr_snapshot_bufs) == kNumCols * sizeof(void *), "kCols must
 static_assert(sizeof(SnapDev) == kNumCols * sizeof(void *), "SnapDev must mirror kr_snapshot_bufs");
 static_assert(sizeof(kr_cluster_result) == 96 && sizeof(kr_group_result) == 32 && sizeof(kr_job_result) == 8, "result record sizes");
 
-// how a changed row of each object column is treated by the on-device diff of an object commit (kr_incr.cuh, KR_OC_*)
+// how a changed row of each object column is treated by the on-device diff of an object commit (kr_incr.cuh, KR_OC_*).
+// (g_num_hosts is an ordinary group column: k_decide2 reads numOfHosts from the group rows / the refreshed input record, never from
+// the multi-host bit of the resident cluster table, which only the sort pipeline reads and a full pass rebuilds.)
 static const uint8_t kObjClass[kNumCols] = {
         KR_OC_STRUCT, KR_OC_STRUCT, KR_OC_COPY, KR_OC_CLUSTER, KR_OC_CLUSTER, KR_OC_CLUSTER, KR_OC_CLUSTER, KR_OC_STRUCT, KR_OC_STRUCT, KR_OC_COPY, KR_OC_COPY,
         KR_OC_CLUSTER, KR_OC_CLUSTER, KR_OC_CLUSTER, KR_OC_CLUSTER, KR_OC_CLUSTER, KR_OC_CLUSTER, KR_OC_CLUSTER, KR_OC_CLUSTER, KR_OC_CLUSTER, KR_OC_CLUSTER, KR_OC_CLUSTER,
-        KR_OC_STRUCT, KR_OC_STRUCT, KR_OC_GROUP, KR_OC_GROUP, KR_OC_GROUP, KR_OC_STRUCT, KR_OC_GROUP, KR_OC_STRUCT, KR_OC_STRUCT,
+        KR_OC_STRUCT, KR_OC_STRUCT, KR_OC_GROUP, KR_OC_GROUP, KR_OC_GROUP, KR_OC_GROUP, KR_OC_GROUP, KR_OC_STRUCT, KR_OC_STRUCT,
         KR_OC_STRUCT,
         0, 0, 0, 0, 0, 0, 0,
         KR_OC_HEADKEY, KR_OC_HEAD, KR_OC_HEAD, KR_OC_HEAD, KR_OC_HEAD, KR_OC_HEAD, KR_OC_HEAD, KR_OC_HEAD,
@@ -257,6 +259,7 @@ struct kr_engine {
   cudaEvent_t ev_orow = nullptr; bool orow_busy = false;
   uint32_t bstride = 0;         // bucket stride of this layout (64 / 128 / 256); 0 = the layout does not qualify (a cluster outgrew 256 pods, ...)
   bool snap_has_mh = false;     // some worker group has numOfHosts > 1
+  std::vector<uint8_t> mh_bit;  // ... per cluster row, as of the last commit (kr_snapshot_commit_object_rows keeps snap_has_mh current with it)
   uint32_t snap_max_groups = 0; // most worker groups in one RayCluster
   bool ran_bucket = false;
   uint64_t h2d_accum = 0;       // bytes uploaded by the commits since the last pass (kr_profile.h2d_bytes)
@@ -407,10 +410,10 @@ int launch_pass(kr_engine *e, const kr_flags &f, bool profile, bool capturing = 
   // the committed snapshot: columns gate stream M, the JSON arena gates the hash
   const unsigned wflag = capturing ? cudaEventWaitExternal : cudaEventWaitDefault;
   // (the fork comes first so the hash can start while the columns are still landing — an incremental pod-row epoch leaves the JSON untouched)
-  // bucket pipeline (kr_bucket2.cuh): the caller does not fetch the full pod lists, no multi-host group is in play, every
-  // RayCluster has few worker groups and (checked on the device) at most `bstride` pods
+  // bucket pipeline (kr_bucket2.cuh): the caller does not fetch the full pod lists, every RayCluster has few worker groups and
+  // (checked on the device) at most `bstride` pods
   const bool bucket = !e->no_bucket && !f.fetch_pod_lists && e->bstride != 0 && !e->force_radix && e->snap_max_groups <= KR_SMEM_GROUPS &&
-                      !(e->snap_has_mh && f.gate_multihost_indexing) && (size_t)n.n_clusters * e->bstride <= e->sl.bucket_entries;
+                      (size_t)n.n_clusters * e->bstride <= e->sl.bucket_entries;
   // ... and there the clusters whose Recreate gate reads a digest wait for it inside the decide kernel (the hash runs beside it)
   const bool spin = bucket && !profile && do_hash && e->hash_spin && e->n_recreate > 0;
   auto launch_hash = [&]() {
@@ -471,10 +474,12 @@ int launch_pass(kr_engine *e, const kr_flags &f, bool profile, bool capturing = 
       CK(launch_pdl(k_match2<kMatchItems>, dim3(mtiles), dim3(kSortThreads), n.n_wtd ? e->sl.wt_bits_n / 8 : 0, M, pdl, s, sc, r, z, n.n_wtd ? 1 : 0));
     }
     Decide2Args da{s, sc, r, z, f, IncStage{}, e->cfg.max_creates, spin ? 1 : 0, 0};
+    const bool mh = e->snap_has_mh && f.gate_multihost_indexing;  // the instantiations with the multi-host branch
     auto launch_decide2 = [&](dim3 grid, bool with_pdl) -> cudaError_t {
-      if (e->bstride <= 64) return launch_pdl(k_decide2<2>, grid, dim3(kD2Warps * 32), 0, M, with_pdl, da);
-      if (e->bstride <= 128) return launch_pdl(k_decide2<4>, grid, dim3(kD2Warps * 32), 0, M, with_pdl, da);
-      return launch_pdl(k_decide2<8>, grid, dim3(kD2Warps * 32), 0, M, with_pdl, da);
+      const dim3 block(kD2Warps * 32);
+      if (e->bstride <= 64) return launch_pdl(mh ? k_decide2<2, false, true> : k_decide2<2>, grid, block, 0, M, with_pdl, da);
+      if (e->bstride <= 128) return launch_pdl(mh ? k_decide2<4, false, true> : k_decide2<4>, grid, block, 0, M, with_pdl, da);
+      return launch_pdl(mh ? k_decide2<8, false, true> : k_decide2<8>, grid, block, 0, M, with_pdl, da);
     };
     if (n.n_clusters) {
       mark("k_decide2");
@@ -710,9 +715,11 @@ int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile
     Decide2Args da{s, sc, r, z, f, st, e->cfg.max_creates, 0, 2};
     const dim3 dgrid((n.n_clusters + kD2Warps - 1) / kD2Warps), dblock(kD2Warps * 32);
     mark("k_decide2_dirty");
-    if (e->bstride <= 64) k_decide2<2, true><<<dgrid, dblock, 0, M>>>(da);
-    else if (e->bstride <= 128) k_decide2<4, true><<<dgrid, dblock, 0, M>>>(da);
-    else k_decide2<8, true><<<dgrid, dblock, 0, M>>>(da);
+    // (snap_has_mh as of the latest commit: an object commit may have brought the snapshot's first multi-host group or taken its last)
+    const bool mh = e->snap_has_mh && f.gate_multihost_indexing;
+    if (e->bstride <= 64) (mh ? k_decide2<2, true, true> : k_decide2<2, true>)<<<dgrid, dblock, 0, M>>>(da);
+    else if (e->bstride <= 128) (mh ? k_decide2<4, true, true> : k_decide2<4, true>)<<<dgrid, dblock, 0, M>>>(da);
+    else (mh ? k_decide2<8, true, true> : k_decide2<8, true>)<<<dgrid, dblock, 0, M>>>(da);
   }
   if (n.n_jobs) { mark("k_jobs"); k_jobs<<<(n.n_jobs + 255) / 256, 256, 0, M>>>(s, sc, r, z); }
   if (profile && k <= KR_MAX_KERNEL_TIMES) cudaEventRecord(e->ev_k[k < KR_MAX_KERNEL_TIMES ? k : KR_MAX_KERNEL_TIMES], M);
@@ -984,7 +991,8 @@ int kr_engine_create(const kr_config *cfg, kr_engine **out) {
                         (const void *)k_match2<kMatchItems>, (const void *)k_decide2<2>, (const void *)k_decide2<4>, (const void *)k_decide2<8>, (const void *)k_hash3<1, 0>,
                         (const void *)k_inc_retire, (const void *)k_inc_objects, (const void *)k_inc_objects_keys, (const void *)k_inc_aux_clear, (const void *)k_inc_aux_insert,
                         (const void *)k_inc_mark_recreate, (const void *)k_decide2<2, true>, (const void *)k_decide2<4, true>, (const void *)k_decide2<8, true>, (const void *)k_inc_refresh, (const void *)k_inc_admit,
-                        (const void *)k_inc_finish};
+                        (const void *)k_inc_finish, (const void *)k_decide2<2, false, true>, (const void *)k_decide2<4, false, true>, (const void *)k_decide2<8, false, true>,
+                        (const void *)k_decide2<2, true, true>, (const void *)k_decide2<4, true, true>, (const void *)k_decide2<8, true, true>};
     for (const void *k : ks) cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, pct);
   }
   if (const char *g = getenv("KR_NO_GRAPH")) e->use_graph = !(g[0] == '1');
@@ -1119,6 +1127,7 @@ int kr_snapshot_commit_parts(kr_engine *e, uint32_t parts) {
   uint32_t n_recreate = 0, max_groups = 0;
   bool has_mh = false;
   uint64_t goff = 0, woff = 0;
+  e->mh_bit.assign(n.n_clusters, 0);
   for (uint32_t c = 0; c < n.n_clusters; c++) {
     if (hb.c_group_off[c] != goff) return fail(e, KR_E_INVALID, "cluster %u: groups must be stored in cluster order (group_off %u != %llu)", c, hb.c_group_off[c], (unsigned long long)goff);
     if (hb.c_group_cnt[c] >= 0xFFFFu) return fail(e, KR_E_CAPACITY, "cluster %u has %u worker groups (limit 65534)", c, hb.c_group_cnt[c]);
@@ -1129,7 +1138,7 @@ int kr_snapshot_commit_parts(kr_engine *e, uint32_t parts) {
       if (hb.g_wtd_off[g] != woff) return fail(e, KR_E_INVALID, "group %llu: workersToDelete names must be stored in group order (wtd_off %u != %llu)", (unsigned long long)g, hb.g_wtd_off[g], (unsigned long long)woff);
       woff += hb.g_wtd_cnt[g];
       if (woff > n.n_wtd) return fail(e, KR_E_INVALID, "group %llu: workersToDelete names run past n_wtd", (unsigned long long)g);
-      has_mh |= hb.g_num_hosts[g] > 1;
+      if (hb.g_num_hosts[g] > 1) { has_mh = true; e->mh_bit[c] = 1; }
     }
     max_groups = std::max(max_groups, hb.c_group_cnt[c]);
     goff += hb.c_group_cnt[c];
@@ -1347,7 +1356,7 @@ int kr_snapshot_commit_object_rows(kr_engine *e, const uint32_t *cluster_rows, u
   // are — no resident state, a Recreate gate or a JSON range that changed (hash order / digests), head rows added or removed —
   // the whole object part is committed instead.
   bool whole = !e->inc_valid || e->no_incr || !e->committed_full || e->res_n_heads != n.n_heads || e->recreate_bit.size() != n.n_clusters ||
-               e->prev_json_off.size() != n.n_clusters;
+               e->prev_json_off.size() != n.n_clusters || e->mh_bit.size() != n.n_clusters;
   for (uint32_t i = 0; i < n_cl && !whole; i++) {
     const uint32_t c = cluster_rows[i];
     if (c >= n.n_clusters) return fail(e, KR_E_INVALID, "cluster row %u out of range", c);
@@ -1360,6 +1369,19 @@ int kr_snapshot_commit_object_rows(kr_engine *e, const uint32_t *cluster_rows, u
   }
   if (whole) return kr_snapshot_commit_parts(e, KR_PART_OBJECTS);
   CK(cudaSetDevice(e->cfg.device));
+  // a numOfHosts edit may bring the snapshot's first multi-host group or take its last: the decide kernel's instantiation follows
+  bool mh_moved = false;
+  for (uint32_t i = 0; i < n_cl; i++) {
+    const uint32_t c = cluster_rows[i];
+    uint8_t bit = 0;
+    for (uint32_t g = hb.c_group_off[c]; g < hb.c_group_off[c] + hb.c_group_cnt[c]; g++) bit |= hb.g_num_hosts[g] > 1 ? 1 : 0;
+    if (bit != e->mh_bit[c]) { e->mh_bit[c] = bit; mh_moved = true; }
+  }
+  if (mh_moved) {
+    const bool has_mh = std::find(e->mh_bit.begin(), e->mh_bit.end(), 1) != e->mh_bit.end();
+    if (has_mh != e->snap_has_mh) e->gvalid = false;  // (the captured full pass launches the other instantiation)
+    e->snap_has_mh = has_mh;
+  }
   // group rows of the named clusters
   std::vector<uint32_t> grows;
   for (uint32_t i = 0; i < n_cl; i++) for (uint32_t g = 0; g < hb.c_group_cnt[cluster_rows[i]]; g++) grows.push_back(hb.c_group_off[cluster_rows[i]] + g);

@@ -30,6 +30,8 @@ CONFIGS = {
     "C3x10": dict(n_clusters=100000, pods_per_cluster=100, groups=1),
     "C4": dict(n_clusters=10000, pods_per_cluster=100, groups=1, jobs=True),
     "C5": dict(n_clusters=1000, pods_per_cluster=100, groups=1, autoscaling_frac=1.0),
+    # C3 with TPU-slice style worker groups: a quarter of the groups have numOfHosts=4 (about 44 % of the RayClusters hold one)
+    "C3MH": dict(n_clusters=10000, pods_per_cluster=100, groups=2, multihost_frac=0.25),
 }
 
 

@@ -75,6 +75,8 @@ def incremental(snap, flags, label):
 
 def main():
     incremental(*synthetic.generate(synthetic.config("C2", n_clusters=300, pods_per_cluster=20, groups=2, jobs=True, wtd_group_frac=0.3)), "incremental epochs")
+    incremental(*synthetic.generate(synthetic.config("C2", n_clusters=300, pods_per_cluster=41, groups=2, wtd_group_frac=0.3, multihost_frac=0.5)),
+                "incremental epochs, multi-host groups")
     one(*synthetic.generate(synthetic.config("C2", n_clusters=200, jobs=True)), "fast pipeline")
     one(*synthetic.generate(synthetic.SynthParams(n_clusters=60, pods_per_cluster=41, groups=2, multihost_frac=0.5)), "multi-host")
     one(*synthetic.generate(synthetic.SynthParams(n_clusters=20, pods_per_cluster=200, groups=40)), "many groups")
