@@ -416,7 +416,12 @@ class Results:
                     out.append(f"{name}: {int(neq.sum())} entries differ, first at action #{i}: {getattr(self, name)[sa][i]} != {getattr(other, name)[sb][i]}")
         if self.groups.shape == other.groups.shape and not (self.groups["n_create"] != other.groups["n_create"]).any():
             sa, sb = _gather_owned(self.groups["create_off"], self.groups["n_create"]), _gather_owned(other.groups["create_off"], other.groups["n_create"])
-            neq = self.create_idx[sa] != other.create_idx[sb]
+            bad = False
+            for res, idx in ((self, sa), (other, sb)):
+                if np.unique(idx).size != idx.size or (idx.size and int(idx.max()) >= res.create_idx.size):
+                    out.append("create_off / n_create: two groups' runs overlap or leave the list")
+                    bad = True
+            neq = np.zeros(0, dtype=bool) if bad else self.create_idx[sa] != other.create_idx[sb]
             if neq.any():
                 i = int(np.flatnonzero(neq)[0])
                 out.append(f"create_idx: {int(neq.sum())} entries differ, first at create #{i}: {self.create_idx[sa][i]} != {other.create_idx[sb][i]}")

@@ -644,7 +644,9 @@ int run_pass_once(kr_engine *e, const kr_flags &f) {
 
 // a bucket-pipeline pass leaves everything an incremental epoch needs on the device
 void after_full_pass(kr_engine *e, const kr_flags &f) {
-  e->inc_valid = e->ran_bucket && !e->no_incr;
+  // (a pass whose create runs overran kr_config.max_creates is reported as KR_E_CAPACITY and left groups' runs unwritten: an
+  // incremental epoch would inherit that cursor and fail the same way, so the next pass starts over)
+  e->inc_valid = e->ran_bucket && !e->no_incr && e->h_totals[9] <= e->cfg.max_creates;
   e->inc_flags = f; e->inc_n_pods = e->sizes.n_pods; e->inc_n_heads = e->sizes.n_heads;
   e->host_results_stale = false; e->inc_n_dirty = 0; e->fetched = false; e->ran_inc = false; e->heads_rebuild = false;
   if (!f.skip_hash) e->hash_dirty = false;

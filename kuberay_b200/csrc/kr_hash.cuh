@@ -82,6 +82,38 @@ __device__ __forceinline__ void sha1_rounds2(uint32_t (&w)[16], uint32_t (&h)[5]
   h[0] += a; h[1] += b; h[2] += c; h[3] += d; h[4] += e;
 }
 
+// SHA-1 state -> the 32 base32hex characters of the digest (no padding: 160 bits are exactly 32 characters).
+__device__ __forceinline__ void digest_to_base32hex(const uint32_t (&h)[5], char *__restrict__ out32) {
+  uint32_t o32[8];
+#pragma unroll
+  for (int j = 0; j < 4; j++) {
+    uint64_t v;
+    switch (j) {
+      case 0: v = ((uint64_t)h[0] << 8) | (h[1] >> 24); break;
+      case 1: v = ((uint64_t)(h[1] & 0xFFFFFFu) << 16) | (h[2] >> 16); break;
+      case 2: v = ((uint64_t)(h[2] & 0xFFFFu) << 24) | (h[3] >> 8); break;
+      default: v = ((uint64_t)(h[3] & 0xFFu) << 32) | h[4]; break;
+    }
+    uint32_t lo = 0, hi = 0;
+#pragma unroll
+    for (int kk = 0; kk < 8; kk++) {
+      const uint32_t cc = (uint32_t)(v >> (35 - 5 * kk)) & 31u;
+      const uint32_t ch = cc < 10 ? ('0' + cc) : ('A' + cc - 10);
+      if (kk < 4) lo |= ch << (8 * kk); else hi |= ch << (8 * (kk - 4));
+    }
+    o32[2 * j] = lo; o32[2 * j + 1] = hi;
+  }
+  // The last word is the digest's "ready" mark: a decide warp of the concurrently running main chain may be polling it
+  // (k_decide2: Recreate gate), so both hash kernels (k_hash2, k_hash3) store it after a fence, once the other 28 bytes are
+  // visible.
+  uint4 *dst = reinterpret_cast<uint4 *>(out32);
+  dst[0] = make_uint4(o32[0], o32[1], o32[2], o32[3]);
+  reinterpret_cast<uint2 *>(out32)[2] = make_uint2(o32[4], o32[5]);
+  reinterpret_cast<uint32_t *>(out32)[6] = o32[6];
+  __threadfence();
+  reinterpret_cast<volatile uint32_t *>(out32)[7] = o32[7];
+}
+
 template <int WARPS, int VARIANT>
 __global__ void __launch_bounds__(WARPS * 32) k_hash2(const uint8_t *__restrict__ bytes, const uint64_t *__restrict__ off,
                                                       const uint32_t *__restrict__ len32, const uint32_t *__restrict__ order,
@@ -161,30 +193,7 @@ __global__ void __launch_bounds__(WARPS * 32) k_hash2(const uint8_t *__restrict_
     }
     __syncwarp();  // every lane is done reading this buffer before the fetch two iterations ahead overwrites it
   }
-  if (have) {
-  uint32_t o32[8];
-#pragma unroll
-  for (int j = 0; j < 4; j++) {
-    uint64_t v;
-    switch (j) {
-      case 0: v = ((uint64_t)h[0] << 8) | (h[1] >> 24); break;
-      case 1: v = ((uint64_t)(h[1] & 0xFFFFFFu) << 16) | (h[2] >> 16); break;
-      case 2: v = ((uint64_t)(h[2] & 0xFFFFu) << 24) | (h[3] >> 8); break;
-      default: v = ((uint64_t)(h[3] & 0xFFu) << 32) | h[4]; break;
-    }
-    uint32_t lo = 0, hi = 0;
-#pragma unroll
-    for (int kk = 0; kk < 8; kk++) {
-      uint32_t cc = (uint32_t)(v >> (35 - 5 * kk)) & 31u;
-      uint32_t ch = cc < 10 ? ('0' + cc) : ('A' + cc - 10);
-      if (kk < 4) lo |= ch << (8 * kk); else hi |= ch << (8 * (kk - 4));
-    }
-    o32[2 * j] = lo; o32[2 * j + 1] = hi;
-  }
-  uint4 *dst = reinterpret_cast<uint4 *>(out + 32 * (size_t)m);
-  dst[0] = make_uint4(o32[0], o32[1], o32[2], o32[3]);
-  dst[1] = make_uint4(o32[4], o32[5], o32[6], o32[7]);
-  }
+  if (have) digest_to_base32hex(h, out + 32 * (size_t)m);
   __syncwarp();
   }  // next group of messages
 }
@@ -298,36 +307,6 @@ __device__ __forceinline__ void sha1_expand_block(const uint4 *__restrict__ tile
     }
     *reinterpret_cast<uint4 *>(wk_row + 4 * q) = make_uint4(o[0], o[1], o[2], o[3]);
   }
-}
-
-__device__ __forceinline__ void digest_to_base32hex(const uint32_t (&h)[5], char *__restrict__ out32) {
-  uint32_t o32[8];
-#pragma unroll
-  for (int j = 0; j < 4; j++) {
-    uint64_t v;
-    switch (j) {
-      case 0: v = ((uint64_t)h[0] << 8) | (h[1] >> 24); break;
-      case 1: v = ((uint64_t)(h[1] & 0xFFFFFFu) << 16) | (h[2] >> 16); break;
-      case 2: v = ((uint64_t)(h[2] & 0xFFFFu) << 24) | (h[3] >> 8); break;
-      default: v = ((uint64_t)(h[3] & 0xFFu) << 32) | h[4]; break;
-    }
-    uint32_t lo = 0, hi = 0;
-#pragma unroll
-    for (int kk = 0; kk < 8; kk++) {
-      const uint32_t cc = (uint32_t)(v >> (35 - 5 * kk)) & 31u;
-      const uint32_t ch = cc < 10 ? ('0' + cc) : ('A' + cc - 10);
-      if (kk < 4) lo |= ch << (8 * kk); else hi |= ch << (8 * (kk - 4));
-    }
-    o32[2 * j] = lo; o32[2 * j + 1] = hi;
-  }
-  // The last word is the digest's "ready" mark: a decide warp of the concurrently running main chain may be polling it
-  // (k_decide2: Recreate gate), so it is stored after a fence, once the other 28 bytes are visible.
-  uint4 *dst = reinterpret_cast<uint4 *>(out32);
-  dst[0] = make_uint4(o32[0], o32[1], o32[2], o32[3]);
-  reinterpret_cast<uint2 *>(out32)[2] = make_uint2(o32[4], o32[5]);
-  reinterpret_cast<uint32_t *>(out32)[6] = o32[6];
-  __threadfence();
-  reinterpret_cast<volatile uint32_t *>(out32)[7] = o32[7];
 }
 
 // grid: CTAs of PAIRS x 64 threads (even warp = consumer, odd warp = producer); G = total pairs; group g of 32 messages (in

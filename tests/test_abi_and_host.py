@@ -171,3 +171,35 @@ def test_two_rank_gloo_sharded_pass_and_delta_allgather():
         cmd = [sys.executable, "-m", "torch.distributed.run", "--nnodes=1", "--nproc-per-node=2", "--master-addr", "127.0.0.1", "--master-port", "29517", script, ROOT]
         out = subprocess.run(cmd, capture_output=True, text=True, timeout=600)
     assert "GLOO_OK" in out.stdout, out.stdout[-2000:] + out.stderr[-2000:]
+
+
+def test_results_diff_reports_create_runs_that_overlap_or_leave_the_list():
+    """Results.diff compares the replica-index arena group by group through (create_off, n_create).  Runs that share places or
+    run past the end of create_idx are a fault of the producer, even where the values they read happen to agree."""
+    sizes = abi.kr_sizes(n_clusters=1, n_groups=3, n_wtd=0, n_pods=0, n_heads=0, n_jobs=0, json_bytes=0)
+
+    def results(offs, cnts, idx):
+        r = abi.Results(sizes, len(idx))
+        r.groups["create_off"], r.groups["n_create"] = offs, cnts
+        r.create_idx[:] = idx
+        r.n_create_total = int(sum(cnts))
+        return r
+
+    want = results([0, 2, 4], [2, 2, 1], [0, 1, 0, 1, 7])
+    assert not want.diff(results([3, 1, 0], [2, 2, 1], [7, 0, 1, 0, 1]))   # another layout of the same runs
+    # groups 0 and 1 share their two places: the values agree ([0, 1] both), only the layout check sees it
+    overlap = results([0, 0, 4], [2, 2, 1], [0, 1, 9, 9, 7])
+    d = want.diff(overlap)
+    assert any("overlap or leave the list" in m for m in d), d
+    # a run past the end of the list
+    past = results([0, 2, 4], [2, 2, 1], [0, 1, 0, 1, 7])
+    past.groups["create_off"][2] = 5
+    d = want.diff(past)
+    assert any("overlap or leave the list" in m for m in d), d
+    assert any("overlap or leave the list" in m for m in past.diff(want))
+    # an empty group may sit anywhere, even at the end of the list
+    empty = results([0, 2, 4], [2, 2, 1], [0, 1, 0, 1, 7])
+    empty.groups["n_create"][2], empty.n_create_total = 0, 4
+    want_empty = results([0, 2, 99], [2, 2, 0], [0, 1, 0, 1, 7])
+    want_empty.n_create_total = 4
+    assert not want_empty.diff(empty)

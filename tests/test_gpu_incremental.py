@@ -19,10 +19,10 @@ OBJ_COLS = [name for name, _dt, _m, dim in abi.COLUMNS if dim not in ("pods", "j
 
 
 class Driver:
-    def __init__(self, snap, flags, slack=1.0):
+    def __init__(self, snap, flags, slack=1.0, max_creates=None):
         self.snap, self.flags = snap, flags
         self.flags.fetch_pod_lists = 0
-        self.eng = Engine.for_snapshot(snap, slack=slack)
+        self.eng = Engine.for_snapshot(snap, slack=slack, max_creates=max_creates)
         self.eng.set_fixed_layout(True)
         self.views = self.eng.begin(snap.sizes())
         self.eng.fill(self.views, snap)

@@ -16,8 +16,9 @@ def _compact(flags):
     return f
 
 
-def _parity(snap, flags, oracle_mod, **kw):
-    """Engine vs oracle, twice: with the full pod lists (sort / radix pipeline) and without (bucket pipeline)."""
+def _parity(snap, flags, oracle_mod, both=False, **kw):
+    """Engine vs oracle, twice: with the full pod lists (sort / radix pipeline) and without (bucket pipeline).
+    -> the first run's results, or both runs' with `both`."""
     eng = Engine.for_snapshot(snap, **kw)
     try:
         eng.load(snap)
@@ -31,7 +32,7 @@ def _parity(snap, flags, oracle_mod, **kw):
     d = want.diff(lean)
     assert not d, "compact results (fetch_pod_lists = 0):\n" + "\n".join(d[:20])
     assert lean.sorted_pod_idx.size == 0
-    return got
+    return (got, lean) if both else got
 
 
 def _kernels(snap, flags):

@@ -90,7 +90,15 @@ def main():
     eng = Engine(0, 1, 1, 1, 1, 1, 1, 16, 4096)
     msgs = [bytes([65 + i % 26]) * n for i, n in enumerate((0, 1, 55, 56, 63, 64, 65, 119, 120, 128, 1000, 4097))]
     print("hash_batch", len(eng.hash_batch(msgs)), flush=True)
+    # above the throughput threshold ((n + 31) / 32 > 4 x SMs, kr_engine.cu) the engine hashes with k_hash2<4, 1>
+    import torch
+    n = 128 * torch.cuda.get_device_properties(0).multi_processor_count + 500
+    msgs = [bytes([65 + i % 26]) * (i % 300) for i in range(n)]
+    print("hash_batch, throughput regime", len(eng.hash_batch(msgs)), flush=True)
     eng.close()
+    snap, flags = synthetic.generate(synthetic.SynthParams(n_clusters=n, pods_per_cluster=2, groups=1, recreate_frac=0.3))
+    flags.fetch_pod_lists = 0   # bucket pipeline: the Recreate-gate warps wait for k_hash2's digests inside k_decide2
+    one(snap, flags, "throughput-regime hash with Recreate gates")
 
 
 if __name__ == "__main__":
