@@ -386,8 +386,8 @@ typedef struct kr_results_view {
    * absorb (a changed table key or CSR offset, wholesale column commits, different flags, an overflowing bucket) silently
    * takes the full pass.  Snapshots with multi-host worker groups (numOfHosts > 1) keep incremental epochs, and so does an edit of
    * numOfHosts.  Every pass is a full one on the sort pipeline — no resident state — while the caller fetches the full pod lists
-   * (fetch_pod_lists = 1), while some RayCluster lists more than 256 pods or has more than 32 worker groups, or when
-   * KR_NO_INCR=1 is set in the environment. */
+   * (fetch_pod_lists = 1), while some RayCluster lists more than 256 pods (more than KR_LARGE_MAX_PODS with KR_OPT_LARGE_CLUSTERS)
+   * or has more than 32 worker groups, or when KR_NO_INCR=1 is set in the environment. */
   uint32_t n_changed;
   const uint32_t          *changed_clusters; /* [n_changed] cluster rows, unordered */
 } kr_results_view;
@@ -512,11 +512,23 @@ int kr_last_profile(kr_engine *e, kr_profile *prof);
  *   incremental epoch: kr_snapshot_begin(new counts) + KR_PART_OBJECTS + kr_snapshot_commit_pod_rows/_values. */
 enum {
   KR_OPT_FIXED_LAYOUT = 1,
-  KR_OPT_INCREMENTAL = 2   /* 1 (default): passes after a full bucket-pipeline pass are incremental on the device whenever the commits in
+  KR_OPT_INCREMENTAL = 2,  /* 1 (default): passes after a full bucket-pipeline pass are incremental on the device whenever the commits in
                               between allow it (kr_results_view docs); 0: every pass is a full pass (benchmarks of the full pass, tests).
                               May be changed at any time. */
+  KR_OPT_LARGE_CLUSTERS = 3,  /* 1: RayClusters listing more than 256 and at most KR_LARGE_MAX_PODS pods stay on the bucket pipeline
+                              (DESIGN §4.1): a bucket attempt that meets one gives it a region of its own instead of widening the stride
+                              of the whole fleet or leaving the pipeline, so such a fleet keeps its incremental epochs.  Results are the
+                              same as with 0 (the default: one such RayCluster sends every pass to the sort pipeline).  May be set at any
+                              time; takes effect at the next full pass.  A RayCluster of more than KR_LARGE_MAX_PODS pods still sends
+                              the pass to the sort / radix pipelines.  Turning it on allocates the region arena once, for the
+                              capacities: about 22 B per max_pods + 20 B per max_clusters of device memory. */
+  KR_OPT_BUCKET_STRIDE = 4    /* read only (kr_engine_get_option): records per RayCluster bucket of the current layout (64 / 128 / 256);
+                              0 = the passes take the sort pipeline */
 };
+enum { KR_LARGE_MAX_PODS = 8192 };  /* largest RayCluster KR_OPT_LARGE_CLUSTERS keeps on the bucket pipeline */
 int kr_engine_set_option(kr_engine *e, uint32_t option, uint64_t value);
+/* Current value of an option (KR_OPT_*), and the read-only KR_OPT_BUCKET_STRIDE. */
+int kr_engine_get_option(kr_engine *e, uint32_t option, uint64_t *value);
 
 /* Device pointer + byte size of the per-group delta records (kr_group_result[n_groups]) of the last pass:
  * the payload of the optional cross-GPU all-gather (SURVEY §8(e)); the caller owns the collective. */

@@ -133,7 +133,16 @@ func (e *Engine) err(rc C.int) error {
 	return fmt.Errorf("krengine: %s (%d)", C.GoString(C.kr_last_error(e.h)), int(rc))
 }
 
-// SetOption: KR_OPT_FIXED_LAYOUT (before the first Begin), KR_OPT_INCREMENTAL, ...
+// Engine options (kr_engine_set_option).
+const (
+	OptFixedLayout   = uint32(C.KR_OPT_FIXED_LAYOUT)
+	OptIncremental   = uint32(C.KR_OPT_INCREMENTAL)
+	OptLargeClusters = uint32(C.KR_OPT_LARGE_CLUSTERS)
+)
+
+// SetOption: KR_OPT_FIXED_LAYOUT (before the first Begin), KR_OPT_INCREMENTAL, KR_OPT_LARGE_CLUSTERS (1: RayClusters of 257 to
+// KR_LARGE_MAX_PODS pods stay on the bucket pipeline and keep incremental epochs; recommended for fleets that have them; takes
+// effect at the next full pass).  For a Packer, call it on Packer.Engine().
 func (e *Engine) SetOption(option uint32, value uint64) error {
 	if rc := C.kr_engine_set_option(e.h, C.uint32_t(option), C.uint64_t(value)); rc != C.KR_OK {
 		return e.err(rc)

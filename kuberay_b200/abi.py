@@ -82,6 +82,9 @@ SVCIP_NORMAL, SVCIP_EMPTY, SVCIP_NONE = 0, 1, 2
 PART_COLUMNS, PART_JSON, PART_ALL, PART_OBJECTS = 1, 2, 3, 4
 OPT_FIXED_LAYOUT = 1
 OPT_INCREMENTAL = 2
+OPT_LARGE_CLUSTERS = 3
+OPT_BUCKET_STRIDE = 4
+LARGE_MAX_PODS = 8192
 SPEC_JSON_UNMUTED = 1
 KR_OK, KR_E_INVALID, KR_E_CAPACITY, KR_E_CUDA, KR_E_STATE, KR_E_NO_DEVICE = 0, -1, -2, -3, -4, -5
 MAX_KERNEL_TIMES = 24
@@ -299,7 +302,7 @@ class kr_oracle_out(C.Structure):  # oracle/kr_oracle.h (test infrastructure; de
 
 # every symbol include/kr_engine.h declares
 ENGINE_SYMBOLS = [
-    "kr_device_count", "kr_engine_create", "kr_engine_destroy", "kr_snapshot_begin", "kr_snapshot_commit", "kr_snapshot_commit_parts", "kr_snapshot_commit_pod_rows", "kr_snapshot_commit_pod_values", "kr_snapshot_commit_object_rows", "kr_engine_set_option",
+    "kr_device_count", "kr_engine_create", "kr_engine_destroy", "kr_snapshot_begin", "kr_snapshot_commit", "kr_snapshot_commit_parts", "kr_snapshot_commit_pod_rows", "kr_snapshot_commit_pod_values", "kr_snapshot_commit_object_rows", "kr_engine_set_option", "kr_engine_get_option",
     "kr_reconcile_batch", "kr_reconcile_device_only", "kr_reconcile_batch_profiled", "kr_results_fetch",
     "kr_hash_batch", "kr_last_profile", "kr_group_results_device", "kr_group_results_copy", "kr_last_error", "kr_algorithmic_bytes",
     "kr_spec_json_emit", "kr_spec_json_emit_arena", "kr_quantity_canonical", "kr_spec_json_last_error", "kr_hash_compare_batch",

@@ -34,6 +34,21 @@ __device__ __forceinline__ uint32_t inc_epoch_of(const ScratchDev &sc) { return 
 static constexpr int kD2Warps = KR_D2WARPS;  // RayClusters per k_decide2 CTA
 #define KR_ROW_UNHEALTHY (1u << 13)  // bucket record word: shouldDeletePod(pod) (k_match2 evaluates it once per pod)
 #define KR_ROW_FRESH (1u << 14)      // bucket record word: appended by k_inc_admit in the running incremental epoch (cleared by the decide warp)
+#define KR_LG_OWNED (1u << 31)       // lg[c].w: k_large_sort took the RayCluster this pass (the low bits are its kept pod count)
+
+// Where the record of arrival rank `rank` >= bucket_stride of RayCluster c goes: its region of the large-cluster arena
+// (KR_OPT_LARGE_CLUSTERS, kr_large.cuh), which holds ranks [stride, stride + capacity).  nullptr: no room (an ordinary RayCluster,
+// or a large one that outgrew its region): the attempt is void.  Ranks below the stride stay in the cluster's bucket, so an
+// ordinary pod never reaches this lookup.
+__device__ __forceinline__ uint4 *large_slot(const ScratchDev &sc, uint32_t c, uint32_t rank) {
+  if (!sc.lg) return nullptr;
+  const uint4 l = __ldcg(&sc.lg[c]);
+  const uint32_t j = rank - sc.bucket_stride;
+  return j < l.y ? sc.region + l.x + j : nullptr;
+}
+__device__ __forceinline__ uint4 *rec_slot(const ScratchDev &sc, uint32_t c, uint32_t rank) {
+  return rank < sc.bucket_stride ? sc.bucket + (size_t)c * sc.bucket_stride + rank : large_slot(sc, c, rank);
+}
 
 
 // ------------------------------------------------------------------------------------------------ k_match2
@@ -152,7 +167,10 @@ __global__ void __launch_bounds__(kSortThreads) k_match2(SnapDev s, ScratchDev s
     if (rank[it] < sc.bucket_stride) {
       sc.bucket[(size_t)cidx[it] * sc.bucket_stride + rank[it]] = make_uint4(base + it * 32, roww[it], ri[it], nm[it]);
       sc.pos[base + it * 32] = rank[it];  // (coalesced; incremental epochs rewrite a row's record in place)
-    } else KR_MARK_ATTEMPT_VOID(r.totals);  // the engine reruns the pass with a wider stride / on the sort pipeline
+    } else if (uint4 *slot = large_slot(sc, cidx[it], rank[it])) {
+      *slot = make_uint4(base + it * 32, roww[it], ri[it], nm[it]);
+      sc.pos[base + it * 32] = rank[it];
+    } else KR_MARK_ATTEMPT_VOID(r.totals);  // the engine reruns the pass with a wider stride / large regions / on the sort pipeline
   }
   // pods that match no RayCluster of the snapshot (free rows of an incrementally maintained arena are not orphans)
   if (lane == 0) s_orph[warp] = orphans;
@@ -180,6 +198,30 @@ struct Decide2Args {
   int phase;  // 0: every RayCluster; 1: only the clusters phase 0 deferred (Recreate gate waiting for the hash kernel);
               // 2: only the clusters an incremental epoch marked dirty (kr_incr.cuh) — digests resident, places reused while they suffice
 };
+
+// Incremental epochs: the records of RayCluster c (entry i of the dirty list) as they now stand in the result arrays, packed at its
+// place in the staging buffer by one warp (the host copies the whole arrays instead when the list outgrew the staging area).
+__device__ __forceinline__ void stage_cluster(const Decide2Args &a, uint32_t i, uint32_t c, uint32_t act_off, uint32_t n_act, uint32_t g0, uint32_t G, uint32_t lane) {
+  const uint32_t n_dirty = __ldcg(&a.sc.inc[KR_INC_DIRTY]);
+  if (n_dirty > a.st.cap_clusters) return;
+  uint32_t at = 0;
+  if (lane == 0) at = atomicAdd(&a.sc.inc[KR_INC_GROUPS], G);
+  at = __shfl_sync(0xFFFFFFFFu, at, 0);
+  if (lane == 0) {
+    uint32_t *m = a.st.meta + 8 * (size_t)i;
+    m[0] = c; m[1] = act_off; m[2] = n_act; m[3] = g0; m[4] = G; m[5] = at; m[6] = 0; m[7] = 0;
+  }
+  static_assert(sizeof(kr_cluster_result) % 4 == 0 && sizeof(kr_cluster_result) / 4 <= 32 && sizeof(kr_group_result) % 4 == 0, "record sizes");
+  const uint32_t *csrc = reinterpret_cast<const uint32_t *>(&a.r.clusters[c]);
+  uint32_t *cdst = reinterpret_cast<uint32_t *>(&a.st.clusters[i]);
+  if (lane < sizeof(kr_cluster_result) / 4) cdst[lane] = __ldcg(csrc + lane);
+  if ((uint64_t)at + G <= a.st.cap_groups) {
+    const uint32_t words = G * (uint32_t)(sizeof(kr_group_result) / 4);
+    const uint32_t *gsrc = reinterpret_cast<const uint32_t *>(&a.r.groups[g0]);
+    uint32_t *gdst = reinterpret_cast<uint32_t *>(&a.st.groups[at]);
+    for (uint32_t w = lane; w < words; w += 32) gdst[w] = __ldcg(gsrc + w);
+  }
+}
 
 // reconcileMultiHostWorkerGroup (raycluster_controller.go:963-1125) for worker group `gi` of the warp's RayCluster, from the
 // registers of k_decide2 — the decisions of decide_multihost (kr_decide.cuh), which the sort pipeline takes, bit for bit.
@@ -816,30 +858,8 @@ __global__ void __launch_bounds__(kD2Warps * 32, (K <= 4 && !kMH ? 32 : 16) / kD
     for (uint32_t gi = lane; gi < G; gi += 32) { a.r.groups[g0 + gi].create_off = create_off; a.sc.gcreate[g0 + gi] = create_off; }
   }
   if (kInc) {
-    // the cluster's records as they now stand in the result arrays, packed at its place in the dirty list (the host copies the whole
-    // arrays instead when the list outgrew the staging area)
-    __syncwarp();  // this warp's own stores to r.clusters / r.groups above are ordered before the loads below
-    const uint32_t n_dirty = __ldcg(&a.sc.inc[KR_INC_DIRTY]);
-    if (n_dirty <= a.st.cap_clusters) {
-      const uint32_t i = blockIdx.x * kD2Warps + warp;
-      uint32_t at = 0;
-      if (lane == 0) at = atomicAdd(&a.sc.inc[KR_INC_GROUPS], G);
-      at = __shfl_sync(0xFFFFFFFFu, at, 0);
-      if (lane == 0) {
-        uint32_t *m = a.st.meta + 8 * (size_t)i;
-        m[0] = c; m[1] = act_off; m[2] = n_act; m[3] = g0; m[4] = G; m[5] = at; m[6] = 0; m[7] = 0;
-      }
-      static_assert(sizeof(kr_cluster_result) % 4 == 0 && sizeof(kr_cluster_result) / 4 <= 32 && sizeof(kr_group_result) % 4 == 0, "record sizes");
-      const uint32_t *csrc = reinterpret_cast<const uint32_t *>(&a.r.clusters[c]);
-      uint32_t *cdst = reinterpret_cast<uint32_t *>(&a.st.clusters[i]);
-      if (lane < sizeof(kr_cluster_result) / 4) cdst[lane] = __ldcg(csrc + lane);
-      if ((uint64_t)at + G <= a.st.cap_groups) {
-        const uint32_t words = G * (uint32_t)(sizeof(kr_group_result) / 4);
-        const uint32_t *gsrc = reinterpret_cast<const uint32_t *>(&a.r.groups[g0]);
-        uint32_t *gdst = reinterpret_cast<uint32_t *>(&a.st.groups[at]);
-        for (uint32_t w = lane; w < words; w += 32) gdst[w] = __ldcg(gsrc + w);
-      }
-    }
+    __syncwarp();  // this warp's own stores to r.clusters / r.groups above are ordered before the loads of the staging copy
+    stage_cluster(a, blockIdx.x * kD2Warps + warp, c, act_off, n_act, g0, G, lane);
   }
 }
 

@@ -97,6 +97,9 @@ struct ScratchDev {
   uint32_t *dirty_list;                                        // [n_clusters] RayClusters to decide again, count in inc[KR_INC_DIRTY]
   uint32_t *act_res, *cre_res;                                 // [n_clusters] places the cluster holds in the action list / create arena (reused while they suffice)
   uint32_t *inc;                                               // [16] counters / flags of the running epoch (KR_INC_*)
+  // large RayClusters (KR_OPT_LARGE_CLUSTERS, kr_large.cuh): records of arrival rank >= bucket_stride go to the cluster's region
+  uint4 *lg;                                                   // [n_clusters] {region offset, region capacity (0: not large), scratch segment, kept pods | KR_LG_OWNED}; nullptr: none
+  uint4 *region;                                               // large-cluster record arena (16-byte bucket records)
 };
 enum {
   KR_INC_TOUCHED = 0, KR_INC_DIRTY = 1,
@@ -105,6 +108,7 @@ enum {
   KR_INC_HEADS = 4,        // the pod idx -> head-aux row table must be rebuilt
   KR_INC_VOID = 5,         // the incremental attempt is void (a bucket or an arena overflowed): take a full pass
   KR_INC_GROUPS = 6,       // gather: group records staged so far
+  KR_INC_LSEG = 7,         // large RayClusters: scratch positions handed out so far (k_large_sort)
 };
 // words of a cl_in record (built by k_build_tables; k_decide2 loads it with one coalesced 128-byte access, lane i = word i)
 enum {

@@ -20,6 +20,7 @@
 
 #include "kr_kernels.cuh"
 #include "kr_incr.cuh"
+#include "kr_large.cuh"
 
 using namespace kr;
 
@@ -31,6 +32,15 @@ namespace {
 constexpr size_t kAlign = 256;
 inline size_t align_up(size_t x, size_t a = kAlign) { return (x + a - 1) / a * a; }
 inline uint32_t pow2_at_least(uint64_t x) { uint32_t p = 16; while (p < x) p <<= 1; return p; }
+
+// bucket stride of a new layout: a power of two with 25 % head room over the mean cluster size (a cluster that outgrows it voids the
+// attempt; the pass then widens the stride, up to 256, or leaves the bucket pipeline for this layout)
+uint32_t first_stride(const kr_sizes &n) {
+  uint32_t st = 64;
+  const uint64_t want = n.n_clusters ? ((uint64_t)n.n_pods * 5 / 4 + n.n_clusters - 1) / n.n_clusters : 0;
+  while (st < want && st < 512) st <<= 1;
+  return st <= 256 ? st : 0;
+}
 
 struct InLayout {  // offsets of every input column inside the snapshot arena
   size_t off[64];
@@ -258,6 +268,13 @@ struct kr_engine {
   uint8_t *orow_h = nullptr, *orow_d = nullptr; size_t orow_cap = 0;  // kr_snapshot_commit_object_rows staging
   cudaEvent_t ev_orow = nullptr; bool orow_busy = false;
   uint32_t bstride = 0;         // bucket stride of this layout (64 / 128 / 256); 0 = the layout does not qualify (a cluster outgrew 256 pods, ...)
+  bool large_on = false;        // KR_OPT_LARGE_CLUSTERS
+  uint32_t n_large = 0;         // ... RayClusters of this layout with a region, sticky like bstride
+  // KR_OPT_LARGE_CLUSTERS arena, allocated when the option is first turned on (an engine without it pays nothing), sized for the
+  // capacities so that it never grows: [lg: 16 B x max_clusters | lg_list: 4 B x max_clusters | regions: 16 B x large_entries]
+  uint8_t *d_large = nullptr;
+  size_t large_entries = 0;
+  std::vector<uint4> h_lg; std::vector<uint32_t> h_lg_list;  // host side of the last upload (kept alive while it is in flight)
   bool snap_has_mh = false;     // some worker group has numOfHosts > 1
   std::vector<uint8_t> mh_bit;  // ... per cluster row, as of the last commit (kr_snapshot_commit_object_rows keeps snap_has_mh current with it)
   uint32_t snap_max_groups = 0; // most worker groups in one RayCluster
@@ -374,6 +391,7 @@ ScratchDev bind_scratch(const ScratchLayout &L, uint8_t *b) {
   s.dirty_flag = reinterpret_cast<uint32_t *>(b + L.dirty_flag); s.dirty_list = reinterpret_cast<uint32_t *>(b + L.dirty_list);
   s.act_res = reinterpret_cast<uint32_t *>(b + L.act_res); s.cre_res = reinterpret_cast<uint32_t *>(b + L.cre_res);
   s.inc = reinterpret_cast<uint32_t *>(b + L.inc);
+  s.lg = nullptr; s.region = nullptr;  // (set by the pass when the layout has large RayClusters: bind_large)
   return s;
 }
 
@@ -389,6 +407,15 @@ cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t sme
   return cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
 }
 
+// Points the pass at the large-cluster arena when the layout has large RayClusters; returns the device list of their rows.
+const uint32_t *bind_large(const kr_engine *e, ScratchDev &sc) {
+  if (!e->n_large) return nullptr;
+  const size_t Nc = e->cfg.max_clusters;
+  sc.lg = reinterpret_cast<uint4 *>(e->d_large);
+  sc.region = reinterpret_cast<uint4 *>(e->d_large + align_up(16 * Nc) + align_up(4 * Nc));
+  return reinterpret_cast<const uint32_t *>(e->d_large + align_up(16 * Nc));
+}
+
 // Launches the whole pass.  profile: serialise everything on stream M and bracket each kernel with events.
 int launch_pass(kr_engine *e, const kr_flags &f, bool profile, bool capturing = false) {
   const kr_sizes &n = e->sizes;
@@ -396,6 +423,7 @@ int launch_pass(kr_engine *e, const kr_flags &f, bool profile, bool capturing = 
   bind_in(e->il, e->d_in, &s);
   ResDev r = bind_out(e->ol, e->d_out);
   ScratchDev sc = bind_scratch(e->sl, e->d_scratch);
+  const uint32_t *lg_list = bind_large(e, sc);
   Sizes z{n.n_clusters, n.n_groups, n.n_wtd, n.n_pods, n.n_heads, n.n_jobs};
   cudaStream_t M = e->sm, H = profile ? e->sm : e->sh;
   int k = 0;
@@ -486,12 +514,15 @@ int launch_pass(kr_engine *e, const kr_flags &f, bool profile, bool capturing = 
       CK(launch_decide2(dim3((n.n_clusters + kD2Warps - 1) / kD2Warps), pdl && n.n_pods != 0));
     } else CK(cudaMemsetAsync(r.act_start, 0, 4, M));
     if (n.n_jobs) { mark("k_jobs"); k_jobs<<<(n.n_jobs + 255) / 256, 256, 0, M>>>(s, sc, r, z); }
+    const bool large = e->n_large && sc.lg && n.n_clusters;  // large RayClusters (kr_large.cuh): sorted beside the hash, decided after it
+    if (large) { mark("k_large_sort"); k_large_sort<false><<<e->n_large, kLargeSortThreads, 0, M>>>(da, lg_list); }
     if (profile) {
       if (do_hash) { mark("k_hash"); launch_hash(); }
       else if (n.n_clusters) CK(cudaMemsetAsync(r.hash, 0, 32 * (size_t)n.n_clusters, M));
     } else {
       CK(cudaStreamWaitEvent(M, e->ev_hash, 0));
     }
+    if (large) { mark("k_decide_large"); k_decide_large<false><<<e->n_large, kLargeDecideThreads, 0, M>>>(da, lg_list); }
     if (e->n_recreate > 0 && do_hash && !spin) {  // clusters whose Recreate gate needs the digest: decided again, in the places phase 0 reserved
       da.phase = 1;
       mark("k_decide2_phase1");
@@ -642,6 +673,45 @@ int run_pass_once(kr_engine *e, const kr_flags &f) {
 }
 
 
+// A bucket attempt voided: some RayCluster listed more pods than the stride holds (k_match2 counted them all in cl_dyn[].x) or
+// outgrew its region.  Widen the stride (64 -> 128 -> 256) or leave the bucket pipeline for this layout; with KR_OPT_LARGE_CLUSTERS
+// the RayClusters of more than 256 (and at most KR_LARGE_MAX_PODS) pods get regions instead, and only the others widen the stride.
+int after_bucket_void(kr_engine *e) {
+  const uint32_t Nc = e->sizes.n_clusters;
+  auto fits = [&](uint32_t st) { return st <= 256 && (size_t)Nc * st <= e->sl.bucket_entries; };
+  e->n_large = 0;  // (rebuilt below from this attempt's counts)
+  if (!e->large_on) { e->bstride = fits(e->bstride * 2) ? e->bstride * 2 : 0; return KR_OK; }
+  std::vector<uint4> dyn(Nc);
+  CK(cudaMemcpyAsync(dyn.data(), e->d_scratch + e->sl.cl_dyn, 16 * (size_t)Nc, cudaMemcpyDeviceToHost, e->sm));
+  CK(cudaStreamSynchronize(e->sm));
+  uint32_t st = e->bstride, n_big = 0, most = 0;
+  for (const uint4 &d : dyn) { if (d.x > 256) n_big++; if (d.x <= 256) most = std::max(most, d.x); }
+  for (const uint4 &d : dyn) if (d.x > KR_LARGE_MAX_PODS) { e->bstride = 0; return KR_OK; }  // the sort / radix pipelines take it, as before
+  if (n_big == 0) { e->bstride = fits(st * 2) ? st * 2 : 0; return KR_OK; }
+  while (st < most && fits(st * 2)) st <<= 1;
+  if (st < most) { e->bstride = 0; return KR_OK; }
+  // regions: ranks [st, st + cap) of every large cluster, cap = 1.25x its pods rounded up to 32, less the stride
+  std::vector<uint4> lg(Nc, make_uint4(0, 0, 0, 0));
+  std::vector<uint32_t> list;
+  size_t off = 0;
+  for (uint32_t c = 0; c < Nc; c++) {
+    if (dyn[c].x <= 256) continue;
+    const uint32_t want = ((dyn[c].x + dyn[c].x / 4 + 31) / 32) * 32;
+    const uint32_t cap = std::min<uint32_t>(want, KR_LARGE_MAX_PODS) - st;
+    lg[c] = make_uint4((uint32_t)off, cap, 0, 0);
+    list.push_back(c);
+    off += cap;
+  }
+  if (off > e->large_entries) { e->bstride = 0; return KR_OK; }
+  // on the pass's stream (ordered before the rerun); the host copies stay alive until the stream has consumed them (the stream
+  // was synchronised above, so the previous upload is done)
+  e->h_lg.swap(lg); e->h_lg_list.swap(list);
+  CK(cudaMemcpyAsync(e->d_large, e->h_lg.data(), 16 * (size_t)Nc, cudaMemcpyHostToDevice, e->sm));
+  CK(cudaMemcpyAsync(e->d_large + align_up(16 * (size_t)e->cfg.max_clusters), e->h_lg_list.data(), 4 * e->h_lg_list.size(), cudaMemcpyHostToDevice, e->sm));
+  e->n_large = (uint32_t)e->h_lg_list.size();
+  e->bstride = st;
+  return KR_OK;
+}
 // a bucket-pipeline pass leaves everything an incremental epoch needs on the device
 void after_full_pass(kr_engine *e, const kr_flags &f) {
   // (a pass whose create runs overran kr_config.max_creates is reported as KR_E_CAPACITY and left groups' runs unwritten: an
@@ -662,6 +732,7 @@ int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile
   ResDev r = bind_out(e->ol, e->d_out);
   ScratchDev sc = bind_scratch(e->sl, e->d_scratch);
   sc.bucket_stride = e->bstride;
+  const uint32_t *lg_list = bind_large(e, sc);
   Sizes z{n.n_clusters, n.n_groups, n.n_wtd, n.n_pods, n.n_heads, n.n_jobs};
   cudaStream_t M = e->sm, H = profile ? e->sm : e->sh;
   int k = 0;
@@ -722,6 +793,13 @@ int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile
     if (e->bstride <= 64) (mh ? k_decide2<2, true, true> : k_decide2<2, true>)<<<dgrid, dblock, 0, M>>>(da);
     else if (e->bstride <= 128) (mh ? k_decide2<4, true, true> : k_decide2<4, true>)<<<dgrid, dblock, 0, M>>>(da);
     else (mh ? k_decide2<8, true, true> : k_decide2<8, true>)<<<dgrid, dblock, 0, M>>>(da);
+    if (e->n_large) {  // the dirty large RayClusters (k_decide2 left every cluster past the stride alone)
+      CK(cudaMemsetAsync(sc.inc + KR_INC_LSEG, 0, 4, M));
+      mark("k_large_sort");
+      k_large_sort<true><<<e->n_large, kLargeSortThreads, 0, M>>>(da, lg_list);
+      mark("k_decide_large");
+      k_decide_large<true><<<e->n_large, kLargeDecideThreads, 0, M>>>(da, lg_list);
+    }
   }
   if (n.n_jobs) { mark("k_jobs"); k_jobs<<<(n.n_jobs + 255) / 256, 256, 0, M>>>(s, sc, r, z); }
   if (profile && k <= KR_MAX_KERNEL_TIMES) cudaEventRecord(e->ev_k[k < KR_MAX_KERNEL_TIMES ? k : KR_MAX_KERNEL_TIMES], M);
@@ -788,8 +866,7 @@ int run_pass(kr_engine *e, const kr_flags &f, cudaEvent_t done) {
     if (!(e->h_totals[3] & KR_TOTALS_BIG_BUCKET)) { after_full_pass(e, f); return KR_OK; }
     // some RayCluster outgrew what this pipeline holds per bucket: bucket pipeline -> wider stride -> sort pipeline -> radix pipeline
     if (e->ran_bucket) {
-      const uint32_t wider = e->bstride * 2;
-      e->bstride = (wider <= 256 && (size_t)e->sizes.n_clusters * wider <= e->sl.bucket_entries) ? wider : 0;
+      if (int rc = after_bucket_void(e)) return rc;
     } else if (e->ran_fast) e->force_radix = true;
     else break;
     e->gvalid = false;
@@ -925,7 +1002,38 @@ int kr_engine_set_option(kr_engine *e, uint32_t option, uint64_t value) {
     if (e->no_incr) e->inc_valid = false;
     return KR_OK;
   }
+  if (option == KR_OPT_LARGE_CLUSTERS) {
+    if (e->large_on == (value != 0)) return KR_OK;
+    if (value && !e->d_large) {
+      // every region holds about 1.25x its cluster's pods rounded up to 32 records, and a large cluster lists more than 256 pods:
+      // this many records hold the regions of any snapshot within the capacities
+      const size_t Nc = e->cfg.max_clusters, Np = e->cfg.max_pods;
+      const size_t entries = Np * 5 / 4 + 32 * (Np / 257 + 1);
+      CK(cudaSetDevice(e->cfg.device));
+      CK(cudaMalloc((void **)&e->d_large, align_up(16 * Nc) + align_up(4 * Nc) + 16 * entries));
+      e->large_entries = entries;
+    }
+    e->large_on = value != 0;
+    // the next full pass starts again from the layout's first stride and the fast sort pipeline: a pass with the option off may
+    // have left the bucket pipeline (and the fast pipeline, for a cluster above 1024 pods) for this layout
+    e->n_large = 0; e->inc_valid = false; e->gvalid = false;
+    e->force_radix = e->env_radix;
+    if (e->begun) e->bstride = first_stride(e->sizes);
+    return KR_OK;
+  }
+  if (option == KR_OPT_BUCKET_STRIDE) return fail(e, KR_E_INVALID, "KR_OPT_BUCKET_STRIDE can only be read");
   return fail(e, KR_E_INVALID, "unknown option %u", option);
+}
+
+int kr_engine_get_option(kr_engine *e, uint32_t option, uint64_t *value) {
+  if (!e || !value) return KR_E_INVALID;
+  switch (option) {
+    case KR_OPT_FIXED_LAYOUT: *value = e->fixed_layout; return KR_OK;
+    case KR_OPT_INCREMENTAL: *value = !e->no_incr; return KR_OK;
+    case KR_OPT_LARGE_CLUSTERS: *value = e->large_on; return KR_OK;
+    case KR_OPT_BUCKET_STRIDE: *value = e->bstride; return KR_OK;
+    default: return fail(e, KR_E_INVALID, "unknown option %u", option);
+  }
 }
 
 int kr_device_count(void) {
@@ -994,7 +1102,8 @@ int kr_engine_create(const kr_config *cfg, kr_engine **out) {
                         (const void *)k_inc_retire, (const void *)k_inc_objects, (const void *)k_inc_objects_keys, (const void *)k_inc_aux_clear, (const void *)k_inc_aux_insert,
                         (const void *)k_inc_mark_recreate, (const void *)k_decide2<2, true>, (const void *)k_decide2<4, true>, (const void *)k_decide2<8, true>, (const void *)k_inc_refresh, (const void *)k_inc_admit,
                         (const void *)k_inc_finish, (const void *)k_decide2<2, false, true>, (const void *)k_decide2<4, false, true>, (const void *)k_decide2<8, false, true>,
-                        (const void *)k_decide2<2, true, true>, (const void *)k_decide2<4, true, true>, (const void *)k_decide2<8, true, true>};
+                        (const void *)k_decide2<2, true, true>, (const void *)k_decide2<4, true, true>, (const void *)k_decide2<8, true, true>,
+                        (const void *)k_large_sort<false>, (const void *)k_large_sort<true>, (const void *)k_decide_large<false>, (const void *)k_decide_large<true>};
     for (const void *k : ks) cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, pct);
   }
   if (const char *g = getenv("KR_NO_GRAPH")) e->use_graph = !(g[0] == '1');
@@ -1049,6 +1158,7 @@ void kr_engine_destroy(kr_engine *e) {
   if (e->h_inc_stage) cudaFreeHost(e->h_inc_stage);
   if (e->d_inc_stage) cudaFree(e->d_inc_stage);
   if (e->d_obj_stage) cudaFree(e->d_obj_stage);
+  if (e->d_large) cudaFree(e->d_large);
   if (e->d_order) cudaFree(e->d_order);
   if (e->ev_order) cudaEventDestroy(e->ev_order);
   if (e->d_in) cudaFree(e->d_in);
@@ -1093,12 +1203,8 @@ int kr_snapshot_begin(kr_engine *e, const kr_sizes *sizes, kr_snapshot_bufs *out
     if (!keep) {
       e->inc_valid = false;
       e->force_radix = e->env_radix;
-      // bucket stride: a power of two with 25 % head room over the mean cluster size (a cluster that outgrows it voids the
-      // attempt; the pass then widens the stride, up to 256, or leaves the bucket pipeline for this layout)
-      uint32_t st = 64;
-      const uint64_t want = sizes->n_clusters ? ((uint64_t)sizes->n_pods * 5 / 4 + sizes->n_clusters - 1) / sizes->n_clusters : 0;
-      while (st < want && st < 512) st <<= 1;
-      e->bstride = st <= 256 ? st : 0;
+      e->bstride = first_stride(*sizes);
+      e->n_large = 0;
     }
   }
   e->sizes = *sizes;
@@ -1542,8 +1648,7 @@ int kr_reconcile_batch_profiled(kr_engine *e, const kr_flags *flags, kr_profile 
     if (!(e->h_totals[3] & KR_TOTALS_BIG_BUCKET)) { after_full_pass(e, *flags); break; }
     if (attempt >= 4) return fail(e, KR_E_STATE, "internal: radix pipeline flagged a big bucket");
     if (e->ran_bucket) {
-      const uint32_t wider = e->bstride * 2;
-      e->bstride = (wider <= 256 && (size_t)e->sizes.n_clusters * wider <= e->sl.bucket_entries) ? wider : 0;
+      if (int rc = after_bucket_void(e)) return rc;
     } else if (e->ran_fast) e->force_radix = true;
     e->gvalid = false;
   }

@@ -233,7 +233,9 @@ __global__ void __launch_bounds__(256) k_inc_admit(SnapDev s, ScratchDev sc, Res
     if (matched && c == c_old) {
       // the usual event — a status update: the row stays in its RayCluster, its record is rewritten where it sits and the row's
       // stamp is lifted (nothing of this cluster has to be dropped on its account)
-      sc.bucket[(size_t)c * sc.bucket_stride + sc.pos[p]] = make_uint4(p, (slot << 16) | flags, ri, nm);
+      uint4 *at = rec_slot(sc, c, sc.pos[p]);  // (a record of a large RayCluster may sit in its region)
+      if (!at) { sc.inc[KR_INC_VOID] = 1u; continue; }
+      *at = make_uint4(p, (slot << 16) | flags, ri, nm);
       sc.stamp[p] = 0u;
       continue;  // (k_inc_retire marked the cluster dirty)
     }
@@ -244,8 +246,8 @@ __global__ void __launch_bounds__(256) k_inc_admit(SnapDev s, ScratchDev sc, Res
     }
     mark_dirty(sc, c, epoch);  // the row joined this cluster: a fresh record at the end of its bucket
     const uint32_t rank = atomicAdd(&sc.cl_dyn[c].x, 1u);
-    if (rank < sc.bucket_stride) { sc.bucket[(size_t)c * sc.bucket_stride + rank] = make_uint4(p, (slot << 16) | flags | KR_ROW_FRESH, ri, nm); sc.pos[p] = rank; }
-    else sc.inc[KR_INC_VOID] = 1u;
+    if (uint4 *at = rec_slot(sc, c, rank)) { *at = make_uint4(p, (slot << 16) | flags | KR_ROW_FRESH, ri, nm); sc.pos[p] = rank; }
+    else sc.inc[KR_INC_VOID] = 1u;  // (an ordinary RayCluster outgrew its bucket, a large one its region: the full pass reclassifies)
   }
 }
 
@@ -255,7 +257,7 @@ __global__ void __launch_bounds__(256) k_inc_admit(SnapDev s, ScratchDev sc, Res
 // closes the epoch (after the host's copy of the counters was enqueued): next epoch's stamps differ from every stamp written so far
 __global__ void k_inc_finish(ScratchDev sc) {
   if (threadIdx.x == 0 && blockIdx.x == 0) {
-    sc.inc[KR_INC_TOUCHED] = 0; sc.inc[KR_INC_DIRTY] = 0; sc.inc[KR_INC_STRUCTURAL] = 0; sc.inc[KR_INC_HEADS] = 0; sc.inc[KR_INC_VOID] = 0; sc.inc[KR_INC_GROUPS] = 0;
+    sc.inc[KR_INC_TOUCHED] = 0; sc.inc[KR_INC_DIRTY] = 0; sc.inc[KR_INC_STRUCTURAL] = 0; sc.inc[KR_INC_HEADS] = 0; sc.inc[KR_INC_VOID] = 0; sc.inc[KR_INC_GROUPS] = 0; sc.inc[KR_INC_LSEG] = 0;
     sc.inc[KR_INC_EPOCH] += 1u;
   }
 }

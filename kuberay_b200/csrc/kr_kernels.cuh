@@ -18,6 +18,8 @@
 //                    + consumer warp (the 80-round chain) per 32 messages, messages ordered by block count   [> 19 k messages: k_hash2<4,1>]
 //   k_decide2 ph. 1  the clusters whose Recreate gate needs the digest, in the places phase 0 reserved
 //   k_jobs           RayJob -> RayCluster status roll-up join
+//   k_large_sort / k_decide_large   KR_OPT_LARGE_CLUSTERS only (kr_large.cuh): the RayClusters of 257..KR_LARGE_MAX_PODS pods, one
+//                    CTA each — List order by a shared-memory sort beside the hash, then the sort pipeline's memory-resident decide
 // When the caller asks for the full per-cluster pod lists (fetch_pod_lists == 1) or the snapshot does not qualify — the SORT pipeline:
 //   k_match -> k_place_fused -> k_decide_small (+ k_decide on a side stream) -> [phase 1] -> k_creates_fused
 //   (buckets restored to List order by an in-register bitonic sort), and for RayClusters with > 1024 pods the RADIX pipeline

@@ -1,0 +1,196 @@
+// kr_large.cuh — large RayClusters on the bucket pipeline (KR_OPT_LARGE_CLUSTERS): more than 256 and at most KR_LARGE_MAX_PODS pods.
+// Part of the sm_90a kernel set of the batched reconcile engine; see kr_kernels.cuh for the pipeline overview.
+//
+// The engine classifies them on the host after a bucket attempt that voided (k_match2 counts every cluster's pods past the stride)
+// and gives each one a region of the large-cluster record arena: k_match2 and k_inc_admit put the records of arrival rank
+// >= bucket_stride there (rec_slot, kr_bucket2.cuh), so the rest of the fleet keeps its stride and an ordinary pod never looks at
+// the region table.  k_decide2 leaves every cluster whose count exceeds the stride alone; these two kernels, one CTA per large
+// RayCluster, decide them instead:
+//   k_large_sort    (beside the hash) loads the cluster's records, drops the stale ones of an incremental epoch and stores the rest
+//                   back compacted, writes each pod's 16-byte row (what the memory-resident decide reads), sorts the pod indices
+//                   into List order in shared memory and publishes them at a scratch segment (sorted_pod_idx);
+//   k_decide_large  (after the join with the hash stream: a Recreate gate reads a finished digest) decides the cluster with the
+//                   memory-resident warp decide of the sort pipeline (decide_cluster<0, true>), reserves its action run and create
+//                   run at the bucket pipeline's cursors, moves the actions into place and fills the replica indices.
+// Two kernels, because decide_cluster reads sorted_pod_idx and the rows through the read-only cache, which is only coherent with
+// stores of an earlier grid.
+#pragma once
+
+#include "kr_incr.cuh"
+
+namespace kr {
+
+static constexpr int kLargeSortThreads = 512;
+static constexpr int kLargeDecideThreads = 128;
+
+// One CTA per large RayCluster (lg_list).  kInc: only the ones the epoch marked dirty.
+template <bool kInc>
+__global__ void __launch_bounds__(kLargeSortThreads) k_large_sort(Decide2Args a, const uint32_t *__restrict__ lg_list) {
+  __shared__ uint32_t s_idx[KR_LARGE_MAX_PODS];
+  __shared__ uint32_t s_warp[kLargeSortThreads / 32];
+  __shared__ uint32_t s_seg;
+  const ScratchDev &sc = a.sc;
+  const uint32_t c = lg_list[blockIdx.x];
+  const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const uint32_t S = sc.bucket_stride;
+  const uint32_t epoch = kInc ? inc_epoch_of(sc) : 0u;
+  const uint4 dyn = __ldcg(&sc.cl_dyn[c]);
+  const uint32_t P = dyn.x;
+  if (tid == 0) {  // (decided once for the CTA: other CTAs may flag the attempt void meanwhile)
+    const uint32_t cap = __ldcg(&sc.lg[c].y);
+    sc.lg[c].w = 0;  // not taken (yet) this pass
+    bool go = !KR_ATTEMPT_VOID(a.r.totals);
+    if (kInc) go = go && !__ldcg(&sc.inc[KR_INC_VOID]) && !__ldcg(&sc.inc[KR_INC_STRUCTURAL]) && __ldcg(&sc.dirty_flag[c]) == epoch;
+    s_seg = go && P > S && P - S <= cap;  // else k_decide2 decides it (or the attempt is void: k_match2 / k_inc_admit flagged it)
+  }
+  __syncthreads();
+  if (!s_seg) return;
+  const bool lost = kInc && dyn.y == epoch;  // the cluster lost a row this epoch: the records of stamped rows are stale
+  // each thread owns a contiguous run of ranks, so the kept records keep their arrival order
+  const uint32_t per = (P + kLargeSortThreads - 1) / kLargeSortThreads;
+  const uint32_t j0 = min(tid * per, P), j1 = min(j0 + per, P);
+  uint32_t kept = 0;
+  for (uint32_t j = j0; j < j1; j++) {
+    const uint4 rec = __ldcg(rec_slot(sc, c, j));
+    const bool keep = !lost || (rec.y & KR_ROW_FRESH) || __ldcg(&sc.stamp[rec.x]) != epoch;
+    if (keep) { sc.rows[rec.x] = make_uint4(rec.w, a.s.p_replica_name_id[rec.x], rec.z, rec.y & ~KR_ROW_FRESH); kept++; }
+  }
+  // exclusive prefix of the kept counts over the CTA
+  uint32_t x = kept;
+#pragma unroll
+  for (int d = 1; d < 32; d <<= 1) { const uint32_t y = __shfl_up_sync(0xFFFFFFFFu, x, d); if (lane >= (uint32_t)d) x += y; }
+  if (lane == 31) s_warp[warp] = x;
+  __syncthreads();
+  uint32_t before = 0, total = 0;
+  for (uint32_t w = 0; w < kLargeSortThreads / 32; w++) { const uint32_t v = s_warp[w]; before += w < warp ? v : 0u; total += v; }
+  uint32_t o = before + x - kept;
+  for (uint32_t j = j0; j < j1; j++) {
+    const uint4 rec = __ldcg(rec_slot(sc, c, j));
+    const bool keep = !lost || (rec.y & KR_ROW_FRESH) || __ldcg(&sc.stamp[rec.x]) != epoch;
+    if (keep) s_idx[o++] = rec.x;
+  }
+  if (tid == 0) {
+    s_seg = atomicAdd(&sc.inc[KR_INC_LSEG], total);
+    if ((uint64_t)s_seg + total > a.n.n_pods) {  // cannot happen while the regions hold distinct live rows; void rather than overrun
+      if (kInc) sc.inc[KR_INC_VOID] = 1u; else KR_MARK_ATTEMPT_VOID(a.r.totals);
+    }
+  }
+  __syncthreads();  // (also orders every rows[] store of the CTA before the record rewrite below)
+  const uint32_t seg = s_seg;
+  if ((uint64_t)seg + total > a.n.n_pods) return;
+  if (kInc) {
+    // the region (and bucket) compacted in arrival order, FRESH marks cleared; pos[] follows the records that moved
+    for (uint32_t k = tid; k < total; k += kLargeSortThreads) {
+      const uint32_t p = s_idx[k];
+      const uint4 row = sc.rows[p];
+      *rec_slot(sc, c, k) = make_uint4(p, row.w, row.z, row.x);
+      sc.pos[p] = k;
+    }
+    if (tid == 0) { sc.cl_dyn[c].x = total; sc.cl_dyn[c].y = 0u; }
+  }
+  // informer List order = ascending pod index: bitonic sort of the next power of two in shared memory
+  uint32_t n2 = 2;
+  while (n2 < total) n2 <<= 1;
+  for (uint32_t k = total + tid; k < n2; k += kLargeSortThreads) s_idx[k] = 0xFFFFFFFFu;
+  __syncthreads();
+  for (uint32_t size = 2; size <= n2; size <<= 1) {
+    for (uint32_t stride = size >> 1; stride > 0; stride >>= 1) {
+      for (uint32_t t = tid; t < n2 / 2; t += kLargeSortThreads) {
+        const uint32_t lo = 2 * stride * (t / stride) + (t % stride), hi = lo + stride;
+        const bool asc = (lo & size) == 0;
+        const uint32_t u = s_idx[lo], v = s_idx[hi];
+        if ((u > v) == asc) { s_idx[lo] = v; s_idx[hi] = u; }
+      }
+      __syncthreads();
+    }
+  }
+  for (uint32_t k = tid; k < total; k += kLargeSortThreads) a.r.sorted_pod_idx[seg + k] = s_idx[k];
+  if (tid == 0) { sc.lg[c].z = seg; sc.lg[c].w = total | KR_LG_OWNED; }
+}
+
+// One CTA per large RayCluster that k_large_sort took: warp 0 decides, every warp fills replica indices.
+template <bool kInc>
+__global__ void __launch_bounds__(kLargeDecideThreads) k_decide_large(Decide2Args a, const uint32_t *__restrict__ lg_list) {
+  __shared__ int32_t s_acc[4][KR_SMEM_GROUPS];
+  __shared__ int32_t s_mode[2][KR_SMEM_GROUPS];
+  __shared__ uint32_t s_bits[kLargeDecideThreads / 32][32];
+  __shared__ uint32_t s_place[4];  // act_off, n_act, stage index, go on
+  const ScratchDev &sc = a.sc;
+  const ResDev &r = a.r;
+  const uint32_t c = lg_list[blockIdx.x];
+  const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const uint4 l = __ldcg(&sc.lg[c]);  // (written by k_large_sort: an earlier grid)
+  if (!(l.w & KR_LG_OWNED)) return;
+  const uint32_t seg = l.z, P = l.w & ~KR_LG_OWNED;
+  const uint32_t G = a.s.c_group_cnt[c], g0 = a.s.c_group_off[c];
+  if (kInc) {  // this cluster's place in the dirty list (= its entry of the staging buffer)
+    if (tid == 0) s_place[2] = 0xFFFFFFFFu;
+    __syncthreads();
+    const uint32_t n_dirty = __ldcg(&sc.inc[KR_INC_DIRTY]);
+    for (uint32_t i = tid; i < n_dirty; i += kLargeDecideThreads) if (__ldcg(&sc.dirty_list[i]) == c) s_place[2] = i;
+  }
+  if (warp == 0) {
+    // what the cluster holds in the resident results (an incremental epoch keeps its places while they suffice)
+    uint32_t old_create = 0, old_act = 0, old_create_off = 0;
+    if (kInc) {
+      for (uint32_t gi = lane; gi < G; gi += 32) old_create += r.groups[g0 + gi].n_create;
+      old_create = __reduce_add_sync(0xFFFFFFFFu, old_create);
+      old_act = r.act_cnt[c];
+      old_create_off = G ? sc.gcreate[g0] : 0u;
+    }
+    __syncwarp();
+    DecideArgs da{a.s, a.sc, a.r, a.n, a.f, nullptr, nullptr, 0, 1};  // phase 1: the digests are final
+    uint32_t d0[1] = {0}, d1[1] = {0};
+    decide_cluster<0, true>(da, c, seg, seg + P, d0, d1, s_acc, s_mode, lane);
+    __syncwarp();
+    // decide_cluster left n_create per group in gcreate[] and the action count in cact[]
+    uint32_t n_create = 0;
+    for (uint32_t gi = lane; gi < G; gi += 32) n_create += sc.gcreate[g0 + gi];
+    n_create = __reduce_add_sync(0xFFFFFFFFu, n_create);
+    const uint32_t n_act = sc.cact[c];
+    if (lane == 0) {
+      uint32_t act_off, create_off;
+      if (!kInc) {
+        const unsigned long long base = (n_act | n_create) ? atomicAdd(reinterpret_cast<unsigned long long *>(&r.totals[8]), ((unsigned long long)n_create << 32) | n_act) : 0ull;
+        act_off = (uint32_t)base; create_off = (uint32_t)(base >> 32);
+        if (n_create) atomicAdd(&r.totals[6], n_create);
+      } else {
+        const uint32_t need = (n_act > sc.act_res[c] ? 1u : 0u) | (n_create > sc.cre_res[c] ? 2u : 0u);
+        unsigned long long base = 0;
+        if (need) base = atomicAdd(reinterpret_cast<unsigned long long *>(&r.totals[8]), ((unsigned long long)((need & 2u) ? n_create : 0u) << 32) | ((need & 1u) ? n_act : 0u));
+        act_off = (need & 1u) ? (uint32_t)base : r.act_start[c];
+        create_off = (need & 2u) ? (uint32_t)(base >> 32) : old_create_off;
+        if ((need & 1u) && (uint64_t)act_off + n_act > a.n.n_pods) sc.inc[KR_INC_VOID] = 1u;             // the action list is full of abandoned runs:
+        if ((need & 2u) && (uint64_t)create_off + n_create > a.create_cap) sc.inc[KR_INC_VOID] = 1u;  // a full pass packs it again
+        if (need & 1u) sc.act_res[c] = n_act;
+        if (need & 2u) sc.cre_res[c] = n_create;
+        if (old_act) atomicSub(&r.totals[2], old_act);  // (decide_cluster added this pass's n_act)
+        if (n_create != old_create) atomicAdd(&r.totals[6], n_create - old_create);
+      }
+      if (!kInc) { sc.act_res[c] = n_act; sc.cre_res[c] = n_create; }
+      r.act_start[c] = act_off; r.act_cnt[c] = n_act;
+      // create runs per group, in spec order (gcreate[] keeps the offsets afterwards, as k_decide2 leaves them)
+      uint32_t off = create_off;
+      for (uint32_t gi = 0; gi < G; gi++) {
+        const uint32_t want = sc.gcreate[g0 + gi];
+        r.groups[g0 + gi].create_off = off; sc.gcreate[g0 + gi] = off;
+        off += want;
+      }
+      s_place[0] = act_off; s_place[1] = n_act;
+      s_place[3] = !kInc || !__ldcg(&sc.inc[KR_INC_VOID]);  // (a void epoch is redone by a full pass: nothing more to write)
+    }
+  }
+  __syncthreads();
+  if (!s_place[3]) return;
+  for (uint32_t gi = warp; gi < G; gi += kLargeDecideThreads / 32)
+    create_fill_group(a.s, sc, r, a.f, g0 + gi, r.groups[g0 + gi].create_off, a.create_cap, s_bits[warp], lane);
+  if (warp == 0) compact_cluster_actions(r, sc, c, s_place[0], s_place[1], lane);
+  __syncthreads();  // both read the cluster's pod_start
+  if (tid == 0) r.clusters[c].pod_start = 0;  // as everywhere on the bucket pipeline (kr_flags.fetch_pod_lists = 0)
+  if (kInc && warp == 0 && s_place[2] != 0xFFFFFFFFu) {
+    __syncwarp();
+    stage_cluster(a, s_place[2], c, s_place[0], s_place[1], g0, G, lane);
+  }
+}
+
+}  // namespace kr

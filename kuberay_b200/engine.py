@@ -61,6 +61,7 @@ def lib() -> C.CDLL:
         L.kr_snapshot_commit_pod_values.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32]
         L.kr_snapshot_commit_object_rows.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32]
         L.kr_engine_set_option.argtypes = [C.c_void_p, C.c_uint32, C.c_uint64]
+        L.kr_engine_get_option.argtypes = [C.c_void_p, C.c_uint32, P(C.c_uint64)]
         L.kr_reconcile_batch.argtypes = [C.c_void_p, P(abi.kr_flags), P(abi.kr_results_view)]
         L.kr_reconcile_device_only.argtypes = [C.c_void_p, P(abi.kr_flags)]
         L.kr_reconcile_batch_profiled.argtypes = [C.c_void_p, P(abi.kr_flags), P(abi.kr_profile)]
@@ -209,13 +210,17 @@ class Engine:
         self.sizes = None
 
     @classmethod
-    def for_snapshot(cls, snap: Snapshot, device: int = 0, max_creates: int | None = None, slack: float = 1.0) -> "Engine":
+    def for_snapshot(cls, snap: Snapshot, device: int = 0, max_creates: int | None = None, slack: float = 1.0,
+                     large_clusters: bool = False) -> "Engine":
         d = snap.dims
         up = lambda x: int(x * slack) + 1  # noqa: E731
         if max_creates is None:
             max_creates = max(1024, d["pods"] // 2)
-        return cls(device, up(d["clusters"]), up(d["groups"]), up(d["wtd"]), up(d["pods"]), up(d["heads"]), up(d["jobs"]),
-                   max_creates, up(d["json"]))
+        eng = cls(device, up(d["clusters"]), up(d["groups"]), up(d["wtd"]), up(d["pods"]), up(d["heads"]), up(d["jobs"]),
+                  max_creates, up(d["json"]))
+        if large_clusters:
+            eng.set_large_clusters(True)
+        return eng
 
     def _check(self, rc: int):
         if rc != 0:
@@ -240,6 +245,17 @@ class Engine:
     def set_incremental(self, on: bool = True):
         """KR_OPT_INCREMENTAL: allow (default) or forbid device-side incremental passes; off = every pass is a full pass."""
         self._check(self._L.kr_engine_set_option(self._h, abi.OPT_INCREMENTAL, 1 if on else 0))
+
+    def set_large_clusters(self, on: bool = True):
+        """KR_OPT_LARGE_CLUSTERS: keep RayClusters of 257..LARGE_MAX_PODS pods on the bucket pipeline (their own regions) instead of
+        widening every cluster's bucket or leaving the pipeline; takes effect at the next full pass."""
+        self._check(self._L.kr_engine_set_option(self._h, abi.OPT_LARGE_CLUSTERS, 1 if on else 0))
+
+    def get_option(self, option: int) -> int:
+        """kr_engine_get_option: an option's current value, or the read-only OPT_BUCKET_STRIDE (0: the sort pipeline)."""
+        v = C.c_uint64()
+        self._check(self._L.kr_engine_get_option(self._h, option, C.byref(v)))
+        return v.value
 
     def begin(self, sizes: abi.kr_sizes) -> dict[str, np.ndarray]:
         """kr_snapshot_begin: returns numpy views over the engine-owned pinned arenas, keyed by column name."""

@@ -32,6 +32,9 @@ CONFIGS = {
     "C5": dict(n_clusters=1000, pods_per_cluster=100, groups=1, autoscaling_frac=1.0),
     # C3 with TPU-slice style worker groups: a quarter of the groups have numOfHosts=4 (about 44 % of the RayClusters hold one)
     "C3MH": dict(n_clusters=10000, pods_per_cluster=100, groups=2, multihost_frac=0.25),
+    # C3 with 20 large RayClusters of 2 000 pods each (worker pods of the other RayClusters move into them; the total stays 1 M):
+    # the fleet KR_OPT_LARGE_CLUSTERS keeps on the bucket pipeline
+    "C3L": dict(n_clusters=10000, pods_per_cluster=100, groups=1, n_large=20, large_pods=2000),
 }
 
 
@@ -56,6 +59,8 @@ class SynthParams:
     rank: int = 0                     # UID-hash shard (SURVEY §8(e)): keep clusters with uid_hash % world == rank
     world: int = 1
     cluster_id_base: int = 0          # global index of the first generated cluster (weak-scaling shards)
+    n_large: int = 0                  # RayClusters (spread over the fleet) grown to large_pods pods with worker pods of the others
+    large_pods: int = 2000
 
 
 def _splitmix64(x: np.ndarray) -> np.ndarray:
@@ -364,7 +369,34 @@ def generate(params: SynthParams | None = None, **kw) -> tuple[Snapshot, abi.kr_
         s.j_cluster_name_id[missing] = ghost_cluster_id
 
     flags = abi.default_flags(id_head_not_found_reason=ID_HEAD_NOT_FOUND_REASON, id_head_not_found_msg=ID_HEAD_NOT_FOUND_MSG)
+    if p.n_large:
+        grow_clusters(s, np.linspace(0, Nc - 1, p.n_large).astype(np.int64), p.large_pods)
     return s.validate(), flags
+
+
+def grow_clusters(snap: Snapshot, clusters, size: int) -> None:
+    """Move worker pods of the other RayClusters (first rows first) into worker group 0 of each of `clusters` until it lists
+    `size` pods; the pod rows and every other table keep their shape."""
+    taken = np.zeros(snap.dims["clusters"], dtype=bool)
+    taken[np.asarray(clusters)] = True
+    ckey = (snap.c_ns_id.astype(np.uint64) << np.uint64(32)) | snap.c_name_id.astype(np.uint64)
+    order = np.argsort(ckey)
+    pkey = (snap.p_ns_id.astype(np.uint64) << np.uint64(32)) | snap.p_cluster_name_id.astype(np.uint64)
+    pos = np.minimum(np.searchsorted(ckey[order], pkey), order.size - 1)
+    owner = np.where(ckey[order][pos] == pkey, order[pos], -1)
+    worker = ((snap.p_packed >> abi.PP_NODE_TYPE_SHIFT) & 3) == abi.NT_WORKER
+    donors = np.flatnonzero(worker & (owner >= 0) & ~taken[np.maximum(owner, 0)])
+    at = 0
+    for c in clusters:
+        need = size - int((owner == c).sum())
+        if need <= 0:
+            continue
+        if at + need > donors.size:
+            raise ValueError("not enough worker pods to grow the RayClusters")
+        move = donors[at:at + need]
+        at += need
+        g0 = int(snap.c_group_off[c])
+        snap.p_ns_id[move], snap.p_cluster_name_id[move], snap.p_group_name_id[move] = snap.c_ns_id[c], snap.c_name_id[c], snap.g_name_id[g0]
 
 
 def config(name: str, **overrides) -> SynthParams:
