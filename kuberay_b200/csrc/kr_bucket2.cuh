@@ -17,8 +17,9 @@
 //              replica indices from the registers and reserves its places in the action list / create arena with one returning
 //              atomic, so nothing follows it: no scan, no creates kernel, no compaction kernel.
 // A bucket stride too small for some cluster voids the attempt (the engine widens the stride or falls back to the sort
-// pipeline); snapshots with a RayCluster of more than KR_SMEM_GROUPS worker groups are routed to the sort pipeline by the host
-// before the pass.  Multi-host worker groups (numOfHosts > 1 under the RayMultiHostIndexing gate) are decided here too, by the
+// pipeline).  k_decide2 leaves every RayCluster of more than KR_SMEM_GROUPS worker groups alone: with KR_OPT_WIDE_CLUSTERS the
+// per-cluster kernels of kr_large.cuh decide them, without it the host routes such a snapshot to the sort pipeline before the
+// pass.  Multi-host worker groups (numOfHosts > 1 under the RayMultiHostIndexing gate) are decided here too, by the
 // k_decide2<K, kInc, true> instantiations the engine launches only when the snapshot has such a group (decide_multihost2).
 #pragma once
 
@@ -376,6 +377,9 @@ __global__ void __launch_bounds__(kD2Warps * 32, (K <= 4 && !kMH ? 32 : 16) / kD
     }
   }
   if (KR_ATTEMPT_VOID(a.r.totals)) mine = false;
+  // A RayCluster of more than KR_SMEM_GROUPS worker groups is k_large_sort / k_decide_large's (KR_OPT_WIDE_CLUSTERS, kr_large.cuh):
+  // the lane-per-group arrays below hold 32 groups.  Left before the Recreate deferral, the digest wait and the epoch's compaction.
+  if (ci.group_cnt() > KR_SMEM_GROUPS) mine = false;
   // An incremental epoch launches one warp per RayCluster of the snapshot but only the first n_dirty have work: the others leave here
   // (the kernel has no CTA-wide barrier, and `mine` is uniform across a warp) instead of walking the whole decision path predicated off —
   // that walk was 4 M of the 13.8 M warp instructions of a 63 %-dirty epoch and nearly all of a 1 %-dirty one.

@@ -269,10 +269,18 @@ struct kr_engine {
   cudaEvent_t ev_orow = nullptr; bool orow_busy = false;
   uint32_t bstride = 0;         // bucket stride of this layout (64 / 128 / 256); 0 = the layout does not qualify (a cluster outgrew 256 pods, ...)
   bool large_on = false;        // KR_OPT_LARGE_CLUSTERS
-  uint32_t n_large = 0;         // ... RayClusters of this layout with a region, sticky like bstride
-  // KR_OPT_LARGE_CLUSTERS arena, allocated when the option is first turned on (an engine without it pays nothing), sized for the
-  // capacities so that it never grows: [lg: 16 B x max_clusters | lg_list: 4 B x max_clusters | regions: 16 B x large_entries]
-  uint8_t *d_large = nullptr;
+  bool wide_on = false;         // KR_OPT_WIDE_CLUSTERS
+  // The per-cluster kernels (kr_large.cuh) take the RayClusters of one list: the large half (rows and regions {offset, capacity}
+  // from the last bucket attempt that voided, sticky like bstride) and, with KR_OPT_WIDE_CLUSTERS, the wide ones of the last commit.
+  std::vector<uint32_t> large_rows; std::vector<uint2> large_reg;
+  std::vector<uint32_t> wide_rows;  // RayClusters of more than KR_SMEM_GROUPS worker groups, ascending
+  std::vector<uint32_t> group_cnt;  // c_group_cnt of the last commit (kr_snapshot_commit_object_rows: a moved count takes the whole object commit)
+  bool lg_stale = false;        // the device table / list do not reflect the two halves yet (upload_lg at the next pass)
+  uint32_t n_large = 0;         // RayClusters in the device list
+  // Sized for the capacities so that they never grow, allocated when an option first needs them (an engine without either pays
+  // nothing): [lg: 16 B x max_clusters | lg_list: 4 B x max_clusters] for both options, regions (16 B x large_entries) for large ones
+  uint8_t *d_lg = nullptr;
+  uint4 *d_region = nullptr;
   size_t large_entries = 0;
   std::vector<uint4> h_lg; std::vector<uint32_t> h_lg_list;  // host side of the last upload (kept alive while it is in flight)
   bool snap_has_mh = false;     // some worker group has numOfHosts > 1
@@ -407,13 +415,32 @@ cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t sme
   return cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
 }
 
-// Points the pass at the large-cluster arena when the layout has large RayClusters; returns the device list of their rows.
+// Points the pass at the cluster table of the per-cluster kernels when their list is not empty; returns the device list.
 const uint32_t *bind_large(const kr_engine *e, ScratchDev &sc) {
   if (!e->n_large) return nullptr;
-  const size_t Nc = e->cfg.max_clusters;
-  sc.lg = reinterpret_cast<uint4 *>(e->d_large);
-  sc.region = reinterpret_cast<uint4 *>(e->d_large + align_up(16 * Nc) + align_up(4 * Nc));
-  return reinterpret_cast<const uint32_t *>(e->d_large + align_up(16 * Nc));
+  sc.lg = reinterpret_cast<uint4 *>(e->d_lg);
+  sc.region = e->d_region;  // (nullptr without KR_OPT_LARGE_CLUSTERS: every capacity is then 0)
+  return reinterpret_cast<const uint32_t *>(e->d_lg + align_up(16 * (size_t)e->cfg.max_clusters));
+}
+
+// Rebuilds the cluster table and the list of the per-cluster kernels from the large half and, with KR_OPT_WIDE_CLUSTERS, the wide
+// RayClusters, and uploads them on stream M, ahead of the next pass.  A new list length is a new grid of the captured graph.
+int upload_lg(kr_engine *e) {
+  e->lg_stale = false;
+  std::vector<uint32_t> list(e->large_rows);  // (both halves ascending: a wide cluster with a region is listed once)
+  if (e->wide_on)
+    for (uint32_t c : e->wide_rows) if (!std::binary_search(e->large_rows.begin(), e->large_rows.end(), c)) list.push_back(c);
+  if ((uint32_t)list.size() != e->n_large) e->gvalid = false;
+  e->n_large = (uint32_t)list.size();
+  if (list.empty()) return KR_OK;
+  const uint32_t Nc = e->sizes.n_clusters;
+  std::vector<uint4> lg(Nc, make_uint4(0, 0, 0, 0));  // a wide cluster without a region: capacity 0
+  for (size_t i = 0; i < e->large_rows.size(); i++) lg[e->large_rows[i]] = make_uint4(e->large_reg[i].x, e->large_reg[i].y, 0, 0);
+  CK(cudaStreamSynchronize(e->sm));  // the previous upload has left the host copies
+  e->h_lg.swap(lg); e->h_lg_list.swap(list);
+  CK(cudaMemcpyAsync(e->d_lg, e->h_lg.data(), 16 * (size_t)Nc, cudaMemcpyHostToDevice, e->sm));
+  CK(cudaMemcpyAsync(e->d_lg + align_up(16 * (size_t)e->cfg.max_clusters), e->h_lg_list.data(), 4 * e->h_lg_list.size(), cudaMemcpyHostToDevice, e->sm));
+  return KR_OK;
 }
 
 // Launches the whole pass.  profile: serialise everything on stream M and bracket each kernel with events.
@@ -438,9 +465,9 @@ int launch_pass(kr_engine *e, const kr_flags &f, bool profile, bool capturing = 
   // the committed snapshot: columns gate stream M, the JSON arena gates the hash
   const unsigned wflag = capturing ? cudaEventWaitExternal : cudaEventWaitDefault;
   // (the fork comes first so the hash can start while the columns are still landing — an incremental pod-row epoch leaves the JSON untouched)
-  // bucket pipeline (kr_bucket2.cuh): the caller does not fetch the full pod lists, every RayCluster has few worker groups and
-  // (checked on the device) at most `bstride` pods
-  const bool bucket = !e->no_bucket && !f.fetch_pod_lists && e->bstride != 0 && !e->force_radix && e->snap_max_groups <= KR_SMEM_GROUPS &&
+  // bucket pipeline (kr_bucket2.cuh): the caller does not fetch the full pod lists, every RayCluster has few worker groups (or
+  // KR_OPT_WIDE_CLUSTERS lists the others for the per-cluster kernels) and (checked on the device) at most `bstride` pods
+  const bool bucket = !e->no_bucket && !f.fetch_pod_lists && e->bstride != 0 && !e->force_radix && (e->snap_max_groups <= KR_SMEM_GROUPS || e->wide_on) &&
                       (size_t)n.n_clusters * e->bstride <= e->sl.bucket_entries;
   // ... and there the clusters whose Recreate gate reads a digest wait for it inside the decide kernel (the hash runs beside it)
   const bool spin = bucket && !profile && do_hash && e->hash_spin && e->n_recreate > 0;
@@ -676,41 +703,37 @@ int run_pass_once(kr_engine *e, const kr_flags &f) {
 // A bucket attempt voided: some RayCluster listed more pods than the stride holds (k_match2 counted them all in cl_dyn[].x) or
 // outgrew its region.  Widen the stride (64 -> 128 -> 256) or leave the bucket pipeline for this layout; with KR_OPT_LARGE_CLUSTERS
 // the RayClusters of more than 256 (and at most KR_LARGE_MAX_PODS) pods get regions instead, and only the others widen the stride.
+// A void rebuilds only the large half of the per-cluster kernels' list: the wide RayClusters stay on it.
 int after_bucket_void(kr_engine *e) {
   const uint32_t Nc = e->sizes.n_clusters;
   auto fits = [&](uint32_t st) { return st <= 256 && (size_t)Nc * st <= e->sl.bucket_entries; };
-  e->n_large = 0;  // (rebuilt below from this attempt's counts)
-  if (!e->large_on) { e->bstride = fits(e->bstride * 2) ? e->bstride * 2 : 0; return KR_OK; }
+  if (!e->large_on) { e->bstride = fits(e->bstride * 2) ? e->bstride * 2 : 0; return KR_OK; }  // (no large half)
   std::vector<uint4> dyn(Nc);
   CK(cudaMemcpyAsync(dyn.data(), e->d_scratch + e->sl.cl_dyn, 16 * (size_t)Nc, cudaMemcpyDeviceToHost, e->sm));
   CK(cudaStreamSynchronize(e->sm));
+  e->large_rows.clear(); e->large_reg.clear();  // (rebuilt below from this attempt's counts)
+  e->lg_stale = true;  // (uploaded below; a layout that leaves the bucket pipeline uploads nothing it would read)
   uint32_t st = e->bstride, n_big = 0, most = 0;
   for (const uint4 &d : dyn) { if (d.x > 256) n_big++; if (d.x <= 256) most = std::max(most, d.x); }
   for (const uint4 &d : dyn) if (d.x > KR_LARGE_MAX_PODS) { e->bstride = 0; return KR_OK; }  // the sort / radix pipelines take it, as before
-  if (n_big == 0) { e->bstride = fits(st * 2) ? st * 2 : 0; return KR_OK; }
+  if (n_big == 0) {
+    e->bstride = fits(st * 2) ? st * 2 : 0;
+    return e->bstride ? upload_lg(e) : KR_OK;
+  }
   while (st < most && fits(st * 2)) st <<= 1;
   if (st < most) { e->bstride = 0; return KR_OK; }
   // regions: ranks [st, st + cap) of every large cluster, cap = 1.25x its pods rounded up to 32, less the stride
-  std::vector<uint4> lg(Nc, make_uint4(0, 0, 0, 0));
-  std::vector<uint32_t> list;
   size_t off = 0;
   for (uint32_t c = 0; c < Nc; c++) {
     if (dyn[c].x <= 256) continue;
     const uint32_t want = ((dyn[c].x + dyn[c].x / 4 + 31) / 32) * 32;
     const uint32_t cap = std::min<uint32_t>(want, KR_LARGE_MAX_PODS) - st;
-    lg[c] = make_uint4((uint32_t)off, cap, 0, 0);
-    list.push_back(c);
+    e->large_rows.push_back(c); e->large_reg.push_back(make_uint2((uint32_t)off, cap));
     off += cap;
   }
-  if (off > e->large_entries) { e->bstride = 0; return KR_OK; }
-  // on the pass's stream (ordered before the rerun); the host copies stay alive until the stream has consumed them (the stream
-  // was synchronised above, so the previous upload is done)
-  e->h_lg.swap(lg); e->h_lg_list.swap(list);
-  CK(cudaMemcpyAsync(e->d_large, e->h_lg.data(), 16 * (size_t)Nc, cudaMemcpyHostToDevice, e->sm));
-  CK(cudaMemcpyAsync(e->d_large + align_up(16 * (size_t)e->cfg.max_clusters), e->h_lg_list.data(), 4 * e->h_lg_list.size(), cudaMemcpyHostToDevice, e->sm));
-  e->n_large = (uint32_t)e->h_lg_list.size();
+  if (off > e->large_entries) { e->large_rows.clear(); e->large_reg.clear(); e->bstride = 0; return KR_OK; }
   e->bstride = st;
-  return KR_OK;
+  return upload_lg(e);  // (on the pass's stream: ordered before the rerun)
 }
 // a bucket-pipeline pass leaves everything an incremental epoch needs on the device
 void after_full_pass(kr_engine *e, const kr_flags &f) {
@@ -836,6 +859,8 @@ int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile
 // switches this layout to the radix pipeline and runs again.  Leaves the stream synchronised (after an incremental pass only its one-thread epoch-closing kernel may still be in flight: it touches the epoch counters, nothing a reader of the results sees).
 int run_pass(kr_engine *e, const kr_flags &f, cudaEvent_t done) {
   e->last_flags = f;
+  // (the list moves only with a group count, which no incremental epoch absorbs, an option or a new layout: a full pass follows)
+  if (e->lg_stale) if (int rc = upload_lg(e)) return rc;
   if (e->inc_valid && !e->no_incr && memcmp(&e->inc_flags, &f, sizeof f) == 0) {
     bool ok = false;
     if (int rc = run_pass_inc(e, f, done, false, &ok)) return rc;
@@ -1002,21 +1027,26 @@ int kr_engine_set_option(kr_engine *e, uint32_t option, uint64_t value) {
     if (e->no_incr) e->inc_valid = false;
     return KR_OK;
   }
-  if (option == KR_OPT_LARGE_CLUSTERS) {
-    if (e->large_on == (value != 0)) return KR_OK;
-    if (value && !e->d_large) {
+  if (option == KR_OPT_LARGE_CLUSTERS || option == KR_OPT_WIDE_CLUSTERS) {
+    bool &on = option == KR_OPT_LARGE_CLUSTERS ? e->large_on : e->wide_on;
+    if (on == (value != 0)) return KR_OK;
+    if (value) CK(cudaSetDevice(e->cfg.device));
+    if (value && !e->d_lg) {  // the cluster table and list of the per-cluster kernels
+      const size_t Nc = e->cfg.max_clusters;
+      CK(cudaMalloc((void **)&e->d_lg, align_up(16 * Nc) + 4 * Nc));
+    }
+    if (value && option == KR_OPT_LARGE_CLUSTERS && !e->d_region) {
       // every region holds about 1.25x its cluster's pods rounded up to 32 records, and a large cluster lists more than 256 pods:
       // this many records hold the regions of any snapshot within the capacities
-      const size_t Nc = e->cfg.max_clusters, Np = e->cfg.max_pods;
+      const size_t Np = e->cfg.max_pods;
       const size_t entries = Np * 5 / 4 + 32 * (Np / 257 + 1);
-      CK(cudaSetDevice(e->cfg.device));
-      CK(cudaMalloc((void **)&e->d_large, align_up(16 * Nc) + align_up(4 * Nc) + 16 * entries));
+      CK(cudaMalloc((void **)&e->d_region, 16 * entries));
       e->large_entries = entries;
     }
-    e->large_on = value != 0;
+    on = value != 0;
     // the next full pass starts again from the layout's first stride and the fast sort pipeline: a pass with the option off may
     // have left the bucket pipeline (and the fast pipeline, for a cluster above 1024 pods) for this layout
-    e->n_large = 0; e->inc_valid = false; e->gvalid = false;
+    e->large_rows.clear(); e->large_reg.clear(); e->lg_stale = true; e->inc_valid = false; e->gvalid = false;
     e->force_radix = e->env_radix;
     if (e->begun) e->bstride = first_stride(e->sizes);
     return KR_OK;
@@ -1031,6 +1061,7 @@ int kr_engine_get_option(kr_engine *e, uint32_t option, uint64_t *value) {
     case KR_OPT_FIXED_LAYOUT: *value = e->fixed_layout; return KR_OK;
     case KR_OPT_INCREMENTAL: *value = !e->no_incr; return KR_OK;
     case KR_OPT_LARGE_CLUSTERS: *value = e->large_on; return KR_OK;
+    case KR_OPT_WIDE_CLUSTERS: *value = e->wide_on; return KR_OK;
     case KR_OPT_BUCKET_STRIDE: *value = e->bstride; return KR_OK;
     default: return fail(e, KR_E_INVALID, "unknown option %u", option);
   }
@@ -1158,7 +1189,8 @@ void kr_engine_destroy(kr_engine *e) {
   if (e->h_inc_stage) cudaFreeHost(e->h_inc_stage);
   if (e->d_inc_stage) cudaFree(e->d_inc_stage);
   if (e->d_obj_stage) cudaFree(e->d_obj_stage);
-  if (e->d_large) cudaFree(e->d_large);
+  if (e->d_lg) cudaFree(e->d_lg);
+  if (e->d_region) cudaFree(e->d_region);
   if (e->d_order) cudaFree(e->d_order);
   if (e->ev_order) cudaEventDestroy(e->ev_order);
   if (e->d_in) cudaFree(e->d_in);
@@ -1204,7 +1236,7 @@ int kr_snapshot_begin(kr_engine *e, const kr_sizes *sizes, kr_snapshot_bufs *out
       e->inc_valid = false;
       e->force_radix = e->env_radix;
       e->bstride = first_stride(*sizes);
-      e->n_large = 0;
+      e->large_rows.clear(); e->large_reg.clear(); e->lg_stale = true;
     }
   }
   e->sizes = *sizes;
@@ -1265,6 +1297,14 @@ int kr_snapshot_commit_parts(kr_engine *e, uint32_t parts) {
     if (hb.h_pod_idx[h] >= n.n_pods) return fail(e, KR_E_INVALID, "head-aux row %u: h_pod_idx %u >= n_pods %u", h, hb.h_pod_idx[h], n.n_pods);
   if (n_recreate != e->n_recreate || has_mh != e->snap_has_mh || (max_groups > KR_SMEM_GROUPS) != (e->snap_max_groups > KR_SMEM_GROUPS)) e->gvalid = false;  // launch shape / pipeline depend on them
   e->n_recreate = n_recreate; e->snap_has_mh = has_mh; e->snap_max_groups = max_groups;
+  // the wide RayClusters (KR_OPT_WIDE_CLUSTERS): a different set is a different list, and grid, of the per-cluster kernels
+  e->group_cnt.assign(hb.c_group_cnt, hb.c_group_cnt + n.n_clusters);
+  {
+    std::vector<uint32_t> wide;
+    if (max_groups > KR_SMEM_GROUPS)
+      for (uint32_t c = 0; c < n.n_clusters; c++) if (hb.c_group_cnt[c] > KR_SMEM_GROUPS) wide.push_back(c);
+    if (wide != e->wide_rows) { e->wide_rows.swap(wide); if (e->wide_on) e->lg_stale = true; }
+  }
   // hash order: message ids by descending SHA-1 block count (counting sort; the kernels run length-homogeneous warps, longest first)
   if (e->order_pending) { CK(cudaEventSynchronize(e->ev_order)); e->order_pending = false; }  // a previous upload may still be reading h_order
   // The RayClusters whose Recreate gate compares a digest lead the order: their digests are ready when the decide kernel, running
@@ -1461,15 +1501,15 @@ int kr_snapshot_commit_object_rows(kr_engine *e, const uint32_t *cluster_rows, u
   kr_snapshot_bufs hb;
   bind_in(e->il, e->h_in, &hb);
   // Only an optimisation of kr_snapshot_commit_parts(KR_PART_OBJECTS): whenever the resident state cannot take the rows as they
-  // are — no resident state, a Recreate gate or a JSON range that changed (hash order / digests), head rows added or removed —
-  // the whole object part is committed instead.
+  // are — no resident state, a Recreate gate or a JSON range that changed (hash order / digests), head rows added or removed, a
+  // group count that moved (the pipeline, the widest RayCluster and the wide set follow it) — the whole object part is committed instead.
   bool whole = !e->inc_valid || e->no_incr || !e->committed_full || e->res_n_heads != n.n_heads || e->recreate_bit.size() != n.n_clusters ||
-               e->prev_json_off.size() != n.n_clusters || e->mh_bit.size() != n.n_clusters;
+               e->prev_json_off.size() != n.n_clusters || e->mh_bit.size() != n.n_clusters || e->group_cnt.size() != n.n_clusters;
   for (uint32_t i = 0; i < n_cl && !whole; i++) {
     const uint32_t c = cluster_rows[i];
     if (c >= n.n_clusters) return fail(e, KR_E_INVALID, "cluster row %u out of range", c);
     whole = e->recreate_bit[c] != ((hb.c_flags[c] & KR_CF_UPGRADE_RECREATE) ? 1 : 0) || e->prev_json_off[c] != hb.c_json_off[c] || e->prev_json_len[c] != hb.c_json_len[c] ||
-            (uint64_t)hb.c_group_off[c] + hb.c_group_cnt[c] > n.n_groups;
+            hb.c_group_cnt[c] != e->group_cnt[c] || (uint64_t)hb.c_group_off[c] + hb.c_group_cnt[c] > n.n_groups;
   }
   for (uint32_t i = 0; i < n_hd && !whole; i++) {
     if (head_rows[i] >= n.n_heads) return fail(e, KR_E_INVALID, "head-aux row %u out of range", head_rows[i]);
@@ -1624,6 +1664,7 @@ int kr_reconcile_batch_profiled(kr_engine *e, const kr_flags *flags, kr_profile 
   if (!e->committed) return fail(e, KR_E_STATE, "no committed snapshot");
   CK(cudaSetDevice(e->cfg.device));
   e->last_flags = *flags;
+  if (e->lg_stale) if (int rc = upload_lg(e)) return rc;
   bool inc_done = false;
   if (e->inc_valid && !e->no_incr && memcmp(&e->inc_flags, flags, sizeof *flags) == 0) {
     CK(cudaEventRecord(e->ev_a, e->sm));

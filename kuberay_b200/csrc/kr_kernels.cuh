@@ -5,7 +5,7 @@
 // match_any group-by, grids sized in multiples of the SM count.
 //
 // A FULL pass is one CUDA graph (stream M unless noted), programmatic dependent launch along the chain.  Production configuration
-// (kr_flags.fetch_pod_lists == 0, no multi-host group, <= KR_SMEM_GROUPS worker groups and <= 256 pods per RayCluster) — the
+// (kr_flags.fetch_pod_lists == 0, <= KR_SMEM_GROUPS worker groups unless KR_OPT_WIDE_CLUSTERS, <= 256 pods per RayCluster) — the
 // BUCKET pipeline (kr_bucket2.cuh):
 //   k_clear          per-pass clears (hash tables, workersToDelete resolutions, totals, bucket counters / first-head cells) in one launch
 //   k_build_tables   cluster table (ns,name)->{idx, flags, name of worker group 0}, the 128-byte per-cluster input record (cl_in),
@@ -18,8 +18,9 @@
 //                    + consumer warp (the 80-round chain) per 32 messages, messages ordered by block count   [> 19 k messages: k_hash2<4,1>]
 //   k_decide2 ph. 1  the clusters whose Recreate gate needs the digest, in the places phase 0 reserved
 //   k_jobs           RayJob -> RayCluster status roll-up join
-//   k_large_sort / k_decide_large   KR_OPT_LARGE_CLUSTERS only (kr_large.cuh): the RayClusters of 257..KR_LARGE_MAX_PODS pods, one
-//                    CTA each — List order by a shared-memory sort beside the hash, then the sort pipeline's memory-resident decide
+//   k_large_sort / k_decide_large   KR_OPT_LARGE_CLUSTERS / KR_OPT_WIDE_CLUSTERS only (kr_large.cuh): the RayClusters of
+//                    257..KR_LARGE_MAX_PODS pods and those of more than KR_SMEM_GROUPS worker groups, one CTA each — List order by a
+//                    shared-memory sort beside the hash, then the sort pipeline's memory-resident decide
 // When the caller asks for the full per-cluster pod lists (fetch_pod_lists == 1) or the snapshot does not qualify — the SORT pipeline:
 //   k_match -> k_place_fused -> k_decide_small (+ k_decide on a side stream) -> [phase 1] -> k_creates_fused
 //   (buckets restored to List order by an in-register bitonic sort), and for RayClusters with > 1024 pods the RADIX pipeline

@@ -1,11 +1,14 @@
-// kr_large.cuh — large RayClusters on the bucket pipeline (KR_OPT_LARGE_CLUSTERS): more than 256 and at most KR_LARGE_MAX_PODS pods.
+// kr_large.cuh — RayClusters the bucket pipeline decides one CTA per cluster: large ones (KR_OPT_LARGE_CLUSTERS: more than 256 and
+// at most KR_LARGE_MAX_PODS pods) and wide ones (KR_OPT_WIDE_CLUSTERS: more than KR_SMEM_GROUPS worker groups).
 // Part of the sm_90a kernel set of the batched reconcile engine; see kr_kernels.cuh for the pipeline overview.
 //
-// The engine classifies them on the host after a bucket attempt that voided (k_match2 counts every cluster's pods past the stride)
-// and gives each one a region of the large-cluster record arena: k_match2 and k_inc_admit put the records of arrival rank
-// >= bucket_stride there (rec_slot, kr_bucket2.cuh), so the rest of the fleet keeps its stride and an ordinary pod never looks at
-// the region table.  k_decide2 leaves every cluster whose count exceeds the stride alone; these two kernels, one CTA per large
-// RayCluster, decide them instead:
+// The engine classifies large clusters on the host after a bucket attempt that voided (k_match2 counts every cluster's pods past
+// the stride) and gives each one a region of the large-cluster record arena: k_match2 and k_inc_admit put the records of arrival
+// rank >= bucket_stride there (rec_slot, kr_bucket2.cuh), so the rest of the fleet keeps its stride and an ordinary pod never looks
+// at the region table.  Wide clusters are known at commit (their group counts); one without a region keeps its pods in its bucket,
+// and an overflow past the stride voids the attempt as for any cluster.  Both kinds share one cluster table and one list (lg,
+// lg_list).  k_decide2 leaves every cluster whose count exceeds the stride, and every wide one, alone; these two kernels, one CTA per
+// listed RayCluster, decide them instead (decide_cluster spills the accumulators of a wide one to gacc, as the sort pipeline does):
 //   k_large_sort    (beside the hash) loads the cluster's records, drops the stale ones of an incremental epoch and stores the rest
 //                   back compacted, writes each pod's 16-byte row (what the memory-resident decide reads), sorts the pod indices
 //                   into List order in shared memory and publishes them at a scratch segment (sorted_pod_idx);
@@ -41,7 +44,10 @@ __global__ void __launch_bounds__(kLargeSortThreads) k_large_sort(Decide2Args a,
     sc.lg[c].w = 0;  // not taken (yet) this pass
     bool go = !KR_ATTEMPT_VOID(a.r.totals);
     if (kInc) go = go && !__ldcg(&sc.inc[KR_INC_VOID]) && !__ldcg(&sc.inc[KR_INC_STRUCTURAL]) && __ldcg(&sc.dirty_flag[c]) == epoch;
-    s_seg = go && P > S && P - S <= cap;  // else k_decide2 decides it (or the attempt is void: k_match2 / k_inc_admit flagged it)
+    // a large cluster past the stride, within its region; a wide one (k_decide2 leaves it alone) also with every pod in its bucket.
+    // Else k_decide2 decides it, or the attempt is void (k_match2 / k_inc_admit flagged it: a wide cluster without a region has cap 0)
+    const bool wide = a.s.c_group_cnt[c] > KR_SMEM_GROUPS;
+    s_seg = go && (P > S ? P - S <= cap : wide);
   }
   __syncthreads();
   if (!s_seg) return;

@@ -211,7 +211,7 @@ class Engine:
 
     @classmethod
     def for_snapshot(cls, snap: Snapshot, device: int = 0, max_creates: int | None = None, slack: float = 1.0,
-                     large_clusters: bool = False) -> "Engine":
+                     large_clusters: bool = False, wide_clusters: bool = False) -> "Engine":
         d = snap.dims
         up = lambda x: int(x * slack) + 1  # noqa: E731
         if max_creates is None:
@@ -220,6 +220,8 @@ class Engine:
                   max_creates, up(d["json"]))
         if large_clusters:
             eng.set_large_clusters(True)
+        if wide_clusters:
+            eng.set_wide_clusters(True)
         return eng
 
     def _check(self, rc: int):
@@ -250,6 +252,11 @@ class Engine:
         """KR_OPT_LARGE_CLUSTERS: keep RayClusters of 257..LARGE_MAX_PODS pods on the bucket pipeline (their own regions) instead of
         widening every cluster's bucket or leaving the pipeline; takes effect at the next full pass."""
         self._check(self._L.kr_engine_set_option(self._h, abi.OPT_LARGE_CLUSTERS, 1 if on else 0))
+
+    def set_wide_clusters(self, on: bool = True):
+        """KR_OPT_WIDE_CLUSTERS: keep RayClusters of more than 32 worker groups on the bucket pipeline (one CTA decides each) instead
+        of sending every pass to the sort pipeline; takes effect at the next full pass."""
+        self._check(self._L.kr_engine_set_option(self._h, abi.OPT_WIDE_CLUSTERS, 1 if on else 0))
 
     def get_option(self, option: int) -> int:
         """kr_engine_get_option: an option's current value, or the read-only OPT_BUCKET_STRIDE (0: the sort pipeline)."""

@@ -35,6 +35,9 @@ CONFIGS = {
     # C3 with 20 large RayClusters of 2 000 pods each (worker pods of the other RayClusters move into them; the total stays 1 M):
     # the fleet KR_OPT_LARGE_CLUSTERS keeps on the bucket pipeline
     "C3L": dict(n_clusters=10000, pods_per_cluster=100, groups=1, n_large=20, large_pods=2000),
+    # C3 with 100 wide RayClusters (1 %) of 48 worker groups each (one per accelerator type / node pool): the fleet
+    # KR_OPT_WIDE_CLUSTERS keeps on the bucket pipeline
+    "C3W": dict(n_clusters=10000, pods_per_cluster=100, groups=1, n_wide=100, wide_groups=48),
 }
 
 
@@ -61,6 +64,8 @@ class SynthParams:
     cluster_id_base: int = 0          # global index of the first generated cluster (weak-scaling shards)
     n_large: int = 0                  # RayClusters (spread over the fleet) grown to large_pods pods with worker pods of the others
     large_pods: int = 2000
+    n_wide: int = 0                   # RayClusters (spread over the fleet) whose worker group 0 is split into wide_groups groups
+    wide_groups: int = 48
 
 
 def _splitmix64(x: np.ndarray) -> np.ndarray:
@@ -371,6 +376,8 @@ def generate(params: SynthParams | None = None, **kw) -> tuple[Snapshot, abi.kr_
     flags = abi.default_flags(id_head_not_found_reason=ID_HEAD_NOT_FOUND_REASON, id_head_not_found_msg=ID_HEAD_NOT_FOUND_MSG)
     if p.n_large:
         grow_clusters(s, np.linspace(0, Nc - 1, p.n_large).astype(np.int64), p.large_pods)
+    if p.n_wide:
+        s = widen_clusters(s, np.linspace(0, Nc - 1, p.n_wide).astype(np.int64), p.wide_groups)
     return s.validate(), flags
 
 
@@ -397,6 +404,54 @@ def grow_clusters(snap: Snapshot, clusters, size: int) -> None:
         at += need
         g0 = int(snap.c_group_off[c])
         snap.p_ns_id[move], snap.p_cluster_name_id[move], snap.p_group_name_id[move] = snap.c_ns_id[c], snap.c_name_id[c], snap.g_name_id[g0]
+
+
+_ID_COLUMNS = ("c_ns_id", "c_name_id", "c_ext_err_msg_id", "c_old_cond_reason_id", "c_old_cond_msg_id", "c_old_head_ids", "c_svc_ip_id",
+               "c_svc_name_id", "c_summary_id", "g_name_id", "w_name_id", "p_ns_id", "p_cluster_name_id", "p_group_name_id", "p_name_id",
+               "p_replica_name_id", "h_ready_reason_id", "h_ready_msg_id", "h_pod_ip_id", "j_ns_id", "j_cluster_name_id", "j_summary_id")
+
+
+def widen_clusters(snap: Snapshot, clusters, n_groups: int) -> Snapshot:
+    """A copy of `snap` in which worker group 0 of each of `clusters` is split into `n_groups` worker groups: the group row is copied
+    under new names (its workersToDelete names stay with group 0), its worker pods are relabelled round-robin in row order and its
+    replicas and minReplicas are split.  Every other row keeps its values; the group table (offsets, workersToDelete offsets) is
+    rebuilt around the new rows."""
+    d = snap.dims
+    Nc = d["clusters"]
+    clusters = np.unique(np.asarray(clusters, dtype=np.int64))
+    assert n_groups >= 1 and (snap.c_group_cnt[clusters] >= 1).all()
+    gcnt = snap.c_group_cnt.astype(np.int64)
+    gcnt[clusters] += n_groups - 1
+    # source row of every new group: group 0 of a widened cluster n_groups times, every other group once
+    reps = np.ones(d["groups"], dtype=np.int64)
+    reps[snap.c_group_off[clusters].astype(np.int64)] += n_groups - 1
+    src = np.repeat(np.arange(d["groups"]), reps)
+    out = Snapshot(Nc, int(gcnt.sum()), d["wtd"], d["pods"], d["heads"], d["jobs"], d["json"])
+    for name, _dt, mult, dim in abi.COLUMNS:
+        if dim == "groups":
+            out.cols[name][:] = snap.cols[name][src]
+        else:
+            out.cols[name][:] = snap.cols[name]
+    new_off = np.concatenate([[0], np.cumsum(gcnt)[:-1]]).astype(np.int64)
+    out.c_group_off[:] = new_off.astype(np.uint32)
+    out.c_group_cnt[:] = gcnt.astype(np.uint32)
+    out.g_cluster_idx[:] = np.repeat(np.arange(Nc), gcnt).astype(np.uint32)
+    next_id = max(int(snap.cols[c].max()) for c in _ID_COLUMNS if snap.cols[c].size) + 1
+    worker = ((snap.p_packed >> abi.PP_NODE_TYPE_SHIFT) & 3) == abi.NT_WORKER
+    for c in clusters:
+        g_old, g_new = int(snap.c_group_off[c]), int(new_off[c])
+        rows = np.arange(g_new, g_new + n_groups)
+        out.g_name_id[rows[1:]] = np.arange(next_id, next_id + n_groups - 1, dtype=np.uint32)
+        next_id += n_groups - 1
+        out.g_wtd_cnt[rows[1:]] = 0
+        for col in ("g_replicas", "g_min"):
+            v = int(snap.cols[col][g_old])
+            out.cols[col][rows] = [v // n_groups + (k < v % n_groups) for k in range(n_groups)]
+        members = np.flatnonzero(worker & (snap.p_ns_id == snap.c_ns_id[c]) & (snap.p_cluster_name_id == snap.c_name_id[c])
+                                 & (snap.p_group_name_id == snap.g_name_id[g_old]))
+        out.p_group_name_id[members] = out.g_name_id[rows[np.arange(members.size) % n_groups]]
+    out.g_wtd_off[:] = np.concatenate([[0], np.cumsum(out.g_wtd_cnt)[:-1]]).astype(np.uint32) if out.dims["groups"] else 0
+    return out.validate()
 
 
 def config(name: str, **overrides) -> SynthParams:

@@ -31,10 +31,10 @@ def one(snap, flags, label):
         eng.close()
 
 
-def incremental(snap, flags, label, large=False):
+def incremental(snap, flags, label, large=False, wide=False):
     """Bucket pipeline + device-side incremental epochs (kr_incr.cuh): pod rows, object rows, a structural change, unfetched passes."""
     flags.fetch_pod_lists = 0
-    eng = Engine.for_snapshot(snap, slack=1.2, large_clusters=large, **({"max_creates": 1 << 16} if large else {}))
+    eng = Engine.for_snapshot(snap, slack=1.2, large_clusters=large, wide_clusters=wide, **({"max_creates": 1 << 16} if large else {}))
     eng.set_fixed_layout(True)
     try:
         views = eng.begin(snap.sizes())
@@ -80,6 +80,9 @@ def main():
     # large RayClusters in their own regions (KR_OPT_LARGE_CLUSTERS, kr_large.cuh): a full pass, then incremental epochs
     incremental(*synthetic.generate(synthetic.config("C3L", n_clusters=300, pods_per_cluster=20, large_pods=1200, n_large=3)),
                 "incremental epochs, large RayClusters", large=True)
+    # RayClusters of 48 worker groups decided one CTA each (KR_OPT_WIDE_CLUSTERS, kr_large.cuh): a full pass, then incremental epochs
+    incremental(*synthetic.generate(synthetic.config("C3W", n_clusters=300, pods_per_cluster=60, n_wide=6)),
+                "incremental epochs, wide RayClusters", wide=True)
     one(*synthetic.generate(synthetic.config("C2", n_clusters=200, jobs=True)), "fast pipeline")
     one(*synthetic.generate(synthetic.SynthParams(n_clusters=60, pods_per_cluster=41, groups=2, multihost_frac=0.5)), "multi-host")
     one(*synthetic.generate(synthetic.SynthParams(n_clusters=20, pods_per_cluster=200, groups=40)), "many groups")

@@ -1,0 +1,101 @@
+"""KR_OPT_WIDE_CLUSTERS on one GPU: the option off and on, alternated, three runs each (one JSON line per measurement).
+
+  C3W   (C3 with 100 RayClusters of 48 worker groups) and ALLW (2 000 RayClusters x 100 pods x 40 worker groups, every one wide):
+        full-pass ms (incremental epochs off; host clock around kr_reconcile_batch, so the results copy is included); then 20 epochs
+        of 1 % pod churn (PodReady flips) with incremental epochs on: how many ran incrementally on the device and their median
+        kernel ms; k_large_sort / k_decide_large alone in a profiled pass;
+  C3    full-pass ms with the option on and off (no wide RayCluster: the option changes nothing the pass launches).
+Usage: python tools/wide_bench.py [--steps 30] [--runs 3] [--out DIR]"""
+import argparse
+import json
+import os
+import subprocess
+import sys
+import time
+
+import numpy as np
+
+sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from kuberay_b200 import abi, synthetic  # noqa: E402
+from kuberay_b200.engine import Engine  # noqa: E402
+
+POD_COLS = [name for name, _dt, _m, dim in abi.COLUMNS if dim == "pods"]
+WORKLOADS = {
+    "C3W": lambda: synthetic.config("C3W"),
+    "ALLW": lambda: synthetic.SynthParams(n_clusters=2000, pods_per_cluster=100, groups=40),
+    "C3": lambda: synthetic.config("C3"),
+}
+
+
+def full_pass_ms(snap, flags, wide, steps):
+    eng = Engine.for_snapshot(snap, wide_clusters=wide)
+    try:
+        eng.set_incremental(False)
+        eng.load(snap)
+        for _ in range(3):
+            eng.reconcile(flags)
+        t = time.perf_counter()
+        for _ in range(steps):
+            eng.reconcile(flags)
+        ms = (time.perf_counter() - t) * 1e3 / steps
+        kern = {k: v for k, v in eng.reconcile_profiled(flags)["kernels"]}
+        return ms, kern.get("k_large_sort"), kern.get("k_decide_large"), eng.get_option(abi.OPT_BUCKET_STRIDE)
+    finally:
+        eng.close()
+
+
+def churn(snap, flags, wide, epochs=20, frac=0.01, seed=1):
+    eng = Engine.for_snapshot(snap, wide_clusters=wide)
+    rng = np.random.default_rng(seed)
+    try:
+        eng.set_fixed_layout(True)
+        views = eng.begin(snap.sizes())
+        eng.fill(views, snap)
+        eng.commit()
+        eng.reconcile(flags)
+        n_inc, kms = 0, []
+        for _ in range(epochs):
+            rows = np.unique(rng.choice(snap.dims["pods"], int(snap.dims["pods"] * frac), replace=False)).astype(np.uint32)
+            snap.cols["p_packed"][rows] ^= np.uint32(1 << abi.PP_READY_SHIFT)
+            for c in POD_COLS:
+                views[c][rows] = snap.cols[c][rows]
+            eng.commit_pod_values(rows, np.stack([snap.cols[c][rows].view(np.uint32) for c in POD_COLS], axis=1))
+            got = eng.reconcile(flags)
+            n_inc += got.changed_clusters is not None
+            kms.append(eng.last_profile()["kernels_ms"])
+        return n_inc, float(np.median(kms))
+    finally:
+        eng.close()
+
+
+def main():
+    ap = argparse.ArgumentParser()
+    ap.add_argument("--steps", type=int, default=30)
+    ap.add_argument("--runs", type=int, default=3)
+    ap.add_argument("--workloads", default="C3W,ALLW,C3")
+    ap.add_argument("--out", default=None)
+    a = ap.parse_args()
+    gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
+    lines = [{"gpu": gpu}]
+    print(json.dumps(lines[0]), flush=True)
+    for name in a.workloads.split(","):
+        snap, flags = synthetic.generate(WORKLOADS[name]())
+        flags.fetch_pod_lists = 0
+        for run in range(a.runs):
+            for wide in (False, True):
+                ms, ls, dl, stride = full_pass_ms(snap, flags, wide, a.steps)
+                rec = {"workload": name, "run": run, "wide_clusters": wide, "full_pass_ms": round(ms, 4), "stride": stride,
+                       "k_large_sort_ms": ls, "k_decide_large_ms": dl}
+                if name != "C3":
+                    s2, _ = synthetic.generate(WORKLOADS[name]())
+                    rec["incremental_epochs_of_20"], rec["epoch_kernel_ms_median"] = churn(s2, flags, wide)
+                lines.append(rec)
+                print(json.dumps(rec), flush=True)
+    if a.out:
+        os.makedirs(a.out, exist_ok=True)
+        with open(os.path.join(a.out, "wide_bench.jsonl"), "w") as f:
+            f.write("\n".join(json.dumps(x) for x in lines) + "\n")
+
+
+if __name__ == "__main__":
+    main()
