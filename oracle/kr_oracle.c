@@ -10,6 +10,7 @@
 
 #include <limits.h>
 #include <pthread.h>
+#include <stdio.h>
 #include <stdlib.h>
 #include <string.h>
 
@@ -418,6 +419,15 @@ static int reconcile_multihost(const octx *x, oscratch *t, uint32_t c, uint32_t 
 /* ------------------------------------------------------------------ reconcilePods (raycluster_controller.go:619-935) */
 
 typedef struct { int32_t *v; uint32_t n, cap; } ivec;
+/* Room for `need` entries.  The sum is taken in 64 bits: a RayCluster's groups may together ask for more than 2^31 pods, and a
+ * 32-bit size would wrap to a short buffer.  A stream the 32-bit counts cannot describe (or memory cannot hold) stops the process. */
+static void ivec_reserve(ivec *v, uint64_t need) {
+  if (need <= v->cap) return;
+  const uint64_t cap = need * 2 <= UINT32_MAX ? need * 2 : need;
+  int32_t *p = cap <= UINT32_MAX ? (int32_t *)realloc(v->v, (size_t)cap * sizeof(int32_t)) : NULL;
+  if (!p) { fprintf(stderr, "kr_oracle: a create stream of %llu entries\n", (unsigned long long)need); abort(); }
+  v->v = p; v->cap = (uint32_t)cap;
+}
 
 static void reconcile_pods(const octx *x, oscratch *t, uint32_t c, const char *hash32, kr_cluster_result *cr,
                            ivec *creates /* (group, n, indices...) stream */) {
@@ -515,7 +525,7 @@ static void reconcile_pods(const octx *x, oscratch *t, uint32_t c, const char *h
       int ek = reconcile_multihost(x, t, c, g, expected, gr, &earg, tmp, &want);
       if (ek == KR_ERR_NONE && want) {
         gr->n_create = want;
-        if (creates->n + 2 + want > creates->cap) { creates->cap = 2 * (creates->n + 2 + want); creates->v = (int32_t *)realloc(creates->v, creates->cap * sizeof(int32_t)); }
+        ivec_reserve(creates, (uint64_t)creates->n + 2 + want);
         creates->v[creates->n++] = (int32_t)g; creates->v[creates->n++] = (int32_t)want;
         memcpy(creates->v + creates->n, tmp, want * sizeof(int32_t)); creates->n += want;
       }
@@ -549,12 +559,15 @@ static void reconcile_pods(const octx *x, oscratch *t, uint32_t c, const char *h
     int32_t running = 0;
     for (uint32_t i = 0; i < L->n; i++) if (!t->deleted[i]) running++;
     gr->n_running = running;
-    int32_t diff = expected - running;
+    /* Go's int32 arithmetic wraps (:836): an expected count near -2^31 turns into billions of pods to create.  The subtraction is done
+     * in uint32_t so that the wrap is defined here too; such a stream is a capacity error, and ivec_reserve stops the process if it
+     * cannot even be counted (tests/fuzz_objects.py keeps |expected| <= 300 for that reason). */
+    int32_t diff = (int32_t)((uint32_t)expected - (uint32_t)running);
     gr->diff = diff;
     if (diff > 0) { /* :865-890 */
       uint32_t want = (uint32_t)diff;
       gr->n_create = want;
-      if (creates->n + 2 + want > creates->cap) { creates->cap = 2 * (creates->n + 2 + want); creates->v = (int32_t *)realloc(creates->v, creates->cap * sizeof(int32_t)); }
+      ivec_reserve(creates, (uint64_t)creates->n + 2 + want);
       creates->v[creates->n++] = (int32_t)g; creates->v[creates->n++] = (int32_t)want;
       int32_t *dst = creates->v + creates->n;
       if (f->gate_multihost_indexing) {

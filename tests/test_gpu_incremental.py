@@ -45,8 +45,13 @@ class Driver:
             np.copyto(self.views[c], self.snap.cols[c])
         self.eng.commit(abi.PART_OBJECTS)
 
-    def check(self, oracle_mod, expect_incremental=None):
-        got = self.eng.reconcile(self.flags)
+    def check(self, oracle_mod, expect_incremental=None, device_only=False):
+        """One pass (device_only: kr_reconcile_device_only, then kr_results_fetch) compared with the oracle."""
+        if device_only:
+            self.eng.reconcile_device_only(self.flags)
+            got = self.eng.fetch()
+        else:
+            got = self.eng.reconcile(self.flags)
         want = oracle_mod.run(self.snap, self.flags)
         d = want.diff(got)
         assert not d, (d[:6], got.n_changed)

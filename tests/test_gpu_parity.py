@@ -300,11 +300,94 @@ def test_hash_batch_and_passes_share_an_engine(oracle_mod):
         eng.close()
 
 
-@pytest.mark.parametrize("seed0", [0, 100, 200, 300])
-def test_fuzz_adversarial_snapshots(seed0, oracle_mod, monkeypatch):
+def _per_cluster_case(snap, arm, seed):
+    """The fuzz snapshot carried into the per-cluster kernels of the bucket pipeline (kr_large.cuh) -> (snapshot, the RayCluster
+    grown past 256 pods or None), or None when the seed has no candidate.
+      wide:  worker group 0 of every RayCluster that has a group split into 33..64 groups;
+      large: the non-head pods of one RayCluster (adversarial phases and labels included) cloned into appended rows under fresh
+             names until it lists 257..1200 pods — as far as the layout's first stride, which holds 1.25x the mean cluster, stays
+             at 256 or below (past that the pass never tries the bucket pipeline)."""
+    from kuberay_b200.snapshot import Snapshot
+    from oracle import oracle
+    rng = np.random.default_rng(seed ^ 0xC1A55)
+    grown = None
+    if arm == "wide":
+        cs = np.flatnonzero(snap.c_group_cnt >= 1)
+        if not cs.size:
+            return None
+        out = synthetic.widen_clusters(snap, cs, int(rng.integers(33, 65)))
+    else:
+        ckey = (snap.c_ns_id.astype(np.uint64) << np.uint64(32)) | snap.c_name_id.astype(np.uint64)
+        pkey = (snap.p_ns_id.astype(np.uint64) << np.uint64(32)) | snap.p_cluster_name_id.astype(np.uint64)
+        head = ((snap.p_packed >> abi.PP_NODE_TYPE_SHIFT) & 3) == abi.NT_HEAD
+        cands = [(c, np.flatnonzero((pkey == ckey[c]) & ~head & (snap.p_cluster_name_id != 0))) for c in range(snap.dims["clusters"])]
+        cands = [(c, m) for c, m in cands if m.size]
+        if not cands:
+            return None
+        grown, src = cands[int(rng.integers(len(cands)))]
+        members = int(np.sum(pkey == ckey[grown]))
+        d = snap.dims
+        most = min(1200, members + (256 * d["clusters"] * 4) // 5 - d["pods"])
+        if members > most or most < 257:
+            return None
+        extra = np.resize(src, int(rng.integers(max(257, members), most + 1)) - members)
+        out = Snapshot(d["clusters"], d["groups"], d["wtd"], d["pods"] + extra.size, d["heads"], d["jobs"], d["json"])
+        for name, _dt, _m, dim in abi.COLUMNS:
+            out.cols[name][:] = np.concatenate([snap.cols[name], snap.cols[name][extra]]) if dim == "pods" else snap.cols[name]
+        out.p_name_id[d["pods"]:] = np.uint32(max(int(snap.p_name_id.max(initial=0)), 0x10000) + 1) + np.arange(extra.size, dtype=np.uint32)
+    # split replicas times numOfHosts can reach billions of pods to create (and an expected count near -2^31 wraps expected - running):
+    # a capacity error on both sides, not a parity case (fuzz_objects.generate keeps |expected| <= 300 for the same reason)
+    L = oracle.lib()
+    big = any(abs(L.kr_oracle_desired_replicas(int(out.g_replicas[g]), int(out.g_min[g]), int(out.g_max[g]), int(out.g_num_hosts[g]),
+                                               int(out.g_flags[g]))) > 300 for g in range(out.dims["groups"]))
+    return None if big else (out, grown)
+
+
+FUZZ_ARMS = [pytest.param(s0, None, id=str(s0)) for s0 in (0, 100, 200, 300)] + \
+            [pytest.param(s0, arm, id=f"{arm}-{s0}") for arm in ("wide", "large") for s0 in (0, 100, 200)]
+
+
+@pytest.mark.parametrize("seed0,arm", FUZZ_ARMS)
+def test_fuzz_adversarial_snapshots(seed0, arm, oracle_mod, monkeypatch):
     """Differential fuzz: tiny snapshots drawn from the whole input domain (tests/fuzz_objects.py), packed like the golden
-    scenarios, engine vs oracle byte for byte.  Every fourth seed also runs the radix / unfused pipeline."""
+    scenarios, engine vs oracle byte for byte.  Every fourth seed also runs the radix / unfused pipeline.
+    The wide and large arms carry the same contents into the per-cluster kernels of the bucket pipeline (KR_OPT_WIDE_CLUSTERS and
+    KR_OPT_LARGE_CLUSTERS on, compact results): the first (captured) full pass == oracle == engine with both options off; then a
+    profiled epoch shows the per-cluster kernels on the list, and in the large arm the grown RayCluster past the stride, i.e. in its
+    region of the large-cluster arena."""
     import fuzz_objects
+    if arm:
+        cases = regions = 0
+        for seed in range(seed0, seed0 + 100):
+            snap, flags = fuzz_objects.snapshot(seed, big=(seed % 10 == 0))
+            case = _per_cluster_case(snap, arm, seed)
+            if case is None:
+                continue
+            snap, grown = case
+            cases += 1
+            flags = _compact(flags)
+            want = oracle_mod.run(snap, flags, threads=1)
+            runs = []
+            for on in (True, False):
+                eng = Engine.for_snapshot(snap, large_clusters=on, wide_clusters=on, max_creates=1 << 16)
+                try:
+                    eng.load(snap)
+                    got = eng.reconcile(flags)
+                    names = {k for k, _ in eng.reconcile_profiled(flags)["kernels"]} if on else set()
+                    runs.append((got, names, eng.get_option(abi.OPT_BUCKET_STRIDE)))
+                finally:
+                    eng.close()
+            (got, names, stride), (off, _, _) = runs
+            d = want.diff(got)
+            assert not d, (arm, seed, d[:8])
+            d = off.diff(got)
+            assert not d, (arm, "options off", seed, d[:8])
+            assert "k_decide_large" in names and stride, (arm, seed, sorted(names), stride)
+            if grown is not None:
+                n = int(np.sum((snap.p_ns_id == snap.c_ns_id[grown]) & (snap.p_cluster_name_id == snap.c_name_id[grown])))
+                regions += n > stride
+        assert cases >= 50 and (arm != "large" or regions >= 50), (cases, regions)
+        return
     for seed in range(seed0, seed0 + 100):
         snap, flags = fuzz_objects.snapshot(seed, big=(seed % 10 == 0))
         want = oracle_mod.run(snap, flags, threads=1)
