@@ -386,8 +386,8 @@ typedef struct kr_results_view {
    * absorb (a changed table key or CSR offset, wholesale column commits, different flags, an overflowing bucket) silently
    * takes the full pass.  Snapshots with multi-host worker groups (numOfHosts > 1) keep incremental epochs, and so does an edit of
    * numOfHosts.  Every pass is a full one on the sort pipeline — no resident state — while the caller fetches the full pod lists
-   * (fetch_pod_lists = 1), while some RayCluster lists more than 256 pods (more than KR_LARGE_MAX_PODS with KR_OPT_LARGE_CLUSTERS)
-   * or has more than 32 worker groups (unless KR_OPT_WIDE_CLUSTERS is set), or when KR_NO_INCR=1 is set in the environment. */
+   * (fetch_pod_lists = 1), while some RayCluster lists more than 256 pods (more than KR_LARGE_MAX_PODS with KR_OPT_LARGE_CLUSTERS,
+   * unless KR_OPT_HUGE_CLUSTERS) or has more than 32 worker groups (unless KR_OPT_WIDE_CLUSTERS is set), or when KR_NO_INCR=1 is set in the environment. */
   uint32_t n_changed;
   const uint32_t          *changed_clusters; /* [n_changed] cluster rows, unordered */
 } kr_results_view;
@@ -520,17 +520,24 @@ enum {
                               of the whole fleet or leaving the pipeline, so such a fleet keeps its incremental epochs.  Results are the
                               same as with 0 (the default: one such RayCluster sends every pass to the sort pipeline).  May be set at any
                               time; takes effect at the next full pass.  A RayCluster of more than KR_LARGE_MAX_PODS pods still sends
-                              the pass to the sort / radix pipelines.  Turning it on allocates the region arena once, for the
+                              the pass to the sort / radix pipelines, unless KR_OPT_HUGE_CLUSTERS.  Turning it on allocates the region arena once, for the
                               capacities: about 22 B per max_pods + 20 B per max_clusters of device memory. */
   KR_OPT_BUCKET_STRIDE = 4,   /* read only (kr_engine_get_option): records per RayCluster bucket of the current layout (64 / 128 / 256);
                               0 = the passes take the sort pipeline */
-  KR_OPT_WIDE_CLUSTERS = 5    /* 1: RayClusters with more than 32 worker groups stay on the bucket pipeline (DESIGN §4.1): one CTA per
+  KR_OPT_WIDE_CLUSTERS = 5,   /* 1: RayClusters with more than 32 worker groups stay on the bucket pipeline (DESIGN §4.1): one CTA per
                               such RayCluster decides it beside the warp-per-cluster decide of the others, so such a fleet keeps its
                               incremental epochs.  Results are the same as with 0 (the default: one such RayCluster sends every pass to
                               the sort pipeline).  May be set at any time; takes effect at the next full pass.  A wide RayCluster of more
                               than 256 pods is treated like any other such RayCluster: with KR_OPT_LARGE_CLUSTERS it gets a region,
                               without it the stride widens or the pass leaves the bucket pipeline.  Turning it on allocates 20 B per
                               max_clusters of device memory once (shared with KR_OPT_LARGE_CLUSTERS). */
+  KR_OPT_HUGE_CLUSTERS = 6    /* 1, together with KR_OPT_LARGE_CLUSTERS: RayClusters of more than KR_LARGE_MAX_PODS pods also stay on
+                              the bucket pipeline (DESIGN §4.1): they get regions like the large ones, and their pods are put in List
+                              order tile by tile and merged on the device, so no RayCluster is too large for incremental epochs.  No
+                              effect while KR_OPT_LARGE_CLUSTERS is 0.  Results are the same as with 0 (the default: one such RayCluster
+                              sends every pass to the sort / radix pipelines).  May be set at any time; takes effect at the next full
+                              pass.  Turning it on allocates the tile scratch once, for the capacities: about 18 B per max_pods of device
+                              memory (at least 128 KB). */
 };
 enum { KR_LARGE_MAX_PODS = 8192 };  /* largest RayCluster KR_OPT_LARGE_CLUSTERS keeps on the bucket pipeline */
 int kr_engine_set_option(kr_engine *e, uint32_t option, uint64_t value);

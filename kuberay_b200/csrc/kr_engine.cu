@@ -21,6 +21,7 @@
 #include "kr_kernels.cuh"
 #include "kr_incr.cuh"
 #include "kr_large.cuh"
+#include "kr_huge.cuh"
 
 using namespace kr;
 
@@ -270,6 +271,7 @@ struct kr_engine {
   uint32_t bstride = 0;         // bucket stride of this layout (64 / 128 / 256); 0 = the layout does not qualify (a cluster outgrew 256 pods, ...)
   bool large_on = false;        // KR_OPT_LARGE_CLUSTERS
   bool wide_on = false;         // KR_OPT_WIDE_CLUSTERS
+  bool huge_on = false;         // KR_OPT_HUGE_CLUSTERS (only with KR_OPT_LARGE_CLUSTERS)
   // The per-cluster kernels (kr_large.cuh) take the RayClusters of one list: the large half (rows and regions {offset, capacity}
   // from the last bucket attempt that voided, sticky like bstride) and, with KR_OPT_WIDE_CLUSTERS, the wide ones of the last commit.
   std::vector<uint32_t> large_rows; std::vector<uint2> large_reg;
@@ -277,12 +279,19 @@ struct kr_engine {
   std::vector<uint32_t> group_cnt;  // c_group_cnt of the last commit (kr_snapshot_commit_object_rows: a moved count takes the whole object commit)
   bool lg_stale = false;        // the device table / list do not reflect the two halves yet (upload_lg at the next pass)
   uint32_t n_large = 0;         // RayClusters in the device list
+  uint32_t n_lsort = 0;         // ... of which the first n_lsort are k_large_sort's; the huge ones after them go to k_huge_tiles / k_huge_merge
+  uint32_t n_tiles = 0;         // tiles of the huge RayClusters in the device tile table
   // Sized for the capacities so that they never grow, allocated when an option first needs them (an engine without either pays
   // nothing): [lg: 16 B x max_clusters | lg_list: 4 B x max_clusters] for both options, regions (16 B x large_entries) for large ones
   uint8_t *d_lg = nullptr;
   uint4 *d_region = nullptr;
   size_t large_entries = 0;
   std::vector<uint4> h_lg; std::vector<uint32_t> h_lg_list;  // host side of the last upload (kept alive while it is in flight)
+  // KR_OPT_HUGE_CLUSTERS, allocated when first turned on, for the capacities: the tile table {cluster, first rank, first tile, tiles}
+  // and per-tile count / counter words (24 B x huge_tiles), then each tile's sorted run and arrival-order stash (2 x 4 B x kHugeTile)
+  uint8_t *d_huge = nullptr;
+  size_t huge_tiles = 0;
+  std::vector<uint4> h_tiles;
   bool snap_has_mh = false;     // some worker group has numOfHosts > 1
   std::vector<uint8_t> mh_bit;  // ... per cluster row, as of the last commit (kr_snapshot_commit_object_rows keeps snap_has_mh current with it)
   uint32_t snap_max_groups = 0; // most worker groups in one RayCluster
@@ -423,23 +432,56 @@ const uint32_t *bind_large(const kr_engine *e, ScratchDev &sc) {
   return reinterpret_cast<const uint32_t *>(e->d_lg + align_up(16 * (size_t)e->cfg.max_clusters));
 }
 
+// The tile scratch of KR_OPT_HUGE_CLUSTERS (layout: kr_engine::d_huge).
+HugeDev bind_huge(const kr_engine *e) {
+  HugeDev h{};
+  if (!e->d_huge) return h;
+  const size_t T = e->huge_tiles;
+  uint8_t *b = e->d_huge;
+  h.tiles = reinterpret_cast<const uint4 *>(b); b += align_up(16 * T);
+  h.cnt = reinterpret_cast<uint32_t *>(b); b += align_up(4 * T);
+  h.done = reinterpret_cast<uint32_t *>(b); b += align_up(4 * T);
+  h.runs = reinterpret_cast<uint32_t *>(b); b += align_up(4 * (size_t)kHugeTile * T);
+  h.stash = reinterpret_cast<uint32_t *>(b);
+  return h;
+}
+size_t huge_bytes(size_t T) { return align_up(16 * T) + 2 * align_up(4 * T) + 2 * align_up(4 * (size_t)kHugeTile * T); }
+// Tiles a huge RayCluster's bucket and region take: its arrival ranks [0, stride + region capacity) in kHugeTile-rank tiles.
+uint32_t huge_tile_count(uint32_t stride, uint32_t cap) { return (stride + cap + kHugeTile - 1) / kHugeTile; }
+// A RayCluster of the large half is huge when its region reaches past KR_LARGE_MAX_PODS ranks (it listed more than that many pods):
+// k_large_sort's shared memory could not hold it.
+bool is_huge(uint32_t stride, uint32_t cap) { return stride + cap > KR_LARGE_MAX_PODS; }
+
 // Rebuilds the cluster table and the list of the per-cluster kernels from the large half and, with KR_OPT_WIDE_CLUSTERS, the wide
-// RayClusters, and uploads them on stream M, ahead of the next pass.  A new list length is a new grid of the captured graph.
+// RayClusters, and uploads them on stream M, ahead of the next pass.  The huge RayClusters go last, after the ones k_large_sort
+// takes, and their tiles into the tile table.  A new list length, split or tile count is a new grid of the captured graph.
 int upload_lg(kr_engine *e) {
   e->lg_stale = false;
-  std::vector<uint32_t> list(e->large_rows);  // (both halves ascending: a wide cluster with a region is listed once)
+  std::vector<uint32_t> list, huge;  // (both halves ascending: a wide cluster with a region is listed once)
+  std::vector<uint4> tiles;
+  for (size_t i = 0; i < e->large_rows.size(); i++) {
+    const uint32_t c = e->large_rows[i], cap = e->large_reg[i].y;
+    if (!is_huge(e->bstride, cap)) { list.push_back(c); continue; }
+    huge.push_back(c);
+    const uint32_t nt = huge_tile_count(e->bstride, cap), first = (uint32_t)tiles.size();
+    for (uint32_t t = 0; t < nt; t++) tiles.push_back(make_uint4(c, t * kHugeTile, first, nt));
+  }
   if (e->wide_on)
     for (uint32_t c : e->wide_rows) if (!std::binary_search(e->large_rows.begin(), e->large_rows.end(), c)) list.push_back(c);
-  if ((uint32_t)list.size() != e->n_large) e->gvalid = false;
-  e->n_large = (uint32_t)list.size();
+  const uint32_t n_lsort = (uint32_t)list.size();
+  list.insert(list.end(), huge.begin(), huge.end());
+  if (tiles.size() > e->huge_tiles) return fail(e, KR_E_STATE, "internal: %zu huge-cluster tiles, room for %zu", tiles.size(), e->huge_tiles);
+  if ((uint32_t)list.size() != e->n_large || n_lsort != e->n_lsort || (uint32_t)tiles.size() != e->n_tiles) e->gvalid = false;
+  e->n_large = (uint32_t)list.size(); e->n_lsort = n_lsort; e->n_tiles = (uint32_t)tiles.size();
   if (list.empty()) return KR_OK;
   const uint32_t Nc = e->sizes.n_clusters;
   std::vector<uint4> lg(Nc, make_uint4(0, 0, 0, 0));  // a wide cluster without a region: capacity 0
   for (size_t i = 0; i < e->large_rows.size(); i++) lg[e->large_rows[i]] = make_uint4(e->large_reg[i].x, e->large_reg[i].y, 0, 0);
   CK(cudaStreamSynchronize(e->sm));  // the previous upload has left the host copies
-  e->h_lg.swap(lg); e->h_lg_list.swap(list);
+  e->h_lg.swap(lg); e->h_lg_list.swap(list); e->h_tiles.swap(tiles);
   CK(cudaMemcpyAsync(e->d_lg, e->h_lg.data(), 16 * (size_t)Nc, cudaMemcpyHostToDevice, e->sm));
   CK(cudaMemcpyAsync(e->d_lg + align_up(16 * (size_t)e->cfg.max_clusters), e->h_lg_list.data(), 4 * e->h_lg_list.size(), cudaMemcpyHostToDevice, e->sm));
+  if (!e->h_tiles.empty()) CK(cudaMemcpyAsync(e->d_huge, e->h_tiles.data(), 16 * e->h_tiles.size(), cudaMemcpyHostToDevice, e->sm));
   return KR_OK;
 }
 
@@ -451,6 +493,7 @@ int launch_pass(kr_engine *e, const kr_flags &f, bool profile, bool capturing = 
   ResDev r = bind_out(e->ol, e->d_out);
   ScratchDev sc = bind_scratch(e->sl, e->d_scratch);
   const uint32_t *lg_list = bind_large(e, sc);
+  const HugeDev hd = bind_huge(e);
   Sizes z{n.n_clusters, n.n_groups, n.n_wtd, n.n_pods, n.n_heads, n.n_jobs};
   cudaStream_t M = e->sm, H = profile ? e->sm : e->sh;
   int k = 0;
@@ -542,7 +585,11 @@ int launch_pass(kr_engine *e, const kr_flags &f, bool profile, bool capturing = 
     } else CK(cudaMemsetAsync(r.act_start, 0, 4, M));
     if (n.n_jobs) { mark("k_jobs"); k_jobs<<<(n.n_jobs + 255) / 256, 256, 0, M>>>(s, sc, r, z); }
     const bool large = e->n_large && sc.lg && n.n_clusters;  // large RayClusters (kr_large.cuh): sorted beside the hash, decided after it
-    if (large) { mark("k_large_sort"); k_large_sort<false><<<e->n_large, kLargeSortThreads, 0, M>>>(da, lg_list); }
+    if (large && e->n_lsort) { mark("k_large_sort"); k_large_sort<false><<<e->n_lsort, kLargeSortThreads, 0, M>>>(da, lg_list); }
+    if (large && e->n_tiles) {  // huge RayClusters (kr_huge.cuh): sorted tile by tile, then merged, also beside the hash
+      mark("k_huge_tiles"); k_huge_tiles<false><<<e->n_tiles, kHugeThreads, 0, M>>>(da, hd);
+      mark("k_huge_merge"); k_huge_merge<false><<<e->n_tiles, kHugeThreads, 0, M>>>(da, hd);
+    }
     if (profile) {
       if (do_hash) { mark("k_hash"); launch_hash(); }
       else if (n.n_clusters) CK(cudaMemsetAsync(r.hash, 0, 32 * (size_t)n.n_clusters, M));
@@ -702,7 +749,8 @@ int run_pass_once(kr_engine *e, const kr_flags &f) {
 
 // A bucket attempt voided: some RayCluster listed more pods than the stride holds (k_match2 counted them all in cl_dyn[].x) or
 // outgrew its region.  Widen the stride (64 -> 128 -> 256) or leave the bucket pipeline for this layout; with KR_OPT_LARGE_CLUSTERS
-// the RayClusters of more than 256 (and at most KR_LARGE_MAX_PODS) pods get regions instead, and only the others widen the stride.
+// the RayClusters of more than 256 (and at most KR_LARGE_MAX_PODS, or any number with KR_OPT_HUGE_CLUSTERS) pods get regions
+// instead, and only the others widen the stride.
 // A void rebuilds only the large half of the per-cluster kernels' list: the wide RayClusters stay on it.
 int after_bucket_void(kr_engine *e) {
   const uint32_t Nc = e->sizes.n_clusters;
@@ -715,23 +763,26 @@ int after_bucket_void(kr_engine *e) {
   e->lg_stale = true;  // (uploaded below; a layout that leaves the bucket pipeline uploads nothing it would read)
   uint32_t st = e->bstride, n_big = 0, most = 0;
   for (const uint4 &d : dyn) { if (d.x > 256) n_big++; if (d.x <= 256) most = std::max(most, d.x); }
-  for (const uint4 &d : dyn) if (d.x > KR_LARGE_MAX_PODS) { e->bstride = 0; return KR_OK; }  // the sort / radix pipelines take it, as before
+  if (!e->huge_on)
+    for (const uint4 &d : dyn) if (d.x > KR_LARGE_MAX_PODS) { e->bstride = 0; return KR_OK; }  // the sort / radix pipelines take it, as before
   if (n_big == 0) {
     e->bstride = fits(st * 2) ? st * 2 : 0;
     return e->bstride ? upload_lg(e) : KR_OK;
   }
   while (st < most && fits(st * 2)) st <<= 1;
   if (st < most) { e->bstride = 0; return KR_OK; }
-  // regions: ranks [st, st + cap) of every large cluster, cap = 1.25x its pods rounded up to 32, less the stride
-  size_t off = 0;
+  // regions: ranks [st, st + cap) of every large cluster, cap = 1.25x its pods rounded up to 32 (at most KR_LARGE_MAX_PODS unless
+  // the cluster is huge), less the stride
+  size_t off = 0, tiles = 0;
   for (uint32_t c = 0; c < Nc; c++) {
     if (dyn[c].x <= 256) continue;
     const uint32_t want = ((dyn[c].x + dyn[c].x / 4 + 31) / 32) * 32;
-    const uint32_t cap = std::min<uint32_t>(want, KR_LARGE_MAX_PODS) - st;
+    const uint32_t cap = (dyn[c].x > KR_LARGE_MAX_PODS ? want : std::min<uint32_t>(want, KR_LARGE_MAX_PODS)) - st;
     e->large_rows.push_back(c); e->large_reg.push_back(make_uint2((uint32_t)off, cap));
     off += cap;
+    if (is_huge(st, cap)) tiles += huge_tile_count(st, cap);
   }
-  if (off > e->large_entries) { e->large_rows.clear(); e->large_reg.clear(); e->bstride = 0; return KR_OK; }
+  if (off > e->large_entries || tiles > e->huge_tiles) { e->large_rows.clear(); e->large_reg.clear(); e->bstride = 0; return KR_OK; }
   e->bstride = st;
   return upload_lg(e);  // (on the pass's stream: ordered before the rerun)
 }
@@ -756,6 +807,7 @@ int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile
   ScratchDev sc = bind_scratch(e->sl, e->d_scratch);
   sc.bucket_stride = e->bstride;
   const uint32_t *lg_list = bind_large(e, sc);
+  const HugeDev hd = bind_huge(e);
   Sizes z{n.n_clusters, n.n_groups, n.n_wtd, n.n_pods, n.n_heads, n.n_jobs};
   cudaStream_t M = e->sm, H = profile ? e->sm : e->sh;
   int k = 0;
@@ -818,8 +870,11 @@ int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile
     else (mh ? k_decide2<8, true, true> : k_decide2<8, true>)<<<dgrid, dblock, 0, M>>>(da);
     if (e->n_large) {  // the dirty large RayClusters (k_decide2 left every cluster past the stride alone)
       CK(cudaMemsetAsync(sc.inc + KR_INC_LSEG, 0, 4, M));
-      mark("k_large_sort");
-      k_large_sort<true><<<e->n_large, kLargeSortThreads, 0, M>>>(da, lg_list);
+      if (e->n_lsort) { mark("k_large_sort"); k_large_sort<true><<<e->n_lsort, kLargeSortThreads, 0, M>>>(da, lg_list); }
+      if (e->n_tiles) {
+        mark("k_huge_tiles"); k_huge_tiles<true><<<e->n_tiles, kHugeThreads, 0, M>>>(da, hd);
+        mark("k_huge_merge"); k_huge_merge<true><<<e->n_tiles, kHugeThreads, 0, M>>>(da, hd);
+      }
       mark("k_decide_large");
       k_decide_large<true><<<e->n_large, kLargeDecideThreads, 0, M>>>(da, lg_list);
     }
@@ -1027,11 +1082,11 @@ int kr_engine_set_option(kr_engine *e, uint32_t option, uint64_t value) {
     if (e->no_incr) e->inc_valid = false;
     return KR_OK;
   }
-  if (option == KR_OPT_LARGE_CLUSTERS || option == KR_OPT_WIDE_CLUSTERS) {
-    bool &on = option == KR_OPT_LARGE_CLUSTERS ? e->large_on : e->wide_on;
+  if (option == KR_OPT_LARGE_CLUSTERS || option == KR_OPT_WIDE_CLUSTERS || option == KR_OPT_HUGE_CLUSTERS) {
+    bool &on = option == KR_OPT_LARGE_CLUSTERS ? e->large_on : option == KR_OPT_WIDE_CLUSTERS ? e->wide_on : e->huge_on;
     if (on == (value != 0)) return KR_OK;
     if (value) CK(cudaSetDevice(e->cfg.device));
-    if (value && !e->d_lg) {  // the cluster table and list of the per-cluster kernels
+    if (value && option != KR_OPT_HUGE_CLUSTERS && !e->d_lg) {  // the cluster table and list of the per-cluster kernels
       const size_t Nc = e->cfg.max_clusters;
       CK(cudaMalloc((void **)&e->d_lg, align_up(16 * Nc) + 4 * Nc));
     }
@@ -1042,6 +1097,15 @@ int kr_engine_set_option(kr_engine *e, uint32_t option, uint64_t value) {
       const size_t entries = Np * 5 / 4 + 32 * (Np / 257 + 1);
       CK(cudaMalloc((void **)&e->d_region, 16 * entries));
       e->large_entries = entries;
+    }
+    if (value && option == KR_OPT_HUGE_CLUSTERS && !e->d_huge) {
+      // a huge cluster's tiles cover about 1.25x its pods rounded up to 32, plus at most one partial tile, and it lists more than
+      // KR_LARGE_MAX_PODS pods: this many tiles hold those of any snapshot within the capacities
+      const size_t Np = e->cfg.max_pods, n_huge = Np / (KR_LARGE_MAX_PODS + 1);
+      const size_t T = (Np * 5 / 4 + 32 * (n_huge + 1)) / kHugeTile + n_huge + 2;
+      CK(cudaMalloc((void **)&e->d_huge, huge_bytes(T)));
+      CK(cudaMemset(e->d_huge, 0, huge_bytes(T)));  // (the per-cluster tile counters start at 0; every pass leaves them there)
+      e->huge_tiles = T;
     }
     on = value != 0;
     // the next full pass starts again from the layout's first stride and the fast sort pipeline: a pass with the option off may
@@ -1062,6 +1126,7 @@ int kr_engine_get_option(kr_engine *e, uint32_t option, uint64_t *value) {
     case KR_OPT_INCREMENTAL: *value = !e->no_incr; return KR_OK;
     case KR_OPT_LARGE_CLUSTERS: *value = e->large_on; return KR_OK;
     case KR_OPT_WIDE_CLUSTERS: *value = e->wide_on; return KR_OK;
+    case KR_OPT_HUGE_CLUSTERS: *value = e->huge_on; return KR_OK;
     case KR_OPT_BUCKET_STRIDE: *value = e->bstride; return KR_OK;
     default: return fail(e, KR_E_INVALID, "unknown option %u", option);
   }
@@ -1134,7 +1199,8 @@ int kr_engine_create(const kr_config *cfg, kr_engine **out) {
                         (const void *)k_inc_mark_recreate, (const void *)k_decide2<2, true>, (const void *)k_decide2<4, true>, (const void *)k_decide2<8, true>, (const void *)k_inc_refresh, (const void *)k_inc_admit,
                         (const void *)k_inc_finish, (const void *)k_decide2<2, false, true>, (const void *)k_decide2<4, false, true>, (const void *)k_decide2<8, false, true>,
                         (const void *)k_decide2<2, true, true>, (const void *)k_decide2<4, true, true>, (const void *)k_decide2<8, true, true>,
-                        (const void *)k_large_sort<false>, (const void *)k_large_sort<true>, (const void *)k_decide_large<false>, (const void *)k_decide_large<true>};
+                        (const void *)k_large_sort<false>, (const void *)k_large_sort<true>, (const void *)k_decide_large<false>, (const void *)k_decide_large<true>,
+                        (const void *)k_huge_tiles<false>, (const void *)k_huge_tiles<true>, (const void *)k_huge_merge<false>, (const void *)k_huge_merge<true>};
     for (const void *k : ks) cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, pct);
   }
   if (const char *g = getenv("KR_NO_GRAPH")) e->use_graph = !(g[0] == '1');
@@ -1191,6 +1257,7 @@ void kr_engine_destroy(kr_engine *e) {
   if (e->d_obj_stage) cudaFree(e->d_obj_stage);
   if (e->d_lg) cudaFree(e->d_lg);
   if (e->d_region) cudaFree(e->d_region);
+  if (e->d_huge) cudaFree(e->d_huge);
   if (e->d_order) cudaFree(e->d_order);
   if (e->ev_order) cudaEventDestroy(e->ev_order);
   if (e->d_in) cudaFree(e->d_in);

@@ -26,6 +26,27 @@ namespace kr {
 static constexpr int kLargeSortThreads = 512;
 static constexpr int kLargeDecideThreads = 128;
 
+// Ascending bitonic sort of s[0, total) in shared memory, padded to the next power of two (at least 2) with 0xFFFFFFFF: s must
+// hold that many words.  Every thread of the CTA calls it; the stores of s[0, total) are ordered before by its first barrier.
+template <int kThreads>
+__device__ __forceinline__ void block_sort_asc(uint32_t *s, uint32_t total, uint32_t tid) {
+  uint32_t n2 = 2;
+  while (n2 < total) n2 <<= 1;
+  for (uint32_t k = total + tid; k < n2; k += kThreads) s[k] = 0xFFFFFFFFu;
+  __syncthreads();
+  for (uint32_t size = 2; size <= n2; size <<= 1) {
+    for (uint32_t stride = size >> 1; stride > 0; stride >>= 1) {
+      for (uint32_t t = tid; t < n2 / 2; t += kThreads) {
+        const uint32_t lo = 2 * stride * (t / stride) + (t % stride), hi = lo + stride;
+        const bool asc = (lo & size) == 0;
+        const uint32_t u = s[lo], v = s[hi];
+        if ((u > v) == asc) { s[lo] = v; s[hi] = u; }
+      }
+      __syncthreads();
+    }
+  }
+}
+
 // One CTA per large RayCluster (lg_list).  kInc: only the ones the epoch marked dirty.
 template <bool kInc>
 __global__ void __launch_bounds__(kLargeSortThreads) k_large_sort(Decide2Args a, const uint32_t *__restrict__ lg_list) {
@@ -94,22 +115,8 @@ __global__ void __launch_bounds__(kLargeSortThreads) k_large_sort(Decide2Args a,
     }
     if (tid == 0) { sc.cl_dyn[c].x = total; sc.cl_dyn[c].y = 0u; }
   }
-  // informer List order = ascending pod index: bitonic sort of the next power of two in shared memory
-  uint32_t n2 = 2;
-  while (n2 < total) n2 <<= 1;
-  for (uint32_t k = total + tid; k < n2; k += kLargeSortThreads) s_idx[k] = 0xFFFFFFFFu;
-  __syncthreads();
-  for (uint32_t size = 2; size <= n2; size <<= 1) {
-    for (uint32_t stride = size >> 1; stride > 0; stride >>= 1) {
-      for (uint32_t t = tid; t < n2 / 2; t += kLargeSortThreads) {
-        const uint32_t lo = 2 * stride * (t / stride) + (t % stride), hi = lo + stride;
-        const bool asc = (lo & size) == 0;
-        const uint32_t u = s_idx[lo], v = s_idx[hi];
-        if ((u > v) == asc) { s_idx[lo] = v; s_idx[hi] = u; }
-      }
-      __syncthreads();
-    }
-  }
+  // informer List order = ascending pod index
+  block_sort_asc<kLargeSortThreads>(s_idx, total, tid);
   for (uint32_t k = tid; k < total; k += kLargeSortThreads) a.r.sorted_pod_idx[seg + k] = s_idx[k];
   if (tid == 0) { sc.lg[c].z = seg; sc.lg[c].w = total | KR_LG_OWNED; }
 }

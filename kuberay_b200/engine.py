@@ -211,7 +211,7 @@ class Engine:
 
     @classmethod
     def for_snapshot(cls, snap: Snapshot, device: int = 0, max_creates: int | None = None, slack: float = 1.0,
-                     large_clusters: bool = False, wide_clusters: bool = False) -> "Engine":
+                     large_clusters: bool = False, wide_clusters: bool = False, huge_clusters: bool = False) -> "Engine":
         d = snap.dims
         up = lambda x: int(x * slack) + 1  # noqa: E731
         if max_creates is None:
@@ -222,6 +222,8 @@ class Engine:
             eng.set_large_clusters(True)
         if wide_clusters:
             eng.set_wide_clusters(True)
+        if huge_clusters:
+            eng.set_huge_clusters(True)
         return eng
 
     def _check(self, rc: int):
@@ -257,6 +259,12 @@ class Engine:
         """KR_OPT_WIDE_CLUSTERS: keep RayClusters of more than 32 worker groups on the bucket pipeline (one CTA decides each) instead
         of sending every pass to the sort pipeline; takes effect at the next full pass."""
         self._check(self._L.kr_engine_set_option(self._h, abi.OPT_WIDE_CLUSTERS, 1 if on else 0))
+
+    def set_huge_clusters(self, on: bool = True):
+        """KR_OPT_HUGE_CLUSTERS: with set_large_clusters, keep RayClusters of more than LARGE_MAX_PODS pods on the bucket pipeline
+        too (their pods are sorted tile by tile and merged) instead of sending every pass to the sort pipeline; no effect without
+        it; takes effect at the next full pass."""
+        self._check(self._L.kr_engine_set_option(self._h, abi.OPT_HUGE_CLUSTERS, 1 if on else 0))
 
     def get_option(self, option: int) -> int:
         """kr_engine_get_option: an option's current value, or the read-only OPT_BUCKET_STRIDE (0: the sort pipeline)."""

@@ -38,6 +38,9 @@ CONFIGS = {
     # C3 with 100 wide RayClusters (1 %) of 48 worker groups each (one per accelerator type / node pool): the fleet
     # KR_OPT_WIDE_CLUSTERS keeps on the bucket pipeline
     "C3W": dict(n_clusters=10000, pods_per_cluster=100, groups=1, n_wide=100, wide_groups=48),
+    # C3 with 2 huge RayClusters of 20 000 pods each (a batch-inference or data-processing job of CPU workers): the fleet
+    # KR_OPT_HUGE_CLUSTERS (with KR_OPT_LARGE_CLUSTERS) keeps on the bucket pipeline
+    "C3H": dict(n_clusters=10000, pods_per_cluster=100, groups=1, n_large=2, large_pods=20000),
 }
 
 

@@ -31,10 +31,11 @@ def one(snap, flags, label):
         eng.close()
 
 
-def incremental(snap, flags, label, large=False, wide=False):
+def incremental(snap, flags, label, large=False, wide=False, huge=False):
     """Bucket pipeline + device-side incremental epochs (kr_incr.cuh): pod rows, object rows, a structural change, unfetched passes."""
     flags.fetch_pod_lists = 0
-    eng = Engine.for_snapshot(snap, slack=1.2, large_clusters=large, wide_clusters=wide, **({"max_creates": 1 << 16} if large else {}))
+    eng = Engine.for_snapshot(snap, slack=1.2, large_clusters=large, wide_clusters=wide, huge_clusters=huge,
+                              **({"max_creates": 1 << 16} if large else {}))
     eng.set_fixed_layout(True)
     try:
         views = eng.begin(snap.sizes())
@@ -83,6 +84,10 @@ def main():
     # RayClusters of 48 worker groups decided one CTA each (KR_OPT_WIDE_CLUSTERS, kr_large.cuh): a full pass, then incremental epochs
     incremental(*synthetic.generate(synthetic.config("C3W", n_clusters=300, pods_per_cluster=60, n_wide=6)),
                 "incremental epochs, wide RayClusters", wide=True)
+    # a RayCluster of more than KR_LARGE_MAX_PODS pods sorted tile by tile (KR_OPT_HUGE_CLUSTERS, kr_huge.cuh): a full pass, then
+    # incremental epochs (the deletions compact its bucket and region across tiles)
+    incremental(*synthetic.generate(synthetic.config("C3H", n_clusters=700, pods_per_cluster=20, large_pods=9000, n_large=1)),
+                "incremental epochs, huge RayCluster", large=True, huge=True)
     one(*synthetic.generate(synthetic.config("C2", n_clusters=200, jobs=True)), "fast pipeline")
     one(*synthetic.generate(synthetic.SynthParams(n_clusters=60, pods_per_cluster=41, groups=2, multihost_frac=0.5)), "multi-host")
     one(*synthetic.generate(synthetic.SynthParams(n_clusters=20, pods_per_cluster=200, groups=40)), "many groups")
