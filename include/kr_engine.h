@@ -385,7 +385,7 @@ typedef struct kr_results_view {
    * recomputed: n_changed == n_clusters and changed_clusters == NULL after a full pass.  Anything the resident state cannot
    * absorb (a changed table key or CSR offset, wholesale column commits, different flags, an overflowing bucket) silently
    * takes the full pass.  Snapshots with multi-host worker groups (numOfHosts > 1) keep incremental epochs, and so does an edit of
-   * numOfHosts.  Every pass is a full one on the sort pipeline — no resident state — while the caller fetches the full pod lists
+   * numOfHosts; so does an edit of a workersToDelete list with KR_OPT_WTD_EDITS (a length change only under KR_OPT_FIXED_LAYOUT).  Every pass is a full one on the sort pipeline — no resident state — while the caller fetches the full pod lists
    * (fetch_pod_lists = 1), while some RayCluster lists more than 256 pods (more than KR_LARGE_MAX_PODS with KR_OPT_LARGE_CLUSTERS,
    * unless KR_OPT_HUGE_CLUSTERS) or has more than 32 worker groups (unless KR_OPT_WIDE_CLUSTERS is set), or when KR_NO_INCR=1 is set in the environment. */
   uint32_t n_changed;
@@ -531,13 +531,21 @@ enum {
                               than 256 pods is treated like any other such RayCluster: with KR_OPT_LARGE_CLUSTERS it gets a region,
                               without it the stride widens or the pass leaves the bucket pipeline.  Turning it on allocates 20 B per
                               max_clusters of device memory once (shared with KR_OPT_LARGE_CLUSTERS). */
-  KR_OPT_HUGE_CLUSTERS = 6    /* 1, together with KR_OPT_LARGE_CLUSTERS: RayClusters of more than KR_LARGE_MAX_PODS pods also stay on
+  KR_OPT_HUGE_CLUSTERS = 6,   /* 1, together with KR_OPT_LARGE_CLUSTERS: RayClusters of more than KR_LARGE_MAX_PODS pods also stay on
                               the bucket pipeline (DESIGN §4.1): they get regions like the large ones, and their pods are put in List
                               order tile by tile and merged on the device, so no RayCluster is too large for incremental epochs.  No
                               effect while KR_OPT_LARGE_CLUSTERS is 0.  Results are the same as with 0 (the default: one such RayCluster
                               sends every pass to the sort / radix pipelines).  May be set at any time; takes effect at the next full
                               pass.  Turning it on allocates the tile scratch once, for the capacities: about 18 B per max_pods of device
                               memory (at least 128 KB). */
+  KR_OPT_WTD_EDITS = 7        /* 1: an edit of a scaleStrategy.workersToDelete list (a name renamed, a list grown or shrunk, as the
+                              autoscaler writes on every scale-down and clears once the Pods are gone) keeps the incremental epoch: the
+                              next pass rebuilds the name table on the device and re-decides only the RayClusters whose Pods were named
+                              before or are named now.  A list whose length changes moves n_wtd, which needs KR_OPT_FIXED_LAYOUT (without
+                              it every new row count is a full pass); a rename does not.  Results are the same as with 0 (the default:
+                              any such edit makes the next pass a full one).  May be set at any time; read at each object commit.
+                              kr_snapshot_commit_object_rows still expects unchanged lists: with this option, rows whose lists changed
+                              are committed as the whole object part. */
 };
 enum { KR_LARGE_MAX_PODS = 8192 };  /* largest RayCluster KR_OPT_LARGE_CLUSTERS keeps on the bucket pipeline */
 int kr_engine_set_option(kr_engine *e, uint32_t option, uint64_t value);

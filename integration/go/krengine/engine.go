@@ -140,13 +140,15 @@ const (
 	OptLargeClusters = uint32(C.KR_OPT_LARGE_CLUSTERS)
 	OptWideClusters  = uint32(C.KR_OPT_WIDE_CLUSTERS)
 	OptHugeClusters  = uint32(C.KR_OPT_HUGE_CLUSTERS)
+	OptWtdEdits      = uint32(C.KR_OPT_WTD_EDITS)
 )
 
 // SetOption: KR_OPT_FIXED_LAYOUT (before the first Begin), KR_OPT_INCREMENTAL, KR_OPT_LARGE_CLUSTERS (1: RayClusters of 257 to
 // KR_LARGE_MAX_PODS pods stay on the bucket pipeline and keep incremental epochs; recommended for fleets that have them; takes
 // effect at the next full pass), KR_OPT_WIDE_CLUSTERS (1: the same for RayClusters with more than 32 worker groups; takes effect
 // at the next full pass), KR_OPT_HUGE_CLUSTERS (1, with KR_OPT_LARGE_CLUSTERS: the same for RayClusters of more than
-// KR_LARGE_MAX_PODS pods; takes effect at the next full pass).  For a Packer, call it on Packer.Engine().
+// KR_LARGE_MAX_PODS pods; takes effect at the next full pass), KR_OPT_WTD_EDITS (1: scaleStrategy.workersToDelete edits keep
+// incremental epochs; recommended for autoscaling fleets; read at each object commit).  For a Packer, call it on Packer.Engine().
 func (e *Engine) SetOption(option uint32, value uint64) error {
 	if rc := C.kr_engine_set_option(e.h, C.uint32_t(option), C.uint64_t(value)); rc != C.KR_OK {
 		return e.err(rc)

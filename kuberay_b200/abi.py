@@ -86,6 +86,7 @@ OPT_LARGE_CLUSTERS = 3
 OPT_BUCKET_STRIDE = 4
 OPT_WIDE_CLUSTERS = 5
 OPT_HUGE_CLUSTERS = 6
+OPT_WTD_EDITS = 7
 LARGE_MAX_PODS = 8192
 SPEC_JSON_UNMUTED = 1
 KR_OK, KR_E_INVALID, KR_E_CAPACITY, KR_E_CUDA, KR_E_STATE, KR_E_NO_DEVICE = 0, -1, -2, -3, -4, -5

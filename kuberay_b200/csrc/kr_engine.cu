@@ -86,6 +86,22 @@ static const uint8_t kObjClass[kNumCols] = {
         0};
 constexpr int kHeadKeyCol = 39, kGroupClusterCol = 22;
 static_assert(kCols[kHeadKeyCol].dim == D_HEADS && kCols[kHeadKeyCol - 1].dim == D_PODS && kCols[kGroupClusterCol].dim == D_GROUPS && kCols[kGroupClusterCol - 1].dim == D_CLUSTERS, "column indices of the object diff");
+// g_wtd_off, g_wtd_cnt, w_name_id.  With KR_OPT_WTD_EDITS a staged object commit classifies them as copy / group / copy instead:
+// the next pass rebuilds the name table and recomputes KR_ROW_WTD_OWN (the only use of the offsets), and the multi-host decide
+// reads the count.
+constexpr int kWtdOffCol = 29, kWtdCntCol = 30, kWtdNameCol = 31;
+static_assert(kCols[kWtdCntCol].dim == D_GROUPS && kCols[kWtdNameCol].dim == D_WTD && kCols[kWtdNameCol + 1].dim == D_PODS, "workersToDelete column indices");
+uint8_t obj_class(int col, bool wtd_edits) {
+  if (wtd_edits && (col == kWtdOffCol || col == kWtdNameCol)) return KR_OC_COPY;
+  if (wtd_edits && col == kWtdCntCol) return KR_OC_GROUP;
+  return kObjClass[col];
+}
+// the snapshot's workersToDelete lists equal `prev` ({n_groups, g_wtd_off, g_wtd_cnt, w_name_id} of an earlier commit)
+bool wtd_lists_equal(const std::vector<uint32_t> &prev, const kr_snapshot_bufs &hb, const kr_sizes &n) {
+  const size_t G = n.n_groups, W = n.n_wtd;
+  return prev.size() == 1 + 2 * G + W && prev[0] == G && memcmp(prev.data() + 1, hb.g_wtd_off, 4 * G) == 0 &&
+         memcmp(prev.data() + 1 + G, hb.g_wtd_cnt, 4 * G) == 0 && memcmp(prev.data() + 1 + 2 * G, hb.w_name_id, 4 * W) == 0;
+}
 
 
 void dims_of(const kr_sizes &n, uint64_t d[7]) {
@@ -312,6 +328,10 @@ struct kr_engine {
   uint32_t res_n_heads = 0;                  // head-aux rows the resident device columns hold (object commits move it)
   std::vector<uint32_t> prev_h_pod_idx;      // ... and their keys: a change means the pod -> head-aux row table must be rebuilt
   bool heads_rebuild = false;
+  bool wtd_edits = false;        // KR_OPT_WTD_EDITS
+  std::vector<uint32_t> prev_wtd;  // ... the workersToDelete lists of the last commit, {n_groups, g_wtd_off, g_wtd_cnt, w_name_id} (empty while the option is off)
+  bool wtd_rebuild = false;      // ... a commit changed them since the last pass: it rebuilds the name table (kr_incr.cuh)
+  uint32_t res_n_wtd = 0;        // names in the resident name table and its resolutions (wtd_pod_idx)
   bool hash_dirty = false;       // spec JSON (or a JSON range) committed since the digests were computed
   bool ran_inc = false;          // the last pass was an incremental one
   bool host_results_stale = false;  // an incremental pass went unfetched: the host copy misses its records, the next fetch copies everything
@@ -793,6 +813,7 @@ void after_full_pass(kr_engine *e, const kr_flags &f) {
   e->inc_valid = e->ran_bucket && !e->no_incr && e->h_totals[9] <= e->cfg.max_creates;
   e->inc_flags = f; e->inc_n_pods = e->sizes.n_pods; e->inc_n_heads = e->sizes.n_heads;
   e->host_results_stale = false; e->inc_n_dirty = 0; e->fetched = false; e->ran_inc = false; e->heads_rebuild = false;
+  e->wtd_rebuild = false; e->res_n_wtd = e->sizes.n_wtd;
   if (!f.skip_hash) e->hash_dirty = false;
 }
 
@@ -835,6 +856,19 @@ int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile
     mark("k_inc_aux_rebuild");
     k_inc_aux_clear<<<std::min<uint32_t>(grid, (e->sl.aux_slots + 255) / 256), 256, 0, M>>>(sc);
     k_inc_aux_insert<<<std::min<uint32_t>(grid, (n.n_heads + 255) / 256 + 1), 256, 0, M>>>(s, sc, z);
+  }
+  if (e->wtd_rebuild) {  // a workersToDelete list changed since the name table was built (KR_OPT_WTD_EDITS; the commit compared them on the host)
+    if (e->res_n_wtd) { mark("k_inc_wtd_release"); k_inc_wtd_release<<<(e->res_n_wtd + 255) / 256, 256, 0, M>>>(s, sc, r, e->res_n_wtd, e->inc_n_pods); }
+    mark("k_inc_wtd_clear");
+    k_inc_wtd_clear<<<std::min<uint32_t>(grid, (e->sl.wt_slots + 255) / 256), 256, 0, M>>>(sc, r, n.n_wtd);
+    if (n.n_wtd) {
+      mark("k_inc_wtd_insert");
+      k_inc_wtd_insert<<<std::min<uint32_t>(grid, (n.n_groups + 255) / 256 + 1), 256, 0, M>>>(s, sc, z);
+      mark("k_inc_wtd_resolve");
+      k_inc_wtd_resolve<<<std::min<uint32_t>((uint32_t)e->sm_count * 4, (n.n_pods + 255) / 256 + 1), 256, e->sl.wt_bits_n / 8, M>>>(s, sc, r, z, e->inc_n_pods);
+    }
+    e->res_n_wtd = n.n_wtd;
+    e->wtd_rebuild = false;
   }
   // (k_inc_refresh ran behind the object commits' diff kernels: the input records are current)
   mark("k_inc_admit");
@@ -1082,6 +1116,10 @@ int kr_engine_set_option(kr_engine *e, uint32_t option, uint64_t value) {
     if (e->no_incr) e->inc_valid = false;
     return KR_OK;
   }
+  if (option == KR_OPT_WTD_EDITS) {  // (read at each object commit: nothing resident depends on it)
+    e->wtd_edits = value != 0;
+    return KR_OK;
+  }
   if (option == KR_OPT_LARGE_CLUSTERS || option == KR_OPT_WIDE_CLUSTERS || option == KR_OPT_HUGE_CLUSTERS) {
     bool &on = option == KR_OPT_LARGE_CLUSTERS ? e->large_on : option == KR_OPT_WIDE_CLUSTERS ? e->wide_on : e->huge_on;
     if (on == (value != 0)) return KR_OK;
@@ -1127,6 +1165,7 @@ int kr_engine_get_option(kr_engine *e, uint32_t option, uint64_t *value) {
     case KR_OPT_LARGE_CLUSTERS: *value = e->large_on; return KR_OK;
     case KR_OPT_WIDE_CLUSTERS: *value = e->wide_on; return KR_OK;
     case KR_OPT_HUGE_CLUSTERS: *value = e->huge_on; return KR_OK;
+    case KR_OPT_WTD_EDITS: *value = e->wtd_edits; return KR_OK;
     case KR_OPT_BUCKET_STRIDE: *value = e->bstride; return KR_OK;
     default: return fail(e, KR_E_INVALID, "unknown option %u", option);
   }
@@ -1295,9 +1334,10 @@ int kr_snapshot_begin(kr_engine *e, const kr_sizes *sizes, kr_snapshot_bufs *out
   if (memcmp(&e->sizes, sizes, sizeof *sizes) != 0) {  // row counts (and, without KR_OPT_FIXED_LAYOUT, every column address) change
     e->gvalid = false;
     // The resident state of the incremental path survives new live counts under a fixed layout as long as the object tables keep
-    // their shape: pod rows appended (they arrive as committed rows), head-aux rows come and go, the JSON arena grows.
+    // their shape: pod rows appended (they arrive as committed rows), head-aux rows come and go, the JSON arena grows; with
+    // KR_OPT_WTD_EDITS workersToDelete lists grow and shrink as well (the name table is sized for the capacity).
     const bool keep = e->inc_valid && e->fixed_layout && sizes->n_clusters == e->sizes.n_clusters && sizes->n_groups == e->sizes.n_groups &&
-                      sizes->n_wtd == e->sizes.n_wtd && sizes->n_jobs == e->sizes.n_jobs && sizes->n_pods >= e->sizes.n_pods;
+                      (sizes->n_wtd == e->sizes.n_wtd || e->wtd_edits) && sizes->n_jobs == e->sizes.n_jobs && sizes->n_pods >= e->sizes.n_pods;
     if (!e->fixed_layout) { e->committed_full = false; e->inc_zero_needed = true; }
     if (!keep) {
       e->inc_valid = false;
@@ -1445,7 +1485,7 @@ int kr_snapshot_commit_parts(kr_engine *e, uint32_t parts) {
       oa.first[nc] = first;
       oa.rows_old[nc] = kCols[i].dim == D_HEADS ? e->res_n_heads : (uint32_t)dn[kCols[i].dim];
       oa.row_bytes[nc] = (uint16_t)(kCols[i].elem * kCols[i].mult);
-      oa.cls[nc] = kObjClass[i];
+      oa.cls[nc] = obj_class(i, e->wtd_edits);
       first += (uint32_t)dn[kCols[i].dim];
       nc++;
     }
@@ -1472,6 +1512,14 @@ int kr_snapshot_commit_parts(kr_engine *e, uint32_t parts) {
       e->prev_h_pod_idx.assign(hb.h_pod_idx, hb.h_pod_idx + n.n_heads);
     }
     e->res_n_heads = n.n_heads;
+    if (!e->wtd_edits) e->prev_wtd.clear();  // (the first commit after the option is turned on rebuilds the name table once)
+    else if (!wtd_lists_equal(e->prev_wtd, hb, n)) {
+      e->wtd_rebuild = true;
+      e->prev_wtd.assign(1, n.n_groups);
+      e->prev_wtd.insert(e->prev_wtd.end(), hb.g_wtd_off, hb.g_wtd_off + n.n_groups);
+      e->prev_wtd.insert(e->prev_wtd.end(), hb.g_wtd_cnt, hb.g_wtd_cnt + n.n_groups);
+      e->prev_wtd.insert(e->prev_wtd.end(), hb.w_name_id, hb.w_name_id + n.n_wtd);
+    }
   }
   CK(cudaEventRecord(e->ev_cols, e->scopy));
   if (ranges_moved) {  // digests of moved ranges are stale
@@ -1569,9 +1617,11 @@ int kr_snapshot_commit_object_rows(kr_engine *e, const uint32_t *cluster_rows, u
   bind_in(e->il, e->h_in, &hb);
   // Only an optimisation of kr_snapshot_commit_parts(KR_PART_OBJECTS): whenever the resident state cannot take the rows as they
   // are — no resident state, a Recreate gate or a JSON range that changed (hash order / digests), head rows added or removed, a
-  // group count that moved (the pipeline, the widest RayCluster and the wide set follow it) — the whole object part is committed instead.
+  // group count that moved (the pipeline, the widest RayCluster and the wide set follow it), with KR_OPT_WTD_EDITS a workersToDelete
+  // list that changed — the whole object part is committed instead.
   bool whole = !e->inc_valid || e->no_incr || !e->committed_full || e->res_n_heads != n.n_heads || e->recreate_bit.size() != n.n_clusters ||
-               e->prev_json_off.size() != n.n_clusters || e->mh_bit.size() != n.n_clusters || e->group_cnt.size() != n.n_clusters;
+               e->prev_json_off.size() != n.n_clusters || e->mh_bit.size() != n.n_clusters || e->group_cnt.size() != n.n_clusters ||
+               (e->wtd_edits && !wtd_lists_equal(e->prev_wtd, hb, n));
   for (uint32_t i = 0; i < n_cl && !whole; i++) {
     const uint32_t c = cluster_rows[i];
     if (c >= n.n_clusters) return fail(e, KR_E_INVALID, "cluster row %u out of range", c);

@@ -47,6 +47,25 @@ __device__ __forceinline__ bool cl_probe(const ScratchDev &sc, uint32_t ns, uint
   }
 }
 
+// Touches pod row p once per epoch: stamps it and appends it to the touched list (k_inc_admit re-matches it), then marks the
+// RayCluster its current device columns probe to dirty, or takes it out of the orphan count.  Those columns must still hold the
+// values its resident record was built from.  Returns false when p was touched already this epoch or was appended since the last
+// pass (n_resident rows existed then: a newer row holds nothing resident); else ns / nm are its namespace and name.
+__device__ __forceinline__ bool inc_touch(const SnapDev &s, const ScratchDev &sc, const ResDev &r, uint32_t p, uint32_t epoch, uint32_t n_resident, uint32_t &ns, uint32_t &nm) {
+  if (atomicExch(&sc.stamp[p], epoch) == epoch) return false;  // touched twice since the last pass: retired already
+  const uint32_t ti = atomicAdd(&sc.inc[KR_INC_TOUCHED], 1u);
+  sc.touched[ti] = p; sc.touched_old[ti] = KR_EMPTY32;
+  if (p >= n_resident) return false;
+  ns = s.p_ns_id[p];
+  const uint32_t cn = s.p_cluster_name_id[p];
+  nm = s.p_name_id[p];
+  const uint32_t pk = s.p_packed[p];
+  uint32_t c = 0, cflags, gname0;
+  if (cl_probe(sc, ns, cn, c, cflags, gname0)) { mark_dirty(sc, c, epoch); sc.touched_old[ti] = c; }  // (k_inc_admit rewrites the record in place if the row stays)
+  else if (!(pk & KR_PP_TOMBSTONE)) atomicSub(&r.totals[1], 1u);  // it was an orphan
+  return true;
+}
+
 // ------------------------------------------------------------------------------------------------ k_inc_retire
 // One thread per committed row, launched in front of the patch kernel: the device columns still hold the row's previous
 // values.  n_resident = pod rows that existed at the last pass (rows appended since hold nothing to retire).
@@ -54,15 +73,8 @@ __global__ void __launch_bounds__(256) k_inc_retire(const uint32_t *rows, uint32
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n_rows) return;
   const uint32_t p = rows[i];
-  const uint32_t epoch = inc_epoch(sc);
-  if (atomicExch(&sc.stamp[p], epoch) == epoch) return;  // committed twice since the last pass: retired already
-  const uint32_t ti = atomicAdd(&sc.inc[KR_INC_TOUCHED], 1u);
-  sc.touched[ti] = p; sc.touched_old[ti] = KR_EMPTY32;
-  if (p >= n_resident) return;
-  const uint32_t ns = s.p_ns_id[p], cn = s.p_cluster_name_id[p], nm = s.p_name_id[p], pk = s.p_packed[p];
-  uint32_t c = 0, cflags, gname0;
-  if (cl_probe(sc, ns, cn, c, cflags, gname0)) { mark_dirty(sc, c, epoch); sc.touched_old[ti] = c; }  // (k_inc_admit rewrites the record in place if the row stays)
-  else if (!(pk & KR_PP_TOMBSTONE)) atomicSub(&r.totals[1], 1u);  // it was an orphan
+  uint32_t ns, nm;
+  if (!inc_touch(s, sc, r, p, inc_epoch(sc), n_resident, ns, nm)) return;
   if (has_wtd) {  // names that resolved to this row: (namespace, name) is unique among live Pods, so nothing else holds them
     const uint32_t hk = hash_pair(ns, nm);
     if ((__ldcg(&sc.wt_bits[(hk & sc.wt_bits_mask) >> 5]) & (1u << (hk & 31))) && (__ldcg(&sc.wt_bits[(bloom2(hk) & sc.wt_bits_mask) >> 5]) & (1u << (bloom2(hk) & 31)))) {
@@ -77,6 +89,62 @@ __global__ void __launch_bounds__(256) k_inc_retire(const uint32_t *rows, uint32
         j = (j + 1) & sc.wt_mask;
         kk = __ldcg(&sc.wt_keys[j]);
       }
+    }
+  }
+}
+
+// ------------------------------------------------------------------------------------------------ workersToDelete edits
+// KR_OPT_WTD_EDITS: an epoch whose object commits changed a workersToDelete list (a name, a length, an offset) rebuilds the name
+// table in front of k_inc_admit, after every commit of the epoch has landed:
+//   k_inc_wtd_release  touches every row a name of the OLD table resolved to (wtd_pod_idx as the last pass left it);
+//   k_inc_wtd_clear    empties the table and its Bloom bitmap and sets the new resolutions to -1;
+//   k_inc_wtd_insert   inserts the new names (k_build_tables' group part);
+//   k_inc_wtd_resolve  probes every pod row against them, resolves wtd_pod_idx as k_match2 does and touches each row that hits.
+// k_inc_admit then rewrites each touched record with KR_ROW_WTD_OWN from the new table, and the decide kernels re-decide the
+// RayClusters those rows sit in.  k_inc_retire of this epoch's committed rows ran against the old table: its writes to wtd_pod_idx
+// are cleared here, and a committed row is stamped already, so the touches below skip it.
+__global__ void __launch_bounds__(256) k_inc_wtd_release(SnapDev s, ScratchDev sc, ResDev r, uint32_t n_wtd_old, uint32_t n_resident) {
+  const uint32_t e = blockIdx.x * blockDim.x + threadIdx.x;
+  if (e >= n_wtd_old) return;
+  const uint32_t p = r.wtd_pod_idx[e];
+  uint32_t ns, nm;
+  if (p != 0xFFFFFFFFu) inc_touch(s, sc, r, p, inc_epoch(sc), n_resident, ns, nm);
+}
+
+__global__ void __launch_bounds__(256) k_inc_wtd_clear(ScratchDev sc, ResDev r, uint32_t n_wtd) {
+  const uint32_t stride = gridDim.x * blockDim.x, t0 = blockIdx.x * blockDim.x + threadIdx.x;
+  for (uint32_t i = t0; i <= sc.wt_mask; i += stride) { sc.wt_keys[i] = KR_EMPTY64; sc.wt_head[i] = KR_EMPTY32; }
+  for (uint32_t i = t0; i < (sc.wt_bits_mask + 1) >> 5; i += stride) sc.wt_bits[i] = 0u;
+  for (uint32_t i = t0; i < n_wtd; i += stride) r.wtd_pod_idx[i] = 0xFFFFFFFFu;
+}
+
+__global__ void __launch_bounds__(256) k_inc_wtd_insert(SnapDev s, ScratchDev sc, Sizes n) {
+  for (uint32_t t = blockIdx.x * blockDim.x + threadIdx.x; t < n.n_groups; t += gridDim.x * blockDim.x) wt_insert_group(s, sc, t);
+}
+
+// grid-stride over the pod rows: 8 bytes per row and a Bloom test in shared memory (the bitmap copied per CTA, as k_match2 does)
+__global__ void __launch_bounds__(256) k_inc_wtd_resolve(SnapDev s, ScratchDev sc, ResDev r, Sizes n, uint32_t n_resident) {
+  extern __shared__ uint32_t sm_bits[];
+  const uint32_t words = (sc.wt_bits_mask + 1) >> 5;
+  for (uint32_t i = threadIdx.x; i < words; i += blockDim.x) sm_bits[i] = __ldcg(&sc.wt_bits[i]);
+  __syncthreads();
+  const uint32_t epoch = inc_epoch(sc);
+  for (uint32_t p = blockIdx.x * blockDim.x + threadIdx.x; p < n.n_pods; p += gridDim.x * blockDim.x) {
+    const uint32_t ns = __ldg(&s.p_ns_id[p]), nm = __ldg(&s.p_name_id[p]);
+    const uint32_t hk = hash_pair(ns, nm), h2 = bloom2(hk);
+    if (!(sm_bits[(hk & sc.wt_bits_mask) >> 5] & (1u << (hk & 31))) || !(sm_bits[(h2 & sc.wt_bits_mask) >> 5] & (1u << (h2 & 31)))) continue;
+    const uint64_t k = key2(ns, nm);
+    uint32_t j = hk & sc.wt_mask;
+    uint64_t kk = __ldcg(&sc.wt_keys[j]);
+    while (kk != KR_EMPTY64) {
+      if (kk == k) {
+        for (uint32_t e = __ldcg(&sc.wt_head[j]); e != KR_EMPTY32; e = __ldcg(&sc.wt_next[e])) atomicMin(&r.wtd_pod_idx[e], p);
+        uint32_t ns2, nm2;
+        inc_touch(s, sc, r, p, epoch, n_resident, ns2, nm2);
+        break;
+      }
+      j = (j + 1) & sc.wt_mask;
+      kk = __ldcg(&sc.wt_keys[j]);
     }
   }
 }

@@ -47,6 +47,33 @@ __device__ __forceinline__ void write_cl_in(const SnapDev &s, const ScratchDev &
   o[5] = w5; o[6] = w6; o[7] = make_uint4(0, 0, 0, 0);
 }
 
+// every workersToDelete name of group t: Delete(ns of the cluster, name) (raycluster_controller.go:817-822), into the name table
+// and its Bloom bitmap (cleared beforehand: keys and chain heads to 0xFF, bits to 0).  k_build_tables, and k_inc_wtd_insert when
+// an incremental epoch rebuilds the table.
+__device__ __forceinline__ void wt_insert_group(const SnapDev &s, const ScratchDev &sc, uint32_t t) {
+  uint32_t c = s.g_cluster_idx[t];
+  uint32_t ns = s.c_ns_id[c];
+  uint32_t off = s.g_wtd_off[t], cnt = s.g_wtd_cnt[t];
+  for (uint32_t w = 0; w < cnt; w++) {
+    uint32_t e = off + w;
+    uint64_t k = key2(ns, s.w_name_id[e]);
+    const uint32_t hk = hash_pair(ns, s.w_name_id[e]);
+    atomicOr(&sc.wt_bits[(hk & sc.wt_bits_mask) >> 5], 1u << (hk & 31));  // Bloom bits: k_match2 probes the table only for pods whose two bits are set
+    { const uint32_t h2 = bloom2(hk); atomicOr(&sc.wt_bits[(h2 & sc.wt_bits_mask) >> 5], 1u << (h2 & 31)); }
+    uint32_t i = hk & sc.wt_mask;
+    while (true) {
+      unsigned long long prev = atomicCAS((unsigned long long *)&sc.wt_keys[i], KR_EMPTY64, k);
+      if (prev == KR_EMPTY64 || prev == k) {
+        // push e on the slot's chain
+        uint32_t old = atomicExch(&sc.wt_head[i], e);
+        sc.wt_next[e] = old;  // KR_EMPTY32 terminates (wt_head memset to 0xFF)
+        break;
+      }
+      i = (i + 1) & sc.wt_mask;
+    }
+  }
+}
+
 // ------------------------------------------------------------------------------------------------ k_build_tables
 // One thread per cluster / workersToDelete entry / head-aux row.  Tables were memset to 0xFF.
 
@@ -82,28 +109,7 @@ __global__ void __launch_bounds__(256) k_build_tables(SnapDev s, ScratchDev sc, 
   }
   t -= n.n_clusters;
   if (t < n.n_groups) {
-    // every workersToDelete name of this group: Delete(ns of the cluster, name) (raycluster_controller.go:817-822)
-    uint32_t c = s.g_cluster_idx[t];
-    uint32_t ns = s.c_ns_id[c];
-    uint32_t off = s.g_wtd_off[t], cnt = s.g_wtd_cnt[t];
-    for (uint32_t w = 0; w < cnt; w++) {
-      uint32_t e = off + w;
-      uint64_t k = key2(ns, s.w_name_id[e]);
-      const uint32_t hk = hash_pair(ns, s.w_name_id[e]);
-      atomicOr(&sc.wt_bits[(hk & sc.wt_bits_mask) >> 5], 1u << (hk & 31));  // Bloom bits: k_match2 probes the table only for pods whose two bits are set
-      { const uint32_t h2 = bloom2(hk); atomicOr(&sc.wt_bits[(h2 & sc.wt_bits_mask) >> 5], 1u << (h2 & 31)); }
-      uint32_t i = hk & sc.wt_mask;
-      while (true) {
-        unsigned long long prev = atomicCAS((unsigned long long *)&sc.wt_keys[i], KR_EMPTY64, k);
-        if (prev == KR_EMPTY64 || prev == k) {
-          // push e on the slot's chain
-          uint32_t old = atomicExch(&sc.wt_head[i], e);
-          sc.wt_next[e] = old;  // KR_EMPTY32 terminates (wt_head memset to 0xFF)
-          break;
-        }
-        i = (i + 1) & sc.wt_mask;
-      }
-    }
+    wt_insert_group(s, sc, t);
     return;
   }
   t -= n.n_groups;

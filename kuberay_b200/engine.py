@@ -211,7 +211,8 @@ class Engine:
 
     @classmethod
     def for_snapshot(cls, snap: Snapshot, device: int = 0, max_creates: int | None = None, slack: float = 1.0,
-                     large_clusters: bool = False, wide_clusters: bool = False, huge_clusters: bool = False) -> "Engine":
+                     large_clusters: bool = False, wide_clusters: bool = False, huge_clusters: bool = False,
+                     wtd_edits: bool = False) -> "Engine":
         d = snap.dims
         up = lambda x: int(x * slack) + 1  # noqa: E731
         if max_creates is None:
@@ -224,6 +225,8 @@ class Engine:
             eng.set_wide_clusters(True)
         if huge_clusters:
             eng.set_huge_clusters(True)
+        if wtd_edits:
+            eng.set_wtd_edits(True)
         return eng
 
     def _check(self, rc: int):
@@ -265,6 +268,11 @@ class Engine:
         too (their pods are sorted tile by tile and merged) instead of sending every pass to the sort pipeline; no effect without
         it; takes effect at the next full pass."""
         self._check(self._L.kr_engine_set_option(self._h, abi.OPT_HUGE_CLUSTERS, 1 if on else 0))
+
+    def set_wtd_edits(self, on: bool = True):
+        """KR_OPT_WTD_EDITS: keep incremental epochs across scaleStrategy.workersToDelete edits (renames always, list length changes
+        under the fixed layout) instead of taking a full pass; read at each object commit."""
+        self._check(self._L.kr_engine_set_option(self._h, abi.OPT_WTD_EDITS, 1 if on else 0))
 
     def get_option(self, option: int) -> int:
         """kr_engine_get_option: an option's current value, or the read-only OPT_BUCKET_STRIDE (0: the sort pipeline)."""

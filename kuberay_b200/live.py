@@ -33,7 +33,8 @@ def _is_head(pod: dict) -> bool:
 
 class LiveArena:
     def __init__(self, clusters: list[dict], pods: list[dict], jobs: list[dict] | None = None, spare_rows: int = 64, device: int = 0,
-                 engine: bool = True, large_clusters: bool = False, wide_clusters: bool = False, huge_clusters: bool = False):
+                 engine: bool = True, large_clusters: bool = False, wide_clusters: bool = False, huge_clusters: bool = False,
+                 wtd_edits: bool = False):
         self.clusters = {(c.get("namespace", "default"), c["name"]): c for c in clusters}
         self.jobs = list(jobs or [])
         self.rows: list[dict | None] = list(pods) + [None] * spare_rows
@@ -43,6 +44,7 @@ class LiveArena:
         self.large_clusters = large_clusters  # KR_OPT_LARGE_CLUSTERS on every engine this arena creates
         self.wide_clusters = wide_clusters    # ... and KR_OPT_WIDE_CLUSTERS
         self.huge_clusters = huge_clusters    # ... and KR_OPT_HUGE_CLUSTERS
+        self.wtd_edits = wtd_edits            # ... and KR_OPT_WTD_EDITS
         self.engine: Engine | None = None
         self.stats = {"rebase": 0, "incremental": 0, "rows": 0}
         self._need_rebase = True
@@ -103,7 +105,8 @@ class LiveArena:
             if self.engine is not None:
                 self.engine.close()
             self.engine = Engine.for_snapshot(snap, device=self.device, slack=1.5, large_clusters=self.large_clusters,
-                                              wide_clusters=self.wide_clusters, huge_clusters=self.huge_clusters)
+                                              wide_clusters=self.wide_clusters, huge_clusters=self.huge_clusters,
+                                              wtd_edits=self.wtd_edits)
             self.engine.set_fixed_layout(True)
             self.views = self.engine.begin(snap.sizes())
             self.engine.fill(self.views, snap)

@@ -74,7 +74,46 @@ def incremental(snap, flags, label, large=False, wide=False, huge=False):
         eng.close()
 
 
+def wtd_edits(snap, flags, label):
+    """KR_OPT_WTD_EDITS (kr_incr.cuh): workersToDelete renames, a list grown past the old n_wtd, then every list cleared — each epoch
+    rebuilds the name table on the device (k_inc_wtd_release / _clear / _insert / _resolve)."""
+    flags.fetch_pod_lists = 0
+    d = snap.dims
+    eng = Engine(0, d["clusters"], d["groups"], d["wtd"] + 64, d["pods"], d["heads"], d["jobs"], max(1024, d["pods"]), d["json"])
+    eng.set_wtd_edits(True)
+    eng.set_fixed_layout(True)
+    try:
+        views = eng.load(snap)
+        eng.reconcile(flags)
+        inc = 0
+        names = views["p_name_id"][::97][:8].copy()
+        for step in range(3):
+            w = d["wtd"] + (4 if step == 1 else 0) if step < 2 else 0
+            cnt = np.zeros(d["groups"], dtype=np.uint32)
+            if w:
+                cnt[:] = snap.g_wtd_cnt
+                cnt[0] += w - d["wtd"]
+            s2 = synthetic.Snapshot(d["clusters"], d["groups"], w, d["pods"], d["heads"], d["jobs"], d["json"])
+            for c, _dt, _m, dim in abi.COLUMNS:
+                if dim not in ("wtd", "json"):
+                    s2.cols[c][:] = views[c]
+            s2.g_wtd_cnt[:] = cnt
+            s2.g_wtd_off[:] = np.concatenate([[0], np.cumsum(cnt)[:-1]]).astype(np.uint32)
+            s2.w_name_id[:] = np.resize(names, w) if w else 0
+            views = eng.begin(s2.sizes())
+            for c, _dt, _m, dim in abi.COLUMNS:
+                if dim not in ("pods", "json"):
+                    np.copyto(views[c], s2.cols[c])
+            eng.commit(abi.PART_OBJECTS)
+            inc += eng.reconcile(flags).changed_clusters is not None
+        print(label, "ok:", inc, "of 3 epochs incremental", flush=True)
+    finally:
+        eng.close()
+
+
 def main():
+    wtd_edits(*synthetic.generate(synthetic.config("C2", n_clusters=300, pods_per_cluster=20, groups=2, autoscaling_frac=1.0, wtd_group_frac=0.3)),
+              "workersToDelete edits")
     incremental(*synthetic.generate(synthetic.config("C2", n_clusters=300, pods_per_cluster=20, groups=2, jobs=True, wtd_group_frac=0.3)), "incremental epochs")
     incremental(*synthetic.generate(synthetic.config("C2", n_clusters=300, pods_per_cluster=41, groups=2, wtd_group_frac=0.3, multihost_frac=0.5)),
                 "incremental epochs, multi-host groups")
