@@ -25,7 +25,11 @@ extern "C" {
 #endif
 
 /* Interner convention: id 0 = "absent" (label/annotation/field not present), id 1 = the empty string "".
- * In HeadInfo-like fields (pod IP, names, service IP) the empty string MUST be encoded as 0. */
+ * In HeadInfo-like fields (pod IP, names, service IP) the empty string MUST be encoded as 0.
+ * Id domain: every other id is an opaque u32 in [2, 0xFFFFFFFE]; the engine compares ids only for equality, so any assignment of
+ * distinct values gives the same decisions.  0xFFFFFFFF is not an id: the engine's join tables and the oracle's map mark an empty
+ * slot with the all-ones key, so a (namespace, name) pair of two 0xFFFFFFFF ids would read as an empty slot.  The packers never
+ * produce it. */
 #define KR_ID_ABSENT 0u
 #define KR_ID_EMPTY_STRING 1u
 

@@ -711,21 +711,10 @@ __global__ void __launch_bounds__(kDecideWarps * 32) k_decide(DecideArgs a) {
   const uint32_t Nc = a.n.n_clusters, Np = a.n.n_pods;
   if (a.fast && KR_ATTEMPT_VOID(a.r.totals)) return;
   uint32_t c = blockIdx.x * kDecideWarps + warp;
-  if (a.phase == 1) {  // compact list of the clusters phase 0 deferred
-    if (c >= a.r.totals[4]) return;
-    c = a.sc.deferred_list[c];
-  } else if (c > Nc) return;
-
-  uint32_t seg0, seg1;
-  if (a.fast) { seg0 = LDG(a.sc.cstart[c]); seg1 = LDG(a.sc.cstart[c + 1]); }
-  else {
-    seg0 = warp_lower_bound(a.sorted_keys, Np, c, lane);
-    seg1 = (c == Nc) ? Np : warp_lower_bound(a.sorted_keys, Np, c + 1, lane);
-  }
-  const uint32_t P = seg1 - seg0;
   if (a.phase == 0) {
     // The orphans' segment: pods whose (namespace, ray.io/cluster) names no RayCluster in the snapshot, and the free rows of an
-    // incrementally maintained arena (KR_PP_TOMBSTONE; there can be many).  Every warp of the grid labels a strided share.
+    // incrementally maintained arena (KR_PP_TOMBSTONE; there can be many).  Every warp of the grid labels a strided share — the
+    // warps past the last cluster of the rounded-up grid as well, so this comes before their early return.
     const uint32_t o0 = a.fast ? LDG(a.sc.cstart[Nc]) : warp_lower_bound(a.sorted_keys, Np, Nc, lane);
     const uint32_t gw = blockIdx.x * kDecideWarps + warp, nw = gridDim.x * kDecideWarps;
     uint32_t real = 0;
@@ -739,6 +728,18 @@ __global__ void __launch_bounds__(kDecideWarps * 32) k_decide(DecideArgs a) {
     real = __reduce_add_sync(0xFFFFFFFFu, real);
     if (lane == 0 && real) atomicAdd(&a.r.totals[1], real);
   }
+  if (a.phase == 1) {  // compact list of the clusters phase 0 deferred
+    if (c >= a.r.totals[4]) return;
+    c = a.sc.deferred_list[c];
+  } else if (c > Nc) return;
+
+  uint32_t seg0, seg1;
+  if (a.fast) { seg0 = LDG(a.sc.cstart[c]); seg1 = LDG(a.sc.cstart[c + 1]); }
+  else {
+    seg0 = warp_lower_bound(a.sorted_keys, Np, c, lane);
+    seg1 = (c == Nc) ? Np : warp_lower_bound(a.sorted_keys, Np, c + 1, lane);
+  }
+  const uint32_t P = seg1 - seg0;
   if (c == Nc) return;
   if (small_path(a, c, P)) return;  // k_decide_small owns it
   // fast pipeline, phase 0: informer List order inside the bucket = ascending pod index (phase 1 finds it already sorted)
