@@ -403,7 +403,8 @@ typedef struct kr_profile {
   uint32_t n_kernels;                       /* kernels launched by the last batch (our own, not library) */
   float    kernel_ms[KR_MAX_KERNEL_TIMES];  /* valid only after kr_reconcile_batch_profiled */
   const char *kernel_name[KR_MAX_KERNEL_TIMES];
-  uint64_t h2d_bytes, d2h_bytes;            /* bytes uploaded by the commits since the previous pass / moved by the last results fetch */
+  uint64_t h2d_bytes, d2h_bytes;            /* bytes uploaded by the commits since the previous pass (after a pass: plus the hash order it
+                                               uploaded itself) / moved by the last results fetch */
 } kr_profile;
 
 /* --------------------------------------------------------- entry points */
@@ -462,6 +463,22 @@ int kr_snapshot_commit_pod_values(kr_engine *e, const uint32_t *rows, const uint
  * updates and head Pod status updates at a few hundred bytes per object instead of the whole object part: whenever the engine has
  * no resident state, or a Recreate gate, a JSON range or the number of head rows changed, it commits the whole object part itself. */
 int kr_snapshot_commit_object_rows(kr_engine *e, const uint32_t *cluster_rows, uint32_t n_cluster_rows, const uint32_t *head_rows, uint32_t n_head_rows);
+
+/* Row-granular spec commit: the caller rewrote, in the pinned arenas, the muted-spec JSON of the RayClusters `cluster_rows` — in
+ * place or at a new 16-byte aligned range inside the live json_bytes — and their c_json_off / c_json_len.  Only those ranges
+ * (padded to 16 bytes) and those two column entries travel; the next pass re-hashes only these messages and re-decides only those
+ * of them whose Recreate gate reads the digest.  Results equal kr_snapshot_commit_parts(KR_PART_JSON).  Rows may repeat and may be
+ * given in several calls per epoch (the engine takes the union); `cluster_rows` is copied before the call returns.  The device
+ * pulls the ranges from the arenas asynchronously: do not rewrite them until the next pass has returned.  Call it BEFORE the
+ * epoch's object commit (kr_snapshot_commit_parts(KR_PART_OBJECTS) / kr_snapshot_commit_object_rows): an object commit that finds a
+ * moved range re-hashes every RayCluster — correct, only slower.  A whole-arena commit (KR_PART_JSON) in the same epoch wins.
+ * A row listed again before the pass that hashes it is pulled once per pass in between (after a skip_hash pass, which leaves the rows
+ * pending, the caller may have rewritten it) and hashed once.  kr_profile.h2d_bytes counts 16 B per pulled row (row id, offset,
+ * length) plus its padded range, and, at the pass that hashes them, 4 B per row for their hash order (the pending rows sorted by
+ * SHA-1 block count, uploaded once).
+ * KR_E_STATE before a full commit of the layout; KR_E_INVALID for a row >= n_clusters, an offset that is not 16-byte aligned or a
+ * range past json_bytes (nothing is committed then). */
+int kr_snapshot_commit_spec_rows(kr_engine *e, const uint32_t *cluster_rows, uint32_t n);
 
 /* Run the whole decision + status pass over the committed snapshot and copy the results back.
  * Replaces the decision halves of reconcilePods (raycluster_controller.go:619-935), reconcileMultiHostWorkerGroup
@@ -542,7 +559,7 @@ enum {
                               sends every pass to the sort / radix pipelines).  May be set at any time; takes effect at the next full
                               pass.  Turning it on allocates the tile scratch once, for the capacities: about 18 B per max_pods of device
                               memory (at least 128 KB). */
-  KR_OPT_WTD_EDITS = 7        /* 1: an edit of a scaleStrategy.workersToDelete list (a name renamed, a list grown or shrunk, as the
+  KR_OPT_WTD_EDITS = 7,       /* 1: an edit of a scaleStrategy.workersToDelete list (a name renamed, a list grown or shrunk, as the
                               autoscaler writes on every scale-down and clears once the Pods are gone) keeps the incremental epoch: the
                               next pass rebuilds the name table on the device and re-decides only the RayClusters whose Pods were named
                               before or are named now.  A list whose length changes moves n_wtd, which needs KR_OPT_FIXED_LAYOUT (without
@@ -550,6 +567,9 @@ enum {
                               any such edit makes the next pass a full one).  May be set at any time; read at each object commit.
                               kr_snapshot_commit_object_rows still expects unchanged lists: with this option, rows whose lists changed
                               are committed as the whole object part. */
+  KR_OPT_SPEC_ROWS = 8        /* 1: the native packer (kr_packer_flush) commits re-emitted specs with kr_snapshot_commit_spec_rows and
+                              reports KR_PACK_SPEC_ROWS instead of KR_PART_JSON (a flush that compacts the JSON arena still sends
+                              KR_PART_JSON).  The engine call itself needs no option.  Results are the same as with 0 (the default). */
 };
 enum { KR_LARGE_MAX_PODS = 8192 };  /* largest RayCluster KR_OPT_LARGE_CLUSTERS keeps on the bucket pipeline */
 int kr_engine_set_option(kr_engine *e, uint32_t option, uint64_t value);
@@ -657,7 +677,7 @@ typedef struct kr_cluster_obj {
 } kr_cluster_obj;
 typedef struct kr_job_obj { kr_str ns, name, cluster_name, status_summary; } kr_job_obj;
 typedef struct kr_packer kr_packer;
-enum { KR_PACK_POD_ROWS = 8, KR_PACK_FULL = 16, KR_PACK_OBJECT_ROWS = 32 };  /* kr_packer_flush mode bits, beside KR_PART_OBJECTS / KR_PART_JSON (OBJECT_ROWS: kr_snapshot_commit_object_rows instead of the whole object part) */
+enum { KR_PACK_POD_ROWS = 8, KR_PACK_FULL = 16, KR_PACK_OBJECT_ROWS = 32, KR_PACK_SPEC_ROWS = 64 };  /* kr_packer_flush mode bits, beside KR_PART_OBJECTS / KR_PART_JSON (OBJECT_ROWS: kr_snapshot_commit_object_rows instead of the whole object part; SPEC_ROWS: kr_snapshot_commit_spec_rows instead of KR_PART_JSON, with KR_OPT_SPEC_ROWS) */
 int        kr_packer_create(const kr_config *capacities, kr_packer **out);
 void       kr_packer_destroy(kr_packer *p);
 kr_engine *kr_packer_engine(kr_packer *p);

@@ -141,6 +141,7 @@ const (
 	OptWideClusters  = uint32(C.KR_OPT_WIDE_CLUSTERS)
 	OptHugeClusters  = uint32(C.KR_OPT_HUGE_CLUSTERS)
 	OptWtdEdits      = uint32(C.KR_OPT_WTD_EDITS)
+	OptSpecRows      = uint32(C.KR_OPT_SPEC_ROWS)
 )
 
 // SetOption: KR_OPT_FIXED_LAYOUT (before the first Begin), KR_OPT_INCREMENTAL, KR_OPT_LARGE_CLUSTERS (1: RayClusters of 257 to
@@ -148,7 +149,9 @@ const (
 // effect at the next full pass), KR_OPT_WIDE_CLUSTERS (1: the same for RayClusters with more than 32 worker groups; takes effect
 // at the next full pass), KR_OPT_HUGE_CLUSTERS (1, with KR_OPT_LARGE_CLUSTERS: the same for RayClusters of more than
 // KR_LARGE_MAX_PODS pods; takes effect at the next full pass), KR_OPT_WTD_EDITS (1: scaleStrategy.workersToDelete edits keep
-// incremental epochs; recommended for autoscaling fleets; read at each object commit).  For a Packer, call it on Packer.Engine().
+// incremental epochs; recommended for autoscaling fleets; read at each object commit), KR_OPT_SPEC_ROWS (1: Packer.Flush commits
+// re-emitted specs with CommitSpecRows instead of the whole JSON arena and reports PackSpecRows).  For a Packer, call it on
+// Packer.Engine().
 func (e *Engine) SetOption(option uint32, value uint64) error {
 	if rc := C.kr_engine_set_option(e.h, C.uint32_t(option), C.uint64_t(value)); rc != C.KR_OK {
 		return e.err(rc)
@@ -220,6 +223,19 @@ func (e *Engine) CommitObjectRows(clusterRows, headRows []uint32) error {
 		hp = (*C.uint32_t)(unsafe.Pointer(&headRows[0]))
 	}
 	if rc := C.kr_snapshot_commit_object_rows(e.h, cp, C.uint32_t(len(clusterRows)), hp, C.uint32_t(len(headRows))); rc != C.KR_OK {
+		return e.err(rc)
+	}
+	return nil
+}
+
+// CommitSpecRows uploads only the muted-spec JSON ranges (and c_json_off / c_json_len) of the RayClusters whose spec was rewritten
+// in the arenas; the next pass re-hashes only them.  Call it before CommitParts(KR_PART_OBJECTS) / CommitObjectRows; the arenas must
+// not be rewritten until the next pass has returned.  clusterRows is ordinary Go memory without pointers: C copies it before returning.
+func (e *Engine) CommitSpecRows(clusterRows []uint32) error {
+	if len(clusterRows) == 0 {
+		return nil
+	}
+	if rc := C.kr_snapshot_commit_spec_rows(e.h, (*C.uint32_t)(unsafe.Pointer(&clusterRows[0])), C.uint32_t(len(clusterRows))); rc != C.KR_OK {
 		return e.err(rc)
 	}
 	return nil

@@ -182,7 +182,11 @@ func (p *Packer) DeleteJob(ns, name string) error {
 	return nil
 }
 
-// Flush uploads what moved since the last flush; mode reports how (KR_PACK_FULL | KR_PACK_POD_ROWS | KR_PACK_OBJECT_ROWS | KR_PART_*).
+// PackSpecRows is the Flush mode bit of a flush that committed re-emitted specs row by row (OptSpecRows) instead of KR_PART_JSON.
+const PackSpecRows = uint32(C.KR_PACK_SPEC_ROWS)
+
+// Flush uploads what moved since the last flush; mode reports how (KR_PACK_FULL | KR_PACK_POD_ROWS | KR_PACK_OBJECT_ROWS |
+// KR_PACK_SPEC_ROWS | KR_PART_*).
 func (p *Packer) Flush() (mode uint32, err error) {
 	var m C.uint32_t
 	if rc := C.kr_packer_flush(p.h, &m); rc != C.KR_OK {

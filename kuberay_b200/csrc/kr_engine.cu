@@ -33,6 +33,13 @@ namespace {
 constexpr size_t kAlign = 256;
 inline size_t align_up(size_t x, size_t a = kAlign) { return (x + a - 1) / a * a; }
 inline uint32_t pow2_at_least(uint64_t x) { uint32_t p = 16; while (p < x) p <<= 1; return p; }
+// staging of an incremental pass's changed records: [meta 32 B | cluster record] x capc, group records x capg, then the re-hashed
+// digests of a spec-row epoch (32 B x capc); returns the bytes, *dig_off the digests' offset
+size_t inc_stage_bytes(uint32_t capc, uint32_t capg, size_t *dig_off) {
+  const size_t d = align_up(32 * (size_t)capc) + align_up(sizeof(kr_cluster_result) * (size_t)capc) + align_up(sizeof(kr_group_result) * (size_t)capg);
+  *dig_off = d;
+  return d + 32 * (size_t)capc + 1024;
+}
 
 // bucket stride of a new layout: a power of two with 25 % head room over the mean cluster size (a cluster that outgrows it voids the
 // attempt; the pass then widens the stride, up to 256, or leaves the bucket pipeline for this layout)
@@ -84,7 +91,8 @@ static const uint8_t kObjClass[kNumCols] = {
         KR_OC_HEADKEY, KR_OC_HEAD, KR_OC_HEAD, KR_OC_HEAD, KR_OC_HEAD, KR_OC_HEAD, KR_OC_HEAD, KR_OC_HEAD,
         KR_OC_COPY, KR_OC_COPY, KR_OC_COPY, KR_OC_COPY,
         0};
-constexpr int kHeadKeyCol = 39, kGroupClusterCol = 22;
+constexpr int kHeadKeyCol = 39, kGroupClusterCol = 22, kJsonOffCol = 9;
+static_assert(kCols[kJsonOffCol].elem == 8 && kCols[kJsonOffCol + 1].elem == 4 && kCols[kJsonOffCol + 1].dim == D_CLUSTERS, "c_json_off / c_json_len column indices");
 static_assert(kCols[kHeadKeyCol].dim == D_HEADS && kCols[kHeadKeyCol - 1].dim == D_PODS && kCols[kGroupClusterCol].dim == D_GROUPS && kCols[kGroupClusterCol - 1].dim == D_CLUSTERS, "column indices of the object diff");
 // g_wtd_off, g_wtd_cnt, w_name_id.  With KR_OPT_WTD_EDITS a staged object commit classifies them as copy / group / copy instead:
 // the next pass rebuilds the name table and recomputes KR_ROW_WTD_OWN (the only use of the offsets), and the multi-host decide
@@ -340,6 +348,21 @@ struct kr_engine {
   bool inc_gathered = false;     // ... and their records sit packed in the staging buffer
   bool inc_hash_ran = false;
   std::vector<uint64_t> prev_json_off; std::vector<uint32_t> prev_json_len;  // JSON ranges the digests were computed from
+  // kr_snapshot_commit_spec_rows, pinned mirror and device copy of {pull rows u32 | lens u32 | offs u64 | hash order u32}[max_clusters]:
+  // each call appends the rows it pulls to the pull lists; the pass that hashes them sorts the pending rows once and uploads them as
+  // the hash order
+  uint8_t *h_spec = nullptr, *d_spec = nullptr;
+  uint32_t n_pull = 0;                 // pull-list entries since the last pass
+  std::vector<uint32_t> spec_pending;  // rows listed since the last pass that hashed (each once)
+  std::vector<uint32_t> spec_stamp;    // cluster row -> spec_epoch that listed it (the union of the calls until they are hashed)
+  uint32_t spec_epoch = 1;
+  std::vector<uint32_t> pull_stamp;    // cluster row -> pull_epoch that pulled it: a pass in between lets the caller rewrite the arena,
+  uint32_t pull_epoch = 1;             // so a row listed again after a pass (skip_hash leaves it pending) is pulled again
+  bool spec_order_stale = false;       // a spec commit changed a block count the full-pass hash order (d_order) was built from
+  bool spec_rows_opt = false;          // KR_OPT_SPEC_ROWS (read by kr_packer_flush)
+  uint32_t inc_spec_n = 0;             // rows the last incremental pass re-hashed ...
+  bool inc_spec_gathered = false;      // ... and their digests sit packed in the staging buffer
+  std::vector<uint32_t> spec_hashed;   // ... which rows (the fetch scatters the digests)
   uint8_t *d_obj_stage = nullptr; size_t obj_stage_cap = 0;   // KR_PART_OBJECTS uploads land here while the state is resident
   uint8_t *d_inc_stage = nullptr, *h_inc_stage = nullptr; size_t inc_stage_cap = 0; uint32_t inc_stage_clusters = 0, inc_stage_groups = 0;
   uint32_t *h_inc = nullptr;     // pinned copy of the epoch counters (16 words) + the changed-cluster list
@@ -503,6 +526,72 @@ int upload_lg(kr_engine *e) {
   CK(cudaMemcpyAsync(e->d_lg + align_up(16 * (size_t)e->cfg.max_clusters), e->h_lg_list.data(), 4 * e->h_lg_list.size(), cudaMemcpyHostToDevice, e->sm));
   if (!e->h_tiles.empty()) CK(cudaMemcpyAsync(e->d_huge, e->h_tiles.data(), 16 * e->h_tiles.size(), cudaMemcpyHostToDevice, e->sm));
   return KR_OK;
+}
+
+// hash order: message ids by descending SHA-1 block count (counting sort; the kernels run length-homogeneous warps, longest first).
+// The RayClusters whose Recreate gate compares a digest lead the order: their digests are ready when the decide kernel, running
+// beside the hash, gets to them (k_decide2 waits for a digest's last word otherwise).  Fills h_order (no upload still reading it).
+void build_order(kr_engine *e, const kr_snapshot_bufs &hb) {
+  const kr_sizes &n = e->sizes;
+  uint32_t maxb = 0;
+  for (uint32_t c = 0; c < n.n_clusters; c++) maxb = std::max(maxb, (hb.c_json_len[c] + 8) / 64 + 1);
+  auto blocks_of = [&](uint32_t c) { return (hb.c_json_len[c] + 8) / 64 + 1; };
+  auto lead = [&](uint32_t c) { return (hb.c_flags[c] & KR_CF_UPGRADE_RECREATE) ? 0u : 1u; };
+  if (maxb <= (1u << 20)) {  // counting sort on (not Recreate, descending block count): bucket 0 = the longest Recreate message
+    std::vector<uint32_t> start(2 * ((size_t)maxb + 1) + 1, 0);
+    auto key = [&](uint32_t c) { return lead(c) * (maxb + 1) + (maxb - blocks_of(c)); };
+    for (uint32_t c = 0; c < n.n_clusters; c++) start[key(c) + 1]++;
+    for (size_t b = 0; b + 1 < start.size(); b++) start[b + 1] += start[b];
+    for (uint32_t c = 0; c < n.n_clusters; c++) e->h_order[start[key(c)]++] = c;
+  } else {
+    for (uint32_t c = 0; c < n.n_clusters; c++) e->h_order[c] = c;
+    std::stable_sort(e->h_order, e->h_order + n.n_clusters, [&](uint32_t a, uint32_t b) { return lead(a) != lead(b) ? lead(a) < lead(b) : blocks_of(a) > blocks_of(b); });
+  }
+}
+
+// Spec-row commits keep the full-pass hash order as it was; a pass that hashes every message rebuilds it first when their block
+// counts moved (uploaded on stream M, ahead of the pass).
+int refresh_order(kr_engine *e) {
+  e->spec_order_stale = false;
+  if (!e->sizes.n_clusters) return KR_OK;
+  if (e->order_pending) { CK(cudaEventSynchronize(e->ev_order)); e->order_pending = false; }
+  kr_snapshot_bufs hb;
+  bind_in(e->il, e->h_in, &hb);
+  build_order(e, hb);
+  CK(cudaMemcpyAsync(e->d_order, e->h_order, 4 * (size_t)e->sizes.n_clusters, cudaMemcpyHostToDevice, e->sm));
+  CK(cudaEventRecord(e->ev_order, e->sm));
+  e->order_pending = true;
+  e->prof.h2d_bytes = (e->h2d_accum += 4 * (uint64_t)e->sizes.n_clusters);  // (as when a commit uploads the order)
+  return KR_OK;
+}
+
+// the spec rows were hashed (or every message was): a new epoch of the row stamps
+void clear_spec_rows(kr_engine *e) {
+  e->spec_pending.clear();
+  if (++e->spec_epoch == 0) { std::fill(e->spec_stamp.begin(), e->spec_stamp.end(), 0u); e->spec_epoch = 1; }
+}
+
+// every pass: the caller may rewrite the arenas once it returns, so the next spec commit pulls its rows again (the pass waits for
+// the pulls enqueued so far: their pinned list entries are free again)
+void new_pull_epoch(kr_engine *e) {
+  e->n_pull = 0;
+  if (++e->pull_epoch == 0) { std::fill(e->pull_stamp.begin(), e->pull_stamp.end(), 0u); e->pull_epoch = 1; }
+}
+
+// The hash order of the pending spec rows (descending SHA-1 block count, so warps are length-homogeneous), uploaded on stream M ahead
+// of the pass that hashes them; returns its device address.
+const uint32_t *upload_spec_order(kr_engine *e) {
+  const size_t cap = (size_t)e->cfg.max_clusters + 1;
+  kr_snapshot_bufs hb;
+  bind_in(e->il, e->h_in, &hb);
+  uint32_t *h = reinterpret_cast<uint32_t *>(e->h_spec + 16 * cap);
+  const uint32_t n = (uint32_t)e->spec_pending.size();
+  std::copy(e->spec_pending.begin(), e->spec_pending.end(), h);
+  std::stable_sort(h, h + n, [&](uint32_t a, uint32_t b) { return (hb.c_json_len[a] + 8) / 64 > (hb.c_json_len[b] + 8) / 64; });
+  uint32_t *d = reinterpret_cast<uint32_t *>(e->d_spec + 16 * cap);
+  if (cudaMemcpyAsync(d, h, 4 * (size_t)n, cudaMemcpyHostToDevice, e->sm) != cudaSuccess) return nullptr;
+  e->prof.h2d_bytes = (e->h2d_accum += 4 * (uint64_t)n);  // (the pass's own upload: reported with the commits that fed it)
+  return d;
 }
 
 // Launches the whole pass.  profile: serialise everything on stream M and bracket each kernel with events.
@@ -814,7 +903,7 @@ void after_full_pass(kr_engine *e, const kr_flags &f) {
   e->inc_flags = f; e->inc_n_pods = e->sizes.n_pods; e->inc_n_heads = e->sizes.n_heads;
   e->host_results_stale = false; e->inc_n_dirty = 0; e->fetched = false; e->ran_inc = false; e->heads_rebuild = false;
   e->wtd_rebuild = false; e->res_n_wtd = e->sizes.n_wtd;
-  if (!f.skip_hash) e->hash_dirty = false;
+  if (!f.skip_hash) { e->hash_dirty = false; clear_spec_rows(e); }
 }
 
 // One incremental pass over the resident state (kr_incr.cuh).  Returns KR_OK with *done_inc = true when its results stand;
@@ -839,17 +928,25 @@ int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile
   e->prof.n_kernels = 0;
   CK(cudaStreamWaitEvent(M, e->ev_cols, 0));
   const bool do_hash = e->hash_dirty && !f.skip_hash && n.n_clusters > 0;
-  if (do_hash) {  // the spec JSON was committed again: every digest is recomputed (on its own stream), every Recreate gate re-read
+  // ... or only the messages kr_snapshot_commit_spec_rows listed (a whole-arena commit wins; a skip_hash pass leaves them pending)
+  const uint32_t n_rows = (!e->hash_dirty && !f.skip_hash) ? (uint32_t)e->spec_pending.size() : 0;
+  const uint32_t *spec_rows = n_rows ? upload_spec_order(e) : nullptr;
+  if (n_rows && !spec_rows) return fail(e, KR_E_CUDA, "upload of the spec rows' hash order failed");
+  if (do_hash && e->spec_order_stale) if (int rc = refresh_order(e)) return rc;
+  if (do_hash || n_rows) {  // the spec JSON was committed again: the digests are recomputed (on their own stream), the Recreate gates re-read
+    const uint32_t *order = do_hash ? e->d_order : spec_rows;
+    const uint32_t nm = do_hash ? n.n_clusters : n_rows;
     if (!profile) { CK(cudaEventRecord(e->ev_fork, M)); CK(cudaStreamWaitEvent(H, e->ev_fork, 0)); }
     CK(cudaStreamWaitEvent(H, e->ev_json, 0));
-    if (profile) mark("k_hash");
-    const uint32_t ngroups = (n.n_clusters + 31) / 32;
+    if (profile) mark(do_hash ? "k_hash" : "k_hash_rows");
+    const uint32_t ngroups = (nm + 31) / 32;
     if (ngroups <= (uint32_t)e->sm_count * 4)
-      k_hash3<1, 0><<<std::min<uint32_t>(ngroups, (uint32_t)e->sm_count * 2), 64, sizeof(H3Smem), H>>>(s.json, s.c_json_off, s.c_json_len, e->d_order, n.n_clusters, r.hash);
+      k_hash3<1, 0><<<std::min<uint32_t>(ngroups, (uint32_t)e->sm_count * 2), 64, sizeof(H3Smem), H>>>(s.json, s.c_json_off, s.c_json_len, order, nm, r.hash);
     else
-      k_hash2<4, 1><<<std::min<uint32_t>((n.n_clusters + 127) / 128, (uint32_t)e->sm_count * e->hash_ctas_per_sm), 128, 0, H>>>(s.json, s.c_json_off, s.c_json_len, e->d_order, n.n_clusters, r.hash, 1u);
+      k_hash2<4, 1><<<std::min<uint32_t>((nm + 127) / 128, (uint32_t)e->sm_count * e->hash_ctas_per_sm), 128, 0, H>>>(s.json, s.c_json_off, s.c_json_len, order, nm, r.hash, 1u);
     if (!profile) CK(cudaEventRecord(e->ev_hash, H));
-    if (e->n_recreate) { mark("k_inc_mark_recreate"); k_inc_mark_recreate<<<(n.n_clusters + 255) / 256, 256, 0, M>>>(s, sc, z); }
+    if (e->n_recreate && do_hash) { mark("k_inc_mark_recreate"); k_inc_mark_recreate<<<(n.n_clusters + 255) / 256, 256, 0, M>>>(s, sc, z); }
+    if (e->n_recreate && !do_hash) { mark("k_inc_mark_rows"); k_inc_mark_rows<<<(n_rows + 255) / 256, 256, 0, M>>>(s, sc, spec_rows, n_rows); }
   }
   const int grid = e->sm_count * 2;
   if (e->heads_rebuild) {  // a head Pod came or went since the table was built (the commit compared the keys on the host)
@@ -873,12 +970,13 @@ int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile
   // (k_inc_refresh ran behind the object commits' diff kernels: the input records are current)
   mark("k_inc_admit");
   k_inc_admit<<<grid, 256, 0, M>>>(s, sc, r, z, n.n_wtd ? 1 : 0);
-  if (do_hash && !profile) CK(cudaStreamWaitEvent(M, e->ev_hash, 0));
+  if ((do_hash || n_rows) && !profile) CK(cudaStreamWaitEvent(M, e->ev_hash, 0));
   // staging for the changed records: up to a quarter of the RayClusters (beyond that the whole record arrays are as cheap to move)
   IncStage st{};
+  size_t dig_off = 0;
   {
     const uint32_t capc = std::max<uint32_t>(64, n.n_clusters / 4), capg = (uint32_t)std::min<uint64_t>((uint64_t)capc * KR_SMEM_GROUPS, (uint64_t)n.n_groups + 1);
-    const size_t need = align_up(32 * (size_t)capc) + align_up(sizeof(kr_cluster_result) * (size_t)capc) + sizeof(kr_group_result) * (size_t)capg + 1024;
+    const size_t need = inc_stage_bytes(capc, capg, &dig_off);
     if (need > e->inc_stage_cap) {
       if (e->d_inc_stage) cudaFree(e->d_inc_stage);
       if (e->h_inc_stage) cudaFreeHost(e->h_inc_stage);
@@ -892,6 +990,11 @@ int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile
     st.clusters = reinterpret_cast<kr_cluster_result *>(e->d_inc_stage + align_up(32 * (size_t)capc));
     st.groups = reinterpret_cast<kr_group_result *>(e->d_inc_stage + align_up(32 * (size_t)capc) + align_up(sizeof(kr_cluster_result) * (size_t)capc));
     st.cap_clusters = capc; st.cap_groups = capg;
+  }
+  const bool gather_rows = n_rows && n_rows <= e->inc_stage_clusters;  // (more re-hashed digests than that: the fetch copies them all)
+  if (gather_rows) {
+    mark("k_inc_digest_gather");
+    k_inc_digest_gather<<<(2 * n_rows + 255) / 256, 256, 0, M>>>(spec_rows, n_rows, r.hash, reinterpret_cast<char *>(e->d_inc_stage + dig_off));
   }
   if (n.n_clusters) {
     Decide2Args da{s, sc, r, z, f, st, e->cfg.max_creates, 0, 2};
@@ -939,6 +1042,12 @@ int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile
   e->inc_gathered = e->inc_n_dirty <= e->inc_stage_clusters && e->h_inc[KR_INC_GROUPS] <= e->inc_stage_groups;
   e->inc_hash_ran = do_hash;
   if (do_hash) e->hash_dirty = false;
+  e->inc_spec_n = n_rows; e->inc_spec_gathered = gather_rows;
+  if (n_rows) {
+    const uint32_t *h = reinterpret_cast<const uint32_t *>(e->h_spec + 16 * ((size_t)e->cfg.max_clusters + 1));
+    e->spec_hashed.assign(h, h + n_rows);
+  }
+  if (do_hash || n_rows) clear_spec_rows(e);
   e->ran_inc = true;
   *done_inc = true;
   return KR_OK;
@@ -948,6 +1057,7 @@ int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile
 // switches this layout to the radix pipeline and runs again.  Leaves the stream synchronised (after an incremental pass only its one-thread epoch-closing kernel may still be in flight: it touches the epoch counters, nothing a reader of the results sees).
 int run_pass(kr_engine *e, const kr_flags &f, cudaEvent_t done) {
   e->last_flags = f;
+  new_pull_epoch(e);
   // (the list moves only with a group count, which no incremental epoch absorbs, an option or a new layout: a full pass follows)
   if (e->lg_stale) if (int rc = upload_lg(e)) return rc;
   if (e->inc_valid && !e->no_incr && memcmp(&e->inc_flags, &f, sizeof f) == 0) {
@@ -960,6 +1070,7 @@ int run_pass(kr_engine *e, const kr_flags &f, cudaEvent_t done) {
     CK(cudaMemsetAsync(e->d_scratch + e->sl.inc_zero, 0, e->sl.inc_zero_end - e->sl.inc_zero, e->sm));
     e->inc_zero_needed = false;
   }
+  if (e->spec_order_stale && !f.skip_hash) if (int rc = refresh_order(e)) return rc;
   for (int attempt = 0; attempt < 5; attempt++) {
     int rc = run_pass_once(e, f);
     if (rc) return rc;
@@ -1007,6 +1118,9 @@ int fetch_results(kr_engine *e, kr_results_view *out) {
   uint64_t bytes = 0;
   const uint32_t nd = e->inc_n_dirty, ngr = inc ? e->h_inc[KR_INC_GROUPS] : 0;
   const size_t st_cl = align_up(32 * (size_t)e->inc_stage_clusters), st_gr = st_cl + align_up(sizeof(kr_cluster_result) * (size_t)e->inc_stage_clusters);
+  size_t st_dig;
+  inc_stage_bytes(e->inc_stage_clusters, e->inc_stage_groups, &st_dig);
+  const bool spec_packed = packed && e->inc_spec_n && e->inc_spec_gathered && !e->inc_hash_ran;
   if (packed) {
     // incremental pass: the changed cluster / group records come back packed (k_inc_gather) and are scattered into the host
     // arena below; the flat arrays an epoch can touch anywhere (name resolutions, RayJob rows, digests when they were
@@ -1020,7 +1134,11 @@ int fetch_results(kr_engine *e, kr_results_view *out) {
     CK(cudaMemcpyAsync(e->h_out + e->ol.totals, e->d_out + e->ol.totals, 256, cudaMemcpyDeviceToHost, e->sm));
     if (n.n_wtd) { CK(cudaMemcpyAsync(e->h_out + e->ol.wtd, e->d_out + e->ol.wtd, 4 * (size_t)n.n_wtd, cudaMemcpyDeviceToHost, e->sm)); bytes += 4ull * n.n_wtd; }
     if (n.n_jobs) { CK(cudaMemcpyAsync(e->h_out + e->ol.jobs, e->d_out + e->ol.jobs, sizeof(kr_job_result) * (size_t)n.n_jobs, cudaMemcpyDeviceToHost, e->sm)); bytes += sizeof(kr_job_result) * (uint64_t)n.n_jobs; }
-    if (e->inc_hash_ran && n.n_clusters) { CK(cudaMemcpyAsync(e->h_out + e->ol.hash, e->d_out + e->ol.hash, 32 * (size_t)n.n_clusters, cudaMemcpyDeviceToHost, e->sm)); bytes += 32ull * n.n_clusters; }
+    if ((e->inc_hash_ran || (e->inc_spec_n && !e->inc_spec_gathered)) && n.n_clusters) { CK(cudaMemcpyAsync(e->h_out + e->ol.hash, e->d_out + e->ol.hash, 32 * (size_t)n.n_clusters, cudaMemcpyDeviceToHost, e->sm)); bytes += 32ull * n.n_clusters; }
+    else if (e->inc_spec_n) {  // the digests of the spec rows, packed by k_inc_digest_gather
+      CK(cudaMemcpyAsync(e->h_inc_stage + st_dig, e->d_inc_stage + st_dig, 32 * (size_t)e->inc_spec_n, cudaMemcpyDeviceToHost, e->sm));
+      bytes += 32ull * e->inc_spec_n;
+    }
   } else {
     bytes = e->ol.small_total;
     CK(cudaMemcpyAsync(e->h_out, e->d_out, e->ol.small_total, cudaMemcpyDeviceToHost, e->sm));
@@ -1069,6 +1187,10 @@ int fetch_results(kr_engine *e, kr_results_view *out) {
       hr.clusters[c] = scl[i]; hr.act_start[c] = m[1]; hr.act_cnt[c] = m[2];
       if (m[4]) memcpy(&hr.groups[m[3]], &sgr[m[5]], sizeof(kr_group_result) * (size_t)m[4]);
     }
+  }
+  if (spec_packed) {  // ... and the re-hashed digests
+    char *hh = reinterpret_cast<char *>(e->h_out + e->ol.hash);
+    for (uint32_t i = 0; i < e->inc_spec_n; i++) memcpy(hh + 32 * (size_t)e->spec_hashed[i], e->h_inc_stage + st_dig + 32 * (size_t)i, 32);
   }
   e->fetched = true; e->host_results_stale = false;
   if (out) {
@@ -1120,6 +1242,10 @@ int kr_engine_set_option(kr_engine *e, uint32_t option, uint64_t value) {
     e->wtd_edits = value != 0;
     return KR_OK;
   }
+  if (option == KR_OPT_SPEC_ROWS) {  // (read by kr_packer_flush only)
+    e->spec_rows_opt = value != 0;
+    return KR_OK;
+  }
   if (option == KR_OPT_LARGE_CLUSTERS || option == KR_OPT_WIDE_CLUSTERS || option == KR_OPT_HUGE_CLUSTERS) {
     bool &on = option == KR_OPT_LARGE_CLUSTERS ? e->large_on : option == KR_OPT_WIDE_CLUSTERS ? e->wide_on : e->huge_on;
     if (on == (value != 0)) return KR_OK;
@@ -1166,6 +1292,7 @@ int kr_engine_get_option(kr_engine *e, uint32_t option, uint64_t *value) {
     case KR_OPT_WIDE_CLUSTERS: *value = e->wide_on; return KR_OK;
     case KR_OPT_HUGE_CLUSTERS: *value = e->huge_on; return KR_OK;
     case KR_OPT_WTD_EDITS: *value = e->wtd_edits; return KR_OK;
+    case KR_OPT_SPEC_ROWS: *value = e->spec_rows_opt; return KR_OK;
     case KR_OPT_BUCKET_STRIDE: *value = e->bstride; return KR_OK;
     default: return fail(e, KR_E_INVALID, "unknown option %u", option);
   }
@@ -1260,7 +1387,8 @@ int kr_engine_create(const kr_config *cfg, kr_engine **out) {
     if (cudaMalloc((void **)&e->d_obj_stage, objs) != cudaSuccess) return bail(KR_E_CUDA);
     e->obj_stage_cap = objs;
     const uint32_t capc = std::max<uint32_t>(64, cfg->max_clusters / 4), capg = (uint32_t)std::min<uint64_t>((uint64_t)capc * KR_SMEM_GROUPS, (uint64_t)cfg->max_groups + 1);
-    const size_t need = align_up(32 * (size_t)capc) + align_up(sizeof(kr_cluster_result) * (size_t)capc) + sizeof(kr_group_result) * (size_t)capg + 1024;
+    size_t dig_off;
+    const size_t need = inc_stage_bytes(capc, capg, &dig_off);
     if (cudaMalloc((void **)&e->d_inc_stage, need) != cudaSuccess) return bail(KR_E_CUDA);
     if (cudaHostAlloc((void **)&e->h_inc_stage, need, cudaHostAllocDefault) != cudaSuccess) return bail(KR_E_CUDA);
     e->inc_stage_cap = need;
@@ -1270,6 +1398,8 @@ int kr_engine_create(const kr_config *cfg, kr_engine **out) {
   }
   if (cudaHostAlloc((void **)&e->h_order, 4 * ((size_t)cfg->max_clusters + 1), cudaHostAllocDefault) != cudaSuccess) return bail(KR_E_CUDA);
   if (cudaMalloc((void **)&e->d_order, 4 * ((size_t)cfg->max_clusters + 1)) != cudaSuccess) return bail(KR_E_CUDA);
+  if (cudaHostAlloc((void **)&e->h_spec, 20 * ((size_t)cfg->max_clusters + 1), cudaHostAllocDefault) != cudaSuccess) return bail(KR_E_CUDA);
+  if (cudaMalloc((void **)&e->d_spec, 20 * ((size_t)cfg->max_clusters + 1)) != cudaSuccess) return bail(KR_E_CUDA);
   cudaEventCreateWithFlags(&e->ev_order, cudaEventDisableTiming);
   cudaFuncSetAttribute(k_hash3<1, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(H3Smem));
   *out = e;
@@ -1298,6 +1428,8 @@ void kr_engine_destroy(kr_engine *e) {
   if (e->d_region) cudaFree(e->d_region);
   if (e->d_huge) cudaFree(e->d_huge);
   if (e->d_order) cudaFree(e->d_order);
+  if (e->h_spec) cudaFreeHost(e->h_spec);
+  if (e->d_spec) cudaFree(e->d_spec);
   if (e->ev_order) cudaEventDestroy(e->ev_order);
   if (e->d_in) cudaFree(e->d_in);
   if (e->d_scratch) cudaFree(e->d_scratch);
@@ -1339,6 +1471,8 @@ int kr_snapshot_begin(kr_engine *e, const kr_sizes *sizes, kr_snapshot_bufs *out
     const bool keep = e->inc_valid && e->fixed_layout && sizes->n_clusters == e->sizes.n_clusters && sizes->n_groups == e->sizes.n_groups &&
                       (sizes->n_wtd == e->sizes.n_wtd || e->wtd_edits) && sizes->n_jobs == e->sizes.n_jobs && sizes->n_pods >= e->sizes.n_pods;
     if (!e->fixed_layout) { e->committed_full = false; e->inc_zero_needed = true; }
+    // (the next pass is a full one, which hashes every message: listed rows may not exist any more)
+    if (sizes->n_clusters != e->sizes.n_clusters) clear_spec_rows(e);
     if (!keep) {
       e->inc_valid = false;
       e->force_radix = e->env_radix;
@@ -1412,29 +1546,13 @@ int kr_snapshot_commit_parts(kr_engine *e, uint32_t parts) {
       for (uint32_t c = 0; c < n.n_clusters; c++) if (hb.c_group_cnt[c] > KR_SMEM_GROUPS) wide.push_back(c);
     if (wide != e->wide_rows) { e->wide_rows.swap(wide); if (e->wide_on) e->lg_stale = true; }
   }
-  // hash order: message ids by descending SHA-1 block count (counting sort; the kernels run length-homogeneous warps, longest first)
+  // hash order (build_order)
   if (e->order_pending) { CK(cudaEventSynchronize(e->ev_order)); e->order_pending = false; }  // a previous upload may still be reading h_order
-  // The RayClusters whose Recreate gate compares a digest lead the order: their digests are ready when the decide kernel, running
-  // beside the hash, gets to them (k_decide2 waits for a digest's last word otherwise).
   uint64_t rsig = 0x9E3779B97F4A7C15ull * (n_recreate + 1);
   for (uint32_t c = 0; c < n.n_clusters; c++) if (hb.c_flags[c] & KR_CF_UPGRADE_RECREATE) rsig = (rsig ^ c) * 0x100000001B3ull;
-  const bool order_stale = ranges_moved || rsig != e->recreate_sig;
-  if (order_stale) {  // (unchanged lengths and gates: the resident order stands — an object / pod epoch does not pay for it)
-    uint32_t maxb = 0;
-    for (uint32_t c = 0; c < n.n_clusters; c++) maxb = std::max(maxb, (hb.c_json_len[c] + 8) / 64 + 1);
-    auto blocks_of = [&](uint32_t c) { return (hb.c_json_len[c] + 8) / 64 + 1; };
-    auto lead = [&](uint32_t c) { return (hb.c_flags[c] & KR_CF_UPGRADE_RECREATE) ? 0u : 1u; };
-    if (maxb <= (1u << 20)) {  // counting sort on (not Recreate, descending block count): bucket 0 = the longest Recreate message
-      std::vector<uint32_t> start(2 * ((size_t)maxb + 1) + 1, 0);
-      auto key = [&](uint32_t c) { return lead(c) * (maxb + 1) + (maxb - blocks_of(c)); };
-      for (uint32_t c = 0; c < n.n_clusters; c++) start[key(c) + 1]++;
-      for (size_t b = 0; b + 1 < start.size(); b++) start[b + 1] += start[b];
-      for (uint32_t c = 0; c < n.n_clusters; c++) e->h_order[start[key(c)]++] = c;
-    } else {
-      for (uint32_t c = 0; c < n.n_clusters; c++) e->h_order[c] = c;
-      std::stable_sort(e->h_order, e->h_order + n.n_clusters, [&](uint32_t a, uint32_t b) { return lead(a) != lead(b) ? lead(a) < lead(b) : blocks_of(a) > blocks_of(b); });
-    }
-  }
+  // (a spec-row commit updates the recorded ranges itself: its own flag says the order no longer follows them)
+  const bool order_stale = ranges_moved || rsig != e->recreate_sig || e->spec_order_stale;
+  if (order_stale) build_order(e, hb);  // (unchanged lengths and gates: the resident order stands — an object / pod epoch does not pay for it)
   // Asynchronous, in two parts on the copy stream: every column first, the spec-JSON arena (the larger half) second.
   // The pass waits on the two events, so match/place/decide run while the JSON is still crossing PCIe and only the hash
   // (and what depends on it) waits for the second part.  Nothing here blocks the host.
@@ -1527,7 +1645,7 @@ int kr_snapshot_commit_parts(kr_engine *e, uint32_t parts) {
     e->prev_json_off.assign(hb.c_json_off, hb.c_json_off + n.n_clusters); e->prev_json_len.assign(hb.c_json_len, hb.c_json_len + n.n_clusters);
   }
   if (order_stale) {  // the new order travels with this commit: from here on the recorded ranges / gates are the ones it was built from
-    e->recreate_sig = rsig;
+    e->recreate_sig = rsig; e->spec_order_stale = false;
     if (n.n_clusters) {
       CK(cudaMemcpyAsync(e->d_order, e->h_order, 4 * (size_t)n.n_clusters, cudaMemcpyHostToDevice, e->scopy)); bytes += 4 * (size_t)n.n_clusters;
       CK(cudaEventRecord(e->ev_order, e->scopy));
@@ -1727,6 +1845,72 @@ int kr_snapshot_commit_object_rows(kr_engine *e, const uint32_t *cluster_rows, u
   return KR_OK;
 }
 
+int kr_snapshot_commit_spec_rows(kr_engine *e, const uint32_t *rows, uint32_t n) {
+  if (!e || (!rows && n)) return KR_E_INVALID;
+  if (!e->begun || !e->committed_full) return fail(e, KR_E_STATE, "a spec-row commit needs a full commit of this layout first");
+  if (n == 0) return KR_OK;
+  const kr_sizes &z = e->sizes;
+  kr_snapshot_bufs hb;
+  bind_in(e->il, e->h_in, &hb);
+  for (uint32_t i = 0; i < n; i++) {  // (every row before anything moves: an invalid call commits nothing)
+    const uint32_t c = rows[i];
+    if (c >= z.n_clusters) return fail(e, KR_E_INVALID, "cluster row %u out of range", c);
+    if (hb.c_json_off[c] & 15) return fail(e, KR_E_INVALID, "cluster %u: json offset not 16-byte aligned", c);
+    if (hb.c_json_off[c] + hb.c_json_len[c] > z.json_bytes) return fail(e, KR_E_INVALID, "cluster %u: json range outside arena", c);
+  }
+  CK(cudaSetDevice(e->cfg.device));
+  if (e->spec_stamp.size() < z.n_clusters) e->spec_stamp.resize(z.n_clusters, 0u);
+  if (e->pull_stamp.size() < z.n_clusters) e->pull_stamp.resize(z.n_clusters, 0u);
+  if (e->n_pull == 0) CK(cudaStreamSynchronize(e->scopy));  // (the pinned pull list is rewritten from its start)
+  // the rows this call pulls, appended to the pull list: a row pulled since the last pass is in the device arena already (the caller
+  // may not rewrite the arenas before the next pass returns); a row listed before that pass, still pending, is pulled again
+  const size_t cap = (size_t)e->cfg.max_clusters + 1, base = e->n_pull;
+  uint32_t *lr = reinterpret_cast<uint32_t *>(e->h_spec) + base;
+  uint32_t *ll = reinterpret_cast<uint32_t *>(e->h_spec + 4 * cap) + base;
+  uint64_t *lo = reinterpret_cast<uint64_t *>(e->h_spec + 8 * cap) + base;
+  uint32_t m = 0;
+  for (uint32_t i = 0; i < n; i++) {
+    const uint32_t c = rows[i];
+    if (e->pull_stamp[c] == e->pull_epoch) continue;
+    e->pull_stamp[c] = e->pull_epoch;
+    lr[m++] = c;
+    if (e->spec_stamp[c] != e->spec_epoch) { e->spec_stamp[c] = e->spec_epoch; e->spec_pending.push_back(c); }  // (hashed once)
+  }
+  if (m == 0) return KR_OK;
+  size_t bytes = 16 * (size_t)m;
+  const bool track = e->prev_json_off.size() == z.n_clusters;  // (otherwise the next object commit sees every range as moved anyway)
+  for (uint32_t i = 0; i < m; i++) {
+    const uint32_t c = lr[i];
+    ll[i] = hb.c_json_len[c]; lo[i] = hb.c_json_off[c];
+    bytes += ((size_t)ll[i] + 15) & ~(size_t)15;
+    if (!track) continue;
+    // the recorded ranges follow (a later object commit does not re-hash everything on their account); the full-pass order does not
+    if ((e->prev_json_len[c] + 8) / 64 != (ll[i] + 8) / 64) e->spec_order_stale = true;
+    e->prev_json_off[c] = lo[i]; e->prev_json_len[c] = ll[i];
+  }
+  if (!e->h_in_dev) CK(cudaHostGetDevicePointer((void **)&e->h_in_dev, e->h_in, 0));
+  CK(cudaStreamSynchronize(e->sm));  // a pass still reading the arena must finish first
+  CK(cudaEventRecord(e->ev_h2d0, e->scopy));
+  uint32_t *dr = reinterpret_cast<uint32_t *>(e->d_spec) + base;
+  uint32_t *dl = reinterpret_cast<uint32_t *>(e->d_spec + 4 * cap) + base;
+  uint64_t *dof = reinterpret_cast<uint64_t *>(e->d_spec + 8 * cap) + base;
+  CK(cudaMemcpyAsync(dr, lr, 4 * (size_t)m, cudaMemcpyHostToDevice, e->scopy));
+  CK(cudaMemcpyAsync(dl, ll, 4 * (size_t)m, cudaMemcpyHostToDevice, e->scopy));
+  CK(cudaMemcpyAsync(dof, lo, 8 * (size_t)m, cudaMemcpyHostToDevice, e->scopy));
+  const size_t json_off = e->il.off[kNumCols - 1];
+  k_spec_pull<<<m, 128, 0, e->scopy>>>(dr, dof, dl, e->h_in_dev + json_off, e->d_in + json_off, reinterpret_cast<uint64_t *>(e->d_in + e->il.off[kJsonOffCol]),
+                                       reinterpret_cast<uint32_t *>(e->d_in + e->il.off[kJsonOffCol + 1]));
+  CK(cudaGetLastError());
+  CK(cudaEventRecord(e->ev_h2d1, e->scopy));
+  CK(cudaEventRecord(e->ev_cols, e->scopy));
+  CK(cudaEventRecord(e->ev_json, e->scopy));
+  e->n_pull += m;
+  e->h2d_timed = false;
+  e->prof.h2d_bytes = (e->h2d_accum += bytes);
+  e->committed = true;
+  return KR_OK;
+}
+
 int kr_snapshot_commit_pod_rows(kr_engine *e, const uint32_t *rows, uint32_t n) { return commit_pod_patch(e, rows, nullptr, n); }
 
 // for kr_packer.cpp: its journal holds every row once (row_dirty), so the duplicate scan is skipped
@@ -1781,6 +1965,7 @@ int kr_reconcile_batch_profiled(kr_engine *e, const kr_flags *flags, kr_profile 
   if (!e->committed) return fail(e, KR_E_STATE, "no committed snapshot");
   CK(cudaSetDevice(e->cfg.device));
   e->last_flags = *flags;
+  new_pull_epoch(e);
   if (e->lg_stale) if (int rc = upload_lg(e)) return rc;
   bool inc_done = false;
   if (e->inc_valid && !e->no_incr && memcmp(&e->inc_flags, flags, sizeof *flags) == 0) {
@@ -1794,6 +1979,7 @@ int kr_reconcile_batch_profiled(kr_engine *e, const kr_flags *flags, kr_profile 
       CK(cudaMemsetAsync(e->d_scratch + e->sl.inc_zero, 0, e->sl.inc_zero_end - e->sl.inc_zero, e->sm));
       e->inc_zero_needed = false;
     }
+    if (e->spec_order_stale && !flags->skip_hash) if (int rc = refresh_order(e)) return rc;
   }
   for (int attempt = 0; !inc_done; attempt++) {  // same fallback ladder as run_pass
     CK(cudaEventRecord(e->ev_a, e->sm));

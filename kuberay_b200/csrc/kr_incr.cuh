@@ -237,6 +237,35 @@ __global__ void __launch_bounds__(256) k_inc_mark_recreate(SnapDev s, ScratchDev
   if (c < n.n_clusters && (s.c_flags[c] & KR_CF_UPGRADE_RECREATE)) mark_dirty(sc, c, inc_epoch(sc));
 }
 
+// ------------------------------------------------------------------------------------------------ spec rows
+// kr_snapshot_commit_spec_rows: the device pulls the rewritten muted-spec JSON ranges out of the mapped pinned arena (one CTA per
+// row, 16-byte loads over PCIe) and sets the rows' c_json_off / c_json_len from the uploaded list; the next pass hashes only the
+// listed messages (the hash kernels take the list as their order), marks the listed Recreate-gated RayClusters dirty and gathers
+// the new digests for the fetch.
+__global__ void __launch_bounds__(128) k_spec_pull(const uint32_t *__restrict__ rows, const uint64_t *__restrict__ offs, const uint32_t *__restrict__ lens,
+                                                   const uint8_t *__restrict__ h_json, uint8_t *__restrict__ d_json, uint64_t *c_json_off, uint32_t *c_json_len) {
+  const uint32_t i = blockIdx.x;
+  const uint64_t off = offs[i];
+  const uint32_t len = lens[i];
+  const uint4 *src = reinterpret_cast<const uint4 *>(h_json + off);
+  uint4 *dst = reinterpret_cast<uint4 *>(d_json + off);
+  for (uint32_t k = threadIdx.x; k < (len + 15) / 16; k += blockDim.x) dst[k] = src[k];
+  if (threadIdx.x == 0) { c_json_off[rows[i]] = off; c_json_len[rows[i]] = len; }
+}
+
+// the listed RayClusters whose Recreate gate reads the digest (k_inc_mark_recreate's test, for the listed rows only)
+__global__ void __launch_bounds__(256) k_inc_mark_rows(SnapDev s, ScratchDev sc, const uint32_t *__restrict__ rows, uint32_t n) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i < n && (s.c_flags[rows[i]] & KR_CF_UPGRADE_RECREATE)) mark_dirty(sc, rows[i], inc_epoch(sc));
+}
+
+// the listed digests, packed in list order (two 16-byte pieces per digest)
+__global__ void __launch_bounds__(256) k_inc_digest_gather(const uint32_t *__restrict__ rows, uint32_t n, const char *__restrict__ hash, char *__restrict__ out) {
+  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= 2 * n) return;
+  reinterpret_cast<uint4 *>(out)[t] = reinterpret_cast<const uint4 *>(hash + 32 * (size_t)rows[t >> 1])[t & 1];
+}
+
 // ------------------------------------------------------------------------------------------------ k_inc_refresh
 // Input records (cl_in) of the RayClusters one of whose RayCluster / group rows an object commit changed (grid-stride over the
 // dirty list as the commits left it; clusters k_inc_admit adds later had no object change).

@@ -103,6 +103,11 @@ struct kr_packer {
   std::vector<uint32_t> dirty_cl, dirty_hd;
   std::vector<uint8_t> cl_flag, hd_flag;
   bool wtd_changed = false;           // a workersToDelete name was rewritten in place (same count): the whole object part travels
+  // RayClusters whose muted-spec JSON was placed since the last flush (kr_snapshot_commit_spec_rows with KR_OPT_SPEC_ROWS, unless the
+  // arena was compacted or a RayCluster row moved)
+  std::vector<uint32_t> json_rows;
+  std::vector<uint8_t> json_flag;
+  bool json_compacted = false, clusters_moved = false;
 
   uint32_t intern(const kr_str &s) {
     if (!s.p) return KR_ID_ABSENT;
@@ -191,11 +196,13 @@ int place_json(kr_packer *p, ClusterRec &c) {  // put the cluster's blob at the 
   c.json_off = p->json_cursor; c.json_placed = true;
   p->b.c_json_off[c.row] = c.json_off; p->b.c_json_len[c.row] = (uint32_t)c.json.size();
   p->json_cursor += padded;
+  if (c.row >= p->json_flag.size()) p->json_flag.resize((size_t)c.row + 256, 0);
+  if (!p->json_flag[c.row]) { p->json_flag[c.row] = 1; p->json_rows.push_back(c.row); }
   return KR_OK;
 }
 
 int compact_json(kr_packer *p) {
-  p->json_cursor = 0; p->json_dead = 0;
+  p->json_cursor = 0; p->json_dead = 0; p->json_compacted = true;
   for (auto &c : p->clusters) if (int rc = place_json(p, c)) return pfail(p, rc, "kr_packer: muted-spec JSON exceeds kr_config.max_json_bytes");
   return KR_OK;
 }
@@ -379,6 +386,7 @@ int kr_packer_cluster_delete(kr_packer *p, kr_str ns, kr_str name) {
   const uint32_t row = it->second, last = (uint32_t)p->clusters.size() - 1;
   p->json_dead += (p->clusters[row].json.size() + 15) & ~15ull;
   p->cluster_row.erase(it);
+  p->clusters_moved = true;
   if (row != last) {  // the last RayCluster moves into the hole: copy its scalar columns
     ClusterRec moved = std::move(p->clusters[last]);
     moved.row = row;
@@ -444,6 +452,10 @@ int kr_packer_flush(kr_packer *p, uint32_t *mode_out) {
   kr_snapshot_bufs same;
   p->sizes = want;
   if (want.n_clusters != p->engine_sizes.n_clusters || want.n_groups != p->engine_sizes.n_groups || want.n_wtd != p->engine_sizes.n_wtd || want.n_jobs != p->engine_sizes.n_jobs) rows_ok = false;
+  // Row-granular spec commit (KR_OPT_SPEC_ROWS): only the re-emitted blobs travel, while every other one stays where it was.
+  uint64_t spec_opt = 0;
+  kr_engine_get_option(p->e, KR_OPT_SPEC_ROWS, &spec_opt);
+  const bool spec_ok = spec_opt && p->json_dirty && !p->first && !p->json_compacted && !p->clusters_moved && want.n_clusters == p->engine_sizes.n_clusters;
   if (memcmp(&want, &p->engine_sizes, sizeof want) != 0 || p->first) {
     if (int rc = kr_snapshot_begin(p->e, &p->sizes, &same)) return rc;  // fixed layout: new live counts, same addresses, resident data kept
     p->engine_sizes = want;
@@ -454,7 +466,11 @@ int kr_packer_flush(kr_packer *p, uint32_t *mode_out) {
     mode = KR_PACK_FULL;
   } else {
     if (trace) t2 = now();
-    uint32_t parts = ((p->objects_dirty && !rows_ok) ? KR_PART_OBJECTS : 0u) | (p->json_dirty ? KR_PART_JSON : 0u);
+    if (spec_ok) {  // (before the object commit, which would otherwise see the moved ranges and re-hash every RayCluster)
+      if (int rc = kr_snapshot_commit_spec_rows(p->e, p->json_rows.data(), (uint32_t)p->json_rows.size())) return rc;
+      mode |= KR_PACK_SPEC_ROWS;
+    }
+    uint32_t parts = ((p->objects_dirty && !rows_ok) ? KR_PART_OBJECTS : 0u) | ((p->json_dirty && !spec_ok) ? KR_PART_JSON : 0u);
     if (parts) { if (int rc = kr_snapshot_commit_parts(p->e, parts)) return rc; mode |= parts; }
     if (rows_ok) {
       if (int rc = kr_snapshot_commit_object_rows(p->e, p->dirty_cl.data(), (uint32_t)p->dirty_cl.size(), p->dirty_hd.data(), (uint32_t)p->dirty_hd.size())) return rc;
@@ -472,6 +488,8 @@ int kr_packer_flush(kr_packer *p, uint32_t *mode_out) {
   for (uint32_t r : p->dirty_cl) p->cl_flag[r] = 0;
   for (uint32_t r : p->dirty_hd) if (r < p->hd_flag.size()) p->hd_flag[r] = 0;
   p->dirty_cl.clear(); p->dirty_hd.clear(); p->wtd_changed = false;
+  for (uint32_t r : p->json_rows) p->json_flag[r] = 0;
+  p->json_rows.clear(); p->json_compacted = p->clusters_moved = false;
   p->first = p->objects_dirty = p->tables_dirty = p->heads_dirty = p->jobs_dirty = p->json_dirty = false;
   p->epoch++;
   p->last_mode = mode;

@@ -60,6 +60,7 @@ def lib() -> C.CDLL:
         L.kr_snapshot_commit_pod_rows.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
         L.kr_snapshot_commit_pod_values.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32]
         L.kr_snapshot_commit_object_rows.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32]
+        L.kr_snapshot_commit_spec_rows.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
         L.kr_engine_set_option.argtypes = [C.c_void_p, C.c_uint32, C.c_uint64]
         L.kr_engine_get_option.argtypes = [C.c_void_p, C.c_uint32, P(C.c_uint64)]
         L.kr_reconcile_batch.argtypes = [C.c_void_p, P(abi.kr_flags), P(abi.kr_results_view)]
@@ -212,7 +213,7 @@ class Engine:
     @classmethod
     def for_snapshot(cls, snap: Snapshot, device: int = 0, max_creates: int | None = None, slack: float = 1.0,
                      large_clusters: bool = False, wide_clusters: bool = False, huge_clusters: bool = False,
-                     wtd_edits: bool = False) -> "Engine":
+                     wtd_edits: bool = False, spec_rows: bool = False) -> "Engine":
         d = snap.dims
         up = lambda x: int(x * slack) + 1  # noqa: E731
         if max_creates is None:
@@ -227,6 +228,8 @@ class Engine:
             eng.set_huge_clusters(True)
         if wtd_edits:
             eng.set_wtd_edits(True)
+        if spec_rows:
+            eng.set_spec_rows(True)
         return eng
 
     def _check(self, rc: int):
@@ -274,6 +277,11 @@ class Engine:
         under the fixed layout) instead of taking a full pass; read at each object commit."""
         self._check(self._L.kr_engine_set_option(self._h, abi.OPT_WTD_EDITS, 1 if on else 0))
 
+    def set_spec_rows(self, on: bool = True):
+        """KR_OPT_SPEC_ROWS: the native packer (and LiveArena) commit re-emitted specs row by row (kr_snapshot_commit_spec_rows)
+        instead of re-sending the whole JSON arena; commit_spec_rows itself works either way."""
+        self._check(self._L.kr_engine_set_option(self._h, abi.OPT_SPEC_ROWS, 1 if on else 0))
+
     def get_option(self, option: int) -> int:
         """kr_engine_get_option: an option's current value, or the read-only OPT_BUCKET_STRIDE (0: the sort pipeline)."""
         v = C.c_uint64()
@@ -319,6 +327,12 @@ class Engine:
         cr = np.ascontiguousarray(cluster_rows, dtype=np.uint32)
         hr = np.ascontiguousarray(head_rows, dtype=np.uint32)
         self._check(self._L.kr_snapshot_commit_object_rows(self._h, cr.ctypes.data if cr.size else None, cr.size, hr.ctypes.data if hr.size else None, hr.size))
+
+    def commit_spec_rows(self, rows):
+        """kr_snapshot_commit_spec_rows: only the rewritten muted-spec JSON ranges (and c_json_off / c_json_len) of these RayClusters
+        travel; the next pass re-hashes only them.  Call before the epoch's object commit."""
+        r = np.ascontiguousarray(rows, dtype=np.uint32)
+        self._check(self._L.kr_snapshot_commit_spec_rows(self._h, r.ctypes.data if r.size else None, r.size))
 
     def load(self, snap: Snapshot):
         views = self.begin(snap.sizes())

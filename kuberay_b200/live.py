@@ -34,7 +34,7 @@ def _is_head(pod: dict) -> bool:
 class LiveArena:
     def __init__(self, clusters: list[dict], pods: list[dict], jobs: list[dict] | None = None, spare_rows: int = 64, device: int = 0,
                  engine: bool = True, large_clusters: bool = False, wide_clusters: bool = False, huge_clusters: bool = False,
-                 wtd_edits: bool = False):
+                 wtd_edits: bool = False, spec_rows: bool = False):
         self.clusters = {(c.get("namespace", "default"), c["name"]): c for c in clusters}
         self.jobs = list(jobs or [])
         self.rows: list[dict | None] = list(pods) + [None] * spare_rows
@@ -45,6 +45,7 @@ class LiveArena:
         self.wide_clusters = wide_clusters    # ... and KR_OPT_WIDE_CLUSTERS
         self.huge_clusters = huge_clusters    # ... and KR_OPT_HUGE_CLUSTERS
         self.wtd_edits = wtd_edits            # ... and KR_OPT_WTD_EDITS
+        self.spec_rows = spec_rows            # ... and KR_OPT_SPEC_ROWS: changed specs travel as kr_snapshot_commit_spec_rows
         self.engine: Engine | None = None
         self.stats = {"rebase": 0, "incremental": 0, "rows": 0}
         self._need_rebase = True
@@ -106,7 +107,7 @@ class LiveArena:
                 self.engine.close()
             self.engine = Engine.for_snapshot(snap, device=self.device, slack=1.5, large_clusters=self.large_clusters,
                                               wide_clusters=self.wide_clusters, huge_clusters=self.huge_clusters,
-                                              wtd_edits=self.wtd_edits)
+                                              wtd_edits=self.wtd_edits, spec_rows=self.spec_rows)
             self.engine.set_fixed_layout(True)
             self.views = self.engine.begin(snap.sizes())
             self.engine.fill(self.views, snap)
@@ -119,13 +120,22 @@ class LiveArena:
             if bytes(snap.sizes()) != bytes(self.snap.sizes()):
                 self.views = self.engine.begin(snap.sizes())
             parts = 0
+            if not np.array_equal(self.views["json"], snap.cols["json"]):
+                if self.spec_rows and snap.dims["clusters"] == self.snap.dims["clusters"]:
+                    # every RayCluster whose range or bytes differ (a repack moves every range after a length change), committed
+                    # before the object part so that it finds the ranges where the digests say they are
+                    rows = self._spec_rows_changed(snap)
+                    np.copyto(self.views["json"], snap.cols["json"])
+                    self.views["c_json_off"][rows] = snap.cols["c_json_off"][rows]
+                    self.views["c_json_len"][rows] = snap.cols["c_json_len"][rows]
+                    self.engine.commit_spec_rows(rows)
+                else:
+                    np.copyto(self.views["json"], snap.cols["json"])
+                    parts |= abi.PART_JSON
             if any(not np.array_equal(self.views[c], snap.cols[c]) for c in _OBJ_COLS):
                 for c in _OBJ_COLS:
                     np.copyto(self.views[c], snap.cols[c])
                 parts |= abi.PART_OBJECTS
-            if not np.array_equal(self.views["json"], snap.cols["json"]):
-                np.copyto(self.views["json"], snap.cols["json"])
-                parts |= abi.PART_JSON
             if parts:
                 self.engine.commit(parts)
             self._dirty.update(range(old_pods, snap.dims["pods"]))  # rows appended past the old end of the arena
@@ -146,6 +156,14 @@ class LiveArena:
         self._dirty.clear()
         self.stats[mode] += 1
         return mode
+
+    def _spec_rows_changed(self, snap) -> np.ndarray:
+        old, new = self.snap.cols, snap.cols
+        moved = (old["c_json_off"] != new["c_json_off"]) | (old["c_json_len"] != new["c_json_len"])
+        for c in np.flatnonzero(~moved):
+            o, n = int(new["c_json_off"][c]), int(new["c_json_len"][c])
+            moved[c] = not np.array_equal(old["json"][o:o + n], new["json"][o:o + n])
+        return np.flatnonzero(moved).astype(np.uint32)
 
     def _fits(self, snap) -> bool:
         d, c = snap.dims, self.engine.cfg

@@ -23,7 +23,7 @@ def _s(v) -> abi.kr_str:
 class Packer:
     def __init__(self, device=0, max_clusters=1024, max_groups=4096, max_wtd=4096, max_pods=65536, max_heads=2048, max_jobs=1024,
                  max_creates=65536, max_json_bytes=64 << 20, large_clusters=False, wide_clusters=False,
-                 huge_clusters=False, wtd_edits=False):
+                 huge_clusters=False, wtd_edits=False, spec_rows=False):
         L = self._L = lib()
         P = C.POINTER
         L.kr_packer_create.argtypes = [P(abi.kr_config), P(C.c_void_p)]
@@ -63,6 +63,8 @@ class Packer:
             self.engine.set_huge_clusters(True)
         if wtd_edits:  # KR_OPT_WTD_EDITS, likewise
             self.engine.set_wtd_edits(True)
+        if spec_rows:  # KR_OPT_SPEC_ROWS, likewise: flush commits re-emitted specs row by row (PACK_SPEC_ROWS)
+            self.engine.set_spec_rows(True)
 
     def _check(self, rc):
         if rc != 0:

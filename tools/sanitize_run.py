@@ -111,7 +111,40 @@ def wtd_edits(snap, flags, label):
         eng.close()
 
 
+def spec_rows(snap, flags, label):
+    """kr_snapshot_commit_spec_rows (kr_incr.cuh): specs rewritten in place and moved to the arena's end, pulled by k_spec_pull, then
+    re-hashed over the row list, the listed Recreate gates marked (k_inc_mark_rows) and the digests gathered (k_inc_digest_gather)."""
+    flags.fetch_pod_lists = 0
+    d = snap.dims
+    eng = Engine(0, d["clusters"], d["groups"], d["wtd"], d["pods"], d["heads"], d["jobs"], max(1024, d["pods"]), d["json"] + (1 << 20))
+    eng.set_fixed_layout(True)
+    try:
+        views = eng.load(snap)
+        eng.reconcile(flags)
+        inc, end = 0, d["json"]
+        for step in range(3):
+            rows = np.arange(step, d["clusters"], 7, dtype=np.uint32)
+            if step == 1:  # moved: every listed spec one byte longer at the arena's end
+                s2 = synthetic.Snapshot(d["clusters"], d["groups"], d["wtd"], d["pods"], d["heads"], d["jobs"], end + 16 * (rows.size + 1) + int(views["c_json_len"][rows].sum()))
+                views = eng.begin(s2.sizes())
+                for c in rows.tolist():
+                    o, n = int(views["c_json_off"][c]), int(views["c_json_len"][c])
+                    views["json"][end:end + n] = views["json"][o:o + n]
+                    views["json"][end + n:end + (n + 16) // 16 * 16] = 32
+                    views["c_json_off"][c], views["c_json_len"][c] = end, n + 1
+                    end += (n + 16) // 16 * 16
+            else:  # in place: one byte rewritten
+                for c in rows.tolist():
+                    views["json"][int(views["c_json_off"][c])] ^= 1
+            eng.commit_spec_rows(rows)
+            inc += eng.reconcile(flags).changed_clusters is not None
+        print(label, "ok:", inc, "of 3 epochs incremental", flush=True)
+    finally:
+        eng.close()
+
+
 def main():
+    spec_rows(*synthetic.generate(synthetic.config("C2", n_clusters=300, pods_per_cluster=20, groups=2, recreate_frac=0.3)), "spec rows")
     wtd_edits(*synthetic.generate(synthetic.config("C2", n_clusters=300, pods_per_cluster=20, groups=2, autoscaling_frac=1.0, wtd_group_frac=0.3)),
               "workersToDelete edits")
     incremental(*synthetic.generate(synthetic.config("C2", n_clusters=300, pods_per_cluster=20, groups=2, jobs=True, wtd_group_frac=0.3)), "incremental epochs")
