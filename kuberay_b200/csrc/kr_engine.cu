@@ -1,11 +1,12 @@
 // kr_engine.cu — C ABI (include/kr_engine.h) of the batched reconcile engine: arenas, streams, kernel schedule.
 //
-// One engine = one device and four streams: M (clear -> tables -> match -> place -> decide -> creates), H (hash),
-// G (general decide kernel beside the small one) and a copy stream; the pass is one CUDA graph joined by events.
-// Inputs live in ONE pinned host arena and ONE device arena with identical layouts computed per snapshot from
-// kr_sizes: a full commit is two contiguous asynchronous H2D copies (columns, then the spec-JSON arena), partial and
-// per-row commits upload less (kr_snapshot_commit_parts / kr_snapshot_commit_pod_rows).  Results come back with the
-// exact sizes read from a 32-byte totals record and a single host wait (fetch_results).
+// One engine = one device and four streams: M (the pass's main chain), H (the hash beside it), G (the general decide kernel beside
+// k_decide_small) and a copy stream for the commits.  Inputs live in ONE pinned host arena and ONE device arena with identical
+// layouts computed per snapshot from kr_sizes.  PassCtx, launch_hash, launch_decide2 and launch_large_sort are the launch helpers of
+// the full pass (launch_pass, replayed as a CUDA graph by run_pass_once) and the incremental one (run_pass_inc); run_pass drives both
+// for every reconcile call, profiled or not.  fetch_results copies the results back with the exact sizes of the totals words the
+// pass left, behind one host wait.  The commits upload on the copy stream and end in finish_commit; the two object commits diff
+// their rows against the resident tables on the device (launch_object_diff).
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -33,12 +34,19 @@ namespace {
 constexpr size_t kAlign = 256;
 inline size_t align_up(size_t x, size_t a = kAlign) { return (x + a - 1) / a * a; }
 inline uint32_t pow2_at_least(uint64_t x) { uint32_t p = 16; while (p < x) p <<= 1; return p; }
-// staging of an incremental pass's changed records: [meta 32 B | cluster record] x capc, group records x capg, then the re-hashed
-// digests of a spec-row epoch (32 B x capc); returns the bytes, *dig_off the digests' offset
-size_t inc_stage_bytes(uint32_t capc, uint32_t capg, size_t *dig_off) {
-  const size_t d = align_up(32 * (size_t)capc) + align_up(sizeof(kr_cluster_result) * (size_t)capc) + align_up(sizeof(kr_group_result) * (size_t)capg);
-  *dig_off = d;
-  return d + 32 * (size_t)capc + 1024;
+// staging of an incremental pass's changed records, for up to a quarter of the RayClusters (beyond that the whole record arrays are
+// as cheap to move): meta 32 B x capc, cluster records x capc, group records x capg, then the re-hashed digests of a spec-row epoch
+// (32 B x capc)
+struct IncStageLayout { uint32_t capc, capg; size_t clusters, groups, digests, total; };
+IncStageLayout inc_stage_layout(uint32_t n_clusters, uint32_t n_groups) {
+  IncStageLayout L;
+  L.capc = std::max<uint32_t>(64, n_clusters / 4);
+  L.capg = (uint32_t)std::min<uint64_t>((uint64_t)L.capc * KR_SMEM_GROUPS, (uint64_t)n_groups + 1);
+  L.clusters = align_up(32 * (size_t)L.capc);
+  L.groups = L.clusters + align_up(sizeof(kr_cluster_result) * (size_t)L.capc);
+  L.digests = L.groups + align_up(sizeof(kr_group_result) * (size_t)L.capg);
+  L.total = L.digests + 32 * (size_t)L.capc + 1024;
+  return L;
 }
 
 // bucket stride of a new layout: a power of two with 25 % head room over the mean cluster size (a cluster that outgrows it voids the
@@ -116,6 +124,7 @@ void dims_of(const kr_sizes &n, uint64_t d[7]) {
   d[D_CLUSTERS] = n.n_clusters; d[D_GROUPS] = n.n_groups; d[D_WTD] = n.n_wtd; d[D_PODS] = n.n_pods;
   d[D_HEADS] = n.n_heads; d[D_JOBS] = n.n_jobs; d[D_JSON] = n.json_bytes;
 }
+Sizes sizes_of(const kr_sizes &n) { return Sizes{n.n_clusters, n.n_groups, n.n_wtd, n.n_pods, n.n_heads, n.n_jobs}; }
 
 InLayout in_layout(const kr_sizes &n) {
   InLayout L;
@@ -237,6 +246,29 @@ ScratchLayout scratch_layout(const kr_sizes &n) {
   return L;
 }
 
+// A pinned staging buffer and its device twin.  A caller whose upload may still be reading `h` when it returns records `ev` on the
+// copy stream and sets `busy`; wait() is the next call's wait for it.
+struct Staging {
+  uint8_t *h = nullptr, *d = nullptr; size_t cap = 0;
+  cudaEvent_t ev = nullptr; bool busy = false;
+  // room for `need` bytes; a buffer that has to grow takes `slack` bytes more
+  cudaError_t reserve(size_t need, size_t slack) {
+    if (need <= cap) return cudaSuccess;
+    if (h) cudaFreeHost(h);
+    if (d) cudaFree(d);
+    h = nullptr; d = nullptr; cap = 0;
+    cudaError_t rc = cudaHostAlloc((void **)&h, need + slack, cudaHostAllocDefault);
+    if (rc == cudaSuccess && (rc = cudaMalloc((void **)&d, need + slack)) == cudaSuccess) cap = need + slack;
+    return rc;
+  }
+  cudaError_t wait() {
+    const cudaError_t rc = busy ? cudaEventSynchronize(ev) : cudaSuccess;
+    if (rc == cudaSuccess) busy = false;
+    return rc;
+  }
+  void release() { if (h) cudaFreeHost(h); if (d) cudaFree(d); if (ev) cudaEventDestroy(ev); }
+};
+
 }  // namespace
 
 struct kr_engine {
@@ -260,14 +292,10 @@ struct kr_engine {
   uint32_t n_recreate = 0;  // clusters with KR_CF_UPGRADE_RECREATE (decide phase 1 needed)
   kr_profile prof{};
   std::string err;
-  // kr_hash_batch staging
-  uint8_t *hb_h = nullptr, *hb_d = nullptr;
-  size_t hb_cap = 0;
-  uint8_t *h_in_dev = nullptr;               // device-side address of h_in
-  uint8_t *pr_h = nullptr, *pr_d = nullptr;  // incremental pod commits: staging
-  cudaEvent_t ev_pr = nullptr;               // staging buffer consumed by the copy stream
-  bool pr_busy = false;
-  size_t pr_cap = 0;
+  Staging hb;                  // kr_hash_batch
+  Staging pr;                  // incremental pod commits
+  Staging orow;                // kr_snapshot_commit_object_rows
+  uint8_t *h_in_dev = nullptr;  // device-side address of h_in
   int sm_count = 148;
   // the whole pass (both streams) captured once per (layout, flags, n_recreate) and replayed
   cudaGraphExec_t gexec = nullptr;
@@ -290,8 +318,6 @@ struct kr_engine {
                                 // (KR_NO_HASH_SPIN=1, or a pass in which a warp gave up waiting, turns it off)
   uint64_t recreate_sig = 0;    // which RayClusters carry KR_CF_UPGRADE_RECREATE (their messages lead the hash order)
   std::vector<uint8_t> recreate_bit;  // ... per cluster row, as of the last object commit (kr_snapshot_commit_object_rows checks against it)
-  uint8_t *orow_h = nullptr, *orow_d = nullptr; size_t orow_cap = 0;  // kr_snapshot_commit_object_rows staging
-  cudaEvent_t ev_orow = nullptr; bool orow_busy = false;
   uint32_t bstride = 0;         // bucket stride of this layout (64 / 128 / 256); 0 = the layout does not qualify (a cluster outgrew 256 pods, ...)
   bool large_on = false;        // KR_OPT_LARGE_CLUSTERS
   bool wide_on = false;         // KR_OPT_WIDE_CLUSTERS
@@ -351,8 +377,8 @@ struct kr_engine {
   // kr_snapshot_commit_spec_rows, pinned mirror and device copy of {pull rows u32 | lens u32 | offs u64 | hash order u32}[max_clusters]:
   // each call appends the rows it pulls to the pull lists; the pass that hashes them sorts the pending rows once and uploads them as
   // the hash order
-  uint8_t *h_spec = nullptr, *d_spec = nullptr;
-  uint32_t n_pull = 0;                 // pull-list entries since the last pass
+  Staging spec;
+  uint32_t n_pull = 0;                // pull-list entries since the last pass
   std::vector<uint32_t> spec_pending;  // rows listed since the last pass that hashed (each once)
   std::vector<uint32_t> spec_stamp;    // cluster row -> spec_epoch that listed it (the union of the calls until they are hashed)
   uint32_t spec_epoch = 1;
@@ -364,7 +390,8 @@ struct kr_engine {
   bool inc_spec_gathered = false;      // ... and their digests sit packed in the staging buffer
   std::vector<uint32_t> spec_hashed;   // ... which rows (the fetch scatters the digests)
   uint8_t *d_obj_stage = nullptr; size_t obj_stage_cap = 0;   // KR_PART_OBJECTS uploads land here while the state is resident
-  uint8_t *d_inc_stage = nullptr, *h_inc_stage = nullptr; size_t inc_stage_cap = 0; uint32_t inc_stage_clusters = 0, inc_stage_groups = 0;
+  Staging inc_stage;             // an incremental pass's changed records, sized for the capacities
+  IncStageLayout inc_layout{};   // ... as the last incremental pass laid them out
   uint32_t *h_inc = nullptr;     // pinned copy of the epoch counters (16 words) + the changed-cluster list
   uint32_t *h_changed = nullptr; size_t h_changed_cap = 0;
 };
@@ -584,33 +611,85 @@ const uint32_t *upload_spec_order(kr_engine *e) {
   const size_t cap = (size_t)e->cfg.max_clusters + 1;
   kr_snapshot_bufs hb;
   bind_in(e->il, e->h_in, &hb);
-  uint32_t *h = reinterpret_cast<uint32_t *>(e->h_spec + 16 * cap);
+  uint32_t *h = reinterpret_cast<uint32_t *>(e->spec.h + 16 * cap);
   const uint32_t n = (uint32_t)e->spec_pending.size();
   std::copy(e->spec_pending.begin(), e->spec_pending.end(), h);
   std::stable_sort(h, h + n, [&](uint32_t a, uint32_t b) { return (hb.c_json_len[a] + 8) / 64 > (hb.c_json_len[b] + 8) / 64; });
-  uint32_t *d = reinterpret_cast<uint32_t *>(e->d_spec + 16 * cap);
+  uint32_t *d = reinterpret_cast<uint32_t *>(e->spec.d + 16 * cap);
   if (cudaMemcpyAsync(d, h, 4 * (size_t)n, cudaMemcpyHostToDevice, e->sm) != cudaSuccess) return nullptr;
   e->prof.h2d_bytes = (e->h2d_accum += 4 * (uint64_t)n);  // (the pass's own upload: reported with the commits that fed it)
   return d;
 }
 
-// Launches the whole pass.  profile: serialise everything on stream M and bracket each kernel with events.
-int launch_pass(kr_engine *e, const kr_flags &f, bool profile, bool capturing = false) {
-  const kr_sizes &n = e->sizes;
-  SnapDev s;
-  bind_in(e->il, e->d_in, &s);
-  ResDev r = bind_out(e->ol, e->d_out);
-  ScratchDev sc = bind_scratch(e->sl, e->d_scratch);
-  const uint32_t *lg_list = bind_large(e, sc);
-  const HugeDev hd = bind_huge(e);
-  Sizes z{n.n_clusters, n.n_groups, n.n_wtd, n.n_pods, n.n_heads, n.n_jobs};
-  cudaStream_t M = e->sm, H = profile ? e->sm : e->sh;
+// What the launches of a pass share: the arenas and the per-cluster kernels' tables bound for this layout, stream M and the hash
+// stream H (M as well when profiling).  mark() counts a kernel in kr_profile.n_kernels and, profiling, names it and records its
+// start event on M; close() records the last kernel's end event and stores the count.
+struct PassCtx {
+  kr_engine *e; bool profile;
+  SnapDev s; ResDev r; ScratchDev sc; const uint32_t *lg_list; HugeDev hd; Sizes z;
+  cudaStream_t M, H;
   int k = 0;
-  auto mark = [&](const char *name) {
+  PassCtx(kr_engine *e_, bool profile_)
+      : e(e_), profile(profile_), r(bind_out(e->ol, e->d_out)), sc(bind_scratch(e->sl, e->d_scratch)), lg_list(bind_large(e, sc)),
+        hd(bind_huge(e)), z(sizes_of(e->sizes)), M(e->sm), H(profile ? e->sm : e->sh) {
+    bind_in(e->il, e->d_in, &s);
+    sc.bucket_stride = e->bstride;
+    e->prof.n_kernels = 0;
+  }
+  void mark(const char *name) {
     if (profile && k < KR_MAX_KERNEL_TIMES) { e->prof.kernel_name[k] = name; cudaEventRecord(e->ev_k[k], M); }
     k++;
-  };
-  e->prof.n_kernels = 0;
+  }
+  void close() {
+    if (profile && k <= KR_MAX_KERNEL_TIMES) cudaEventRecord(e->ev_k[k], M);
+    e->prof.n_kernels = (uint32_t)k;
+  }
+};
+
+// SHA-1 digests of the n messages (json + off[i], len[i]) taken in `order` (descending block count: length-homogeneous warps,
+// longest first).  Latency regime (C3: 313 groups of 32): the caller waits for the longest message's serial chain — warp-specialised
+// pairs, two per SM so that every hash warp has a scheduler to itself.  Throughput regime: up to ctas_per_sm resident CTAs per SM of
+// four one-lane-per-message warps walk the groups, round adds on the FMA pipe.
+void launch_hash(const kr_engine *e, cudaStream_t st, const uint8_t *json, const uint64_t *off, const uint32_t *len, const uint32_t *order,
+                 uint32_t n, char *out, int ctas_per_sm) {
+  const uint32_t ngroups = (n + 31) / 32;
+  if (ngroups <= (uint32_t)e->sm_count * 4)
+    k_hash3<1, 0><<<std::min<uint32_t>(ngroups, (uint32_t)e->sm_count * 2), 64, sizeof(H3Smem), st>>>(json, off, len, order, n, out);
+  else
+    k_hash2<4, 1><<<std::min<uint32_t>((n + 127) / 128, (uint32_t)e->sm_count * ctas_per_sm), 128, 0, st>>>(json, off, len, order, n, out, 1u);
+}
+
+// k_decide2 for this layout's bucket stride; the instantiation with the multi-host branch when the snapshot has a multi-host
+// group and the gate is on, and the incremental epoch's one (phase 2) when `inc`.
+cudaError_t launch_decide2(const PassCtx &c, const Decide2Args &da, dim3 grid, bool inc, bool pdl) {
+  using Kernel = void (*)(Decide2Args);
+  static const Kernel kern[3][2][2] = {  // [stride 64 / 128 / 256][inc][multi-host]
+      {{k_decide2<2>, k_decide2<2, false, true>}, {k_decide2<2, true>, k_decide2<2, true, true>}},
+      {{k_decide2<4>, k_decide2<4, false, true>}, {k_decide2<4, true>, k_decide2<4, true, true>}},
+      {{k_decide2<8>, k_decide2<8, false, true>}, {k_decide2<8, true>, k_decide2<8, true, true>}}};
+  const int st = c.e->bstride <= 64 ? 0 : c.e->bstride <= 128 ? 1 : 2;
+  const bool mh = c.e->snap_has_mh && da.f.gate_multihost_indexing;
+  return launch_pdl(kern[st][inc][mh], grid, dim3(kD2Warps * 32), 0, c.M, pdl, da);
+}
+
+// The sorts of the per-cluster kernels' RayClusters (kr_large.cuh): k_large_sort for the first n_lsort of the list, the huge ones
+// after them tile by tile, then merged (kr_huge.cuh).
+template <bool kInc>
+void launch_large_sort(PassCtx &c, const Decide2Args &da) {
+  const kr_engine *e = c.e;
+  if (e->n_lsort) { c.mark("k_large_sort"); k_large_sort<kInc><<<e->n_lsort, kLargeSortThreads, 0, c.M>>>(da, c.lg_list); }
+  if (e->n_tiles) {
+    c.mark("k_huge_tiles"); k_huge_tiles<kInc><<<e->n_tiles, kHugeThreads, 0, c.M>>>(da, c.hd);
+    c.mark("k_huge_merge"); k_huge_merge<kInc><<<e->n_tiles, kHugeThreads, 0, c.M>>>(da, c.hd);
+  }
+}
+
+// Launches the whole pass.  profile: serialise everything on stream M and bracket each kernel with events.
+int launch_pass(kr_engine *e, const kr_flags &f, bool profile, bool capturing = false) {
+  PassCtx c(e, profile);
+  const kr_sizes &n = e->sizes;
+  const SnapDev &s = c.s; const ResDev &r = c.r; const ScratchDev &sc = c.sc; const Sizes &z = c.z;
+  const cudaStream_t M = c.M, H = c.H;
 
   // --- stream H: hash (only needs the committed snapshot)
   const bool do_hash = !f.skip_hash && n.n_clusters > 0;
@@ -623,37 +702,30 @@ int launch_pass(kr_engine *e, const kr_flags &f, bool profile, bool capturing = 
                       (size_t)n.n_clusters * e->bstride <= e->sl.bucket_entries;
   // ... and there the clusters whose Recreate gate reads a digest wait for it inside the decide kernel (the hash runs beside it)
   const bool spin = bucket && !profile && do_hash && e->hash_spin && e->n_recreate > 0;
-  auto launch_hash = [&]() {
-    // messages are taken in e->d_order (descending SHA-1 block count, built at commit): length-homogeneous warps, longest first
-    const uint32_t ngroups = (n.n_clusters + 31) / 32;
-    if (ngroups <= (uint32_t)e->sm_count * 4) {
-      // latency regime (C3: 313 groups): the pass waits for the longest message's serial chain — warp-specialised pairs,
-      // two per SM so that every hash warp has a scheduler to itself
-      const uint32_t G = std::min<uint32_t>(ngroups, (uint32_t)e->sm_count * 2);
-      k_hash3<1, 0><<<G, 64, sizeof(H3Smem), H>>>(s.json, s.c_json_off, s.c_json_len, e->d_order, n.n_clusters, r.hash);
-    } else {
-      // throughput regime: resident CTAs of four one-lane-per-message warps walk the groups, round adds on the FMA pipe
-      uint32_t blocks = std::min<uint32_t>((n.n_clusters + 127) / 128, (uint32_t)e->sm_count * e->hash_ctas_per_sm);
-      k_hash2<4, 1><<<blocks, 128, 0, H>>>(s.json, s.c_json_off, s.c_json_len, e->d_order, n.n_clusters, r.hash, 1u);
-    }
-  };
-  auto start_hash_stream = [&]() -> int {
-    if (profile) return KR_OK;
-    CK(cudaEventRecord(e->ev_fork, M)); CK(cudaStreamWaitEvent(H, e->ev_fork, 0));
-    CK(cudaStreamWaitEvent(H, e->ev_json, wflag));
-    if (do_hash && spin && n.n_clusters) CK(cudaMemsetAsync(r.hash, 0, 32 * (size_t)n.n_clusters, H));  // the digests' last words are "ready" marks (k_decide2)
-    if (do_hash) { launch_hash(); k++; }  // (counted among the pass's kernels: kr_profile.n_kernels)
+  // the digests, messages taken in e->d_order (built at commit), or zeros when the pass skips the hash
+  auto hash_or_zero = [&]() -> int {
+    if (do_hash) { c.mark("k_hash"); launch_hash(e, H, s.json, s.c_json_off, s.c_json_len, e->d_order, n.n_clusters, r.hash, e->hash_ctas_per_sm); }
     else if (n.n_clusters) CK(cudaMemsetAsync(r.hash, 0, 32 * (size_t)n.n_clusters, H));
-    CK(cudaEventRecord(e->ev_hash, H));
+    return KR_OK;
+  };
+  // where stream M needs the digests: it joins the hash stream (profiled, it runs the hash itself there)
+  auto join_hash = [&]() -> int {
+    if (profile) return hash_or_zero();
+    CK(cudaStreamWaitEvent(M, e->ev_hash, 0));
     return KR_OK;
   };
   // The hash goes first: its 313 one-warp CTAs must be resident before the main chain fills the SMs (launched after
   // k_build_tables instead, they queue behind the chain's blocks and the hash takes more than twice as long).
-  { int rc = start_hash_stream(); if (rc) return rc; }
+  if (!profile) {
+    CK(cudaEventRecord(e->ev_fork, M)); CK(cudaStreamWaitEvent(H, e->ev_fork, 0));
+    CK(cudaStreamWaitEvent(H, e->ev_json, wflag));
+    if (spin) CK(cudaMemsetAsync(r.hash, 0, 32 * (size_t)n.n_clusters, H));  // the digests' last words are "ready" marks (k_decide2)
+    if (int rc = hash_or_zero()) return rc;  // (the hash counts among the pass's kernels: kr_profile.n_kernels)
+    CK(cudaEventRecord(e->ev_hash, H));
+  }
 
   // --- stream M
   e->ran_bucket = bucket;
-  sc.bucket_stride = e->bstride;
   const bool pdl = !profile && e->use_pdl;
   bool fuse_place_done = false;    // k_decide_small directly follows k_place_fused on stream M
   bool creates_after_kernel = false;  // k_creates_fused directly follows a kernel on stream M (no event wait in between)
@@ -665,51 +737,35 @@ int launch_pass(kr_engine *e, const kr_flags &f, bool profile, bool capturing = 
     // per-cluster counts + the chained-scan cells + the workersToDelete Bloom bitmap + the bucket fill counters / first-head
     // cells (one region)
     ca.ptr[3] = sc.ccount; ca.words[3] = (uint32_t)((e->sl.cstart - e->sl.ccount) / 4); ca.value[3] = 0;
-    mark("k_clear");
+    c.mark("k_clear");
     k_clear<<<e->sm_count * 2, 256, 0, M>>>(ca);
   }
   CK(cudaStreamWaitEvent(M, e->ev_cols, wflag));  // the scratch clears above overlap the tail of the upload
   {
     uint32_t items = n.n_clusters + n.n_groups + n.n_heads;
-    if (items) { mark("k_build_tables"); k_build_tables<<<(items + 255) / 256, 256, 0, M>>>(s, sc, r, z); }
+    if (items) { c.mark("k_build_tables"); k_build_tables<<<(items + 255) / 256, 256, 0, M>>>(s, sc, r, z); }
   }
   if (bucket) {
     e->ran_fast = false;
     const uint32_t mtiles = e->sl.mtiles;
     if (n.n_pods) {
-      mark("k_match2");
+      c.mark("k_match2");
       CK(launch_pdl(k_match2<kMatchItems>, dim3(mtiles), dim3(kSortThreads), n.n_wtd ? e->sl.wt_bits_n / 8 : 0, M, pdl, s, sc, r, z, n.n_wtd ? 1 : 0));
     }
     Decide2Args da{s, sc, r, z, f, IncStage{}, e->cfg.max_creates, spin ? 1 : 0, 0};
-    const bool mh = e->snap_has_mh && f.gate_multihost_indexing;  // the instantiations with the multi-host branch
-    auto launch_decide2 = [&](dim3 grid, bool with_pdl) -> cudaError_t {
-      const dim3 block(kD2Warps * 32);
-      if (e->bstride <= 64) return launch_pdl(mh ? k_decide2<2, false, true> : k_decide2<2>, grid, block, 0, M, with_pdl, da);
-      if (e->bstride <= 128) return launch_pdl(mh ? k_decide2<4, false, true> : k_decide2<4>, grid, block, 0, M, with_pdl, da);
-      return launch_pdl(mh ? k_decide2<8, false, true> : k_decide2<8>, grid, block, 0, M, with_pdl, da);
-    };
     if (n.n_clusters) {
-      mark("k_decide2");
-      CK(launch_decide2(dim3((n.n_clusters + kD2Warps - 1) / kD2Warps), pdl && n.n_pods != 0));
+      c.mark("k_decide2");
+      CK(launch_decide2(c, da, dim3((n.n_clusters + kD2Warps - 1) / kD2Warps), false, pdl && n.n_pods != 0));
     } else CK(cudaMemsetAsync(r.act_start, 0, 4, M));
-    if (n.n_jobs) { mark("k_jobs"); k_jobs<<<(n.n_jobs + 255) / 256, 256, 0, M>>>(s, sc, r, z); }
+    if (n.n_jobs) { c.mark("k_jobs"); k_jobs<<<(n.n_jobs + 255) / 256, 256, 0, M>>>(s, sc, r, z); }
     const bool large = e->n_large && sc.lg && n.n_clusters;  // large RayClusters (kr_large.cuh): sorted beside the hash, decided after it
-    if (large && e->n_lsort) { mark("k_large_sort"); k_large_sort<false><<<e->n_lsort, kLargeSortThreads, 0, M>>>(da, lg_list); }
-    if (large && e->n_tiles) {  // huge RayClusters (kr_huge.cuh): sorted tile by tile, then merged, also beside the hash
-      mark("k_huge_tiles"); k_huge_tiles<false><<<e->n_tiles, kHugeThreads, 0, M>>>(da, hd);
-      mark("k_huge_merge"); k_huge_merge<false><<<e->n_tiles, kHugeThreads, 0, M>>>(da, hd);
-    }
-    if (profile) {
-      if (do_hash) { mark("k_hash"); launch_hash(); }
-      else if (n.n_clusters) CK(cudaMemsetAsync(r.hash, 0, 32 * (size_t)n.n_clusters, M));
-    } else {
-      CK(cudaStreamWaitEvent(M, e->ev_hash, 0));
-    }
-    if (large) { mark("k_decide_large"); k_decide_large<false><<<e->n_large, kLargeDecideThreads, 0, M>>>(da, lg_list); }
+    if (large) launch_large_sort<false>(c, da);
+    if (int rc = join_hash()) return rc;
+    if (large) { c.mark("k_decide_large"); k_decide_large<false><<<e->n_large, kLargeDecideThreads, 0, M>>>(da, c.lg_list); }
     if (e->n_recreate > 0 && do_hash && !spin) {  // clusters whose Recreate gate needs the digest: decided again, in the places phase 0 reserved
       da.phase = 1;
-      mark("k_decide2_phase1");
-      CK(launch_decide2(dim3((e->n_recreate + kD2Warps - 1) / kD2Warps), false));
+      c.mark("k_decide2_phase1");
+      CK(launch_decide2(c, da, dim3((e->n_recreate + kD2Warps - 1) / kD2Warps), false, false));
     }
   } else {
   const uint32_t ntiles = e->sl.ntiles;
@@ -717,35 +773,35 @@ int launch_pass(kr_engine *e, const kr_flags &f, bool profile, bool capturing = 
   e->ran_fast = fast;
   const uint32_t *sorted_keys = sc.keys[0];
   if (n.n_pods && fast) {
-    mark("k_match");
+    c.mark("k_match");
     const uint32_t mtiles = e->sl.mtiles;
     CK(launch_pdl(k_match<true, kMatchItems>, dim3(mtiles), dim3(kSortThreads), 0, M, pdl, s, sc, r, z, n.n_wtd ? 1 : 0));
     const bool fuse_place = !e->no_fuse && (uint64_t)n.n_clusters + 2 + mtiles <= kFusedMaxCounters;
     if (fuse_place) {
       fuse_place_done = true;
-      mark("k_place_fused");
+      c.mark("k_place_fused");
       size_t smem = 4 * ((size_t)n.n_clusters + 2 + mtiles);
       CK(launch_pdl(k_place_fused, dim3(e->sm_count * e->place_ctas), dim3(1024), smem, M, pdl, (const uint32_t *)sc.keys[0], (const uint32_t *)sc.keys[1], (const uint32_t *)sc.ccount, sc.cstart,
                     (const uint32_t *)sc.tile_orph, sc.vals[0], n.n_pods, n.n_clusters, mtiles, r.totals));
     } else {
-    mark("k_scan_counts");
+    c.mark("k_scan_counts");
     const uint32_t nch_c = (n.n_clusters + 1 + kScanChunk - 1) / kScanChunk, nch_t = (mtiles + kScanChunk - 1) / kScanChunk;
     k_scan_counts<<<nch_c + nch_t, 1024, 0, M>>>(sc.ccount, sc.cstart, n.n_clusters + 1, nch_c, sc.tile_orph, mtiles, sc.chain, r.totals);
-    mark("k_place");
+    c.mark("k_place");
     k_place<<<(n.n_pods + 1023) / 1024, 256, 0, M>>>(sc.keys[0], sc.keys[1], sc.cstart, sc.tile_orph, sc.vals[0], n.n_pods, n.n_clusters);
     }
   } else if (n.n_pods) {
     uint32_t bits = 1;
     while ((1ull << bits) <= n.n_clusters) bits++;  // keys are in [0, n_clusters]
     const int passes = (int)((bits + kRadixBits - 1) / kRadixBits);
-    mark("k_match");
+    c.mark("k_match");
     k_match<false, kSortItems><<<ntiles, kSortThreads, 0, M>>>(s, sc, r, z, n.n_wtd ? 1 : 0);
     int cur = 0;
     for (int p = 0; p < passes; p++) {
-      if (p > 0) { mark("k_hist"); k_hist<<<ntiles, kSortThreads, 0, M>>>(sc.keys[cur], sc.hist, n.n_pods, p * kRadixBits); }
-      mark("k_scan_rows");
+      if (p > 0) { c.mark("k_hist"); k_hist<<<ntiles, kSortThreads, 0, M>>>(sc.keys[cur], sc.hist, n.n_pods, p * kRadixBits); }
+      c.mark("k_scan_rows");
       k_scan_rows<<<kRadix, kRowScanThreads, 0, M>>>(sc.hist, sc.row_total, ntiles);
-      mark("k_scatter");
+      c.mark("k_scatter");
       uint32_t *vout = (p == passes - 1) ? r.sorted_pod_idx : sc.vals[cur ^ 1];
       k_scatter<<<ntiles, kSortThreads, 0, M>>>(sc.keys[cur], sc.vals[cur], sc.keys[cur ^ 1], vout, sc.hist, sc.row_total, n.n_pods, p * kRadixBits, p == 0);
       cur ^= 1;
@@ -760,21 +816,16 @@ int launch_pass(kr_engine *e, const kr_flags &f, bool profile, bool capturing = 
     cudaStream_t G2 = (fast && !profile) ? e->sg : M;
     if (fast && !profile) { CK(cudaEventRecord(e->ev_fork2, M)); CK(cudaStreamWaitEvent(G2, e->ev_fork2, 0)); }
     uint32_t warps = n.n_clusters + 1;
-    mark("k_decide");
+    c.mark("k_decide");
     k_decide<<<(warps + kDecideWarps - 1) / kDecideWarps, kDecideWarps * 32, 0, G2>>>(da);
     if (fast && n.n_clusters) {
-      mark("k_decide_small");
+      c.mark("k_decide_small");
       CK(launch_pdl(k_decide_small, dim3((n.n_clusters + kDecideWarps - 1) / kDecideWarps), dim3(kDecideWarps * 32), 0, M, pdl && fuse_place_done, da));
     }
     if (fast && !profile) { CK(cudaEventRecord(e->ev_join2, G2)); CK(cudaStreamWaitEvent(M, e->ev_join2, 0)); }
   }
-  if (n.n_jobs) { mark("k_jobs"); k_jobs<<<(n.n_jobs + 255) / 256, 256, 0, M>>>(s, sc, r, z); }
-  if (profile) {
-    if (do_hash) { mark("k_hash"); launch_hash(); }
-    else if (n.n_clusters) CK(cudaMemsetAsync(r.hash, 0, 32 * (size_t)n.n_clusters, M));
-  } else {
-    CK(cudaStreamWaitEvent(M, e->ev_hash, 0));
-  }
+  if (n.n_jobs) { c.mark("k_jobs"); k_jobs<<<(n.n_jobs + 255) / 256, 256, 0, M>>>(s, sc, r, z); }
+  if (int rc = join_hash()) return rc;
   if (e->n_recreate > 0 && do_hash) {
     da.phase = 1;
     uint32_t warps = e->n_recreate;  // upper bound on the deferred list
@@ -782,38 +833,37 @@ int launch_pass(kr_engine *e, const kr_flags &f, bool profile, bool capturing = 
     // like phase 0: the register-resident kernel on M for the small clusters, the general one beside it on G for the rest
     cudaStream_t G1 = (fast && !profile) ? e->sg : M;
     if (fast && !profile) { CK(cudaEventRecord(e->ev_fork3, M)); CK(cudaStreamWaitEvent(G1, e->ev_fork3, 0)); }
-    mark("k_decide_phase1");
+    c.mark("k_decide_phase1");
     k_decide<<<grid1, block1, 0, G1>>>(da);
-    if (fast) { mark("k_decide_small_phase1"); k_decide_small<<<grid1, block1, 0, M>>>(da); }
+    if (fast) { c.mark("k_decide_small_phase1"); k_decide_small<<<grid1, block1, 0, M>>>(da); }
     if (fast && !profile) { CK(cudaEventRecord(e->ev_join3, G1)); CK(cudaStreamWaitEvent(M, e->ev_join3, 0)); }
     creates_after_kernel = !(fast && !profile);
   }
   if (!e->no_fuse && (uint64_t)n.n_groups + n.n_clusters + 1 <= kFusedMaxCounters) {
-    mark("k_creates_fused");
+    c.mark("k_creates_fused");
     CK(launch_pdl(k_creates_fused, dim3(e->sm_count), dim3(1024), 4 * ((size_t)n.n_groups + n.n_clusters + 1), M, pdl && creates_after_kernel, s, sc, r, z, f, e->cfg.max_creates));
   } else {
     const uint32_t nch_a = (n.n_clusters + kScanChunk - 1) / kScanChunk;
     uint32_t *achain = sc.chain + 2 * ((size_t)(n.n_clusters + 1 + kScanChunk - 1) / kScanChunk + (e->sl.mtiles + kScanChunk - 1) / kScanChunk + (n.n_groups + kScanChunk - 1) / kScanChunk + 1);
     if (n.n_clusters) {
       if (e->force_radix) CK(cudaMemsetAsync(achain, 0, 8 * (size_t)nch_a, M));
-      mark("k_scan_actions");
+      c.mark("k_scan_actions");
       k_scan_actions<<<nch_a, 1024, 0, M>>>(r, sc.cact, n.n_clusters, achain);
-      mark("k_compact_actions");
+      c.mark("k_compact_actions");
       k_compact_actions<<<(n.n_clusters + 3) / 4, 128, 0, M>>>(r, sc, n.n_clusters);
     } else CK(cudaMemsetAsync(r.act_start, 0, 4, M));
   }
   if (e->no_fuse || (uint64_t)n.n_groups + n.n_clusters + 1 > kFusedMaxCounters) if (n.n_groups) {
-    mark("k_scan_creates");
+    c.mark("k_scan_creates");
     const uint32_t nch_g = (n.n_groups + kScanChunk - 1) / kScanChunk;
     uint32_t *gchain = sc.chain + 2 * ((size_t)(n.n_clusters + 1 + kScanChunk - 1) / kScanChunk + (e->sl.mtiles + kScanChunk - 1) / kScanChunk);
     if (e->force_radix) CK(cudaMemsetAsync(gchain, 0, 8 * (size_t)nch_g, M));  // (the fast pipeline cleared the cells together with ccount)
     k_scan_creates<<<nch_g, 1024, 0, M>>>(r, sc.gcreate, n.n_groups, gchain);
-    mark("k_create_fill");
+    c.mark("k_create_fill");
     k_create_fill<<<(n.n_groups + 3) / 4, 128, 0, M>>>(s, sc, r, z, f, e->cfg.max_creates);
   }
   }  // sort / radix pipelines
-  if (profile && k <= KR_MAX_KERNEL_TIMES) cudaEventRecord(e->ev_k[k < KR_MAX_KERNEL_TIMES ? k : KR_MAX_KERNEL_TIMES], M);
-  e->prof.n_kernels = (uint32_t)k;
+  c.close();
   CK(cudaGetLastError());
   return KR_OK;
 }
@@ -906,26 +956,26 @@ void after_full_pass(kr_engine *e, const kr_flags &f) {
   if (!f.skip_hash) { e->hash_dirty = false; clear_spec_rows(e); }
 }
 
+// A pass has read what the commits since the previous one uploaded: the pinned hash order is free again, and kr_profile keeps the
+// commits' bytes (h2d_bytes) and copy time (h2d_ms).
+void commits_read(kr_engine *e) {
+  e->order_pending = false;
+  e->h2d_accum = 0;  // (kr_profile.h2d_bytes keeps the sum of the commits that fed this pass)
+  if (!e->h2d_timed) {
+    float ms = 0;
+    if (cudaEventElapsedTime(&ms, e->ev_h2d0, e->ev_h2d1) == cudaSuccess) e->prof.h2d_ms = ms;
+    e->h2d_timed = true;
+  }
+}
+
 // One incremental pass over the resident state (kr_incr.cuh).  Returns KR_OK with *done_inc = true when its results stand;
 // *done_inc = false means the attempt was void (structural object change, bucket / arena overflow) and a full pass must follow.
 int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile, bool *done_inc) {
   *done_inc = false;
+  PassCtx c(e, profile);
   const kr_sizes &n = e->sizes;
-  SnapDev s;
-  bind_in(e->il, e->d_in, &s);
-  ResDev r = bind_out(e->ol, e->d_out);
-  ScratchDev sc = bind_scratch(e->sl, e->d_scratch);
-  sc.bucket_stride = e->bstride;
-  const uint32_t *lg_list = bind_large(e, sc);
-  const HugeDev hd = bind_huge(e);
-  Sizes z{n.n_clusters, n.n_groups, n.n_wtd, n.n_pods, n.n_heads, n.n_jobs};
-  cudaStream_t M = e->sm, H = profile ? e->sm : e->sh;
-  int k = 0;
-  auto mark = [&](const char *name) {
-    if (profile && k < KR_MAX_KERNEL_TIMES) { e->prof.kernel_name[k] = name; cudaEventRecord(e->ev_k[k], M); }
-    k++;
-  };
-  e->prof.n_kernels = 0;
+  const SnapDev &s = c.s; const ResDev &r = c.r; const ScratchDev &sc = c.sc; const Sizes &z = c.z;
+  const cudaStream_t M = c.M, H = c.H;
   CK(cudaStreamWaitEvent(M, e->ev_cols, 0));
   const bool do_hash = e->hash_dirty && !f.skip_hash && n.n_clusters > 0;
   // ... or only the messages kr_snapshot_commit_spec_rows listed (a whole-arena commit wins; a skip_hash pass leaves them pending)
@@ -938,113 +988,77 @@ int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile
     const uint32_t nm = do_hash ? n.n_clusters : n_rows;
     if (!profile) { CK(cudaEventRecord(e->ev_fork, M)); CK(cudaStreamWaitEvent(H, e->ev_fork, 0)); }
     CK(cudaStreamWaitEvent(H, e->ev_json, 0));
-    if (profile) mark(do_hash ? "k_hash" : "k_hash_rows");
-    const uint32_t ngroups = (nm + 31) / 32;
-    if (ngroups <= (uint32_t)e->sm_count * 4)
-      k_hash3<1, 0><<<std::min<uint32_t>(ngroups, (uint32_t)e->sm_count * 2), 64, sizeof(H3Smem), H>>>(s.json, s.c_json_off, s.c_json_len, order, nm, r.hash);
-    else
-      k_hash2<4, 1><<<std::min<uint32_t>((nm + 127) / 128, (uint32_t)e->sm_count * e->hash_ctas_per_sm), 128, 0, H>>>(s.json, s.c_json_off, s.c_json_len, order, nm, r.hash, 1u);
+    if (profile) c.mark(do_hash ? "k_hash" : "k_hash_rows");  // (unprofiled, an incremental pass does not count its hash)
+    launch_hash(e, H, s.json, s.c_json_off, s.c_json_len, order, nm, r.hash, e->hash_ctas_per_sm);
     if (!profile) CK(cudaEventRecord(e->ev_hash, H));
-    if (e->n_recreate && do_hash) { mark("k_inc_mark_recreate"); k_inc_mark_recreate<<<(n.n_clusters + 255) / 256, 256, 0, M>>>(s, sc, z); }
-    if (e->n_recreate && !do_hash) { mark("k_inc_mark_rows"); k_inc_mark_rows<<<(n_rows + 255) / 256, 256, 0, M>>>(s, sc, spec_rows, n_rows); }
+    if (e->n_recreate && do_hash) { c.mark("k_inc_mark_recreate"); k_inc_mark_recreate<<<(n.n_clusters + 255) / 256, 256, 0, M>>>(s, sc, z); }
+    if (e->n_recreate && !do_hash) { c.mark("k_inc_mark_rows"); k_inc_mark_rows<<<(n_rows + 255) / 256, 256, 0, M>>>(s, sc, spec_rows, n_rows); }
   }
   const int grid = e->sm_count * 2;
   if (e->heads_rebuild) {  // a head Pod came or went since the table was built (the commit compared the keys on the host)
-    mark("k_inc_aux_rebuild");
+    c.mark("k_inc_aux_rebuild");
     k_inc_aux_clear<<<std::min<uint32_t>(grid, (e->sl.aux_slots + 255) / 256), 256, 0, M>>>(sc);
     k_inc_aux_insert<<<std::min<uint32_t>(grid, (n.n_heads + 255) / 256 + 1), 256, 0, M>>>(s, sc, z);
   }
   if (e->wtd_rebuild) {  // a workersToDelete list changed since the name table was built (KR_OPT_WTD_EDITS; the commit compared them on the host)
-    if (e->res_n_wtd) { mark("k_inc_wtd_release"); k_inc_wtd_release<<<(e->res_n_wtd + 255) / 256, 256, 0, M>>>(s, sc, r, e->res_n_wtd, e->inc_n_pods); }
-    mark("k_inc_wtd_clear");
+    if (e->res_n_wtd) { c.mark("k_inc_wtd_release"); k_inc_wtd_release<<<(e->res_n_wtd + 255) / 256, 256, 0, M>>>(s, sc, r, e->res_n_wtd, e->inc_n_pods); }
+    c.mark("k_inc_wtd_clear");
     k_inc_wtd_clear<<<std::min<uint32_t>(grid, (e->sl.wt_slots + 255) / 256), 256, 0, M>>>(sc, r, n.n_wtd);
     if (n.n_wtd) {
-      mark("k_inc_wtd_insert");
+      c.mark("k_inc_wtd_insert");
       k_inc_wtd_insert<<<std::min<uint32_t>(grid, (n.n_groups + 255) / 256 + 1), 256, 0, M>>>(s, sc, z);
-      mark("k_inc_wtd_resolve");
+      c.mark("k_inc_wtd_resolve");
       k_inc_wtd_resolve<<<std::min<uint32_t>((uint32_t)e->sm_count * 4, (n.n_pods + 255) / 256 + 1), 256, e->sl.wt_bits_n / 8, M>>>(s, sc, r, z, e->inc_n_pods);
     }
     e->res_n_wtd = n.n_wtd;
     e->wtd_rebuild = false;
   }
   // (k_inc_refresh ran behind the object commits' diff kernels: the input records are current)
-  mark("k_inc_admit");
+  c.mark("k_inc_admit");
   k_inc_admit<<<grid, 256, 0, M>>>(s, sc, r, z, n.n_wtd ? 1 : 0);
   if ((do_hash || n_rows) && !profile) CK(cudaStreamWaitEvent(M, e->ev_hash, 0));
-  // staging for the changed records: up to a quarter of the RayClusters (beyond that the whole record arrays are as cheap to move)
-  IncStage st{};
-  size_t dig_off = 0;
-  {
-    const uint32_t capc = std::max<uint32_t>(64, n.n_clusters / 4), capg = (uint32_t)std::min<uint64_t>((uint64_t)capc * KR_SMEM_GROUPS, (uint64_t)n.n_groups + 1);
-    const size_t need = inc_stage_bytes(capc, capg, &dig_off);
-    if (need > e->inc_stage_cap) {
-      if (e->d_inc_stage) cudaFree(e->d_inc_stage);
-      if (e->h_inc_stage) cudaFreeHost(e->h_inc_stage);
-      e->d_inc_stage = nullptr; e->h_inc_stage = nullptr; e->inc_stage_cap = 0;
-      CK(cudaMalloc((void **)&e->d_inc_stage, need));
-      CK(cudaHostAlloc((void **)&e->h_inc_stage, need, cudaHostAllocDefault));
-      e->inc_stage_cap = need;
-    }
-    e->inc_stage_clusters = capc; e->inc_stage_groups = capg;
-    st.meta = reinterpret_cast<uint32_t *>(e->d_inc_stage);
-    st.clusters = reinterpret_cast<kr_cluster_result *>(e->d_inc_stage + align_up(32 * (size_t)capc));
-    st.groups = reinterpret_cast<kr_group_result *>(e->d_inc_stage + align_up(32 * (size_t)capc) + align_up(sizeof(kr_cluster_result) * (size_t)capc));
-    st.cap_clusters = capc; st.cap_groups = capg;
-  }
-  const bool gather_rows = n_rows && n_rows <= e->inc_stage_clusters;  // (more re-hashed digests than that: the fetch copies them all)
+  const IncStageLayout sl = e->inc_layout = inc_stage_layout(n.n_clusters, n.n_groups);  // staging for the changed records
+  if (sl.total > e->inc_stage.cap) return fail(e, KR_E_STATE, "internal: incremental staging of %zu bytes, room for %zu", sl.total, e->inc_stage.cap);
+  const IncStage st{reinterpret_cast<uint32_t *>(e->inc_stage.d), reinterpret_cast<kr_cluster_result *>(e->inc_stage.d + sl.clusters),
+                    reinterpret_cast<kr_group_result *>(e->inc_stage.d + sl.groups), sl.capc, sl.capg};
+  const bool gather_rows = n_rows && n_rows <= sl.capc;  // (more re-hashed digests than that: the fetch copies them all)
   if (gather_rows) {
-    mark("k_inc_digest_gather");
-    k_inc_digest_gather<<<(2 * n_rows + 255) / 256, 256, 0, M>>>(spec_rows, n_rows, r.hash, reinterpret_cast<char *>(e->d_inc_stage + dig_off));
+    c.mark("k_inc_digest_gather");
+    k_inc_digest_gather<<<(2 * n_rows + 255) / 256, 256, 0, M>>>(spec_rows, n_rows, r.hash, reinterpret_cast<char *>(e->inc_stage.d + sl.digests));
   }
   if (n.n_clusters) {
     Decide2Args da{s, sc, r, z, f, st, e->cfg.max_creates, 0, 2};
-    const dim3 dgrid((n.n_clusters + kD2Warps - 1) / kD2Warps), dblock(kD2Warps * 32);
-    mark("k_decide2_dirty");
+    c.mark("k_decide2_dirty");
     // (snap_has_mh as of the latest commit: an object commit may have brought the snapshot's first multi-host group or taken its last)
-    const bool mh = e->snap_has_mh && f.gate_multihost_indexing;
-    if (e->bstride <= 64) (mh ? k_decide2<2, true, true> : k_decide2<2, true>)<<<dgrid, dblock, 0, M>>>(da);
-    else if (e->bstride <= 128) (mh ? k_decide2<4, true, true> : k_decide2<4, true>)<<<dgrid, dblock, 0, M>>>(da);
-    else (mh ? k_decide2<8, true, true> : k_decide2<8, true>)<<<dgrid, dblock, 0, M>>>(da);
+    CK(launch_decide2(c, da, dim3((n.n_clusters + kD2Warps - 1) / kD2Warps), true, false));
     if (e->n_large) {  // the dirty large RayClusters (k_decide2 left every cluster past the stride alone)
       CK(cudaMemsetAsync(sc.inc + KR_INC_LSEG, 0, 4, M));
-      if (e->n_lsort) { mark("k_large_sort"); k_large_sort<true><<<e->n_lsort, kLargeSortThreads, 0, M>>>(da, lg_list); }
-      if (e->n_tiles) {
-        mark("k_huge_tiles"); k_huge_tiles<true><<<e->n_tiles, kHugeThreads, 0, M>>>(da, hd);
-        mark("k_huge_merge"); k_huge_merge<true><<<e->n_tiles, kHugeThreads, 0, M>>>(da, hd);
-      }
-      mark("k_decide_large");
-      k_decide_large<true><<<e->n_large, kLargeDecideThreads, 0, M>>>(da, lg_list);
+      launch_large_sort<true>(c, da);
+      c.mark("k_decide_large");
+      k_decide_large<true><<<e->n_large, kLargeDecideThreads, 0, M>>>(da, c.lg_list);
     }
   }
-  if (n.n_jobs) { mark("k_jobs"); k_jobs<<<(n.n_jobs + 255) / 256, 256, 0, M>>>(s, sc, r, z); }
-  if (profile && k <= KR_MAX_KERNEL_TIMES) cudaEventRecord(e->ev_k[k < KR_MAX_KERNEL_TIMES ? k : KR_MAX_KERNEL_TIMES], M);
-  e->prof.n_kernels = (uint32_t)k;
+  if (n.n_jobs) { c.mark("k_jobs"); k_jobs<<<(n.n_jobs + 255) / 256, 256, 0, M>>>(s, sc, r, z); }
+  c.close();
   if (done) CK(cudaEventRecord(done, M));
   CK(cudaMemcpyAsync(e->h_totals, e->d_out + e->ol.totals, 48, cudaMemcpyDeviceToHost, M));
   CK(cudaMemcpyAsync(e->h_inc, sc.inc, 64, cudaMemcpyDeviceToHost, M));
-  if (!e->ev_inc) CK(cudaEventCreateWithFlags(&e->ev_inc, cudaEventDisableTiming));
   CK(cudaEventRecord(e->ev_inc, M));
   k_inc_finish<<<1, 32, 0, M>>>(sc);  // (the host does not wait for it: whatever comes next is ordered behind it on this stream)
   CK(cudaGetLastError());
   CK(cudaEventSynchronize(e->ev_inc));
-  e->order_pending = false;
-  e->h2d_accum = 0;
-  if (!e->h2d_timed) {
-    float ms = 0;
-    if (cudaEventElapsedTime(&ms, e->ev_h2d0, e->ev_h2d1) == cudaSuccess) e->prof.h2d_ms = ms;
-    e->h2d_timed = true;
-  }
+  commits_read(e);
   e->heads_rebuild = false;  // (rebuilt here, or about to be rebuilt by the full pass)
   if (e->h_inc[KR_INC_VOID] || e->h_inc[KR_INC_STRUCTURAL]) return KR_OK;  // the caller takes the full pass
   if (!e->fetched) e->host_results_stale = true;  // the previous pass's records never reached the host copy
   e->fetched = false;
   e->inc_n_dirty = e->h_inc[KR_INC_DIRTY];
-  e->inc_gathered = e->inc_n_dirty <= e->inc_stage_clusters && e->h_inc[KR_INC_GROUPS] <= e->inc_stage_groups;
+  e->inc_gathered = e->inc_n_dirty <= sl.capc && e->h_inc[KR_INC_GROUPS] <= sl.capg;
   e->inc_hash_ran = do_hash;
   if (do_hash) e->hash_dirty = false;
   e->inc_spec_n = n_rows; e->inc_spec_gathered = gather_rows;
   if (n_rows) {
-    const uint32_t *h = reinterpret_cast<const uint32_t *>(e->h_spec + 16 * ((size_t)e->cfg.max_clusters + 1));
+    const uint32_t *h = reinterpret_cast<const uint32_t *>(e->spec.h + 16 * ((size_t)e->cfg.max_clusters + 1));
     e->spec_hashed.assign(h, h + n_rows);
   }
   if (do_hash || n_rows) clear_spec_rows(e);
@@ -1053,17 +1067,32 @@ int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile
   return KR_OK;
 }
 
-// Runs the pass; if the fast pipeline met a bucket it cannot sort (> 1024 pods in one RayCluster or among the orphans),
-// switches this layout to the radix pipeline and runs again.  Leaves the stream synchronised (after an incremental pass only its one-thread epoch-closing kernel may still be in flight: it touches the epoch counters, nothing a reader of the results sees).
-int run_pass(kr_engine *e, const kr_flags &f, cudaEvent_t done) {
+// The pass's results stand: kernels_ms is the time from ev_a to `done`.
+int pass_done(kr_engine *e, cudaEvent_t done) {
+  float ms = 0;
+  if (cudaEventElapsedTime(&ms, e->ev_a, done) == cudaSuccess) e->prof.kernels_ms = ms;
+  e->ran = true;
+  return KR_OK;
+}
+
+// Runs the pass: an incremental epoch when the resident state allows one, else the full pass, which runs again on the next pipeline
+// of its ladder while it meets a RayCluster its pipeline cannot hold.  Records `done` behind the kernels and leaves the stream
+// synchronised (after an incremental pass only its one-thread epoch-closing kernel may still be in flight: it touches the epoch
+// counters, nothing a reader of the results sees).  ev_a is recorded once, first; profile: each kernel between events, no graph,
+// and ev_a recorded again before each attempt, so that kernels_ms covers the last one.
+int run_pass(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile) {
+  if (!e->committed) return fail(e, KR_E_STATE, "no committed snapshot");
+  CK(cudaSetDevice(e->cfg.device));
+  if (!profile) CK(cudaEventRecord(e->ev_a, e->sm));
   e->last_flags = f;
   new_pull_epoch(e);
   // (the list moves only with a group count, which no incremental epoch absorbs, an option or a new layout: a full pass follows)
   if (e->lg_stale) if (int rc = upload_lg(e)) return rc;
   if (e->inc_valid && !e->no_incr && memcmp(&e->inc_flags, &f, sizeof f) == 0) {
+    if (profile) CK(cudaEventRecord(e->ev_a, e->sm));
     bool ok = false;
-    if (int rc = run_pass_inc(e, f, done, false, &ok)) return rc;
-    if (ok) { e->inc_n_pods = e->sizes.n_pods; e->inc_n_heads = e->sizes.n_heads; return KR_OK; }
+    if (int rc = run_pass_inc(e, f, done, profile, &ok)) return rc;
+    if (ok) { e->inc_n_pods = e->sizes.n_pods; e->inc_n_heads = e->sizes.n_heads; return pass_done(e, done); }
   }
   e->inc_valid = false; e->ran_inc = false;
   if (e->inc_zero_needed) {  // first pass on this layout: stamps, dirty flags and epoch counters start from zero
@@ -1072,23 +1101,20 @@ int run_pass(kr_engine *e, const kr_flags &f, cudaEvent_t done) {
   }
   if (e->spec_order_stale && !f.skip_hash) if (int rc = refresh_order(e)) return rc;
   for (int attempt = 0; attempt < 5; attempt++) {
-    int rc = run_pass_once(e, f);
-    if (rc) return rc;
+    if (profile) CK(cudaEventRecord(e->ev_a, e->sm));
+    if (int rc = profile ? launch_pass(e, f, true) : run_pass_once(e, f)) return rc;
     if (done) CK(cudaEventRecord(done, e->sm));
     CK(cudaMemcpyAsync(e->h_totals, e->d_out + e->ol.totals, 48, cudaMemcpyDeviceToHost, e->sm));
     CK(cudaStreamSynchronize(e->sm));
-    e->order_pending = false;
-    e->h2d_accum = 0;  // (kr_profile.h2d_bytes keeps the sum of the commits that fed this pass)
-    if (!e->h2d_timed) {
-      float ms = 0;
-      if (cudaEventElapsedTime(&ms, e->ev_h2d0, e->ev_h2d1) == cudaSuccess) e->prof.h2d_ms = ms;
-      e->h2d_timed = true;
-    }
-    if (e->h_totals[3] & KR_TOTALS_HASH_WAIT) {  // a decide warp gave up waiting for its digest: rerun on the two-phase schedule
+    // A profiled full pass frees the pinned hash order but leaves the commits' h2d_accum and h2d_ms alone: h2d_bytes then keeps
+    // adding up until an unprofiled pass or an incremental one reads the commits.
+    if (!profile) commits_read(e);
+    else e->order_pending = false;
+    if (e->h_totals[3] & KR_TOTALS_HASH_WAIT) {  // a decide warp gave up waiting for its digest (a profiled pass never waits): rerun on the two-phase schedule
       e->hash_spin = false; e->gvalid = false;
       continue;
     }
-    if (!(e->h_totals[3] & KR_TOTALS_BIG_BUCKET)) { after_full_pass(e, f); return KR_OK; }
+    if (!(e->h_totals[3] & KR_TOTALS_BIG_BUCKET)) { after_full_pass(e, f); return pass_done(e, done); }
     // some RayCluster outgrew what this pipeline holds per bucket: bucket pipeline -> wider stride -> sort pipeline -> radix pipeline
     if (e->ran_bucket) {
       if (int rc = after_bucket_void(e)) return rc;
@@ -1099,7 +1125,7 @@ int run_pass(kr_engine *e, const kr_flags &f, cudaEvent_t done) {
   return fail(e, KR_E_STATE, "internal: radix pipeline flagged a big bucket");
 }
 
-// Results back to the pinned host arena.  run_pass already brought the 32-byte totals over, so every copy is issued with its
+// Results back to the pinned host arena.  run_pass already brought the totals words over, so every copy is issued with its
 // exact size up front and the host waits once: [small fixed part] (+ the full pod lists when asked for) + the compact action
 // list + the replica-index arena.
 int fetch_results(kr_engine *e, kr_results_view *out) {
@@ -1117,18 +1143,16 @@ int fetch_results(kr_engine *e, kr_results_view *out) {
   const bool packed = inc && e->inc_gathered;
   uint64_t bytes = 0;
   const uint32_t nd = e->inc_n_dirty, ngr = inc ? e->h_inc[KR_INC_GROUPS] : 0;
-  const size_t st_cl = align_up(32 * (size_t)e->inc_stage_clusters), st_gr = st_cl + align_up(sizeof(kr_cluster_result) * (size_t)e->inc_stage_clusters);
-  size_t st_dig;
-  inc_stage_bytes(e->inc_stage_clusters, e->inc_stage_groups, &st_dig);
+  const size_t st_cl = e->inc_layout.clusters, st_gr = e->inc_layout.groups, st_dig = e->inc_layout.digests;
   const bool spec_packed = packed && e->inc_spec_n && e->inc_spec_gathered && !e->inc_hash_ran;
   if (packed) {
     // incremental pass: the changed cluster / group records come back packed (k_inc_gather) and are scattered into the host
     // arena below; the flat arrays an epoch can touch anywhere (name resolutions, RayJob rows, digests when they were
     // recomputed) are small and come back whole
     if (nd) {
-      CK(cudaMemcpyAsync(e->h_inc_stage, e->d_inc_stage, 32 * (size_t)nd, cudaMemcpyDeviceToHost, e->sm));
-      CK(cudaMemcpyAsync(e->h_inc_stage + st_cl, e->d_inc_stage + st_cl, sizeof(kr_cluster_result) * (size_t)nd, cudaMemcpyDeviceToHost, e->sm));
-      if (ngr) CK(cudaMemcpyAsync(e->h_inc_stage + st_gr, e->d_inc_stage + st_gr, sizeof(kr_group_result) * (size_t)ngr, cudaMemcpyDeviceToHost, e->sm));
+      CK(cudaMemcpyAsync(e->inc_stage.h, e->inc_stage.d, 32 * (size_t)nd, cudaMemcpyDeviceToHost, e->sm));
+      CK(cudaMemcpyAsync(e->inc_stage.h + st_cl, e->inc_stage.d + st_cl, sizeof(kr_cluster_result) * (size_t)nd, cudaMemcpyDeviceToHost, e->sm));
+      if (ngr) CK(cudaMemcpyAsync(e->inc_stage.h + st_gr, e->inc_stage.d + st_gr, sizeof(kr_group_result) * (size_t)ngr, cudaMemcpyDeviceToHost, e->sm));
       bytes += (32 + sizeof(kr_cluster_result)) * (uint64_t)nd + sizeof(kr_group_result) * (uint64_t)ngr;
     }
     CK(cudaMemcpyAsync(e->h_out + e->ol.totals, e->d_out + e->ol.totals, 256, cudaMemcpyDeviceToHost, e->sm));
@@ -1136,7 +1160,7 @@ int fetch_results(kr_engine *e, kr_results_view *out) {
     if (n.n_jobs) { CK(cudaMemcpyAsync(e->h_out + e->ol.jobs, e->d_out + e->ol.jobs, sizeof(kr_job_result) * (size_t)n.n_jobs, cudaMemcpyDeviceToHost, e->sm)); bytes += sizeof(kr_job_result) * (uint64_t)n.n_jobs; }
     if ((e->inc_hash_ran || (e->inc_spec_n && !e->inc_spec_gathered)) && n.n_clusters) { CK(cudaMemcpyAsync(e->h_out + e->ol.hash, e->d_out + e->ol.hash, 32 * (size_t)n.n_clusters, cudaMemcpyDeviceToHost, e->sm)); bytes += 32ull * n.n_clusters; }
     else if (e->inc_spec_n) {  // the digests of the spec rows, packed by k_inc_digest_gather
-      CK(cudaMemcpyAsync(e->h_inc_stage + st_dig, e->d_inc_stage + st_dig, 32 * (size_t)e->inc_spec_n, cudaMemcpyDeviceToHost, e->sm));
+      CK(cudaMemcpyAsync(e->inc_stage.h + st_dig, e->inc_stage.d + st_dig, 32 * (size_t)e->inc_spec_n, cudaMemcpyDeviceToHost, e->sm));
       bytes += 32ull * e->inc_spec_n;
     }
   } else {
@@ -1144,13 +1168,7 @@ int fetch_results(kr_engine *e, kr_results_view *out) {
     CK(cudaMemcpyAsync(e->h_out, e->d_out, e->ol.small_total, cudaMemcpyDeviceToHost, e->sm));
   }
   if (inc && nd) {  // the changed-cluster list itself
-    if ((size_t)nd > e->h_changed_cap) {
-      if (e->h_changed) cudaFreeHost(e->h_changed);
-      e->h_changed = nullptr; e->h_changed_cap = 0;
-      const size_t cap = std::max<size_t>(1024, (size_t)e->cfg.max_clusters);
-      CK(cudaHostAlloc((void **)&e->h_changed, 4 * cap, cudaHostAllocDefault));
-      e->h_changed_cap = cap;
-    }
+    if ((size_t)nd > e->h_changed_cap) return fail(e, KR_E_STATE, "internal: %u changed RayClusters, room for %zu", nd, e->h_changed_cap);
     CK(cudaMemcpyAsync(e->h_changed, e->d_scratch + e->sl.dirty_list, 4 * (size_t)nd, cudaMemcpyDeviceToHost, e->sm));
     bytes += 4ull * nd;
   }
@@ -1178,9 +1196,9 @@ int fetch_results(kr_engine *e, kr_results_view *out) {
   CK(cudaStreamSynchronize(e->sm));
   if (packed && nd) {  // scatter the packed records into the host arena
     ResDev hr = bind_out(e->ol, e->h_out);
-    const uint32_t *meta = reinterpret_cast<const uint32_t *>(e->h_inc_stage);
-    const kr_cluster_result *scl = reinterpret_cast<const kr_cluster_result *>(e->h_inc_stage + st_cl);
-    const kr_group_result *sgr = reinterpret_cast<const kr_group_result *>(e->h_inc_stage + st_gr);
+    const uint32_t *meta = reinterpret_cast<const uint32_t *>(e->inc_stage.h);
+    const kr_cluster_result *scl = reinterpret_cast<const kr_cluster_result *>(e->inc_stage.h + st_cl);
+    const kr_group_result *sgr = reinterpret_cast<const kr_group_result *>(e->inc_stage.h + st_gr);
     for (uint32_t i = 0; i < nd; i++) {
       const uint32_t *m = meta + 8 * (size_t)i;
       const uint32_t c = m[0];
@@ -1190,7 +1208,7 @@ int fetch_results(kr_engine *e, kr_results_view *out) {
   }
   if (spec_packed) {  // ... and the re-hashed digests
     char *hh = reinterpret_cast<char *>(e->h_out + e->ol.hash);
-    for (uint32_t i = 0; i < e->inc_spec_n; i++) memcpy(hh + 32 * (size_t)e->spec_hashed[i], e->h_inc_stage + st_dig + 32 * (size_t)i, 32);
+    for (uint32_t i = 0; i < e->inc_spec_n; i++) memcpy(hh + 32 * (size_t)e->spec_hashed[i], e->inc_stage.h + st_dig + 32 * (size_t)i, 32);
   }
   e->fetched = true; e->host_results_stale = false;
   if (out) {
@@ -1208,6 +1226,37 @@ int fetch_results(kr_engine *e, kr_results_view *out) {
   float ms = 0;
   if (cudaEventElapsedTime(&ms, e->ev_b, e->ev_c) == cudaSuccess) e->prof.d2h_ms = ms;
   e->prof.d2h_bytes = bytes;
+  return KR_OK;
+}
+
+// The on-device diff of an object commit (kr_incr.cuh), on the copy stream: the staged rows of oa's columns against the resident
+// ones (changed rows mark their RayCluster dirty, a changed key makes the next pass a full one), the head-aux keys of the n_hd rows
+// head_rows (device list; nullptr: rows 0 .. n_hd - 1), then with `refresh` the input records (cl_in) of the RayClusters the diff
+// found changed, now that every column of theirs is in place.
+int launch_object_diff(kr_engine *e, ObjDiffArgs oa, uint32_t n_hd, const uint32_t *head_rows, bool refresh) {
+  oa.h_pod_idx_old = reinterpret_cast<const uint32_t *>(e->d_in + e->il.off[kHeadKeyCol]);
+  oa.n_heads_old = e->res_n_heads;
+  SnapDev sd;
+  bind_in(e->il, e->d_in, &sd);
+  ScratchDev scd = bind_scratch(e->sl, e->d_scratch);
+  const uint32_t rows = oa.first[oa.n_cols];
+  if (rows) k_inc_objects<<<(rows + 255) / 256, 256, 0, e->scopy>>>(oa, sd, scd, sizes_of(e->sizes));
+  if (n_hd) k_inc_objects_keys<<<(n_hd + 255) / 256, 256, 0, e->scopy>>>(oa.h_pod_idx_new, const_cast<uint32_t *>(sd.h_pod_idx), n_hd, head_rows);
+  if (refresh) k_inc_refresh<<<std::min<uint32_t>((uint32_t)e->sm_count * 2, (e->sizes.n_clusters + 255) / 256 + 1), 256, 0, e->scopy>>>(sd, scd);
+  CK(cudaGetLastError());
+  return KR_OK;
+}
+
+// The end of every commit on the copy stream: ev_h2d1 closes its copy time (kr_profile.h2d_ms), ev_cols (cols; else the caller
+// recorded it ahead of its JSON copy) gates stream M of the next pass, and ev_json (json) its hash, which need not wait for commits
+// that leave the JSON alone.
+int finish_commit(kr_engine *e, uint64_t bytes, bool cols, bool json) {
+  CK(cudaEventRecord(e->ev_h2d1, e->scopy));
+  if (cols) CK(cudaEventRecord(e->ev_cols, e->scopy));
+  if (json) CK(cudaEventRecord(e->ev_json, e->scopy));
+  e->h2d_timed = false;
+  e->prof.h2d_bytes = (e->h2d_accum += bytes);
+  e->committed = true;
   return KR_OK;
 }
 
@@ -1328,16 +1377,13 @@ int kr_engine_create(const kr_config *cfg, kr_engine **out) {
   if (cudaStreamCreateWithPriority(&e->sh, cudaStreamNonBlocking, prio_least) != cudaSuccess) return bail(KR_E_CUDA);
   if (cudaStreamCreateWithPriority(&e->sg, cudaStreamNonBlocking, prio_greatest) != cudaSuccess) return bail(KR_E_CUDA);
   if (cudaStreamCreateWithFlags(&e->scopy, cudaStreamNonBlocking) != cudaSuccess) return bail(KR_E_CUDA);
-  cudaEventCreate(&e->ev_h2d0); cudaEventCreate(&e->ev_h2d1); cudaEventCreateWithFlags(&e->ev_pr, cudaEventDisableTiming); cudaEventCreate(&e->ev_cols); cudaEventCreate(&e->ev_json);
-  cudaEventCreateWithFlags(&e->ev_fork2, cudaEventDisableTiming);
-  cudaEventCreateWithFlags(&e->ev_join2, cudaEventDisableTiming);
-  cudaEventCreateWithFlags(&e->ev_fork3, cudaEventDisableTiming);
-  cudaEventCreateWithFlags(&e->ev_join3, cudaEventDisableTiming);
-  cudaEventCreateWithFlags(&e->ev_fork, cudaEventDisableTiming);
-  cudaEventCreateWithFlags(&e->ev_hash, cudaEventDisableTiming);
+  cudaEventCreate(&e->ev_h2d0); cudaEventCreate(&e->ev_h2d1); cudaEventCreate(&e->ev_cols); cudaEventCreate(&e->ev_json);
+  for (cudaEvent_t *ev : {&e->pr.ev, &e->orow.ev, &e->ev_inc, &e->ev_order, &e->ev_fork2, &e->ev_join2, &e->ev_fork3, &e->ev_join3, &e->ev_fork, &e->ev_hash})
+    cudaEventCreateWithFlags(ev, cudaEventDisableTiming);
   cudaEventCreate(&e->ev_a); cudaEventCreate(&e->ev_b); cudaEventCreate(&e->ev_c);
   for (auto &ev : e->ev_k) cudaEventCreate(&ev);
   if (cudaHostAlloc((void **)&e->h_in, e->in_cap, cudaHostAllocDefault) != cudaSuccess) return bail(KR_E_CUDA);
+  if (cudaHostGetDevicePointer((void **)&e->h_in_dev, e->h_in, 0) != cudaSuccess) return bail(KR_E_CUDA);  // (mapped under UVA)
   if (cudaHostAlloc((void **)&e->h_out, e->out_cap, cudaHostAllocDefault) != cudaSuccess) return bail(KR_E_CUDA);
   if (cudaMalloc((void **)&e->d_in, e->in_cap) != cudaSuccess) return bail(KR_E_CUDA);
   if (cudaMalloc((void **)&e->d_scratch, e->scratch_cap) != cudaSuccess) return bail(KR_E_CUDA);
@@ -1386,21 +1432,14 @@ int kr_engine_create(const kr_config *cfg, kr_engine **out) {
     const size_t objs = capl.off[kFirstPodCol] + (capl.off[kNumCols - 1] - capl.off[kFirstPodCol + 7]);
     if (cudaMalloc((void **)&e->d_obj_stage, objs) != cudaSuccess) return bail(KR_E_CUDA);
     e->obj_stage_cap = objs;
-    const uint32_t capc = std::max<uint32_t>(64, cfg->max_clusters / 4), capg = (uint32_t)std::min<uint64_t>((uint64_t)capc * KR_SMEM_GROUPS, (uint64_t)cfg->max_groups + 1);
-    size_t dig_off;
-    const size_t need = inc_stage_bytes(capc, capg, &dig_off);
-    if (cudaMalloc((void **)&e->d_inc_stage, need) != cudaSuccess) return bail(KR_E_CUDA);
-    if (cudaHostAlloc((void **)&e->h_inc_stage, need, cudaHostAllocDefault) != cudaSuccess) return bail(KR_E_CUDA);
-    e->inc_stage_cap = need;
+    if (e->inc_stage.reserve(inc_stage_layout(cfg->max_clusters, cfg->max_groups).total, 0) != cudaSuccess) return bail(KR_E_CUDA);
     const size_t chg = std::max<size_t>(1024, (size_t)cfg->max_clusters);
     if (cudaHostAlloc((void **)&e->h_changed, 4 * chg, cudaHostAllocDefault) != cudaSuccess) return bail(KR_E_CUDA);
     e->h_changed_cap = chg;
   }
   if (cudaHostAlloc((void **)&e->h_order, 4 * ((size_t)cfg->max_clusters + 1), cudaHostAllocDefault) != cudaSuccess) return bail(KR_E_CUDA);
   if (cudaMalloc((void **)&e->d_order, 4 * ((size_t)cfg->max_clusters + 1)) != cudaSuccess) return bail(KR_E_CUDA);
-  if (cudaHostAlloc((void **)&e->h_spec, 20 * ((size_t)cfg->max_clusters + 1), cudaHostAllocDefault) != cudaSuccess) return bail(KR_E_CUDA);
-  if (cudaMalloc((void **)&e->d_spec, 20 * ((size_t)cfg->max_clusters + 1)) != cudaSuccess) return bail(KR_E_CUDA);
-  cudaEventCreateWithFlags(&e->ev_order, cudaEventDisableTiming);
+  if (e->spec.reserve(20 * ((size_t)cfg->max_clusters + 1), 0) != cudaSuccess) return bail(KR_E_CUDA);
   cudaFuncSetAttribute(k_hash3<1, 0>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)sizeof(H3Smem));
   *out = e;
   return KR_OK;
@@ -1413,30 +1452,19 @@ void kr_engine_destroy(kr_engine *e) {
   if (e->sh) cudaStreamSynchronize(e->sh);
   if (e->h_in) cudaFreeHost(e->h_in);
   if (e->h_out) cudaFreeHost(e->h_out);
-  if (e->hb_h) cudaFreeHost(e->hb_h);
+  e->hb.release(); e->pr.release(); e->orow.release(); e->inc_stage.release(); e->spec.release();
   if (e->h_totals) cudaFreeHost(e->h_totals);
   if (e->h_order) cudaFreeHost(e->h_order);
   if (e->h_inc) cudaFreeHost(e->h_inc);
-  if (e->orow_h) cudaFreeHost(e->orow_h);
-  if (e->orow_d) cudaFree(e->orow_d);
-  if (e->ev_orow) cudaEventDestroy(e->ev_orow);
   if (e->h_changed) cudaFreeHost(e->h_changed);
-  if (e->h_inc_stage) cudaFreeHost(e->h_inc_stage);
-  if (e->d_inc_stage) cudaFree(e->d_inc_stage);
   if (e->d_obj_stage) cudaFree(e->d_obj_stage);
   if (e->d_lg) cudaFree(e->d_lg);
   if (e->d_region) cudaFree(e->d_region);
   if (e->d_huge) cudaFree(e->d_huge);
   if (e->d_order) cudaFree(e->d_order);
-  if (e->h_spec) cudaFreeHost(e->h_spec);
-  if (e->d_spec) cudaFree(e->d_spec);
-  if (e->ev_order) cudaEventDestroy(e->ev_order);
   if (e->d_in) cudaFree(e->d_in);
   if (e->d_scratch) cudaFree(e->d_scratch);
   if (e->d_out) cudaFree(e->d_out);
-  if (e->hb_d) cudaFree(e->hb_d);
-  if (e->pr_h) cudaFreeHost(e->pr_h);
-  if (e->pr_d) cudaFree(e->pr_d);
   if (e->gexec) cudaGraphExecDestroy(e->gexec);
   for (auto ev : {e->ev_fork, e->ev_hash, e->ev_a, e->ev_b, e->ev_c}) if (ev) cudaEventDestroy(ev);
   for (auto ev : e->ev_k) if (ev) cudaEventDestroy(ev);
@@ -1444,12 +1472,7 @@ void kr_engine_destroy(kr_engine *e) {
   if (e->sh) cudaStreamDestroy(e->sh);
   if (e->sg) cudaStreamDestroy(e->sg);
   if (e->scopy) { cudaStreamSynchronize(e->scopy); cudaStreamDestroy(e->scopy); }
-  for (auto ev : {e->ev_h2d0, e->ev_h2d1, e->ev_cols, e->ev_json, e->ev_pr}) if (ev) cudaEventDestroy(ev);
-  if (e->ev_inc) cudaEventDestroy(e->ev_inc);
-  if (e->ev_fork2) cudaEventDestroy(e->ev_fork2);
-  if (e->ev_join2) cudaEventDestroy(e->ev_join2);
-  if (e->ev_fork3) cudaEventDestroy(e->ev_fork3);
-  if (e->ev_join3) cudaEventDestroy(e->ev_join3);
+  for (auto ev : {e->ev_h2d0, e->ev_h2d1, e->ev_cols, e->ev_json, e->ev_inc, e->ev_order, e->ev_fork2, e->ev_join2, e->ev_fork3, e->ev_join3}) if (ev) cudaEventDestroy(ev);
   delete e;
 }
 
@@ -1566,12 +1589,8 @@ int kr_snapshot_commit_parts(kr_engine *e, uint32_t parts) {
   // While the incremental state is resident, an object commit lands beside the resident tables and is diffed against them on
   // the device (k_inc_objects): changed rows mark their RayCluster dirty, a changed key makes the next pass a full one.
   const bool stage_objects = e->inc_valid && !e->no_incr && (parts & KR_PART_OBJECTS) && !(parts & KR_PART_COLUMNS);
-  if (stage_objects && a1 + (json_off - b0) > e->obj_stage_cap) {
-    if (e->d_obj_stage) cudaFree(e->d_obj_stage);
-    e->d_obj_stage = nullptr; e->obj_stage_cap = 0;
-    CK(cudaMalloc((void **)&e->d_obj_stage, a1 + (json_off - b0)));
-    e->obj_stage_cap = a1 + (json_off - b0);
-  }
+  if (stage_objects && a1 + (json_off - b0) > e->obj_stage_cap)
+    return fail(e, KR_E_STATE, "internal: object part of %zu bytes, staging room for %zu", a1 + (json_off - b0), e->obj_stage_cap);
   auto stage_of = [&](size_t off) { return off < a1 ? off : a1 + (off - b0); };
   auto up = [&](size_t off, size_t len) -> int {
     if (!len) return KR_OK;
@@ -1610,17 +1629,7 @@ int kr_snapshot_commit_parts(kr_engine *e, uint32_t parts) {
     oa.first[nc] = first; oa.n_cols = nc;
     oa.g_cluster_idx_new = reinterpret_cast<const uint32_t *>(e->d_obj_stage + stage_of(e->il.off[kGroupClusterCol]));
     oa.h_pod_idx_new = reinterpret_cast<const uint32_t *>(e->d_obj_stage + stage_of(e->il.off[kHeadKeyCol]));
-    oa.h_pod_idx_old = reinterpret_cast<const uint32_t *>(e->d_in + e->il.off[kHeadKeyCol]);
-    oa.n_heads_old = e->res_n_heads;
-    SnapDev sd;
-    bind_in(e->il, e->d_in, &sd);
-    ScratchDev scd = bind_scratch(e->sl, e->d_scratch);
-    Sizes zz{n.n_clusters, n.n_groups, n.n_wtd, n.n_pods, n.n_heads, n.n_jobs};
-    if (first) k_inc_objects<<<(first + 255) / 256, 256, 0, e->scopy>>>(oa, sd, scd, zz);
-    if (n.n_heads) k_inc_objects_keys<<<(n.n_heads + 255) / 256, 256, 0, e->scopy>>>(oa.h_pod_idx_new, const_cast<uint32_t *>(sd.h_pod_idx), n.n_heads, nullptr);
-    // the input records (cl_in) of the RayClusters the diff found changed, now that every column of theirs is in place
-    if (n.n_clusters) k_inc_refresh<<<std::min<uint32_t>((uint32_t)e->sm_count * 2, (n.n_clusters + 255) / 256 + 1), 256, 0, e->scopy>>>(sd, scd);
-    CK(cudaGetLastError());
+    if (int rc = launch_object_diff(e, oa, n.n_heads, nullptr, n.n_clusters != 0)) return rc;
   }
   if (parts & (KR_PART_COLUMNS | KR_PART_OBJECTS)) {
     e->recreate_bit.resize(n.n_clusters);
@@ -1653,13 +1662,8 @@ int kr_snapshot_commit_parts(kr_engine *e, uint32_t parts) {
     }
   }
   if (parts & KR_PART_JSON) { if (int rc = up(json_off, e->fixed_layout ? (size_t)n.json_bytes : e->il.total - json_off)) return rc; }
-  CK(cudaEventRecord(e->ev_json, e->scopy));
-  CK(cudaEventRecord(e->ev_h2d1, e->scopy));
   if ((parts & KR_PART_ALL) == KR_PART_ALL) e->committed_full = true;
-  e->h2d_timed = false;
-  e->prof.h2d_bytes = (e->h2d_accum += bytes);
-  e->committed = true;
-  return KR_OK;
+  return finish_commit(e, bytes, false, true);
 }
 
 // Shared by the two incremental pod commits: stage the row list (and, journal style, the 7 values per row), upload, scatter.
@@ -1669,16 +1673,8 @@ static int commit_pod_patch(kr_engine *e, const uint32_t *rows, const uint32_t *
   if (n == 0) return KR_OK;
   CK(cudaSetDevice(e->cfg.device));
   const size_t bytes = (values ? 32 : 4) * (size_t)n;  // row list (+ 7 values per row); kr_snapshot_commit_pod_rows lets the device pull the rows
-  if (e->pr_busy) { CK(cudaEventSynchronize(e->ev_pr)); e->pr_busy = false; }  // a previous patch may still be reading the staging buffer
-  if (bytes > e->pr_cap) {
-    if (e->pr_h) cudaFreeHost(e->pr_h);
-    if (e->pr_d) cudaFree(e->pr_d);
-    e->pr_h = nullptr; e->pr_d = nullptr; e->pr_cap = 0;
-    size_t cap = bytes + bytes / 2 + 4096;
-    CK(cudaHostAlloc((void **)&e->pr_h, cap, cudaHostAllocDefault));
-    CK(cudaMalloc((void **)&e->pr_d, cap));
-    e->pr_cap = cap;
-  }
+  CK(e->pr.wait());  // a previous patch may still be reading the staging buffer
+  CK(e->pr.reserve(bytes, bytes / 2 + 4096));
   for (uint32_t i = 0; i < n; i++)
     if (rows[i] >= e->sizes.n_pods) return fail(e, KR_E_INVALID, "pod row %u out of range", rows[i]);
   if (values && !rows_known_distinct) {  // the scatter kernel writes one thread per entry: two entries for one row would race
@@ -1689,8 +1685,8 @@ static int commit_pod_patch(kr_engine *e, const uint32_t *rows, const uint32_t *
       e->row_stamp[rows[i]] = e->row_epoch;
     }
   }
-  memcpy(e->pr_h, rows, 4 * (size_t)n);
-  if (values) memcpy(e->pr_h + 4 * (size_t)n, values, 28 * (size_t)n);
+  memcpy(e->pr.h, rows, 4 * (size_t)n);
+  if (values) memcpy(e->pr.h + 4 * (size_t)n, values, 28 * (size_t)n);
   kr_snapshot_bufs hb;
   bind_in(e->il, e->h_in, &hb);
   SnapDev s;
@@ -1698,31 +1694,26 @@ static int commit_pod_patch(kr_engine *e, const uint32_t *rows, const uint32_t *
   PodCols hc, dc;
   const void *hsrc[7] = {hb.p_ns_id, hb.p_cluster_name_id, hb.p_group_name_id, hb.p_name_id, hb.p_packed, hb.p_replica_index, hb.p_replica_name_id};
   const void *dsrc[7] = {s.p_ns_id, s.p_cluster_name_id, s.p_group_name_id, s.p_name_id, s.p_packed, s.p_replica_index, s.p_replica_name_id};
-  if (!e->h_in_dev) CK(cudaHostGetDevicePointer((void **)&e->h_in_dev, e->h_in, 0));  // device-side address of the pinned arena (mapped under UVA)
   for (int k = 0; k < 7; k++) {
     hc.c[k] = reinterpret_cast<uint32_t *>(e->h_in_dev + (static_cast<const uint8_t *>(hsrc[k]) - e->h_in));
     dc.c[k] = static_cast<uint32_t *>(const_cast<void *>(dsrc[k]));
   }
   CK(cudaStreamSynchronize(e->sm));  // a pass still reading the columns must finish first
   CK(cudaEventRecord(e->ev_h2d0, e->scopy));
-  CK(cudaMemcpyAsync(e->pr_d, e->pr_h, bytes, cudaMemcpyHostToDevice, e->scopy));
-  CK(cudaEventRecord(e->ev_pr, e->scopy));
-  e->pr_busy = true;
+  CK(cudaMemcpyAsync(e->pr.d, e->pr.h, bytes, cudaMemcpyHostToDevice, e->scopy));
+  CK(cudaEventRecord(e->pr.ev, e->scopy));
+  e->pr.busy = true;
+  const uint32_t *drows = reinterpret_cast<const uint32_t *>(e->pr.d);
   if (e->inc_valid && !e->no_incr) {  // the rows' previous values leave the resident state before the new ones land
     ScratchDev scd = bind_scratch(e->sl, e->d_scratch);
     ResDev rd = bind_out(e->ol, e->d_out);
-    Sizes zz{e->sizes.n_clusters, e->sizes.n_groups, e->sizes.n_wtd, e->sizes.n_pods, e->sizes.n_heads, e->sizes.n_jobs};
-    k_inc_retire<<<(n + 255) / 256, 256, 0, e->scopy>>>(reinterpret_cast<const uint32_t *>(e->pr_d), n, s, scd, rd, zz, e->inc_n_pods, e->sizes.n_wtd ? 1 : 0);
+    k_inc_retire<<<(n + 255) / 256, 256, 0, e->scopy>>>(drows, n, s, scd, rd, sizes_of(e->sizes), e->inc_n_pods, e->sizes.n_wtd ? 1 : 0);
   }
-  if (values) k_patch_pod_values<<<(n + 255) / 256, 256, 0, e->scopy>>>(reinterpret_cast<const uint32_t *>(e->pr_d), n, dc);
-  else k_patch_pods<<<(n + 255) / 256, 256, 0, e->scopy>>>(reinterpret_cast<const uint32_t *>(e->pr_d), n, hc, dc);
+  if (values) k_patch_pod_values<<<(n + 255) / 256, 256, 0, e->scopy>>>(drows, n, dc);
+  else k_patch_pods<<<(n + 255) / 256, 256, 0, e->scopy>>>(drows, n, hc, dc);
   CK(cudaGetLastError());
-  CK(cudaEventRecord(e->ev_h2d1, e->scopy));
-  CK(cudaEventRecord(e->ev_cols, e->scopy));  // ev_json keeps pointing at the last JSON upload: the hash need not wait for the patch
-  e->h2d_timed = false;
-  e->prof.h2d_bytes = (e->h2d_accum += 32 * (size_t)n);  // row list + the 28-byte row payload (pulled one 32-byte sector per value in the rows-only variant)
-  e->committed = true;
-  return KR_OK;
+  // row list + the 28-byte row payload (pulled one 32-byte sector per value in the rows-only variant); the JSON is untouched
+  return finish_commit(e, 32 * (uint64_t)n, true, false);
 }
 
 
@@ -1779,18 +1770,9 @@ int kr_snapshot_commit_object_rows(kr_engine *e, const uint32_t *cluster_rows, u
     if (d == D_PODS || !cnt[d]) continue;
     col_off[i] = need; need = align_up(need + (size_t)kCols[i].elem * kCols[i].mult * cnt[d]);
   }
-  if (e->orow_busy) { CK(cudaEventSynchronize(e->ev_orow)); e->orow_busy = false; }
-  if (need > e->orow_cap) {
-    if (e->orow_h) cudaFreeHost(e->orow_h);
-    if (e->orow_d) cudaFree(e->orow_d);
-    e->orow_h = nullptr; e->orow_d = nullptr; e->orow_cap = 0;
-    const size_t cap = need + need / 2 + 65536;
-    CK(cudaHostAlloc((void **)&e->orow_h, cap, cudaHostAllocDefault));
-    CK(cudaMalloc((void **)&e->orow_d, cap));
-    e->orow_cap = cap;
-  }
-  if (!e->ev_orow) CK(cudaEventCreateWithFlags(&e->ev_orow, cudaEventDisableTiming));
-  for (int d = 0; d < 7; d++) if (cnt[d]) memcpy(e->orow_h + list_off[d], lists[d], 4 * (size_t)cnt[d]);
+  CK(e->orow.wait());
+  CK(e->orow.reserve(need, need / 2 + 65536));
+  for (int d = 0; d < 7; d++) if (cnt[d]) memcpy(e->orow.h + list_off[d], lists[d], 4 * (size_t)cnt[d]);
   ObjDiffArgs oa{};
   int nc = 0;
   uint32_t first = 0;
@@ -1799,50 +1781,36 @@ int kr_snapshot_commit_object_rows(kr_engine *e, const uint32_t *cluster_rows, u
     if (d == D_PODS || !cnt[d]) continue;
     const size_t rb = (size_t)kCols[i].elem * kCols[i].mult;
     const uint8_t *col = e->h_in + e->il.off[i];
-    uint8_t *dst = e->orow_h + col_off[i];
+    uint8_t *dst = e->orow.h + col_off[i];
     // (row sizes are 1, 4 or 8 bytes for almost every column: fixed-size copies instead of ~10 k variable-length memcpy calls per epoch)
     const uint32_t *rl = lists[d];
     if (rb == 4) { const uint32_t *c4 = reinterpret_cast<const uint32_t *>(col); uint32_t *d4 = reinterpret_cast<uint32_t *>(dst); for (uint32_t k = 0; k < cnt[d]; k++) d4[k] = c4[rl[k]]; }
     else if (rb == 1) { for (uint32_t k = 0; k < cnt[d]; k++) dst[k] = col[rl[k]]; }
     else if (rb == 8) { const uint64_t *c8 = reinterpret_cast<const uint64_t *>(col); uint64_t *d8 = reinterpret_cast<uint64_t *>(dst); for (uint32_t k = 0; k < cnt[d]; k++) d8[k] = c8[rl[k]]; }
     else for (uint32_t k = 0; k < cnt[d]; k++) memcpy(dst + k * rb, col + (size_t)rl[k] * rb, rb);
-    oa.src[nc] = e->orow_d + col_off[i];
-    oa.rowlist[nc] = reinterpret_cast<const uint32_t *>(e->orow_d + list_off[d]);
+    oa.src[nc] = e->orow.d + col_off[i];
+    oa.rowlist[nc] = reinterpret_cast<const uint32_t *>(e->orow.d + list_off[d]);
     oa.dst[nc] = e->d_in + e->il.off[i];
     oa.first[nc] = first;
     oa.rows_old[nc] = d == D_HEADS ? e->res_n_heads : (d == D_CLUSTERS ? n.n_clusters : n.n_groups);
     oa.row_bytes[nc] = (uint16_t)rb;
     oa.cls[nc] = kObjClass[i];
-    if (i == kGroupClusterCol) oa.g_cluster_idx_new = reinterpret_cast<const uint32_t *>(e->orow_d + col_off[i]);
-    if (i == kHeadKeyCol) oa.h_pod_idx_new = reinterpret_cast<const uint32_t *>(e->orow_d + col_off[i]);
+    if (i == kGroupClusterCol) oa.g_cluster_idx_new = reinterpret_cast<const uint32_t *>(e->orow.d + col_off[i]);
+    if (i == kHeadKeyCol) oa.h_pod_idx_new = reinterpret_cast<const uint32_t *>(e->orow.d + col_off[i]);
     first += cnt[d];
     nc++;
   }
   oa.first[nc] = first; oa.n_cols = nc;
-  oa.h_pod_idx_old = reinterpret_cast<const uint32_t *>(e->d_in + e->il.off[kHeadKeyCol]);
-  oa.n_heads_old = e->res_n_heads;
   // the pod -> head-aux row table follows the keys (compared here, on the host shadow)
   for (uint32_t i = 0; i < n_hd; i++)
     if (e->prev_h_pod_idx[head_rows[i]] != hb.h_pod_idx[head_rows[i]]) { e->heads_rebuild = true; e->prev_h_pod_idx[head_rows[i]] = hb.h_pod_idx[head_rows[i]]; }
   CK(cudaStreamSynchronize(e->sm));  // a pass still reading the tables must finish first
   CK(cudaEventRecord(e->ev_h2d0, e->scopy));
-  CK(cudaMemcpyAsync(e->orow_d, e->orow_h, need, cudaMemcpyHostToDevice, e->scopy));
-  CK(cudaEventRecord(e->ev_orow, e->scopy));
-  e->orow_busy = true;
-  SnapDev sd;
-  bind_in(e->il, e->d_in, &sd);
-  ScratchDev scd = bind_scratch(e->sl, e->d_scratch);
-  Sizes zz{n.n_clusters, n.n_groups, n.n_wtd, n.n_pods, n.n_heads, n.n_jobs};
-  if (first) k_inc_objects<<<(first + 255) / 256, 256, 0, e->scopy>>>(oa, sd, scd, zz);
-  if (n_hd) k_inc_objects_keys<<<(n_hd + 255) / 256, 256, 0, e->scopy>>>(oa.h_pod_idx_new, const_cast<uint32_t *>(sd.h_pod_idx), n_hd, reinterpret_cast<const uint32_t *>(e->orow_d + list_off[D_HEADS]));
-  if (n_cl) k_inc_refresh<<<std::min<uint32_t>((uint32_t)e->sm_count * 2, (n.n_clusters + 255) / 256 + 1), 256, 0, e->scopy>>>(sd, scd);  // (see kr_snapshot_commit_parts)
-  CK(cudaGetLastError());
-  CK(cudaEventRecord(e->ev_h2d1, e->scopy));
-  CK(cudaEventRecord(e->ev_cols, e->scopy));
-  e->h2d_timed = false;
-  e->prof.h2d_bytes = (e->h2d_accum += need);
-  e->committed = true;
-  return KR_OK;
+  CK(cudaMemcpyAsync(e->orow.d, e->orow.h, need, cudaMemcpyHostToDevice, e->scopy));
+  CK(cudaEventRecord(e->orow.ev, e->scopy));
+  e->orow.busy = true;
+  if (int rc = launch_object_diff(e, oa, n_hd, reinterpret_cast<const uint32_t *>(e->orow.d + list_off[D_HEADS]), n_cl != 0)) return rc;
+  return finish_commit(e, need, true, false);
 }
 
 int kr_snapshot_commit_spec_rows(kr_engine *e, const uint32_t *rows, uint32_t n) {
@@ -1865,9 +1833,9 @@ int kr_snapshot_commit_spec_rows(kr_engine *e, const uint32_t *rows, uint32_t n)
   // the rows this call pulls, appended to the pull list: a row pulled since the last pass is in the device arena already (the caller
   // may not rewrite the arenas before the next pass returns); a row listed before that pass, still pending, is pulled again
   const size_t cap = (size_t)e->cfg.max_clusters + 1, base = e->n_pull;
-  uint32_t *lr = reinterpret_cast<uint32_t *>(e->h_spec) + base;
-  uint32_t *ll = reinterpret_cast<uint32_t *>(e->h_spec + 4 * cap) + base;
-  uint64_t *lo = reinterpret_cast<uint64_t *>(e->h_spec + 8 * cap) + base;
+  uint32_t *lr = reinterpret_cast<uint32_t *>(e->spec.h) + base;
+  uint32_t *ll = reinterpret_cast<uint32_t *>(e->spec.h + 4 * cap) + base;
+  uint64_t *lo = reinterpret_cast<uint64_t *>(e->spec.h + 8 * cap) + base;
   uint32_t m = 0;
   for (uint32_t i = 0; i < n; i++) {
     const uint32_t c = rows[i];
@@ -1888,12 +1856,11 @@ int kr_snapshot_commit_spec_rows(kr_engine *e, const uint32_t *rows, uint32_t n)
     if ((e->prev_json_len[c] + 8) / 64 != (ll[i] + 8) / 64) e->spec_order_stale = true;
     e->prev_json_off[c] = lo[i]; e->prev_json_len[c] = ll[i];
   }
-  if (!e->h_in_dev) CK(cudaHostGetDevicePointer((void **)&e->h_in_dev, e->h_in, 0));
   CK(cudaStreamSynchronize(e->sm));  // a pass still reading the arena must finish first
   CK(cudaEventRecord(e->ev_h2d0, e->scopy));
-  uint32_t *dr = reinterpret_cast<uint32_t *>(e->d_spec) + base;
-  uint32_t *dl = reinterpret_cast<uint32_t *>(e->d_spec + 4 * cap) + base;
-  uint64_t *dof = reinterpret_cast<uint64_t *>(e->d_spec + 8 * cap) + base;
+  uint32_t *dr = reinterpret_cast<uint32_t *>(e->spec.d) + base;
+  uint32_t *dl = reinterpret_cast<uint32_t *>(e->spec.d + 4 * cap) + base;
+  uint64_t *dof = reinterpret_cast<uint64_t *>(e->spec.d + 8 * cap) + base;
   CK(cudaMemcpyAsync(dr, lr, 4 * (size_t)m, cudaMemcpyHostToDevice, e->scopy));
   CK(cudaMemcpyAsync(dl, ll, 4 * (size_t)m, cudaMemcpyHostToDevice, e->scopy));
   CK(cudaMemcpyAsync(dof, lo, 8 * (size_t)m, cudaMemcpyHostToDevice, e->scopy));
@@ -1901,14 +1868,8 @@ int kr_snapshot_commit_spec_rows(kr_engine *e, const uint32_t *rows, uint32_t n)
   k_spec_pull<<<m, 128, 0, e->scopy>>>(dr, dof, dl, e->h_in_dev + json_off, e->d_in + json_off, reinterpret_cast<uint64_t *>(e->d_in + e->il.off[kJsonOffCol]),
                                        reinterpret_cast<uint32_t *>(e->d_in + e->il.off[kJsonOffCol + 1]));
   CK(cudaGetLastError());
-  CK(cudaEventRecord(e->ev_h2d1, e->scopy));
-  CK(cudaEventRecord(e->ev_cols, e->scopy));
-  CK(cudaEventRecord(e->ev_json, e->scopy));
   e->n_pull += m;
-  e->h2d_timed = false;
-  e->prof.h2d_bytes = (e->h2d_accum += bytes);
-  e->committed = true;
-  return KR_OK;
+  return finish_commit(e, bytes, true, true);  // (k_spec_pull wrote the columns' ranges as well as the JSON)
 }
 
 int kr_snapshot_commit_pod_rows(kr_engine *e, const uint32_t *rows, uint32_t n) { return commit_pod_patch(e, rows, nullptr, n); }
@@ -1926,31 +1887,16 @@ int kr_snapshot_commit_pod_values(kr_engine *e, const uint32_t *rows, const uint
 
 int kr_reconcile_device_only(kr_engine *e, const kr_flags *flags) {
   if (!e || !flags) return KR_E_INVALID;
-  if (!e->committed) return fail(e, KR_E_STATE, "no committed snapshot");
-  CK(cudaSetDevice(e->cfg.device));
-  CK(cudaEventRecord(e->ev_a, e->sm));
-  int rc = run_pass(e, *flags, e->ev_b);
-  if (rc) return rc;
-  float ms = 0;
-  if (cudaEventElapsedTime(&ms, e->ev_a, e->ev_b) == cudaSuccess) e->prof.kernels_ms = ms;
-  e->ran = true;
-  return KR_OK;
+  return run_pass(e, *flags, e->ev_b, false);
 }
 
 int kr_reconcile_batch(kr_engine *e, const kr_flags *flags, kr_results_view *out) {
   if (!e || !flags || !out) return KR_E_INVALID;
-  if (!e->committed) return fail(e, KR_E_STATE, "no committed snapshot");
-  CK(cudaSetDevice(e->cfg.device));
   static const bool trace = getenv("KR_ENGINE_TRACE") != nullptr;  // development aid: host time of the two halves of a call (stderr)
   const auto t0 = std::chrono::steady_clock::now();
-  CK(cudaEventRecord(e->ev_a, e->sm));
-  int rc = run_pass(e, *flags, e->ev_k[KR_MAX_KERNEL_TIMES]);
-  if (rc) return rc;
-  e->ran = true;
-  float ms = 0;
-  if (cudaEventElapsedTime(&ms, e->ev_a, e->ev_k[KR_MAX_KERNEL_TIMES]) == cudaSuccess) e->prof.kernels_ms = ms;
+  if (int rc = run_pass(e, *flags, e->ev_k[KR_MAX_KERNEL_TIMES], false)) return rc;
   const auto t1 = std::chrono::steady_clock::now();
-  rc = fetch_results(e, out);  // d2h_ms = ev_b..ev_c
+  const int rc = fetch_results(e, out);  // d2h_ms = ev_b..ev_c
   if (trace) {
     const auto t2 = std::chrono::steady_clock::now();
     auto us = [](auto a, auto b) { return std::chrono::duration<double, std::micro>(b - a).count(); };
@@ -1962,49 +1908,13 @@ int kr_reconcile_batch(kr_engine *e, const kr_flags *flags, kr_results_view *out
 
 int kr_reconcile_batch_profiled(kr_engine *e, const kr_flags *flags, kr_profile *prof) {
   if (!e || !flags) return KR_E_INVALID;
-  if (!e->committed) return fail(e, KR_E_STATE, "no committed snapshot");
-  CK(cudaSetDevice(e->cfg.device));
-  e->last_flags = *flags;
-  new_pull_epoch(e);
-  if (e->lg_stale) if (int rc = upload_lg(e)) return rc;
-  bool inc_done = false;
-  if (e->inc_valid && !e->no_incr && memcmp(&e->inc_flags, flags, sizeof *flags) == 0) {
-    CK(cudaEventRecord(e->ev_a, e->sm));
-    if (int rc = run_pass_inc(e, *flags, e->ev_b, true, &inc_done)) return rc;
-    if (inc_done) { e->inc_n_pods = e->sizes.n_pods; e->inc_n_heads = e->sizes.n_heads; }
-  }
-  if (!inc_done) {
-    e->inc_valid = false; e->ran_inc = false;
-    if (e->inc_zero_needed) {
-      CK(cudaMemsetAsync(e->d_scratch + e->sl.inc_zero, 0, e->sl.inc_zero_end - e->sl.inc_zero, e->sm));
-      e->inc_zero_needed = false;
-    }
-    if (e->spec_order_stale && !flags->skip_hash) if (int rc = refresh_order(e)) return rc;
-  }
-  for (int attempt = 0; !inc_done; attempt++) {  // same fallback ladder as run_pass
-    CK(cudaEventRecord(e->ev_a, e->sm));
-    int rc = launch_pass(e, *flags, true);
-    if (rc) return rc;
-    CK(cudaEventRecord(e->ev_b, e->sm));
-    CK(cudaMemcpyAsync(e->h_totals, e->d_out + e->ol.totals, 48, cudaMemcpyDeviceToHost, e->sm));
-    CK(cudaStreamSynchronize(e->sm));
-    e->order_pending = false;
-    if (!(e->h_totals[3] & KR_TOTALS_BIG_BUCKET)) { after_full_pass(e, *flags); break; }
-    if (attempt >= 4) return fail(e, KR_E_STATE, "internal: radix pipeline flagged a big bucket");
-    if (e->ran_bucket) {
-      if (int rc = after_bucket_void(e)) return rc;
-    } else if (e->ran_fast) e->force_radix = true;
-    e->gvalid = false;
-  }
-  float ms = 0;
-  if (cudaEventElapsedTime(&ms, e->ev_a, e->ev_b) == cudaSuccess) e->prof.kernels_ms = ms;
+  if (int rc = run_pass(e, *flags, e->ev_b, true)) return rc;
   uint32_t k = e->prof.n_kernels < KR_MAX_KERNEL_TIMES ? e->prof.n_kernels : KR_MAX_KERNEL_TIMES;
   for (uint32_t i = 0; i < k; i++) {
     float t = 0;
     cudaEventElapsedTime(&t, e->ev_k[i], e->ev_k[i + 1]);
     e->prof.kernel_ms[i] = t;
   }
-  e->ran = true;
   if (prof) *prof = e->prof;
   return KR_OK;
 }
@@ -2028,22 +1938,14 @@ static int hash_pieces(kr_engine *e, const uint8_t *const *ptr, const uint64_t *
     data += align_up(len[i], 16);
   }
   size_t o_off = 0, o_len = align_up(8 * (size_t)n), o_ord = align_up(o_len + 4 * (size_t)n), o_data = align_up(o_ord + 4 * (size_t)n), o_out = align_up(o_data + data + 16), total = o_out + 32 * (size_t)n;
-  if (total > e->hb_cap) {
-    if (e->hb_h) cudaFreeHost(e->hb_h);
-    if (e->hb_d) cudaFree(e->hb_d);
-    e->hb_h = nullptr; e->hb_d = nullptr; e->hb_cap = 0;
-    size_t cap = total + total / 4;
-    CK(cudaHostAlloc((void **)&e->hb_h, cap, cudaHostAllocDefault));
-    CK(cudaMalloc((void **)&e->hb_d, cap));
-    e->hb_cap = cap;
-  }
-  uint64_t *so = reinterpret_cast<uint64_t *>(e->hb_h + o_off);
-  uint32_t *sl = reinterpret_cast<uint32_t *>(e->hb_h + o_len);
+  CK(e->hb.reserve(total, total / 4));
+  uint64_t *so = reinterpret_cast<uint64_t *>(e->hb.h + o_off);
+  uint32_t *sl = reinterpret_cast<uint32_t *>(e->hb.h + o_len);
   size_t cur = 0;
   for (uint32_t i = 0; i < n; i++) { so[i] = cur; sl[i] = (uint32_t)len[i]; cur += align_up(len[i], 16); }
   auto fill = [&](uint32_t lo, uint32_t hi) {
     for (uint32_t i = lo; i < hi; i++) {
-      uint8_t *dst = e->hb_h + o_data + so[i];
+      uint8_t *dst = e->hb.h + o_data + so[i];
       if (len[i]) memcpy(dst, ptr[i], len[i]);
       const size_t pad = align_up(len[i], 16) - len[i];
       if (pad) memset(dst + len[i], 0, pad);
@@ -2058,22 +1960,19 @@ static int hash_pieces(kr_engine *e, const uint8_t *const *ptr, const uint64_t *
     for (auto &th : pool) th.join();
   }
   // message ids by descending block count, staged behind the lengths
-  uint32_t *ord = reinterpret_cast<uint32_t *>(e->hb_h + o_ord);
+  uint32_t *ord = reinterpret_cast<uint32_t *>(e->hb.h + o_ord);
   for (uint32_t i = 0; i < n; i++) ord[i] = i;
   std::stable_sort(ord, ord + n, [&](uint32_t a, uint32_t b) { return (sl[a] + 8) / 64 > (sl[b] + 8) / 64; });
-  CK(cudaMemcpyAsync(e->hb_d, e->hb_h, o_data + data, cudaMemcpyHostToDevice, e->sh));
-  const uint8_t *db = e->hb_d + o_data;
-  const uint64_t *doff = reinterpret_cast<const uint64_t *>(e->hb_d + o_off);
-  const uint32_t *dlen = reinterpret_cast<const uint32_t *>(e->hb_d + o_len);
-  const uint32_t *dord = reinterpret_cast<const uint32_t *>(e->hb_d + o_ord);
-  char *dout = reinterpret_cast<char *>(e->hb_d + o_out);
-  const uint32_t ngroups = (n + 31) / 32;
-  if (ngroups <= (uint32_t)e->sm_count * 4) k_hash3<1, 0><<<std::min<uint32_t>(ngroups, (uint32_t)e->sm_count * 2), 64, sizeof(H3Smem), e->sh>>>(db, doff, dlen, dord, n, dout);
-  else k_hash2<4, 1><<<std::min<uint32_t>((n + 127) / 128, (uint32_t)e->sm_count * 4), 128, 0, e->sh>>>(db, doff, dlen, dord, n, dout, 1u);
+  CK(cudaMemcpyAsync(e->hb.d, e->hb.h, o_data + data, cudaMemcpyHostToDevice, e->sh));
+  const uint64_t *doff = reinterpret_cast<const uint64_t *>(e->hb.d + o_off);
+  const uint32_t *dlen = reinterpret_cast<const uint32_t *>(e->hb.d + o_len);
+  const uint32_t *dord = reinterpret_cast<const uint32_t *>(e->hb.d + o_ord);
+  char *dout = reinterpret_cast<char *>(e->hb.d + o_out);
+  launch_hash(e, e->sh, e->hb.d + o_data, doff, dlen, dord, n, dout, 4);  // (a batch takes up to sm_count * 4 CTAs of k_hash2, a pass hash_ctas_per_sm per SM)
   CK(cudaGetLastError());
-  CK(cudaMemcpyAsync(e->hb_h + o_out, dout, 32 * (size_t)n, cudaMemcpyDeviceToHost, e->sh));
+  CK(cudaMemcpyAsync(e->hb.h + o_out, dout, 32 * (size_t)n, cudaMemcpyDeviceToHost, e->sh));
   CK(cudaStreamSynchronize(e->sh));
-  memcpy(out32xN, e->hb_h + o_out, 32 * (size_t)n);
+  memcpy(out32xN, e->hb.h + o_out, 32 * (size_t)n);
   return KR_OK;
 }
 

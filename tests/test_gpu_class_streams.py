@@ -41,8 +41,8 @@ def _counts(snap, own):
 
 
 class Model:
-    """The engine's host-side classification (kr_engine.cu: first_stride, after_bucket_void, upload_lg, kr_engine_set_option) and
-    the capacities an incremental epoch is checked against on the device."""
+    """The engine's host-side classification (kr_engine.cu: first_stride, run_pass's ladder through after_bucket_void, upload_lg,
+    kr_engine_set_option) and the capacities an incremental epoch is checked against on the device."""
 
     def __init__(self, n_clusters, n_pods, large, wide):
         self.nc, self.n_pods, self.large, self.wide = n_clusters, n_pods, large, wide

@@ -19,10 +19,11 @@ pytestmark = pytest.mark.gpu
 
 
 class Regimes:
-    """The engine's size thresholds for this device.  Mirrors kuberay_b200/csrc/kr_engine.cu: launch_hash (full pass),
-    run_pass_inc (re-hash after a JSON commit) and kr_hash_batch all take k_hash3 while `(n + 31) / 32 <= sm_count * 4` and
-    k_hash2<4, 1> above; k_hash2's grid is capped at sm_count * hash_ctas_per_sm (2, KR_HASH_CTAS) CTAs of 128 lanes in a
-    pass and at sm_count * 4 CTAs in kr_hash_batch, so more messages than that make its grid-stride loop take a second trip.
+    """The engine's size thresholds for this device.  Mirrors launch_hash in kuberay_b200/csrc/kr_engine.cu, which the full
+    pass, the incremental pass's re-hash after a JSON commit and kr_hash_batch all call: k_hash3 while
+    `(n + 31) / 32 <= sm_count * 4` and k_hash2<4, 1> above; k_hash2's grid is capped at sm_count * hash_ctas_per_sm
+    (2, KR_HASH_CTAS) CTAs of 128 lanes in a pass and at sm_count * 4 CTAs in kr_hash_batch, so more messages than that make
+    its grid-stride loop take a second trip.
     KR_SMEM_GROUPS (kr_decide.cuh) is the widest RayCluster the bucket pipeline takes; 256 pods is the widest bucket stride."""
 
     def __init__(self):
