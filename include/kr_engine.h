@@ -430,7 +430,8 @@ int kr_snapshot_commit(kr_engine *e);
  * KR_PART_COLUMNS and keep the spec-JSON arena resident (the hash is still recomputed from it every pass). */
 enum {
   KR_PART_COLUMNS = 1,  /* every column */
-  KR_PART_JSON = 2,     /* the muted-spec JSON arena */
+  KR_PART_JSON = 2,     /* the muted-spec JSON arena.  Without KR_PART_OBJECTS / KR_PART_COLUMNS the c_json_off / c_json_len
+                           columns stay behind: the RayClusters whose range moved need an object commit of their rows. */
   KR_PART_ALL = 3,
   KR_PART_OBJECTS = 4   /* every column except the seven per-pod ones: RayCluster / group / workersToDelete / head-aux / RayJob
                            rows (about 2 MB at C3).  Together with kr_snapshot_commit_pod_rows this is an incremental epoch. */
@@ -461,7 +462,9 @@ int kr_snapshot_commit_pod_values(kr_engine *e, const uint32_t *rows, const uint
  * `head_rows` (same row count as before).  Only those rows travel (packed) and are applied by the on-device object diff.  It is
  * purely an optimisation of kr_snapshot_commit_parts(KR_PART_OBJECTS) — the informer's RayCluster status / replica / expectation
  * updates and head Pod status updates at a few hundred bytes per object instead of the whole object part: whenever the engine has
- * no resident state, or a Recreate gate, a JSON range or the number of head rows changed, it commits the whole object part itself. */
+ * no resident state, or a Recreate gate, a JSON range or the number of head rows changed, it commits the whole object part itself.
+ * That includes a range an earlier KR_PART_JSON-only commit moved (an arena compaction moves every range): unless every such
+ * RayCluster is among `cluster_rows`, the whole object part is committed. */
 int kr_snapshot_commit_object_rows(kr_engine *e, const uint32_t *cluster_rows, uint32_t n_cluster_rows, const uint32_t *head_rows, uint32_t n_head_rows);
 
 /* Row-granular spec commit: the caller rewrote, in the pinned arenas, the muted-spec JSON of the RayClusters `cluster_rows` — in

@@ -374,6 +374,9 @@ struct kr_engine {
   bool inc_gathered = false;     // ... and their records sit packed in the staging buffer
   bool inc_hash_ran = false;
   std::vector<uint64_t> prev_json_off; std::vector<uint32_t> prev_json_len;  // JSON ranges the digests were computed from
+  // rows whose range a JSON-only commit recorded above while the device's c_json_off / c_json_len kept the old one (sorted, distinct):
+  // kr_snapshot_commit_object_rows commits the whole object part unless it is given every one of them
+  std::vector<uint32_t> json_cols_behind;
   // kr_snapshot_commit_spec_rows, pinned mirror and device copy of {pull rows u32 | lens u32 | offs u64 | hash order u32}[max_clusters]:
   // each call appends the rows it pulls to the pull lists; the pass that hashes them sorts the pending rows once and uploads them as
   // the hash order
@@ -1649,6 +1652,13 @@ int kr_snapshot_commit_parts(kr_engine *e, uint32_t parts) {
     }
   }
   CK(cudaEventRecord(e->ev_cols, e->scopy));
+  if (parts & (KR_PART_COLUMNS | KR_PART_OBJECTS)) e->json_cols_behind.clear();
+  else if (ranges_moved) {  // the device's range columns keep the old ranges of the rows that moved
+    for (uint32_t c = 0; c < n.n_clusters; c++)
+      if (c >= e->prev_json_off.size() || e->prev_json_off[c] != hb.c_json_off[c] || e->prev_json_len[c] != hb.c_json_len[c]) e->json_cols_behind.push_back(c);
+    std::sort(e->json_cols_behind.begin(), e->json_cols_behind.end());
+    e->json_cols_behind.erase(std::unique(e->json_cols_behind.begin(), e->json_cols_behind.end()), e->json_cols_behind.end());
+  }
   if (ranges_moved) {  // digests of moved ranges are stale
     e->hash_dirty = true;
     e->prev_json_off.assign(hb.c_json_off, hb.c_json_off + n.n_clusters); e->prev_json_len.assign(hb.c_json_len, hb.c_json_len + n.n_clusters);
@@ -1737,6 +1747,15 @@ int kr_snapshot_commit_object_rows(kr_engine *e, const uint32_t *cluster_rows, u
     whole = e->recreate_bit[c] != ((hb.c_flags[c] & KR_CF_UPGRADE_RECREATE) ? 1 : 0) || e->prev_json_off[c] != hb.c_json_off[c] || e->prev_json_len[c] != hb.c_json_len[c] ||
             hb.c_group_cnt[c] != e->group_cnt[c] || (uint64_t)hb.c_group_off[c] + hb.c_group_cnt[c] > n.n_groups;
   }
+  // a range an earlier JSON-only commit moved is recorded as current, yet only an object commit of its row brings it to the device
+  if (!whole && !e->json_cols_behind.empty()) {
+    whole = e->json_cols_behind.size() > n_cl;
+    if (!whole) {
+      std::vector<uint32_t> given(cluster_rows, cluster_rows + n_cl);
+      std::sort(given.begin(), given.end());
+      whole = !std::includes(given.begin(), given.end(), e->json_cols_behind.begin(), e->json_cols_behind.end());
+    }
+  }
   for (uint32_t i = 0; i < n_hd && !whole; i++) {
     if (head_rows[i] >= n.n_heads) return fail(e, KR_E_INVALID, "head-aux row %u out of range", head_rows[i]);
     if (hb.h_pod_idx[head_rows[i]] >= n.n_pods) return fail(e, KR_E_INVALID, "head-aux row %u: h_pod_idx %u >= n_pods %u", head_rows[i], hb.h_pod_idx[head_rows[i]], n.n_pods);
@@ -1810,6 +1829,7 @@ int kr_snapshot_commit_object_rows(kr_engine *e, const uint32_t *cluster_rows, u
   CK(cudaEventRecord(e->orow.ev, e->scopy));
   e->orow.busy = true;
   if (int rc = launch_object_diff(e, oa, n_hd, reinterpret_cast<const uint32_t *>(e->orow.d + list_off[D_HEADS]), n_cl != 0)) return rc;
+  e->json_cols_behind.clear();  // (every recorded row was among the ones uploaded)
   return finish_commit(e, need, true, false);
 }
 

@@ -204,6 +204,9 @@ class Packer:
                            _s(snp.status_summary_key((j.get("status") or {}).get("rayClusterStatus"))))
         self._check(self._L.kr_packer_job_upsert(self._h, C.byref(o)))
 
+    def delete_job(self, ns: str, name: str):
+        self._check(self._L.kr_packer_job_delete(self._h, _s(ns), _s(name)))
+
     # ------------------------------------------------------------------ epoch
     def flush(self) -> int:
         mode = C.c_uint32()

@@ -62,11 +62,26 @@ class Mirror:
         self.clusters[(c.get("namespace", "default"), c["name"])] = c
         self.pk.upsert_cluster(c)
 
+    def delete_cluster(self, ns, name):
+        self.clusters.pop((ns, name), None)
+        self.pk.delete_cluster(ns, name)
+
+    def upsert_job(self, j):
+        key = (j.get("namespace", "default"), j["name"])
+        keys = [(x.get("namespace", "default"), x["name"]) for x in self.jobs]
+        self.jobs = [j if k == key else x for k, x in zip(keys, self.jobs)] + ([] if key in keys else [j])
+        self.pk.upsert_job(j)
+
+    def delete_job(self, ns, name):
+        self.jobs = [x for x in self.jobs if (x.get("namespace", "default"), x["name"]) != (ns, name)]
+        self.pk.delete_job(ns, name)
+
     def live_pods(self):
         return [p for p in self.rows if p is not None]
 
 
-def check(m: Mirror, oracle_mod, lean: bool):
+def check(m: Mirror, oracle_mod, lean: bool, run=None):
+    """`run(flags) -> Results` takes the packer's pass another way than kr_reconcile_batch (default: pk.engine.reconcile)."""
     pk = m.pk
     clusters = [m.clusters[k] for k in sorted(m.clusters)]
     pods = m.live_pods()
@@ -75,7 +90,7 @@ def check(m: Mirror, oracle_mod, lean: bool):
     flags.fetch_pod_lists = 0 if lean else 1
     want = oracle_mod.run(snap, flags)
     f2 = pk.flags(fetch_pod_lists=flags.fetch_pod_lists)
-    got = pk.engine.reconcile(f2)
+    got = (run or pk.engine.reconcile)(f2)
     it = meta.interner
     assert got.n_orphans == want.n_orphans and got.n_actions == want.n_actions and got.n_create_total == want.n_create_total
     for ci, key in enumerate(meta.cluster_keys):

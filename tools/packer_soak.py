@@ -2,7 +2,12 @@
 """A longer run of the native packer's random informer-event streams than tests/test_packer.py affords (4 seeds x 10 epochs there): per seed a
 fuzz-generated object set, then epochs of mixed Pod / RayCluster / RayJob events — structural ones included — through kr_packer_*, every
 epoch compared with the oracle on an independently re-packed snapshot (the test's own Mirror / check).  usage (GPU box):
-python tools/packer_soak.py [first_seed] [seeds] [epochs]"""
+python tools/packer_soak.py [first_seed] [seeds] [epochs] [--all-options] [--json-bytes N]
+
+--all-options turns on every opt-in engine option (large / wide / huge RayClusters, workersToDelete edits, spec rows) and adds spec edits
+with a bumped generation to every epoch (tests/test_gpu_packer_streams.py runs the same configuration at suite length); --json-bytes sets
+kr_config.max_json_bytes, small enough (a few KiB above the fleet's muted specs) that the stream compacts the JSON arena as it goes."""
+import argparse
 import copy
 import os
 import sys
@@ -17,26 +22,35 @@ import test_packer as tp  # noqa: E402
 from kuberay_b200 import abi  # noqa: E402
 from kuberay_b200.packer import Packer  # noqa: E402
 from oracle import oracle  # noqa: E402
+from test_gpu_spec_rows import _spec_edits  # noqa: E402
 
-first = int(sys.argv[1]) if len(sys.argv) > 1 else 10
-seeds = int(sys.argv[2]) if len(sys.argv) > 2 else 40
-epochs = int(sys.argv[3]) if len(sys.argv) > 3 else 30
+ap = argparse.ArgumentParser()
+ap.add_argument("first", nargs="?", type=int, default=10)
+ap.add_argument("seeds", nargs="?", type=int, default=40)
+ap.add_argument("epochs", nargs="?", type=int, default=30)
+ap.add_argument("--all-options", action="store_true")
+ap.add_argument("--json-bytes", type=int, default=4 << 20)
+a = ap.parse_args()
+opts = dict(large_clusters=True, wide_clusters=True, huge_clusters=True, wtd_edits=True, spec_rows=True) if a.all_options else {}
 oracle.lib()
 total = inc = 0
-for seed in range(first, first + seeds):
+for seed in range(a.first, a.first + a.seeds):
     rng = np.random.default_rng(seed)
     clusters, pods, jobs = fuzz_objects.generate(seed, big=True)
     for i, c in enumerate(clusters):
         c["generation"], c["resourceVersion"] = 1, 100 + i
     for i, j in enumerate(jobs):
         j.setdefault("name", f"rayjob-{i}")
-    pk = Packer(max_clusters=64, max_groups=512, max_wtd=512, max_pods=8192, max_heads=256, max_jobs=64, max_creates=1 << 16, max_json_bytes=4 << 20)
+    pk = Packer(max_clusters=64, max_groups=512, max_wtd=512, max_pods=8192, max_heads=256, max_jobs=64, max_creates=1 << 16,
+                max_json_bytes=a.json_bytes, **opts)
     try:
         m = tp.Mirror(copy.deepcopy(clusters), copy.deepcopy(pods), jobs, pk)
         assert pk.flush() == abi.PACK_FULL
         tp.check(m, oracle, lean=True)
-        counter = [0]
-        for epoch in range(epochs):
+        counter, gen = [0], [2]
+        for epoch in range(a.epochs):
+            if a.all_options:
+                _spec_edits(rng, m, gen, int(rng.integers(1, 4)))
             tp._events(rng, m, counter, structural=True)
             mode = pk.flush()
             assert not mode & abi.PACK_FULL, (seed, epoch)
@@ -45,4 +59,5 @@ for seed in range(first, first + seeds):
             inc += bool(mode & abi.PACK_POD_ROWS)
     finally:
         pk.close()
-print(f"packer soak ok: seeds {first}..{first + seeds - 1} x {epochs} epochs = {total} epochs ({inc} with pod-row commits), every one equal to the oracle")
+print(f"packer soak ok: seeds {a.first}..{a.first + a.seeds - 1} x {a.epochs} epochs = {total} epochs ({inc} with pod-row commits), "
+      f"options {'all on' if a.all_options else 'default'}, max_json_bytes {a.json_bytes}, every one equal to the oracle")
