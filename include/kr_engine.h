@@ -705,6 +705,39 @@ int        kr_packer_epoch(kr_packer *p, uint64_t *epoch, uint64_t *podset_versi
 int        kr_packer_cluster_epoch(kr_packer *p, uint32_t cluster_row, uint64_t *resource_version, uint64_t *generation);
 const char *kr_packer_last_error(kr_packer *p);
 
+/* ---- group packer: the native packer sharded over GPUs (DESIGN §6).  One kr_packer per shard behind one handle; each is created
+ * on its shard's worker thread of a kr_group (NUMA-local pinned arenas), and flush / reconcile run every shard on its worker in
+ * parallel, each on the single-device incremental path.
+ * Routing key (namespace, RayCluster name): a RayCluster by its own name, a Pod by its ray.io/cluster label, a RayJob by its
+ * cluster name; shard = kr_shard_of_key.  A Pod therefore always sits on the shard of every RayCluster its label can match
+ * (common/association.go:83-130): an orphan needs no move when its RayCluster arrives, and a RayCluster deleted and re-created
+ * under its name (a new UID) lands where its old Pods are.  kr_group_route / kr_group_shard_of_uid keep UID routing for the
+ * global-snapshot path; a RayCluster's decisions depend only on its own objects, so the key that shards changes no result.
+ * Event calls run on the caller thread (O(1) plus at most n Pod-table lookups, no hop to a worker).  A Pod whose label changed, or
+ * a RayJob whose cluster name changed, is upserted on its new shard and deleted from its old one; deleting an unknown key is KR_OK.
+ * kr_group_packer_shard(i) is shard i's kr_packer for reads and per-shard settings (kr_packer_string / _pod_key / _cluster_row /
+ * _epoch / _intern / _set_kuberay_version, options through kr_packer_engine — they are not forwarded); kr_group_packer_group is
+ * the kr_group over the shards' engines (kr_group_engine / _device / _allgather_group_results; kr_group_route / _commit /
+ * _reconcile do not belong to a group packer).  On an error the first failing shard's code is returned and
+ * kr_group_packer_last_error names that shard with its packer's message.  One caller thread at a time for the whole handle. */
+typedef struct kr_group_packer kr_group_packer;
+uint32_t   kr_shard_of_key(kr_str ns, kr_str cluster_name, uint32_t n);  /* FNV-1a 64 over ns "/" name, % n (an absent name hashes as ""); no handle, no device */
+int        kr_group_packer_create(const kr_config *per_shard_capacities, const int32_t *devices, uint32_t n, kr_group_packer **out);  /* devices as kr_group_create */
+void       kr_group_packer_destroy(kr_group_packer *gp);
+uint32_t   kr_group_packer_size(kr_group_packer *gp);
+kr_packer *kr_group_packer_shard(kr_group_packer *gp, uint32_t shard);
+kr_group  *kr_group_packer_group(kr_group_packer *gp);
+int        kr_group_packer_pod_upsert(kr_group_packer *gp, const kr_pod_obj *pod);
+int        kr_group_packer_pod_delete(kr_group_packer *gp, kr_str ns, kr_str name);
+int        kr_group_packer_cluster_upsert(kr_group_packer *gp, const kr_cluster_obj *c);
+int        kr_group_packer_cluster_delete(kr_group_packer *gp, kr_str ns, kr_str name);
+int        kr_group_packer_job_upsert(kr_group_packer *gp, const kr_job_obj *j);
+int        kr_group_packer_job_delete(kr_group_packer *gp, kr_str ns, kr_str name);
+int        kr_group_packer_flush(kr_group_packer *gp, uint32_t *modes_out /* [n], optional: each shard's kr_packer_flush mode */);
+/* flags[i] for shard i (id_head_not_found_* are ids of shard i's interner: kr_packer_intern on kr_group_packer_shard(i)) */
+int        kr_group_packer_reconcile(kr_group_packer *gp, const kr_flags *flags /* [n] */, kr_results_view *views /* [n] */);
+const char *kr_group_packer_last_error(kr_group_packer *gp);
+
 /* ------------------------------------------------------------------------------------------------------------------------------
  * Pod metadata builder (SURVEY §8 f3, first part): what createHeadPod / createWorkerPodWithIndex put into the new Pod's
  * ObjectMeta — the part of buildHeadPod / buildWorkerPod that depends on the engine's create tuples (group, replica index,

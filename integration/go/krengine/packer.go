@@ -82,6 +82,15 @@ func (p *Packer) err(rc C.int) error {
 func (p *Packer) UpsertPod(o *PodObj) error {
 	var s strs
 	defer s.release()
+	c := o.c(&s)
+	if rc := C.kr_packer_pod_upsert(p.h, &c); rc != C.KR_OK {
+		return p.err(rc)
+	}
+	return nil
+}
+
+// c fills the kr_pod_obj; its strings stay pinned until s.release().
+func (o *PodObj) c(s *strs) C.kr_pod_obj {
 	c := C.kr_pod_obj{ns: s.str(o.Namespace), name: s.str(o.Name), cluster: s.str(o.Cluster), group: s.str(o.Group), replica_name: s.str(o.ReplicaName),
 		replica_index: s.str(o.ReplicaIndex), node_type: C.uint8_t(o.NodeType), phase: C.uint8_t(o.Phase), ready_cond: C.uint8_t(o.ReadyCond),
 		restart_never: b2u(o.RestartNever), ray_terminated: b2u(o.RayTerminated), has_deletion_ts: b2u(o.HasDeletion), head_ready_status: C.uint8_t(o.HeadReadyStatus),
@@ -92,10 +101,7 @@ func (p *Packer) UpsertPod(o *PodObj) error {
 	if o.HasKubeRayVersion {
 		c.kuberay_version = s.present(o.KubeRayVersion)
 	}
-	if rc := C.kr_packer_pod_upsert(p.h, &c); rc != C.KR_OK {
-		return p.err(rc)
-	}
-	return nil
+	return c
 }
 
 func (p *Packer) DeletePod(ns, name string) error {
@@ -110,6 +116,15 @@ func (p *Packer) DeletePod(ns, name string) error {
 func (p *Packer) UpsertCluster(o *ClusterObj) error {
 	var s strs
 	defer s.release()
+	c := o.c(&s)
+	if rc := C.kr_packer_cluster_upsert(p.h, &c); rc != C.KR_OK {
+		return p.err(rc)
+	}
+	return nil
+}
+
+// c fills the kr_cluster_obj; its strings, groups, name lists and spec stay pinned until s.release().
+func (o *ClusterObj) c(s *strs) C.kr_cluster_obj {
 	groups := make([]C.kr_group_obj, len(o.Groups))
 	names := make([][]C.kr_str, len(o.Groups)) // one C-visible array of names per group, pinned below
 	for i := range o.Groups {
@@ -147,10 +162,7 @@ func (p *Packer) UpsertCluster(o *ClusterObj) error {
 		c.spec_json = (*C.uint8_t)(unsafe.Pointer(&o.SpecJSON[0]))
 		c.spec_json_len = C.uint64_t(len(o.SpecJSON))
 	}
-	if rc := C.kr_packer_cluster_upsert(p.h, &c); rc != C.KR_OK {
-		return p.err(rc)
-	}
-	return nil
+	return c
 }
 
 func (p *Packer) DeleteCluster(ns, name string) error {

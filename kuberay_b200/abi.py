@@ -316,10 +316,16 @@ ENGINE_SYMBOLS = [
     "kr_packer_cluster_upsert", "kr_packer_cluster_delete", "kr_packer_job_upsert", "kr_packer_job_delete", "kr_packer_flush", "kr_packer_sizes", "kr_packer_bufs",
     "kr_packer_intern", "kr_packer_string", "kr_packer_cluster_row", "kr_packer_pod_row", "kr_packer_pod_key", "kr_packer_epoch",
     "kr_packer_cluster_epoch", "kr_packer_last_error",
+    "kr_shard_of_key", "kr_group_packer_create", "kr_group_packer_destroy", "kr_group_packer_size", "kr_group_packer_pod_upsert",
+    "kr_group_packer_pod_delete", "kr_group_packer_cluster_upsert", "kr_group_packer_cluster_delete", "kr_group_packer_job_upsert",
+    "kr_group_packer_job_delete", "kr_group_packer_flush", "kr_group_packer_reconcile", "kr_group_packer_last_error",
     "kr_pod_name", "kr_check_name", "kr_check_label", "kr_pod_meta_build", "kr_pod_creates_expand", "kr_pod_meta_last_error",
     "kr_ray_start_command", "kr_ray_container_env", "kr_ray_probes", "kr_ray_volumes", "kr_quantity_value", "kr_ray_start_last_error",
     "kr_pod_build", "kr_pod_build_last_error", "kr_ray_ft_env", "kr_ray_auth", "kr_ray_autoscaler_container", "kr_ray_init_container", "kr_ray_template_last_error",
 ]
+
+# declared with a handle return type (kr_packer * / kr_group *): exported as well
+ENGINE_HANDLE_SYMBOLS = ["kr_group_packer_shard", "kr_group_packer_group"]
 
 
 def default_flags(**kw) -> kr_flags:

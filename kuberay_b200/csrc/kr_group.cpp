@@ -13,6 +13,8 @@
 //     delta records (kr_group_result, 32 B each) — over NCCL (ncclAllGather issued from the coordinator thread, one
 //     communicator per device; the library is looked up at run time) when every shard sits on its own device, by peer
 //     copies otherwise (several shards on one GPU: tests on a single-GPU box).
+// The worker threads, NUMA placement and exchange are shared with the group packer (kr_group_packer.cpp): its shards are
+// kr_packers, made on the same workers by kr_internal_group_create, and the group frees each engine through its owner.
 #include <cuda_runtime.h>
 #include <dlfcn.h>
 #include <sched.h>
@@ -145,6 +147,7 @@ struct kr_group {
   std::vector<int> rc;
   std::string err;
   bool distinct_devices = true;
+  std::function<void(uint32_t, kr_engine *)> release;  // frees shard i's engine (kr_group_create: kr_engine_destroy; a group packer: its kr_packer)
   // exchange step
   Nccl nccl;
   bool nccl_tried = false, nccl_ok = false;
@@ -158,26 +161,29 @@ namespace {
 
 int gfail(kr_group *g, int code, const std::string &m) { if (g) g->err = m; return code; }
 
-template <class F>
-int for_all(kr_group *g, F f) {  // f(i) on shard i's thread; first failing code wins
+}  // namespace
+
+// Shared with kr_group_packer.cpp: f(i) on shard i's thread, all joined; returns the first failing code and its shard.
+int kr_internal_group_run(kr_group *g, const std::function<int(uint32_t)> &f, uint32_t *failed_shard) {
   const size_t n = g->eng.size();
-  for (size_t i = 0; i < n; i++) g->worker[i]->submit([g, i, f] { g->rc[i] = f((uint32_t)i); });
+  for (size_t i = 0; i < n; i++) g->worker[i]->submit([g, i, &f] { g->rc[i] = f((uint32_t)i); });
   for (size_t i = 0; i < n; i++) g->worker[i]->wait();
   for (size_t i = 0; i < n; i++)
-    if (g->rc[i]) { g->err = std::string("shard ") + std::to_string(i) + ": " + kr_last_error(g->eng[i]); return g->rc[i]; }
+    if (g->rc[i]) { if (failed_shard) *failed_shard = (uint32_t)i; return g->rc[i]; }
   return KR_OK;
 }
 
-}  // namespace
-
-extern "C" {
-
-int kr_group_create(const kr_config *per_shard, const int32_t *devices, uint32_t n, kr_group **out) {
-  if (!per_shard || !out || n == 0 || n > 64) return KR_E_INVALID;
+// One worker thread per shard (pinned to its device's NUMA node), and on it make(i, device, &engine): whatever owns the engine is
+// created there, so its pinned arenas are node-local.  kr_group_destroy calls release(i, engine) on the same thread for every shard
+// that got an engine — the engine is freed there and nowhere else.
+int kr_internal_group_create(const int32_t *devices, uint32_t n, const std::function<int(uint32_t, int, kr_engine **)> &make,
+                             std::function<void(uint32_t, kr_engine *)> release, kr_group **out) {
+  if (!out || n == 0 || n > 64) return KR_E_INVALID;
   *out = nullptr;
   int ndev = kr_device_count();
   if (ndev <= 0) return KR_E_NO_DEVICE;
   kr_group *g = new kr_group();
+  g->release = std::move(release);
   g->eng.assign(n, nullptr); g->device.resize(n); g->rc.assign(n, 0); g->bufs.resize(n); g->sizes.resize(n);
   for (uint32_t i = 0; i < n; i++) {
     g->device[i] = devices ? devices[i] : (int)(i % (uint32_t)ndev);
@@ -185,17 +191,38 @@ int kr_group_create(const kr_config *per_shard, const int32_t *devices, uint32_t
     for (uint32_t j = 0; j < i; j++) if (g->device[j] == g->device[i]) g->distinct_devices = false;
   }
   for (uint32_t i = 0; i < n; i++) { g->worker.push_back(new Worker()); g->worker[i]->start(g->device[i]); }
-  // every engine is created by its own (NUMA-bound) thread: its pinned arenas land on the GPU's node
-  for (uint32_t i = 0; i < n; i++) {
-    kr_config cfg = *per_shard;
-    cfg.device = g->device[i];
-    g->worker[i]->submit([g, i, cfg] { g->rc[i] = kr_engine_create(&cfg, &g->eng[i]); });
-  }
-  int rc = KR_OK;
-  for (uint32_t i = 0; i < n; i++) { g->worker[i]->wait(); if (g->rc[i] && !rc) rc = g->rc[i]; }
+  int rc = kr_internal_group_run(g, [g, &make](uint32_t i) { return make(i, g->device[i], &g->eng[i]); }, nullptr);
   if (rc) { kr_group_destroy(g); return rc; }
   *out = g;
   return KR_OK;
+}
+
+// The live row counts of shard i (kr_group_allgather_group_results sizes its slots by them): kr_group_route sets them, a group
+// packer after each flush.
+kr_sizes *kr_internal_group_sizes(kr_group *g, uint32_t i) { return &g->sizes[i]; }
+
+namespace {
+
+template <class F>
+int for_all(kr_group *g, F f) {  // f(i) on shard i's thread; first failing code wins
+  uint32_t bad = 0;
+  const int rc = kr_internal_group_run(g, f, &bad);
+  if (rc) g->err = std::string("shard ") + std::to_string(bad) + ": " + kr_last_error(g->eng[bad]);
+  return rc;
+}
+
+}  // namespace
+
+extern "C" {
+
+int kr_group_create(const kr_config *per_shard, const int32_t *devices, uint32_t n, kr_group **out) {
+  if (!per_shard) return KR_E_INVALID;
+  const kr_config base = *per_shard;
+  return kr_internal_group_create(devices, n, [&base](uint32_t, int device, kr_engine **e) {
+    kr_config cfg = base;
+    cfg.device = device;
+    return kr_engine_create(&cfg, e);
+  }, [](uint32_t, kr_engine *e) { kr_engine_destroy(e); }, out);
 }
 
 void kr_group_destroy(kr_group *g) {
@@ -207,7 +234,7 @@ void kr_group_destroy(kr_group *g) {
         if (i < g->xstream.size() && g->xstream[i]) cudaStreamDestroy(g->xstream[i]);
         if (i < g->xsend.size() && g->xsend[i]) cudaFree(g->xsend[i]);
         if (i < g->xrecv.size() && g->xrecv[i]) cudaFree(g->xrecv[i]);
-        if (g->eng[i]) kr_engine_destroy(g->eng[i]);
+        if (g->eng[i]) g->release((uint32_t)i, g->eng[i]);
         g->rc[i] = 0;
       });
       g->worker[i]->wait();

@@ -509,6 +509,15 @@ int64_t kr_packer_pod_row(kr_packer *p, kr_str ns, kr_str name) {
   auto it = p->pod_row.find(Key{p->intern(ns), p->intern(name)});
   return it == p->pod_row.end() ? -1 : (int64_t)it->second;
 }
+// kr_packer_pod_row without interning the key (kr_group_packer.cpp asks every shard for a Pod that lives on at most one of them:
+// the others must not collect its strings).
+int64_t kr_internal_packer_find_pod(kr_packer *p, kr_str ns, kr_str name) {
+  if (!p || !ns.p || !name.p) return -1;
+  auto a = p->ids.find(std::string_view(ns.p, ns.n)), b = p->ids.find(std::string_view(name.p, name.n));
+  if (a == p->ids.end() || b == p->ids.end()) return -1;
+  auto it = p->pod_row.find(Key{a->second, b->second});
+  return it == p->pod_row.end() ? -1 : (int64_t)it->second;
+}
 int kr_packer_pod_key(kr_packer *p, uint32_t row, kr_str *ns, kr_str *name) {
   if (!p || row >= p->row_key.size() || !ns || !name) return KR_E_INVALID;
   const Key k = p->row_key[row];

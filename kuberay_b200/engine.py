@@ -95,7 +95,28 @@ def lib() -> C.CDLL:
         L.kr_group_allgather_group_results.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64, P(C.c_uint64), P(C.c_int)]
         L.kr_group_last_error.argtypes = [C.c_void_p]
         L.kr_group_last_error.restype = C.c_char_p
-        for name in abi.ENGINE_SYMBOLS:
+        L.kr_shard_of_key.argtypes = [abi.kr_str, abi.kr_str, C.c_uint32]
+        L.kr_shard_of_key.restype = C.c_uint32
+        L.kr_group_packer_create.argtypes = [P(abi.kr_config), C.c_void_p, C.c_uint32, P(C.c_void_p)]
+        L.kr_group_packer_destroy.argtypes = [C.c_void_p]
+        L.kr_group_packer_destroy.restype = None
+        L.kr_group_packer_size.argtypes = [C.c_void_p]
+        L.kr_group_packer_size.restype = C.c_uint32
+        L.kr_group_packer_shard.argtypes = [C.c_void_p, C.c_uint32]
+        L.kr_group_packer_shard.restype = C.c_void_p
+        L.kr_group_packer_group.argtypes = [C.c_void_p]
+        L.kr_group_packer_group.restype = C.c_void_p
+        L.kr_group_packer_pod_upsert.argtypes = [C.c_void_p, P(abi.kr_pod_obj)]
+        L.kr_group_packer_pod_delete.argtypes = [C.c_void_p, abi.kr_str, abi.kr_str]
+        L.kr_group_packer_cluster_upsert.argtypes = [C.c_void_p, P(abi.kr_cluster_obj)]
+        L.kr_group_packer_cluster_delete.argtypes = [C.c_void_p, abi.kr_str, abi.kr_str]
+        L.kr_group_packer_job_upsert.argtypes = [C.c_void_p, P(abi.kr_job_obj)]
+        L.kr_group_packer_job_delete.argtypes = [C.c_void_p, abi.kr_str, abi.kr_str]
+        L.kr_group_packer_flush.argtypes = [C.c_void_p, C.c_void_p]
+        L.kr_group_packer_reconcile.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p]
+        L.kr_group_packer_last_error.argtypes = [C.c_void_p]
+        L.kr_group_packer_last_error.restype = C.c_char_p
+        for name in abi.ENGINE_SYMBOLS + abi.ENGINE_HANDLE_SYMBOLS:
             getattr(L, name)  # raises AttributeError if the header and the library drifted apart
         _LIB = L
     return _LIB
