@@ -16,11 +16,8 @@ import json
 import numpy as np
 import pytest
 
+from harness import OBJ_COLS, SORT_KERNELS, Driver, b32, head_row, incremental, scale_to, set_phase, spec_bytes, workers
 from kuberay_b200 import abi, synthetic
-
-from test_gpu_incremental import OBJ_COLS, Driver
-from test_gpu_regimes import _b32, _spec
-from test_gpu_wide_clusters import SORT_KERNELS, _head_row, _scale_to, _set_phase, _workers
 
 pytestmark = pytest.mark.gpu
 
@@ -138,12 +135,10 @@ class Stream(Driver):
         flags.fetch_pod_lists = 0
         # B behind a Recreate gate whose annotation is the digest of its spec (a JSON re-commit flips it)
         snap.c_flags[self.B] |= np.uint32(abi.CF_UPGRADE_RECREATE)
-        h = _head_row(snap, self.B)
+        h = head_row(snap, self.B)
         snap.h_version_state[h], snap.h_annot_state[h] = abi.VER_CURRENT, abi.ANNOT_HASH32
-        snap.h_annot_hash.reshape(-1, 32)[h] = np.frombuffer(_b32(_spec(snap, self.B)).encode(), dtype=np.uint8)
-        super().__init__(snap, flags, max_creates=1 << 21)
-        self.eng.set_large_clusters(True)
-        self.eng.set_wide_clusters(True)
+        snap.h_annot_hash.reshape(-1, 32)[h] = np.frombuffer(b32(spec_bytes(snap, self.B)), dtype=np.uint8)
+        super().__init__(snap, flags, max_creates=1 << 21, large_clusters=True, wide_clusters=True)
         self.model = Model(nc, snap.dims["pods"], True, True)
         self.own = _owners(snap)
         self.free, self.saved, self.next_name = [], {}, 0x7E000000
@@ -159,7 +154,7 @@ class Stream(Driver):
     # ------------------------------------------------------------------------------------------------ snapshot edits
     def _healthy(self, snap, c):
         m = np.flatnonzero(_owners(snap) == c)
-        _set_phase(snap, m, abi.PHASE_RUNNING)
+        set_phase(snap, m, abi.PHASE_RUNNING)
         snap.p_packed[m] = (snap.p_packed[m] & ~np.uint32((3 << abi.PP_READY_SHIFT) | abi.PP_RAY_TERMINATED)) | np.uint32(abi.COND_TRUE << abi.PP_READY_SHIFT)
         snap.c_flags[c] &= ~np.uint32(abi.CF_SKIP | abi.CF_SUSPEND | abi.CF_UPGRADE_RECREATE | abi.CF_AUTOSCALING)
         snap.c_flags[c] |= np.uint32(abi.CF_HEAD_EXPECT_OK)
@@ -167,7 +162,7 @@ class Stream(Driver):
         for gi in range(int(snap.c_group_cnt[c])):
             g = g0 + gi
             snap.g_num_hosts[g] = 1
-            _scale_to(snap, g, int((snap.p_group_name_id[_workers(snap, c)] == snap.g_name_id[g]).sum()))
+            scale_to(snap, g, int((snap.p_group_name_id[workers(snap, c)] == snap.g_name_id[g]).sum()))
         return m
 
     def _relabel(self, rows, c):
@@ -213,7 +208,7 @@ class Stream(Driver):
         for r in rng.choice(workers, int(rng.integers(10, 40)), replace=False).tolist():
             s.p_packed[r] ^= np.uint32(1 << abi.PP_READY_SHIFT)
             if not large[r] and rng.random() < 0.3:
-                _set_phase(s, [r], int(rng.integers(1, 6)))
+                set_phase(s, [r], int(rng.integers(1, 6)))
             self.touched.add(r)
         workers = workers[~large[workers]]
         for r in rng.choice(workers, int(rng.integers(0, 10)), replace=False).tolist():  # deletions -> free rows
@@ -372,7 +367,8 @@ class Stream(Driver):
         elif any(counts[c] == lim[c] for c in m.caps):
             self.seen.add("region edge")
         self.predicted = cause
-        got, inc = self.check(self.oracle, device_only=self.device_only)
+        got, _ = self.check(self.oracle, device_only=self.device_only)
+        inc = incremental(got, s.dims["clusters"])
         decided = got.clusters["path"] != abi.PATH_SKIPPED
         if self.json:  # B's Recreate gate flipped: every pod deleted after an odd number of re-commits, none after an even one
             assert (got.clusters["path"][self.B] == abi.PATH_RECREATE_DELETE_ALL) == bool(self.json_flips % 2), (self.json_flips, got.clusters[self.B])

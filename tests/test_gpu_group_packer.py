@@ -1,9 +1,9 @@
 """The group packer (kr_group_packer_*, kuberay_b200/csrc/kr_group_packer.cpp; DESIGN §6): one native packer per shard behind one
 handle, events routed by (namespace, RayCluster name), every shard flushed and reconciled on its own worker thread.
 
-Every event goes to the group packer, to one test_packer.Mirror per shard (the objects routed by kr_shard_of_key, so the oracle
+Every event goes to the group packer, to one harness.Mirror per shard (the objects routed by kr_shard_of_key, so the oracle
 sees each shard's own snapshot) and to a single-device Packer twin.  Each epoch, every shard's view from ONE GroupPacker.reconcile
-must equal the oracle on its shard's objects (test_packer.check), and the shards together must decide every RayCluster exactly as
+must equal the oracle on its shard's objects (harness.packer_check), and the shards together must decide every RayCluster exactly as
 the twin does.  Each shard reuses its own lowest free Pod row, so List order differs from the twin's: order-dependent choices are
 checked only against the shard's own oracle.  The shards share device 0; with several GPUs one more run puts each on its own."""
 import copy
@@ -11,17 +11,14 @@ import copy
 import numpy as np
 import pytest
 
-import fuzz_objects
+from harness import L_CLUSTER, L_GROUP, L_TYPE, PACKER_CAPS, Mirror, events, objects, packer_check
 from kuberay_b200 import abi
 from kuberay_b200 import snapshot as snp
 from kuberay_b200.engine import EngineError, lib
 from kuberay_b200.packer import GroupPacker, Packer, shard_of_key
-from test_live_arena import L_CLUSTER, L_GROUP, L_TYPE, _events
-from test_packer import Mirror, check
 
 pytestmark = pytest.mark.gpu
 
-CAP = dict(max_clusters=64, max_groups=512, max_wtd=512, max_pods=4096, max_heads=256, max_jobs=64, max_creates=1 << 16, max_json_bytes=4 << 20)
 NS = "gp"
 
 
@@ -51,7 +48,7 @@ def _job_cluster(j):
 
 class Router:
     """The informer side: every event goes to the group packer, to the Mirror of the shard kr_shard_of_key names, and to the twin.
-    Looks like a LiveArena to test_live_arena._events (rows, row_of, clusters, upsert / delete)."""
+    Looks like a LiveArena to harness.events (rows, row_of, clusters, upsert / delete)."""
 
     def __init__(self, clusters, pods, jobs, gp: GroupPacker, twin: Packer | None):
         self.gp, self.n = gp, gp.n
@@ -132,7 +129,7 @@ class Router:
         modes = self.gp.flush()
         res = self.gp.reconcile(self.gp.flags(fetch_pod_lists=0 if lean else 1))
         for i, m in enumerate(self.m):
-            want, _ = check(m, oracle_mod, lean, run=lambda _f, i=i: res[i])
+            want, _ = packer_check(m, oracle_mod, lean, run=lambda _f, i=i: res[i])
             _check_jobs(m, want, res[i])
         self.check_placement()
         if twin and self.twin is not None:
@@ -187,11 +184,7 @@ def _check_jobs(m: Mirror, want, got):
 
 
 def _fuzz(seed):
-    clusters, pods, jobs = fuzz_objects.generate(seed, big=True)
-    for i, c in enumerate(clusters):
-        c["generation"], c["resourceVersion"] = 1, 100 + i
-    for i, j in enumerate(jobs):
-        j.setdefault("name", f"rayjob-{i}")
+    clusters, pods, jobs = objects(seed, big=True)
     return copy.deepcopy(clusters), copy.deepcopy(pods), jobs
 
 
@@ -205,7 +198,7 @@ def _devices(n):
 def test_every_shard_equals_its_oracle_and_the_twin_every_epoch(seed, n, oracle_mod):
     rng = np.random.default_rng(seed)
     clusters, pods, jobs = _fuzz(seed)
-    gp, twin = GroupPacker(_devices(n), **CAP), Packer(**CAP)
+    gp, twin = GroupPacker(_devices(n), **PACKER_CAPS), Packer(**PACKER_CAPS)
     try:
         r = Router(clusters, pods, jobs, gp, twin)
         modes, _, _ = r.epoch(oracle_mod, lean=False)
@@ -213,7 +206,7 @@ def test_every_shard_equals_its_oracle_and_the_twin_every_epoch(seed, n, oracle_
         r.epoch(oracle_mod, lean=True)
         counter = [0]
         for epoch in range(8):
-            _events(rng, r, counter, structural=True)
+            events(rng, r, counter, structural=True)
             modes, _, _ = r.epoch(oracle_mod, lean=bool(epoch % 2))
             assert not any(mo & abi.PACK_FULL for mo in modes)
     finally:
@@ -266,7 +259,7 @@ def _one_cluster_per_shard(r: Router):
 @pytest.mark.parametrize("n", [2, 3])
 def test_churn_and_replica_edits_stay_incremental_on_every_shard(n, oracle_mod):
     clusters, pods = _fleet(8 * n)
-    gp, twin = GroupPacker(_devices(n), **CAP), Packer(**CAP)
+    gp, twin = GroupPacker(_devices(n), **PACKER_CAPS), Packer(**PACKER_CAPS)
     try:
         r = Router(clusters, pods, [], gp, twin)
         assert all(len(m.clusters) >= 2 for m in r.m), [len(m.clusters) for m in r.m]
@@ -315,7 +308,7 @@ def test_churn_and_replica_edits_stay_incremental_on_every_shard(n, oracle_mod):
 @pytest.mark.parametrize("n", [2, 3])
 def test_routing_edge_cases(n, oracle_mod):
     clusters, pods = _fleet(6)
-    gp, twin = GroupPacker(_devices(n), **CAP), Packer(**CAP)
+    gp, twin = GroupPacker(_devices(n), **PACKER_CAPS), Packer(**PACKER_CAPS)
     try:
         r = Router(clusters, pods, [{"namespace": NS, "name": "job-a", "status": {}}], gp, twin)
         r.epoch(oracle_mod, lean=True)
@@ -379,7 +372,7 @@ def test_every_option_on_equals_the_all_off_twin(oracle_mod):
     wide = [(f"g{k}", 1) for k in range(40)]
     clusters.append(_cluster("wide", wide))
     pods += [_head("wide")] + [_worker("wide", 0, group=g) for g, _ in wide]
-    cap = dict(CAP, max_pods=8192)
+    cap = dict(PACKER_CAPS, max_pods=8192)
     gp = GroupPacker(_devices(n), large_clusters=True, wide_clusters=True, huge_clusters=True, wtd_edits=True, spec_rows=True, **cap)
     twin = Packer(**cap)
     try:
@@ -390,7 +383,7 @@ def test_every_option_on_equals_the_all_off_twin(oracle_mod):
         r.epoch(oracle_mod, lean=True)
         counter = [0]
         for epoch in range(8):
-            _events(rng, r, counter, structural=epoch % 3 == 2)
+            events(rng, r, counter, structural=epoch % 3 == 2)
             if epoch % 2 == 0:  # a workersToDelete edit and a spec edit
                 key = (NS, "large")
                 c = copy.deepcopy(r.clusters[key])
@@ -408,7 +401,7 @@ def test_every_option_on_equals_the_all_off_twin(oracle_mod):
 # ---------------------------------------------------------------------------------------------------------------- (7)
 def test_a_shard_over_capacity_fails_the_flush_and_is_named(oracle_mod):
     n = 2
-    gp = GroupPacker(_devices(n), **dict(CAP, max_groups=4))
+    gp = GroupPacker(_devices(n), **dict(PACKER_CAPS, max_groups=4))
     try:
         names = [f"rc{i}" for i in range(64)]
         full = next(s for s in range(n) if sum(shard_of_key(NS, x, n) == s for x in names) >= 3)
@@ -429,13 +422,13 @@ def test_one_shard_per_device_when_the_box_has_several(oracle_mod):
     if n < 2:
         pytest.skip("one GPU: the shards share device 0 in the tests above")
     clusters, pods, jobs = _fuzz(5)
-    gp, twin = GroupPacker(list(range(n)), **CAP), Packer(**CAP)
+    gp, twin = GroupPacker(list(range(n)), **PACKER_CAPS), Packer(**PACKER_CAPS)
     try:
         r = Router(clusters, pods, jobs, gp, twin)
         r.epoch(oracle_mod, lean=True)
         rng, counter = np.random.default_rng(5), [0]
         for epoch in range(4):
-            _events(rng, r, counter, structural=True)
+            events(rng, r, counter, structural=True)
             r.epoch(oracle_mod, lean=bool(epoch % 2))
         assert [gp.group._L.kr_group_device(gp.group._h, i) for i in range(n)] == list(range(n))
     finally:

@@ -8,79 +8,11 @@ must name the records it recomputed; records it did not name must be the ones th
 import numpy as np
 import pytest
 
+from harness import OBJ_COLS, POD_COLS, Driver, flip_ready, incremental, set_phase
 from kuberay_b200 import abi, synthetic
-from kuberay_b200.engine import Engine
 from kuberay_b200.snapshot import Snapshot
 
 pytestmark = pytest.mark.gpu
-
-POD_COLS = [name for name, _dt, _m, dim in abi.COLUMNS if dim == "pods"]
-OBJ_COLS = [name for name, _dt, _m, dim in abi.COLUMNS if dim not in ("pods", "json")]
-
-
-class Driver:
-    def __init__(self, snap, flags, slack=1.0, max_creates=None):
-        self.snap, self.flags = snap, flags
-        self.flags.fetch_pod_lists = 0
-        self.eng = Engine.for_snapshot(snap, slack=slack, max_creates=max_creates)
-        self.eng.set_fixed_layout(True)
-        self.views = self.eng.begin(snap.sizes())
-        self.eng.fill(self.views, snap)
-        self.eng.commit()
-        self.prev = None
-
-    def commit_rows(self, rows, journal=True):
-        rows = np.unique(np.asarray(rows, dtype=np.uint32))
-        for c in POD_COLS:
-            self.views[c][rows] = self.snap.cols[c][rows]
-        if not rows.size:
-            return
-        if journal:
-            self.eng.commit_pod_values(rows, np.stack([self.snap.cols[c][rows].view(np.uint32) for c in POD_COLS], axis=1))
-        else:
-            self.eng.commit_pod_rows(rows)
-
-    def commit_objects(self):
-        for c in OBJ_COLS:
-            np.copyto(self.views[c], self.snap.cols[c])
-        self.eng.commit(abi.PART_OBJECTS)
-
-    def check(self, oracle_mod, expect_incremental=None, device_only=False):
-        """One pass (device_only: kr_reconcile_device_only, then kr_results_fetch) compared with the oracle."""
-        if device_only:
-            self.eng.reconcile_device_only(self.flags)
-            got = self.eng.fetch()
-        else:
-            got = self.eng.reconcile(self.flags)
-        want = oracle_mod.run(self.snap, self.flags)
-        d = want.diff(got)
-        assert not d, (d[:6], got.n_changed)
-        inc = got.changed_clusters is not None or got.n_changed < self.snap.dims["clusters"]
-        if expect_incremental is not None:
-            assert inc == expect_incremental, (inc, got.n_changed)
-        if inc and self.prev is not None:
-            # records the pass did not name are unchanged since the previous epoch
-            ch = np.zeros(self.snap.dims["clusters"], dtype=bool)
-            if got.changed_clusters is not None:
-                ch[got.changed_clusters] = True
-            same = ~ch
-            assert np.array_equal(got.clusters[same], self.prev.clusters[same])
-            assert np.array_equal(got.act_cnt[same], self.prev.act_cnt[same])
-        self.prev = got
-        return got, inc
-
-    def close(self):
-        self.eng.close()
-
-
-def _flip_ready(snap, rows):
-    snap.cols["p_packed"][rows] ^= np.uint32(1 << abi.PP_READY_SHIFT)
-
-
-def _set_phase(snap, rows, phase):
-    pk = snap.cols["p_packed"]
-    pk[rows] = (pk[rows] & ~np.uint32(7 << abi.PP_PHASE_SHIFT)) | np.uint32(phase << abi.PP_PHASE_SHIFT)
-
 
 def _node_type(snap):
     return (snap.cols["p_packed"] >> abi.PP_NODE_TYPE_SHIFT) & 3
@@ -102,7 +34,7 @@ def test_pod_and_object_epochs_match_a_full_pass(seed, groups, jobs, oracle_mod)
             workers = np.nonzero((_node_type(snap) == abi.NT_WORKER) & ((snap.cols["p_packed"] & abi.PP_TOMBSTONE) == 0))[0].astype(np.uint32)
             # status updates
             upd = rng.choice(workers, 40, replace=False)
-            _flip_ready(snap, upd[:20]); _set_phase(snap, upd[20:30], 4); _set_phase(snap, upd[30:], 2)
+            flip_ready(snap, upd[:20]); set_phase(snap, upd[20:30], 4); set_phase(snap, upd[30:], 2)
             touched += upd.tolist()
             # additions into the rows freed one epoch earlier (the same pods come back, some under another RayCluster)
             for r in free.tolist():
@@ -125,7 +57,7 @@ def test_pod_and_object_epochs_match_a_full_pass(seed, groups, jobs, oracle_mod)
             # a head pod flips its phase (its cluster's head decisions change); head-aux rows keep their keys
             heads = np.nonzero(_node_type(snap) == abi.NT_HEAD)[0]
             h = rng.choice(heads, 3, replace=False)
-            _set_phase(snap, h[:1], 4); _flip_ready(snap, h[1:])
+            set_phase(snap, h[:1], 4); flip_ready(snap, h[1:])
             touched += h.tolist()
             if epoch % 2 == 0:  # object rows: replicas, expectation flags, old status, head-aux readiness
                 cs = rng.choice(nc, 8, replace=False)
@@ -142,7 +74,8 @@ def test_pod_and_object_epochs_match_a_full_pass(seed, groups, jobs, oracle_mod)
             elif epoch % 4 == 1:
                 dr.commit_objects()  # unchanged object rows: nothing may become dirty because of them
             dr.commit_rows(touched, journal=bool(epoch % 3))
-            got, inc = dr.check(oracle_mod)
+            got, _ = dr.check(oracle_mod)
+            inc = incremental(got, nc)
             n_inc += inc
             if inc:
                 assert 0 < got.n_changed < nc
@@ -157,7 +90,7 @@ def test_structural_changes_and_other_flags_take_the_full_pass(oracle_mod):
     try:
         dr.check(oracle_mod, expect_incremental=False)
         rows = np.arange(5, dtype=np.uint32)
-        _flip_ready(snap, rows)
+        flip_ready(snap, rows)
         dr.commit_rows(rows)
         dr.check(oracle_mod, expect_incremental=True)
         # a renamed worker group is a table key: the resident tables are stale
@@ -174,7 +107,7 @@ def test_structural_changes_and_other_flags_take_the_full_pass(oracle_mod):
         # different process-level flags: full pass, then incremental again under the new flags
         dr.flags.env_random_pod_delete = 1
         dr.check(oracle_mod, expect_incremental=False)
-        _flip_ready(snap, rows)
+        flip_ready(snap, rows)
         dr.commit_rows(rows, journal=False)
         dr.check(oracle_mod, expect_incremental=True)
         # asking for the full pod lists leaves the bucket pipeline (and the resident state) altogether
@@ -184,7 +117,7 @@ def test_structural_changes_and_other_flags_take_the_full_pass(oracle_mod):
         dr.flags.fetch_pod_lists = 0
         dr.check(oracle_mod, expect_incremental=False)
         # pod columns uploaded wholesale
-        _flip_ready(snap, rows)
+        flip_ready(snap, rows)
         for c in POD_COLS:
             np.copyto(dr.views[c], snap.cols[c])
         dr.eng.commit(abi.PART_COLUMNS)
@@ -201,15 +134,15 @@ def test_unfetched_passes_and_repeated_rows(oracle_mod):
         rng = np.random.default_rng(2)
         for it in range(3):  # passes whose results never reach the host, then one fetch: the host copy must still be complete
             rows = rng.choice(snap.dims["pods"], 30, replace=False).astype(np.uint32)
-            _flip_ready(snap, rows)
+            flip_ready(snap, rows)
             dr.commit_rows(rows[:20])
-            _set_phase(snap, rows[10:], 3)
+            set_phase(snap, rows[10:], 3)
             dr.commit_rows(rows[10:])      # rows 10..19 are committed twice before the pass
             dr.eng.reconcile_device_only(dr.flags)
         got = dr.eng.fetch()
         assert not oracle_mod.run(snap, dr.flags).diff(got)
         rows = rng.choice(snap.dims["pods"], 10, replace=False).astype(np.uint32)
-        _flip_ready(snap, rows)
+        flip_ready(snap, rows)
         dr.commit_rows(rows)
         dr.prev = None
         dr.check(oracle_mod, expect_incremental=True)
@@ -244,12 +177,11 @@ def test_appended_rows_and_head_rows_come_and_go(oracle_mod):
             snap2.cols[name][:] = a
         snap2.cols["p_name_id"][-3:] = np.uint32(0x7FFF0000) + np.arange(3, dtype=np.uint32)
         assert snap2.dims["heads"] == nh - 1 and snap2.dims["pods"] == snap.dims["pods"] + 3
-        dr.snap = snap2
-        dr.views = dr.eng.begin(snap2.sizes())
+        dr.use(snap2)
         dr.commit_objects()
         dr.commit_rows([p] + list(range(snap.dims["pods"], snap2.dims["pods"])))
-        got, inc = dr.check(oracle_mod)
-        assert inc, "appended rows / a removed head row must not force a full pass"
+        got, _ = dr.check(oracle_mod)
+        assert incremental(got, snap2.dims["clusters"]), "appended rows / a removed head row must not force a full pass"
         assert heads.size
     finally:
         dr.close()
@@ -283,9 +215,9 @@ def test_object_row_commits_equal_whole_object_commits(oracle_mod):
                 np.copyto(dr.views[c], snap.cols[c])
             dr.eng.commit_object_rows(cs, hs)
             rows = rng.choice(snap.dims["pods"], 15, replace=False).astype(np.uint32)
-            _flip_ready(snap, rows)
+            flip_ready(snap, rows)
             dr.commit_rows(rows)
-            got, inc = dr.check(oracle_mod, expect_incremental=True)
+            got, _ = dr.check(oracle_mod, expect_incremental=True)
             assert got.n_changed <= 9 + 4 + 15 + 1
             if epoch != 4:
                 assert dr.eng.last_profile()["h2d_bytes"] < 40000, dr.eng.last_profile()   # a few KB, not the 100+ KB object part

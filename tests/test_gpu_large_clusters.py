@@ -3,73 +3,26 @@
 Every pass is compared with the oracle and with the same snapshot run with the option off (the sort pipeline then decides it):
 Results.diff covers every result array except the run order inside the two arenas and pod_start, which only mean something when
 the full pod lists are fetched."""
-import collections
 import copy
+import functools
 
 import numpy as np
 import pytest
 
-import fuzz_objects
+from harness import (OBJ_COLS, PACKER_CAPS, SORT_KERNELS, Driver, Mirror, b32, compact, device_incremental, events, grown_fleet, head_row,
+                     members, most_workers, objects, packer_check, packer_stream, parity_on_off, run, scale_to, set_phase, spec_bytes, workers)
 from kuberay_b200 import abi, synthetic
 from kuberay_b200.engine import Engine
 from kuberay_b200.packer import Packer
 
-from test_gpu_incremental import OBJ_COLS, Driver
-from test_gpu_regimes import _b32, _spec
-from test_live_arena import _events
-from test_packer import Mirror, check as packer_check
-
 pytestmark = pytest.mark.gpu
 
-SORT_KERNELS = {"k_match", "k_place_fused", "k_decide_small", "k_decide"}
-
-
-def _compact(flags):
-    flags.fetch_pod_lists = 0
-    return flags
-
-
-def _members(snap, c):
-    return np.flatnonzero((snap.p_ns_id == snap.c_ns_id[c]) & (snap.p_cluster_name_id == snap.c_name_id[c]))
-
-
-def _fleet(size, n_clusters=300, seed=12):
-    """n_clusters RayClusters x 20 pods (the 64-pod stride, for up to 6 000 pods); worker pods of the others move into cluster 0
-    until it lists `size` pods."""
-    n_clusters = max(n_clusters, (size * 3 // 2) // 20 + 1)
-    snap, flags = synthetic.generate(synthetic.SynthParams(n_clusters=n_clusters, pods_per_cluster=20, groups=1, seed=seed))
-    synthetic.grow_clusters(snap, [0], size)
-    assert _members(snap, 0).size == size
-    return snap, _compact(flags)
-
-
-def _run(snap, flags, large, profiled=False, max_creates=1 << 16):
-    eng = Engine.for_snapshot(snap, large_clusters=large, max_creates=max_creates)  # (drained donor clusters ask for many pods)
-    try:
-        eng.load(snap)
-        names = [k for k, _ in eng.reconcile_profiled(flags)["kernels"]] if profiled else None
-        got = eng.reconcile(flags)
-        stride = eng.get_option(abi.OPT_BUCKET_STRIDE)
-    finally:
-        eng.close()
-    return got, names, stride
-
-
-def _parity(snap, flags, oracle_mod, **kw):
-    """Engine with the option on == oracle == engine with it off; returns (results, kernel names, stride) of the option-on run."""
-    on, names, stride = _run(snap, flags, True, profiled=True, **kw)
-    off, _, _ = _run(snap, flags, False, **kw)
-    want = oracle_mod.run(snap, flags)
-    d = want.diff(on)
-    assert not d, d[:6]
-    d = off.diff(on)
-    assert not d, d[:6]
-    return on, names, stride
+_parity = functools.partial(parity_on_off, option="large_clusters")
 
 
 @pytest.mark.parametrize("size", [257, 1000, 1024, 1025, 4096, 8192])
 def test_one_large_cluster_stays_on_the_bucket_pipeline(size, oracle_mod):
-    snap, flags = _fleet(size)
+    snap, flags = grown_fleet(size)
     got, names, stride = _parity(snap, flags, oracle_mod)
     assert got.clusters["n_pods"][0] == size
     assert {"k_match2", "k_decide2", "k_large_sort", "k_decide_large"} <= set(names), names
@@ -78,40 +31,22 @@ def test_one_large_cluster_stays_on_the_bucket_pipeline(size, oracle_mod):
 
 
 def test_past_the_largest_cluster_the_sort_pipeline_decides(oracle_mod):
-    snap, flags = _fleet(abi.LARGE_MAX_PODS + 1)
+    snap, flags = grown_fleet(abi.LARGE_MAX_PODS + 1)
     _, names, stride = _parity(snap, flags, oracle_mod)
     assert "k_match2" not in names and "k_decide_large" not in names and stride == 0
 
 
 def test_option_off_keeps_the_sort_pipeline(oracle_mod):
-    snap, flags = _fleet(257)
-    got, names, stride = _run(snap, flags, False, profiled=True)
+    snap, flags = grown_fleet(257)
+    got, names, stride = run(snap, flags, profiled=True, large_clusters=False)
     assert not oracle_mod.run(snap, flags).diff(got)
     assert "k_match2" not in names and "k_decide_large" not in names and stride == 0
 
 
 def test_more_than_32_worker_groups_still_take_the_sort_pipeline(oracle_mod):
     snap, flags = synthetic.generate(synthetic.SynthParams(n_clusters=200, pods_per_cluster=40, groups=33, seed=5))
-    _, names, _ = _parity(snap, _compact(flags), oracle_mod)
+    _, names, _ = _parity(snap, compact(flags), oracle_mod)
     assert "k_match2" not in names and "k_decide_large" not in names
-
-
-def _workers(snap, c):
-    m = _members(snap, c)
-    return m[((snap.p_packed[m] >> abi.PP_NODE_TYPE_SHIFT) & 3) == abi.NT_WORKER]
-
-
-def _set_phase(snap, rows, phase):
-    pk = snap.p_packed
-    pk[rows] = (pk[rows] & ~np.uint32(7 << abi.PP_PHASE_SHIFT)) | np.uint32(phase << abi.PP_PHASE_SHIFT)
-
-
-def _scale_to(snap, g, replicas):
-    snap.g_replicas[g] = replicas
-    snap.g_max[g] = 2 ** 31 - 1
-    snap.g_min[g] = 0
-    snap.g_flags[g] &= ~np.uint32(abi.GF_REPLICAS_NIL | abi.GF_MAX_NIL | abi.GF_MIN_NIL | abi.GF_SUSPEND)
-    snap.g_flags[g] |= np.uint32(abi.GF_EXPECT_OK)
 
 
 def _decision_fleet(seed, size=3000, n_large=3):
@@ -122,24 +57,24 @@ def _decision_fleet(seed, size=3000, n_large=3):
     for c in big:
         snap.c_flags[c] &= ~np.uint32(abi.CF_SKIP | abi.CF_SUSPEND | abi.CF_UPGRADE_RECREATE)
         snap.c_flags[c] |= np.uint32(abi.CF_HEAD_EXPECT_OK)
-        _scale_to(snap, int(snap.c_group_off[c]), _workers(snap, c).size)
-    return snap, _compact(flags), big
+        scale_to(snap, int(snap.c_group_off[c]), workers(snap, c).size)
+    return snap, compact(flags), big
 
 
 @pytest.mark.parametrize("random_delete", [False, True])
 def test_decisions_inside_large_clusters(random_delete, oracle_mod):
     snap, flags, (a, b, c) = _decision_fleet(3)
     flags.env_random_pod_delete = int(random_delete)
-    wa, wb, wc = _workers(snap, a), _workers(snap, b), _workers(snap, c)
+    wa, wb, wc = workers(snap, a), workers(snap, b), workers(snap, c)
     # a: unhealthy pods -> the group aborts after them
-    _set_phase(snap, wa[100:140], abi.PHASE_FAILED)
+    set_phase(snap, wa[100:140], abi.PHASE_FAILED)
     # b: scale down by 300 (a long delete prefix), autoscaling on so random delete matters
     snap.c_flags[b] |= np.uint32(abi.CF_AUTOSCALING)
-    _scale_to(snap, int(snap.c_group_off[b]), wb.size - 300)
+    scale_to(snap, int(snap.c_group_off[b]), wb.size - 300)
     # c: scale up across the replica-index windows at 1024 and 2048, labels on every pod
     snap.p_packed[wc] |= np.uint32(abi.PP_HAS_REPLICA_IDX)
     snap.p_replica_index[wc] = np.arange(wc.size, dtype=np.int32) * 2  # every even index in use
-    _scale_to(snap, int(snap.c_group_off[c]), wc.size + 1500)
+    scale_to(snap, int(snap.c_group_off[c]), wc.size + 1500)
     got, names, stride = _parity(snap, flags, oracle_mod, max_creates=1 << 16)
     assert "k_decide_large" in names and stride == 64
     assert got.groups["n_unhealthy"][snap.c_group_off[a]] == 40
@@ -151,7 +86,7 @@ def test_decisions_inside_large_clusters(random_delete, oracle_mod):
 def test_heads_and_suspend_inside_large_clusters(oracle_mod):
     snap, flags, (a, b, c) = _decision_fleet(4)
     # b: a second head
-    wb = _workers(snap, b)
+    wb = workers(snap, b)
     snap.p_packed[wb[7]] = (snap.p_packed[wb[7]] & ~np.uint32(3 << abi.PP_NODE_TYPE_SHIFT)) | np.uint32(abi.NT_HEAD << abi.PP_NODE_TYPE_SHIFT)
     # c: suspended worker group
     snap.g_flags[snap.c_group_off[c]] |= np.uint32(abi.GF_SUSPEND)
@@ -168,7 +103,7 @@ def test_heads_and_suspend_inside_large_clusters(oracle_mod):
 def test_several_large_clusters_keep_the_fleet_stride(oracle_mod):
     """The C3L shape at a tenth of its size: 20 RayClusters of 2 000 pods among 1 000 ordinary ones."""
     snap, flags = synthetic.generate(synthetic.config("C3L", n_clusters=1000))
-    _, names, stride = _parity(snap, _compact(flags), oracle_mod)
+    _, names, stride = _parity(snap, compact(flags), oracle_mod)
     assert "k_decide_large" in names and stride == 128  # (the stride of the mean cluster size, as without large clusters)
 
 
@@ -177,39 +112,33 @@ def test_multihost_group_inside_a_large_cluster(oracle_mod):
     synthetic.grow_clusters(snap, [0], 1200)
     for gate in (1, 0):
         flags.gate_multihost_indexing = gate
-        _, names, _ = _parity(snap, _compact(flags), oracle_mod)
+        _, names, _ = _parity(snap, compact(flags), oracle_mod)
         assert "k_decide_large" in names
 
 
 # ------------------------------------------------------------------------------------------------ incremental epochs
 
-class LargeDriver(Driver):
-    def __init__(self, snap, flags):
-        super().__init__(snap, flags, max_creates=1 << 16)
-        self.eng.set_large_clusters(True)
-
-
 def test_incremental_epochs_in_large_clusters(oracle_mod):
     snap, flags, big = _decision_fleet(6)
     rng = np.random.default_rng(3)
-    dr = LargeDriver(snap, flags)
+    dr = Driver(snap, flags, max_creates=1 << 16, large_clusters=True)
     try:
         dr.check(oracle_mod, expect_incremental=False)
         assert dr.eng.get_option(abi.OPT_BUCKET_STRIDE) == 64
         for epoch in range(6):
-            wa, wb = _workers(snap, big[0]), _workers(snap, big[1])
+            wa, wb = workers(snap, big[0]), workers(snap, big[1])
             rows = []
             # status flips in a large cluster
             flip = rng.choice(wa, 30, replace=False)
             snap.p_packed[flip] ^= np.uint32(1 << abi.PP_READY_SHIFT); rows += flip.tolist()
             fail = rng.choice(wb, 5, replace=False)
-            _set_phase(snap, fail, abi.PHASE_FAILED if epoch % 2 == 0 else abi.PHASE_RUNNING); rows += fail.tolist()
+            set_phase(snap, fail, abi.PHASE_FAILED if epoch % 2 == 0 else abi.PHASE_RUNNING); rows += fail.tolist()
             # pods moving between a large and an ordinary cluster, both ways
             small = int(rng.integers(600 // 2 + 1, 599))
             out = rng.choice(wa, 4, replace=False)
             snap.p_ns_id[out], snap.p_cluster_name_id[out] = snap.c_ns_id[small], snap.c_name_id[small]
             snap.p_group_name_id[out] = snap.g_name_id[snap.c_group_off[small]]
-            into = _workers(snap, small)[:2]
+            into = workers(snap, small)[:2]
             snap.p_ns_id[into], snap.p_cluster_name_id[into] = snap.c_ns_id[big[2]], snap.c_name_id[big[2]]
             snap.p_group_name_id[into] = snap.g_name_id[snap.c_group_off[big[2]]]
             rows += out.tolist() + into.tolist()
@@ -237,27 +166,27 @@ def test_incremental_epochs_in_large_clusters(oracle_mod):
 
 def test_a_large_cluster_outgrowing_its_region(oracle_mod):
     snap, flags, big = _decision_fleet(7, size=1000, n_large=1)
-    dr = LargeDriver(snap, flags)
+    dr = Driver(snap, flags, max_creates=1 << 16, large_clusters=True)
     try:
         dr.check(oracle_mod, expect_incremental=False)
         # its region holds about 1.25x: 400 more pods do not fit -> one full pass, then incremental again
-        donors = np.concatenate([_workers(snap, c) for c in range(300, 600)])[:400]
+        donors = np.concatenate([workers(snap, c) for c in range(300, 600)])[:400]
         snap.p_ns_id[donors], snap.p_cluster_name_id[donors] = snap.c_ns_id[big[0]], snap.c_name_id[big[0]]
         snap.p_group_name_id[donors] = snap.g_name_id[snap.c_group_off[big[0]]]
         dr.commit_rows(donors)
         dr.check(oracle_mod, expect_incremental=False)
-        flip = _workers(snap, big[0])[::50]
+        flip = workers(snap, big[0])[::50]
         snap.p_packed[flip] ^= np.uint32(1 << abi.PP_READY_SHIFT)
         dr.commit_rows(flip)
         dr.check(oracle_mod, expect_incremental=True)
         # an ordinary cluster crossing 256 pods: a full pass classifies it, then incremental again
-        donors = np.concatenate([_workers(snap, c) for c in range(100, 200)])[:300]
+        donors = np.concatenate([workers(snap, c) for c in range(100, 200)])[:300]
         snap.p_ns_id[donors], snap.p_cluster_name_id[donors] = snap.c_ns_id[50], snap.c_name_id[50]
         snap.p_group_name_id[donors] = snap.g_name_id[snap.c_group_off[50]]
         dr.commit_rows(donors)
         dr.check(oracle_mod, expect_incremental=False)
         assert dr.eng.get_option(abi.OPT_BUCKET_STRIDE) == 64
-        flip = _workers(snap, 50)[::10]
+        flip = workers(snap, 50)[::10]
         snap.p_packed[flip] ^= np.uint32(1 << abi.PP_READY_SHIFT)
         dr.commit_rows(flip)
         dr.check(oracle_mod, expect_incremental=True)
@@ -268,7 +197,7 @@ def test_a_large_cluster_outgrowing_its_region(oracle_mod):
 def test_turning_the_option_on_after_a_pass(oracle_mod):
     """A pass with the option off sends a fleet with a RayCluster of more than 1024 pods to the radix pipeline; turning the option
     on afterwards takes effect at the next pass (same snapshot, same sizes), and turning it off goes back."""
-    snap, flags = _fleet(2000)
+    snap, flags = grown_fleet(2000)
     want = oracle_mod.run(snap, flags)
     eng = Engine.for_snapshot(snap, max_creates=1 << 16)
     try:
@@ -286,12 +215,6 @@ def test_turning_the_option_on_after_a_pass(oracle_mod):
         eng.close()
 
 
-def _head_row(snap, c):
-    rows = np.flatnonzero(np.isin(snap.h_pod_idx, _members(snap, c)))
-    assert rows.size == 1
-    return int(rows[0])
-
-
 @pytest.mark.parametrize("spin", [True, False])
 def test_recreate_gate_inside_large_clusters(spin, oracle_mod, monkeypatch):
     """Recreate-gated large RayClusters: one whose annotation names another spec (every pod deleted), one whose annotation is the
@@ -305,15 +228,15 @@ def test_recreate_gate_inside_large_clusters(spin, oracle_mod, monkeypatch):
     for cl, match in ((a, False), (b, True)):
         assert snap.c_json_len[cl] > 8
         snap.c_flags[cl] |= np.uint32(abi.CF_UPGRADE_RECREATE)
-        h = _head_row(snap, cl)
+        h = head_row(snap, cl)
         snap.h_version_state[h] = abi.VER_CURRENT
         snap.h_annot_state[h] = abi.ANNOT_HASH32
-        digest = _b32(_spec(snap, cl)).encode()
+        digest = b32(spec_bytes(snap, cl))
         ah[h] = np.frombuffer(digest if match else digest[::-1], dtype=np.uint8)
     got, names, _ = _parity(snap, flags, oracle_mod)
     assert "k_decide_large" in names
     assert got.clusters["path"][a] == abi.PATH_RECREATE_DELETE_ALL and got.clusters["path"][b] == abi.PATH_NORMAL
-    dr = LargeDriver(snap, flags)
+    dr = Driver(snap, flags, max_creates=1 << 16, large_clusters=True)
     try:
         dr.check(oracle_mod, expect_incremental=False)
         p = int(snap.c_json_off[b]) + 3
@@ -332,22 +255,22 @@ def test_workers_to_delete_inside_large_clusters(random_delete, oracle_mod):
     other RayClusters and names no pod carries."""
     snap, flags = synthetic.generate(synthetic.SynthParams(n_clusters=600, pods_per_cluster=20, groups=1, autoscaling_frac=1.0,
                                                            wtd_group_frac=1.0, seed=21))
-    flags = _compact(flags)
+    flags = compact(flags)
     flags.env_random_pod_delete = int(random_delete)
     cand = [c for c in range(300, 600) if snap.g_wtd_cnt[snap.c_group_off[c]] >= 2]
     big = cand[:2]
     synthetic.grow_clusters(snap, big, 1500)
     for c in big:
-        m = _members(snap, c)
-        _set_phase(snap, m, abi.PHASE_RUNNING)
+        m = members(snap, c)
+        set_phase(snap, m, abi.PHASE_RUNNING)
         snap.p_packed[m] &= ~np.uint32(abi.PP_RAY_TERMINATED)
         snap.c_flags[c] &= ~np.uint32(abi.CF_SKIP | abi.CF_SUSPEND | abi.CF_UPGRADE_RECREATE)
         snap.c_flags[c] |= np.uint32(abi.CF_HEAD_EXPECT_OK | abi.CF_AUTOSCALING)
         g = int(snap.c_group_off[c])
-        w = _workers(snap, c)
-        _scale_to(snap, g, w.size - 5)
+        w = workers(snap, c)
+        scale_to(snap, g, w.size - 5)
         off, cnt = int(snap.g_wtd_off[g]), int(snap.g_wtd_cnt[g])
-        other = snap.p_name_id[_workers(snap, c + 1)[0]]  # a pod of another RayCluster of the namespace
+        other = snap.p_name_id[workers(snap, c + 1)[0]]  # a pod of another RayCluster of the namespace
         snap.w_name_id[off:off + cnt] = [snap.p_name_id[w[-1]], np.uint32(0x7F000000 + c)] + [other] * (cnt - 2)
     got, names, _ = _parity(snap, flags, oracle_mod)
     assert "k_decide_large" in names
@@ -364,20 +287,14 @@ def test_native_packer_keeps_incremental_epochs_with_large_clusters(oracle_mod):
     """A fleet with a RayCluster of 600 pods behind the native packer, KR_OPT_LARGE_CLUSTERS set through kr_packer_engine: every
     epoch equals the oracle and the pod-row epochs (KR_PACK_POD_ROWS) stay incremental on the device."""
     rng = np.random.default_rng(31)
-    clusters, pods, jobs = fuzz_objects.generate(5, max_clusters=16)
-    for i, c in enumerate(clusters):
-        c["generation"], c["resourceVersion"] = 1, 100 + i
-    for i, j in enumerate(jobs):
-        j.setdefault("name", f"rayjob-{i}")
-    owner = collections.Counter((p.get("namespace"), p["labels"].get("ray.io/cluster")) for p in pods
-                                if p["labels"].get("ray.io/node-type") == "worker").most_common(1)[0][0]
+    clusters, pods, jobs = objects(5, max_clusters=16)
+    owner = most_workers(pods)
     src = [p for p in pods if (p.get("namespace"), p["labels"].get("ray.io/cluster")) == owner and p["labels"].get("ray.io/node-type") == "worker"]
     for i in range(600 - len(src)):
         q = copy.deepcopy(src[i % len(src)])
         q["name"] = f"{q['name']}-big-{i}"
         pods.append(q)
-    pk = Packer(max_clusters=64, max_groups=512, max_wtd=512, max_pods=4096, max_heads=256, max_jobs=64, max_creates=1 << 16,
-                max_json_bytes=4 << 20, large_clusters=True)
+    pk = Packer(**PACKER_CAPS, large_clusters=True)
     try:
         m = Mirror(copy.deepcopy(clusters), copy.deepcopy(pods), jobs, pk)
         pk.flush()
@@ -385,12 +302,8 @@ def test_native_packer_keeps_incremental_epochs_with_large_clusters(oracle_mod):
         assert int(first.clusters["n_pods"].max()) >= 600
         assert pk.engine.get_option(abi.OPT_LARGE_CLUSTERS) == 1 and pk.engine.get_option(abi.OPT_BUCKET_STRIDE) != 0
         counter = [0]
-        incremental, modes = [], []
-        for _ in range(10):
-            _events(rng, m, counter, structural=False)
-            modes.append(pk.flush())
-            _, got = packer_check(m, oracle_mod, lean=True)
-            incremental.append(got.changed_clusters is not None or got.n_changed == 0)
+        gots, modes = packer_stream(m, oracle_mod, 10, lambda epoch: events(rng, m, counter, structural=False))
+        incremental = [device_incremental(g) for g in gots]
         assert any(mo & abi.PACK_POD_ROWS for mo in modes)
         assert incremental[0] and sum(incremental) >= 5, incremental
     finally:

@@ -6,13 +6,10 @@ import copy
 import numpy as np
 import pytest
 
-import fuzz_objects
+from harness import (OBJ_COLS, PACKER_CAPS, POD_COLS, Driver, Mirror, compact, device_incremental, events, flip_ready, kernels, objects,
+                     packer_check, packer_stream, parity, set_phase)
 from kuberay_b200 import abi, synthetic
 from kuberay_b200.packer import Packer
-from test_gpu_incremental import OBJ_COLS, POD_COLS, Driver, _flip_ready, _set_phase
-from test_gpu_parity import _compact, _kernels, _parity
-from test_live_arena import _events
-from test_packer import Mirror, check as packer_check
 
 pytestmark = pytest.mark.gpu
 
@@ -34,7 +31,7 @@ def _mh_snapshot(seed, **kw):
     names, inv, cnt = np.unique(rn, return_inverse=True, return_counts=True)
     spare = np.flatnonzero((rn != 0) & (cnt[inv] < 4))
     rn[spare] = 0
-    _set_phase(snap, spare[rng.random(spare.size) < 0.3], abi.PHASE_FAILED)
+    set_phase(snap, spare[rng.random(spare.size) < 0.3], abi.PHASE_FAILED)
     named = names[names != 0]
     rn[np.isin(rn, named[rng.random(named.size) < 0.2])] = abi.ID_EMPTY_STRING
     split = np.flatnonzero(rn > 1)
@@ -46,9 +43,9 @@ def _mh_snapshot(seed, **kw):
 def test_multihost_snapshot_takes_the_bucket_pipeline(oracle_mod):
     snap, flags = synthetic.generate(synthetic.SynthParams(n_clusters=400, pods_per_cluster=41, groups=2, multihost_frac=0.5))
     assert flags.gate_multihost_indexing == 1 and (snap.g_num_hosts > 1).any()
-    names = _kernels(snap, _compact(flags))
+    names = kernels(snap, compact(flags))
     assert _bucket_only(names), names
-    got = _parity(snap, flags, oracle_mod)
+    got = parity(snap, flags, oracle_mod)
     assert (got.groups["flags"] & abi.GR_MULTIHOST).any()
 
 
@@ -61,10 +58,10 @@ def test_multihost_branch_matches_the_oracle_across_flags(oracle_mod):
     for (snap, flags), gate, rdel in runs:
         f = abi.kr_flags.from_buffer_copy(flags)
         f.gate_multihost_indexing, f.env_random_pod_delete = gate, rdel
-        got = _parity(snap, f, oracle_mod)
+        got = parity(snap, f, oracle_mod)
         acts = set(np.unique(got.sorted_action).tolist())
         if gate:
-            assert _bucket_only(_kernels(snap, _compact(f)))
+            assert _bucket_only(kernels(snap, compact(f)))
             seen |= acts & MH_ACTS
             assert (got.groups["flags"] & abi.GR_MULTIHOST).any()
         else:
@@ -109,7 +106,7 @@ def test_incremental_epochs_with_multihost_groups(oracle_mod):
 
         # 1. status flips inside replicas
         rows = [p for g in groups[:40] for p in replica(g)[:2]]
-        _flip_ready(snap, rows[::2]); _set_phase(snap, rows[1::2], abi.PHASE_PENDING)
+        flip_ready(snap, rows[::2]); set_phase(snap, rows[1::2], abi.PHASE_PENDING)
         dr.commit_rows(rows)
         dr.check(oracle_mod, expect_incremental=True)
         # 2. a replica loses a pod (deleted: a free row) -> incomplete
@@ -122,7 +119,7 @@ def test_incremental_epochs_with_multihost_groups(oracle_mod):
         dr.check(oracle_mod, expect_incremental=True)
         # 3. an unhealthy pod deletes its whole replica
         bad = [replica(next(pick))[2] for _ in range(6)]
-        _set_phase(snap, bad, abi.PHASE_FAILED)
+        set_phase(snap, bad, abi.PHASE_FAILED)
         dr.commit_rows(bad)
         dr.check(oracle_mod, expect_incremental=True)
         # 4. a pod's replica-name label rewritten (one replica short, another one pod over)
@@ -218,24 +215,16 @@ def test_native_packer_keeps_incremental_epochs_with_multihost_groups(seed, orac
     """A fleet with multi-host worker groups behind the native packer: every epoch equals the oracle, and after the first one the
     passes are incremental on the device (the results name the RayClusters they recomputed)."""
     rng = np.random.default_rng(seed)
-    clusters, pods, jobs = fuzz_objects.generate(seed, max_clusters=16)
-    for i, c in enumerate(clusters):
-        c["generation"], c["resourceVersion"] = 1, 100 + i
-    for i, j in enumerate(jobs):
-        j.setdefault("name", f"rayjob-{i}")
+    clusters, pods, jobs = objects(seed, max_clusters=16)
     assert any(g["numOfHosts"] > 1 for c in clusters for g in c["spec"]["workerGroupSpecs"])
-    pk = Packer(max_clusters=64, max_groups=512, max_wtd=512, max_pods=4096, max_heads=256, max_jobs=64, max_creates=1 << 16, max_json_bytes=4 << 20)
+    pk = Packer(**PACKER_CAPS)
     try:
         m = Mirror(copy.deepcopy(clusters), copy.deepcopy(pods), jobs, pk)
         pk.flush()
         packer_check(m, oracle_mod, lean=True)
         counter = [0]
-        incremental = []
-        for epoch in range(10):
-            _events(rng, m, counter, structural=False)
-            pk.flush()
-            _, got = packer_check(m, oracle_mod, lean=True)
-            incremental.append(got.changed_clusters is not None or got.n_changed == 0)
+        gots, _ = packer_stream(m, oracle_mod, 10, lambda epoch: events(rng, m, counter, structural=False))
+        incremental = [device_incremental(g) for g in gots]
         # (an epoch may still take the full pass for a reason of its own — e.g. a small fleet's action list filling up with the
         # abandoned runs of re-decided clusters is packed again by a full pass)
         assert incremental[0] and sum(incremental) >= 5, incremental

@@ -4,7 +4,7 @@ changes shape, RayCluster deletion (the last row moves into the hole) and an are
 
 A compaction re-places every RayCluster's blob, so every c_json_off moves, while the epoch's object rows may still go row by row
 (kr_snapshot_commit_object_rows of the edited RayClusters only).  Every epoch is checked against the oracle on an independently
-packed snapshot (test_packer.check, digests included) and directly: each RayCluster's digest must be the base32hex SHA-1 of its
+packed snapshot (packer_check, digests included) and directly: each RayCluster's digest must be the base32hex SHA-1 of its
 current specJson (passed verbatim, so sizes are exact), and the Recreate-gated RayClusters, whose head Pods carry the digest of their
 spec and which are never edited, must stay on PATH_NORMAL: a digest computed from a stale range would delete all their Pods."""
 import copy
@@ -12,13 +12,11 @@ import copy
 import numpy as np
 import pytest
 
+from harness import L_CLUSTER, L_GROUP, L_TYPE, Mirror, b32, packer_check, spec_bytes
 from kuberay_b200 import abi, synthetic
 from kuberay_b200 import snapshot as snp
 from kuberay_b200.engine import Engine, EngineError
 from kuberay_b200.packer import Packer
-from test_gpu_spec_rows import _recreate_rows, digest
-from test_live_arena import L_CLUSTER, L_GROUP, L_TYPE
-from test_packer import Mirror, check as packer_check
 
 pytestmark = pytest.mark.gpu
 
@@ -35,7 +33,7 @@ def _body(rng, n: int) -> bytes:
 
 def _head(name, body: bytes, head_no=0):
     return {"namespace": NS, "name": f"{name}-head{head_no or ''}", "labels": {L_CLUSTER: name, L_TYPE: "head", L_GROUP: "headgroup"},
-            "annotations": {snp.RECREATE_HASH_ANNOT: digest(body).decode(), snp.KUBERAY_VERSION_ANNOT: snp.KUBERAY_VERSION},
+            "annotations": {snp.RECREATE_HASH_ANNOT: b32(body).decode(), snp.KUBERAY_VERSION_ANNOT: snp.KUBERAY_VERSION},
             "phase": "Running", "conditions": [{"type": "Ready", "status": "True"}], "podIP": "10.1.0.1", "restartPolicy": "Always"}
 
 
@@ -97,12 +95,12 @@ def _offsets(m):
 
 
 def _verify(m, oracle_mod):
-    """Every digest against its specJson and every gated RayCluster on PATH_NORMAL, then test_packer.check (the same pass again:
+    """Every digest against its specJson and every gated RayCluster on PATH_NORMAL, then packer_check (the same pass again:
     an epoch without commits)."""
     got = m.pk.engine.reconcile(m.pk.flags(fetch_pod_lists=0))
     for key, c in m.clusters.items():
         r = m.pk.cluster_row(*key)
-        assert bytes(got.hash[r]) == digest(c["specJson"]), (key, r)
+        assert bytes(got.hash[r]) == b32(c["specJson"]), (key, r)
     for key in _gated(m):
         assert got.clusters["path"][m.pk.cluster_row(*key)] == abi.PATH_NORMAL, key
     _, got = packer_check(m, oracle_mod, lean=True)
@@ -303,11 +301,11 @@ def test_json_only_commit_then_object_rows(oracle_mod):
         assert not oracle_mod.run(snap, flags).diff(first)
         s = snap
         nc = s.dims["clusters"]
-        body = lambda c: s.json[int(s.c_json_off[c]):int(s.c_json_off[c]) + int(s.c_json_len[c])].tobytes()  # noqa: E731
+        body = lambda c: spec_bytes(s, c)  # noqa: E731
         head_of = {(int(s.p_ns_id[p]), int(s.p_cluster_name_id[p])): h for h, p in enumerate(s.h_pod_idx.tolist())}
         ann = s.h_annot_hash.reshape(-1, 32)
-        gated = [c for c in _recreate_rows(s) if first.clusters["path"][c] == abi.PATH_NORMAL and
-                 (int(s.c_ns_id[c]), int(s.c_name_id[c])) in head_of and bytes(ann[head_of[(int(s.c_ns_id[c]), int(s.c_name_id[c]))]]) == digest(body(c))]
+        gated = [c for c in range(nc) if s.c_flags[c] & abi.CF_UPGRADE_RECREATE and first.clusters["path"][c] == abi.PATH_NORMAL and
+                 (int(s.c_ns_id[c]), int(s.c_name_id[c])) in head_of and bytes(ann[head_of[(int(s.c_ns_id[c]), int(s.c_name_id[c]))]]) == b32(body(c))]
         assert gated
         plain = [c for c in range(nc) if not s.c_flags[c] & abi.CF_UPGRADE_RECREATE]
         # 1. every range moves: the blobs laid out again starting from RayCluster 1, RayCluster 0 last
@@ -333,7 +331,7 @@ def test_json_only_commit_then_object_rows(oracle_mod):
         d = oracle_mod.run(s, flags).diff(got)
         assert not d, d[:6]
         for r in range(nc):
-            assert bytes(got.hash[r]) == digest(blobs[r]), r
+            assert bytes(got.hash[r]) == b32(blobs[r]), r
         assert (got.clusters["path"][gated] == abi.PATH_NORMAL).all()
         # 2. the ordinary spec edit: one range moves (shorter, same offset), the row commit lists its RayCluster
         c = plain[1]
@@ -352,7 +350,7 @@ def test_json_only_commit_then_object_rows(oracle_mod):
         got = eng.reconcile(flags)
         d = oracle_mod.run(s, flags).diff(got)
         assert not d, d[:6]
-        assert bytes(got.hash[c]) == digest(body(c))
+        assert bytes(got.hash[c]) == b32(body(c))
         assert (got.clusters["path"][gated] == abi.PATH_NORMAL).all()
     finally:
         eng.close()

@@ -3,8 +3,8 @@ _HUGE_CLUSTERS, _WTD_EDITS, _SPEC_ROWS), against a twin packer with all of them 
 
 The fleet: about 150 RayClusters cloned from fuzz objects (multi-host groups, Recreate gates, RayJobs, every adversarial field),
 plus healthy RayClusters of about 1 500 and 8 190 Pods, one of 9 000 Pods, three of 33-40 worker groups, one of 250 Pods and one of
-32 worker groups.  Each epoch mixes Pod traffic and RayCluster status (test_live_arena._events), autoscaler workersToDelete edits
-(test_gpu_wtd_edits._autoscale_objects) and spec edits with a bumped generation (test_gpu_spec_rows._spec_edits); some epochs also
+32 worker groups.  Each epoch mixes Pod traffic and RayCluster status (harness.events), autoscaler workersToDelete edits
+(harness.autoscale_objects) and spec edits with a bumped generation (harness.spec_edits); some epochs also
 move a RayCluster across a class boundary (256 -> 257 Pods, 8 192 -> 8 193 Pods, 32 -> 33 worker groups, and back), create or delete
 a RayCluster and a RayJob, and the JSON arena is small enough to be compacted a few times per stream.
 
@@ -19,14 +19,10 @@ import json
 import numpy as np
 import pytest
 
+from harness import L_CLUSTER, L_GROUP, L_TYPE, Mirror, autoscale_objects, events, huge_objects, packer_check, spec_edits
 from kuberay_b200 import abi
 from kuberay_b200.engine import spec_json_emit
 from kuberay_b200.packer import Packer
-from test_gpu_huge_clusters import _huge_objects
-from test_gpu_spec_rows import _spec_edits
-from test_gpu_wtd_edits import _autoscale_objects
-from test_live_arena import L_CLUSTER, L_GROUP, L_TYPE, _events
-from test_packer import Mirror, check as packer_check
 
 pytestmark = pytest.mark.gpu
 
@@ -64,7 +60,7 @@ BIG = {  # name -> worker groups
 
 
 def _fleet(seed):
-    clusters, pods, jobs = _huge_objects(seed, 0, n_clusters=150)
+    clusters, pods, jobs = huge_objects(seed, 0, n_clusters=150)
     for i, (name, groups) in enumerate(BIG.items()):
         c, p = _healthy(name, groups, i)
         clusters.append(c)
@@ -86,7 +82,7 @@ EDGE = ("edge256", "edge8192", "edge32")  # (their sizes move only in _class_mov
 
 class _Side:
     """The Mirror as the shared event generators see it, without the RayCluster objects `clusters_out` and the Pods of
-    `pods_out`: test_live_arena._events would set a big RayCluster's replicas to 0-6 (thousands of deletes on one RayCluster are
+    `pods_out`: harness.events would set a big RayCluster's replicas to 0-6 (thousands of deletes on one RayCluster are
     not the traffic this stream is about), and random Pod traffic would move the edge RayClusters across their boundaries."""
 
     def __init__(self, m, clusters_out, pods_out):
@@ -214,9 +210,9 @@ def test_all_options_on_against_all_off(seed, oracle_mod):
             for i, (pk, m) in enumerate(zip(pks, ms)):
                 r = np.random.default_rng(1000 * seed + epoch)  # the same events on both sides
                 before = _offsets(m)
-                _spec_edits(r, m, gens[i], int(r.integers(1, 4)))
-                _autoscale_objects(r, _Side(m, EDGE, EDGE), pendings[i])
-                _events(r, _Side(m, BIG, EDGE), counters[i], structural=False)
+                spec_edits(r, m, gens[i], int(r.integers(1, 4)))
+                autoscale_objects(r, _Side(m, EDGE, EDGE), pendings[i])
+                events(r, _Side(m, BIG, EDGE), counters[i], structural=False)
                 move = _class_moves(m, epoch)
                 mode = pk.flush()
                 after = _offsets(m)

@@ -2,147 +2,107 @@
 import numpy as np
 import pytest
 
+from harness import b32, compact, kernels, parity
 from kuberay_b200 import abi, synthetic
 from kuberay_b200.engine import Engine
 
 pytestmark = pytest.mark.gpu
 
 
-def _compact(flags):
-    """The same switches with kr_flags.fetch_pod_lists = 0: the pass takes the bucket pipeline (kr_bucket2.cuh) when the snapshot
-    qualifies and the sort / radix pipeline otherwise; only the compact results come back."""
-    f = abi.kr_flags.from_buffer_copy(flags)
-    f.fetch_pod_lists = 0
-    return f
-
-
-def _parity(snap, flags, oracle_mod, both=False, **kw):
-    """Engine vs oracle, twice: with the full pod lists (sort / radix pipeline) and without (bucket pipeline).
-    -> the first run's results, or both runs' with `both`."""
-    eng = Engine.for_snapshot(snap, **kw)
-    try:
-        eng.load(snap)
-        got = eng.reconcile(flags)
-        lean = eng.reconcile(_compact(flags))
-    finally:
-        eng.close()
-    want = oracle_mod.run(snap, flags, threads=8)
-    d = want.diff(got)
-    assert not d, "\n".join(d[:20])
-    d = want.diff(lean)
-    assert not d, "compact results (fetch_pod_lists = 0):\n" + "\n".join(d[:20])
-    assert lean.sorted_pod_idx.size == 0
-    return (got, lean) if both else got
-
-
-def _kernels(snap, flags):
-    eng = Engine.for_snapshot(snap)
-    try:
-        eng.load(snap)
-        return [k for k, _ in eng.reconcile_profiled(flags)["kernels"]]
-    finally:
-        eng.close()
-
-
 @pytest.mark.parametrize("cfg", ["C1", "C2"])
 def test_parity_small_configs(cfg, oracle_mod):
     snap, flags = synthetic.generate(synthetic.config(cfg))
-    _parity(snap, flags, oracle_mod)
+    parity(snap, flags, oracle_mod)
 
 
 def test_parity_c3_headline(oracle_mod):
     snap, flags = synthetic.generate(synthetic.config("C3"))
-    got = _parity(snap, flags, oracle_mod)
+    got = parity(snap, flags, oracle_mod)
     assert got.n_actions > 0 and got.n_create_total > 0
 
 
 def test_parity_multi_group(oracle_mod):
     snap, flags = synthetic.generate(synthetic.config("C2", groups=3, pods_per_cluster=40))
-    _parity(snap, flags, oracle_mod)
+    parity(snap, flags, oracle_mod)
 
 
 def test_parity_many_groups_spill(oracle_mod):
     # > 32 worker groups per cluster: accumulators spill from shared memory to global scratch
     snap, flags = synthetic.generate(synthetic.SynthParams(n_clusters=50, pods_per_cluster=200, groups=40))
-    _parity(snap, flags, oracle_mod)
+    parity(snap, flags, oracle_mod)
 
 
 def test_parity_multihost_groups(oracle_mod, monkeypatch):
     # numOfHosts=4 groups with replica-name labels, incomplete / unhealthy / scale-down replicas in the mix
     params = synthetic.SynthParams(n_clusters=400, pods_per_cluster=41, groups=2, multihost_frac=0.5)
     snap, flags = synthetic.generate(params)
-    got = _parity(snap, flags, oracle_mod)
+    got = parity(snap, flags, oracle_mod)
     acts = set(np.unique(got.sorted_action).tolist())
     assert {abi.ACT_DELETE_MH_UNHEALTHY, abi.ACT_DELETE_MH_INCOMPLETE} & acts
     assert (got.groups["flags"] & abi.GR_MULTIHOST).any()
     monkeypatch.setenv("KR_FORCE_RADIX", "1")
-    _parity(snap, flags, oracle_mod)
+    parity(snap, flags, oracle_mod)
 
 
 def test_parity_flag_variants(oracle_mod):
     snap, flags = synthetic.generate(synthetic.config("C2"))
     for kw in (dict(env_random_pod_delete=1), dict(gate_status_conditions=0), dict(gate_multihost_indexing=0)):
         f = abi.default_flags(id_head_not_found_reason=flags.id_head_not_found_reason, id_head_not_found_msg=flags.id_head_not_found_msg, **kw)
-        _parity(snap, f, oracle_mod)
+        parity(snap, f, oracle_mod)
 
 
 def test_parity_big_bucket_falls_back_to_radix(oracle_mod):
     # one RayCluster with 3000 pods: the fast pipeline's in-warp sort takes <= 1024 per bucket, the engine must switch
     # to the radix pipeline by itself and still be bit-exact
     snap, flags = synthetic.generate(synthetic.SynthParams(n_clusters=20, pods_per_cluster=3000, groups=2))
-    _parity(snap, flags, oracle_mod)
+    parity(snap, flags, oracle_mod)
 
 
 def test_many_orphans_stay_on_the_fast_pipeline(oracle_mod):
     # 20 % of the pods name a RayCluster that is not in the snapshot: the orphan bucket (5000 pods) is ordered without a sort
     snap, flags = synthetic.generate(synthetic.SynthParams(n_clusters=500, pods_per_cluster=50, groups=1, orphan_frac=0.2))
-    got = _parity(snap, flags, oracle_mod)
+    got = parity(snap, flags, oracle_mod)
     assert got.n_orphans == 5000
-    eng = Engine.for_snapshot(snap)
-    try:
-        eng.load(snap)
-        names = [k for k, _ in eng.reconcile_profiled(flags)["kernels"]]
-    finally:
-        eng.close()
+    names = kernels(snap, flags)
     assert any(k.startswith("k_place") for k in names) and "k_scatter" not in names
 
 
 def test_parity_radix_pipeline_forced(oracle_mod, monkeypatch):
     monkeypatch.setenv("KR_FORCE_RADIX", "1")
     snap, flags = synthetic.generate(synthetic.config("C2", groups=2))
-    _parity(snap, flags, oracle_mod)
+    parity(snap, flags, oracle_mod)
     snap, flags = synthetic.generate(synthetic.config("C3"))
-    _parity(snap, flags, oracle_mod)
+    parity(snap, flags, oracle_mod)
 
 
 @pytest.mark.parametrize("ppc", [1, 2, 33, 41, 63, 64, 65, 127])
 def test_parity_odd_cluster_sizes_both_pipelines(ppc, oracle_mod, monkeypatch):
     params = synthetic.SynthParams(n_clusters=257, pods_per_cluster=ppc, groups=1)
     snap, flags = synthetic.generate(params)
-    _parity(snap, flags, oracle_mod)
+    parity(snap, flags, oracle_mod)
     monkeypatch.setenv("KR_FORCE_RADIX", "1")
-    _parity(snap, flags, oracle_mod)
+    parity(snap, flags, oracle_mod)
 
 
 def test_parity_unfused_scan_kernels(oracle_mod, monkeypatch):
     # large snapshots use separate chained-scan kernels instead of the shared-memory fused ones: force that path
     monkeypatch.setenv("KR_NO_FUSE", "1")
     snap, flags = synthetic.generate(synthetic.config("C2", groups=2, orphan_frac=0.05))
-    _parity(snap, flags, oracle_mod)
+    parity(snap, flags, oracle_mod)
     snap, flags = synthetic.generate(synthetic.config("C3"))
-    _parity(snap, flags, oracle_mod)
+    parity(snap, flags, oracle_mod)
 
 
 def test_parity_rayjob_rollup_c4(oracle_mod):
     snap, flags = synthetic.generate(synthetic.config("C4"))
-    got = _parity(snap, flags, oracle_mod)
+    got = parity(snap, flags, oracle_mod)
     assert got.jobs["status_changed"].sum() > 0 and (got.jobs["cluster_idx"] < 0).sum() > 0
 
 
 def test_parity_without_cuda_graph(oracle_mod, monkeypatch):
     monkeypatch.setenv("KR_NO_GRAPH", "1")
     snap, flags = synthetic.generate(synthetic.config("C2"))
-    _parity(snap, flags, oracle_mod)
+    parity(snap, flags, oracle_mod)
 
 
 def test_repeated_passes_are_identical(oracle_mod):
@@ -234,9 +194,9 @@ def test_bucket_pipeline_is_taken_and_widens_its_stride(oracle_mod):
     larger than the first stride voids the attempt: the engine widens the stride (64 -> 128 -> 256), then leaves for the sort
     pipeline (here: a 300-pod cluster), every time bit-exact."""
     snap, flags = synthetic.generate(synthetic.config("C3"))
-    names = _kernels(snap, _compact(flags))
+    names = kernels(snap, compact(flags))
     assert {"k_match2", "k_decide2", "k_hash"} <= set(names) and not any(k.startswith(("k_place", "k_creates", "k_decide_small")) for k in names)
-    names = _kernels(snap, flags)
+    names = kernels(snap, flags)
     assert "k_match2" not in names and "k_decide_small" in names
     for big in (100, 200, 300):
         # 300 RayClusters x 20 pods; the pods of clusters 1 .. k are relabelled into cluster 0 (same namespace), which then
@@ -245,8 +205,8 @@ def test_bucket_pipeline_is_taken_and_widens_its_stride(oracle_mod):
         k = big // 20 - 1
         moved = np.isin(both.p_cluster_name_id, both.c_name_id[1:k + 1])
         both.p_cluster_name_id[moved] = both.c_name_id[0]
-        _parity(both, f, oracle_mod)
-        names = _kernels(both, _compact(f))   # (a fresh engine starts at the narrow stride again and ends where the ladder ends)
+        parity(both, f, oracle_mod)
+        names = kernels(both, compact(f))   # (a fresh engine starts at the narrow stride again and ends where the ladder ends)
         assert ("k_match2" in names) == (big <= 256), (big, names)
 
 
@@ -261,13 +221,11 @@ def test_bucket_pipeline_long_delete_prefix_and_delete_all(oracle_mod):
     snap.g_min[shrink] = 0
     snap.g_flags[shrink] &= ~np.uint32(abi.GF_REPLICAS_NIL | abi.GF_MIN_NIL)
     flags.env_random_pod_delete = 1
-    got = _parity(snap, flags, oracle_mod)
+    got = parity(snap, flags, oracle_mod)
     assert (got.groups["diff"] < -8).sum() > 50 and (got.clusters["path"] == abi.PATH_RECREATE_DELETE_ALL).sum() > 5
 
 
 def test_hash_batch_matches_hashlib():
-    import base64
-    import hashlib
     rng = np.random.default_rng(1)
     msgs = [b"", b"abc", b"a" * 55, b"a" * 56, b"a" * 63, b"a" * 64, b"a" * 65, b"a" * 119, b"a" * 120, b"a" * 127, b"a" * 128]
     msgs += [rng.integers(0, 256, int(n), dtype=np.uint8).tobytes() for n in rng.integers(0, 9000, 300)]
@@ -276,7 +234,7 @@ def test_hash_batch_matches_hashlib():
         got = eng.hash_batch(msgs)
     finally:
         eng.close()
-    want = [base64.b32hexencode(hashlib.sha1(m).digest()).decode() for m in msgs]
+    want = [b32(m).decode() for m in msgs]
     assert got == want
     from oracle import oracle as _oracle
     assert got[:40] == [_oracle.hash32(m) for m in msgs[:40]]      # and the oracle's own SHA-1 / base32hex (kr_oracle_hash32) agrees with both
@@ -285,8 +243,6 @@ def test_hash_batch_matches_hashlib():
 def test_hash_batch_and_passes_share_an_engine(oracle_mod):
     """kr_hash_batch (the RayService callers' entry point) between passes of the same engine: its staging buffers grow
     without disturbing the pass's own pinned buffers (a stray free there once corrupted the totals record)."""
-    import base64
-    import hashlib
     snap, flags = synthetic.generate(synthetic.config("C2"))
     eng = Engine.for_snapshot(snap)
     try:
@@ -294,7 +250,7 @@ def test_hash_batch_and_passes_share_an_engine(oracle_mod):
         want = oracle_mod.run(snap, flags, threads=8)
         for size in (10, 1000, 40000):
             msgs = [bytes([i % 251]) * (i % 700) for i in range(size // 10)]
-            assert eng.hash_batch(msgs) == [base64.b32hexencode(hashlib.sha1(m).digest()).decode() for m in msgs]
+            assert eng.hash_batch(msgs) == [b32(m).decode() for m in msgs]
             assert not want.diff(eng.reconcile(flags)), size
     finally:
         eng.close()
@@ -365,7 +321,7 @@ def test_fuzz_adversarial_snapshots(seed0, arm, oracle_mod, monkeypatch):
                 continue
             snap, grown = case
             cases += 1
-            flags = _compact(flags)
+            flags = compact(flags)
             want = oracle_mod.run(snap, flags, threads=1)
             runs = []
             for on in (True, False):
@@ -395,7 +351,7 @@ def test_fuzz_adversarial_snapshots(seed0, arm, oracle_mod, monkeypatch):
         try:
             eng.load(snap)
             got = eng.reconcile(flags)
-            lean = eng.reconcile(_compact(flags))
+            lean = eng.reconcile(compact(flags))
         finally:
             eng.close()
         d = want.diff(got)
@@ -449,7 +405,7 @@ def test_parity_c5_autoscaling_sharded_over_8(oracle_mod):
     world, seen = 8, 0
     for rank in range(world):
         sh = synthetic.shard_by_uid(snap, rank, world)
-        got = _parity(sh, flags, oracle_mod)
+        got = parity(sh, flags, oracle_mod)
         keep = (snap.c_uid_hash % np.uint64(world)) == np.uint64(rank)
         for fld in ("path", "head_action", "err_kind", "err_arg", "n_pods", "new_state", "needs_status_write", "counts", "cond_status"):
             assert np.array_equal(got.clusters[fld], glob.clusters[keep][fld]), (rank, fld)
@@ -552,11 +508,11 @@ def test_parity_stressed_distributions(seed, oracle_mod, monkeypatch):
         seed=synthetic.SEED + seed)
     snap, flags = synthetic.generate(params)
     flags.env_random_pod_delete = seed % 2
-    got = _parity(snap, flags, oracle_mod)
+    got = parity(snap, flags, oracle_mod)
     assert got.n_actions > 0
     if seed % 3 == 0:
         monkeypatch.setenv("KR_FORCE_RADIX", "1")
-        _parity(snap, flags, oracle_mod)
+        parity(snap, flags, oracle_mod)
 
 
 def test_remaining_entry_points(oracle_mod):

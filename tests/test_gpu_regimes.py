@@ -4,16 +4,12 @@ the 32-worker-group and 64 / 128 / 256-pod limits of the bucket pipeline, and in
 
 Every threshold is derived from the device's SM count in `Regimes`, the way the engine derives it; a test that claims to cross
 one asserts that its sizes fall on each side of it."""
-import base64
-import hashlib
-
 import numpy as np
 import pytest
 
+from harness import Driver, b32, compact, flip_ready, incremental, kernels, parity, set_phase, spec_bytes
 from kuberay_b200 import abi, synthetic
 from kuberay_b200.engine import Engine, EngineError
-from test_gpu_incremental import Driver, _flip_ready, _set_phase
-from test_gpu_parity import _compact, _parity
 
 pytestmark = pytest.mark.gpu
 
@@ -44,10 +40,6 @@ def regimes():
     return Regimes()
 
 
-def _b32(data: bytes) -> str:
-    return base64.b32hexencode(hashlib.sha1(data).digest()).decode()
-
-
 # ------------------------------------------------------------------------------------------------ hash, throughput regime
 
 def _hash_messages(n, rng):
@@ -75,7 +67,7 @@ def test_hash_batch_on_both_sides_of_the_throughput_threshold(regimes):
         for n in sizes:
             msgs = _hash_messages(n, rng)
             got = eng.hash_batch(msgs)
-            bad = [i for i, (m, h) in enumerate(zip(msgs, got)) if _b32(m) != h]
+            bad = [i for i, (m, h) in enumerate(zip(msgs, got)) if b32(m).decode() != h]
             assert not bad, (n, len(bad), [len(msgs[i]) for i in bad[:10]])
     finally:
         eng.close()
@@ -98,18 +90,13 @@ def _throughput_snapshot(n_clusters, seed=7):
     gate = np.flatnonzero(((snap.c_flags & abi.CF_UPGRADE_RECREATE) != 0) & (snap.h_annot_state == abi.ANNOT_HASH32))
     ah = snap.h_annot_hash.reshape(-1, 32)                     # head-aux row c is cluster c's head (generator order)
     for i, c in enumerate(gate):
-        h = _b32(_spec(snap, c)).encode()
+        h = b32(spec_bytes(snap, c))
         ah[c] = np.frombuffer(h if i % 2 == 0 else h[::-1], dtype=np.uint8)
     return snap, flags
 
 
-def _spec(snap, c):
-    off, ln = int(snap.c_json_off[c]), int(snap.c_json_len[c])
-    return snap.json[off:off + ln].tobytes()
-
-
 def _check_digests(snap, res):
-    want = np.frombuffer("".join(_b32(_spec(snap, c)) for c in range(snap.dims["clusters"])).encode(), dtype=np.uint8).reshape(-1, 32)
+    want = np.frombuffer(b"".join(b32(spec_bytes(snap, c)) for c in range(snap.dims["clusters"])), dtype=np.uint8).reshape(-1, 32)
     bad = np.flatnonzero((res.hash != want).any(axis=1))
     assert not bad.size, (bad.size, bad[:10].tolist(), [int(snap.c_json_len[c]) for c in bad[:10]])
 
@@ -121,7 +108,7 @@ def test_full_pass_in_the_throughput_regime(trips, regimes, oracle_mod, monkeypa
     n = regimes.latency_max + 3000 if trips == 1 else regimes.pass_trip + 1500
     assert regimes.throughput(n) and (n <= regimes.pass_trip) == (trips == 1)
     snap, flags = _throughput_snapshot(n)
-    got, lean = _parity(snap, flags, oracle_mod, both=True)
+    got, lean = parity(snap, flags, oracle_mod, both=True)
     _check_digests(snap, got)
     _check_digests(snap, lean)
     rec = (snap.c_flags & abi.CF_UPGRADE_RECREATE) != 0
@@ -129,7 +116,7 @@ def test_full_pass_in_the_throughput_regime(trips, regimes, oracle_mod, monkeypa
     assert (paths == abi.PATH_RECREATE_DELETE_ALL).sum() > 100 and (paths == abi.PATH_NORMAL).sum() > 100
     assert _bucket_taken(snap, flags)
     monkeypatch.setenv("KR_NO_HASH_SPIN", "1")
-    got, lean = _parity(snap, flags, oracle_mod, both=True)
+    got, lean = parity(snap, flags, oracle_mod, both=True)
     _check_digests(snap, lean)
 
 
@@ -145,15 +132,15 @@ def test_incremental_json_recommit_in_the_throughput_regime(regimes, oracle_mod)
     cand = np.flatnonzero(((snap.c_flags & abi.CF_UPGRADE_RECREATE) != 0) & ((snap.c_flags & abi.CF_SKIP) == 0) & (snap.h_annot_state == abi.ANNOT_HASH32)
                           & (snap.h_version_state == abi.VER_CURRENT) & (snap.c_json_len > 0))
     path = oracle_mod.run(snap, flags, threads=8).clusters["path"]
-    match = np.array([c for c in cand if bytes(ah[c]) == _b32(_spec(snap, c)).encode()])
+    match = np.array([c for c in cand if bytes(ah[c]) == b32(spec_bytes(snap, c))])
     spoil = rng.choice(match[path[match] == abi.PATH_NORMAL], 60, replace=False)
     miss = np.setdiff1d(cand, match)
     arm = rng.choice(miss[path[miss] == abi.PATH_RECREATE_DELETE_ALL], 60, replace=False)
     edit = {int(c): int(snap.c_json_off[c]) + int(rng.integers(0, int(snap.c_json_len[c]))) for c in np.concatenate([spoil, arm])}
     for c in arm:                                              # the annotation already names the spec as it will be edited
-        b = bytearray(_spec(snap, c))
+        b = bytearray(spec_bytes(snap, c))
         b[edit[int(c)] - int(snap.c_json_off[c])] ^= 0x20
-        ah[c] = np.frombuffer(_b32(bytes(b)).encode(), dtype=np.uint8)
+        ah[c] = np.frombuffer(b32(bytes(b)), dtype=np.uint8)
     dr = Driver(snap, flags)
     try:
         first, _ = dr.check(oracle_mod, expect_incremental=False)
@@ -172,7 +159,7 @@ def test_incremental_json_recommit_in_the_throughput_regime(regimes, oracle_mod)
 
 # ------------------------------------------------------------------------------------------------ replica-index windows
 
-def _members(snap):
+def _group_members(snap):
     """Worker pod rows by group row (pods keyed to their RayCluster and worker group)."""
     ckey = {(int(snap.c_ns_id[c]), int(snap.c_name_id[c])): c for c in range(snap.dims["clusters"])}
     gkey = {(int(snap.g_cluster_idx[g]), int(snap.g_name_id[g])): g for g in range(snap.dims["groups"])}
@@ -197,7 +184,8 @@ def _set_labels(snap, rows, labels):
             snap.p_replica_index[p] = v
 
 
-def _scale_to(snap, g, replicas):
+def _set_replicas(snap, g, replicas):
+    """Group row g asks for `replicas`, no maximum (its minimum, suspension and expectations stay as they are)."""
     snap.g_replicas[g] = replicas
     snap.g_max[g] = 2 ** 31 - 1
     snap.g_flags[g] &= ~np.uint32(abi.GF_REPLICAS_NIL | abi.GF_MAX_NIL)
@@ -248,12 +236,12 @@ _WINDOW_CASES = [
 
 def _window_snapshot():
     snap, flags = synthetic.generate(synthetic.SynthParams(n_clusters=64, pods_per_cluster=41, groups=2, healthy=True, seed=3))
-    members = _members(snap)
+    members = _group_members(snap)
     assert all(len(members[g]) == 20 for g in range(snap.dims["groups"]))
     cases = {}
     for i, (replicas, labels) in enumerate(_WINDOW_CASES):
         for g in (5 * i + 1, 5 * i + 66):                                    # two groups per case, in different RayClusters
-            _scale_to(snap, g, replicas)
+            _set_replicas(snap, g, replicas)
             _set_labels(snap, members[g], labels)
             cases[g] = replicas
     return snap, flags, members, cases
@@ -262,14 +250,14 @@ def _window_snapshot():
 def test_replica_index_windows_on_every_pipeline(oracle_mod, monkeypatch):
     snap, flags, members, cases = _window_snapshot()
     cap = 1 << 17
-    got, lean = _parity(snap, flags, oracle_mod, both=True, max_creates=cap)
+    got, lean = parity(snap, flags, oracle_mod, both=True, max_creates=cap)
     assert _bucket_taken(snap, flags, max_creates=cap)
     for res in (got, lean):
         for g in cases:
             assert res.groups["n_create"][g] > 0, g
         assert _check_creates(snap, res, members) > 40000
     monkeypatch.setenv("KR_FORCE_RADIX", "1")
-    got, lean = _parity(snap, flags, oracle_mod, both=True, max_creates=cap)
+    got, lean = parity(snap, flags, oracle_mod, both=True, max_creates=cap)
     for res in (got, lean):
         _check_creates(snap, res, members)
 
@@ -277,7 +265,7 @@ def test_replica_index_windows_on_every_pipeline(oracle_mod, monkeypatch):
 def test_replica_index_windows_with_the_gate_off(oracle_mod):
     snap, flags, _, _ = _window_snapshot()
     flags.gate_multihost_indexing = 0
-    got, lean = _parity(snap, flags, oracle_mod, both=True, max_creates=1 << 17)
+    got, lean = parity(snap, flags, oracle_mod, both=True, max_creates=1 << 17)
     for res in (got, lean):
         own = abi._gather_owned(res.groups["create_off"], res.groups["n_create"])
         assert own.size > 40000 and (res.create_idx[own] == -1).all()
@@ -287,20 +275,20 @@ def test_replica_index_window_filled_by_one_group(oracle_mod, monkeypatch):
     """Groups of 1100 workers (sort, then radix pipeline; the bucket pipeline leaves such a RayCluster to them): the in-use
     labels fill the whole second window, or the whole first one."""
     snap, flags = synthetic.generate(synthetic.SynthParams(n_clusters=6, pods_per_cluster=1101, groups=1, healthy=True, seed=4))
-    members = _members(snap)
-    _scale_to(snap, 0, 2100)
+    members = _group_members(snap)
+    _set_replicas(snap, 0, 2100)
     _set_labels(snap, members[0], list(range(1024, 2048)) + list(range(76)))      # free: 76..1023, then 2048..2099
-    _scale_to(snap, 1, 1150)
+    _set_replicas(snap, 1, 1150)
     _set_labels(snap, members[1], list(range(1100)))                             # free from 1100 on
-    _scale_to(snap, 2, 1500)
+    _set_replicas(snap, 2, 1500)
     _set_labels(snap, members[2], list(range(0, 2200, 2))[:1100])                # every even label below 2200
-    got, lean = _parity(snap, flags, oracle_mod, both=True, max_creates=1 << 14)
+    got, lean = parity(snap, flags, oracle_mod, both=True, max_creates=1 << 14)
     for res in (got, lean):
         _check_creates(snap, res, members)
     assert got.creates_of(0)[[0, 947, 948, 999]].tolist() == [76, 1023, 2048, 2099]
     assert got.creates_of(1)[[0, 49]].tolist() == [1100, 1149]
     monkeypatch.setenv("KR_FORCE_RADIX", "1")
-    for res in _parity(snap, flags, oracle_mod, both=True, max_creates=1 << 14):
+    for res in parity(snap, flags, oracle_mod, both=True, max_creates=1 << 14):
         _check_creates(snap, res, members)
 
 
@@ -309,13 +297,13 @@ def test_replica_index_windows_multihost(oracle_mod):
     replicas.  Both pipelines against the oracle."""
     snap, flags = synthetic.generate(synthetic.SynthParams(n_clusters=64, pods_per_cluster=41, groups=2, healthy=True, multihost_frac=1.0, seed=5))
     assert (snap.g_num_hosts == 4).all()
-    members = _members(snap)
+    members = _group_members(snap)
     cases = [(3000, [1023, 1024, 2047, 2048, 0]), (1500, [5, 5, -1, 1024, 7]), (4100, [4095, 4096, 4097, 0, 1]), (1025, [1024, 0, 1, 2, 3]),
              (2050, [2049, 2048, 2047, 1024, 1023])]
     rng = np.random.default_rng(5)
     for i, (replicas, labels) in enumerate(cases):
         for g in (3 * i + 1, 3 * i + 70):
-            _scale_to(snap, g, replicas)
+            _set_replicas(snap, g, replicas)
             rows = members[g]
             names = np.unique(snap.p_replica_name_id[rows])
             assert names.size == 5
@@ -324,7 +312,7 @@ def test_replica_index_windows_multihost(oracle_mod):
                 _set_labels(snap, in_rep, [v] * len(in_rep))
                 if i == 1:                                     # a replica whose first pod carries another label than the rest
                     _set_labels(snap, [min(in_rep)], [int(rng.integers(1000, 1100))])
-    got, lean = _parity(snap, flags, oracle_mod, both=True, max_creates=1 << 16)
+    got, lean = parity(snap, flags, oracle_mod, both=True, max_creates=1 << 16)
     assert _bucket_taken(snap, flags, max_creates=1 << 16)
     scaled = [g for i in range(len(cases)) for g in (3 * i + 1, 3 * i + 70)]
     for res in (got, lean):
@@ -334,13 +322,7 @@ def test_replica_index_windows_multihost(oracle_mod):
 
 def _bucket_taken(snap, flags, **kw):
     """Whether a compact-results pass over `snap` runs the bucket pipeline (k_match2 + k_decide2)."""
-    eng = Engine.for_snapshot(snap, **kw)
-    try:
-        eng.load(snap)
-        names = [k for k, _ in eng.reconcile_profiled(_compact(flags))["kernels"]]
-    finally:
-        eng.close()
-    return {"k_match2", "k_decide2"} <= set(names)
+    return {"k_match2", "k_decide2"} <= set(kernels(snap, compact(flags), **kw))
 
 
 # ------------------------------------------------------------------------------------------------ pipeline limits
@@ -370,7 +352,7 @@ def _wide_snapshot(n_groups, multihost_frac=0.0, seed=9):
 def test_widest_cluster_at_the_worker_group_limit(n_groups, regimes, oracle_mod):
     snap, flags = _wide_snapshot(n_groups)
     assert int(snap.c_group_cnt.max()) == n_groups
-    got = _parity(snap, flags, oracle_mod)
+    got = parity(snap, flags, oracle_mod)
     g31 = snap.c_group_off.astype(np.int64) + _last_slot(n_groups)
     assert (got.groups["n_create"][g31] > 0).any() and (got.groups["diff"][g31] < 0).any()
     assert _bucket_taken(snap, flags) == (n_groups <= regimes.smem_groups)
@@ -378,21 +360,21 @@ def test_widest_cluster_at_the_worker_group_limit(n_groups, regimes, oracle_mod)
         mh, mflags = _wide_snapshot(n_groups, multihost_frac=0.3)
         slot31 = mh.c_group_off.astype(np.int64) + 31
         assert (mh.g_num_hosts[slot31] > 1).any()
-        got = _parity(mh, mflags, oracle_mod)
+        got = parity(mh, mflags, oracle_mod)
         assert (got.groups["flags"][slot31] & abi.GR_MULTIHOST).any()
         assert _bucket_taken(mh, mflags)
 
 
 def test_incremental_epochs_touch_group_slot_31(oracle_mod):
     snap, flags = _wide_snapshot(32)
-    members = _members(snap)
+    members = _group_members(snap)
     slot31 = (snap.c_group_off.astype(np.int64) + 31).tolist()
     dr = Driver(snap, flags)
     try:
         dr.check(oracle_mod, expect_incremental=False)
         rows = [p for g in slot31[:20] for p in members.get(g, [])]
         assert rows
-        _flip_ready(snap, rows[::2]); _set_phase(snap, rows[1::2], abi.PHASE_FAILED)
+        flip_ready(snap, rows[::2]); set_phase(snap, rows[1::2], abi.PHASE_FAILED)
         dr.commit_rows(rows)
         got, _ = dr.check(oracle_mod, expect_incremental=True)
         assert got.changed_clusters is not None and np.isin(snap.g_cluster_idx[slot31[:20]], got.changed_clusters).all()
@@ -420,7 +402,7 @@ def _one_cluster_of(size, multihost=False):
         snap.g_num_hosts[0] = 4
         snap.p_replica_name_id[ws] = np.uint32(0x7D000000) + (np.arange(ws.size) // 4).astype(np.uint32)
         _set_labels(snap, ws, (np.arange(ws.size) // 4).tolist())
-        _scale_to(snap, 0, ws.size // 4 + 2)
+        _set_replicas(snap, 0, ws.size // 4 + 2)
     return snap, flags
 
 
@@ -430,7 +412,7 @@ def test_one_cluster_at_each_bucket_stride_edge(multihost, regimes, oracle_mod):
         snap, flags = _one_cluster_of(size, multihost)
         n, c = snap.dims, snap.dims["clusters"]
         assert (n["pods"] * 5 // 4 + c - 1) // c <= 64                 # the commit's stride: 64 (kr_snapshot_begin)
-        got = _parity(snap, flags, oracle_mod)
+        got = parity(snap, flags, oracle_mod)
         assert got.clusters["n_pods"][0] == size
         if multihost:
             assert got.groups["flags"][0] & abi.GR_MULTIHOST
@@ -444,7 +426,7 @@ def test_incremental_epochs_that_run_out_of_arena(oracle_mod):
     pods grow action runs; once a cursor passes its end the epoch is void and a full pass packs the arenas again."""
     snap, flags = synthetic.generate(synthetic.SynthParams(n_clusters=400, pods_per_cluster=12, groups=1, healthy=True, seed=14))
     nc = snap.dims["clusters"]
-    members = _members(snap)
+    members = _group_members(snap)
     cap = 600
     dr = Driver(snap, flags, max_creates=cap)
     try:
@@ -456,12 +438,13 @@ def test_incremental_epochs_that_run_out_of_arena(oracle_mod):
             up = np.arange(40 * epoch, 40 * epoch + 40) % nc                   # a rotating set of RayClusters scales up ...
             snap.g_replicas[prev_up] = base[prev_up]                          # ... and the previous one back down
             snap.g_replicas[up] = base[up] + 3
-            _set_phase(snap, prev_bad, abi.PHASE_RUNNING)
+            set_phase(snap, prev_bad, abi.PHASE_RUNNING)
             bad = [members[int(g)][k] for g in (up + 200) % nc for k in (0, 1)][:40]   # pods of other RayClusters fail
-            _set_phase(snap, bad, abi.PHASE_FAILED)
+            set_phase(snap, bad, abi.PHASE_FAILED)
             dr.commit_objects()
             dr.commit_rows(list(bad) + list(prev_bad))
-            got, inc = dr.check(oracle_mod)
+            got, _ = dr.check(oracle_mod)
+            inc = incremental(got, nc)
             full = got.changed_clusters is None and got.n_changed == nc
             assert inc != full
             kinds.append(inc)
@@ -476,12 +459,12 @@ def test_incremental_epochs_that_run_out_of_arena(oracle_mod):
             dr.eng.reconcile(dr.flags)
         assert ei.value.code == abi.KR_E_CAPACITY and "max_creates" in str(ei.value)
         snap.g_replicas[:] = base
-        _set_phase(snap, prev_bad, abi.PHASE_RUNNING)
+        set_phase(snap, prev_bad, abi.PHASE_RUNNING)
         dr.commit_objects()
         dr.commit_rows(prev_bad)
         dr.prev = None
         dr.check(oracle_mod, expect_incremental=False)   # (the overrun left runs unwritten: this pass starts over)
-        _flip_ready(snap, bad)
+        flip_ready(snap, bad)
         dr.commit_rows(bad)
         dr.check(oracle_mod, expect_incremental=True)
     finally:

@@ -4,22 +4,17 @@ RayClusters (k_inc_mark_rows) and fetches only their digests (k_inc_digest_gathe
 
 Every epoch is compared with the CPU oracle (digests included), with a second engine fed the same stream through KR_PART_JSON,
 records the pass did not name must be unchanged, and the epoch must stay incremental."""
-import base64
 import copy
-import hashlib
 
 import numpy as np
 import pytest
 
+from harness import (PACKER_CAPS, Mirror, SpecDriver, arena_stream, b32, device_incremental, events, flip_ready, incremental, objects,
+                     packer_check, packer_stream, spec_edits)
 from kuberay_b200 import abi, synthetic
 from kuberay_b200.engine import Engine, EngineError
 from kuberay_b200.live import LiveArena
 from kuberay_b200.packer import Packer
-from kuberay_b200.snapshot import Snapshot
-from test_gpu_incremental import OBJ_COLS, POD_COLS, _flip_ready
-from test_gpu_wtd_edits import _objects
-from test_live_arena import _events
-from test_packer import Mirror, check as packer_check
 
 pytestmark = pytest.mark.gpu
 
@@ -28,142 +23,6 @@ def _snap(seed, **kw):
     p = dict(n_clusters=300, pods_per_cluster=16, groups=3, recreate_frac=0.2, seed=seed)
     p.update(kw)
     return synthetic.generate(synthetic.config("C2", **p))
-
-
-def with_json(snap, json_bytes):
-    """A copy of `snap` whose JSON arena holds json_bytes bytes (the old bytes first)."""
-    d = snap.dims
-    out = Snapshot(d["clusters"], d["groups"], d["wtd"], d["pods"], d["heads"], d["jobs"], json_bytes)
-    for name, _dt, _m, dim in abi.COLUMNS:
-        if dim != "json":
-            out.cols[name][:] = snap.cols[name]
-    n = min(json_bytes, d["json"])
-    out.json[:n] = snap.json[:n]
-    return out
-
-
-def digest(b: bytes) -> bytes:
-    return base64.b32hexencode(hashlib.sha1(b).digest())
-
-
-class SpecDriver:
-    """One engine committing spec edits row by row and a twin committing KR_PART_JSON, on the same fixed layout."""
-
-    def __init__(self, snap, flags, json_room=1 << 20, **opts):
-        d = snap.dims
-        self.snap, self.flags = snap, flags
-        flags.fetch_pod_lists = 0
-        up = lambda x: int(x * 1.25) + 16  # noqa: E731
-        self.engs, self.views = [], []
-        for _ in range(2):
-            e = Engine(0, up(d["clusters"]), up(d["groups"]), up(d["wtd"]), up(d["pods"]), up(d["heads"]), up(d["jobs"]),
-                       4 * d["pods"] + 4096, d["json"] + json_room)
-            for k, v in opts.items():
-                getattr(e, f"set_{k}")(v)
-            e.set_fixed_layout(True)
-            v = e.begin(snap.sizes())
-            e.fill(v, snap)
-            e.commit()
-            self.engs.append(e)
-            self.views.append(v)
-        self.prev = None
-        self.pending, self.edits = set(), {}
-
-    @property
-    def eng(self):
-        return self.engs[0]
-
-    def edit(self, c, body: bytes, move=False):
-        """Rewrite cluster c's muted spec with `body` (applied by apply()): in place when the padded size stays and `move` is not
-        asked for, else at a new range at the arena's end."""
-        self.edits[int(c)] = (body, move or (len(body) + 15) // 16 != (int(self.snap.c_json_len[c]) + 15) // 16)
-
-    def apply(self):
-        if not self.edits:
-            return
-        s = self.snap
-        end = (s.dims["json"] + 15) // 16 * 16
-        grow = sum((len(b) + 15) // 16 * 16 for b, mv in self.edits.values() if mv)
-        if grow:
-            s = self.snap = with_json(s, end + grow)
-            for i, e in enumerate(self.engs):
-                self.views[i] = e.begin(s.sizes())
-        for c, (body, mv) in self.edits.items():
-            if mv:
-                off, end = end, end + (len(body) + 15) // 16 * 16
-            else:
-                off = int(s.c_json_off[c])
-            s.json[off:off + (len(body) + 15) // 16 * 16] = 0
-            s.json[off:off + len(body)] = np.frombuffer(body, dtype=np.uint8)
-            s.c_json_off[c], s.c_json_len[c] = off, len(body)
-            self.pending.add(c)
-        self.edits = {}
-
-    def commit_specs(self, rows=None, calls=1):
-        """The edited specs: row by row on the first engine (`rows` as given, possibly split over several calls), the whole arena
-        plus the object part on the twin."""
-        self.apply()
-        rows = sorted(self.pending) if rows is None else rows
-        v = self.views[0]
-        np.copyto(v["json"], self.snap.json)
-        for name in ("c_json_off", "c_json_len"):
-            v[name][:] = self.snap.cols[name]
-        for part in np.array_split(np.asarray(rows, dtype=np.uint32), calls):
-            self.eng.commit_spec_rows(part)
-        np.copyto(self.views[1]["json"], self.snap.json)
-        self.commit_objects(which=(1,), parts=abi.PART_OBJECTS | abi.PART_JSON)
-        self.pending.clear()
-
-    def commit_objects(self, which=(0, 1), parts=abi.PART_OBJECTS):
-        for i in which:
-            for c in OBJ_COLS:
-                np.copyto(self.views[i][c], self.snap.cols[c])
-            self.engs[i].commit(parts)
-
-    def commit_rows(self, rows):
-        rows = np.unique(np.asarray(rows, dtype=np.uint32))
-        for i, e in enumerate(self.engs):
-            for c in POD_COLS:
-                self.views[i][c][rows] = self.snap.cols[c][rows]
-            e.commit_pod_rows(rows)
-
-    def check(self, oracle_mod, expect_incremental=True, profiled=False, h2d=None, h2d_after=None):
-        """h2d: the commits' counted bytes before the pass; h2d_after: with the hash order the pass uploaded."""
-        names = []
-        if h2d is not None:
-            assert self.eng.last_profile()["h2d_bytes"] == h2d
-        if profiled:
-            names = [k for k, _ in self.eng.reconcile_profiled(self.flags)["kernels"]]
-            got = self.eng.fetch()
-        else:
-            got = self.eng.reconcile(self.flags)
-        if h2d_after is not None:
-            assert self.eng.last_profile()["h2d_bytes"] == h2d_after
-        twin = self.engs[1].reconcile(self.flags)
-        d = oracle_mod.run(self.snap, self.flags).diff(got)
-        assert not d, (d[:6], got.n_changed)
-        d = twin.diff(got)
-        assert not d, d[:6]
-        nc = self.snap.dims["clusters"]
-        inc = got.changed_clusters is not None or got.n_changed < nc
-        if expect_incremental is not None:
-            assert inc == expect_incremental, (inc, got.n_changed, names)
-        if inc and self.prev is not None:
-            same = np.ones(nc, dtype=bool)
-            if got.changed_clusters is not None:
-                same[got.changed_clusters] = False
-            assert np.array_equal(got.clusters[same], self.prev.clusters[same])
-            assert np.array_equal(got.act_cnt[same], self.prev.act_cnt[same])
-        self.prev = got
-        return got, names
-
-    def body(self, c):
-        o, n = int(self.snap.c_json_off[c]), int(self.snap.c_json_len[c])
-        return self.snap.json[o:o + n].tobytes()
-
-    def close(self):
-        for e in self.engs:
-            e.close()
 
 
 def counted(dr, rows):
@@ -197,7 +56,7 @@ def test_edit_in_place_and_moved(oracle_mod):
         got, names = dr.check(oracle_mod, profiled=True, h2d=counted(dr, rows[:3]), h2d_after=counted(dr, rows[:3]) + 4 * 3)
         assert "k_hash_rows" in names and "k_hash" not in names and "k_inc_mark_recreate" not in names, names
         for c in rows[:3]:
-            assert bytes(got.hash[c]) == digest(dr.body(c))
+            assert bytes(got.hash[c]) == b32(dr.body(c))
     finally:
         dr.close()
 
@@ -214,7 +73,7 @@ def test_sha1_padding_edges(length, oracle_mod):
         dr.commit_specs()
         got, _ = dr.check(oracle_mod, h2d=counted(dr, rows))
         for c in rows:
-            assert bytes(got.hash[c]) == digest(dr.body(c))
+            assert bytes(got.hash[c]) == b32(dr.body(c))
     finally:
         dr.close()
 
@@ -231,7 +90,7 @@ def test_recreate_gate_switches_and_unedited_gates_stay(oracle_mod):
         def annotated(c):
             h = head_of.get((int(s.c_ns_id[c]), int(s.c_name_id[c])))
             return h is not None and s.h_annot_state[h] == abi.ANNOT_HASH32 and s.h_version_state[h] == abi.VER_CURRENT and \
-                bytes(s.h_annot_hash.reshape(-1, 32)[h]) == digest(dr.body(c))
+                bytes(s.h_annot_hash.reshape(-1, 32)[h]) == b32(dr.body(c))
         on = [c for c in rec if first.clusters["path"][c] == abi.PATH_NORMAL and annotated(c)]
         assert len(on) >= 1 and len(rec) >= 6, (len(on), len(rec))
         c = on[0]
@@ -263,14 +122,14 @@ def test_edit_with_pod_churn_and_object_rows(specs_first, oracle_mod):
             dr.edit(c, dr.body(c) + b"  ", move=True)
         dr.apply()
         pods =np.flatnonzero((dr.snap.p_cluster_name_id == dr.snap.c_name_id[rows[0]]) & (dr.snap.p_ns_id == dr.snap.c_ns_id[rows[0]]))[:3]
-        _flip_ready(dr.snap, pods)
+        flip_ready(dr.snap, pods)
         dr.snap.c_old_counts[5 * rows[1]] += 1
         if specs_first:
             dr.commit_specs()
-            dr.commit_objects(which=(0,))
+            dr.commit_objects(twin=False)
             dr.commit_rows(pods)
         else:  # the object commit finds moved ranges: the whole re-hash, still incremental
-            dr.commit_objects(which=(0,))
+            dr.commit_objects(twin=False)
             dr.commit_rows(pods)
             dr.commit_specs()
         dr.check(oracle_mod)
@@ -289,7 +148,7 @@ def test_repeated_rows_and_two_calls(oracle_mod):
         dr.commit_specs(rows=rows + rows[:3] + rows[::2], calls=3)
         got, _ = dr.check(oracle_mod, h2d=counted(dr, rows), h2d_after=counted(dr, rows) + 4 * len(rows))
         for c in rows:
-            assert bytes(got.hash[c]) == digest(dr.body(c))
+            assert bytes(got.hash[c]) == b32(dr.body(c))
     finally:
         dr.close()
 
@@ -304,7 +163,7 @@ def test_spec_rows_with_whole_arena_commit(oracle_mod):
         dr.commit_specs()
         dr.edit(b, _mutate(dr.body(b), 4))
         dr.apply()
-        np.copyto(dr.views[0]["json"], dr.snap.json)
+        np.copyto(dr.views["json"], dr.snap.json)
         dr.eng.commit(abi.PART_JSON)  # (the whole arena wins)
         dr.commit_specs(rows=[b])
         _, names = dr.check(oracle_mod, profiled=True)
@@ -331,7 +190,7 @@ def test_state_errors_and_full_pass_without_resident_state(oracle_mod):
         dr.edit(c, _mutate(dr.body(c), 9), move=True)
         dr.commit_specs()
         got, _ = dr.check(oracle_mod, expect_incremental=False)
-        assert bytes(got.hash[c]) == digest(dr.body(c))
+        assert bytes(got.hash[c]) == b32(dr.body(c))
         # an option toggle drops the resident state as well
         dr.edit(c, _mutate(dr.body(c), 10))
         dr.commit_specs()
@@ -356,11 +215,11 @@ def test_skip_hash_leaves_rows_pending(oracle_mod):
         dr.check(oracle_mod)
         dr.flags.skip_hash = 0  # other flags: the full pass hashes the listed message with the others
         got, _ = dr.check(oracle_mod, expect_incremental=False)
-        assert bytes(got.hash[c]) == digest(dr.body(c))
+        assert bytes(got.hash[c]) == b32(dr.body(c))
         dr.edit(c, _mutate(dr.body(c), 12))
         dr.commit_specs()
         got, _ = dr.check(oracle_mod)
-        assert bytes(got.hash[c]) == digest(dr.body(c))
+        assert bytes(got.hash[c]) == b32(dr.body(c))
     finally:
         dr.close()
 
@@ -385,15 +244,15 @@ def test_row_edited_again_after_skip_hash_passes(moved, oracle_mod):
         dr.edit(c, dr.body(c) + b"   ", move=moved)                  # then longer: a new range (moved) or the padded one
         dr.commit_specs()
         if moved:
-            dr.commit_objects(which=(0,))
+            dr.commit_objects(twin=False)
         dr.check(oracle_mod)
         dr.flags.skip_hash = 0  # the next pass hashes: the full pass over the arena as it now is on the device
         got, _ = dr.check(oracle_mod, expect_incremental=False)
-        assert bytes(got.hash[c]) == digest(dr.body(c)) and bytes(got.hash[other]) == digest(dr.body(other))
+        assert bytes(got.hash[c]) == b32(dr.body(c)) and bytes(got.hash[other]) == b32(dr.body(other))
         dr.edit(c, _mutate(dr.body(c), 4))
         dr.commit_specs()
         got, _ = dr.check(oracle_mod)
-        assert bytes(got.hash[c]) == digest(dr.body(c))
+        assert bytes(got.hash[c]) == b32(dr.body(c))
     finally:
         dr.close()
 
@@ -440,7 +299,7 @@ def test_edits_inside_large_huge_wide_and_multihost_clusters(kind, oracle_mod):
         h = head_of[(int(s.c_ns_id[c]), int(s.c_name_id[c]))]
         s.h_annot_state[h], s.h_version_state[h] = abi.ANNOT_HASH32, abi.VER_CURRENT
         o, n = int(s.c_json_off[c]), int(s.c_json_len[c])
-        ann[h] = np.frombuffer(digest(s.json[o:o + n].tobytes() if i == 0 else b"another spec"), dtype=np.uint8)
+        ann[h] = np.frombuffer(b32(s.json[o:o + n].tobytes() if i == 0 else b"another spec"), dtype=np.uint8)
     opts = dict(large_clusters=True, wide_clusters=True, huge_clusters=True, wtd_edits=True)
     dr = SpecDriver(snap, flags, json_room=4 << 20, **opts)
     try:
@@ -455,7 +314,7 @@ def test_edits_inside_large_huge_wide_and_multihost_clusters(kind, oracle_mod):
             # (switching delete-all of a large RayCluster on or off may outgrow the places its decide kept: that epoch may take the
             # full pass; the others must stay incremental)
             got, names = dr.check(oracle_mod, expect_incremental=None if rnd in (0, 2) else True, profiled=True)
-            if got.changed_clusters is not None or got.n_changed < dr.snap.dims["clusters"]:
+            if incremental(got, dr.snap.dims["clusters"]):
                 assert "k_hash_rows" in names and "k_inc_mark_rows" in names and "k_hash" not in names, names
             if got.changed_clusters is not None:
                 assert set(got.changed_clusters.tolist()) <= set(gated), (kind, rnd)
@@ -489,7 +348,7 @@ def test_invalid_rows_offsets_and_ranges(oracle_mod):
         with pytest.raises(EngineError) as ei:
             dr.eng.commit_spec_rows([0, nc])
         assert ei.value.code == abi.KR_E_INVALID
-        v = dr.views[0]
+        v = dr.views
         off, ln = int(v["c_json_off"][1]), int(v["c_json_len"][1])
         v["c_json_off"][1] = off + 8
         with pytest.raises(EngineError) as ei:
@@ -523,59 +382,50 @@ def test_stream_through_the_engine(seed, oracle_mod):
                         move=bool(k and rng.integers(2)))
             live = np.flatnonzero((dr.snap.p_packed & abi.PP_TOMBSTONE) == 0)
             flip = rng.choice(live, max(1, live.size // 100), replace=False)
-            _flip_ready(dr.snap, flip)
+            flip_ready(dr.snap, flip)
             dr.commit_specs()
             if epoch % 2:
                 dr.commit_rows(flip)
             else:
-                dr.commit_objects(which=(0,))
+                dr.commit_objects(twin=False)
                 dr.commit_rows(flip)
             got, _ = dr.check(oracle_mod, expect_incremental=None)
-            n_inc += got.changed_clusters is not None or got.n_changed < nc
+            n_inc += incremental(got, nc)
         assert n_inc >= 38, n_inc
     finally:
         dr.close()
 
 
-def _spec_edits(rng, side, gen, k):
-    keys = sorted(side.clusters)
-    for i in rng.choice(len(keys), min(k, len(keys)), replace=False):
-        c = copy.deepcopy(side.clusters[keys[int(i)]])
-        c.pop("specJson", None)
-        c["spec"]["rayVersion"] = "v" + "9" * int(rng.integers(1, 90))
-        gen[0] += 1
-        c["generation"] = gen[0]
-        c["resourceVersion"] = 10_000 + gen[0]
-        side.upsert_cluster(c)
+def _twin_streams(seed, sides, oracle_mod, stream):
+    """The same 40 epochs of spec edits and informer events (one generator per epoch, seeded alike) on each side."""
+    out = []
+    for side in sides:
+        gen, counter = [2], [0]
+
+        def step(epoch, side=side, gen=gen, counter=counter):
+            r = np.random.default_rng(1000 * seed + epoch)
+            spec_edits(r, side, gen, int(r.integers(1, 4)))
+            events(r, side, counter, structural=False)
+        out.append(stream(side, oracle_mod, 40, step))
+    return out
 
 
 @pytest.mark.parametrize("seed", [1, 2])
 def test_stream_through_the_native_packer(seed, oracle_mod):
-    rng = np.random.default_rng(seed)
-    clusters, pods, jobs = _objects(seed)
-    pks = [Packer(max_clusters=64, max_groups=512, max_wtd=512, max_pods=4096, max_heads=256, max_jobs=64, max_creates=1 << 16,
-                  max_json_bytes=4 << 20, spec_rows=on) for on in (True, False)]
+    clusters, pods, jobs = objects(seed, big=True)
+    pks = [Packer(**PACKER_CAPS, spec_rows=on) for on in (True, False)]
     try:
         assert pks[0].engine.get_option(abi.OPT_SPEC_ROWS) == 1 and pks[1].engine.get_option(abi.OPT_SPEC_ROWS) == 0
         ms = [Mirror(copy.deepcopy(clusters), copy.deepcopy(pods), jobs, pk) for pk in pks]
         for pk, m in zip(pks, ms):
             pk.flush()
             packer_check(m, oracle_mod, lean=True)
-        gens, counters, modes = [[2], [2]], [[0], [0]], []
-        for epoch in range(40):
-            outs = []
-            for i, (pk, m) in enumerate(zip(pks, ms)):
-                r = np.random.default_rng(1000 * seed + epoch)  # the same events on both sides
-                _spec_edits(r, m, gens[i], int(r.integers(1, 4)))
-                _events(r, m, counters[i], structural=False)
-                mode = pk.flush()
-                _, got = packer_check(m, oracle_mod, lean=True)
-                outs.append((mode, got))
-            (mode_on, got_on), (mode_off, got_off) = outs
-            assert mode_on & abi.PACK_SPEC_ROWS and not mode_on & abi.PART_JSON, mode_on
-            assert mode_off & abi.PART_JSON and not mode_off & abi.PACK_SPEC_ROWS, mode_off
-            assert not got_off.diff(got_on)
-            modes.append(got_on.changed_clusters is not None or got_on.n_changed == 0)
+        (gots_on, modes_on), (gots_off, modes_off) = _twin_streams(seed, ms, oracle_mod, packer_stream)
+        for epoch, (mode_on, mode_off, got_on, got_off) in enumerate(zip(modes_on, modes_off, gots_on, gots_off)):
+            assert mode_on & abi.PACK_SPEC_ROWS and not mode_on & abi.PART_JSON, (epoch, mode_on)
+            assert mode_off & abi.PART_JSON and not mode_off & abi.PACK_SPEC_ROWS, (epoch, mode_off)
+            assert not got_off.diff(got_on), epoch
+        modes = [device_incremental(g) for g in gots_on]
         assert sum(modes) >= 36, modes
     finally:
         for pk in pks:
@@ -584,25 +434,13 @@ def test_stream_through_the_native_packer(seed, oracle_mod):
 
 @pytest.mark.parametrize("seed", [1, 2])
 def test_stream_through_the_live_arena(seed, oracle_mod):
-    clusters, pods, jobs = _objects(seed)
+    clusters, pods, jobs = objects(seed, big=True)
     arenas = [LiveArena(copy.deepcopy(clusters), copy.deepcopy(pods), jobs, spare_rows=64, spec_rows=on) for on in (True, False)]
     try:
-        gens, counters, inc = [[2], [2]], [[0], [0]], []
-        for epoch in range(40):
-            gots = []
-            for i, a in enumerate(arenas):
-                r = np.random.default_rng(1000 * seed + epoch)
-                _spec_edits(r, a, gens[i], int(r.integers(1, 4)))
-                _events(r, a, counters[i], structural=False)
-                a.flush()
-                fl = a.meta.flags
-                fl.fetch_pod_lists = 0
-                got = a.reconcile(fl)
-                d = oracle_mod.run(a.snap, fl).diff(got)
-                assert not d, (epoch, i, d[:6])
-                gots.append(got)
-            assert not gots[1].diff(gots[0])
-            inc.append(gots[0].changed_clusters is not None or gots[0].n_changed == 0)
+        gots_on, gots_off = _twin_streams(seed, arenas, oracle_mod, arena_stream)
+        for epoch, (got_on, got_off) in enumerate(zip(gots_on, gots_off)):
+            assert not got_off.diff(got_on), epoch
+        inc = [device_incremental(g) for g in gots_on]
         assert arenas[0].engine.get_option(abi.OPT_SPEC_ROWS) == 1
         assert sum(inc) >= 34 and arenas[0].stats["rebase"] <= 2, (inc, arenas[0].stats)
     finally:

@@ -1,4 +1,4 @@
-"""The engine's hash tables under colliding, wrapping and full-range ids (tests/test_table_keys.py builds the snapshots).
+"""The engine's hash tables under colliding, wrapping and full-range ids (tests/table_keys.py builds the snapshots).
 
 K1 puts about 480 RayCluster keys, orphan Pods' and RayJobs' absent keys and swapped or shared halves in one probe chain that starts in
 the last slot of the cluster table and wraps; K2 does the same for about 3 000 workersToDelete names (Bloom bitmap at its cap, decoy
@@ -9,12 +9,11 @@ import numpy as np
 import pytest
 
 import fuzz_objects
+from harness import OBJ_COLS, REBUILD, Driver, flip_ready, lists_of, members, run, workers_of
 from kuberay_b200 import abi, synthetic
 from kuberay_b200.engine import Engine
 from kuberay_b200.snapshot import Snapshot
-from test_gpu_incremental import OBJ_COLS, _flip_ready
-from test_gpu_wtd_edits import REBUILD, WtdDriver, lists_of, workers_of
-from test_table_keys import hash_pair, ids_in, k1, k2, k3, map_results, members, random_map, relabel
+from table_keys import hash_pair, ids_in, k1, k2, k3, map_results, random_map, relabel
 
 pytestmark = pytest.mark.gpu
 
@@ -41,16 +40,6 @@ def _flags(flags, fetch):
     return f
 
 
-def _run(snap, flags, **opts):
-    eng = Engine.for_snapshot(snap, max_creates=1 << 16, **opts)
-    try:
-        eng.load(snap)
-        got = eng.reconcile(flags)
-        return got, eng.get_option(abi.OPT_BUCKET_STRIDE)
-    finally:
-        eng.close()
-
-
 @pytest.mark.parametrize("variant", list(FETCH))
 @pytest.mark.parametrize("name", ["K1", "K2", "K3"])
 def test_full_pass(name, variant, cases, oracle_mod, monkeypatch):
@@ -58,13 +47,13 @@ def test_full_pass(name, variant, cases, oracle_mod, monkeypatch):
     if variant in ENV:
         monkeypatch.setenv(ENV[variant], "1")
     flags = _flags(k.kflags, FETCH[variant])
-    got, stride = _run(k.snap, flags, **OPTS)
+    got, _, stride = run(k.snap, flags, **OPTS)
     if variant == "bucket":
         assert stride != 0
     d = oracle_mod.run(k.snap, flags, threads=8).diff(got)
     assert not d, (name, variant, d[:8])
     if variant in ("bucket", "lists"):   # the engine's records over the relabelled snapshot are its records over the original, mapped
-        base, _ = _run(k.orig, _flags(k.flags, FETCH[variant]), **OPTS)
+        base, _, _ = run(k.orig, _flags(k.flags, FETCH[variant]), **OPTS)
         d = map_results(base, k.f).diff(got)
         assert not d, (name, variant, "relabelled", d[:8])
 
@@ -102,8 +91,9 @@ def test_full_range_ids_configs(cfg, oracle_mod):
 
 
 # ------------------------------------------------------------------------------------------------ incremental epochs
-def _driver(k, **opts):
-    return WtdDriver(_copy(k.snap), _flags(k.kflags, 0), **opts)
+def _driver(k, wtd_room=512, **opts):
+    """Fixed layout with room for the workersToDelete lists to grow, KR_OPT_WTD_EDITS on."""
+    return Driver(_copy(k.snap), _flags(k.kflags, 0), wtd_room=wtd_room, **opts, wtd_edits=True)
 
 
 def test_epochs_in_the_cluster_chain(cases, oracle_mod):
@@ -117,7 +107,7 @@ def test_epochs_in_the_cluster_chain(cases, oracle_mod):
         s = dr.snap
         owned = np.concatenate([members(s, c) for c in range(s.dims["clusters"])])
         rows = rng.choice(owned, 300, replace=False)
-        _flip_ready(s, rows)
+        flip_ready(s, rows)
         dr.commit_rows(rows)
         got, _ = dr.check(oracle_mod, expect_incremental=True)
         assert got.changed_clusters is not None and got.changed_clusters.size > 100
@@ -178,14 +168,14 @@ def test_epochs_in_the_workers_to_delete_chain(cases, oracle_mod):
             same = [x for h in range(max(0, g - 40), min(len(lists), g + 40)) if ns_of[h] == ns_of[g] for x in old[h]]
             dec = k.decoys[decoy_ns == ns_of[g]]
             lists[g][0] = int(s.p_name_id[dec[0]]) if dec.size and rng.random() < 0.5 else same[int(rng.integers(len(same)))]
-        dr.set_lists(lists)
+        dr.set_wtd_lists(lists)
         got, names = dr.check(oracle_mod, expect_incremental=True, profiled=True)
         assert set(REBUILD) <= set(names), names
         rows = np.concatenate([np.flatnonzero(np.isin(s.p_name_id, s.w_name_id))[:200], k.decoys[:100]])
-        _flip_ready(dr.snap, rows)
+        flip_ready(dr.snap, rows)
         dr.commit_rows(rows)
         dr.check(oracle_mod, expect_incremental=True)
-        dr.set_lists(old)
+        dr.set_wtd_lists(old)
         dr.check(oracle_mod, expect_incremental=True)
     finally:
         dr.close()
@@ -217,7 +207,7 @@ def test_epochs_with_heads_at_colliding_rows(cases, oracle_mod):
             dr.commit_rows(rows)
             dr.check(oracle_mod, expect_incremental=True)
         heads = s.h_pod_idx.copy()
-        _flip_ready(s, heads)
+        flip_ready(s, heads)
         dr.commit_rows(heads)
         got, _ = dr.check(oracle_mod, expect_incremental=True)
         assert (got.clusters["n_heads"] == 2).any() and (got.clusters["n_heads"] == 0).any()

@@ -6,44 +6,21 @@ Results.diff covers every result array except the run order inside the two arena
 the full pod lists are fetched.  Incremental epochs are compared with a from-scratch oracle run after each epoch."""
 import collections
 import copy
+import functools
 
 import numpy as np
 import pytest
 
-import fuzz_objects
+from harness import (BUCKET_KERNELS, OBJ_COLS, PACKER_CAPS, POD_COLS, SORT_KERNELS, Driver, Mirror, b32, compact, device_incremental, events,
+                     group_pods, head_row, lists_of, members, objects, packer_check, packer_stream, parity_on_off, run, scale_to, set_phase,
+                     spec_bytes, with_wtd_lists, workers)
 from kuberay_b200 import abi, synthetic
 from kuberay_b200.engine import Engine
 from kuberay_b200.packer import Packer
-from kuberay_b200.snapshot import Snapshot
-
-from test_gpu_incremental import OBJ_COLS, POD_COLS, Driver
-from test_gpu_regimes import _b32, _spec
-from test_live_arena import _events
-from test_packer import Mirror, check as packer_check
 
 pytestmark = pytest.mark.gpu
 
-SORT_KERNELS = {"k_match", "k_place_fused", "k_decide_small", "k_decide"}
-BUCKET_KERNELS = {"k_match2", "k_decide2", "k_large_sort", "k_decide_large"}
-
-
-def _compact(flags):
-    flags.fetch_pod_lists = 0
-    return flags
-
-
-def _members(snap, c):
-    return np.flatnonzero((snap.p_ns_id == snap.c_ns_id[c]) & (snap.p_cluster_name_id == snap.c_name_id[c]))
-
-
-def _workers(snap, c):
-    m = _members(snap, c)
-    return m[((snap.p_packed[m] >> abi.PP_NODE_TYPE_SHIFT) & 3) == abi.NT_WORKER]
-
-
-def _group_pods(snap, c, gi):
-    w = _workers(snap, c)
-    return w[snap.p_group_name_id[w] == snap.g_name_id[int(snap.c_group_off[c]) + gi]]
+_parity = functools.partial(parity_on_off, option="wide_clusters")
 
 
 def _wide_fleet(n_groups=48, wide=(0,), n_clusters=300, pods=60, seed=12, **kw):
@@ -52,31 +29,7 @@ def _wide_fleet(n_groups=48, wide=(0,), n_clusters=300, pods=60, seed=12, **kw):
     snap, flags = synthetic.generate(synthetic.SynthParams(n_clusters=n_clusters, pods_per_cluster=20, groups=1, seed=seed, **kw))
     synthetic.grow_clusters(snap, list(wide), pods)
     snap = synthetic.widen_clusters(snap, list(wide), n_groups)
-    return snap, _compact(flags)
-
-
-def _run(snap, flags, wide, large=False, profiled=False, max_creates=1 << 16):
-    eng = Engine.for_snapshot(snap, wide_clusters=wide, large_clusters=large, max_creates=max_creates)
-    try:
-        eng.load(snap)
-        names = [k for k, _ in eng.reconcile_profiled(flags)["kernels"]] if profiled else None
-        got = eng.reconcile(flags)
-        stride = eng.get_option(abi.OPT_BUCKET_STRIDE)
-    finally:
-        eng.close()
-    return got, names, stride
-
-
-def _parity(snap, flags, oracle_mod, large=False, **kw):
-    """Engine with the option on == oracle == engine with it off; returns (results, kernel names, stride) of the option-on run."""
-    on, names, stride = _run(snap, flags, True, large=large, profiled=True, **kw)
-    off, _, _ = _run(snap, flags, False, large=large, **kw)
-    want = oracle_mod.run(snap, flags)
-    d = want.diff(on)
-    assert not d, d[:6]
-    d = off.diff(on)
-    assert not d, d[:6]
-    return on, names, stride
+    return snap, compact(flags)
 
 
 def _on_the_bucket_pipeline(names, stride, want_stride=64):
@@ -103,7 +56,7 @@ def test_several_wide_clusters(oracle_mod):
 
 def test_every_cluster_wide(oracle_mod):
     snap, flags = synthetic.generate(synthetic.SynthParams(n_clusters=200, pods_per_cluster=40, groups=33, seed=5))
-    _, names, stride = _parity(snap, _compact(flags), oracle_mod)
+    _, names, stride = _parity(snap, compact(flags), oracle_mod)
     _on_the_bucket_pipeline(names, stride)
 
 
@@ -116,25 +69,12 @@ def test_a_cluster_at_the_worker_group_limit(oracle_mod):
 
 def test_32_worker_groups_stay_on_the_warp_decide(oracle_mod):
     snap, flags = synthetic.generate(synthetic.SynthParams(n_clusters=200, pods_per_cluster=40, groups=32, seed=6))
-    _, names, stride = _parity(snap, _compact(flags), oracle_mod)
+    _, names, stride = _parity(snap, compact(flags), oracle_mod)
     assert {"k_match2", "k_decide2"} <= set(names) and not {"k_large_sort", "k_decide_large"} & set(names), names
     assert not SORT_KERNELS & set(names) and stride == 64
 
 
 # ------------------------------------------------------------------------------------------------ decisions at slots >= 32
-
-def _set_phase(snap, rows, phase):
-    pk = snap.p_packed
-    pk[rows] = (pk[rows] & ~np.uint32(7 << abi.PP_PHASE_SHIFT)) | np.uint32(phase << abi.PP_PHASE_SHIFT)
-
-
-def _scale_to(snap, g, replicas):
-    snap.g_replicas[g] = replicas
-    snap.g_max[g] = 2 ** 31 - 1
-    snap.g_min[g] = 0
-    snap.g_flags[g] &= ~np.uint32(abi.GF_REPLICAS_NIL | abi.GF_MAX_NIL | abi.GF_MIN_NIL | abi.GF_SUSPEND)
-    snap.g_flags[g] |= np.uint32(abi.GF_EXPECT_OK)
-
 
 def _decision_fleet(seed, wide=(0, 100, 200), **kw):
     """Wide RayClusters of 48 groups x 60 pods, healthy, every group at its pod count (see the callers for each one's case)."""
@@ -143,7 +83,7 @@ def _decision_fleet(seed, wide=(0, 100, 200), **kw):
         snap.c_flags[c] &= ~np.uint32(abi.CF_SKIP | abi.CF_SUSPEND | abi.CF_UPGRADE_RECREATE)
         snap.c_flags[c] |= np.uint32(abi.CF_HEAD_EXPECT_OK)
         for gi in range(48):
-            _scale_to(snap, int(snap.c_group_off[c]) + gi, _group_pods(snap, c, gi).size)
+            scale_to(snap, int(snap.c_group_off[c]) + gi, group_pods(snap, c, gi).size)
     return snap, flags, list(wide)
 
 
@@ -153,17 +93,17 @@ def test_creates_scale_downs_and_unhealthy_pods_past_slot_32(random_delete, orac
     flags.env_random_pod_delete = int(random_delete)
     ga, gb, gc = (int(snap.c_group_off[x]) for x in (a, b, c))
     # a: an unhealthy pod in group 40 -> the groups stop after it
-    _set_phase(snap, _group_pods(snap, a, 40)[:1], abi.PHASE_FAILED)
+    set_phase(snap, group_pods(snap, a, 40)[:1], abi.PHASE_FAILED)
     # b: autoscaling; group 33 scaled to 0 and group 47 up by 3
     snap.c_flags[b] |= np.uint32(abi.CF_AUTOSCALING)
-    _scale_to(snap, gb + 33, 0)
-    _scale_to(snap, gb + 47, _group_pods(snap, b, 47).size + 3)
+    scale_to(snap, gb + 33, 0)
+    scale_to(snap, gb + 47, group_pods(snap, b, 47).size + 3)
     # c: creates in groups 32..47 with replica-index labels on every pod
-    wc = _workers(snap, c)
+    wc = workers(snap, c)
     snap.p_packed[wc] |= np.uint32(abi.PP_HAS_REPLICA_IDX)
     snap.p_replica_index[wc] = np.arange(wc.size, dtype=np.int32) % 3
     for gi in range(32, 48):
-        _scale_to(snap, gc + gi, _group_pods(snap, c, gi).size + gi - 30)
+        scale_to(snap, gc + gi, group_pods(snap, c, gi).size + gi - 30)
     got, names, stride = _parity(snap, flags, oracle_mod)
     _on_the_bucket_pipeline(names, stride)
     assert got.groups["n_unhealthy"][ga + 40] == 1 and got.clusters["stop_after_group"][a] == 40
@@ -171,25 +111,6 @@ def test_creates_scale_downs_and_unhealthy_pods_past_slot_32(random_delete, orac
     assert (got.groups["n_create"][gc + 32:gc + 48] == np.arange(2, 18)).all()
     _, codes = got.actions_of(b)
     assert (abi.ACT_DELETE_RANDOM in codes.tolist()) == bool(random_delete)
-
-
-def _with_wtd(snap, lists):
-    """A copy of `snap` whose workersToDelete lists of the groups in `lists` ({group row: [name ids]}) are replaced."""
-    cnt = snap.g_wtd_cnt.astype(np.int64).copy()
-    names = [snap.w_name_id[int(snap.g_wtd_off[g]):int(snap.g_wtd_off[g]) + int(snap.g_wtd_cnt[g])] for g in range(snap.dims["groups"])]
-    for g, ln in lists.items():
-        cnt[g] = len(ln)
-        names[g] = np.asarray(ln, dtype=np.uint32)
-    d = dict(snap.dims)
-    out = Snapshot(d["clusters"], d["groups"], int(cnt.sum()), d["pods"], d["heads"], d["jobs"], d["json"])
-    for name, _dt, _m, dim in abi.COLUMNS:
-        if dim != "wtd":
-            out.cols[name][:] = snap.cols[name]
-    out.g_wtd_cnt[:] = cnt.astype(np.uint32)
-    out.g_wtd_off[:] = np.concatenate([[0], np.cumsum(cnt)[:-1]]).astype(np.uint32)
-    if out.dims["wtd"]:
-        out.w_name_id[:] = np.concatenate([n for n in names if len(n)]).astype(np.uint32)
-    return out.validate()
 
 
 @pytest.mark.parametrize("random_delete", [False, True])
@@ -200,12 +121,15 @@ def test_workers_to_delete_past_slot_32(random_delete, oracle_mod):
     for x in (a, b):
         snap.c_flags[x] |= np.uint32(abi.CF_AUTOSCALING)
         g0 = int(snap.c_group_off[x])
-        own = _group_pods(snap, x, 41)
-        other = _group_pods(snap, x, 3)[0]  # a pod of another group of the same cluster
-        _scale_to(snap, g0 + 41, own.size - 1)
+        own = group_pods(snap, x, 41)
+        other = group_pods(snap, x, 3)[0]  # a pod of another group of the same cluster
+        scale_to(snap, g0 + 41, own.size - 1)
         lists[g0 + 41] = [snap.p_name_id[own[-1]], snap.p_name_id[other], 0x7F000000 + x]
-        lists[g0 + 35] = [snap.p_name_id[_workers(snap, x + 1)[0]]]  # a pod of another RayCluster
-    snap = _with_wtd(snap, lists)
+        lists[g0 + 35] = [snap.p_name_id[workers(snap, x + 1)[0]]]  # a pod of another RayCluster
+    new = lists_of(snap)
+    for g, names in lists.items():
+        new[g] = names
+    snap = with_wtd_lists(snap, new)
     got, names, stride = _parity(snap, flags, oracle_mod)
     _on_the_bucket_pipeline(names, stride)
     for x in (a, b):
@@ -220,10 +144,10 @@ def test_workers_to_delete_past_slot_32(random_delete, oracle_mod):
 def test_heads_and_suspend_inside_wide_clusters(oracle_mod):
     snap, flags, (a, b, c, _d) = _decision_fleet(5, wide=(0, 100, 200, 250))
     # a: a second head; b: an unhealthy head; c: worker group 44 suspended; 250: the whole RayCluster suspended
-    wa = _workers(snap, a)
+    wa = workers(snap, a)
     snap.p_packed[wa[7]] = (snap.p_packed[wa[7]] & ~np.uint32(3 << abi.PP_NODE_TYPE_SHIFT)) | np.uint32(abi.NT_HEAD << abi.PP_NODE_TYPE_SHIFT)
-    head_b = _members(snap, b)[((snap.p_packed[_members(snap, b)] >> abi.PP_NODE_TYPE_SHIFT) & 3) == abi.NT_HEAD]
-    _set_phase(snap, head_b, abi.PHASE_FAILED)
+    head_b = members(snap, b)[((snap.p_packed[members(snap, b)] >> abi.PP_NODE_TYPE_SHIFT) & 3) == abi.NT_HEAD]
+    set_phase(snap, head_b, abi.PHASE_FAILED)
     snap.g_flags[int(snap.c_group_off[c]) + 44] |= np.uint32(abi.GF_SUSPEND)
     snap.c_flags[250] |= np.uint32(abi.CF_SUSPEND)
     got, names, stride = _parity(snap, flags, oracle_mod)
@@ -231,30 +155,6 @@ def test_heads_and_suspend_inside_wide_clusters(oracle_mod):
     assert got.clusters["n_heads"][a] == 2 and got.clusters["head_action"][b] == abi.HEAD_DELETE
     _, codes = got.actions_of(c)
     assert abi.ACT_DELETE_GROUP_SUSPEND in codes.tolist()
-
-
-def _head_row(snap, c):
-    rows = np.flatnonzero(np.isin(snap.h_pod_idx, _members(snap, c)))
-    assert rows.size == 1
-    return int(rows[0])
-
-
-class WideDriver(Driver):
-    def __init__(self, snap, flags, large=False):
-        super().__init__(snap, flags, max_creates=1 << 16)
-        self.eng.set_wide_clusters(True)
-        if large:
-            self.eng.set_large_clusters(True)
-
-    def switch(self, new, rows_commit=True):
-        """Move to snapshot `new` (same row counts): its object part, then every pod row that differs."""
-        changed = np.zeros(new.dims["pods"], dtype=bool)
-        for col in POD_COLS:
-            changed |= self.snap.cols[col] != new.cols[col]
-        self.snap = new
-        if rows_commit:
-            self.commit_objects()
-        return np.flatnonzero(changed)
 
 
 @pytest.mark.parametrize("spin", [True, False])
@@ -267,15 +167,15 @@ def test_recreate_gates_inside_wide_clusters(spin, oracle_mod, monkeypatch):
     ah = snap.h_annot_hash.reshape(-1, 32)
     for cl, match in ((a, False), (b, True)):
         snap.c_flags[cl] |= np.uint32(abi.CF_UPGRADE_RECREATE)
-        h = _head_row(snap, cl)
+        h = head_row(snap, cl)
         snap.h_version_state[h] = abi.VER_CURRENT
         snap.h_annot_state[h] = abi.ANNOT_HASH32
-        digest = _b32(_spec(snap, cl)).encode()
+        digest = b32(spec_bytes(snap, cl))
         ah[h] = np.frombuffer(digest if match else digest[::-1], dtype=np.uint8)
     got, names, stride = _parity(snap, flags, oracle_mod)
     _on_the_bucket_pipeline(names, stride)
     assert got.clusters["path"][a] == abi.PATH_RECREATE_DELETE_ALL and got.clusters["path"][b] == abi.PATH_NORMAL
-    dr = WideDriver(snap, flags)
+    dr = Driver(snap, flags, max_creates=1 << 16, wide_clusters=True)
     try:
         dr.check(oracle_mod, expect_incremental=False)
         snap.json[int(snap.c_json_off[b]) + 3] ^= 0x20  # b's spec no longer matches its annotation
@@ -294,7 +194,7 @@ def test_multihost_groups_inside_a_wide_cluster(oracle_mod):
     snap = synthetic.widen_clusters(snap, [c], 40)  # every one of its first 40 groups multi-host, replicas spread over them
     for gate in (1, 0):
         flags.gate_multihost_indexing = gate
-        _, names, stride = _parity(snap, _compact(flags), oracle_mod)
+        _, names, stride = _parity(snap, compact(flags), oracle_mod)
         _on_the_bucket_pipeline(names, stride)
 
 
@@ -304,11 +204,11 @@ def test_wide_and_large_together(oracle_mod):
     snap, flags = synthetic.generate(synthetic.SynthParams(n_clusters=600, pods_per_cluster=20, groups=1, seed=11))
     synthetic.grow_clusters(snap, [10], 3000)
     snap = synthetic.widen_clusters(snap, [10], 40)
-    flags = _compact(flags)
-    got, names, stride = _parity(snap, flags, oracle_mod, large=True)
+    flags = compact(flags)
+    got, names, stride = _parity(snap, flags, oracle_mod, large_clusters=True)
     _on_the_bucket_pipeline(names, stride)
     assert got.clusters["n_pods"][10] == 3000
-    only_wide, names, stride = _run(snap, flags, True, profiled=True)
+    only_wide, names, stride = run(snap, flags, profiled=True, wide_clusters=True)
     assert not oracle_mod.run(snap, flags).diff(only_wide)
     assert "k_match2" not in names and "k_decide_large" not in names and stride == 0
 
@@ -318,30 +218,30 @@ def test_wide_and_large_together(oracle_mod):
 def test_incremental_epochs_in_wide_clusters(oracle_mod):
     snap, flags, big = _decision_fleet(6)
     rng = np.random.default_rng(3)
-    dr = WideDriver(snap, flags)
+    dr = Driver(snap, flags, max_creates=1 << 16, wide_clusters=True)
     try:
         dr.check(oracle_mod, expect_incremental=False)
         assert dr.eng.get_option(abi.OPT_BUCKET_STRIDE) == 64
         for epoch in range(6):
             rows = []
             # status flips and failures in groups >= 32
-            hi = np.concatenate([_group_pods(snap, big[0], gi) for gi in range(32, 48)])
+            hi = np.concatenate([group_pods(snap, big[0], gi) for gi in range(32, 48)])
             flip = rng.choice(hi, 6, replace=False)
             snap.p_packed[flip] ^= np.uint32(1 << abi.PP_READY_SHIFT); rows += flip.tolist()
-            fail = np.concatenate([_group_pods(snap, big[1], gi) for gi in (33, 40)])
-            _set_phase(snap, fail, abi.PHASE_FAILED if epoch % 2 == 0 else abi.PHASE_RUNNING); rows += fail.tolist()
+            fail = np.concatenate([group_pods(snap, big[1], gi) for gi in (33, 40)])
+            set_phase(snap, fail, abi.PHASE_FAILED if epoch % 2 == 0 else abi.PHASE_RUNNING); rows += fail.tolist()
             # a pod of group 45 deleted (a free row) and pods moving between a wide and an ordinary cluster, both ways (as many
             # leave big[2] as join it: its bucket holds 64 records and the stale ones leave only when the epoch compacts it)
-            gone = _group_pods(snap, big[2], 45)[:1]
+            gone = group_pods(snap, big[2], 45)[:1]
             for col in POD_COLS:
                 snap.cols[col][gone] = 0
             snap.p_packed[gone] = np.uint32(abi.PP_TOMBSTONE)
             rows += gone.tolist()
             small = int(rng.integers(1, 99))
-            out = _group_pods(snap, big[2], 33 + epoch)[:1]
+            out = group_pods(snap, big[2], 33 + epoch)[:1]
             snap.p_ns_id[out], snap.p_cluster_name_id[out] = snap.c_ns_id[small], snap.c_name_id[small]
             snap.p_group_name_id[out] = snap.g_name_id[snap.c_group_off[small]]
-            into = _workers(snap, small)[:1]
+            into = workers(snap, small)[:1]
             g = int(snap.c_group_off[big[2]]) + 40 + epoch
             snap.p_ns_id[into], snap.p_cluster_name_id[into] = snap.c_ns_id[big[2]], snap.c_name_id[big[2]]
             snap.p_group_name_id[into] = snap.g_name_id[g]
@@ -370,13 +270,13 @@ def test_dirty_wide_clusters_overflow_the_group_staging(oracle_mod):
     (2 880 groups) come back as whole arrays; 10 of them come back packed."""
     snap, flags = synthetic.generate(synthetic.SynthParams(n_clusters=200, pods_per_cluster=40, groups=1, seed=13))
     snap = synthetic.widen_clusters(snap, np.arange(200), 48)
-    flags = _compact(flags)
-    dr = WideDriver(snap, flags)
+    flags = compact(flags)
+    dr = Driver(snap, flags, max_creates=1 << 16, wide_clusters=True)
     try:
         dr.check(oracle_mod, expect_incremental=False)
         for n_dirty in (60, 10):
             dirty = np.arange(0, 200, 200 // n_dirty)[:n_dirty]
-            rows = np.concatenate([_group_pods(snap, c, 35)[:1] for c in dirty])  # (39 workers: groups 0..38 hold one each)
+            rows = np.concatenate([group_pods(snap, c, 35)[:1] for c in dirty])  # (39 workers: groups 0..38 hold one each)
             assert rows.size == n_dirty
             snap.p_packed[rows] ^= np.uint32(1 << abi.PP_READY_SHIFT)
             dr.commit_rows(rows)
@@ -399,17 +299,17 @@ def test_a_cluster_crossing_32_groups(first_wide, oracle_mod):
     """Clusters 5 and 6 trade worker groups (same group table size): 30 + 36 -> 34 + 32.  The epoch is structural, the full pass
     after it reclassifies, and the epochs after that are incremental again."""
     base, flags = synthetic.generate(synthetic.SynthParams(n_clusters=300, pods_per_cluster=40, groups=1, seed=14))
-    flags = _compact(flags)
+    flags = compact(flags)
     a = _grouped(base, {5: 30, 6: 36})
     b = _grouped(base, {5: 34, 6: 32})
     start, end = (a, b) if first_wide else (b, a)
-    dr = WideDriver(start, flags)
+    dr = Driver(start, flags, max_creates=1 << 16, wide_clusters=True)
     try:
         dr.check(oracle_mod, expect_incremental=False)
         rows = dr.switch(end)
         dr.commit_rows(rows)
         dr.check(oracle_mod, expect_incremental=False)
-        flip = np.concatenate([_workers(end, 5)[::7], _workers(end, 6)[::7]])
+        flip = np.concatenate([workers(end, 5)[::7], workers(end, 6)[::7]])
         end.p_packed[flip] ^= np.uint32(1 << abi.PP_READY_SHIFT)
         dr.commit_rows(flip)
         dr.check(oracle_mod, expect_incremental=True)
@@ -422,14 +322,14 @@ def test_the_first_wide_cluster_appears_and_the_last_leaves(entry, oracle_mod):
     """Clusters 5 and 6 go from 30 + 4 groups to 33 + 1 (the snapshot's first wide RayCluster) and back, through
     kr_snapshot_commit_parts(KR_PART_OBJECTS) or kr_snapshot_commit_object_rows."""
     base, flags = synthetic.generate(synthetic.SynthParams(n_clusters=300, pods_per_cluster=40, groups=1, seed=15))
-    flags = _compact(flags)
+    flags = compact(flags)
     narrow = _grouped(base, {5: 30, 6: 4})
     wide = _grouped(base, {5: 33})
-    dr = WideDriver(narrow, flags)
+    dr = Driver(narrow, flags, max_creates=1 << 16, wide_clusters=True)
     try:
         got, _ = dr.check(oracle_mod, expect_incremental=False)
         for nxt in (wide, narrow):
-            rows = dr.switch(nxt, rows_commit=entry == "parts")
+            rows = dr.switch(nxt, commit=entry == "parts")
             if entry == "rows":
                 for col in OBJ_COLS:
                     np.copyto(dr.views[col], nxt.cols[col])
@@ -439,7 +339,7 @@ def test_the_first_wide_cluster_appears_and_the_last_leaves(entry, oracle_mod):
             names = {k for k, _ in dr.eng.reconcile_profiled(dr.flags)["kernels"]}  # (an epoch without changes)
             assert ("k_decide_large" in names) == (nxt is wide)
             dr.eng.fetch()  # (an unfetched epoch makes the next one return every record)
-            flip = _workers(nxt, 5)[::5]
+            flip = workers(nxt, 5)[::5]
             nxt.p_packed[flip] ^= np.uint32(1 << abi.PP_READY_SHIFT)
             dr.commit_rows(flip)
             dr.check(oracle_mod, expect_incremental=True)
@@ -471,11 +371,7 @@ def test_native_packer_keeps_incremental_epochs_with_a_wide_cluster(oracle_mod):
     """A fleet with a RayCluster of 40 worker groups behind the native packer, KR_OPT_WIDE_CLUSTERS set through kr_packer_engine:
     every epoch equals the oracle and the pod-row epochs stay incremental on the device."""
     rng = np.random.default_rng(37)
-    clusters, pods, jobs = fuzz_objects.generate(5, max_clusters=16)
-    for i, c in enumerate(clusters):
-        c["generation"], c["resourceVersion"] = 1, 100 + i
-    for i, j in enumerate(jobs):
-        j.setdefault("name", f"rayjob-{i}")
+    clusters, pods, jobs = objects(5, max_clusters=16)
     spec_groups = {(c["namespace"], c["name"], g["groupName"]): (c, g) for c in clusters for g in c["spec"]["workerGroupSpecs"]}
     owner = next(k for k, _ in collections.Counter((p.get("namespace"), p["labels"].get("ray.io/cluster"), p["labels"].get("ray.io/group"))
                                                    for p in pods if p["labels"].get("ray.io/node-type") == "worker").most_common()
@@ -491,20 +387,15 @@ def test_native_packer_keeps_incremental_epochs_with_a_wide_cluster(oracle_mod):
     members = [p for p in pods if (p.get("namespace"), p["labels"].get("ray.io/cluster"), p["labels"].get("ray.io/group")) == owner]
     for i, p in enumerate(members):
         p["labels"]["ray.io/group"] = groups[i % len(groups)]["groupName"]
-    pk = Packer(max_clusters=64, max_groups=512, max_wtd=512, max_pods=4096, max_heads=256, max_jobs=64, max_creates=1 << 16,
-                max_json_bytes=4 << 20, wide_clusters=True)
+    pk = Packer(**PACKER_CAPS, wide_clusters=True)
     try:
         m = Mirror(copy.deepcopy(clusters), copy.deepcopy(pods), jobs, pk)
         pk.flush()
         _, first = packer_check(m, oracle_mod, lean=True)
         assert pk.engine.get_option(abi.OPT_WIDE_CLUSTERS) == 1 and pk.engine.get_option(abi.OPT_BUCKET_STRIDE) != 0
         counter = [0]
-        incremental, modes = [], []
-        for _ in range(10):
-            _events(rng, m, counter, structural=False)
-            modes.append(pk.flush())
-            _, got = packer_check(m, oracle_mod, lean=True)
-            incremental.append(got.changed_clusters is not None or got.n_changed == 0)
+        gots, modes = packer_stream(m, oracle_mod, 10, lambda epoch: events(rng, m, counter, structural=False))
+        incremental = [device_incremental(g) for g in gots]
         assert any(mo & abi.PACK_POD_ROWS for mo in modes)
         assert incremental[0] and sum(incremental) >= 5, incremental
     finally:

@@ -9,121 +9,20 @@ import copy
 import numpy as np
 import pytest
 
-import fuzz_objects
+from harness import (PACKER_CAPS, POD_COLS, REBUILD, Driver, Mirror, arena_stream, autoscale_objects, device_incremental, events, flip_ready,
+                     incremental, lists_of, objects, packer_check, packer_stream, with_wtd_lists, workers_of)
 from kuberay_b200 import abi, synthetic
-from kuberay_b200.engine import Engine
 from kuberay_b200.live import LiveArena
 from kuberay_b200.packer import Packer
-from kuberay_b200.snapshot import Snapshot
-from test_gpu_incremental import OBJ_COLS, POD_COLS, _flip_ready
-from test_live_arena import L_CLUSTER, L_GROUP, L_TYPE, _events
-from test_packer import Mirror, check as packer_check
 
 pytestmark = pytest.mark.gpu
 
 GHOST = 0x7FFE0000      # name ids no Pod carries
-REBUILD = ("k_inc_wtd_release", "k_inc_wtd_clear", "k_inc_wtd_insert", "k_inc_wtd_resolve")
 
 
-def lists_of(snap):
-    off, cnt, w = snap.g_wtd_off, snap.g_wtd_cnt, snap.w_name_id
-    return [w[int(off[g]):int(off[g]) + int(cnt[g])].tolist() for g in range(snap.dims["groups"])]
-
-
-def with_lists(snap, lists):
-    """A copy of `snap` whose workersToDelete lists are `lists` (one list of name ids per group row)."""
-    d = snap.dims
-    cnt = np.array([len(x) for x in lists], dtype=np.uint32)
-    out = Snapshot(d["clusters"], d["groups"], int(cnt.sum()), d["pods"], d["heads"], d["jobs"], d["json"])
-    for name, _dt, _m, dim in abi.COLUMNS:
-        if dim != "wtd":
-            out.cols[name][:] = snap.cols[name]
-    out.g_wtd_cnt[:] = cnt
-    out.g_wtd_off[:] = np.concatenate([[0], np.cumsum(cnt)[:-1]]).astype(np.uint32) if cnt.size else 0
-    out.w_name_id[:] = np.array([x for lst in lists for x in lst], dtype=np.uint32)
-    return out
-
-
-def live(snap):
-    return (snap.p_packed & abi.PP_TOMBSTONE) == 0
-
-
-def workers_of(snap, g, running=False):
-    """Live worker rows of group row g."""
-    c = int(snap.g_cluster_idx[g])
-    pk = snap.p_packed
-    m = live(snap) & (((pk >> abi.PP_NODE_TYPE_SHIFT) & 3) == abi.NT_WORKER) & (snap.p_ns_id == snap.c_ns_id[c]) & \
-        (snap.p_cluster_name_id == snap.c_name_id[c]) & (snap.p_group_name_id == snap.g_name_id[g])
-    if running:
-        m &= ((pk >> abi.PP_PHASE_SHIFT) & 7) == abi.PHASE_RUNNING
-    return np.flatnonzero(m)
-
-
-class WtdDriver:
+def _driver(snap, flags, wtd_edits=True, **opts):
     """Fixed layout with room for the lists to grow; KR_OPT_WTD_EDITS on unless told otherwise; `opts` turns on other options."""
-
-    def __init__(self, snap, flags, wtd_edits=True, wtd_room=512, **opts):
-        d = snap.dims
-        self.snap, self.flags = snap, flags
-        flags.fetch_pod_lists = 0
-        up = lambda x: int(x * 1.25) + 16  # noqa: E731
-        self.eng = Engine(0, up(d["clusters"]), up(d["groups"]), d["wtd"] + wtd_room, up(d["pods"]), up(d["heads"]), up(d["jobs"]),
-                          4 * d["pods"] + 4096, up(d["json"]))
-        for k, v in opts.items():
-            getattr(self.eng, f"set_{k}")(v)
-        self.eng.set_wtd_edits(wtd_edits)
-        self.eng.set_fixed_layout(True)
-        self.views = self.eng.begin(snap.sizes())
-        self.eng.fill(self.views, snap)
-        self.eng.commit()
-        self.prev = None
-
-    def set_lists(self, lists, commit=True):
-        new = with_lists(self.snap, lists)
-        if new.dims["wtd"] != self.snap.dims["wtd"]:
-            self.views = self.eng.begin(new.sizes())
-        self.snap = new
-        if commit:
-            self.commit_objects()
-
-    def commit_objects(self):
-        for c in OBJ_COLS:
-            np.copyto(self.views[c], self.snap.cols[c])
-        self.eng.commit(abi.PART_OBJECTS)
-
-    def commit_rows(self, rows):
-        rows = np.unique(np.asarray(rows, dtype=np.uint32))
-        if rows.size:
-            for c in POD_COLS:
-                self.views[c][rows] = self.snap.cols[c][rows]
-            self.eng.commit_pod_values(rows, np.stack([self.snap.cols[c][rows].view(np.uint32) for c in POD_COLS], axis=1))
-
-    def check(self, oracle_mod, expect_incremental=None, profiled=False):
-        names = []
-        if profiled:
-            names = [k for k, _ in self.eng.reconcile_profiled(self.flags)["kernels"]]
-            got = self.eng.fetch()
-        else:
-            got = self.eng.reconcile(self.flags)
-        d = oracle_mod.run(self.snap, self.flags).diff(got)
-        assert not d, (d[:6], got.n_changed)
-        nc = self.snap.dims["clusters"]
-        inc = got.changed_clusters is not None or got.n_changed < nc
-        if expect_incremental is not None:
-            assert inc == expect_incremental, (inc, got.n_changed, names)
-        if inc and self.prev is not None:  # records the pass did not name are unchanged since the previous epoch
-            same = np.ones(nc, dtype=bool)
-            if got.changed_clusters is not None:
-                same[got.changed_clusters] = False
-            assert np.array_equal(got.clusters[same], self.prev.clusters[same])
-            assert np.array_equal(got.act_cnt[same], self.prev.act_cnt[same])
-            gs = same[self.snap.g_cluster_idx]
-            assert np.array_equal(got.groups[gs], self.prev.groups[gs])
-        self.prev = got
-        return got, names
-
-    def close(self):
-        self.eng.close()
+    return Driver(snap, flags, wtd_room=512, **opts, wtd_edits=wtd_edits)
 
 
 def _snap(seed, **kw):
@@ -142,7 +41,7 @@ def _action_of(got, c, row):
 @pytest.mark.parametrize("target", ["own", "other_group", "nowhere", "orphan"])
 def test_rename_in_place(target, oracle_mod):
     snap, flags = _snap(3)
-    dr = WtdDriver(snap, flags)
+    dr = _driver(snap, flags)
     try:
         dr.check(oracle_mod, expect_incremental=False)
         lists = lists_of(dr.snap)
@@ -166,7 +65,7 @@ def test_rename_in_place(target, oracle_mod):
             dr.check(oracle_mod, expect_incremental=True)
         for g in gs:
             lists[g][0] = GHOST + 100 + g if target == "nowhere" else int(dr.snap.p_name_id[pick[g]])
-        dr.set_lists(lists)
+        dr.set_wtd_lists(lists)
         got, names = dr.check(oracle_mod, expect_incremental=True, profiled=True)
         assert set(REBUILD) <= set(names), names
         for g in gs:
@@ -179,7 +78,7 @@ def test_rename_in_place(target, oracle_mod):
                 assert _action_of(got, int(snap.g_cluster_idx[g]), pick[g]) != abi.ACT_DELETE_WTD
         for g in gs:
             lists[g][0] = old[g]
-        dr.set_lists(lists)
+        dr.set_wtd_lists(lists)
         dr.check(oracle_mod, expect_incremental=True)
     finally:
         dr.close()
@@ -190,7 +89,7 @@ def test_lists_grow_from_empty_and_shrink_to_empty(oracle_mod):
     snapshot move, and an edit of the first group shifts every later offset."""
     snap, flags = _snap(4, wtd_group_frac=0.0)
     assert snap.dims["wtd"] == 0
-    dr = WtdDriver(snap, flags)
+    dr = _driver(snap, flags)
     try:
         dr.check(oracle_mod, expect_incremental=False)
         G = snap.dims["groups"]
@@ -199,22 +98,22 @@ def test_lists_grow_from_empty_and_shrink_to_empty(oracle_mod):
         lists = [[] for _ in range(G)]
         lists[first] = [int(snap.p_name_id[r]) for r in workers_of(snap, first)[:2]]
         lists[last] = [int(snap.p_name_id[workers_of(snap, last)[-1]])]
-        dr.set_lists(lists)
+        dr.set_wtd_lists(lists)
         _, names = dr.check(oracle_mod, expect_incremental=True, profiled=True)
         assert "k_inc_wtd_resolve" in names and "k_inc_wtd_release" not in names, names   # (no old names to release)
         lists[mid] = [int(snap.p_name_id[r]) for r in workers_of(snap, mid)[:3]] + [GHOST]
         lists[first] = lists[first][1:]                                       # every later offset moves
-        dr.set_lists(lists)
+        dr.set_wtd_lists(lists)
         dr.check(oracle_mod, expect_incremental=True)
         lists[first] = [int(snap.p_name_id[r]) for r in workers_of(snap, first)[1:4]]
         lists[last] = []
-        dr.set_lists(lists)
+        dr.set_wtd_lists(lists)
         dr.check(oracle_mod, expect_incremental=True)
-        dr.set_lists([[] for _ in range(G)])
+        dr.set_wtd_lists([[] for _ in range(G)])
         _, names = dr.check(oracle_mod, expect_incremental=True, profiled=True)
         assert "k_inc_wtd_release" in names and "k_inc_wtd_resolve" not in names, names
         rows = np.arange(3, snap.dims["pods"], 97, dtype=np.uint32)
-        _flip_ready(dr.snap, rows)
+        flip_ready(dr.snap, rows)
         dr.commit_rows(rows)
         _, names = dr.check(oracle_mod, expect_incremental=True, profiled=True)
         assert not set(REBUILD) & set(names), names                           # an epoch without an edit rebuilds nothing
@@ -226,7 +125,7 @@ def test_lists_grow_from_empty_and_shrink_to_empty(oracle_mod):
 
 def test_duplicate_names(oracle_mod):
     snap, flags = _snap(5)
-    dr = WtdDriver(snap, flags)
+    dr = _driver(snap, flags)
     try:
         dr.check(oracle_mod, expect_incremental=False)
         lists = lists_of(dr.snap)
@@ -238,12 +137,12 @@ def test_duplicate_names(oracle_mod):
             x = int(snap.p_name_id[workers_of(snap, a)[0]])
             lists[a] = [x, x] + lists[a]          # twice in its own group's list
             lists[b] = lists[b] + [x]             # and in another group's
-        dr.set_lists(lists)
+        dr.set_wtd_lists(lists)
         dr.check(oracle_mod, expect_incremental=True)
         for c in multi:
             a = int(snap.c_group_off[c])
             lists[a] = lists[a][1:]
-        dr.set_lists(lists)
+        dr.set_wtd_lists(lists)
         dr.check(oracle_mod, expect_incremental=True)
     finally:
         dr.close()
@@ -253,7 +152,7 @@ def test_duplicate_names(oracle_mod):
 @pytest.mark.parametrize("what", ["deleted", "readded", "moved"])
 def test_named_pod_changes_in_the_same_epoch(what, pods_first, oracle_mod):
     snap, flags = _snap(6)
-    dr = WtdDriver(snap, flags)
+    dr = _driver(snap, flags)
     try:
         dr.check(oracle_mod, expect_incremental=False)
         s = dr.snap
@@ -269,7 +168,7 @@ def test_named_pod_changes_in_the_same_epoch(what, pods_first, oracle_mod):
         named = [int(workers_of(s, g)[0]) for g in gs]
         for g, r in zip(gs, named):
             lists[g][0] = int(s.p_name_id[r])
-        new = with_lists(s, lists)
+        new = with_wtd_lists(s, lists)
         rows = list(named)
         if what == "deleted":
             for c in POD_COLS:
@@ -288,9 +187,7 @@ def test_named_pod_changes_in_the_same_epoch(what, pods_first, oracle_mod):
                 c2 = int(others[0])
                 new.p_cluster_name_id[r] = new.c_name_id[c2]
                 new.p_group_name_id[r] = new.g_name_id[int(new.c_group_off[c2])]
-        dr.snap = new
-        if new.dims["wtd"] != s.dims["wtd"]:
-            dr.views = dr.eng.begin(new.sizes())
+        dr.use(new)
         if pods_first:
             dr.commit_rows(rows)
             dr.commit_objects()
@@ -298,7 +195,7 @@ def test_named_pod_changes_in_the_same_epoch(what, pods_first, oracle_mod):
             dr.commit_objects()
             dr.commit_rows(rows)
         dr.check(oracle_mod, expect_incremental=True)
-        dr.set_lists([[] for _ in range(s.dims["groups"])])
+        dr.set_wtd_lists([[] for _ in range(s.dims["groups"])])
         dr.check(oracle_mod, expect_incremental=True)
     finally:
         dr.close()
@@ -310,7 +207,7 @@ def test_multihost_lists(oracle_mod):
     snap, flags = synthetic.generate(synthetic.SynthParams(n_clusters=300, pods_per_cluster=42, groups=2, multihost_frac=0.5, autoscaling_frac=1.0,
                                                            wtd_group_frac=0.3, seed=7))
     assert flags.gate_multihost_indexing == 1
-    dr = WtdDriver(snap, flags)
+    dr = _driver(snap, flags)
     try:
         dr.check(oracle_mod, expect_incremental=False)
         lists = lists_of(snap)
@@ -319,17 +216,17 @@ def test_multihost_lists(oracle_mod):
         assert named and ghosts
         for g in named:
             lists[g] = [int(snap.p_name_id[workers_of(snap, g)[4]])]
-        dr.set_lists(lists)
+        dr.set_wtd_lists(lists)
         got, _ = dr.check(oracle_mod, expect_incremental=True)
         assert (got.clusters["err_kind"][snap.g_cluster_idx[named]] == abi.ERR_MH_WTD).any()
         for g in ghosts:
             lists[g] = [GHOST + g]
-        dr.set_lists(lists)
+        dr.set_wtd_lists(lists)
         got, _ = dr.check(oracle_mod, expect_incremental=True)
         assert (got.groups["flags"][ghosts] & abi.GR_WTD_EXECUTED).any()
         for g in named + ghosts:
             lists[g] = []
-        dr.set_lists(lists)
+        dr.set_wtd_lists(lists)
         got, _ = dr.check(oracle_mod, expect_incremental=True)
         assert not (got.groups["flags"][ghosts] & abi.GR_WTD_EXECUTED).any()
     finally:
@@ -344,7 +241,7 @@ def test_edits_inside_large_huge_wide_and_recreate_clusters(oracle_mod):
     synthetic.grow_clusters(snap, [large], 600)
     g35 = int(snap.c_group_off[large]) + 35
     snap.p_group_name_id[workers_of(snap, int(snap.c_group_off[large]))[:6]] = snap.g_name_id[g35]
-    dr = WtdDriver(snap, flags, large_clusters=True, wide_clusters=True, huge_clusters=True)
+    dr = _driver(snap, flags, large_clusters=True, wide_clusters=True, huge_clusters=True)
     try:
         _, names = dr.check(oracle_mod, expect_incremental=False, profiled=True)
         assert dr.eng.get_option(abi.OPT_BUCKET_STRIDE) != 0 and "k_huge_merge" in names, names
@@ -361,17 +258,16 @@ def test_edits_inside_large_huge_wide_and_recreate_clusters(oracle_mod):
         for g, rows in edits.items():
             assert rows.size
             lists[g] = [int(s.p_name_id[r]) for r in rows]
-        dr.set_lists(lists)
+        dr.set_wtd_lists(lists)
         _, names = dr.check(oracle_mod, expect_incremental=True, profiled=True)
         assert {"k_inc_wtd_resolve", "k_decide_large", "k_huge_merge"} <= set(names), names
         # the autoscaler's next step: the named Pods are gone and the lists are cleared
-        new = with_lists(dr.snap, [[] if g in edits else lst for g, lst in enumerate(lists)])
+        new = with_wtd_lists(dr.snap, [[] if g in edits else lst for g, lst in enumerate(lists)])
         gone = np.concatenate(list(edits.values()))
         for c in POD_COLS:
             new.cols[c][gone] = 0
         new.p_packed[gone] = np.uint32(abi.PP_TOMBSTONE)
-        dr.views = dr.eng.begin(new.sizes())
-        dr.snap = new
+        dr.use(new)
         dr.commit_objects()
         dr.commit_rows(gone)
         dr.check(oracle_mod, expect_incremental=True)
@@ -381,7 +277,7 @@ def test_edits_inside_large_huge_wide_and_recreate_clusters(oracle_mod):
 
 def test_option_toggled_mid_stream(oracle_mod):
     snap, flags = _snap(9)
-    dr = WtdDriver(snap, flags, wtd_edits=False)
+    dr = _driver(snap, flags, wtd_edits=False)
     try:
         assert dr.eng.get_option(abi.OPT_WTD_EDITS) == 0
         dr.check(oracle_mod, expect_incremental=False)
@@ -391,7 +287,7 @@ def test_option_toggled_mid_stream(oracle_mod):
         def edit(k):
             for g in gs:
                 lists[g] = [int(snap.p_name_id[r]) for r in workers_of(snap, g)[:k]]
-            dr.set_lists(lists)
+            dr.set_wtd_lists(lists)
 
         for step, (on, k) in enumerate([(False, 1), (True, 2), (True, 2), (False, 2), (True, 1), (True, 0), (False, 1)]):
             dr.eng.set_wtd_edits(on)
@@ -399,12 +295,12 @@ def test_option_toggled_mid_stream(oracle_mod):
             if step == 2:                           # a rename: same lengths, other names
                 for g in gs:
                     lists[g] = [int(snap.p_name_id[r]) for r in workers_of(snap, g)[1:3]]
-                dr.set_lists(lists)
+                dr.set_wtd_lists(lists)
             else:
                 edit(k)
             dr.check(oracle_mod, expect_incremental=on)   # with the option off the same edit takes the full pass, as before
             rows = np.arange(step, snap.dims["pods"], 131, dtype=np.uint32)
-            _flip_ready(dr.snap, rows)
+            flip_ready(dr.snap, rows)
             dr.commit_rows(rows)
             dr.check(oracle_mod, expect_incremental=True)
     finally:
@@ -443,20 +339,18 @@ def _autoscale_arrays(rng, dr, pending):
 def test_stream_through_the_engine(seed, oracle_mod):
     rng = np.random.default_rng(seed)
     snap, flags = _snap(20 + seed, n_clusters=400, groups=2, wtd_group_frac=0.1)
-    dr = WtdDriver(snap, flags)
+    dr = _driver(snap, flags)
     try:
         dr.check(oracle_mod, expect_incremental=False)
         pending = {}
         n_inc = 0
         for epoch in range(40):
             lists, rows = _autoscale_arrays(rng, dr, pending)
-            new = with_lists(dr.snap, lists)
+            new = with_wtd_lists(dr.snap, lists)
             # informer churn: 1 % PodReady flips
-            flip = rng.choice(np.flatnonzero(live(new)), max(1, new.dims["pods"] // 100), replace=False)
-            _flip_ready(new, flip)
-            if new.dims["wtd"] != dr.snap.dims["wtd"]:
-                dr.views = dr.eng.begin(new.sizes())
-            dr.snap = new
+            flip = rng.choice(np.flatnonzero((new.p_packed & abi.PP_TOMBSTONE) == 0), max(1, new.dims["pods"] // 100), replace=False)
+            flip_ready(new, flip)
+            dr.use(new)
             if epoch % 2:
                 dr.commit_rows(rows + flip.tolist())
                 dr.commit_objects()
@@ -464,72 +358,30 @@ def test_stream_through_the_engine(seed, oracle_mod):
                 dr.commit_objects()
                 dr.commit_rows(rows + flip.tolist())
             got, _ = dr.check(oracle_mod)
-            n_inc += got.changed_clusters is not None or got.n_changed < new.dims["clusters"]
+            n_inc += incremental(got, new.dims["clusters"])
         # (an epoch may still take the full pass for a reason of its own: the action list full of abandoned runs is packed again)
         assert n_inc >= 38, n_inc
     finally:
         dr.close()
 
 
-def _autoscale_objects(rng, side, pending):
-    """The same traffic on informer objects (native packer / LiveArena): delete last epoch's named Pods and clear the lists, then
-    name 1-3 own workers of one or two groups and lower their replicas."""
-    for key, (gname, names) in list(pending.items()):
-        for nm in names:
-            side.delete_pod(key[0], nm)
-        c = copy.deepcopy(side.clusters[key])
-        for g in c["spec"].get("workerGroupSpecs") or []:
-            if g["groupName"] == gname:
-                g["workersToDelete"] = []
-        side.upsert_cluster(c)
-    pending.clear()
-    keys = sorted(side.clusters)
-    for _ in range(int(rng.integers(1, 3))):
-        key = keys[int(rng.integers(len(keys)))]
-        c = copy.deepcopy(side.clusters[key])
-        groups = c["spec"].get("workerGroupSpecs") or []
-        if not groups:
-            continue
-        g = groups[int(rng.integers(len(groups)))]
-        mine = [p["name"] for p in side.rows if p is not None and p.get("namespace", "default") == key[0] and (p.get("labels") or {}).get(L_CLUSTER) == key[1]
-                and (p.get("labels") or {}).get(L_GROUP) == g["groupName"] and (p.get("labels") or {}).get(L_TYPE) != "head"]
-        if not mine:
-            continue
-        names = [mine[i] for i in rng.choice(len(mine), min(len(mine), int(rng.integers(1, 4))), replace=False)]
-        g["workersToDelete"] = names
-        if isinstance(g.get("replicas"), int):
-            g["replicas"] = max(0, g["replicas"] - len(names))
-        side.upsert_cluster(c)
-        pending[key] = (g["groupName"], names)
-
-
-def _objects(seed):
-    clusters, pods, jobs = fuzz_objects.generate(seed, big=True)
-    for i, c in enumerate(clusters):
-        c["generation"], c["resourceVersion"] = 1, 100 + i
-    for i, j in enumerate(jobs):
-        j.setdefault("name", f"rayjob-{i}")
-    return clusters, pods, jobs
-
-
 @pytest.mark.parametrize("seed", [1, 2, 3])
 def test_stream_through_the_native_packer(seed, oracle_mod):
     rng = np.random.default_rng(seed)
-    clusters, pods, jobs = _objects(seed)
-    pk = Packer(max_clusters=64, max_groups=512, max_wtd=512, max_pods=4096, max_heads=256, max_jobs=64, max_creates=1 << 16,
-                max_json_bytes=4 << 20, wtd_edits=True)
+    clusters, pods, jobs = objects(seed, big=True)
+    pk = Packer(**PACKER_CAPS, wtd_edits=True)
     try:
         assert pk.engine.get_option(abi.OPT_WTD_EDITS) == 1
         m = Mirror(copy.deepcopy(clusters), copy.deepcopy(pods), jobs, pk)
         pk.flush()
         packer_check(m, oracle_mod, lean=True)
-        pending, counter, inc = {}, [0], []
-        for epoch in range(40):
-            _autoscale_objects(rng, m, pending)
-            _events(rng, m, counter, structural=False)
-            pk.flush()
-            _, got = packer_check(m, oracle_mod, lean=True)
-            inc.append(got.changed_clusters is not None or got.n_changed == 0)
+        pending, counter = {}, [0]
+
+        def step(epoch):
+            autoscale_objects(rng, m, pending)
+            events(rng, m, counter, structural=False)
+        gots, _ = packer_stream(m, oracle_mod, 40, step)
+        inc = [device_incremental(g) for g in gots]
         assert sum(inc) >= 36, inc
     finally:
         pk.close()
@@ -538,20 +390,15 @@ def test_stream_through_the_native_packer(seed, oracle_mod):
 @pytest.mark.parametrize("seed", [1, 2, 3])
 def test_stream_through_the_live_arena(seed, oracle_mod):
     rng = np.random.default_rng(seed)
-    clusters, pods, jobs = _objects(seed)
+    clusters, pods, jobs = objects(seed, big=True)
     arena = LiveArena(clusters, pods, jobs, spare_rows=64, wtd_edits=True)
     try:
-        pending, counter, inc = {}, [0], []
-        for epoch in range(40):
-            _autoscale_objects(rng, arena, pending)
-            _events(rng, arena, counter, structural=False)
-            arena.flush()
-            flags = arena.meta.flags
-            flags.fetch_pod_lists = 0
-            got = arena.reconcile(flags)
-            d = oracle_mod.run(arena.snap, flags).diff(got)
-            assert not d, (epoch, d[:6])
-            inc.append(got.changed_clusters is not None or got.n_changed == 0)
+        pending, counter = {}, [0]
+
+        def step(epoch):
+            autoscale_objects(rng, arena, pending)
+            events(rng, arena, counter, structural=False)
+        inc = [device_incremental(g) for g in arena_stream(arena, oracle_mod, 40, step)]
         assert arena.engine.get_option(abi.OPT_WTD_EDITS) == 1
         assert sum(inc) >= 34 and arena.stats["rebase"] <= 2, (inc, arena.stats)
     finally:

@@ -5,59 +5,13 @@ CPU: an arena with free rows must decide exactly like the same objects packed fr
 GPU: after every epoch of random events the engine (kr_snapshot_commit_parts(KR_PART_OBJECTS) + kr_snapshot_commit_pod_rows)
 must equal the oracle on the arena byte for byte, and most epochs must take the incremental path.
 """
-import copy
-
 import numpy as np
 import pytest
 
 import fuzz_objects
+from harness import events
 from kuberay_b200 import abi
 from kuberay_b200.live import LiveArena
-
-L_TYPE, L_GROUP, L_CLUSTER = "ray.io/node-type", "ray.io/group", "ray.io/cluster"
-
-
-def _events(rng, live: LiveArena, counter: list, structural: bool):
-    """A handful of informer events; `structural` allows the ones that move a table's row count."""
-    pods = [p for p in live.rows if p is not None]
-    for _ in range(int(rng.integers(1, 8))):
-        kind = rng.random()
-        workers = [p for p in pods if (p.get("labels") or {}).get(L_TYPE) != "head" and (p["namespace"], p["name"]) in live.row_of]
-        if kind < 0.35 and pods:  # status update
-            p = copy.deepcopy(pods[int(rng.integers(len(pods)))])
-            if (p["namespace"], p["name"]) not in live.row_of:
-                continue
-            p["phase"] = ["Running", "Pending", "Failed", "Succeeded"][int(rng.integers(4))]
-            p["conditions"] = [{"type": "Ready", "status": ["True", "False"][int(rng.integers(2))]}]
-            live.upsert_pod(p)
-        elif kind < 0.55 and workers:  # pod deleted
-            p = workers[int(rng.integers(len(workers)))]
-            live.delete_pod(p["namespace"], p["name"])
-        elif kind < 0.8 and workers:  # pod created (same labels as an existing worker)
-            src = workers[int(rng.integers(len(workers)))]
-            counter[0] += 1
-            live.upsert_pod({"namespace": src["namespace"], "name": f"new{counter[0]}", "labels": dict(src["labels"]), "phase": "Pending",
-                             "restartPolicy": "Always"})
-        elif kind < 0.95:  # RayCluster spec / status change that keeps every table's row count
-            key = sorted(live.clusters)[int(rng.integers(len(live.clusters)))]
-            c = copy.deepcopy(live.clusters[key])
-            groups = c["spec"].get("workerGroupSpecs") or []
-            if groups:
-                g = groups[int(rng.integers(len(groups)))]
-                g["replicas"] = int(rng.integers(0, 7))
-            c.setdefault("status", {})["readyWorkerReplicas"] = int(rng.integers(0, 5))
-            c["expectations"] = {k: bool(rng.random() < 0.9) for k in (c.get("expectations") or {"head": True})}
-            live.upsert_cluster(c)
-        elif structural:
-            heads = [p for p in pods if (p.get("labels") or {}).get(L_TYPE) == "head" and (p["namespace"], p["name"]) in live.row_of]
-            if heads and rng.random() < 0.5:
-                h = heads[int(rng.integers(len(heads)))]
-                live.delete_pod(h["namespace"], h["name"])
-            else:
-                key = sorted(live.clusters)[int(rng.integers(len(live.clusters)))]
-                counter[0] += 1
-                live.upsert_pod({"namespace": key[0], "name": f"head{counter[0]}", "labels": {L_CLUSTER: key[1], L_TYPE: "head", L_GROUP: "headgroup"},
-                                 "phase": "Running", "conditions": [{"type": "Ready", "status": "True"}], "podIP": "10.9.9.9"})
 
 
 def _same_decisions(arena_snap, a: abi.Results, fresh_snap, b: abi.Results, rows):
@@ -91,7 +45,7 @@ def test_arena_with_free_rows_decides_like_a_fresh_pack(seed, oracle_mod):
     live = LiveArena(clusters, pods, jobs, spare_rows=6, engine=False)
     counter = [0]
     for epoch in range(12):
-        _events(rng, live, counter, structural=True)
+        events(rng, live, counter, structural=True)
         live.flush()
         a = oracle_mod.run(live.snap, live.meta.flags)
         fresh, fmeta = live.fresh_pack()
@@ -113,7 +67,7 @@ def test_incremental_epochs_match_the_oracle(seed, lean, oracle_mod):
     device_incremental = 0
     try:
         for epoch in range(25):
-            _events(rng, live, counter, structural=(epoch % 8 == 7))
+            events(rng, live, counter, structural=(epoch % 8 == 7))
             live.flush()
             flags = live.meta.flags
             flags.fetch_pod_lists = 0 if lean else 1

@@ -1,7 +1,7 @@
 #!/usr/bin/env python
 """A longer run of the native packer's random informer-event streams than tests/test_packer.py affords (4 seeds x 10 epochs there): per seed a
 fuzz-generated object set, then epochs of mixed Pod / RayCluster / RayJob events — structural ones included — through kr_packer_*, every
-epoch compared with the oracle on an independently re-packed snapshot (the test's own Mirror / check).  usage (GPU box):
+epoch compared with the oracle on an independently re-packed snapshot (tests/harness.py's Mirror / packer_check).  usage (GPU box):
 python tools/packer_soak.py [first_seed] [seeds] [epochs] [--all-options] [--json-bytes N]
 
 --all-options turns on every opt-in engine option (large / wide / huge RayClusters, workersToDelete edits, spec rows) and adds spec edits
@@ -17,12 +17,10 @@ import numpy as np
 ROOT = os.path.dirname(os.path.dirname(os.path.abspath(__file__)))
 sys.path.insert(0, ROOT)
 sys.path.insert(0, os.path.join(ROOT, "tests"))
-import fuzz_objects  # noqa: E402
-import test_packer as tp  # noqa: E402
+from harness import PACKER_CAPS, Mirror, events, objects, packer_check, spec_edits  # noqa: E402
 from kuberay_b200 import abi  # noqa: E402
 from kuberay_b200.packer import Packer  # noqa: E402
 from oracle import oracle  # noqa: E402
-from test_gpu_spec_rows import _spec_edits  # noqa: E402
 
 ap = argparse.ArgumentParser()
 ap.add_argument("first", nargs="?", type=int, default=10)
@@ -36,25 +34,20 @@ oracle.lib()
 total = inc = 0
 for seed in range(a.first, a.first + a.seeds):
     rng = np.random.default_rng(seed)
-    clusters, pods, jobs = fuzz_objects.generate(seed, big=True)
-    for i, c in enumerate(clusters):
-        c["generation"], c["resourceVersion"] = 1, 100 + i
-    for i, j in enumerate(jobs):
-        j.setdefault("name", f"rayjob-{i}")
-    pk = Packer(max_clusters=64, max_groups=512, max_wtd=512, max_pods=8192, max_heads=256, max_jobs=64, max_creates=1 << 16,
-                max_json_bytes=a.json_bytes, **opts)
+    clusters, pods, jobs = objects(seed, big=True)
+    pk = Packer(**dict(PACKER_CAPS, max_pods=8192, max_json_bytes=a.json_bytes), **opts)
     try:
-        m = tp.Mirror(copy.deepcopy(clusters), copy.deepcopy(pods), jobs, pk)
+        m = Mirror(copy.deepcopy(clusters), copy.deepcopy(pods), jobs, pk)
         assert pk.flush() == abi.PACK_FULL
-        tp.check(m, oracle, lean=True)
+        packer_check(m, oracle, lean=True)
         counter, gen = [0], [2]
         for epoch in range(a.epochs):
             if a.all_options:
-                _spec_edits(rng, m, gen, int(rng.integers(1, 4)))
-            tp._events(rng, m, counter, structural=True)
+                spec_edits(rng, m, gen, int(rng.integers(1, 4)))
+            events(rng, m, counter, structural=True)
             mode = pk.flush()
             assert not mode & abi.PACK_FULL, (seed, epoch)
-            tp.check(m, oracle, lean=bool(epoch % 3))
+            packer_check(m, oracle, lean=bool(epoch % 3))
             total += 1
             inc += bool(mode & abi.PACK_POD_ROWS)
     finally:

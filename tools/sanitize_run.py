@@ -160,9 +160,9 @@ def main():
     # incremental epochs (the deletions compact its bucket and region across tiles)
     incremental(*synthetic.generate(synthetic.config("C3H", n_clusters=700, pods_per_cluster=20, large_pods=9000, n_large=1)),
                 "incremental epochs, huge RayCluster", large=True, huge=True)
-    # keys built to collide (tests/test_table_keys.py): probe chains that start in the last slot of the cluster, workersToDelete and
+    # keys built to collide (tests/table_keys.py): probe chains that start in the last slot of the cluster, workersToDelete and
     # head-aux tables and wrap, in a full pass and in incremental epochs
-    from test_table_keys import k1, k2, k3
+    from table_keys import k1, k2, k3
     for name, k in (("K1", k1()), ("K2", k2()), ("K3", k3())):
         incremental(k.snap, k.kflags, f"incremental epochs, colliding keys {name}", large=True, wide=True, huge=True)
     one(*synthetic.generate(synthetic.config("C2", n_clusters=200, jobs=True)), "fast pipeline")
