@@ -436,6 +436,10 @@ enum {
   KR_PART_OBJECTS = 4   /* every column except the seven per-pod ones: RayCluster / group / workersToDelete / head-aux / RayJob
                            rows (about 2 MB at C3).  Together with kr_snapshot_commit_pod_rows this is an incremental epoch. */
 };
+/* Every row is checked before anything moves: KR_E_INVALID (KR_E_CAPACITY for a RayCluster of 65 535 or more worker groups) for
+ * groups out of cluster order or naming another RayCluster in g_cluster_idx, workersToDelete names out of group order or past
+ * n_wtd, a JSON offset that is not 16-byte aligned or a range past json_bytes, a head-aux row whose h_pod_idx is not below n_pods;
+ * KR_E_STATE for a partial commit before a full commit of the layout.  An invalid call commits nothing. */
 int kr_snapshot_commit_parts(kr_engine *e, uint32_t parts);
 
 /* Incremental epoch (SURVEY §8(f) rank 1): the caller has rewritten the 7 pod columns of `rows[0..n)` in the pinned arenas;
@@ -464,7 +468,9 @@ int kr_snapshot_commit_pod_values(kr_engine *e, const uint32_t *rows, const uint
  * updates and head Pod status updates at a few hundred bytes per object instead of the whole object part: whenever the engine has
  * no resident state, or a Recreate gate, a JSON range or the number of head rows changed, it commits the whole object part itself.
  * That includes a range an earlier KR_PART_JSON-only commit moved (an arena compaction moves every range): unless every such
- * RayCluster is among `cluster_rows`, the whole object part is committed. */
+ * RayCluster is among `cluster_rows`, the whole object part is committed.  Whichever path it takes, the named rows are checked as
+ * kr_snapshot_commit_parts checks them, and a row >= n_clusters or a head-aux row >= n_heads is KR_E_INVALID; an invalid call
+ * commits nothing. */
 int kr_snapshot_commit_object_rows(kr_engine *e, const uint32_t *cluster_rows, uint32_t n_cluster_rows, const uint32_t *head_rows, uint32_t n_head_rows);
 
 /* Row-granular spec commit: the caller rewrote, in the pinned arenas, the muted-spec JSON of the RayClusters `cluster_rows` — in

@@ -5,8 +5,10 @@
 // layouts computed per snapshot from kr_sizes.  PassCtx, launch_hash, launch_decide2 and launch_large_sort are the launch helpers of
 // the full pass (launch_pass, replayed as a CUDA graph by run_pass_once) and the incremental one (run_pass_inc); run_pass drives both
 // for every reconcile call, profiled or not.  fetch_results copies the results back with the exact sizes of the totals words the
-// pass left, behind one host wait.  The commits upload on the copy stream and end in finish_commit; the two object commits diff
-// their rows against the resident tables on the device (launch_object_diff).
+// pass left, behind one host wait.  Every commit checks its whole input first (check_cluster_row, check_head_row),
+// then moves the host's record of what the device holds (CommitRecord) through that record's update functions, then uploads on the
+// copy stream between begin_commit and finish_commit: an invalid call commits nothing.  The two object commits diff their rows
+// against the resident tables on the device (object_diff_args, launch_object_diff).
 #include <cuda_runtime.h>
 
 #include <algorithm>
@@ -112,12 +114,135 @@ uint8_t obj_class(int col, bool wtd_edits) {
   if (wtd_edits && col == kWtdCntCol) return KR_OC_GROUP;
   return kObjClass[col];
 }
-// the snapshot's workersToDelete lists equal `prev` ({n_groups, g_wtd_off, g_wtd_cnt, w_name_id} of an earlier commit)
-bool wtd_lists_equal(const std::vector<uint32_t> &prev, const kr_snapshot_bufs &hb, const kr_sizes &n) {
-  const size_t G = n.n_groups, W = n.n_wtd;
-  return prev.size() == 1 + 2 * G + W && prev[0] == G && memcmp(prev.data() + 1, hb.g_wtd_off, 4 * G) == 0 &&
-         memcmp(prev.data() + 1 + G, hb.g_wtd_cnt, 4 * G) == 0 && memcmp(prev.data() + 1 + 2 * G, hb.w_name_id, 4 * W) == 0;
-}
+
+// The host's record of what the device's object columns, JSON ranges and hash order were last committed from, and of what the next
+// pass owes them.  Only its three update functions change it, each after its commit has checked the whole input and before the
+// commit uploads anything: commit_whole (kr_snapshot_commit_parts, any parts), commit_rows (the row path of
+// kr_snapshot_commit_object_rows) and commit_spec_rows (kr_snapshot_commit_spec_rows).  The passes clear the four flags at the end.
+struct CommitRecord {
+  struct Row {
+    uint64_t json_off;             // the JSON range the digests and the hash order were computed from: whole, spec rows
+    uint32_t json_len, group_off, group_cnt;  // (groups: whole)
+    uint8_t recreate, mh;          // KR_CF_UPGRADE_RECREATE: whole with the object part; some worker group has numOfHosts > 1: whole, rows
+  };
+  std::vector<Row> rows;             // per RayCluster row (sized, zero-filled, by every whole commit)
+  uint32_t n_recreate = 0;           // RayClusters with KR_CF_UPGRADE_RECREATE (decide phase 1 needed): whole
+  uint64_t recreate_sig = 0;         // which ones (their messages lead the hash order): whole, when it rebuilds the order
+  uint32_t n_mh = 0;                 // rows with a multi-host group: whole, rows
+  uint32_t snap_max_groups = 0;      // most worker groups in one RayCluster: whole
+  std::vector<uint32_t> wide_rows;   // RayClusters of more than KR_SMEM_GROUPS worker groups, ascending: whole
+  // rows whose range a JSON-only whole commit recorded while the device's c_json_off / c_json_len kept the old one (sorted,
+  // distinct): the row path takes them only all together; any object commit clears the list
+  std::vector<uint32_t> json_cols_behind;
+  uint32_t res_n_heads = 0;              // head-aux rows the resident device columns hold: whole with the object part
+  std::vector<uint32_t> prev_h_pod_idx;  // ... and their keys: whole with the object part, rows
+  std::vector<uint32_t> prev_wtd;        // KR_OPT_WTD_EDITS: {n_groups, g_wtd_off, g_wtd_cnt, w_name_id} (empty while it is off): whole with the object part
+  bool hash_dirty = false;        // spec JSON or a JSON range committed since the digests were computed: whole
+  bool heads_rebuild = false;     // a head key changed: the pod -> head-aux row table is rebuilt: whole, rows
+  bool wtd_rebuild = false;       // a workersToDelete list changed: the name table is rebuilt (kr_incr.cuh): whole
+  bool spec_order_stale = false;  // a spec commit changed a block count the full-pass hash order (d_order) was built from: spec rows (whole clears it)
+
+  // the snapshot's workersToDelete lists are the recorded ones
+  bool wtd_same(const kr_snapshot_bufs &hb, const kr_sizes &n) const {
+    const size_t G = n.n_groups, W = n.n_wtd;
+    return prev_wtd.size() == 1 + 2 * G + W && prev_wtd[0] == G && memcmp(prev_wtd.data() + 1, hb.g_wtd_off, 4 * G) == 0 &&
+           memcmp(prev_wtd.data() + 1 + G, hb.g_wtd_cnt, 4 * G) == 0 && memcmp(prev_wtd.data() + 1 + 2 * G, hb.w_name_id, 4 * W) == 0;
+  }
+  // The resident object columns can take the named RayCluster rows as they are: the same row and head-aux counts, per named row the
+  // same Recreate bit (hash order), JSON range (digests) and groups (the pipeline, the widest RayCluster and the wide set follow the
+  // counts), with KR_OPT_WTD_EDITS the same workersToDelete lists, and every row a JSON-only commit left behind among the named ones.
+  bool takes_rows(const kr_snapshot_bufs &hb, const kr_sizes &n, const uint32_t *cl, uint32_t n_cl, bool wtd_edits) const {
+    if (rows.size() != n.n_clusters || res_n_heads != n.n_heads || (wtd_edits && !wtd_same(hb, n))) return false;
+    for (const uint32_t *c = cl; c < cl + n_cl; c++) {
+      const Row &r = rows[*c];
+      if (r.recreate != ((hb.c_flags[*c] & KR_CF_UPGRADE_RECREATE) ? 1 : 0) || r.json_off != hb.c_json_off[*c] || r.json_len != hb.c_json_len[*c] ||
+          r.group_off != hb.c_group_off[*c] || r.group_cnt != hb.c_group_cnt[*c])
+        return false;
+    }
+    if (json_cols_behind.empty()) return true;
+    std::vector<uint32_t> given(cl, cl + n_cl);
+    std::sort(given.begin(), given.end());
+    return std::includes(given.begin(), given.end(), json_cols_behind.begin(), json_cols_behind.end());
+  }
+
+  struct Moved { bool shape, wide, order; };  // what a whole commit moved: the launch shape / pipeline, the wide set, the hash order
+  Moved commit_whole(const kr_snapshot_bufs &hb, const kr_sizes &n, uint32_t parts, bool wtd_edits) {
+    const bool objects = parts & (KR_PART_COLUMNS | KR_PART_OBJECTS);
+    const size_t had = rows.size();
+    bool ranges_moved = had != n.n_clusters;  // some RayCluster's JSON range differs from the one the digests / the hash order were computed from
+    uint32_t n_rc = 0, n_mh_now = 0, max_groups = 0;
+    std::vector<uint32_t> wide;
+    rows.resize(n.n_clusters);
+    for (uint32_t c = 0; c < n.n_clusters; c++) {
+      Row &r = rows[c];
+      const bool moved = c >= had || r.json_off != hb.c_json_off[c] || r.json_len != hb.c_json_len[c];
+      if (moved && !objects) json_cols_behind.push_back(c);  // (the device's range columns keep the old range)
+      ranges_moved |= moved;
+      r.json_off = hb.c_json_off[c]; r.json_len = hb.c_json_len[c];
+      r.group_off = hb.c_group_off[c]; r.group_cnt = hb.c_group_cnt[c];
+      r.mh = 0;
+      for (uint32_t g = r.group_off; g < r.group_off + r.group_cnt; g++) r.mh |= hb.g_num_hosts[g] > 1 ? 1 : 0;
+      n_mh_now += r.mh;
+      max_groups = std::max(max_groups, r.group_cnt);
+      if (r.group_cnt > KR_SMEM_GROUPS) wide.push_back(c);
+      if (hb.c_flags[c] & KR_CF_UPGRADE_RECREATE) n_rc++;
+      if (objects) r.recreate = (hb.c_flags[c] & KR_CF_UPGRADE_RECREATE) ? 1 : 0;
+    }
+    if (objects) json_cols_behind.clear();
+    std::sort(json_cols_behind.begin(), json_cols_behind.end());
+    json_cols_behind.erase(std::unique(json_cols_behind.begin(), json_cols_behind.end()), json_cols_behind.end());
+    const bool shape = n_rc != n_recreate || (n_mh_now > 0) != (n_mh > 0) || (max_groups > KR_SMEM_GROUPS) != (snap_max_groups > KR_SMEM_GROUPS);
+    n_recreate = n_rc; n_mh = n_mh_now; snap_max_groups = max_groups;
+    const bool wide_moved = wide != wide_rows;
+    wide_rows.swap(wide);
+    uint64_t rsig = 0x9E3779B97F4A7C15ull * (n_rc + 1);
+    for (uint32_t c = 0; c < n.n_clusters; c++) if (hb.c_flags[c] & KR_CF_UPGRADE_RECREATE) rsig = (rsig ^ c) * 0x100000001B3ull;
+    // (a spec-row commit updates the recorded ranges itself: its own flag says the order no longer follows them)
+    const bool order = ranges_moved || rsig != recreate_sig || spec_order_stale;
+    if (order) { recreate_sig = rsig; spec_order_stale = false; }  // (the new order travels with this commit)
+    if ((parts & KR_PART_JSON) || ranges_moved) hash_dirty = true;
+    if (objects) {
+      if (prev_h_pod_idx.size() != n.n_heads || (n.n_heads && memcmp(prev_h_pod_idx.data(), hb.h_pod_idx, 4 * (size_t)n.n_heads) != 0)) {
+        heads_rebuild = true;
+        prev_h_pod_idx.assign(hb.h_pod_idx, hb.h_pod_idx + n.n_heads);
+      }
+      res_n_heads = n.n_heads;
+      if (!wtd_edits) prev_wtd.clear();  // (the first commit after the option is turned on rebuilds the name table once)
+      else if (!wtd_same(hb, n)) {
+        wtd_rebuild = true;
+        prev_wtd.assign(1, n.n_groups);
+        prev_wtd.insert(prev_wtd.end(), hb.g_wtd_off, hb.g_wtd_off + n.n_groups);
+        prev_wtd.insert(prev_wtd.end(), hb.g_wtd_cnt, hb.g_wtd_cnt + n.n_groups);
+        prev_wtd.insert(prev_wtd.end(), hb.w_name_id, hb.w_name_id + n.n_wtd);
+      }
+    }
+    return {shape, wide_moved, order};
+  }
+  // -> the snapshot's first multi-host group came or its last went (a numOfHosts edit)
+  bool commit_rows(const kr_snapshot_bufs &hb, const uint32_t *cl, uint32_t n_cl, const uint32_t *hd, uint32_t n_hd) {
+    const bool had_mh = n_mh > 0;
+    for (uint32_t i = 0; i < n_cl; i++) {
+      Row &r = rows[cl[i]];
+      uint8_t bit = 0;
+      for (uint32_t g = r.group_off; g < r.group_off + r.group_cnt; g++) bit |= hb.g_num_hosts[g] > 1 ? 1 : 0;
+      n_mh += bit - r.mh; r.mh = bit;
+    }
+    for (uint32_t i = 0; i < n_hd; i++)  // the pod -> head-aux row table follows the keys
+      if (prev_h_pod_idx[hd[i]] != hb.h_pod_idx[hd[i]]) { heads_rebuild = true; prev_h_pod_idx[hd[i]] = hb.h_pod_idx[hd[i]]; }
+    json_cols_behind.clear();  // (every recorded row is among the named ones)
+    return (n_mh > 0) != had_mh;
+  }
+  // the m pulled rows' new ranges: a later object commit does not re-hash everything on their account; the full-pass hash order
+  // does not follow them (spec_order_stale when a block count moved)
+  void commit_spec_rows(const uint32_t *cl, const uint64_t *off, const uint32_t *len, uint32_t m, uint32_t n_clusters) {
+    if (rows.size() != n_clusters) return;  // (the next object commit sees every range as moved anyway)
+    for (uint32_t i = 0; i < m; i++) {
+      Row &r = rows[cl[i]];
+      if ((r.json_len + 8) / 64 != (len[i] + 8) / 64) spec_order_stale = true;
+      r.json_off = off[i]; r.json_len = len[i];
+    }
+  }
+};
 
 
 void dims_of(const kr_sizes &n, uint64_t d[7]) {
@@ -289,7 +414,7 @@ struct kr_engine {
   kr_flags last_flags{};      // flags of the last pass (kr_results_fetch honours fetch_pod_lists)
   bool committed_full = false;  // every part of the current layout has been uploaded at least once
   bool fixed_layout = false;    // KR_OPT_FIXED_LAYOUT: arenas laid out for the capacities, live counts in `sizes`
-  uint32_t n_recreate = 0;  // clusters with KR_CF_UPGRADE_RECREATE (decide phase 1 needed)
+  CommitRecord rec;            // what the device's object columns, JSON ranges and hash order were last committed from
   kr_profile prof{};
   std::string err;
   Staging hb;                  // kr_hash_batch
@@ -316,8 +441,6 @@ struct kr_engine {
   bool no_bucket = false;       // KR_NO_BUCKET=1: never take it (tests of the sort pipeline)
   bool hash_spin = true;        // bucket pipeline: Recreate gates wait for their digest inside k_decide2 instead of a second decide phase
                                 // (KR_NO_HASH_SPIN=1, or a pass in which a warp gave up waiting, turns it off)
-  uint64_t recreate_sig = 0;    // which RayClusters carry KR_CF_UPGRADE_RECREATE (their messages lead the hash order)
-  std::vector<uint8_t> recreate_bit;  // ... per cluster row, as of the last object commit (kr_snapshot_commit_object_rows checks against it)
   uint32_t bstride = 0;         // bucket stride of this layout (64 / 128 / 256); 0 = the layout does not qualify (a cluster outgrew 256 pods, ...)
   bool large_on = false;        // KR_OPT_LARGE_CLUSTERS
   bool wide_on = false;         // KR_OPT_WIDE_CLUSTERS
@@ -325,8 +448,6 @@ struct kr_engine {
   // The per-cluster kernels (kr_large.cuh) take the RayClusters of one list: the large half (rows and regions {offset, capacity}
   // from the last bucket attempt that voided, sticky like bstride) and, with KR_OPT_WIDE_CLUSTERS, the wide ones of the last commit.
   std::vector<uint32_t> large_rows; std::vector<uint2> large_reg;
-  std::vector<uint32_t> wide_rows;  // RayClusters of more than KR_SMEM_GROUPS worker groups, ascending
-  std::vector<uint32_t> group_cnt;  // c_group_cnt of the last commit (kr_snapshot_commit_object_rows: a moved count takes the whole object commit)
   bool lg_stale = false;        // the device table / list do not reflect the two halves yet (upload_lg at the next pass)
   uint32_t n_large = 0;         // RayClusters in the device list
   uint32_t n_lsort = 0;         // ... of which the first n_lsort are k_large_sort's; the huge ones after them go to k_huge_tiles / k_huge_merge
@@ -342,9 +463,6 @@ struct kr_engine {
   uint8_t *d_huge = nullptr;
   size_t huge_tiles = 0;
   std::vector<uint4> h_tiles;
-  bool snap_has_mh = false;     // some worker group has numOfHosts > 1
-  std::vector<uint8_t> mh_bit;  // ... per cluster row, as of the last commit (kr_snapshot_commit_object_rows keeps snap_has_mh current with it)
-  uint32_t snap_max_groups = 0; // most worker groups in one RayCluster
   bool ran_bucket = false;
   uint64_t h2d_accum = 0;       // bytes uploaded by the commits since the last pass (kr_profile.h2d_bytes)
   // hash order: message ids by descending SHA-1 block count, rebuilt at every commit from c_json_len
@@ -359,24 +477,14 @@ struct kr_engine {
   bool inc_zero_needed = true;   // the stamp / dirty-flag / counter region of this layout has not been zeroed yet
   kr_flags inc_flags{};          // flags of the pass that left the resident state
   uint32_t inc_n_pods = 0, inc_n_heads = 0;  // rows resident at the last pass
-  uint32_t res_n_heads = 0;                  // head-aux rows the resident device columns hold (object commits move it)
-  std::vector<uint32_t> prev_h_pod_idx;      // ... and their keys: a change means the pod -> head-aux row table must be rebuilt
-  bool heads_rebuild = false;
   bool wtd_edits = false;        // KR_OPT_WTD_EDITS
-  std::vector<uint32_t> prev_wtd;  // ... the workersToDelete lists of the last commit, {n_groups, g_wtd_off, g_wtd_cnt, w_name_id} (empty while the option is off)
-  bool wtd_rebuild = false;      // ... a commit changed them since the last pass: it rebuilds the name table (kr_incr.cuh)
   uint32_t res_n_wtd = 0;        // names in the resident name table and its resolutions (wtd_pod_idx)
-  bool hash_dirty = false;       // spec JSON (or a JSON range) committed since the digests were computed
   bool ran_inc = false;          // the last pass was an incremental one
   bool host_results_stale = false;  // an incremental pass went unfetched: the host copy misses its records, the next fetch copies everything
   bool fetched = true;              // the last pass's results have been copied to the host arena
   uint32_t inc_n_dirty = 0;      // changed RayClusters of the last incremental pass
   bool inc_gathered = false;     // ... and their records sit packed in the staging buffer
   bool inc_hash_ran = false;
-  std::vector<uint64_t> prev_json_off; std::vector<uint32_t> prev_json_len;  // JSON ranges the digests were computed from
-  // rows whose range a JSON-only commit recorded above while the device's c_json_off / c_json_len kept the old one (sorted, distinct):
-  // kr_snapshot_commit_object_rows commits the whole object part unless it is given every one of them
-  std::vector<uint32_t> json_cols_behind;
   // kr_snapshot_commit_spec_rows, pinned mirror and device copy of {pull rows u32 | lens u32 | offs u64 | hash order u32}[max_clusters]:
   // each call appends the rows it pulls to the pull lists; the pass that hashes them sorts the pending rows once and uploads them as
   // the hash order
@@ -387,7 +495,6 @@ struct kr_engine {
   uint32_t spec_epoch = 1;
   std::vector<uint32_t> pull_stamp;    // cluster row -> pull_epoch that pulled it: a pass in between lets the caller rewrite the arena,
   uint32_t pull_epoch = 1;             // so a row listed again after a pass (skip_hash leaves it pending) is pulled again
-  bool spec_order_stale = false;       // a spec commit changed a block count the full-pass hash order (d_order) was built from
   bool spec_rows_opt = false;          // KR_OPT_SPEC_ROWS (read by kr_packer_flush)
   uint32_t inc_spec_n = 0;             // rows the last incremental pass re-hashed ...
   bool inc_spec_gathered = false;      // ... and their digests sit packed in the staging buffer
@@ -540,7 +647,7 @@ int upload_lg(kr_engine *e) {
     for (uint32_t t = 0; t < nt; t++) tiles.push_back(make_uint4(c, t * kHugeTile, first, nt));
   }
   if (e->wide_on)
-    for (uint32_t c : e->wide_rows) if (!std::binary_search(e->large_rows.begin(), e->large_rows.end(), c)) list.push_back(c);
+    for (uint32_t c : e->rec.wide_rows) if (!std::binary_search(e->large_rows.begin(), e->large_rows.end(), c)) list.push_back(c);
   const uint32_t n_lsort = (uint32_t)list.size();
   list.insert(list.end(), huge.begin(), huge.end());
   if (tiles.size() > e->huge_tiles) return fail(e, KR_E_STATE, "internal: %zu huge-cluster tiles, room for %zu", tiles.size(), e->huge_tiles);
@@ -582,7 +689,7 @@ void build_order(kr_engine *e, const kr_snapshot_bufs &hb) {
 // Spec-row commits keep the full-pass hash order as it was; a pass that hashes every message rebuilds it first when their block
 // counts moved (uploaded on stream M, ahead of the pass).
 int refresh_order(kr_engine *e) {
-  e->spec_order_stale = false;
+  e->rec.spec_order_stale = false;
   if (!e->sizes.n_clusters) return KR_OK;
   if (e->order_pending) { CK(cudaEventSynchronize(e->ev_order)); e->order_pending = false; }
   kr_snapshot_bufs hb;
@@ -671,7 +778,7 @@ cudaError_t launch_decide2(const PassCtx &c, const Decide2Args &da, dim3 grid, b
       {{k_decide2<4>, k_decide2<4, false, true>}, {k_decide2<4, true>, k_decide2<4, true, true>}},
       {{k_decide2<8>, k_decide2<8, false, true>}, {k_decide2<8, true>, k_decide2<8, true, true>}}};
   const int st = c.e->bstride <= 64 ? 0 : c.e->bstride <= 128 ? 1 : 2;
-  const bool mh = c.e->snap_has_mh && da.f.gate_multihost_indexing;
+  const bool mh = c.e->rec.n_mh > 0 && da.f.gate_multihost_indexing;
   return launch_pdl(kern[st][inc][mh], grid, dim3(kD2Warps * 32), 0, c.M, pdl, da);
 }
 
@@ -701,10 +808,10 @@ int launch_pass(kr_engine *e, const kr_flags &f, bool profile, bool capturing = 
   // (the fork comes first so the hash can start while the columns are still landing — an incremental pod-row epoch leaves the JSON untouched)
   // bucket pipeline (kr_bucket2.cuh): the caller does not fetch the full pod lists, every RayCluster has few worker groups (or
   // KR_OPT_WIDE_CLUSTERS lists the others for the per-cluster kernels) and (checked on the device) at most `bstride` pods
-  const bool bucket = !e->no_bucket && !f.fetch_pod_lists && e->bstride != 0 && !e->force_radix && (e->snap_max_groups <= KR_SMEM_GROUPS || e->wide_on) &&
+  const bool bucket = !e->no_bucket && !f.fetch_pod_lists && e->bstride != 0 && !e->force_radix && (e->rec.snap_max_groups <= KR_SMEM_GROUPS || e->wide_on) &&
                       (size_t)n.n_clusters * e->bstride <= e->sl.bucket_entries;
   // ... and there the clusters whose Recreate gate reads a digest wait for it inside the decide kernel (the hash runs beside it)
-  const bool spin = bucket && !profile && do_hash && e->hash_spin && e->n_recreate > 0;
+  const bool spin = bucket && !profile && do_hash && e->hash_spin && e->rec.n_recreate > 0;
   // the digests, messages taken in e->d_order (built at commit), or zeros when the pass skips the hash
   auto hash_or_zero = [&]() -> int {
     if (do_hash) { c.mark("k_hash"); launch_hash(e, H, s.json, s.c_json_off, s.c_json_len, e->d_order, n.n_clusters, r.hash, e->hash_ctas_per_sm); }
@@ -765,10 +872,10 @@ int launch_pass(kr_engine *e, const kr_flags &f, bool profile, bool capturing = 
     if (large) launch_large_sort<false>(c, da);
     if (int rc = join_hash()) return rc;
     if (large) { c.mark("k_decide_large"); k_decide_large<false><<<e->n_large, kLargeDecideThreads, 0, M>>>(da, c.lg_list); }
-    if (e->n_recreate > 0 && do_hash && !spin) {  // clusters whose Recreate gate needs the digest: decided again, in the places phase 0 reserved
+    if (e->rec.n_recreate > 0 && do_hash && !spin) {  // clusters whose Recreate gate needs the digest: decided again, in the places phase 0 reserved
       da.phase = 1;
       c.mark("k_decide2_phase1");
-      CK(launch_decide2(c, da, dim3((e->n_recreate + kD2Warps - 1) / kD2Warps), false, false));
+      CK(launch_decide2(c, da, dim3((e->rec.n_recreate + kD2Warps - 1) / kD2Warps), false, false));
     }
   } else {
   const uint32_t ntiles = e->sl.ntiles;
@@ -829,9 +936,9 @@ int launch_pass(kr_engine *e, const kr_flags &f, bool profile, bool capturing = 
   }
   if (n.n_jobs) { c.mark("k_jobs"); k_jobs<<<(n.n_jobs + 255) / 256, 256, 0, M>>>(s, sc, r, z); }
   if (int rc = join_hash()) return rc;
-  if (e->n_recreate > 0 && do_hash) {
+  if (e->rec.n_recreate > 0 && do_hash) {
     da.phase = 1;
-    uint32_t warps = e->n_recreate;  // upper bound on the deferred list
+    uint32_t warps = e->rec.n_recreate;  // upper bound on the deferred list
     const dim3 grid1((warps + kDecideWarps - 1) / kDecideWarps), block1(kDecideWarps * 32);
     // like phase 0: the register-resident kernel on M for the small clusters, the general one beside it on G for the rest
     cudaStream_t G1 = (fast && !profile) ? e->sg : M;
@@ -954,9 +1061,9 @@ void after_full_pass(kr_engine *e, const kr_flags &f) {
   // incremental epoch would inherit that cursor and fail the same way, so the next pass starts over)
   e->inc_valid = e->ran_bucket && !e->no_incr && e->h_totals[9] <= e->cfg.max_creates;
   e->inc_flags = f; e->inc_n_pods = e->sizes.n_pods; e->inc_n_heads = e->sizes.n_heads;
-  e->host_results_stale = false; e->inc_n_dirty = 0; e->fetched = false; e->ran_inc = false; e->heads_rebuild = false;
-  e->wtd_rebuild = false; e->res_n_wtd = e->sizes.n_wtd;
-  if (!f.skip_hash) { e->hash_dirty = false; clear_spec_rows(e); }
+  e->host_results_stale = false; e->inc_n_dirty = 0; e->fetched = false; e->ran_inc = false; e->rec.heads_rebuild = false;
+  e->rec.wtd_rebuild = false; e->res_n_wtd = e->sizes.n_wtd;
+  if (!f.skip_hash) { e->rec.hash_dirty = false; clear_spec_rows(e); }
 }
 
 // A pass has read what the commits since the previous one uploaded: the pinned hash order is free again, and kr_profile keeps the
@@ -980,12 +1087,12 @@ int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile
   const SnapDev &s = c.s; const ResDev &r = c.r; const ScratchDev &sc = c.sc; const Sizes &z = c.z;
   const cudaStream_t M = c.M, H = c.H;
   CK(cudaStreamWaitEvent(M, e->ev_cols, 0));
-  const bool do_hash = e->hash_dirty && !f.skip_hash && n.n_clusters > 0;
+  const bool do_hash = e->rec.hash_dirty && !f.skip_hash && n.n_clusters > 0;
   // ... or only the messages kr_snapshot_commit_spec_rows listed (a whole-arena commit wins; a skip_hash pass leaves them pending)
-  const uint32_t n_rows = (!e->hash_dirty && !f.skip_hash) ? (uint32_t)e->spec_pending.size() : 0;
+  const uint32_t n_rows = (!e->rec.hash_dirty && !f.skip_hash) ? (uint32_t)e->spec_pending.size() : 0;
   const uint32_t *spec_rows = n_rows ? upload_spec_order(e) : nullptr;
   if (n_rows && !spec_rows) return fail(e, KR_E_CUDA, "upload of the spec rows' hash order failed");
-  if (do_hash && e->spec_order_stale) if (int rc = refresh_order(e)) return rc;
+  if (do_hash && e->rec.spec_order_stale) if (int rc = refresh_order(e)) return rc;
   if (do_hash || n_rows) {  // the spec JSON was committed again: the digests are recomputed (on their own stream), the Recreate gates re-read
     const uint32_t *order = do_hash ? e->d_order : spec_rows;
     const uint32_t nm = do_hash ? n.n_clusters : n_rows;
@@ -994,16 +1101,16 @@ int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile
     if (profile) c.mark(do_hash ? "k_hash" : "k_hash_rows");  // (unprofiled, an incremental pass does not count its hash)
     launch_hash(e, H, s.json, s.c_json_off, s.c_json_len, order, nm, r.hash, e->hash_ctas_per_sm);
     if (!profile) CK(cudaEventRecord(e->ev_hash, H));
-    if (e->n_recreate && do_hash) { c.mark("k_inc_mark_recreate"); k_inc_mark_recreate<<<(n.n_clusters + 255) / 256, 256, 0, M>>>(s, sc, z); }
-    if (e->n_recreate && !do_hash) { c.mark("k_inc_mark_rows"); k_inc_mark_rows<<<(n_rows + 255) / 256, 256, 0, M>>>(s, sc, spec_rows, n_rows); }
+    if (e->rec.n_recreate && do_hash) { c.mark("k_inc_mark_recreate"); k_inc_mark_recreate<<<(n.n_clusters + 255) / 256, 256, 0, M>>>(s, sc, z); }
+    if (e->rec.n_recreate && !do_hash) { c.mark("k_inc_mark_rows"); k_inc_mark_rows<<<(n_rows + 255) / 256, 256, 0, M>>>(s, sc, spec_rows, n_rows); }
   }
   const int grid = e->sm_count * 2;
-  if (e->heads_rebuild) {  // a head Pod came or went since the table was built (the commit compared the keys on the host)
+  if (e->rec.heads_rebuild) {  // a head Pod came or went since the table was built (the commit compared the keys on the host)
     c.mark("k_inc_aux_rebuild");
     k_inc_aux_clear<<<std::min<uint32_t>(grid, (e->sl.aux_slots + 255) / 256), 256, 0, M>>>(sc);
     k_inc_aux_insert<<<std::min<uint32_t>(grid, (n.n_heads + 255) / 256 + 1), 256, 0, M>>>(s, sc, z);
   }
-  if (e->wtd_rebuild) {  // a workersToDelete list changed since the name table was built (KR_OPT_WTD_EDITS; the commit compared them on the host)
+  if (e->rec.wtd_rebuild) {  // a workersToDelete list changed since the name table was built (KR_OPT_WTD_EDITS; the commit compared them on the host)
     if (e->res_n_wtd) { c.mark("k_inc_wtd_release"); k_inc_wtd_release<<<(e->res_n_wtd + 255) / 256, 256, 0, M>>>(s, sc, r, e->res_n_wtd, e->inc_n_pods); }
     c.mark("k_inc_wtd_clear");
     k_inc_wtd_clear<<<std::min<uint32_t>(grid, (e->sl.wt_slots + 255) / 256), 256, 0, M>>>(sc, r, n.n_wtd);
@@ -1014,7 +1121,7 @@ int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile
       k_inc_wtd_resolve<<<std::min<uint32_t>((uint32_t)e->sm_count * 4, (n.n_pods + 255) / 256 + 1), 256, e->sl.wt_bits_n / 8, M>>>(s, sc, r, z, e->inc_n_pods);
     }
     e->res_n_wtd = n.n_wtd;
-    e->wtd_rebuild = false;
+    e->rec.wtd_rebuild = false;
   }
   // (k_inc_refresh ran behind the object commits' diff kernels: the input records are current)
   c.mark("k_inc_admit");
@@ -1032,7 +1139,7 @@ int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile
   if (n.n_clusters) {
     Decide2Args da{s, sc, r, z, f, st, e->cfg.max_creates, 0, 2};
     c.mark("k_decide2_dirty");
-    // (snap_has_mh as of the latest commit: an object commit may have brought the snapshot's first multi-host group or taken its last)
+    // (the multi-host rows as of the latest commit: an object commit may have brought the snapshot's first multi-host group or taken its last)
     CK(launch_decide2(c, da, dim3((n.n_clusters + kD2Warps - 1) / kD2Warps), true, false));
     if (e->n_large) {  // the dirty large RayClusters (k_decide2 left every cluster past the stride alone)
       CK(cudaMemsetAsync(sc.inc + KR_INC_LSEG, 0, 4, M));
@@ -1051,14 +1158,14 @@ int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile
   CK(cudaGetLastError());
   CK(cudaEventSynchronize(e->ev_inc));
   commits_read(e);
-  e->heads_rebuild = false;  // (rebuilt here, or about to be rebuilt by the full pass)
+  e->rec.heads_rebuild = false;  // (rebuilt here, or about to be rebuilt by the full pass)
   if (e->h_inc[KR_INC_VOID] || e->h_inc[KR_INC_STRUCTURAL]) return KR_OK;  // the caller takes the full pass
   if (!e->fetched) e->host_results_stale = true;  // the previous pass's records never reached the host copy
   e->fetched = false;
   e->inc_n_dirty = e->h_inc[KR_INC_DIRTY];
   e->inc_gathered = e->inc_n_dirty <= sl.capc && e->h_inc[KR_INC_GROUPS] <= sl.capg;
   e->inc_hash_ran = do_hash;
-  if (do_hash) e->hash_dirty = false;
+  if (do_hash) e->rec.hash_dirty = false;
   e->inc_spec_n = n_rows; e->inc_spec_gathered = gather_rows;
   if (n_rows) {
     const uint32_t *h = reinterpret_cast<const uint32_t *>(e->spec.h + 16 * ((size_t)e->cfg.max_clusters + 1));
@@ -1102,7 +1209,7 @@ int run_pass(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile) {
     CK(cudaMemsetAsync(e->d_scratch + e->sl.inc_zero, 0, e->sl.inc_zero_end - e->sl.inc_zero, e->sm));
     e->inc_zero_needed = false;
   }
-  if (e->spec_order_stale && !f.skip_hash) if (int rc = refresh_order(e)) return rc;
+  if (e->rec.spec_order_stale && !f.skip_hash) if (int rc = refresh_order(e)) return rc;
   for (int attempt = 0; attempt < 5; attempt++) {
     if (profile) CK(cudaEventRecord(e->ev_a, e->sm));
     if (int rc = profile ? launch_pass(e, f, true) : run_pass_once(e, f)) return rc;
@@ -1232,13 +1339,69 @@ int fetch_results(kr_engine *e, kr_results_view *out) {
   return KR_OK;
 }
 
+// The checks every commit makes of the rows it takes, before anything moves (an invalid call commits nothing).  The kernels trust
+// these indices: a shim bug must come back as KR_E_INVALID, not as out-of-bounds device reads and writes.  (Inlined: the whole
+// commit runs them on every row.)
+// A RayCluster row: its JSON range 16-byte aligned and inside json_bytes; unless json_only, fewer worker groups than the limit, its
+// groups inside n_groups and naming it in g_cluster_idx, and their workersToDelete names inside n_wtd.
+__attribute__((always_inline)) inline int check_cluster_row(kr_engine *e, const kr_snapshot_bufs &hb, const kr_sizes &n, uint32_t c, bool json_only = false) {
+  if (c >= n.n_clusters) return fail(e, KR_E_INVALID, "cluster row %u out of range", c);
+  if (hb.c_json_off[c] & 15) return fail(e, KR_E_INVALID, "cluster %u: json offset not 16-byte aligned", c);
+  if (hb.c_json_off[c] + hb.c_json_len[c] > n.json_bytes) return fail(e, KR_E_INVALID, "cluster %u: json range outside arena", c);
+  if (json_only) return KR_OK;
+  const uint64_t g0 = hb.c_group_off[c], cnt = hb.c_group_cnt[c];
+  if (cnt >= 0xFFFFu) return fail(e, KR_E_CAPACITY, "cluster %u has %u worker groups (limit 65534)", c, hb.c_group_cnt[c]);
+  if (g0 + cnt > n.n_groups) return fail(e, KR_E_INVALID, "cluster %u: groups run past n_groups", c);
+  for (uint64_t g = g0; g < g0 + cnt; g++) {
+    if (hb.g_cluster_idx[g] != c) return fail(e, KR_E_INVALID, "group %llu: g_cluster_idx %u != owning cluster %u", (unsigned long long)g, hb.g_cluster_idx[g], c);
+    if ((uint64_t)hb.g_wtd_off[g] + hb.g_wtd_cnt[g] > n.n_wtd) return fail(e, KR_E_INVALID, "group %llu: workersToDelete names run past n_wtd", (unsigned long long)g);
+  }
+  return KR_OK;
+}
+__attribute__((always_inline)) inline int check_head_row(kr_engine *e, const kr_snapshot_bufs &hb, const kr_sizes &n, uint32_t h) {
+  if (h >= n.n_heads) return fail(e, KR_E_INVALID, "head-aux row %u out of range", h);
+  if (hb.h_pod_idx[h] >= n.n_pods) return fail(e, KR_E_INVALID, "head-aux row %u: h_pod_idx %u >= n_pods %u", h, hb.h_pod_idx[h], n.n_pods);
+  return KR_OK;
+}
+
+// The start of every commit: a pass still reading what it overwrites must finish first; ev_h2d0 opens its copy time.
+int begin_commit(kr_engine *e) {
+  CK(cudaStreamSynchronize(e->sm));
+  CK(cudaEventRecord(e->ev_h2d0, e->scopy));
+  return KR_OK;
+}
+
+// The column table of an object commit's diff: every object column i, staged at stage + at[i] with cnt[d] rows of its dimension d,
+// against the resident one as the record last left it.  Without row lists, staged row k is resident row k; with them (the row path)
+// it is the k-th row of the list of dimension d at stage + list_at[d], and a dimension without staged rows is left out.
+ObjDiffArgs object_diff_args(const kr_engine *e, const uint8_t *stage, const size_t *at, const uint32_t cnt[7], const size_t *list_at) {
+  uint64_t dn[7];
+  dims_of(e->sizes, dn);
+  ObjDiffArgs oa{};
+  for (int i = 0; i < kNumCols - 1; i++) {
+    const int d = kCols[i].dim;
+    if (d == D_PODS || (list_at && !cnt[d])) continue;
+    const int k = oa.n_cols++;
+    oa.src[k] = stage + at[i];
+    oa.rowlist[k] = list_at ? reinterpret_cast<const uint32_t *>(stage + list_at[d]) : nullptr;
+    oa.dst[k] = e->d_in + e->il.off[i];
+    oa.first[k + 1] = oa.first[k] + cnt[d];
+    oa.rows_old[k] = d == D_HEADS ? e->rec.res_n_heads : (uint32_t)dn[d];
+    oa.row_bytes[k] = (uint16_t)(kCols[i].elem * kCols[i].mult);
+    oa.cls[k] = obj_class(i, e->wtd_edits);
+    if (i == kGroupClusterCol) oa.g_cluster_idx_new = reinterpret_cast<const uint32_t *>(stage + at[i]);
+    if (i == kHeadKeyCol) oa.h_pod_idx_new = reinterpret_cast<const uint32_t *>(stage + at[i]);
+  }
+  oa.h_pod_idx_old = reinterpret_cast<const uint32_t *>(e->d_in + e->il.off[kHeadKeyCol]);
+  oa.n_heads_old = e->rec.res_n_heads;
+  return oa;
+}
+
 // The on-device diff of an object commit (kr_incr.cuh), on the copy stream: the staged rows of oa's columns against the resident
 // ones (changed rows mark their RayCluster dirty, a changed key makes the next pass a full one), the head-aux keys of the n_hd rows
 // head_rows (device list; nullptr: rows 0 .. n_hd - 1), then with `refresh` the input records (cl_in) of the RayClusters the diff
 // found changed, now that every column of theirs is in place.
-int launch_object_diff(kr_engine *e, ObjDiffArgs oa, uint32_t n_hd, const uint32_t *head_rows, bool refresh) {
-  oa.h_pod_idx_old = reinterpret_cast<const uint32_t *>(e->d_in + e->il.off[kHeadKeyCol]);
-  oa.n_heads_old = e->res_n_heads;
+int launch_object_diff(kr_engine *e, const ObjDiffArgs &oa, uint32_t n_hd, const uint32_t *head_rows, bool refresh) {
   SnapDev sd;
   bind_in(e->il, e->d_in, &sd);
   ScratchDev scd = bind_scratch(e->sl, e->d_scratch);
@@ -1527,74 +1690,48 @@ int kr_snapshot_commit(kr_engine *e) { return kr_snapshot_commit_parts(e, KR_PAR
 int kr_snapshot_commit_parts(kr_engine *e, uint32_t parts) {
   if (!e || !e->begun) return e ? fail(e, KR_E_STATE, "kr_snapshot_commit before kr_snapshot_begin") : KR_E_INVALID;
   CK(cudaSetDevice(e->cfg.device));
-  // cheap host-side checks of the invariants the kernels rely on
+  // every row checked, the groups stored in cluster order and their workersToDelete names in group order
   kr_snapshot_bufs hb;
   bind_in(e->il, e->h_in, &hb);
   const kr_sizes &n = e->sizes;
-  uint32_t n_recreate = 0, max_groups = 0;
-  bool has_mh = false;
   uint64_t goff = 0, woff = 0;
-  e->mh_bit.assign(n.n_clusters, 0);
   for (uint32_t c = 0; c < n.n_clusters; c++) {
     if (hb.c_group_off[c] != goff) return fail(e, KR_E_INVALID, "cluster %u: groups must be stored in cluster order (group_off %u != %llu)", c, hb.c_group_off[c], (unsigned long long)goff);
-    if (hb.c_group_cnt[c] >= 0xFFFFu) return fail(e, KR_E_CAPACITY, "cluster %u has %u worker groups (limit 65534)", c, hb.c_group_cnt[c]);
-    if (goff + hb.c_group_cnt[c] > n.n_groups) return fail(e, KR_E_INVALID, "cluster %u: groups run past n_groups", c);
-    // the kernels trust these indices: a shim bug must come back as KR_E_INVALID, not as out-of-bounds device writes
+    if (int rc = check_cluster_row(e, hb, n, c)) return rc;
     for (uint64_t g = goff; g < goff + hb.c_group_cnt[c]; g++) {
-      if (hb.g_cluster_idx[g] != c) return fail(e, KR_E_INVALID, "group %llu: g_cluster_idx %u != owning cluster %u", (unsigned long long)g, hb.g_cluster_idx[g], c);
       if (hb.g_wtd_off[g] != woff) return fail(e, KR_E_INVALID, "group %llu: workersToDelete names must be stored in group order (wtd_off %u != %llu)", (unsigned long long)g, hb.g_wtd_off[g], (unsigned long long)woff);
       woff += hb.g_wtd_cnt[g];
-      if (woff > n.n_wtd) return fail(e, KR_E_INVALID, "group %llu: workersToDelete names run past n_wtd", (unsigned long long)g);
-      if (hb.g_num_hosts[g] > 1) { has_mh = true; e->mh_bit[c] = 1; }
     }
-    max_groups = std::max(max_groups, hb.c_group_cnt[c]);
     goff += hb.c_group_cnt[c];
-    if (hb.c_json_off[c] & 15) return fail(e, KR_E_INVALID, "cluster %u: json offset not 16-byte aligned", c);
-    if (hb.c_json_off[c] + hb.c_json_len[c] > n.json_bytes) return fail(e, KR_E_INVALID, "cluster %u: json range outside arena", c);
-    if (hb.c_flags[c] & KR_CF_UPGRADE_RECREATE) n_recreate++;
   }
-  if (parts & KR_PART_COLUMNS) e->inc_valid = false;  // pod columns uploaded wholesale: the resident buckets no longer describe them
-  if (parts & KR_PART_JSON) e->hash_dirty = true;
-  bool ranges_moved = e->prev_json_off.size() != n.n_clusters;  // some RayCluster's JSON range differs from the one the digests / the hash order were computed from
-  for (uint32_t c = 0; c < n.n_clusters && !ranges_moved; c++)
-    ranges_moved = e->prev_json_off[c] != hb.c_json_off[c] || e->prev_json_len[c] != hb.c_json_len[c];
   if (goff != n.n_groups) return fail(e, KR_E_INVALID, "sum of group_cnt (%llu) != n_groups (%u)", (unsigned long long)goff, n.n_groups);
   if (woff != n.n_wtd) return fail(e, KR_E_INVALID, "sum of g_wtd_cnt (%llu) != n_wtd (%u)", (unsigned long long)woff, n.n_wtd);
   for (uint32_t h = 0; h < n.n_heads; h++)
-    if (hb.h_pod_idx[h] >= n.n_pods) return fail(e, KR_E_INVALID, "head-aux row %u: h_pod_idx %u >= n_pods %u", h, hb.h_pod_idx[h], n.n_pods);
-  if (n_recreate != e->n_recreate || has_mh != e->snap_has_mh || (max_groups > KR_SMEM_GROUPS) != (e->snap_max_groups > KR_SMEM_GROUPS)) e->gvalid = false;  // launch shape / pipeline depend on them
-  e->n_recreate = n_recreate; e->snap_has_mh = has_mh; e->snap_max_groups = max_groups;
-  // the wide RayClusters (KR_OPT_WIDE_CLUSTERS): a different set is a different list, and grid, of the per-cluster kernels
-  e->group_cnt.assign(hb.c_group_cnt, hb.c_group_cnt + n.n_clusters);
-  {
-    std::vector<uint32_t> wide;
-    if (max_groups > KR_SMEM_GROUPS)
-      for (uint32_t c = 0; c < n.n_clusters; c++) if (hb.c_group_cnt[c] > KR_SMEM_GROUPS) wide.push_back(c);
-    if (wide != e->wide_rows) { e->wide_rows.swap(wide); if (e->wide_on) e->lg_stale = true; }
-  }
-  // hash order (build_order)
-  if (e->order_pending) { CK(cudaEventSynchronize(e->ev_order)); e->order_pending = false; }  // a previous upload may still be reading h_order
-  uint64_t rsig = 0x9E3779B97F4A7C15ull * (n_recreate + 1);
-  for (uint32_t c = 0; c < n.n_clusters; c++) if (hb.c_flags[c] & KR_CF_UPGRADE_RECREATE) rsig = (rsig ^ c) * 0x100000001B3ull;
-  // (a spec-row commit updates the recorded ranges itself: its own flag says the order no longer follows them)
-  const bool order_stale = ranges_moved || rsig != e->recreate_sig || e->spec_order_stale;
-  if (order_stale) build_order(e, hb);  // (unchanged lengths and gates: the resident order stands — an object / pod epoch does not pay for it)
-  // Asynchronous, in two parts on the copy stream: every column first, the spec-JSON arena (the larger half) second.
-  // The pass waits on the two events, so match/place/decide run while the JSON is still crossing PCIe and only the hash
-  // (and what depends on it) waits for the second part.  Nothing here blocks the host.
-  CK(cudaStreamSynchronize(e->sm));  // a pass still reading the previous snapshot must finish before it is overwritten
-  const size_t json_off = e->il.off[kNumCols - 1];
+    if (int rc = check_head_row(e, hb, n, h)) return rc;
   if ((parts & KR_PART_ALL) != KR_PART_ALL && !e->committed_full)
     return fail(e, KR_E_STATE, "a partial commit needs a full commit of this layout first");
-  size_t bytes = 0;
-  CK(cudaEventRecord(e->ev_h2d0, e->scopy));
-  const size_t a1 = e->il.off[kFirstPodCol], b0 = e->il.off[kFirstPodCol + 7];
+  const size_t a1 = e->il.off[kFirstPodCol], b0 = e->il.off[kFirstPodCol + 7], json_off = e->il.off[kNumCols - 1];
   // While the incremental state is resident, an object commit lands beside the resident tables and is diffed against them on
   // the device (k_inc_objects): changed rows mark their RayCluster dirty, a changed key makes the next pass a full one.
   const bool stage_objects = e->inc_valid && !e->no_incr && (parts & KR_PART_OBJECTS) && !(parts & KR_PART_COLUMNS);
   if (stage_objects && a1 + (json_off - b0) > e->obj_stage_cap)
     return fail(e, KR_E_STATE, "internal: object part of %zu bytes, staging room for %zu", a1 + (json_off - b0), e->obj_stage_cap);
   auto stage_of = [&](size_t off) { return off < a1 ? off : a1 + (off - b0); };
+  size_t at[kNumCols];
+  for (int i = 0; i < kNumCols; i++) at[i] = stage_of(e->il.off[i]);
+  const uint32_t cnt[7] = {n.n_clusters, n.n_groups, n.n_wtd, n.n_pods, n.n_heads, n.n_jobs, 0};
+  const ObjDiffArgs oa = object_diff_args(e, e->d_obj_stage, at, cnt, nullptr);  // (before the record moves on)
+  if (e->order_pending) { CK(cudaEventSynchronize(e->ev_order)); e->order_pending = false; }  // a previous upload may still be reading h_order
+  if (int rc = begin_commit(e)) return rc;
+  const CommitRecord::Moved moved = e->rec.commit_whole(hb, n, parts, e->wtd_edits);
+  if (moved.shape) e->gvalid = false;  // launch shape / pipeline depend on it
+  if (moved.wide && e->wide_on) e->lg_stale = true;  // a different wide set is a different list, and grid, of the per-cluster kernels
+  if (parts & KR_PART_COLUMNS) e->inc_valid = false;  // pod columns uploaded wholesale: the resident buckets no longer describe them
+  if (moved.order) build_order(e, hb);  // (unchanged lengths and gates: the resident order stands — an object / pod epoch does not pay for it)
+  // Asynchronous, in two parts on the copy stream: every column first, the spec-JSON arena (the larger half) second.
+  // The pass waits on the two events, so match/place/decide run while the JSON is still crossing PCIe and only the hash
+  // (and what depends on it) waits for the second part.  Nothing here blocks the host.
+  size_t bytes = 0;
   auto up = [&](size_t off, size_t len) -> int {
     if (!len) return KR_OK;
     uint8_t *dst = (stage_objects && off < json_off) ? e->d_obj_stage + stage_of(off) : e->d_in + off;
@@ -1612,64 +1749,12 @@ int kr_snapshot_commit_parts(kr_engine *e, uint32_t parts) {
       for (int k = 0; k < 7; k++)
         if (int rc = up(e->il.off[kFirstPodCol + k], 4 * (size_t)n.n_pods)) return rc;
   }
-  if (stage_objects) {
-    uint64_t dn[7];
-    dims_of(n, dn);
-    ObjDiffArgs oa{};
-    int nc = 0;
-    uint32_t first = 0;
-    for (int i = 0; i < kNumCols - 1; i++) {
-      if (kCols[i].dim == D_PODS) continue;
-      oa.src[nc] = e->d_obj_stage + stage_of(e->il.off[i]);
-      oa.dst[nc] = e->d_in + e->il.off[i];
-      oa.first[nc] = first;
-      oa.rows_old[nc] = kCols[i].dim == D_HEADS ? e->res_n_heads : (uint32_t)dn[kCols[i].dim];
-      oa.row_bytes[nc] = (uint16_t)(kCols[i].elem * kCols[i].mult);
-      oa.cls[nc] = obj_class(i, e->wtd_edits);
-      first += (uint32_t)dn[kCols[i].dim];
-      nc++;
-    }
-    oa.first[nc] = first; oa.n_cols = nc;
-    oa.g_cluster_idx_new = reinterpret_cast<const uint32_t *>(e->d_obj_stage + stage_of(e->il.off[kGroupClusterCol]));
-    oa.h_pod_idx_new = reinterpret_cast<const uint32_t *>(e->d_obj_stage + stage_of(e->il.off[kHeadKeyCol]));
-    if (int rc = launch_object_diff(e, oa, n.n_heads, nullptr, n.n_clusters != 0)) return rc;
-  }
-  if (parts & (KR_PART_COLUMNS | KR_PART_OBJECTS)) {
-    e->recreate_bit.resize(n.n_clusters);
-    for (uint32_t c = 0; c < n.n_clusters; c++) e->recreate_bit[c] = (hb.c_flags[c] & KR_CF_UPGRADE_RECREATE) ? 1 : 0;
-    if (e->prev_h_pod_idx.size() != n.n_heads || (n.n_heads && memcmp(e->prev_h_pod_idx.data(), hb.h_pod_idx, 4 * (size_t)n.n_heads) != 0)) {
-      e->heads_rebuild = true;
-      e->prev_h_pod_idx.assign(hb.h_pod_idx, hb.h_pod_idx + n.n_heads);
-    }
-    e->res_n_heads = n.n_heads;
-    if (!e->wtd_edits) e->prev_wtd.clear();  // (the first commit after the option is turned on rebuilds the name table once)
-    else if (!wtd_lists_equal(e->prev_wtd, hb, n)) {
-      e->wtd_rebuild = true;
-      e->prev_wtd.assign(1, n.n_groups);
-      e->prev_wtd.insert(e->prev_wtd.end(), hb.g_wtd_off, hb.g_wtd_off + n.n_groups);
-      e->prev_wtd.insert(e->prev_wtd.end(), hb.g_wtd_cnt, hb.g_wtd_cnt + n.n_groups);
-      e->prev_wtd.insert(e->prev_wtd.end(), hb.w_name_id, hb.w_name_id + n.n_wtd);
-    }
-  }
+  if (stage_objects) { if (int rc = launch_object_diff(e, oa, n.n_heads, nullptr, n.n_clusters != 0)) return rc; }
   CK(cudaEventRecord(e->ev_cols, e->scopy));
-  if (parts & (KR_PART_COLUMNS | KR_PART_OBJECTS)) e->json_cols_behind.clear();
-  else if (ranges_moved) {  // the device's range columns keep the old ranges of the rows that moved
-    for (uint32_t c = 0; c < n.n_clusters; c++)
-      if (c >= e->prev_json_off.size() || e->prev_json_off[c] != hb.c_json_off[c] || e->prev_json_len[c] != hb.c_json_len[c]) e->json_cols_behind.push_back(c);
-    std::sort(e->json_cols_behind.begin(), e->json_cols_behind.end());
-    e->json_cols_behind.erase(std::unique(e->json_cols_behind.begin(), e->json_cols_behind.end()), e->json_cols_behind.end());
-  }
-  if (ranges_moved) {  // digests of moved ranges are stale
-    e->hash_dirty = true;
-    e->prev_json_off.assign(hb.c_json_off, hb.c_json_off + n.n_clusters); e->prev_json_len.assign(hb.c_json_len, hb.c_json_len + n.n_clusters);
-  }
-  if (order_stale) {  // the new order travels with this commit: from here on the recorded ranges / gates are the ones it was built from
-    e->recreate_sig = rsig; e->spec_order_stale = false;
-    if (n.n_clusters) {
-      CK(cudaMemcpyAsync(e->d_order, e->h_order, 4 * (size_t)n.n_clusters, cudaMemcpyHostToDevice, e->scopy)); bytes += 4 * (size_t)n.n_clusters;
-      CK(cudaEventRecord(e->ev_order, e->scopy));
-      e->order_pending = true;
-    }
+  if (moved.order && n.n_clusters) {  // the new order travels with this commit
+    CK(cudaMemcpyAsync(e->d_order, e->h_order, 4 * (size_t)n.n_clusters, cudaMemcpyHostToDevice, e->scopy)); bytes += 4 * (size_t)n.n_clusters;
+    CK(cudaEventRecord(e->ev_order, e->scopy));
+    e->order_pending = true;
   }
   if (parts & KR_PART_JSON) { if (int rc = up(json_off, e->fixed_layout ? (size_t)n.json_bytes : e->il.total - json_off)) return rc; }
   if ((parts & KR_PART_ALL) == KR_PART_ALL) e->committed_full = true;
@@ -1708,8 +1793,7 @@ static int commit_pod_patch(kr_engine *e, const uint32_t *rows, const uint32_t *
     hc.c[k] = reinterpret_cast<uint32_t *>(e->h_in_dev + (static_cast<const uint8_t *>(hsrc[k]) - e->h_in));
     dc.c[k] = static_cast<uint32_t *>(const_cast<void *>(dsrc[k]));
   }
-  CK(cudaStreamSynchronize(e->sm));  // a pass still reading the columns must finish first
-  CK(cudaEventRecord(e->ev_h2d0, e->scopy));
+  if (int rc = begin_commit(e)) return rc;
   CK(cudaMemcpyAsync(e->pr.d, e->pr.h, bytes, cudaMemcpyHostToDevice, e->scopy));
   CK(cudaEventRecord(e->pr.ev, e->scopy));
   e->pr.busy = true;
@@ -1734,47 +1818,16 @@ int kr_snapshot_commit_object_rows(kr_engine *e, const uint32_t *cluster_rows, u
   const kr_sizes &n = e->sizes;
   kr_snapshot_bufs hb;
   bind_in(e->il, e->h_in, &hb);
+  // the named rows are checked as the whole commit checks them, whichever path follows
+  for (uint32_t i = 0; i < n_cl; i++)
+    if (int rc = check_cluster_row(e, hb, n, cluster_rows[i])) return rc;
+  for (uint32_t i = 0; i < n_hd; i++)
+    if (int rc = check_head_row(e, hb, n, head_rows[i])) return rc;
   // Only an optimisation of kr_snapshot_commit_parts(KR_PART_OBJECTS): whenever the resident state cannot take the rows as they
-  // are — no resident state, a Recreate gate or a JSON range that changed (hash order / digests), head rows added or removed, a
-  // group count that moved (the pipeline, the widest RayCluster and the wide set follow it), with KR_OPT_WTD_EDITS a workersToDelete
-  // list that changed — the whole object part is committed instead.
-  bool whole = !e->inc_valid || e->no_incr || !e->committed_full || e->res_n_heads != n.n_heads || e->recreate_bit.size() != n.n_clusters ||
-               e->prev_json_off.size() != n.n_clusters || e->mh_bit.size() != n.n_clusters || e->group_cnt.size() != n.n_clusters ||
-               (e->wtd_edits && !wtd_lists_equal(e->prev_wtd, hb, n));
-  for (uint32_t i = 0; i < n_cl && !whole; i++) {
-    const uint32_t c = cluster_rows[i];
-    if (c >= n.n_clusters) return fail(e, KR_E_INVALID, "cluster row %u out of range", c);
-    whole = e->recreate_bit[c] != ((hb.c_flags[c] & KR_CF_UPGRADE_RECREATE) ? 1 : 0) || e->prev_json_off[c] != hb.c_json_off[c] || e->prev_json_len[c] != hb.c_json_len[c] ||
-            hb.c_group_cnt[c] != e->group_cnt[c] || (uint64_t)hb.c_group_off[c] + hb.c_group_cnt[c] > n.n_groups;
-  }
-  // a range an earlier JSON-only commit moved is recorded as current, yet only an object commit of its row brings it to the device
-  if (!whole && !e->json_cols_behind.empty()) {
-    whole = e->json_cols_behind.size() > n_cl;
-    if (!whole) {
-      std::vector<uint32_t> given(cluster_rows, cluster_rows + n_cl);
-      std::sort(given.begin(), given.end());
-      whole = !std::includes(given.begin(), given.end(), e->json_cols_behind.begin(), e->json_cols_behind.end());
-    }
-  }
-  for (uint32_t i = 0; i < n_hd && !whole; i++) {
-    if (head_rows[i] >= n.n_heads) return fail(e, KR_E_INVALID, "head-aux row %u out of range", head_rows[i]);
-    if (hb.h_pod_idx[head_rows[i]] >= n.n_pods) return fail(e, KR_E_INVALID, "head-aux row %u: h_pod_idx %u >= n_pods %u", head_rows[i], hb.h_pod_idx[head_rows[i]], n.n_pods);
-  }
-  if (whole) return kr_snapshot_commit_parts(e, KR_PART_OBJECTS);
+  // are, the whole object part is committed instead (which checks the layout around them as well).
+  if (!e->inc_valid || e->no_incr || !e->committed_full || !e->rec.takes_rows(hb, n, cluster_rows, n_cl, e->wtd_edits))
+    return kr_snapshot_commit_parts(e, KR_PART_OBJECTS);
   CK(cudaSetDevice(e->cfg.device));
-  // a numOfHosts edit may bring the snapshot's first multi-host group or take its last: the decide kernel's instantiation follows
-  bool mh_moved = false;
-  for (uint32_t i = 0; i < n_cl; i++) {
-    const uint32_t c = cluster_rows[i];
-    uint8_t bit = 0;
-    for (uint32_t g = hb.c_group_off[c]; g < hb.c_group_off[c] + hb.c_group_cnt[c]; g++) bit |= hb.g_num_hosts[g] > 1 ? 1 : 0;
-    if (bit != e->mh_bit[c]) { e->mh_bit[c] = bit; mh_moved = true; }
-  }
-  if (mh_moved) {
-    const bool has_mh = std::find(e->mh_bit.begin(), e->mh_bit.end(), 1) != e->mh_bit.end();
-    if (has_mh != e->snap_has_mh) e->gvalid = false;  // (the captured full pass launches the other instantiation)
-    e->snap_has_mh = has_mh;
-  }
   // group rows of the named clusters
   std::vector<uint32_t> grows;
   for (uint32_t i = 0; i < n_cl; i++) for (uint32_t g = 0; g < hb.c_group_cnt[cluster_rows[i]]; g++) grows.push_back(hb.c_group_off[cluster_rows[i]] + g);
@@ -1792,9 +1845,6 @@ int kr_snapshot_commit_object_rows(kr_engine *e, const uint32_t *cluster_rows, u
   CK(e->orow.wait());
   CK(e->orow.reserve(need, need / 2 + 65536));
   for (int d = 0; d < 7; d++) if (cnt[d]) memcpy(e->orow.h + list_off[d], lists[d], 4 * (size_t)cnt[d]);
-  ObjDiffArgs oa{};
-  int nc = 0;
-  uint32_t first = 0;
   for (int i = 0; i < kNumCols - 1; i++) {
     const int d = kCols[i].dim;
     if (d == D_PODS || !cnt[d]) continue;
@@ -1807,29 +1857,14 @@ int kr_snapshot_commit_object_rows(kr_engine *e, const uint32_t *cluster_rows, u
     else if (rb == 1) { for (uint32_t k = 0; k < cnt[d]; k++) dst[k] = col[rl[k]]; }
     else if (rb == 8) { const uint64_t *c8 = reinterpret_cast<const uint64_t *>(col); uint64_t *d8 = reinterpret_cast<uint64_t *>(dst); for (uint32_t k = 0; k < cnt[d]; k++) d8[k] = c8[rl[k]]; }
     else for (uint32_t k = 0; k < cnt[d]; k++) memcpy(dst + k * rb, col + (size_t)rl[k] * rb, rb);
-    oa.src[nc] = e->orow.d + col_off[i];
-    oa.rowlist[nc] = reinterpret_cast<const uint32_t *>(e->orow.d + list_off[d]);
-    oa.dst[nc] = e->d_in + e->il.off[i];
-    oa.first[nc] = first;
-    oa.rows_old[nc] = d == D_HEADS ? e->res_n_heads : (d == D_CLUSTERS ? n.n_clusters : n.n_groups);
-    oa.row_bytes[nc] = (uint16_t)rb;
-    oa.cls[nc] = kObjClass[i];
-    if (i == kGroupClusterCol) oa.g_cluster_idx_new = reinterpret_cast<const uint32_t *>(e->orow.d + col_off[i]);
-    if (i == kHeadKeyCol) oa.h_pod_idx_new = reinterpret_cast<const uint32_t *>(e->orow.d + col_off[i]);
-    first += cnt[d];
-    nc++;
   }
-  oa.first[nc] = first; oa.n_cols = nc;
-  // the pod -> head-aux row table follows the keys (compared here, on the host shadow)
-  for (uint32_t i = 0; i < n_hd; i++)
-    if (e->prev_h_pod_idx[head_rows[i]] != hb.h_pod_idx[head_rows[i]]) { e->heads_rebuild = true; e->prev_h_pod_idx[head_rows[i]] = hb.h_pod_idx[head_rows[i]]; }
-  CK(cudaStreamSynchronize(e->sm));  // a pass still reading the tables must finish first
-  CK(cudaEventRecord(e->ev_h2d0, e->scopy));
+  const ObjDiffArgs oa = object_diff_args(e, e->orow.d, col_off, cnt, list_off);
+  if (int rc = begin_commit(e)) return rc;
+  if (e->rec.commit_rows(hb, cluster_rows, n_cl, head_rows, n_hd)) e->gvalid = false;  // (the captured full pass launches the other k_decide2 instantiation)
   CK(cudaMemcpyAsync(e->orow.d, e->orow.h, need, cudaMemcpyHostToDevice, e->scopy));
   CK(cudaEventRecord(e->orow.ev, e->scopy));
   e->orow.busy = true;
   if (int rc = launch_object_diff(e, oa, n_hd, reinterpret_cast<const uint32_t *>(e->orow.d + list_off[D_HEADS]), n_cl != 0)) return rc;
-  e->json_cols_behind.clear();  // (every recorded row was among the ones uploaded)
   return finish_commit(e, need, true, false);
 }
 
@@ -1840,12 +1875,8 @@ int kr_snapshot_commit_spec_rows(kr_engine *e, const uint32_t *rows, uint32_t n)
   const kr_sizes &z = e->sizes;
   kr_snapshot_bufs hb;
   bind_in(e->il, e->h_in, &hb);
-  for (uint32_t i = 0; i < n; i++) {  // (every row before anything moves: an invalid call commits nothing)
-    const uint32_t c = rows[i];
-    if (c >= z.n_clusters) return fail(e, KR_E_INVALID, "cluster row %u out of range", c);
-    if (hb.c_json_off[c] & 15) return fail(e, KR_E_INVALID, "cluster %u: json offset not 16-byte aligned", c);
-    if (hb.c_json_off[c] + hb.c_json_len[c] > z.json_bytes) return fail(e, KR_E_INVALID, "cluster %u: json range outside arena", c);
-  }
+  for (uint32_t i = 0; i < n; i++)
+    if (int rc = check_cluster_row(e, hb, z, rows[i], true)) return rc;
   CK(cudaSetDevice(e->cfg.device));
   if (e->spec_stamp.size() < z.n_clusters) e->spec_stamp.resize(z.n_clusters, 0u);
   if (e->pull_stamp.size() < z.n_clusters) e->pull_stamp.resize(z.n_clusters, 0u);
@@ -1866,18 +1897,12 @@ int kr_snapshot_commit_spec_rows(kr_engine *e, const uint32_t *rows, uint32_t n)
   }
   if (m == 0) return KR_OK;
   size_t bytes = 16 * (size_t)m;
-  const bool track = e->prev_json_off.size() == z.n_clusters;  // (otherwise the next object commit sees every range as moved anyway)
   for (uint32_t i = 0; i < m; i++) {
-    const uint32_t c = lr[i];
-    ll[i] = hb.c_json_len[c]; lo[i] = hb.c_json_off[c];
+    ll[i] = hb.c_json_len[lr[i]]; lo[i] = hb.c_json_off[lr[i]];
     bytes += ((size_t)ll[i] + 15) & ~(size_t)15;
-    if (!track) continue;
-    // the recorded ranges follow (a later object commit does not re-hash everything on their account); the full-pass order does not
-    if ((e->prev_json_len[c] + 8) / 64 != (ll[i] + 8) / 64) e->spec_order_stale = true;
-    e->prev_json_off[c] = lo[i]; e->prev_json_len[c] = ll[i];
   }
-  CK(cudaStreamSynchronize(e->sm));  // a pass still reading the arena must finish first
-  CK(cudaEventRecord(e->ev_h2d0, e->scopy));
+  e->rec.commit_spec_rows(lr, lo, ll, m, z.n_clusters);
+  if (int rc = begin_commit(e)) return rc;
   uint32_t *dr = reinterpret_cast<uint32_t *>(e->spec.d) + base;
   uint32_t *dl = reinterpret_cast<uint32_t *>(e->spec.d + 4 * cap) + base;
   uint64_t *dof = reinterpret_cast<uint64_t *>(e->spec.d + 8 * cap) + base;
