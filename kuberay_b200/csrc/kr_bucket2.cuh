@@ -357,6 +357,15 @@ __global__ void __launch_bounds__(kD2Warps * 32, (K <= 4 && !kMH ? 32 : 16) / kD
   __shared__ uint32_t s_list[kD2Warps][32 * K];            // pod indices being ranked (delete candidates / acted pods); per-replica flags
                                                            // of the multi-host group being decided
   __shared__ uint32_t s_bits[kD2Warps][32];                // 1024-bit window of replica indices in use
+  // Per-cluster state that is uniform across the warp sits in the warp's shared memory, not in every lane's registers: the input
+  // record (each field one broadcast load), the result record, and two scalars the placement needs.  With that, and with the
+  // replica indices and the head's name read again from the bucket where they are used and the roll-up ahead of the action list,
+  // the K <= 4 instantiations fit their 64-register cap (32 warps per SM) without spilling.
+  __shared__ uint32_t s_in[kD2Warps][32];                  // the cluster's cl_in record (RecordCI)
+  __shared__ kr_cluster_result s_cr[kD2Warps];             // the cluster's kr_cluster_result, built in place
+  // two scalars the placement reads, kept out of registers through the decisions
+  __shared__ uint32_t s_deferred[kD2Warps];                // phase 0: the Recreate gate waits for phase 1
+  __shared__ uint32_t s_old_create[kInc ? kD2Warps : 1];   // phase 2: pods the cluster asked for in the resident results
   const SnapDev &s = a.s;
   const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint32_t lt = lanemask_lt();
@@ -364,18 +373,21 @@ __global__ void __launch_bounds__(kD2Warps * 32, (K <= 4 && !kMH ? 32 : 16) / kD
   uint32_t c = blockIdx.x * kD2Warps + warp;
   // the cluster's inputs: one 128-byte record (lane i = word i), written by k_build_tables — not by the kernel this one waits for
   bool mine = phase == 0 && c < a.n.n_clusters;
-  RecordCI ci{mine ? __ldg(&a.sc.cl_in[32 * (size_t)c + lane]) : 0u};
+  uint32_t in_word = mine ? __ldg(&a.sc.cl_in[32 * (size_t)c + lane]) : 0u;
   pdl_wait(); pdl_trigger();
   if (phase == 1) {  // compact list of the clusters phase 0 deferred
     mine = c < a.r.totals[4];
-    if (mine) { c = a.sc.deferred_list[c]; ci.word = __ldg(&a.sc.cl_in[32 * (size_t)c + lane]); }
+    if (mine) { c = a.sc.deferred_list[c]; in_word = __ldg(&a.sc.cl_in[32 * (size_t)c + lane]); }
   } else if (kInc) {  // the dirty list of an incremental epoch (input records rewritten by k_inc_prepare: no read-only path)
     mine = c < __ldcg(&a.sc.inc[KR_INC_DIRTY]) && !__ldcg(&a.sc.inc[KR_INC_VOID]) && !__ldcg(&a.sc.inc[KR_INC_STRUCTURAL]);
     if (mine) {
       c = a.sc.dirty_list[c];
-      ci.word = __ldcg(&a.sc.cl_in[32 * (size_t)c + lane]);  // (rewritten by k_inc_refresh if an object row of the cluster changed)
+      in_word = __ldcg(&a.sc.cl_in[32 * (size_t)c + lane]);  // (rewritten by k_inc_refresh if an object row of the cluster changed)
     }
   }
+  s_in[warp][lane] = in_word;
+  __syncwarp();
+  const RecordCI ci{s_in[warp]};
   if (KR_ATTEMPT_VOID(a.r.totals)) mine = false;
   // A RayCluster of more than KR_SMEM_GROUPS worker groups is k_large_sort / k_decide_large's (KR_OPT_WIDE_CLUSTERS, kr_large.cuh):
   // the lane-per-group arrays below hold 32 groups.  Left before the Recreate deferral, the digest wait and the epoch's compaction.
@@ -428,17 +440,18 @@ __global__ void __launch_bounds__(kD2Warps * 32, (K <= 4 && !kMH ? 32 : 16) / kD
       P = kept;
       dyn = make_uint4(kept, 0u, (uint32_t)raw, (uint32_t)(raw >> 32));
       if (lane == 0) a.sc.cl_dyn[c] = dyn;
-#pragma unroll
-      for (int k = 0; k < K; k++) if ((uint32_t)(k * 32) + lane < kept) recs[k] = __ldcg(&bucket[k * 32 + lane]);
     }
+    // the compacted bucket (every register rewritten, so none of the records read before the compaction stays live past it)
+#pragma unroll
+    for (int k = 0; k < K; k++) recs[k] = mine && (uint32_t)(k * 32) + lane < kept ? __ldcg(&bucket[k * 32 + lane]) : make_uint4(0, 0, 0, 0);
   }
   const uint32_t cf = ci.flags(), G = ci.group_cnt(), g0 = ci.group_off();
   const uint8_t suspend_status = ci.suspend_status(), ext_err = ci.ext_err_kind(), old_prov = ci.cond_status(KR_COND_PROVISIONED);
   const bool gate = a.f.gate_status_conditions != 0;
-  uint32_t old_create = 0;  // phase 2: pods this cluster asked for in the resident results (they leave the running total)
-  if (kInc && mine) {
+  if (kInc && mine) {  // phase 2: pods this cluster asked for in the resident results (they leave the running total)
+    uint32_t old_create = 0;
     for (uint32_t gi = lane; gi < G; gi += 32) old_create += a.r.groups[g0 + gi].n_create;
-    old_create = __reduce_add_sync(0xFFFFFFFFu, old_create);
+    s_old_create[warp] = __reduce_add_sync(0xFFFFFFFFu, old_create);  // (read by the placement, after the group loop rewrote the records)
   }
   // first head in List order = the smallest pod index among the heads (k_match2), with its head-aux row
   uint32_t head_pod = 0xFFFFFFFFu;
@@ -450,21 +463,20 @@ __global__ void __launch_bounds__(kD2Warps * 32, (K <= 4 && !kMH ? 32 : 16) / kD
   // what the decisions need from the head-aux table goes out now, beside the bucket
   uint8_t h_ver = KR_VER_EMPTY, h_ast = KR_ANNOT_EMPTY;
   if (head_aux >= 0 && (cf & KR_CF_UPGRADE_RECREATE)) { h_ver = s.h_version_state[head_aux]; h_ast = s.h_annot_state[head_aux]; }
-  uint32_t pidx[K], pw[K], ridx[K], act[K];
-  uint32_t head_pos = 0xFFFFFFFFu, head_name = 0, head_flags = 0;
+  uint32_t pidx[K], pw[K], act[K];
+  uint32_t head_pos = 0xFFFFFFFFu, head_flags = 0;  // (the head's name is read from its bucket record by the roll-up)
 #pragma unroll
   for (int k = 0; k < K; k++) {
     const uint32_t i = k * 32 + lane;
     const bool valid = i < P;
-    pidx[k] = valid ? recs[k].x : 0xFFFFFFFFu; pw[k] = valid ? recs[k].y : (KR_ROW_NO_GROUP << 16); ridx[k] = valid ? recs[k].z : 0u; act[k] = KR_ACT_KEEP;
+    pidx[k] = valid ? recs[k].x : 0xFFFFFFFFu; pw[k] = valid ? recs[k].y : (KR_ROW_NO_GROUP << 16); act[k] = KR_ACT_KEEP;
     const uint32_t hit = __ballot_sync(0xFFFFFFFFu, valid && recs[k].x == head_pod);
     if (hit) {
       const int src = __ffs(hit) - 1;
       head_pos = k * 32 + src;
-      head_name = __shfl_sync(0xFFFFFFFFu, recs[k].w, src); head_flags = __shfl_sync(0xFFFFFFFFu, recs[k].y, src) & 0xFFFFu;
+      head_flags = __shfl_sync(0xFFFFFFFFu, recs[k].y, src) & 0xFFFFu;
     }
   }
-  (void)head_pos;
   int32_t *acc_list = s_acc[warp][0], *acc_unh = s_acc[warp][1], *acc_wtd = s_acc[warp][2];
   int32_t *g_mode = s_mode[warp][0], *g_prefix = s_mode[warp][1], *g_ncreate = s_mode[warp][2], *g_mh_running = s_mode[warp][kMH ? 3 : 2];
   uint32_t mh_head = 0;  // kMH: bit k = this lane's pod of chunk k is the first pod of a healthy replica of a multi-host group
@@ -510,15 +522,19 @@ __global__ void __launch_bounds__(kD2Warps * 32, (K <= 4 && !kMH ? 32 : 16) / kD
   if (G == 1) { if (lane == 0) { acc_list[0] = n0_list; acc_unh[0] = n0_unh; acc_wtd[0] = n0_wtd; } __syncwarp(); }
 
   // ---------------- scalar decisions (uniform across the warp) — same order as decide_cluster / the reference
-  kr_cluster_result cr;
-  {
-    uint32_t *z = reinterpret_cast<uint32_t *>(&cr);
-#pragma unroll
-    for (int k = 0; k < (int)(sizeof(cr) / 4); k++) z[k] = 0;
+  // Every lane stores the same value to each field of cr.  A field stored twice with different values (stop_after_group) has a
+  // __syncwarp between the stores, so no lane's earlier store can land after another lane's later one.  (volatile: each field is
+  // stored where it is decided and loaded where it is read, instead of being carried in registers to a merged store.)
+  volatile kr_cluster_result &cr = s_cr[warp];
+  static_assert(sizeof(kr_cluster_result) % 4 == 0 && sizeof(kr_cluster_result) / 4 <= 32, "one word of the result record per lane");
+  if (lane < sizeof(kr_cluster_result) / 4) {  // all zero but head_pod_idx = stop_after_group = -1
+    const bool neg = lane == offsetof(kr_cluster_result, head_pod_idx) / 4 || lane == offsetof(kr_cluster_result, stop_after_group) / 4;
+    reinterpret_cast<volatile uint32_t *>(&cr)[lane] = neg ? 0xFFFFFFFFu : 0u;
   }
-  cr.head_pod_idx = -1; cr.stop_after_group = -1;
+  if (lane == 0) s_deferred[warp] = 0;
+  __syncwarp();
   uint8_t all_action = KR_ACT_KEEP;
-  bool head_delete = false, run_groups = false, deferred = false, any_prefix = false;
+  bool head_delete = false, run_groups = false, any_prefix = false;
   uint32_t n_create_cluster = 0;
   if (mine) {
     if (cf & KR_CF_SKIP) {
@@ -541,7 +557,7 @@ __global__ void __launch_bounds__(kD2Warps * 32, (K <= 4 && !kMH ? 32 : 16) / kD
           if (phase == 0 && !a.spin_hash) {
             // The hash kernel is still running on its own stream.  Decide the cluster as if the digests matched, reserve the
             // whole bucket in the action list (a Recreate deletes every pod) and let phase 1 redo it once the digest is there.
-            deferred = true;
+            s_deferred[warp] = 1;
             if (lane == 0) a.sc.deferred_list[atomicAdd(&a.r.totals[4], 1u)] = c;
           } else {
             const uint8_t *ah = s.h_annot_hash + 32 * (size_t)aux;
@@ -714,6 +730,16 @@ __global__ void __launch_bounds__(kD2Warps * 32, (K <= 4 && !kMH ? 32 : 16) / kD
       }
     }
   }
+  // ---------------- status roll-up + record (needs nothing from the action list and the placement below: it comes first, so no
+  // register of theirs is live through it)
+  if (!(cf & KR_CF_SKIP)) {  // (every lane runs it, uniformly: the inputs are one broadcast load away in the record)
+    const uint32_t head_name = (n_heads == 1 && head_pos != 0xFFFFFFFFu) ? __ldcg(&a.sc.bucket[(size_t)c * S + head_pos].w) : 0u;
+    status_rollup(a.s, a.f, ci, cr, P, (uint32_t)n_heads, n_heads > 0 ? (int32_t)head_pod : -1, head_aux, head_name, ready, available, all_running);
+  }
+  __syncwarp();
+  if (mine && lane < sizeof(kr_cluster_result) / 4)  // one coalesced store: lane i = word i
+    reinterpret_cast<uint32_t *>(&a.r.clusters[c])[lane] = reinterpret_cast<const volatile uint32_t *>(&cr)[lane];
+
   // the cluster's action list in List order: stage the acted pods, rank each by counting the smaller pod indices
   uint32_t n_act = 0;
   uint32_t arank[K];
@@ -737,17 +763,13 @@ __global__ void __launch_bounds__(kD2Warps * 32, (K <= 4 && !kMH ? 32 : 16) / kD
     }
   }
 
-  // ---------------- status roll-up + record (needs nothing from the placement below)
-  if (!(cf & KR_CF_SKIP))  // (every lane runs it, uniformly: the inputs are one shuffle away in the record)
-    status_rollup(a.s, a.f, ci, cr, P, (uint32_t)n_heads, n_heads > 0 ? (int32_t)head_pod : -1, head_aux, head_name, ready, available, all_running);
-  if (mine && lane == 0) a.r.clusters[c] = cr;
-
   // ---------------- placement: where this cluster's action list and replica indices go.  One returning 64-bit atomic per
   // RayCluster on the two arena cursors (pods to create << 32 | action slots), issued by lane 0 and needed only for the stores
   // below.  (A decoupled look-back over the CTAs was built first: placement in cluster order, but the prefix crosses the grid in
   // 32-CTA hops — 39 hops on the critical path of a 10 k-cluster pass, with the kernel's stalls gathered at the barrier
   // in front of it.  The owners' ORDER inside the arenas is therefore unspecified; every owner
   // finds its place through (act_start, act_cnt) / (create_off, n_create), which is what the shim reads anyway.)
+  const bool deferred = s_deferred[warp] != 0;
   const uint32_t slots = deferred ? P : n_act;  // a deferred cluster may still turn into "delete every pod"
   uint32_t act_off = 0, create_off = 0;
   if (phase == 0) {
@@ -768,7 +790,7 @@ __global__ void __launch_bounds__(kD2Warps * 32, (K <= 4 && !kMH ? 32 : 16) / kD
     unsigned long long base = 0;
     uint32_t need = 0;  // bit 0: new action slots, bit 1: new create slots
     if (mine && lane == 0) {
-      const uint32_t old_act = a.r.act_cnt[c];
+      const uint32_t old_act = a.r.act_cnt[c], old_create = s_old_create[warp];
       need = (n_act > a.sc.act_res[c] ? 1u : 0u) | (n_create_cluster > a.sc.cre_res[c] ? 2u : 0u);
       if (need) base = atomicAdd(reinterpret_cast<unsigned long long *>(&a.r.totals[8]), ((unsigned long long)((need & 2u) ? n_create_cluster : 0u) << 32) | ((need & 1u) ? n_act : 0u));
       if ((need & 1u) && (uint64_t)(uint32_t)base + n_act > a.n.n_pods) a.sc.inc[KR_INC_VOID] = 1u;          // the action list is full of abandoned runs:
@@ -830,7 +852,8 @@ __global__ void __launch_bounds__(kD2Warps * 32, (K <= 4 && !kMH ? 32 : 16) / kD
           for (int k = 0; k < K; k++) {
             // runningPods of this group: listed, not deleted by name, label present and numeric
             if ((pw[k] >> 16) == gi && (pw[k] & KR_PP_HAS_REPLICA_IDX) && (mh ? ((mh_head >> k) & 1u) != 0 : (act[k] == KR_ACT_KEEP && pidx[k] != 0xFFFFFFFFu))) {
-              const int32_t idx = (int32_t)ridx[k];
+              // (read again here from the bucket: no register holds it, or the bucket's address, through the decisions)
+              const int32_t idx = (int32_t)__ldcg(&a.sc.bucket[(size_t)c * S + k * 32 + lane].z);
               if (idx >= 0 && (uint64_t)idx >= w0 && (uint64_t)idx < w0 + 1024 && (uint64_t)idx < bound)
                 atomicOr(&s_bits[warp][(idx - w0) >> 5], 1u << ((idx - w0) & 31));
             }

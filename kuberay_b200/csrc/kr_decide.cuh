@@ -70,11 +70,12 @@ struct ColumnsCI {
   __device__ __forceinline__ int32_t g0_max() const { return 0; }
   __device__ __forceinline__ int32_t g0_hosts() const { return 0; }
 };
-// ... or in the 128-byte cl_in record the warp loaded with one access, lane i holding word i (bucket pipeline: every lane runs
-// the roll-up, uniformly, and each field is one shuffle away).
+// ... or in the 128-byte cl_in record the warp loaded with one access (lane i storing word i) into its own shared-memory slot
+// (bucket pipeline: every lane runs the roll-up, uniformly, and each field is one broadcast load away — no shuffle, and no
+// register holds the record).
 struct RecordCI {
-  uint32_t word;  // this lane's word of the record
-  __device__ __forceinline__ uint32_t w(int i) const { return __shfl_sync(0xFFFFFFFFu, word, i); }
+  const uint32_t *rec;  // the warp's 32-word slot in shared memory
+  __device__ __forceinline__ uint32_t w(int i) const { return rec[i]; }
   __device__ __forceinline__ uint8_t byte(int i, int b) const { return (uint8_t)(w(i) >> (8 * b)); }
   __device__ __forceinline__ uint32_t flags() const { return w(KR_CI_FLAGS); }
   __device__ __forceinline__ uint8_t ext_err_kind() const { return byte(KR_CI_B0, 1); }
@@ -102,20 +103,19 @@ struct RecordCI {
 };
 
 // calculateStatus (raycluster_controller.go:1552-1719) + InconsistentRayClusterStatus (utils/consistency.go:16-34).
-// Scalar code: executed by lane 0 only (ColumnsCI) or by every lane uniformly (RecordCI).  aux = head-aux row of the first head
-// pod (-1: none / not in the table).
-template <class CI>
-__device__ __forceinline__ void status_rollup(const SnapDev &s, const kr_flags &f, const CI &ci, kr_cluster_result &cr, uint32_t P, uint32_t n_heads,
+// Scalar code: executed by lane 0 only (ColumnsCI) or by every lane uniformly (RecordCI, with cr a volatile reference to the
+// warp's shared slot: every lane stores the same value).  aux = head-aux row of the first head pod (-1: none / not in the table).
+template <class CI, class CR>
+__device__ __forceinline__ void status_rollup(const SnapDev &s, const kr_flags &f, const CI &ci, CR &cr, uint32_t P, uint32_t n_heads,
                                               int32_t head_pod, int32_t aux, uint32_t head_name_id, int32_t ready, int32_t available, bool all_running) {
   const uint32_t cf = ci.flags();
   const bool gate = f.gate_status_conditions != 0;
   const bool reconcile_err = cr.err_kind != KR_ERR_NONE;
   const uint8_t ek = ci.ext_err_kind();
-  uint8_t cst[KR_NUM_CONDS], cvr[KR_NUM_CONDS], ocst[KR_NUM_CONDS], ocvr[KR_NUM_CONDS];
+  uint8_t cst[KR_NUM_CONDS], cvr[KR_NUM_CONDS];
 #pragma unroll
-  for (int k = 0; k < KR_NUM_CONDS; k++) { ocst[k] = cst[k] = ci.cond_status(k); ocvr[k] = cvr[k] = ci.cond_variant(k); }
-  const uint32_t old_reason = ci.reason(), old_msg0 = ci.msg(0), old_msg1 = ci.msg(1);
-  uint32_t hpr_reason = old_reason, hpr_msg = old_msg0, rf_msg = old_msg1;
+  for (int k = 0; k < KR_NUM_CONDS; k++) { cst[k] = ci.cond_status(k); cvr[k] = ci.cond_variant(k); }
+  uint32_t hpr_reason = ci.reason(), hpr_msg = ci.msg(0), rf_msg = ci.msg(1);
   if (gate) {  // :1563-1577
     if (reconcile_err) {
       if (ek >= KR_EXT_ERR_FAILED_DELETE_ALL_PODS && ek <= KR_EXT_ERR_FAILED_CREATE_WORKER_POD) {
@@ -213,15 +213,17 @@ __device__ __forceinline__ void status_rollup(const SnapDev &s, const kr_flags &
   if (cf & KR_CF_ENDPOINTS_CHANGED) inc = true;
 #pragma unroll
   for (int k = 0; k < 4; k++) if (ci.old_head(k) != head_ids[k]) inc = true;
+  // (the old conditions are read from ci again and the new ones from cr: no copy of either is held through the roll-up)
 #pragma unroll
   for (int k = 0; k < KR_NUM_CONDS; k++) {
-    if (ocst[k] != cst[k]) { inc = true; continue; }
-    if (cst[k] == KR_COND_ABSENT) continue;
+    const uint8_t st = cr.cond_status[k];
+    if (ci.cond_status(k) != st) { inc = true; continue; }
+    if (st == KR_COND_ABSENT) continue;
     if (k == KR_COND_HEAD_POD_READY) {
-      if (old_reason != hpr_reason || old_msg0 != hpr_msg) inc = true;
+      if (ci.reason() != cr.head_ready_reason_id || ci.msg(0) != cr.head_ready_msg_id) inc = true;
     } else if (k == KR_COND_REPLICA_FAILURE) {
-      if (ocvr[k] != cvr[k] || old_msg1 != rf_msg) inc = true;
-    } else if (ocvr[k] != cvr[k]) inc = true;
+      if (ci.cond_variant(k) != cr.cond_variant[k] || ci.msg(1) != rf_msg) inc = true;
+    } else if (ci.cond_variant(k) != cr.cond_variant[k]) inc = true;
   }
   cr.needs_status_write = inc ? 1 : 0;
 }
