@@ -537,9 +537,11 @@ int kr_last_profile(kr_engine *e, kr_profile *prof);
 /* Engine options (call before the first kr_snapshot_begin).
  * KR_OPT_FIXED_LAYOUT = 1: lay the arenas out once, for the capacities given to kr_engine_create, instead of per snapshot.
  *   Column addresses then never move: kr_snapshot_begin(sizes) only sets the live row counts (<= capacities) and returns the
- *   same pointers, what is resident in HBM stays valid across begins, and an informer event that changes a table's row count
- *   (a RayCluster or head Pod appears, workersToDelete lists grow, a Pod is appended after the last row) is still an
- *   incremental epoch: kr_snapshot_begin(new counts) + KR_PART_OBJECTS + kr_snapshot_commit_pod_rows/_values. */
+ *   same pointers, and what is resident in HBM stays valid across begins.  A head Pod appearing or going, or a Pod appended after
+ *   the last row, is still an incremental epoch: kr_snapshot_begin(new counts) + KR_PART_OBJECTS + kr_snapshot_commit_pod_rows/
+ *   _values.  So are workersToDelete lists that grow or shrink, with KR_OPT_WTD_EDITS, and RayClusters appended after the last row
+ *   or RayJobs created or deleted, with KR_OPT_CLUSTER_CREATES.  Any other change of a row count (a RayCluster deleted, a worker
+ *   group added to a RayCluster) makes the next pass a full one. */
 enum {
   KR_OPT_FIXED_LAYOUT = 1,
   KR_OPT_INCREMENTAL = 2,  /* 1 (default): passes after a full bucket-pipeline pass are incremental on the device whenever the commits in
@@ -576,9 +578,22 @@ enum {
                               any such edit makes the next pass a full one).  May be set at any time; read at each object commit.
                               kr_snapshot_commit_object_rows still expects unchanged lists: with this option, rows whose lists changed
                               are committed as the whole object part. */
-  KR_OPT_SPEC_ROWS = 8        /* 1: the native packer (kr_packer_flush) commits re-emitted specs with kr_snapshot_commit_spec_rows and
+  KR_OPT_SPEC_ROWS = 8,       /* 1: the native packer (kr_packer_flush) commits re-emitted specs with kr_snapshot_commit_spec_rows and
                               reports KR_PACK_SPEC_ROWS instead of KR_PART_JSON (a flush that compacts the JSON arena still sends
                               KR_PART_JSON).  The engine call itself needs no option.  Results are the same as with 0 (the default). */
+  KR_OPT_CLUSTER_CREATES = 9  /* 1, together with KR_OPT_FIXED_LAYOUT: RayClusters appended after the last row (every existing
+                              RayCluster keeps its row, its groups and its workersToDelete names, and the new groups and names come after
+                              all the old ones), and RayJobs created or deleted, keep the incremental epoch: kr_snapshot_begin(new
+                              counts), the object part (KR_PART_OBJECTS), then the new RayClusters' specs with
+                              kr_snapshot_commit_spec_rows.  The next pass hashes only those specs, inserts the new RayClusters into
+                              the resident tables, moves the resident Pods labelled for them out of the orphans and into their buckets,
+                              and returns them among changed_clusters.  A RayCluster deleted, a worker group added to an existing one,
+                              fewer RayClusters than before, or a RayCluster the resident state cannot hold (more Pods than its bucket
+                              without KR_OPT_LARGE_CLUSTERS, more than 32 worker groups without KR_OPT_WIDE_CLUSTERS) still takes the
+                              full pass.  Results are the same as with 0 (the default: every such event makes the next pass a full
+                              one).  May be set at any time; read at each kr_snapshot_begin and object commit.  No effect without
+                              KR_OPT_FIXED_LAYOUT.  The native packer's flush takes this path by itself when the engine has the option
+                              and a flush only appended RayClusters or created and deleted RayJobs. */
 };
 enum { KR_LARGE_MAX_PODS = 8192 };  /* largest RayCluster KR_OPT_LARGE_CLUSTERS keeps on the bucket pipeline */
 int kr_engine_set_option(kr_engine *e, uint32_t option, uint64_t value);

@@ -142,6 +142,10 @@ const (
 	OptHugeClusters  = uint32(C.KR_OPT_HUGE_CLUSTERS)
 	OptWtdEdits      = uint32(C.KR_OPT_WTD_EDITS)
 	OptSpecRows      = uint32(C.KR_OPT_SPEC_ROWS)
+	// OptClusterCreates is KR_OPT_CLUSTER_CREATES (1: RayClusters appended after the last row and RayJobs created or deleted keep
+	// incremental epochs; only under KR_OPT_FIXED_LAYOUT; recommended for fleets that create RayClusters, such as RayJob and
+	// RayService fleets; read at each Begin and object commit).
+	OptClusterCreates = uint32(C.KR_OPT_CLUSTER_CREATES)
 )
 
 // SetOption: KR_OPT_FIXED_LAYOUT (before the first Begin), KR_OPT_INCREMENTAL, KR_OPT_LARGE_CLUSTERS (1: RayClusters of 257 to
@@ -150,8 +154,9 @@ const (
 // at the next full pass), KR_OPT_HUGE_CLUSTERS (1, with KR_OPT_LARGE_CLUSTERS: the same for RayClusters of more than
 // KR_LARGE_MAX_PODS pods; takes effect at the next full pass), KR_OPT_WTD_EDITS (1: scaleStrategy.workersToDelete edits keep
 // incremental epochs; recommended for autoscaling fleets; read at each object commit), KR_OPT_SPEC_ROWS (1: Packer.Flush commits
-// re-emitted specs with CommitSpecRows instead of the whole JSON arena and reports PackSpecRows).  For a Packer, call it on
-// Packer.Engine().
+// re-emitted specs with CommitSpecRows instead of the whole JSON arena and reports PackSpecRows), KR_OPT_CLUSTER_CREATES (1, with
+// KR_OPT_FIXED_LAYOUT: RayClusters appended after the last row and RayJobs created or deleted keep incremental epochs; read at each
+// Begin and object commit).  For a Packer, call it on Packer.Engine().
 func (e *Engine) SetOption(option uint32, value uint64) error {
 	if rc := C.kr_engine_set_option(e.h, C.uint32_t(option), C.uint64_t(value)); rc != C.KR_OK {
 		return e.err(rc)

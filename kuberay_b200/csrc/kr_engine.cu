@@ -34,6 +34,9 @@ int kr_specjson_emit_string(const uint8_t *spec_json, uint64_t len, bool muted, 
 namespace {
 
 constexpr size_t kAlign = 256;
+// most RayClusters one incremental epoch appends while there are orphans (k_inc_orphan_adopt: 16 Bloom bits and two 4-byte table
+// slots per RayCluster in shared memory, 40 KB); more take the full pass
+constexpr uint32_t kAdoptMax = 4096;
 inline size_t align_up(size_t x, size_t a = kAlign) { return (x + a - 1) / a * a; }
 inline uint32_t pow2_at_least(uint64_t x) { uint32_t p = 16; while (p < x) p <<= 1; return p; }
 // staging of an incremental pass's changed records, for up to a quarter of the RayClusters (beyond that the whole record arrays are
@@ -109,7 +112,12 @@ static_assert(kCols[kHeadKeyCol].dim == D_HEADS && kCols[kHeadKeyCol - 1].dim ==
 // reads the count.
 constexpr int kWtdOffCol = 29, kWtdCntCol = 30, kWtdNameCol = 31;
 static_assert(kCols[kWtdCntCol].dim == D_GROUPS && kCols[kWtdNameCol].dim == D_WTD && kCols[kWtdNameCol + 1].dim == D_PODS, "workersToDelete column indices");
-uint8_t obj_class(int col, bool wtd_edits) {
+// With KR_OPT_CLUSTER_CREATES a row past the resident rows of a RayCluster / group / workersToDelete column belongs to a RayCluster
+// the epoch appended (`appended`): it marks that RayCluster dirty and refreshes its input record (a group row: its RayCluster's) instead
+// of making the epoch structural.
+uint8_t obj_class(int col, bool wtd_edits, bool appended = false) {
+  if (appended && kObjClass[col] == KR_OC_STRUCT)
+    return kCols[col].dim == D_CLUSTERS ? KR_OC_CLUSTER : kCols[col].dim == D_GROUPS ? KR_OC_GROUP : KR_OC_COPY;
   if (wtd_edits && (col == kWtdOffCol || col == kWtdNameCol)) return KR_OC_COPY;
   if (wtd_edits && col == kWtdCntCol) return KR_OC_GROUP;
   return kObjClass[col];
@@ -135,6 +143,7 @@ struct CommitRecord {
   // distinct): the row path takes them only all together; any object commit clears the list
   std::vector<uint32_t> json_cols_behind;
   uint32_t res_n_heads = 0;              // head-aux rows the resident device columns hold: whole with the object part
+  uint32_t res_clusters = 0, res_groups = 0, res_wtd = 0;  // ... and RayCluster / group / workersToDelete rows: whole with the object part
   std::vector<uint32_t> prev_h_pod_idx;  // ... and their keys: whole with the object part, rows
   std::vector<uint32_t> prev_wtd;        // KR_OPT_WTD_EDITS: {n_groups, g_wtd_off, g_wtd_cnt, w_name_id} (empty while it is off): whole with the object part
   bool hash_dirty = false;        // spec JSON or a JSON range committed since the digests were computed: whole
@@ -165,17 +174,20 @@ struct CommitRecord {
     return std::includes(given.begin(), given.end(), json_cols_behind.begin(), json_cols_behind.end());
   }
 
-  struct Moved { bool shape, wide, order; };  // what a whole commit moved: the launch shape / pipeline, the wide set, the hash order
-  Moved commit_whole(const kr_snapshot_bufs &hb, const kr_sizes &n, uint32_t parts, bool wtd_edits) {
+  // what a whole commit moved: the launch shape / pipeline, the wide set, the hash order; RayClusters from row `appended` on are new
+  // rows of KR_OPT_CLUSTER_CREATES (n_clusters: none), whose specs the caller commits as spec rows
+  struct Moved { bool shape, wide, order; uint32_t appended; };
+  Moved commit_whole(const kr_snapshot_bufs &hb, const kr_sizes &n, uint32_t parts, bool wtd_edits, bool creates) {
     const bool objects = parts & (KR_PART_COLUMNS | KR_PART_OBJECTS);
     const size_t had = rows.size();
-    bool ranges_moved = had != n.n_clusters;  // some RayCluster's JSON range differs from the one the digests / the hash order were computed from
+    const bool appends = creates && objects && n.n_clusters > had;  // (not a moved range: only the new rows are hashed)
+    bool ranges_moved = had != n.n_clusters && !appends;  // some RayCluster's JSON range differs from the one the digests / the hash order were computed from
     uint32_t n_rc = 0, n_mh_now = 0, max_groups = 0;
     std::vector<uint32_t> wide;
     rows.resize(n.n_clusters);
     for (uint32_t c = 0; c < n.n_clusters; c++) {
       Row &r = rows[c];
-      const bool moved = c >= had || r.json_off != hb.c_json_off[c] || r.json_len != hb.c_json_len[c];
+      const bool moved = c >= had ? !appends : r.json_off != hb.c_json_off[c] || r.json_len != hb.c_json_len[c];
       if (moved && !objects) json_cols_behind.push_back(c);  // (the device's range columns keep the old range)
       ranges_moved |= moved;
       r.json_off = hb.c_json_off[c]; r.json_len = hb.c_json_len[c];
@@ -198,15 +210,17 @@ struct CommitRecord {
     uint64_t rsig = 0x9E3779B97F4A7C15ull * (n_rc + 1);
     for (uint32_t c = 0; c < n.n_clusters; c++) if (hb.c_flags[c] & KR_CF_UPGRADE_RECREATE) rsig = (rsig ^ c) * 0x100000001B3ull;
     // (a spec-row commit updates the recorded ranges itself: its own flag says the order no longer follows them)
-    const bool order = ranges_moved || rsig != recreate_sig || spec_order_stale;
-    if (order) { recreate_sig = rsig; spec_order_stale = false; }  // (the new order travels with this commit)
+    bool order = ranges_moved || rsig != recreate_sig || spec_order_stale;
+    if (appends && !ranges_moved) { spec_order_stale = true; order = false; }  // (the order lacks the new rows: the next pass that hashes every message rebuilds it)
+    if (order) spec_order_stale = false;  // (the new order travels with this commit)
+    recreate_sig = rsig;
     if ((parts & KR_PART_JSON) || ranges_moved) hash_dirty = true;
     if (objects) {
       if (prev_h_pod_idx.size() != n.n_heads || (n.n_heads && memcmp(prev_h_pod_idx.data(), hb.h_pod_idx, 4 * (size_t)n.n_heads) != 0)) {
         heads_rebuild = true;
         prev_h_pod_idx.assign(hb.h_pod_idx, hb.h_pod_idx + n.n_heads);
       }
-      res_n_heads = n.n_heads;
+      res_n_heads = n.n_heads; res_clusters = n.n_clusters; res_groups = n.n_groups; res_wtd = n.n_wtd;
       if (!wtd_edits) prev_wtd.clear();  // (the first commit after the option is turned on rebuilds the name table once)
       else if (!wtd_same(hb, n)) {
         wtd_rebuild = true;
@@ -216,7 +230,7 @@ struct CommitRecord {
         prev_wtd.insert(prev_wtd.end(), hb.w_name_id, hb.w_name_id + n.n_wtd);
       }
     }
-    return {shape, wide_moved, order};
+    return {shape, wide_moved, order, appends ? (uint32_t)had : n.n_clusters};
   }
   // -> the snapshot's first multi-host group came or its last went (a numOfHosts edit)
   bool commit_rows(const kr_snapshot_bufs &hb, const uint32_t *cl, uint32_t n_cl, const uint32_t *hd, uint32_t n_hd) {
@@ -234,9 +248,10 @@ struct CommitRecord {
   }
   // the m pulled rows' new ranges: a later object commit does not re-hash everything on their account; the full-pass hash order
   // does not follow them (spec_order_stale when a block count moved)
-  void commit_spec_rows(const uint32_t *cl, const uint64_t *off, const uint32_t *len, uint32_t m, uint32_t n_clusters) {
-    if (rows.size() != n_clusters) return;  // (the next object commit sees every range as moved anyway)
+  // (rows past the recorded ones: the next object commit records them as appended, or sees every range as moved)
+  void commit_spec_rows(const uint32_t *cl, const uint64_t *off, const uint32_t *len, uint32_t m) {
     for (uint32_t i = 0; i < m; i++) {
+      if (cl[i] >= rows.size()) continue;
       Row &r = rows[cl[i]];
       if ((r.json_len + 8) / 64 != (len[i] + 8) / 64) spec_order_stale = true;
       r.json_off = off[i]; r.json_len = len[i];
@@ -478,6 +493,8 @@ struct kr_engine {
   kr_flags inc_flags{};          // flags of the pass that left the resident state
   uint32_t inc_n_pods = 0, inc_n_heads = 0;  // rows resident at the last pass
   bool wtd_edits = false;        // KR_OPT_WTD_EDITS
+  bool cluster_creates = false;  // KR_OPT_CLUSTER_CREATES
+  uint32_t inc_n_clusters = 0;   // RayClusters in the resident tables (those past it were appended since the last pass)
   uint32_t res_n_wtd = 0;        // names in the resident name table and its resolutions (wtd_pod_idx)
   bool ran_inc = false;          // the last pass was an incremental one
   bool host_results_stale = false;  // an incremental pass went unfetched: the host copy misses its records, the next fetch copies everything
@@ -1060,7 +1077,7 @@ void after_full_pass(kr_engine *e, const kr_flags &f) {
   // (a pass whose create runs overran kr_config.max_creates is reported as KR_E_CAPACITY and left groups' runs unwritten: an
   // incremental epoch would inherit that cursor and fail the same way, so the next pass starts over)
   e->inc_valid = e->ran_bucket && !e->no_incr && e->h_totals[9] <= e->cfg.max_creates;
-  e->inc_flags = f; e->inc_n_pods = e->sizes.n_pods; e->inc_n_heads = e->sizes.n_heads;
+  e->inc_flags = f; e->inc_n_pods = e->sizes.n_pods; e->inc_n_heads = e->sizes.n_heads; e->inc_n_clusters = e->sizes.n_clusters;
   e->host_results_stale = false; e->inc_n_dirty = 0; e->fetched = false; e->ran_inc = false; e->rec.heads_rebuild = false;
   e->rec.wtd_rebuild = false; e->res_n_wtd = e->sizes.n_wtd;
   if (!f.skip_hash) { e->rec.hash_dirty = false; clear_spec_rows(e); }
@@ -1082,8 +1099,16 @@ void commits_read(kr_engine *e) {
 // *done_inc = false means the attempt was void (structural object change, bucket / arena overflow) and a full pass must follow.
 int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile, bool *done_inc) {
   *done_inc = false;
-  PassCtx c(e, profile);
   const kr_sizes &n = e->sizes;
+  // RayClusters appended since the last pass (KR_OPT_CLUSTER_CREATES; the keep test of kr_snapshot_begin let nothing else move
+  // n_clusters): their rows must have been committed, the bucket arena must hold them at this stride, a wide one needs
+  // KR_OPT_WIDE_CLUSTERS, and the orphan scan's shared-memory table holds kAdoptMax of them
+  const uint32_t c0 = e->inc_n_clusters, c1 = n.n_clusters;
+  const bool adopt = c1 > c0 && e->h_totals[1] != 0;  // (the last pass counted orphans: some of them may be the new RayClusters' Pods)
+  if (c1 != c0 && (c1 < c0 || e->rec.res_clusters != c1 || e->rec.res_groups != n.n_groups || (size_t)c1 * e->bstride > e->sl.bucket_entries ||
+                   (e->rec.snap_max_groups > KR_SMEM_GROUPS && !e->wide_on) || (adopt && c1 - c0 > kAdoptMax)))
+    return KR_OK;
+  PassCtx c(e, profile);
   const SnapDev &s = c.s; const ResDev &r = c.r; const ScratchDev &sc = c.sc; const Sizes &z = c.z;
   const cudaStream_t M = c.M, H = c.H;
   CK(cudaStreamWaitEvent(M, e->ev_cols, 0));
@@ -1118,10 +1143,29 @@ int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile
       c.mark("k_inc_wtd_insert");
       k_inc_wtd_insert<<<std::min<uint32_t>(grid, (n.n_groups + 255) / 256 + 1), 256, 0, M>>>(s, sc, z);
       c.mark("k_inc_wtd_resolve");
-      k_inc_wtd_resolve<<<std::min<uint32_t>((uint32_t)e->sm_count * 4, (n.n_pods + 255) / 256 + 1), 256, e->sl.wt_bits_n / 8, M>>>(s, sc, r, z, e->inc_n_pods);
+      k_inc_wtd_resolve<<<std::min<uint32_t>((uint32_t)e->sm_count * 4, (n.n_pods + 255) / 256 + 1), 256, e->sl.wt_bits_n / 8, M>>>(s, sc, r, z, e->inc_n_pods, 0u);
     }
     e->res_n_wtd = n.n_wtd;
     e->rec.wtd_rebuild = false;
+  }
+  if (c1 > c0) {  // RayClusters appended (kr_incr.cuh): their orphans touched while the table does not hold them, then they enter it
+    if (adopt) {
+      uint32_t bloom_bits = 1024, slots = 64;
+      while (bloom_bits < 16 * (c1 - c0)) bloom_bits <<= 1;
+      while (slots < 2 * (c1 - c0)) slots <<= 1;
+      c.mark("k_inc_orphan_adopt");
+      k_inc_orphan_adopt<<<std::min<uint32_t>((uint32_t)e->sm_count * 4, (e->inc_n_pods + 255) / 256 + 1), 256, bloom_bits / 8 + 4 * (size_t)slots, M>>>(
+          s, sc, r, c0, c1, bloom_bits - 1, slots - 1, e->inc_n_pods);
+    }
+    // their workersToDelete names: inserted here and resolved against every pod row (unless the whole table was rebuilt above)
+    const bool names = n.n_wtd > e->res_n_wtd;
+    c.mark("k_inc_clusters_insert");
+    k_inc_clusters_insert<<<(c1 - c0 + 255) / 256, 256, 0, M>>>(s, sc, r, c0, c1, names ? 1 : 0);
+    if (names) {
+      c.mark("k_inc_wtd_resolve");
+      k_inc_wtd_resolve<<<std::min<uint32_t>((uint32_t)e->sm_count * 4, (n.n_pods + 255) / 256 + 1), 256, e->sl.wt_bits_n / 8, M>>>(s, sc, r, z, e->inc_n_pods, e->res_n_wtd);
+      e->res_n_wtd = n.n_wtd;  // (a void attempt is followed by the full pass, which sets it again)
+    }
   }
   // (k_inc_refresh ran behind the object commits' diff kernels: the input records are current)
   c.mark("k_inc_admit");
@@ -1196,13 +1240,14 @@ int run_pass(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile) {
   if (!profile) CK(cudaEventRecord(e->ev_a, e->sm));
   e->last_flags = f;
   new_pull_epoch(e);
-  // (the list moves only with a group count, which no incremental epoch absorbs, an option or a new layout: a full pass follows)
+  // (the list moves with a group count, an option or a new layout, when a full pass follows, and with the RayClusters an incremental
+  // epoch of KR_OPT_CLUSTER_CREATES appended)
   if (e->lg_stale) if (int rc = upload_lg(e)) return rc;
   if (e->inc_valid && !e->no_incr && memcmp(&e->inc_flags, &f, sizeof f) == 0) {
     if (profile) CK(cudaEventRecord(e->ev_a, e->sm));
     bool ok = false;
     if (int rc = run_pass_inc(e, f, done, profile, &ok)) return rc;
-    if (ok) { e->inc_n_pods = e->sizes.n_pods; e->inc_n_heads = e->sizes.n_heads; return pass_done(e, done); }
+    if (ok) { e->inc_n_pods = e->sizes.n_pods; e->inc_n_heads = e->sizes.n_heads; e->inc_n_clusters = e->sizes.n_clusters; return pass_done(e, done); }
   }
   e->inc_valid = false; e->ran_inc = false;
   if (e->inc_zero_needed) {  // first pass on this layout: stamps, dirty flags and epoch counters start from zero
@@ -1371,6 +1416,9 @@ int begin_commit(kr_engine *e) {
   return KR_OK;
 }
 
+// KR_OPT_CLUSTER_CREATES has an effect (the tables are sized for the capacities)
+bool creates_on(const kr_engine *e) { return e->cluster_creates && e->fixed_layout; }
+
 // The column table of an object commit's diff: every object column i, staged at stage + at[i] with cnt[d] rows of its dimension d,
 // against the resident one as the record last left it.  Without row lists, staged row k is resident row k; with them (the row path)
 // it is the k-th row of the list of dimension d at stage + list_at[d], and a dimension without staged rows is left out.
@@ -1386,9 +1434,10 @@ ObjDiffArgs object_diff_args(const kr_engine *e, const uint8_t *stage, const siz
     oa.rowlist[k] = list_at ? reinterpret_cast<const uint32_t *>(stage + list_at[d]) : nullptr;
     oa.dst[k] = e->d_in + e->il.off[i];
     oa.first[k + 1] = oa.first[k] + cnt[d];
-    oa.rows_old[k] = d == D_HEADS ? e->rec.res_n_heads : (uint32_t)dn[d];
+    oa.rows_old[k] = d == D_HEADS ? e->rec.res_n_heads : d == D_CLUSTERS ? e->rec.res_clusters : d == D_GROUPS ? e->rec.res_groups : d == D_WTD ? e->rec.res_wtd : (uint32_t)dn[d];
     oa.row_bytes[k] = (uint16_t)(kCols[i].elem * kCols[i].mult);
     oa.cls[k] = obj_class(i, e->wtd_edits);
+    oa.cls_new[k] = obj_class(i, e->wtd_edits, creates_on(e));
     if (i == kGroupClusterCol) oa.g_cluster_idx_new = reinterpret_cast<const uint32_t *>(stage + at[i]);
     if (i == kHeadKeyCol) oa.h_pod_idx_new = reinterpret_cast<const uint32_t *>(stage + at[i]);
   }
@@ -1461,6 +1510,10 @@ int kr_engine_set_option(kr_engine *e, uint32_t option, uint64_t value) {
     e->spec_rows_opt = value != 0;
     return KR_OK;
   }
+  if (option == KR_OPT_CLUSTER_CREATES) {  // (read at each kr_snapshot_begin and object commit)
+    e->cluster_creates = value != 0;
+    return KR_OK;
+  }
   if (option == KR_OPT_LARGE_CLUSTERS || option == KR_OPT_WIDE_CLUSTERS || option == KR_OPT_HUGE_CLUSTERS) {
     bool &on = option == KR_OPT_LARGE_CLUSTERS ? e->large_on : option == KR_OPT_WIDE_CLUSTERS ? e->wide_on : e->huge_on;
     if (on == (value != 0)) return KR_OK;
@@ -1508,6 +1561,7 @@ int kr_engine_get_option(kr_engine *e, uint32_t option, uint64_t *value) {
     case KR_OPT_HUGE_CLUSTERS: *value = e->huge_on; return KR_OK;
     case KR_OPT_WTD_EDITS: *value = e->wtd_edits; return KR_OK;
     case KR_OPT_SPEC_ROWS: *value = e->spec_rows_opt; return KR_OK;
+    case KR_OPT_CLUSTER_CREATES: *value = e->cluster_creates; return KR_OK;
     case KR_OPT_BUCKET_STRIDE: *value = e->bstride; return KR_OK;
     default: return fail(e, KR_E_INVALID, "unknown option %u", option);
   }
@@ -1656,12 +1710,17 @@ int kr_snapshot_begin(kr_engine *e, const kr_sizes *sizes, kr_snapshot_bufs *out
     e->gvalid = false;
     // The resident state of the incremental path survives new live counts under a fixed layout as long as the object tables keep
     // their shape: pod rows appended (they arrive as committed rows), head-aux rows come and go, the JSON arena grows; with
-    // KR_OPT_WTD_EDITS workersToDelete lists grow and shrink as well (the name table is sized for the capacity).
-    const bool keep = e->inc_valid && e->fixed_layout && sizes->n_clusters == e->sizes.n_clusters && sizes->n_groups == e->sizes.n_groups &&
-                      (sizes->n_wtd == e->sizes.n_wtd || e->wtd_edits) && sizes->n_jobs == e->sizes.n_jobs && sizes->n_pods >= e->sizes.n_pods;
+    // KR_OPT_WTD_EDITS workersToDelete lists grow and shrink as well (the name table is sized for the capacity); with
+    // KR_OPT_CLUSTER_CREATES RayClusters are appended (with their groups and names: the object diff checks that every resident row
+    // stayed) while the bucket arena holds them at the current stride, and RayJobs come and go.
+    const bool grow = creates_on(e) && sizes->n_clusters >= e->sizes.n_clusters && sizes->n_groups >= e->sizes.n_groups && sizes->n_wtd >= e->sizes.n_wtd &&
+                      (size_t)sizes->n_clusters * e->bstride <= e->sl.bucket_entries;
+    const bool keep = e->inc_valid && e->fixed_layout && ((sizes->n_clusters == e->sizes.n_clusters && sizes->n_groups == e->sizes.n_groups) || grow) &&
+                      (sizes->n_wtd == e->sizes.n_wtd || e->wtd_edits || grow) && (sizes->n_jobs == e->sizes.n_jobs || creates_on(e)) &&
+                      sizes->n_pods >= e->sizes.n_pods;
     if (!e->fixed_layout) { e->committed_full = false; e->inc_zero_needed = true; }
     // (the next pass is a full one, which hashes every message: listed rows may not exist any more)
-    if (sizes->n_clusters != e->sizes.n_clusters) clear_spec_rows(e);
+    if (sizes->n_clusters != e->sizes.n_clusters && !keep) clear_spec_rows(e);
     if (!keep) {
       e->inc_valid = false;
       e->force_radix = e->env_radix;
@@ -1723,8 +1782,13 @@ int kr_snapshot_commit_parts(kr_engine *e, uint32_t parts) {
   const ObjDiffArgs oa = object_diff_args(e, e->d_obj_stage, at, cnt, nullptr);  // (before the record moves on)
   if (e->order_pending) { CK(cudaEventSynchronize(e->ev_order)); e->order_pending = false; }  // a previous upload may still be reading h_order
   if (int rc = begin_commit(e)) return rc;
-  const CommitRecord::Moved moved = e->rec.commit_whole(hb, n, parts, e->wtd_edits);
+  const CommitRecord::Moved moved = e->rec.commit_whole(hb, n, parts, e->wtd_edits, creates_on(e));
   if (moved.shape) e->gvalid = false;  // launch shape / pipeline depend on it
+  if (moved.appended < n.n_clusters) {  // KR_OPT_CLUSTER_CREATES: the next pass hashes the new RayClusters' specs (committed as spec rows)
+    if (e->spec_stamp.size() < n.n_clusters) e->spec_stamp.resize(n.n_clusters, 0u);
+    for (uint32_t c = moved.appended; c < n.n_clusters; c++)
+      if (e->spec_stamp[c] != e->spec_epoch) { e->spec_stamp[c] = e->spec_epoch; e->spec_pending.push_back(c); }
+  }
   if (moved.wide && e->wide_on) e->lg_stale = true;  // a different wide set is a different list, and grid, of the per-cluster kernels
   if (parts & KR_PART_COLUMNS) e->inc_valid = false;  // pod columns uploaded wholesale: the resident buckets no longer describe them
   if (moved.order) build_order(e, hb);  // (unchanged lengths and gates: the resident order stands — an object / pod epoch does not pay for it)
@@ -1901,7 +1965,7 @@ int kr_snapshot_commit_spec_rows(kr_engine *e, const uint32_t *rows, uint32_t n)
     ll[i] = hb.c_json_len[lr[i]]; lo[i] = hb.c_json_off[lr[i]];
     bytes += ((size_t)ll[i] + 15) & ~(size_t)15;
   }
-  e->rec.commit_spec_rows(lr, lo, ll, m, z.n_clusters);
+  e->rec.commit_spec_rows(lr, lo, ll, m);
   if (int rc = begin_commit(e)) return rc;
   uint32_t *dr = reinterpret_cast<uint32_t *>(e->spec.d) + base;
   uint32_t *dl = reinterpret_cast<uint32_t *>(e->spec.d + 4 * cap) + base;

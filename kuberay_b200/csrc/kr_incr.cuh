@@ -122,8 +122,10 @@ __global__ void __launch_bounds__(256) k_inc_wtd_insert(SnapDev s, ScratchDev sc
   for (uint32_t t = blockIdx.x * blockDim.x + threadIdx.x; t < n.n_groups; t += gridDim.x * blockDim.x) wt_insert_group(s, sc, t);
 }
 
-// grid-stride over the pod rows: 8 bytes per row and a Bloom test in shared memory (the bitmap copied per CTA, as k_match2 does)
-__global__ void __launch_bounds__(256) k_inc_wtd_resolve(SnapDev s, ScratchDev sc, ResDev r, Sizes n, uint32_t n_resident) {
+// grid-stride over the pod rows: 8 bytes per row and a Bloom test in shared memory (the bitmap copied per CTA, as k_match2 does).
+// Only names from entry `first_name` on are resolved, and only rows that hit one of them are touched (0: every name, the rebuild;
+// the first new name: the names of RayClusters an epoch appended, KR_OPT_CLUSTER_CREATES).
+__global__ void __launch_bounds__(256) k_inc_wtd_resolve(SnapDev s, ScratchDev sc, ResDev r, Sizes n, uint32_t n_resident, uint32_t first_name) {
   extern __shared__ uint32_t sm_bits[];
   const uint32_t words = (sc.wt_bits_mask + 1) >> 5;
   for (uint32_t i = threadIdx.x; i < words; i += blockDim.x) sm_bits[i] = __ldcg(&sc.wt_bits[i]);
@@ -138,9 +140,11 @@ __global__ void __launch_bounds__(256) k_inc_wtd_resolve(SnapDev s, ScratchDev s
     uint64_t kk = __ldcg(&sc.wt_keys[j]);
     while (kk != KR_EMPTY64) {
       if (kk == k) {
-        for (uint32_t e = __ldcg(&sc.wt_head[j]); e != KR_EMPTY32; e = __ldcg(&sc.wt_next[e])) atomicMin(&r.wtd_pod_idx[e], p);
+        bool hit = false;
+        for (uint32_t e = __ldcg(&sc.wt_head[j]); e != KR_EMPTY32; e = __ldcg(&sc.wt_next[e]))
+          if (e >= first_name) { atomicMin(&r.wtd_pod_idx[e], p); hit = true; }
         uint32_t ns2, nm2;
-        inc_touch(s, sc, r, p, epoch, n_resident, ns2, nm2);
+        if (hit) inc_touch(s, sc, r, p, epoch, n_resident, ns2, nm2);
         break;
       }
       j = (j + 1) & sc.wt_mask;
@@ -162,6 +166,7 @@ struct ObjDiffArgs {
   uint32_t rows_old[kMaxObjCols];    // rows the resident column held
   uint16_t row_bytes[kMaxObjCols];
   uint8_t cls[kMaxObjCols];
+  uint8_t cls_new[kMaxObjCols];      // class of a row at or past rows_old (KR_OPT_CLUSTER_CREATES: a row of an appended RayCluster)
   int n_cols;
   const uint32_t *g_cluster_idx_new;  // staged g_cluster_idx (group row -> RayCluster)
   const uint32_t *h_pod_idx_new;      // staged h_pod_idx
@@ -185,14 +190,16 @@ __global__ void __launch_bounds__(256) k_inc_objects(ObjDiffArgs a, SnapDev s, S
   const uint32_t row = a.rowlist[col] ? a.rowlist[col][k_st] : k_st;
   const uint8_t *src = a.src[col] + (size_t)k_st * rb;
   uint8_t *dst = a.dst[col] + (size_t)row * rb;
-  bool differ = row >= a.rows_old[col];
+  const bool past = row >= a.rows_old[col];
+  const uint8_t cls = past ? a.cls_new[col] : a.cls[col];
+  bool differ = past;
   if (!differ) {
     if ((rb & 3u) == 0) { for (uint32_t k = 0; k < rb; k += 4) differ |= *reinterpret_cast<const uint32_t *>(src + k) != *reinterpret_cast<const uint32_t *>(dst + k); }
     else for (uint32_t k = 0; k < rb; k++) differ |= src[k] != dst[k];
   }
   if (!differ) return;
   const uint32_t epoch = inc_epoch(sc);
-  switch (a.cls[col]) {
+  switch (cls) {
     case KR_OC_STRUCT: sc.inc[KR_INC_STRUCTURAL] = 1u; break;
     case KR_OC_CLUSTER: if (row < n.n_clusters) { sc.obj_flag[row] = epoch; mark_dirty(sc, row, epoch); } break;
     case KR_OC_GROUP: { const uint32_t c = a.g_cluster_idx_new[k_st]; if (c < n.n_clusters) { sc.obj_flag[c] = epoch; mark_dirty(sc, c, epoch); } break; }
@@ -203,7 +210,7 @@ __global__ void __launch_bounds__(256) k_inc_objects(ObjDiffArgs a, SnapDev s, S
       break;
     default: break;
   }
-  if (a.cls[col] == KR_OC_HEADKEY) return;  // (copied by k_inc_objects_keys once every head row has read the old key)
+  if (cls == KR_OC_HEADKEY) return;  // (copied by k_inc_objects_keys once every head row has read the old key)
   if ((rb & 3u) == 0) { for (uint32_t k = 0; k < rb; k += 4) *reinterpret_cast<uint32_t *>(dst + k) = *reinterpret_cast<const uint32_t *>(src + k); }
   else for (uint32_t k = 0; k < rb; k++) dst[k] = src[k];
 }
@@ -345,6 +352,80 @@ __global__ void __launch_bounds__(256) k_inc_admit(SnapDev s, ScratchDev sc, Res
     const uint32_t rank = atomicAdd(&sc.cl_dyn[c].x, 1u);
     if (uint4 *at = rec_slot(sc, c, rank)) { *at = make_uint4(p, (slot << 16) | flags | KR_ROW_FRESH, ri, nm); sc.pos[p] = rank; }
     else sc.inc[KR_INC_VOID] = 1u;  // (an ordinary RayCluster outgrew its bucket, a large one its region: the full pass reclassifies)
+  }
+}
+
+// ------------------------------------------------------------------------------------------------ RayCluster creation
+// KR_OPT_CLUSTER_CREATES: an epoch whose object commit appended RayClusters [c0, c1) after the last resident row (every resident
+// RayCluster, group and workersToDelete name kept its row; k_inc_objects copied the new rows into place and marked the new RayClusters
+// dirty) brings them into the resident state in front of k_inc_admit:
+//   k_inc_orphan_adopt     touches every resident Pod row labelled for one of them — an orphan until now, or a Pod of an older
+//                          RayCluster of the same key (the lowest row keeps such a key) — while the cluster table does not hold them
+//                          yet: inc_touch takes an orphan out of the orphan count, and k_inc_admit appends it to its new bucket.  The
+//                          host launches it only when the last pass counted orphans;
+//   k_inc_clusters_insert  inserts them into the cluster table (k_build_tables' per-cluster part) and initialises every per-cluster
+//                          cell a decide warp or k_decide_large reads: rows past the previous count may hold values of an earlier,
+//                          larger fleet.  With `names`, it also inserts their groups' workersToDelete names into the name table and
+//                          its Bloom bitmap (k_build_tables' group part) and sets their resolutions to -1;
+//   k_inc_wtd_resolve      (first_name = the first new name; only when there are new names) then probes every pod row once: a new
+//                          name may name any resident Pod.  It resolves the new names and touches the rows that hit one.  A row of
+//                          a new RayCluster was an orphan and k_inc_orphan_adopt touched it already; any other resident row still
+//                          probes to the RayCluster that holds it (the lowest row keeps a duplicate key).
+// (An epoch whose object commit also changed an existing list, KR_OPT_WTD_EDITS, rebuilds the whole name table instead: `names` = 0.)
+__global__ void __launch_bounds__(256) k_inc_clusters_insert(SnapDev s, ScratchDev sc, ResDev r, uint32_t c0, uint32_t c1, int names) {
+  const uint32_t c = c0 + blockIdx.x * blockDim.x + threadIdx.x;
+  if (c >= c1 || __ldcg(&sc.inc[KR_INC_STRUCTURAL])) return;
+  cl_insert_cluster(s, sc, c);
+  sc.cl_dyn[c] = make_uint4(0u, 0u, 0u, 0u);  // no pod yet (k_inc_admit appends them), no first head, not "lost a row"
+  sc.act_res[c] = 0u; sc.cre_res[c] = 0u;     // no reserved places: the decide takes new ones at the cursors
+  r.act_start[c] = 0u; r.act_cnt[c] = 0u;
+  if (sc.lg) sc.lg[c] = make_uint4(0u, 0u, 0u, 0u);  // no region (a RayCluster that outgrows its bucket voids the epoch)
+  const uint32_t g0 = s.c_group_off[c], G = s.c_group_cnt[c];
+  for (uint32_t g = g0; g < g0 + G; g++) {  // no pods asked for in the resident results
+    kr_group_result z; z.expected = 0; z.n_list = 0; z.n_unhealthy = 0; z.n_running = 0; z.diff = 0; z.n_create = 0; z.create_off = 0; z.flags = 0;
+    r.groups[g] = z;
+    sc.gcreate[g] = 0u;
+    if (names) {
+      for (uint32_t e = s.g_wtd_off[g]; e < s.g_wtd_off[g] + s.g_wtd_cnt[g]; e++) r.wtd_pod_idx[e] = 0xFFFFFFFFu;
+      wt_insert_group(s, sc, g);
+    }
+  }
+  mark_dirty(sc, c, inc_epoch(sc));
+}
+
+// Grid-stride over the resident pod rows, 8 bytes per row (namespace, ray.io/cluster), against a Bloom bitmap of the new RayClusters'
+// keys and, behind it, an open-addressed table of their rows (both built per CTA in shared memory: 4 * (slot_mask + 1) bytes of slots
+// after (bloom_mask + 1) / 8 bytes of bits).
+__global__ void __launch_bounds__(256) k_inc_orphan_adopt(SnapDev s, ScratchDev sc, ResDev r, uint32_t c0, uint32_t c1, uint32_t bloom_mask,
+                                                          uint32_t slot_mask, uint32_t n_resident) {
+  extern __shared__ uint32_t sm_adopt[];
+  uint32_t *bits = sm_adopt, *slots = sm_adopt + ((bloom_mask + 1) >> 5);
+  for (uint32_t i = threadIdx.x; i < (bloom_mask + 1) >> 5; i += blockDim.x) bits[i] = 0u;
+  for (uint32_t i = threadIdx.x; i <= slot_mask; i += blockDim.x) slots[i] = KR_EMPTY32;
+  __syncthreads();
+  for (uint32_t c = c0 + threadIdx.x; c < c1; c += blockDim.x) {
+    const uint32_t ns = s.c_ns_id[c], nm = s.c_name_id[c];
+    if (nm == 0) continue;  // (cl_probe matches no pod against an absent name)
+    const uint32_t hk = hash_pair(ns, nm), h2 = bloom2(hk);
+    atomicOr(&bits[(hk & bloom_mask) >> 5], 1u << (hk & 31));
+    atomicOr(&bits[(h2 & bloom_mask) >> 5], 1u << (h2 & 31));
+    uint32_t j = hk & slot_mask;
+    while (atomicCAS(&slots[j], KR_EMPTY32, c) != KR_EMPTY32) j = (j + 1) & slot_mask;
+  }
+  __syncthreads();
+  const uint32_t epoch = inc_epoch(sc);
+  for (uint32_t p = blockIdx.x * blockDim.x + threadIdx.x; p < n_resident; p += gridDim.x * blockDim.x) {
+    const uint32_t ns = __ldg(&s.p_ns_id[p]), cn = __ldg(&s.p_cluster_name_id[p]);
+    if (cn == 0) continue;
+    const uint32_t hk = hash_pair(ns, cn), h2 = bloom2(hk);
+    if (!(bits[(hk & bloom_mask) >> 5] & (1u << (hk & 31))) || !(bits[(h2 & bloom_mask) >> 5] & (1u << (h2 & 31)))) continue;
+    for (uint32_t j = hk & slot_mask, c; (c = slots[j]) != KR_EMPTY32; j = (j + 1) & slot_mask) {
+      if (s.c_ns_id[c] == ns && s.c_name_id[c] == cn) {
+        uint32_t ns2, nm2;
+        inc_touch(s, sc, r, p, epoch, n_resident, ns2, nm2);
+        break;
+      }
+    }
   }
 }
 

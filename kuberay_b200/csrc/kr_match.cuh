@@ -74,6 +74,27 @@ __device__ __forceinline__ void wt_insert_group(const SnapDev &s, const ScratchD
   }
 }
 
+// RayCluster t into the cluster table (namespace, name) -> {idx, flags, name of worker group 0}, and its cl_rec and cl_in records.
+// k_build_tables, and k_inc_clusters_insert for the RayClusters an incremental epoch appended.
+__device__ __forceinline__ void cl_insert_cluster(const SnapDev &s, const ScratchDev &sc, uint32_t t) {
+  uint32_t ns = s.c_ns_id[t], name = s.c_name_id[t];
+  uint32_t i = hash_pair(ns, name) & sc.cl_mask;
+  unsigned long long *slots = reinterpret_cast<unsigned long long *>(sc.cl_slots);  // [2*i] = key (x = name, y = ns), [2*i+1] = payload
+  const unsigned long long kk = ((unsigned long long)ns << 32) | name;
+  uint32_t g0 = s.c_group_off[t], G = s.c_group_cnt[t], mh = 0;
+  for (uint32_t gi = 0; gi < G; gi++) mh |= (s.g_num_hosts[g0 + gi] > 1) ? 1u : 0u;
+  const uint32_t gname0 = G ? s.g_name_id[g0] : 0u;
+  // payload = {z: name id of group 0, w: idx << 2 | flags} as one 64-bit word whose high half orders by cluster index
+  const unsigned long long payload = ((unsigned long long)((t << 2) | (G > 1 ? KR_CL_MULTI : 0u) | mh) << 32) | gname0;
+  while (true) {
+    unsigned long long prev = atomicCAS(&slots[2 * (size_t)i], KR_EMPTY64, kk);
+    if (prev == KR_EMPTY64 || prev == kk) { atomicMin(&slots[2 * (size_t)i + 1], payload); break; }  // duplicate (ns,name): lowest index wins, with its own payload
+    i = (i + 1) & sc.cl_mask;
+  }
+  sc.cl_rec[t] = make_uint4(g0, G, gname0, mh);  // .w bit 0: some worker group has numOfHosts > 1
+  write_cl_in(s, sc, t, g0, G);
+}
+
 // ------------------------------------------------------------------------------------------------ k_build_tables
 // One thread per cluster / workersToDelete entry / head-aux row.  Tables were memset to 0xFF.
 
@@ -89,22 +110,7 @@ __global__ void __launch_bounds__(256) k_build_tables(SnapDev s, ScratchDev sc, 
     sc.inc[KR_INC_EPOCH] += 1u;
   }
   if (t < n.n_clusters) {
-    uint32_t ns = s.c_ns_id[t], name = s.c_name_id[t];
-    uint32_t i = hash_pair(ns, name) & sc.cl_mask;
-    unsigned long long *slots = reinterpret_cast<unsigned long long *>(sc.cl_slots);  // [2*i] = key (x = name, y = ns), [2*i+1] = payload
-    const unsigned long long kk = ((unsigned long long)ns << 32) | name;
-    uint32_t g0 = s.c_group_off[t], G = s.c_group_cnt[t], mh = 0;
-    for (uint32_t gi = 0; gi < G; gi++) mh |= (s.g_num_hosts[g0 + gi] > 1) ? 1u : 0u;
-    const uint32_t gname0 = G ? s.g_name_id[g0] : 0u;
-    // payload = {z: name id of group 0, w: idx << 2 | flags} as one 64-bit word whose high half orders by cluster index
-    const unsigned long long payload = ((unsigned long long)((t << 2) | (G > 1 ? KR_CL_MULTI : 0u) | mh) << 32) | gname0;
-    while (true) {
-      unsigned long long prev = atomicCAS(&slots[2 * (size_t)i], KR_EMPTY64, kk);
-      if (prev == KR_EMPTY64 || prev == kk) { atomicMin(&slots[2 * (size_t)i + 1], payload); break; }  // duplicate (ns,name): lowest index wins, with its own payload
-      i = (i + 1) & sc.cl_mask;
-    }
-    sc.cl_rec[t] = make_uint4(g0, G, gname0, mh);  // .w bit 0: some worker group has numOfHosts > 1
-    write_cl_in(s, sc, t, g0, G);
+    cl_insert_cluster(s, sc, t);
     return;
   }
   t -= n.n_clusters;

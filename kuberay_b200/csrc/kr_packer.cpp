@@ -108,6 +108,7 @@ struct kr_packer {
   std::vector<uint32_t> json_rows;
   std::vector<uint8_t> json_flag;
   bool json_compacted = false, clusters_moved = false;
+  bool reshaped = false;              // a RayCluster the engine holds changed its group count or a workersToDelete list length
 
   uint32_t intern(const kr_str &s) {
     if (!s.p) return KR_ID_ABSENT;
@@ -348,6 +349,7 @@ int kr_packer_cluster_upsert(kr_packer *p, const kr_cluster_obj *o) {
     r.wtd.resize(g.n_workers_to_delete);
     for (uint32_t k = 0; k < g.n_workers_to_delete; k++) r.wtd[k] = p->intern(g.workers_to_delete[k]);
   }
+  if (shape && row < p->engine_sizes.n_clusters) p->reshaped = true;
   if (shape || p->tables_dirty) p->tables_dirty = true;
   else {  // same shape: the group rows are rewritten in place
     const uint32_t g0 = b.c_group_off[row];
@@ -452,10 +454,20 @@ int kr_packer_flush(kr_packer *p, uint32_t *mode_out) {
   kr_snapshot_bufs same;
   p->sizes = want;
   if (want.n_clusters != p->engine_sizes.n_clusters || want.n_groups != p->engine_sizes.n_groups || want.n_wtd != p->engine_sizes.n_wtd || want.n_jobs != p->engine_sizes.n_jobs) rows_ok = false;
+  // KR_OPT_CLUSTER_CREATES: RayClusters only appended after the engine's rows (none deleted, none it holds reshaped, the JSON arena
+  // not compacted) keep the incremental epoch: the object part, then the new RayClusters' specs as spec rows (no KR_PART_JSON on
+  // their account)
+  uint64_t creates_opt = 0;
+  kr_engine_get_option(p->e, KR_OPT_CLUSTER_CREATES, &creates_opt);
+  const uint32_t old_nc = p->engine_sizes.n_clusters;
+  const bool appends = creates_opt && !p->first && !p->clusters_moved && !p->reshaped && !p->json_compacted && want.n_clusters > old_nc;
   // Row-granular spec commit (KR_OPT_SPEC_ROWS): only the re-emitted blobs travel, while every other one stays where it was.
   uint64_t spec_opt = 0;
   kr_engine_get_option(p->e, KR_OPT_SPEC_ROWS, &spec_opt);
-  const bool spec_ok = spec_opt && p->json_dirty && !p->first && !p->json_compacted && !p->clusters_moved && want.n_clusters == p->engine_sizes.n_clusters;
+  const bool spec_ok = spec_opt && p->json_dirty && !p->first && !p->json_compacted && !p->clusters_moved && (want.n_clusters == old_nc || appends);
+  std::vector<uint32_t> new_rows, old_rows;  // blobs placed this flush: of appended RayClusters / of the others
+  for (uint32_t r : p->json_rows) (r >= old_nc ? new_rows : old_rows).push_back(r);
+  const bool json_rows_ok = spec_ok || (appends && old_rows.empty());  // every placed blob travels as a spec row
   if (memcmp(&want, &p->engine_sizes, sizeof want) != 0 || p->first) {
     if (int rc = kr_snapshot_begin(p->e, &p->sizes, &same)) return rc;  // fixed layout: new live counts, same addresses, resident data kept
     p->engine_sizes = want;
@@ -466,15 +478,19 @@ int kr_packer_flush(kr_packer *p, uint32_t *mode_out) {
     mode = KR_PACK_FULL;
   } else {
     if (trace) t2 = now();
-    if (spec_ok) {  // (before the object commit, which would otherwise see the moved ranges and re-hash every RayCluster)
-      if (int rc = kr_snapshot_commit_spec_rows(p->e, p->json_rows.data(), (uint32_t)p->json_rows.size())) return rc;
+    if (json_rows_ok && !old_rows.empty()) {  // (before the object commit, which would otherwise see the moved ranges and re-hash every RayCluster)
+      if (int rc = kr_snapshot_commit_spec_rows(p->e, old_rows.data(), (uint32_t)old_rows.size())) return rc;
       mode |= KR_PACK_SPEC_ROWS;
     }
-    uint32_t parts = ((p->objects_dirty && !rows_ok) ? KR_PART_OBJECTS : 0u) | ((p->json_dirty && !spec_ok) ? KR_PART_JSON : 0u);
+    uint32_t parts = ((p->objects_dirty && !rows_ok) ? KR_PART_OBJECTS : 0u) | ((p->json_dirty && !json_rows_ok) ? KR_PART_JSON : 0u);
     if (parts) { if (int rc = kr_snapshot_commit_parts(p->e, parts)) return rc; mode |= parts; }
     if (rows_ok) {
       if (int rc = kr_snapshot_commit_object_rows(p->e, p->dirty_cl.data(), (uint32_t)p->dirty_cl.size(), p->dirty_hd.data(), (uint32_t)p->dirty_hd.size())) return rc;
       mode |= KR_PACK_OBJECT_ROWS;
+    }
+    if (json_rows_ok && !new_rows.empty()) {  // the appended RayClusters' specs, once the object part has recorded them as new rows
+      if (int rc = kr_snapshot_commit_spec_rows(p->e, new_rows.data(), (uint32_t)new_rows.size())) return rc;
+      mode |= KR_PACK_SPEC_ROWS;
     }
     if (trace) t3 = now();
     if (!p->dirty_rows.empty()) {  // the epoch's journal, as the handlers wrote it
@@ -489,7 +505,7 @@ int kr_packer_flush(kr_packer *p, uint32_t *mode_out) {
   for (uint32_t r : p->dirty_hd) if (r < p->hd_flag.size()) p->hd_flag[r] = 0;
   p->dirty_cl.clear(); p->dirty_hd.clear(); p->wtd_changed = false;
   for (uint32_t r : p->json_rows) p->json_flag[r] = 0;
-  p->json_rows.clear(); p->json_compacted = p->clusters_moved = false;
+  p->json_rows.clear(); p->json_compacted = p->clusters_moved = p->reshaped = false;
   p->first = p->objects_dirty = p->tables_dirty = p->heads_dirty = p->jobs_dirty = p->json_dirty = false;
   p->epoch++;
   p->last_mode = mode;

@@ -234,7 +234,7 @@ class Engine:
     @classmethod
     def for_snapshot(cls, snap: Snapshot, device: int = 0, max_creates: int | None = None, slack: float = 1.0,
                      large_clusters: bool = False, wide_clusters: bool = False, huge_clusters: bool = False,
-                     wtd_edits: bool = False, spec_rows: bool = False) -> "Engine":
+                     wtd_edits: bool = False, spec_rows: bool = False, cluster_creates: bool = False) -> "Engine":
         d = snap.dims
         up = lambda x: int(x * slack) + 1  # noqa: E731
         if max_creates is None:
@@ -251,6 +251,8 @@ class Engine:
             eng.set_wtd_edits(True)
         if spec_rows:
             eng.set_spec_rows(True)
+        if cluster_creates:
+            eng.set_cluster_creates(True)
         return eng
 
     def _check(self, rc: int):
@@ -302,6 +304,12 @@ class Engine:
         """KR_OPT_SPEC_ROWS: the native packer (and LiveArena) commit re-emitted specs row by row (kr_snapshot_commit_spec_rows)
         instead of re-sending the whole JSON arena; commit_spec_rows itself works either way."""
         self._check(self._L.kr_engine_set_option(self._h, abi.OPT_SPEC_ROWS, 1 if on else 0))
+
+    def set_cluster_creates(self, on: bool = True):
+        """KR_OPT_CLUSTER_CREATES: under the fixed layout, keep incremental epochs when RayClusters are appended after the last row or
+        RayJobs are created or deleted (commit the object part, then the new RayClusters' specs with commit_spec_rows); read at each
+        begin and object commit."""
+        self._check(self._L.kr_engine_set_option(self._h, abi.OPT_CLUSTER_CREATES, 1 if on else 0))
 
     def get_option(self, option: int) -> int:
         """kr_engine_get_option: an option's current value, or the read-only OPT_BUCKET_STRIDE (0: the sort pipeline)."""

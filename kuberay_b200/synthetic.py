@@ -457,6 +457,32 @@ def widen_clusters(snap: Snapshot, clusters, n_groups: int) -> Snapshot:
     return out.validate()
 
 
+def first_clusters(snap: Snapshot, k: int, free_from: int | None = None, jobs=None, free_pods: bool = True) -> Snapshot:
+    """The snapshot before RayClusters k.. of `snap` were created: its first k RayClusters with their groups and workersToDelete names
+    (the rows a creation appends come after all of these), every pod row, head-aux row and the JSON arena.  With `free_pods` the Pods
+    labelled for the RayClusters from row `free_from` (default k) on are free rows (KR_PP_TOMBSTONE, every id 0); without it they
+    stay, as orphans.  `jobs`: the RayJob rows kept (default all)."""
+    d = snap.dims
+    g = int(snap.c_group_off[k]) if k < d["clusters"] else d["groups"]
+    w = int(snap.g_wtd_off[g]) if g < d["groups"] else d["wtd"]
+    jobs = np.arange(d["jobs"]) if jobs is None else np.asarray(jobs, dtype=np.int64)
+    out = Snapshot(k, g, w, d["pods"], d["heads"], jobs.size, d["json"])
+    rows = {"clusters": np.arange(k), "groups": np.arange(g), "wtd": np.arange(w), "jobs": jobs}
+    for name, _dt, mult, dim in abi.COLUMNS:
+        src = snap.cols[name]
+        out.cols[name][:] = (src.reshape(-1, mult)[rows[dim]].reshape(-1) if mult > 1 else src[rows[dim]]) if dim in rows else src
+    if free_pods:
+        f0 = k if free_from is None else free_from
+        ckey = (snap.c_ns_id[f0:].astype(np.uint64) << np.uint64(32)) | snap.c_name_id[f0:].astype(np.uint64)
+        pkey = (snap.p_ns_id.astype(np.uint64) << np.uint64(32)) | snap.p_cluster_name_id.astype(np.uint64)
+        gone = np.flatnonzero(np.isin(pkey, ckey) & (snap.p_cluster_name_id != 0))
+        for name, _dt, _m, dim in abi.COLUMNS:
+            if dim == "pods":
+                out.cols[name][gone] = 0
+        out.p_packed[gone] = np.uint32(abi.PP_TOMBSTONE)
+    return out.validate()
+
+
 def config(name: str, **overrides) -> SynthParams:
     d = dict(CONFIGS[name])
     d.update(overrides)

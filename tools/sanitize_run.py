@@ -74,6 +74,46 @@ def incremental(snap, flags, label, large=False, wide=False, huge=False):
         eng.close()
 
 
+def creations(snap, flags, label):
+    """KR_OPT_CLUSTER_CREATES (kr_incr.cuh): the last 20 RayClusters appended under a fixed layout, each time after a full pass over
+    the first ones — once with no resident orphan (k_inc_clusters_insert, and k_inc_wtd_resolve for their workersToDelete names), once
+    with their Pods resident as orphans (k_inc_orphan_adopt as well)."""
+    flags.fetch_pod_lists = 0
+    nc, k = snap.dims["clusters"], snap.dims["clusters"] - 20
+    # no Pod of the fleet is an orphan to begin with: the Pods no RayCluster of the fleet owns become free rows
+    ckey = (snap.c_ns_id.astype(np.uint64) << np.uint64(32)) | snap.c_name_id.astype(np.uint64)
+    pkey = (snap.p_ns_id.astype(np.uint64) << np.uint64(32)) | snap.p_cluster_name_id.astype(np.uint64)
+    lost = np.flatnonzero(~np.isin(pkey, ckey))
+    for c, _d, _m, dim in abi.COLUMNS:
+        if dim == "pods":
+            snap.cols[c][lost] = 0
+    snap.p_packed[lost] = np.uint32(abi.PP_TOMBSTONE)
+    inc = 0
+    for orphans in (False, True):
+        before = synthetic.first_clusters(snap, k, free_pods=not orphans)
+        eng = Engine.for_snapshot(snap, slack=1.2, cluster_creates=True)
+        eng.set_fixed_layout(True)
+        try:
+            views = eng.begin(before.sizes())
+            eng.fill(views, before)
+            eng.commit()
+            eng.reconcile(flags)
+            views = eng.begin(snap.sizes())
+            eng.fill(views, snap)
+            eng.commit(abi.PART_OBJECTS)
+            eng.commit_spec_rows(np.arange(k, nc, dtype=np.uint32))
+            moved = np.flatnonzero(np.any([before.cols[c] != snap.cols[c] for c, _d, _m, dim in abi.COLUMNS if dim == "pods"], axis=0))
+            if moved.size:
+                eng.commit_pod_rows(moved.astype(np.uint32))
+            prof = eng.reconcile_profiled(flags)
+            names = [n for n, _ in prof["kernels"]]
+            assert ("k_inc_orphan_adopt" in names) == orphans and "k_inc_clusters_insert" in names, names
+            inc += eng.fetch().changed_clusters is not None
+        finally:
+            eng.close()
+    print(label, "ok:", inc, "of 2 creation epochs incremental", flush=True)
+
+
 def wtd_edits(snap, flags, label):
     """KR_OPT_WTD_EDITS (kr_incr.cuh): workersToDelete renames, a list grown past the old n_wtd, then every list cleared — each epoch
     rebuilds the name table on the device (k_inc_wtd_release / _clear / _insert / _resolve)."""
@@ -144,6 +184,8 @@ def spec_rows(snap, flags, label):
 
 
 def main():
+    creations(*synthetic.generate(synthetic.config("C2", n_clusters=300, pods_per_cluster=20, groups=2, wtd_group_frac=0.3, recreate_frac=0.3)),
+              "RayCluster creations")
     spec_rows(*synthetic.generate(synthetic.config("C2", n_clusters=300, pods_per_cluster=20, groups=2, recreate_frac=0.3)), "spec rows")
     wtd_edits(*synthetic.generate(synthetic.config("C2", n_clusters=300, pods_per_cluster=20, groups=2, autoscaling_frac=1.0, wtd_group_frac=0.3)),
               "workersToDelete edits")
