@@ -540,8 +540,9 @@ int kr_last_profile(kr_engine *e, kr_profile *prof);
  *   same pointers, and what is resident in HBM stays valid across begins.  A head Pod appearing or going, or a Pod appended after
  *   the last row, is still an incremental epoch: kr_snapshot_begin(new counts) + KR_PART_OBJECTS + kr_snapshot_commit_pod_rows/
  *   _values.  So are workersToDelete lists that grow or shrink, with KR_OPT_WTD_EDITS, and RayClusters appended after the last row
- *   or RayJobs created or deleted, with KR_OPT_CLUSTER_CREATES.  Any other change of a row count (a RayCluster deleted, a worker
- *   group added to a RayCluster) makes the next pass a full one. */
+ *   or RayJobs created or deleted, with KR_OPT_CLUSTER_CREATES, and RayClusters deleted by swap-remove, with KR_OPT_CLUSTER_DELETES.
+ *   Any other change of a row count (a worker group added to a RayCluster, a deletion without that option) makes the next pass a
+ *   full one. */
 enum {
   KR_OPT_FIXED_LAYOUT = 1,
   KR_OPT_INCREMENTAL = 2,  /* 1 (default): passes after a full bucket-pipeline pass are incremental on the device whenever the commits in
@@ -581,7 +582,7 @@ enum {
   KR_OPT_SPEC_ROWS = 8,       /* 1: the native packer (kr_packer_flush) commits re-emitted specs with kr_snapshot_commit_spec_rows and
                               reports KR_PACK_SPEC_ROWS instead of KR_PART_JSON (a flush that compacts the JSON arena still sends
                               KR_PART_JSON).  The engine call itself needs no option.  Results are the same as with 0 (the default). */
-  KR_OPT_CLUSTER_CREATES = 9  /* 1, together with KR_OPT_FIXED_LAYOUT: RayClusters appended after the last row (every existing
+  KR_OPT_CLUSTER_CREATES = 9, /* 1, together with KR_OPT_FIXED_LAYOUT: RayClusters appended after the last row (every existing
                               RayCluster keeps its row, its groups and its workersToDelete names, and the new groups and names come after
                               all the old ones), and RayJobs created or deleted, keep the incremental epoch: kr_snapshot_begin(new
                               counts), the object part (KR_PART_OBJECTS), then the new RayClusters' specs with
@@ -593,7 +594,26 @@ enum {
                               full pass.  Results are the same as with 0 (the default: every such event makes the next pass a full
                               one).  May be set at any time; read at each kr_snapshot_begin and object commit.  No effect without
                               KR_OPT_FIXED_LAYOUT.  The native packer's flush takes this path by itself when the engine has the option
-                              and a flush only appended RayClusters or created and deleted RayJobs. */
+                              and a flush only appended RayClusters or created and deleted RayJobs.  Deleting a RayCluster is
+                              KR_OPT_CLUSTER_DELETES. */
+  KR_OPT_CLUSTER_DELETES = 10 /* 1, together with KR_OPT_FIXED_LAYOUT: RayClusters deleted by swap-remove keep the incremental epoch:
+                              kr_snapshot_begin(new counts), then the object part (KR_PART_OBJECTS), where every surviving RayCluster
+                              either keeps its row or moves from a row at or past the new n_clusters into a row a deleted RayCluster
+                              vacated, keeps its worker-group count, and groups and workersToDelete names stay in row order.  With
+                              KR_OPT_CLUSTER_CREATES the same epoch may also create RayClusters, in vacated rows or after the last one
+                              (their specs then follow with kr_snapshot_commit_spec_rows).  The next pass releases the deleted
+                              RayClusters' Pods (orphans from then on), brings every moved RayCluster's Pods to its new row, moves its
+                              digest when its spec range stayed, shifts the per-group results, and re-decides only the moved and created
+                              RayClusters, which it returns among changed_clusters.  Still full passes: another renumbering, a surviving
+                              RayCluster whose group count changed, a deleted or moved key that another row also holds, more than 4 096
+                              RayClusters deleted, moved or created at once, a deleted or moved RayCluster that is large
+                              (KR_OPT_LARGE_CLUSTERS: its region does not move), and, within one epoch, a renumbering after an object
+                              commit that appended RayClusters, or any object commit after a renumbering that changes a row count or
+                              renumbers again.  With KR_OPT_WIDE_CLUSTERS, RayClusters of more than 32 worker groups are followed too.
+                              Results are the same as with 0 (the default: every deletion makes the next pass a full one).  May be set
+                              at any time; read at each kr_snapshot_begin and object commit.  No effect without KR_OPT_FIXED_LAYOUT.
+                              The native packer's flush takes this path by itself when the engine has the option (the specs it placed
+                              travel as spec rows unless it compacted the JSON arena). */
 };
 enum { KR_LARGE_MAX_PODS = 8192 };  /* largest RayCluster KR_OPT_LARGE_CLUSTERS keeps on the bucket pipeline */
 int kr_engine_set_option(kr_engine *e, uint32_t option, uint64_t value);

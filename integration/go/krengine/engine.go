@@ -146,6 +146,10 @@ const (
 	// incremental epochs; only under KR_OPT_FIXED_LAYOUT; recommended for fleets that create RayClusters, such as RayJob and
 	// RayService fleets; read at each Begin and object commit).
 	OptClusterCreates = uint32(C.KR_OPT_CLUSTER_CREATES)
+	// OptClusterDeletes is KR_OPT_CLUSTER_DELETES (1: RayClusters deleted by swap-remove keep incremental epochs; only under
+	// KR_OPT_FIXED_LAYOUT; recommended for fleets that delete RayClusters, such as RayJob fleets with shutdownAfterJobFinishes;
+	// read at each Begin and object commit).
+	OptClusterDeletes = uint32(C.KR_OPT_CLUSTER_DELETES)
 )
 
 // SetOption: KR_OPT_FIXED_LAYOUT (before the first Begin), KR_OPT_INCREMENTAL, KR_OPT_LARGE_CLUSTERS (1: RayClusters of 257 to
@@ -156,7 +160,8 @@ const (
 // incremental epochs; recommended for autoscaling fleets; read at each object commit), KR_OPT_SPEC_ROWS (1: Packer.Flush commits
 // re-emitted specs with CommitSpecRows instead of the whole JSON arena and reports PackSpecRows), KR_OPT_CLUSTER_CREATES (1, with
 // KR_OPT_FIXED_LAYOUT: RayClusters appended after the last row and RayJobs created or deleted keep incremental epochs; read at each
-// Begin and object commit).  For a Packer, call it on Packer.Engine().
+// Begin and object commit), KR_OPT_CLUSTER_DELETES (1, with KR_OPT_FIXED_LAYOUT: RayClusters deleted by swap-remove keep incremental
+// epochs; read at each Begin and object commit).  For a Packer, call it on Packer.Engine().
 func (e *Engine) SetOption(option uint32, value uint64) error {
 	if rc := C.kr_engine_set_option(e.h, C.uint32_t(option), C.uint64_t(value)); rc != C.KR_OK {
 		return e.err(rc)

@@ -19,6 +19,8 @@
 #include <cstring>
 #include <string>
 #include <thread>
+#include <unordered_map>
+#include <unordered_set>
 #include <vector>
 
 #include "kr_kernels.cuh"
@@ -37,6 +39,9 @@ constexpr size_t kAlign = 256;
 // most RayClusters one incremental epoch appends while there are orphans (k_inc_orphan_adopt: 16 Bloom bits and two 4-byte table
 // slots per RayCluster in shared memory, 40 KB); more take the full pass
 constexpr uint32_t kAdoptMax = 4096;
+// most RayClusters one incremental epoch of KR_OPT_CLUSTER_DELETES deletes, moves and creates together; more take the full pass
+constexpr uint32_t kMapMax = 4096;
+enum MapList { MP_GONE, MP_INIT, MP_DIGESTS, MP_GSRC, MP_WSRC, MP_LISTS };  // the lists of a row map on the device, in this order
 inline size_t align_up(size_t x, size_t a = kAlign) { return (x + a - 1) / a * a; }
 inline uint32_t pow2_at_least(uint64_t x) { uint32_t p = 16; while (p < x) p <<= 1; return p; }
 // staging of an incremental pass's changed records, for up to a quarter of the RayClusters (beyond that the whole record arrays are
@@ -110,7 +115,8 @@ static_assert(kCols[kHeadKeyCol].dim == D_HEADS && kCols[kHeadKeyCol - 1].dim ==
 // g_wtd_off, g_wtd_cnt, w_name_id.  With KR_OPT_WTD_EDITS a staged object commit classifies them as copy / group / copy instead:
 // the next pass rebuilds the name table and recomputes KR_ROW_WTD_OWN (the only use of the offsets), and the multi-host decide
 // reads the count.
-constexpr int kWtdOffCol = 29, kWtdCntCol = 30, kWtdNameCol = 31;
+constexpr int kWtdOffCol = 29, kWtdCntCol = 30, kWtdNameCol = 31, kGroupOffCol = 7;
+static_assert(kCols[kGroupOffCol].dim == D_CLUSTERS && kCols[kGroupOffCol + 1].dim == D_CLUSTERS && kCols[kGroupOffCol + 2].elem == 8, "c_group_off column index");
 static_assert(kCols[kWtdCntCol].dim == D_GROUPS && kCols[kWtdNameCol].dim == D_WTD && kCols[kWtdNameCol + 1].dim == D_PODS, "workersToDelete column indices");
 // With KR_OPT_CLUSTER_CREATES a row past the resident rows of a RayCluster / group / workersToDelete column belongs to a RayCluster
 // the epoch appended (`appended`): it marks that RayCluster dirty and refreshes its input record (a group row: its RayCluster's) instead
@@ -132,8 +138,22 @@ struct CommitRecord {
     uint64_t json_off;             // the JSON range the digests and the hash order were computed from: whole, spec rows
     uint32_t json_len, group_off, group_cnt;  // (groups: whole)
     uint8_t recreate, mh;          // KR_CF_UPGRADE_RECREATE: whole with the object part; some worker group has numOfHosts > 1: whole, rows
+    uint32_t ns, name, wtd_off;    // key and first workersToDelete name: whole with the object part
   };
   std::vector<Row> rows;             // per RayCluster row (sized, zero-filled, by every whole commit)
+  // KR_OPT_CLUSTER_DELETES: how the last object commit renumbered the RayClusters (swap-remove), for the next pass
+  struct RowMap {
+    std::vector<uint32_t> gone;      // old rows no RayCluster keeps (deleted, or moved away), ascending
+    std::vector<uint32_t> init;      // new rows of a moved or created RayCluster, ascending
+    std::vector<uint32_t> created;   // ... those created (their specs are hashed)
+    std::vector<uint32_t> digests;   // (old row, new row) of the moved RayClusters whose spec range stayed: the digest moves
+    std::vector<uint32_t> moved_to;  // per gone row: its new row, or KR_EMPTY32 (deleted)
+    uint32_t gs0 = 0, ws0 = 0;       // groups / names from these on were shifted
+    std::vector<uint32_t> gsrc, wsrc;  // ... and came from these old ones (KR_EMPTY32: of a moved or created RayCluster)
+    uint32_t g_lo = 0, g_hi = 0;     // the old groups gsrc reads
+    bool names_moved = false;        // some workersToDelete name shifted, vanished or appeared
+  };
+  RowMap map;
   uint32_t n_recreate = 0;           // RayClusters with KR_CF_UPGRADE_RECREATE (decide phase 1 needed): whole
   uint64_t recreate_sig = 0;         // which ones (their messages lead the hash order): whole, when it rebuilds the order
   uint32_t n_mh = 0;                 // rows with a multi-host group: whole, rows
@@ -174,24 +194,101 @@ struct CommitRecord {
     return std::includes(given.begin(), given.end(), json_cols_behind.begin(), json_cols_behind.end());
   }
 
+  // KR_OPT_CLUSTER_DELETES: the row map of an object part that renumbered the recorded RayClusters (into `map`).  Only the rows whose
+  // key changed and the old rows at or past the new count are looked at.  -> 0: nothing was renumbered (appended rows are the
+  // creation path's), 1: a swap-remove map, -1: a renumbering the resident state does not follow (the next pass is a full one).
+  // `resident`: the RayCluster rows the device tables hold; `wide_ok`: KR_OPT_WIDE_CLUSTERS.
+  int derive_map(const kr_snapshot_bufs &hb, const kr_sizes &n, bool creates, bool wide_ok, uint32_t resident, uint32_t res_groups_old,
+                 uint32_t res_wtd_old) {
+    const uint32_t had = (uint32_t)rows.size(), nn = n.n_clusters, lo = std::min(had, nn);
+    auto key = [](uint32_t ns, uint32_t name) { return (uint64_t)ns << 32 | name; };
+    std::vector<uint32_t> old_ch, new_ch;
+    for (uint32_t c = 0; c < lo; c++)
+      if (rows[c].ns != hb.c_ns_id[c] || rows[c].name != hb.c_name_id[c]) old_ch.push_back(c), new_ch.push_back(c);
+    for (uint32_t c = nn; c < had; c++) old_ch.push_back(c);
+    if (old_ch.empty()) return 0;
+    if (had != resident) return -1;  // (an earlier object commit of this epoch appended rows the device tables do not hold yet)
+    for (uint32_t c = had; c < nn; c++) new_ch.push_back(c);
+    if (old_ch.size() > kMapMax || new_ch.size() > kMapMax) return -1;
+    // (a RayCluster of more than KR_SMEM_GROUPS worker groups is decided on the bucket pipeline only with KR_OPT_WIDE_CLUSTERS)
+    if (!wide_ok) {
+      for (uint32_t o : old_ch) if (rows[o].group_cnt > KR_SMEM_GROUPS) return -1;
+      for (uint32_t c : new_ch) if (hb.c_group_cnt[c] > KR_SMEM_GROUPS) return -1;
+    }
+    std::unordered_map<uint64_t, uint32_t> old_key;  // key of a gone row -> that row
+    for (uint32_t o : old_ch) if (!old_key.emplace(key(rows[o].ns, rows[o].name), o).second) return -1;
+    for (uint32_t c = 0; c < lo; c++)  // a kept row holding a gone row's key: the table's lowest-row rule would move it
+      if (rows[c].ns == hb.c_ns_id[c] && rows[c].name == hb.c_name_id[c] && old_key.count(key(rows[c].ns, rows[c].name))) return -1;
+    RowMap m;
+    m.gone = old_ch;
+    m.moved_to.assign(old_ch.size(), KR_EMPTY32);
+    std::unordered_set<uint64_t> new_keys;
+    for (uint32_t c : new_ch) {
+      const uint64_t k = key(hb.c_ns_id[c], hb.c_name_id[c]);
+      if (!new_keys.insert(k).second) return -1;
+      const auto it = old_key.find(k);
+      if (it != old_key.end() && it->second >= nn && rows[it->second].group_cnt == hb.c_group_cnt[c]) {  // moved by swap-remove
+        const uint32_t o = it->second;
+        m.moved_to[std::lower_bound(m.gone.begin(), m.gone.end(), o) - m.gone.begin()] = c;
+        if (rows[o].json_off == hb.c_json_off[c] && rows[o].json_len == hb.c_json_len[c]) { m.digests.push_back(o); m.digests.push_back(c); }
+        else m.created.push_back(c);  // (a moved RayCluster whose range moved as well is hashed like a created one)
+      } else if (creates) m.created.push_back(c);
+      else return -1;
+    }
+    if (old_ch.size() - m.digests.size() / 2 + new_ch.size() > kMapMax) return -1;  // deleted + moved + created
+    m.init = new_ch;
+    std::sort(m.created.begin(), m.created.end());
+    // groups and names from the first renumbered row on: a kept RayCluster's come from its old ones, the others' are new
+    const uint32_t c_min = new_ch.empty() ? nn : new_ch.front();
+    m.gs0 = c_min < nn ? hb.c_group_off[c_min] : n.n_groups;
+    m.ws0 = m.gs0 < n.n_groups ? hb.g_wtd_off[m.gs0] : n.n_wtd;
+    m.g_lo = res_groups_old; m.g_hi = 0;
+    for (uint32_t c = c_min; c < nn; c++) {
+      const bool fresh = std::binary_search(new_ch.begin(), new_ch.end(), c);
+      const uint32_t g0 = hb.c_group_off[c], G = hb.c_group_cnt[c];
+      for (uint32_t gi = 0; gi < G; gi++) {
+        const uint32_t og = fresh || gi >= rows[c].group_cnt ? KR_EMPTY32 : rows[c].group_off + gi;
+        const bool ok = og < res_groups_old;
+        m.gsrc.push_back(ok ? og : KR_EMPTY32);
+        if (ok) { m.g_lo = std::min(m.g_lo, og); m.g_hi = std::max(m.g_hi, og + 1); }
+        const uint32_t g = g0 + gi, w0 = hb.g_wtd_off[g];
+        for (uint32_t w = w0; w < w0 + hb.g_wtd_cnt[g]; w++) {
+          const uint32_t ow = ok ? rows[c].wtd_off + (w - hb.g_wtd_off[g0]) : KR_EMPTY32;
+          m.wsrc.push_back(ow < res_wtd_old ? ow : KR_EMPTY32);
+        }
+      }
+    }
+    if (m.g_hi < m.g_lo) m.g_lo = m.g_hi = 0;
+    m.names_moved = m.ws0 < n.n_wtd || n.n_wtd != res_wtd_old;
+    map = std::move(m);
+    return 1;
+  }
+
   // what a whole commit moved: the launch shape / pipeline, the wide set, the hash order; RayClusters from row `appended` on are new
-  // rows of KR_OPT_CLUSTER_CREATES (n_clusters: none), whose specs the caller commits as spec rows
-  struct Moved { bool shape, wide, order; uint32_t appended; };
-  Moved commit_whole(const kr_snapshot_bufs &hb, const kr_sizes &n, uint32_t parts, bool wtd_edits, bool creates) {
+  // rows of KR_OPT_CLUSTER_CREATES (n_clusters: none), whose specs the caller commits as spec rows; `map`: derive_map's verdict
+  struct Moved { bool shape, wide, order; uint32_t appended; int map; };
+  // (`deletes`, `wide_ok`, `resident`: KR_OPT_CLUSTER_DELETES, KR_OPT_WIDE_CLUSTERS, the RayCluster rows the device tables hold)
+  Moved commit_whole(const kr_snapshot_bufs &hb, const kr_sizes &n, uint32_t parts, bool wtd_edits, bool creates, bool deletes, bool wide_ok,
+                     uint32_t resident) {
     const bool objects = parts & (KR_PART_COLUMNS | KR_PART_OBJECTS);
     const size_t had = rows.size();
-    const bool appends = creates && objects && n.n_clusters > had;  // (not a moved range: only the new rows are hashed)
-    bool ranges_moved = had != n.n_clusters && !appends;  // some RayCluster's JSON range differs from the one the digests / the hash order were computed from
+    const int mapped = deletes && objects && had ? derive_map(hb, n, creates, wide_ok, resident, res_groups, res_wtd) : 0;
+    const bool appends = creates && objects && n.n_clusters > had && mapped == 0;  // (not a moved range: only the new rows are hashed)
+    bool ranges_moved = had != n.n_clusters && !appends && mapped != 1;  // some RayCluster's JSON range differs from the one the digests / the hash order were computed from
     uint32_t n_rc = 0, n_mh_now = 0, max_groups = 0;
     std::vector<uint32_t> wide;
     rows.resize(n.n_clusters);
+    uint32_t woff = 0;
     for (uint32_t c = 0; c < n.n_clusters; c++) {
       Row &r = rows[c];
-      const bool moved = c >= had ? !appends : r.json_off != hb.c_json_off[c] || r.json_len != hb.c_json_len[c];
+      const bool fresh = mapped == 1 && std::binary_search(map.init.begin(), map.init.end(), c);  // (derive_map compared its range)
+      const bool moved = fresh ? false : c >= had ? !appends : r.json_off != hb.c_json_off[c] || r.json_len != hb.c_json_len[c];
       if (moved && !objects) json_cols_behind.push_back(c);  // (the device's range columns keep the old range)
       ranges_moved |= moved;
       r.json_off = hb.c_json_off[c]; r.json_len = hb.c_json_len[c];
       r.group_off = hb.c_group_off[c]; r.group_cnt = hb.c_group_cnt[c];
+      if (objects) { r.ns = hb.c_ns_id[c]; r.name = hb.c_name_id[c]; r.wtd_off = woff; }
+      for (uint32_t g = r.group_off; g < r.group_off + r.group_cnt; g++) woff += hb.g_wtd_cnt[g];
       r.mh = 0;
       for (uint32_t g = r.group_off; g < r.group_off + r.group_cnt; g++) r.mh |= hb.g_num_hosts[g] > 1 ? 1 : 0;
       n_mh_now += r.mh;
@@ -211,7 +308,7 @@ struct CommitRecord {
     for (uint32_t c = 0; c < n.n_clusters; c++) if (hb.c_flags[c] & KR_CF_UPGRADE_RECREATE) rsig = (rsig ^ c) * 0x100000001B3ull;
     // (a spec-row commit updates the recorded ranges itself: its own flag says the order no longer follows them)
     bool order = ranges_moved || rsig != recreate_sig || spec_order_stale;
-    if (appends && !ranges_moved) { spec_order_stale = true; order = false; }  // (the order lacks the new rows: the next pass that hashes every message rebuilds it)
+    if ((appends || mapped == 1) && !ranges_moved) { spec_order_stale = true; order = false; }  // (the order lacks the new rows: the next pass that hashes every message rebuilds it)
     if (order) spec_order_stale = false;  // (the new order travels with this commit)
     recreate_sig = rsig;
     if ((parts & KR_PART_JSON) || ranges_moved) hash_dirty = true;
@@ -230,7 +327,7 @@ struct CommitRecord {
         prev_wtd.insert(prev_wtd.end(), hb.w_name_id, hb.w_name_id + n.n_wtd);
       }
     }
-    return {shape, wide_moved, order, appends ? (uint32_t)had : n.n_clusters};
+    return {shape, wide_moved, order, appends ? (uint32_t)had : n.n_clusters, mapped};
   }
   // -> the snapshot's first multi-host group came or its last went (a numOfHosts edit)
   bool commit_rows(const kr_snapshot_bufs &hb, const uint32_t *cl, uint32_t n_cl, const uint32_t *hd, uint32_t n_hd) {
@@ -435,6 +532,10 @@ struct kr_engine {
   Staging hb;                  // kr_hash_batch
   Staging pr;                  // incremental pod commits
   Staging orow;                // kr_snapshot_commit_object_rows
+  Staging mp;                  // KR_OPT_CLUSTER_DELETES: the row map of an object commit (rec.map), for its diff and the next pass
+  bool map_pending = false;    // ... uploaded and not yet applied by a pass
+  kr_sizes map_sizes{};        // ... the live counts of that object commit
+  size_t mp_at[5]{};           // offsets in mp of its lists (MapList)
   uint8_t *h_in_dev = nullptr;  // device-side address of h_in
   int sm_count = 148;
   // the whole pass (both streams) captured once per (layout, flags, n_recreate) and replayed
@@ -494,6 +595,7 @@ struct kr_engine {
   uint32_t inc_n_pods = 0, inc_n_heads = 0;  // rows resident at the last pass
   bool wtd_edits = false;        // KR_OPT_WTD_EDITS
   bool cluster_creates = false;  // KR_OPT_CLUSTER_CREATES
+  bool cluster_deletes = false;  // KR_OPT_CLUSTER_DELETES
   uint32_t inc_n_clusters = 0;   // RayClusters in the resident tables (those past it were appended since the last pass)
   uint32_t res_n_wtd = 0;        // names in the resident name table and its resolutions (wtd_pod_idx)
   bool ran_inc = false;          // the last pass was an incremental one
@@ -1079,7 +1181,7 @@ void after_full_pass(kr_engine *e, const kr_flags &f) {
   e->inc_valid = e->ran_bucket && !e->no_incr && e->h_totals[9] <= e->cfg.max_creates;
   e->inc_flags = f; e->inc_n_pods = e->sizes.n_pods; e->inc_n_heads = e->sizes.n_heads; e->inc_n_clusters = e->sizes.n_clusters;
   e->host_results_stale = false; e->inc_n_dirty = 0; e->fetched = false; e->ran_inc = false; e->rec.heads_rebuild = false;
-  e->rec.wtd_rebuild = false; e->res_n_wtd = e->sizes.n_wtd;
+  e->rec.wtd_rebuild = false; e->res_n_wtd = e->sizes.n_wtd; e->map_pending = false;
   if (!f.skip_hash) { e->rec.hash_dirty = false; clear_spec_rows(e); }
 }
 
@@ -1104,15 +1206,29 @@ int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile
   // n_clusters): their rows must have been committed, the bucket arena must hold them at this stride, a wide one needs
   // KR_OPT_WIDE_CLUSTERS, and the orphan scan's shared-memory table holds kAdoptMax of them
   const uint32_t c0 = e->inc_n_clusters, c1 = n.n_clusters;
-  const bool adopt = c1 > c0 && e->h_totals[1] != 0;  // (the last pass counted orphans: some of them may be the new RayClusters' Pods)
-  if (c1 != c0 && (c1 < c0 || e->rec.res_clusters != c1 || e->rec.res_groups != n.n_groups || (size_t)c1 * e->bstride > e->sl.bucket_entries ||
-                   (e->rec.snap_max_groups > KR_SMEM_GROUPS && !e->wide_on) || (adopt && c1 - c0 > kAdoptMax)))
+  // KR_OPT_CLUSTER_DELETES: an object commit renumbered the RayClusters (rec.map, uploaded to mp): its RayCluster rows must be the
+  // committed ones, and the orphan scan's table holds kAdoptMax created RayClusters
+  const bool mapped = e->map_pending;
+  const CommitRecord::RowMap &m = e->rec.map;
+  const bool adopt = (mapped ? !m.created.empty() : c1 > c0) && e->h_totals[1] != 0;  // (the last pass counted orphans: some of them may be the new RayClusters' Pods)
+  if (mapped && (e->rec.res_clusters != c1 || e->rec.res_groups != n.n_groups || e->map_sizes.n_clusters != c1 || e->map_sizes.n_groups != n.n_groups ||
+                 (size_t)c1 * e->bstride > e->sl.bucket_entries || (adopt && m.init.size() > kAdoptMax)))
+    return KR_OK;
+  if (!mapped && c1 != c0 && (c1 < c0 || e->rec.res_clusters != c1 || e->rec.res_groups != n.n_groups || (size_t)c1 * e->bstride > e->sl.bucket_entries ||
+                              (e->rec.snap_max_groups > KR_SMEM_GROUPS && !e->wide_on) || (adopt && c1 - c0 > kAdoptMax)))
     return KR_OK;
   PassCtx c(e, profile);
   const SnapDev &s = c.s; const ResDev &r = c.r; const ScratchDev &sc = c.sc; const Sizes &z = c.z;
   const cudaStream_t M = c.M, H = c.H;
   CK(cudaStreamWaitEvent(M, e->ev_cols, 0));
   const bool do_hash = e->rec.hash_dirty && !f.skip_hash && n.n_clusters > 0;
+  auto map_dev = [&](MapList i) { return reinterpret_cast<const uint32_t *>(e->mp.d + e->mp_at[i]); };
+  const uint32_t n_gone = mapped ? (uint32_t)m.gone.size() : 0, n_init = mapped ? (uint32_t)m.init.size() : 0;
+  if (mapped && !do_hash && !m.digests.empty()) {  // (ahead of the hash stream's fork: a re-hashed row's digest lands after it)
+    const uint32_t nd = (uint32_t)m.digests.size() / 2;
+    c.mark("k_inc_digest_move");
+    k_inc_digest_move<<<(2 * nd + 255) / 256, 256, 0, M>>>(map_dev(MP_DIGESTS), nd, r.hash);
+  }
   // ... or only the messages kr_snapshot_commit_spec_rows listed (a whole-arena commit wins; a skip_hash pass leaves them pending)
   const uint32_t n_rows = (!e->rec.hash_dirty && !f.skip_hash) ? (uint32_t)e->spec_pending.size() : 0;
   const uint32_t *spec_rows = n_rows ? upload_spec_order(e) : nullptr;
@@ -1130,6 +1246,10 @@ int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile
     if (e->rec.n_recreate && !do_hash) { c.mark("k_inc_mark_rows"); k_inc_mark_rows<<<(n_rows + 255) / 256, 256, 0, M>>>(s, sc, spec_rows, n_rows); }
   }
   const int grid = e->sm_count * 2;
+  if (mapped) {  // RayClusters renumbered (kr_incr.cuh): the gone rows' Pods touched while the table holds the old rows
+    c.mark("k_inc_clusters_release");
+    k_inc_clusters_release<<<(32 * n_gone + 255) / 256, 256, 0, M>>>(s, sc, r, map_dev(MP_GONE), n_gone, e->inc_n_pods);
+  }
   if (e->rec.heads_rebuild) {  // a head Pod came or went since the table was built (the commit compared the keys on the host)
     c.mark("k_inc_aux_rebuild");
     k_inc_aux_clear<<<std::min<uint32_t>(grid, (e->sl.aux_slots + 255) / 256), 256, 0, M>>>(sc);
@@ -1148,19 +1268,42 @@ int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile
     e->res_n_wtd = n.n_wtd;
     e->rec.wtd_rebuild = false;
   }
-  if (c1 > c0) {  // RayClusters appended (kr_incr.cuh): their orphans touched while the table does not hold them, then they enter it
-    if (adopt) {
-      uint32_t bloom_bits = 1024, slots = 64;
-      while (bloom_bits < 16 * (c1 - c0)) bloom_bits <<= 1;
-      while (slots < 2 * (c1 - c0)) slots <<= 1;
-      c.mark("k_inc_orphan_adopt");
-      k_inc_orphan_adopt<<<std::min<uint32_t>((uint32_t)e->sm_count * 4, (e->inc_n_pods + 255) / 256 + 1), 256, bloom_bits / 8 + 4 * (size_t)slots, M>>>(
-          s, sc, r, c0, c1, bloom_bits - 1, slots - 1, e->inc_n_pods);
+  // RayClusters appended or created (kr_incr.cuh): their orphans touched while the table does not hold them
+  const uint32_t *adopt_rows = mapped ? map_dev(MP_INIT) : nullptr;
+  const uint32_t a0 = mapped ? 0 : c0, a1 = mapped ? n_init : c1;
+  if (adopt) {
+    uint32_t bloom_bits = 1024, slots = 64;
+    while (bloom_bits < 16 * (a1 - a0)) bloom_bits <<= 1;
+    while (slots < 2 * (a1 - a0)) slots <<= 1;
+    c.mark("k_inc_orphan_adopt");
+    k_inc_orphan_adopt<<<std::min<uint32_t>((uint32_t)e->sm_count * 4, (e->inc_n_pods + 255) / 256 + 1), 256, bloom_bits / 8 + 4 * (size_t)slots, M>>>(
+        s, sc, r, adopt_rows, a0, a1, bloom_bits - 1, slots - 1, e->inc_n_pods);
+  }
+  if (mapped) {  // ... then the resident state in the new numbering, and the moved and created RayClusters enter it as new ones
+    c.mark("k_inc_clusters_translate");
+    k_inc_clusters_translate<<<1, 1024, 0, M>>>(sc, map_dev(MP_GONE), n_gone, n.n_clusters);
+    c.mark("k_inc_clusters_rekey");
+    CK(cudaMemsetAsync(sc.cl_slots, 0xFF, 16 * (size_t)e->sl.cl_slots, M));
+    k_inc_clusters_rekey<<<std::min<uint32_t>(grid, (n.n_clusters + 255) / 256 + 1), 256, 0, M>>>(s, sc, n.n_clusters);
+    if (m.gs0 < n.n_groups && m.g_hi > m.g_lo) {  // the old group records and create offsets the gather reads, staged first
+      const size_t ng = m.g_hi - m.g_lo;
+      kr_group_result *og = reinterpret_cast<kr_group_result *>(e->inc_stage.d);
+      uint32_t *oc = reinterpret_cast<uint32_t *>(e->inc_stage.d + sizeof(kr_group_result) * ng);
+      CK(cudaMemcpyAsync(og, r.groups + m.g_lo, sizeof(kr_group_result) * ng, cudaMemcpyDeviceToDevice, M));
+      CK(cudaMemcpyAsync(oc, sc.gcreate + m.g_lo, 4 * ng, cudaMemcpyDeviceToDevice, M));
+      c.mark("k_inc_groups_gather");
+      k_inc_groups_gather<<<std::min<uint32_t>(grid, (n.n_groups - m.gs0 + 255) / 256 + 1), 256, 0, M>>>(r, sc, map_dev(MP_GSRC), m.gs0, n.n_groups - m.gs0, og, oc, m.g_lo);
     }
+    if (n_init) {  // (their names, if any, came with the rebuilt name table)
+      c.mark("k_inc_clusters_insert");
+      k_inc_clusters_insert<<<(n_init + 255) / 256, 256, 0, M>>>(s, sc, r, map_dev(MP_INIT), 0u, n_init, 0);
+    }
+  }
+  if (!mapped && c1 > c0) {  // RayClusters appended: they enter the table
     // their workersToDelete names: inserted here and resolved against every pod row (unless the whole table was rebuilt above)
     const bool names = n.n_wtd > e->res_n_wtd;
     c.mark("k_inc_clusters_insert");
-    k_inc_clusters_insert<<<(c1 - c0 + 255) / 256, 256, 0, M>>>(s, sc, r, c0, c1, names ? 1 : 0);
+    k_inc_clusters_insert<<<(c1 - c0 + 255) / 256, 256, 0, M>>>(s, sc, r, nullptr, c0, c1, names ? 1 : 0);
     if (names) {
       c.mark("k_inc_wtd_resolve");
       k_inc_wtd_resolve<<<std::min<uint32_t>((uint32_t)e->sm_count * 4, (n.n_pods + 255) / 256 + 1), 256, e->sl.wt_bits_n / 8, M>>>(s, sc, r, z, e->inc_n_pods, e->res_n_wtd);
@@ -1216,6 +1359,17 @@ int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile
     e->spec_hashed.assign(h, h + n_rows);
   }
   if (do_hash || n_rows) clear_spec_rows(e);
+  if (mapped) {  // the host copy in the new numbering as well: moved digests, shifted group records (re-decided RayClusters come with the fetch)
+    ResDev hr = bind_out(e->ol, e->h_out);
+    if (!do_hash)
+      for (size_t i = 0; i < m.digests.size(); i += 2) memcpy(hr.hash + 32 * (size_t)m.digests[i + 1], hr.hash + 32 * (size_t)m.digests[i], 32);
+    if (m.gs0 < n.n_groups && m.g_hi > m.g_lo) {
+      const std::vector<kr_group_result> old(hr.groups + m.g_lo, hr.groups + m.g_hi);
+      for (uint32_t k = 0; k < n.n_groups - m.gs0; k++)
+        if (m.gsrc[k] != KR_EMPTY32) hr.groups[m.gs0 + k] = old[m.gsrc[k] - m.g_lo];
+    }
+    e->map_pending = false;
+  }
   e->ran_inc = true;
   *done_inc = true;
   return KR_OK;
@@ -1418,6 +1572,8 @@ int begin_commit(kr_engine *e) {
 
 // KR_OPT_CLUSTER_CREATES has an effect (the tables are sized for the capacities)
 bool creates_on(const kr_engine *e) { return e->cluster_creates && e->fixed_layout; }
+// KR_OPT_CLUSTER_DELETES has an effect
+bool deletes_on(const kr_engine *e) { return e->cluster_deletes && e->fixed_layout; }
 
 // The column table of an object commit's diff: every object column i, staged at stage + at[i] with cnt[d] rows of its dimension d,
 // against the resident one as the record last left it.  Without row lists, staged row k is resident row k; with them (the row path)
@@ -1437,13 +1593,71 @@ ObjDiffArgs object_diff_args(const kr_engine *e, const uint8_t *stage, const siz
     oa.rows_old[k] = d == D_HEADS ? e->rec.res_n_heads : d == D_CLUSTERS ? e->rec.res_clusters : d == D_GROUPS ? e->rec.res_groups : d == D_WTD ? e->rec.res_wtd : (uint32_t)dn[d];
     oa.row_bytes[k] = (uint16_t)(kCols[i].elem * kCols[i].mult);
     oa.cls[k] = obj_class(i, e->wtd_edits);
-    oa.cls_new[k] = obj_class(i, e->wtd_edits, creates_on(e));
+    oa.cls_new[k] = obj_class(i, e->wtd_edits, creates_on(e) || deletes_on(e));
     if (i == kGroupClusterCol) oa.g_cluster_idx_new = reinterpret_cast<const uint32_t *>(stage + at[i]);
     if (i == kHeadKeyCol) oa.h_pod_idx_new = reinterpret_cast<const uint32_t *>(stage + at[i]);
   }
   oa.h_pod_idx_old = reinterpret_cast<const uint32_t *>(e->d_in + e->il.off[kHeadKeyCol]);
   oa.n_heads_old = e->rec.res_n_heads;
   return oa;
+}
+
+// KR_OPT_CLUSTER_DELETES, an object commit whose part renumbered the RayClusters, or moved a row count after such a commit in the same
+// epoch (on the copy stream, before its diff): a row map the resident state follows (`ok`, rec.map) is checked against what the pass
+// can move, renumbers the pending spec rows, travels to the device and sets up the diff (oa).  Otherwise `voided`: the resident state
+// does not follow this epoch, and the caller drops it once the diff has copied the object part into place (the next pass is a full
+// one, which re-hashes every spec).
+int commit_map(kr_engine *e, bool ok, ObjDiffArgs &oa, bool &voided) {
+  const CommitRecord::RowMap &m = e->rec.map;
+  const kr_sizes &n = e->sizes;
+  // (a large RayCluster's region and tiles do not move with it; a second renumbering in one epoch would need the two maps composed;
+  // the old groups the gather reads are staged in the incremental staging buffer, which the pass fills only later)
+  ok = ok && !e->map_pending && 36 * (size_t)(m.g_hi - m.g_lo) <= e->inc_stage.cap;
+  for (uint32_t o : m.gone) ok = ok && !std::binary_search(e->large_rows.begin(), e->large_rows.end(), o);
+  if (!ok) {  // (the record took the new rows' ranges as the digests' ones)
+    e->rec.hash_dirty = true;
+    e->map_pending = false;
+    voided = true;
+    return KR_OK;
+  }
+  // the digests the next pass computes: the created RayClusters', and the pending spec rows in the new numbering
+  std::vector<uint32_t> pending;
+  for (uint32_t r : e->spec_pending) {
+    const auto it = std::lower_bound(m.gone.begin(), m.gone.end(), r);
+    if (it == m.gone.end() || *it != r) pending.push_back(r);
+    else if (m.moved_to[it - m.gone.begin()] != KR_EMPTY32) pending.push_back(m.moved_to[it - m.gone.begin()]);
+  }
+  pending.insert(pending.end(), m.created.begin(), m.created.end());
+  clear_spec_rows(e);
+  if (e->spec_stamp.size() < n.n_clusters) e->spec_stamp.resize(n.n_clusters, 0u);
+  for (uint32_t c : pending)
+    if (e->spec_stamp[c] != e->spec_epoch) { e->spec_stamp[c] = e->spec_epoch; e->spec_pending.push_back(c); }
+  const std::vector<uint32_t> *lists[MP_LISTS] = {&m.gone, &m.init, &m.digests, &m.gsrc, &m.wsrc};
+  size_t bytes = 0;
+  for (int i = 0; i < MP_LISTS; i++) { e->mp_at[i] = bytes; bytes += align_up(4 * lists[i]->size(), 16); }
+  CK(e->mp.wait());
+  CK(e->mp.reserve(bytes, bytes / 2 + 4096));  // (reserved at create for the largest map: no pinned allocation here)
+  for (int i = 0; i < MP_LISTS; i++) if (!lists[i]->empty()) memcpy(e->mp.h + e->mp_at[i], lists[i]->data(), 4 * lists[i]->size());
+  CK(cudaMemcpyAsync(e->mp.d, e->mp.h, bytes, cudaMemcpyHostToDevice, e->scopy));
+  CK(cudaEventRecord(e->mp.ev, e->scopy));
+  e->mp.busy = true;
+  e->h2d_accum += bytes;
+  auto dev = [&](MapList i) { return reinterpret_cast<const uint32_t *>(e->mp.d + e->mp_at[i]); };
+  oa.map_pass = 1;
+  oa.init = dev(MP_INIT); oa.n_init = (uint32_t)m.init.size();
+  oa.gsrc = dev(MP_GSRC); oa.wsrc = dev(MP_WSRC);
+  for (int k = 0, i = 0; i < kNumCols - 1; i++) {
+    const int d = kCols[i].dim;
+    if (d == D_PODS) continue;
+    oa.map_kind[k] = d == D_CLUSTERS ? KR_MAP_CLUSTER : d == D_GROUPS ? KR_MAP_GROUP : d == D_WTD ? KR_MAP_NAME : 0;
+    oa.shift_from[k] = d == D_GROUPS ? m.gs0 : d == D_WTD ? m.ws0 : 0u;
+    if (i == kGroupOffCol || i == kWtdOffCol) oa.cls[k] = KR_OC_COPY;  // (the offsets follow from the counts: groups and names stay in row order)
+    k++;
+  }
+  if (m.names_moved) e->rec.wtd_rebuild = true;
+  e->map_pending = true;
+  e->map_sizes = n;
+  return KR_OK;
 }
 
 // The on-device diff of an object commit (kr_incr.cuh), on the copy stream: the staged rows of oa's columns against the resident
@@ -1456,6 +1670,11 @@ int launch_object_diff(kr_engine *e, const ObjDiffArgs &oa, uint32_t n_hd, const
   ScratchDev scd = bind_scratch(e->sl, e->d_scratch);
   const uint32_t rows = oa.first[oa.n_cols];
   if (rows) k_inc_objects<<<(rows + 255) / 256, 256, 0, e->scopy>>>(oa, sd, scd, sizes_of(e->sizes));
+  if (rows && oa.map_pass) {  // (a row map: the shifted rows were diffed by the launch above, this one copies them and diffs the rest)
+    ObjDiffArgs copy = oa;
+    copy.map_pass = 2;
+    k_inc_objects<<<(rows + 255) / 256, 256, 0, e->scopy>>>(copy, sd, scd, sizes_of(e->sizes));
+  }
   if (n_hd) k_inc_objects_keys<<<(n_hd + 255) / 256, 256, 0, e->scopy>>>(oa.h_pod_idx_new, const_cast<uint32_t *>(sd.h_pod_idx), n_hd, head_rows);
   if (refresh) k_inc_refresh<<<std::min<uint32_t>((uint32_t)e->sm_count * 2, (e->sizes.n_clusters + 255) / 256 + 1), 256, 0, e->scopy>>>(sd, scd);
   CK(cudaGetLastError());
@@ -1514,6 +1733,10 @@ int kr_engine_set_option(kr_engine *e, uint32_t option, uint64_t value) {
     e->cluster_creates = value != 0;
     return KR_OK;
   }
+  if (option == KR_OPT_CLUSTER_DELETES) {  // (read at each kr_snapshot_begin and object commit)
+    e->cluster_deletes = value != 0;
+    return KR_OK;
+  }
   if (option == KR_OPT_LARGE_CLUSTERS || option == KR_OPT_WIDE_CLUSTERS || option == KR_OPT_HUGE_CLUSTERS) {
     bool &on = option == KR_OPT_LARGE_CLUSTERS ? e->large_on : option == KR_OPT_WIDE_CLUSTERS ? e->wide_on : e->huge_on;
     if (on == (value != 0)) return KR_OK;
@@ -1562,6 +1785,7 @@ int kr_engine_get_option(kr_engine *e, uint32_t option, uint64_t *value) {
     case KR_OPT_WTD_EDITS: *value = e->wtd_edits; return KR_OK;
     case KR_OPT_SPEC_ROWS: *value = e->spec_rows_opt; return KR_OK;
     case KR_OPT_CLUSTER_CREATES: *value = e->cluster_creates; return KR_OK;
+    case KR_OPT_CLUSTER_DELETES: *value = e->cluster_deletes; return KR_OK;
     case KR_OPT_BUCKET_STRIDE: *value = e->bstride; return KR_OK;
     default: return fail(e, KR_E_INVALID, "unknown option %u", option);
   }
@@ -1598,7 +1822,7 @@ int kr_engine_create(const kr_config *cfg, kr_engine **out) {
   if (cudaStreamCreateWithPriority(&e->sg, cudaStreamNonBlocking, prio_greatest) != cudaSuccess) return bail(KR_E_CUDA);
   if (cudaStreamCreateWithFlags(&e->scopy, cudaStreamNonBlocking) != cudaSuccess) return bail(KR_E_CUDA);
   cudaEventCreate(&e->ev_h2d0); cudaEventCreate(&e->ev_h2d1); cudaEventCreate(&e->ev_cols); cudaEventCreate(&e->ev_json);
-  for (cudaEvent_t *ev : {&e->pr.ev, &e->orow.ev, &e->ev_inc, &e->ev_order, &e->ev_fork2, &e->ev_join2, &e->ev_fork3, &e->ev_join3, &e->ev_fork, &e->ev_hash})
+  for (cudaEvent_t *ev : {&e->pr.ev, &e->orow.ev, &e->mp.ev, &e->ev_inc, &e->ev_order, &e->ev_fork2, &e->ev_join2, &e->ev_fork3, &e->ev_join3, &e->ev_fork, &e->ev_hash})
     cudaEventCreateWithFlags(ev, cudaEventDisableTiming);
   cudaEventCreate(&e->ev_a); cudaEventCreate(&e->ev_b); cudaEventCreate(&e->ev_c);
   for (auto &ev : e->ev_k) cudaEventCreate(&ev);
@@ -1653,6 +1877,8 @@ int kr_engine_create(const kr_config *cfg, kr_engine **out) {
     if (cudaMalloc((void **)&e->d_obj_stage, objs) != cudaSuccess) return bail(KR_E_CUDA);
     e->obj_stage_cap = objs;
     if (e->inc_stage.reserve(inc_stage_layout(cfg->max_clusters, cfg->max_groups).total, 0) != cudaSuccess) return bail(KR_E_CUDA);
+    // the largest row map of KR_OPT_CLUSTER_DELETES: gone / init / digests of kMapMax rows, every group and name shifted
+    if (e->mp.reserve(4 * (4 * (size_t)kMapMax + cfg->max_groups + cfg->max_wtd) + MP_LISTS * 16, 0) != cudaSuccess) return bail(KR_E_CUDA);
     const size_t chg = std::max<size_t>(1024, (size_t)cfg->max_clusters);
     if (cudaHostAlloc((void **)&e->h_changed, 4 * chg, cudaHostAllocDefault) != cudaSuccess) return bail(KR_E_CUDA);
     e->h_changed_cap = chg;
@@ -1672,7 +1898,7 @@ void kr_engine_destroy(kr_engine *e) {
   if (e->sh) cudaStreamSynchronize(e->sh);
   if (e->h_in) cudaFreeHost(e->h_in);
   if (e->h_out) cudaFreeHost(e->h_out);
-  e->hb.release(); e->pr.release(); e->orow.release(); e->inc_stage.release(); e->spec.release();
+  e->hb.release(); e->pr.release(); e->orow.release(); e->mp.release(); e->inc_stage.release(); e->spec.release();
   if (e->h_totals) cudaFreeHost(e->h_totals);
   if (e->h_order) cudaFreeHost(e->h_order);
   if (e->h_inc) cudaFreeHost(e->h_inc);
@@ -1715,8 +1941,14 @@ int kr_snapshot_begin(kr_engine *e, const kr_sizes *sizes, kr_snapshot_bufs *out
     // stayed) while the bucket arena holds them at the current stride, and RayJobs come and go.
     const bool grow = creates_on(e) && sizes->n_clusters >= e->sizes.n_clusters && sizes->n_groups >= e->sizes.n_groups && sizes->n_wtd >= e->sizes.n_wtd &&
                       (size_t)sizes->n_clusters * e->bstride <= e->sl.bucket_entries;
-    const bool keep = e->inc_valid && e->fixed_layout && ((sizes->n_clusters == e->sizes.n_clusters && sizes->n_groups == e->sizes.n_groups) || grow) &&
-                      (sizes->n_wtd == e->sizes.n_wtd || e->wtd_edits || grow) && (sizes->n_jobs == e->sizes.n_jobs || creates_on(e)) &&
+    // With KR_OPT_CLUSTER_DELETES the three counts may also shrink (RayClusters deleted by swap-remove: the object commit's row map
+    // checks the rest), and with both options each may move either way.
+    const bool fits = (size_t)sizes->n_clusters * e->bstride <= e->sl.bucket_entries;
+    auto moves_ok = [&](uint32_t now, uint32_t was) { return now == was || (now < was ? deletes_on(e) : creates_on(e) && fits); };
+    const bool renumber = deletes_on(e) && moves_ok(sizes->n_clusters, e->sizes.n_clusters) && moves_ok(sizes->n_groups, e->sizes.n_groups) &&
+                          moves_ok(sizes->n_wtd, e->sizes.n_wtd);
+    const bool keep = e->inc_valid && e->fixed_layout && ((sizes->n_clusters == e->sizes.n_clusters && sizes->n_groups == e->sizes.n_groups) || grow || renumber) &&
+                      (sizes->n_wtd == e->sizes.n_wtd || e->wtd_edits || grow || renumber) && (sizes->n_jobs == e->sizes.n_jobs || creates_on(e)) &&
                       sizes->n_pods >= e->sizes.n_pods;
     if (!e->fixed_layout) { e->committed_full = false; e->inc_zero_needed = true; }
     // (the next pass is a full one, which hashes every message: listed rows may not exist any more)
@@ -1779,11 +2011,20 @@ int kr_snapshot_commit_parts(kr_engine *e, uint32_t parts) {
   size_t at[kNumCols];
   for (int i = 0; i < kNumCols; i++) at[i] = stage_of(e->il.off[i]);
   const uint32_t cnt[7] = {n.n_clusters, n.n_groups, n.n_wtd, n.n_pods, n.n_heads, n.n_jobs, 0};
-  const ObjDiffArgs oa = object_diff_args(e, e->d_obj_stage, at, cnt, nullptr);  // (before the record moves on)
+  ObjDiffArgs oa = object_diff_args(e, e->d_obj_stage, at, cnt, nullptr);  // (before the record moves on)
   if (e->order_pending) { CK(cudaEventSynchronize(e->ev_order)); e->order_pending = false; }  // a previous upload may still be reading h_order
   if (int rc = begin_commit(e)) return rc;
-  const CommitRecord::Moved moved = e->rec.commit_whole(hb, n, parts, e->wtd_edits, creates_on(e));
+  const bool had_map = e->map_pending;
+  const CommitRecord::Moved moved = e->rec.commit_whole(hb, n, parts, e->wtd_edits, creates_on(e), deletes_on(e), e->wide_on, e->inc_n_clusters);
   if (moved.shape) e->gvalid = false;  // launch shape / pipeline depend on it
+  // KR_OPT_CLUSTER_DELETES: the object part renumbered the RayClusters, or moved a row count after a renumbering of this epoch (the
+  // pending map would no longer describe the rows: not composed)
+  bool voided = false;
+  const bool recounted = had_map && (parts & KR_PART_OBJECTS) &&
+                         (n.n_clusters != e->map_sizes.n_clusters || n.n_groups != e->map_sizes.n_groups || n.n_wtd != e->map_sizes.n_wtd);
+  if (moved.map != 0 || recounted) {
+    if (int rc = commit_map(e, moved.map == 1 && stage_objects, oa, voided)) return rc;
+  }
   if (moved.appended < n.n_clusters) {  // KR_OPT_CLUSTER_CREATES: the next pass hashes the new RayClusters' specs (committed as spec rows)
     if (e->spec_stamp.size() < n.n_clusters) e->spec_stamp.resize(n.n_clusters, 0u);
     for (uint32_t c = moved.appended; c < n.n_clusters; c++)
@@ -1814,6 +2055,7 @@ int kr_snapshot_commit_parts(kr_engine *e, uint32_t parts) {
         if (int rc = up(e->il.off[kFirstPodCol + k], 4 * (size_t)n.n_pods)) return rc;
   }
   if (stage_objects) { if (int rc = launch_object_diff(e, oa, n.n_heads, nullptr, n.n_clusters != 0)) return rc; }
+  if (voided) e->inc_valid = false;  // (the diff above copied the object part into place: the full pass reads it)
   CK(cudaEventRecord(e->ev_cols, e->scopy));
   if (moved.order && n.n_clusters) {  // the new order travels with this commit
     CK(cudaMemcpyAsync(e->d_order, e->h_order, 4 * (size_t)n.n_clusters, cudaMemcpyHostToDevice, e->scopy)); bytes += 4 * (size_t)n.n_clusters;

@@ -156,6 +156,14 @@ __global__ void __launch_bounds__(256) k_inc_wtd_resolve(SnapDev s, ScratchDev s
 // ------------------------------------------------------------------------------------------------ k_inc_objects
 // Diff of a KR_PART_OBJECTS upload (staged beside the resident tables) against the resident copy, then the copy into place.
 enum { KR_OC_COPY = 0, KR_OC_STRUCT = 1, KR_OC_CLUSTER = 2, KR_OC_GROUP = 3, KR_OC_HEAD = 4, KR_OC_HEADKEY = 5 };
+enum { KR_MAP_CLUSTER = 1, KR_MAP_GROUP = 2, KR_MAP_NAME = 3 };
+
+// x among the n ascending values of v
+__device__ __forceinline__ bool sorted_has(const uint32_t *v, uint32_t n, uint32_t x) {
+  uint32_t lo = 0, hi = n;
+  while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (__ldg(&v[mid]) < x) lo = mid + 1; else hi = mid; }
+  return lo < n && __ldg(&v[lo]) == x;
+}
 static constexpr int kMaxObjCols = 48;
 struct ObjDiffArgs {
   const uint8_t *src[kMaxObjCols];   // staged (new) column
@@ -167,6 +175,16 @@ struct ObjDiffArgs {
   uint16_t row_bytes[kMaxObjCols];
   uint8_t cls[kMaxObjCols];
   uint8_t cls_new[kMaxObjCols];      // class of a row at or past rows_old (KR_OPT_CLUSTER_CREATES: a row of an appended RayCluster)
+  // KR_OPT_CLUSTER_DELETES, an object commit that renumbered RayClusters (a row map): per column 0, or KR_MAP_CLUSTER (the rows of
+  // init are new RayCluster rows, classed like rows past rows_old), KR_MAP_GROUP / KR_MAP_NAME (rows from shift_from on were
+  // shifted: row k compares against the resident row src[k - shift_from], KR_EMPTY32: a row of a moved or created RayCluster, classed
+  // like a row past rows_old).  A map commit launches the diff twice, because a shifted row reads a resident row another thread
+  // overwrites: map_pass 1 diffs only the shifted rows and copies nothing, map_pass 2 copies them without a diff and diffs the rest.
+  uint8_t map_kind[kMaxObjCols];
+  uint32_t shift_from[kMaxObjCols];
+  const uint32_t *init; uint32_t n_init;
+  const uint32_t *gsrc, *wsrc;
+  int map_pass;
   int n_cols;
   const uint32_t *g_cluster_idx_new;  // staged g_cluster_idx (group row -> RayCluster)
   const uint32_t *h_pod_idx_new;      // staged h_pod_idx
@@ -190,12 +208,24 @@ __global__ void __launch_bounds__(256) k_inc_objects(ObjDiffArgs a, SnapDev s, S
   const uint32_t row = a.rowlist[col] ? a.rowlist[col][k_st] : k_st;
   const uint8_t *src = a.src[col] + (size_t)k_st * rb;
   uint8_t *dst = a.dst[col] + (size_t)row * rb;
-  const bool past = row >= a.rows_old[col];
+  const uint8_t *old = dst;  // the resident row this one is diffed against
+  bool past = row >= a.rows_old[col];
+  if (a.map_pass) {
+    const uint8_t mk = a.map_kind[col];
+    const bool shifted = mk >= KR_MAP_GROUP && row >= a.shift_from[col];
+    if (shifted && a.map_pass == 2) { for (uint32_t k = 0; k < rb; k++) dst[k] = src[k]; return; }  // (diffed by the first launch)
+    if (!shifted && a.map_pass == 1) return;
+    if (shifted) {
+      const uint32_t o = (mk == KR_MAP_GROUP ? a.gsrc : a.wsrc)[row - a.shift_from[col]];
+      if (o == KR_EMPTY32) past = true;
+      else old = a.dst[col] + (size_t)o * rb;
+    } else if (mk == KR_MAP_CLUSTER && !past) past = sorted_has(a.init, a.n_init, row);
+  }
   const uint8_t cls = past ? a.cls_new[col] : a.cls[col];
   bool differ = past;
   if (!differ) {
-    if ((rb & 3u) == 0) { for (uint32_t k = 0; k < rb; k += 4) differ |= *reinterpret_cast<const uint32_t *>(src + k) != *reinterpret_cast<const uint32_t *>(dst + k); }
-    else for (uint32_t k = 0; k < rb; k++) differ |= src[k] != dst[k];
+    if ((rb & 3u) == 0) { for (uint32_t k = 0; k < rb; k += 4) differ |= *reinterpret_cast<const uint32_t *>(src + k) != *reinterpret_cast<const uint32_t *>(old + k); }
+    else for (uint32_t k = 0; k < rb; k++) differ |= src[k] != old[k];
   }
   if (!differ) return;
   const uint32_t epoch = inc_epoch(sc);
@@ -210,7 +240,7 @@ __global__ void __launch_bounds__(256) k_inc_objects(ObjDiffArgs a, SnapDev s, S
       break;
     default: break;
   }
-  if (cls == KR_OC_HEADKEY) return;  // (copied by k_inc_objects_keys once every head row has read the old key)
+  if (cls == KR_OC_HEADKEY || a.map_pass == 1) return;  // (copied by k_inc_objects_keys once every head row has read the old key)
   if ((rb & 3u) == 0) { for (uint32_t k = 0; k < rb; k += 4) *reinterpret_cast<uint32_t *>(dst + k) = *reinterpret_cast<const uint32_t *>(src + k); }
   else for (uint32_t k = 0; k < rb; k++) dst[k] = src[k];
 }
@@ -372,9 +402,11 @@ __global__ void __launch_bounds__(256) k_inc_admit(SnapDev s, ScratchDev sc, Res
 //                          a new RayCluster was an orphan and k_inc_orphan_adopt touched it already; any other resident row still
 //                          probes to the RayCluster that holds it (the lowest row keeps a duplicate key).
 // (An epoch whose object commit also changed an existing list, KR_OPT_WTD_EDITS, rebuilds the whole name table instead: `names` = 0.)
-__global__ void __launch_bounds__(256) k_inc_clusters_insert(SnapDev s, ScratchDev sc, ResDev r, uint32_t c0, uint32_t c1, int names) {
-  const uint32_t c = c0 + blockIdx.x * blockDim.x + threadIdx.x;
-  if (c >= c1 || __ldcg(&sc.inc[KR_INC_STRUCTURAL])) return;
+// Both take the RayClusters as entries [c0, c1) of the ascending row list `rows` (nullptr: rows c0 .. c1 - 1).
+__global__ void __launch_bounds__(256) k_inc_clusters_insert(SnapDev s, ScratchDev sc, ResDev r, const uint32_t *rows, uint32_t c0, uint32_t c1, int names) {
+  const uint32_t i = c0 + blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= c1 || __ldcg(&sc.inc[KR_INC_STRUCTURAL])) return;
+  const uint32_t c = rows ? rows[i] : i;
   cl_insert_cluster(s, sc, c);
   sc.cl_dyn[c] = make_uint4(0u, 0u, 0u, 0u);  // no pod yet (k_inc_admit appends them), no first head, not "lost a row"
   sc.act_res[c] = 0u; sc.cre_res[c] = 0u;     // no reserved places: the decide takes new ones at the cursors
@@ -396,14 +428,15 @@ __global__ void __launch_bounds__(256) k_inc_clusters_insert(SnapDev s, ScratchD
 // Grid-stride over the resident pod rows, 8 bytes per row (namespace, ray.io/cluster), against a Bloom bitmap of the new RayClusters'
 // keys and, behind it, an open-addressed table of their rows (both built per CTA in shared memory: 4 * (slot_mask + 1) bytes of slots
 // after (bloom_mask + 1) / 8 bytes of bits).
-__global__ void __launch_bounds__(256) k_inc_orphan_adopt(SnapDev s, ScratchDev sc, ResDev r, uint32_t c0, uint32_t c1, uint32_t bloom_mask,
-                                                          uint32_t slot_mask, uint32_t n_resident) {
+__global__ void __launch_bounds__(256) k_inc_orphan_adopt(SnapDev s, ScratchDev sc, ResDev r, const uint32_t *rows, uint32_t c0, uint32_t c1,
+                                                          uint32_t bloom_mask, uint32_t slot_mask, uint32_t n_resident) {
   extern __shared__ uint32_t sm_adopt[];
   uint32_t *bits = sm_adopt, *slots = sm_adopt + ((bloom_mask + 1) >> 5);
   for (uint32_t i = threadIdx.x; i < (bloom_mask + 1) >> 5; i += blockDim.x) bits[i] = 0u;
   for (uint32_t i = threadIdx.x; i <= slot_mask; i += blockDim.x) slots[i] = KR_EMPTY32;
   __syncthreads();
-  for (uint32_t c = c0 + threadIdx.x; c < c1; c += blockDim.x) {
+  for (uint32_t i = c0 + threadIdx.x; i < c1; i += blockDim.x) {
+    const uint32_t c = rows ? rows[i] : i;
     const uint32_t ns = s.c_ns_id[c], nm = s.c_name_id[c];
     if (nm == 0) continue;  // (cl_probe matches no pod against an absent name)
     const uint32_t hk = hash_pair(ns, nm), h2 = bloom2(hk);
@@ -426,6 +459,93 @@ __global__ void __launch_bounds__(256) k_inc_orphan_adopt(SnapDev s, ScratchDev 
         break;
       }
     }
+  }
+}
+
+// ------------------------------------------------------------------------------------------------ RayCluster deletion
+// KR_OPT_CLUSTER_DELETES: an epoch whose object commit renumbered the RayClusters by swap-remove (the commit's row map: the old
+// rows `gone` that no RayCluster keeps — deleted, or moved to a row a deleted one vacated — and the new rows `init` that were moved
+// or created) brings the resident state into the new numbering in front of k_inc_admit:
+//   k_inc_digest_move          first, ahead of the hash stream: the digests of moved RayClusters whose spec range stayed;
+//   k_inc_clusters_release     one warp per gone row, while the cluster table still holds the old rows: touches every Pod in its
+//                              bucket (k_inc_admit re-matches it against the new table: a Pod of a deleted RayCluster becomes an
+//                              orphan, one of a moved RayCluster joins its new bucket) and takes the row's share out of the running
+//                              totals, the way the incremental decide counts it (its act_cnt, its groups' n_create);
+//   (the rebuild of the workersToDelete name table, and k_inc_orphan_adopt for the created RayClusters, still against the old table)
+//   k_inc_clusters_translate   one CTA: a touched row whose old RayCluster is gone had no RayCluster (its stale record went with the
+//                              bucket), and the dirty list drops the old rows at or past the new count (every entry below it names a
+//                              RayCluster of the new numbering: a kept one, or one that k_inc_clusters_insert marks anyway);
+//   k_inc_clusters_rekey       the cluster table cleared and rebuilt from every new row (cl_slots, cl_rec and cl_in: the offsets of
+//                              the shifted groups), the lowest row keeping a duplicate key;
+//   k_inc_groups_gather        the kept RayClusters' group records and create offsets from the first shifted group on, out of a
+//                              copy of the old ones (the ranges overlap);
+//   k_inc_clusters_insert      (rows = init) a moved or created RayCluster starts from an empty bucket at its new row, as a created one.
+// Places in the action list and create arena that a gone RayCluster held are abandoned until the next full pass.
+__global__ void __launch_bounds__(256) k_inc_digest_move(const uint32_t *__restrict__ pairs, uint32_t n, char *hash) {
+  const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
+  if (t >= 2 * n) return;
+  const uint32_t from = pairs[2 * (t >> 1)], to = pairs[2 * (t >> 1) + 1];  // (sources sit at or past the new count, targets below it)
+  reinterpret_cast<uint4 *>(hash + 32 * (size_t)to)[t & 1] = reinterpret_cast<const uint4 *>(hash + 32 * (size_t)from)[t & 1];
+}
+
+__global__ void __launch_bounds__(256) k_inc_clusters_release(SnapDev s, ScratchDev sc, ResDev r, const uint32_t *gone, uint32_t n_gone, uint32_t n_resident) {
+  const uint32_t w = (blockIdx.x * blockDim.x + threadIdx.x) >> 5, lane = threadIdx.x & 31;
+  if (w >= n_gone) return;
+  const uint32_t o = gone[w], epoch = inc_epoch(sc);
+  const uint4 rec = sc.cl_rec[o];  // {group_off, group_cnt} of the old row
+  const uint32_t P = sc.cl_dyn[o].x;
+  for (uint32_t k = lane; k < P; k += 32) {
+    const uint4 *at = rec_slot(sc, o, k);
+    uint32_t ns, nm;
+    if (at) inc_touch(s, sc, r, at->x, epoch, n_resident, ns, nm);
+  }
+  uint32_t cre = 0;
+  for (uint32_t g = rec.x + lane; g < rec.x + rec.y; g += 32) cre += r.groups[g].n_create;
+  cre = __reduce_add_sync(0xFFFFFFFFu, cre);
+  if (lane == 0) {
+    if (r.act_cnt[o]) atomicSub(&r.totals[2], r.act_cnt[o]);
+    if (cre) atomicSub(&r.totals[6], cre);
+  }
+}
+
+__global__ void __launch_bounds__(1024) k_inc_clusters_translate(ScratchDev sc, const uint32_t *gone, uint32_t n_gone, uint32_t n_clusters) {
+  __shared__ uint32_t s_warp[32];
+  const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
+  const uint32_t n_touched = __ldcg(&sc.inc[KR_INC_TOUCHED]), n_dirty = __ldcg(&sc.inc[KR_INC_DIRTY]);
+  for (uint32_t i = tid; i < n_touched; i += blockDim.x) {
+    const uint32_t c = sc.touched_old[i];
+    if (c != KR_EMPTY32 && sorted_has(gone, n_gone, c)) sc.touched_old[i] = KR_EMPTY32;
+  }
+  uint32_t kept = 0;  // entries of the dirty list kept so far (compacted in place: an entry never moves up)
+  for (uint32_t i0 = 0; i0 < n_dirty; i0 += blockDim.x) {
+    const uint32_t i = i0 + tid;
+    const uint32_t c = i < n_dirty ? sc.dirty_list[i] : KR_EMPTY32;
+    const bool keep = c < n_clusters;
+    const uint32_t b = __ballot_sync(0xFFFFFFFFu, keep);
+    if (lane == 0) s_warp[warp] = __popc(b);
+    __syncthreads();
+    uint32_t before = 0, total = 0;
+    for (uint32_t k = 0; k < blockDim.x / 32; k++) { const uint32_t v = s_warp[k]; before += k < warp ? v : 0u; total += v; }
+    if (keep) sc.dirty_list[kept + before + __popc(b & lanemask_lt())] = c;
+    kept += total;
+    __syncthreads();
+  }
+  if (tid == 0) sc.inc[KR_INC_DIRTY] = kept;
+}
+
+__global__ void __launch_bounds__(256) k_inc_clusters_rekey(SnapDev s, ScratchDev sc, uint32_t n_clusters) {
+  for (uint32_t c = blockIdx.x * blockDim.x + threadIdx.x; c < n_clusters; c += gridDim.x * blockDim.x) cl_insert_cluster(s, sc, c);
+}
+
+// new group gs0 + k takes old group gsrc[k] (KR_EMPTY32: a group of a moved or created RayCluster, which k_inc_clusters_insert
+// clears); old_groups / old_gcreate hold the old groups from g_lo on
+__global__ void __launch_bounds__(256) k_inc_groups_gather(ResDev r, ScratchDev sc, const uint32_t *__restrict__ gsrc, uint32_t gs0, uint32_t n_shifted,
+                                                           const kr_group_result *__restrict__ old_groups, const uint32_t *__restrict__ old_gcreate, uint32_t g_lo) {
+  for (uint32_t k = blockIdx.x * blockDim.x + threadIdx.x; k < n_shifted; k += gridDim.x * blockDim.x) {
+    const uint32_t o = gsrc[k];
+    if (o == KR_EMPTY32) continue;
+    r.groups[gs0 + k] = old_groups[o - g_lo];
+    sc.gcreate[gs0 + k] = old_gcreate[o - g_lo];
   }
 }
 

@@ -104,11 +104,20 @@ struct kr_packer {
   std::vector<uint8_t> cl_flag, hd_flag;
   bool wtd_changed = false;           // a workersToDelete name was rewritten in place (same count): the whole object part travels
   // RayClusters whose muted-spec JSON was placed since the last flush (kr_snapshot_commit_spec_rows with KR_OPT_SPEC_ROWS, unless the
-  // arena was compacted or a RayCluster row moved)
+  // arena was compacted or, without KR_OPT_CLUSTER_DELETES, a RayCluster row moved); a deletion moves a row's flag with the row
   std::vector<uint32_t> json_rows;
   std::vector<uint8_t> json_flag;
   bool json_compacted = false, clusters_moved = false;
   bool reshaped = false;              // a RayCluster the engine holds changed its group count or a workersToDelete list length
+  // per row: a RayCluster created in, or moved into, this row since the last flush (its spec travels after the object part, whose
+  // row map tells the engine about it); `fresh_any`: some row is set
+  std::vector<uint8_t> fresh;
+  bool fresh_any = false;
+  void set_fresh(uint32_t row, uint8_t v) {
+    if (row >= fresh.size()) fresh.resize((size_t)row + 256, 0);
+    fresh[row] = v; fresh_any |= v != 0;
+  }
+  bool is_fresh(uint32_t row) const { return row < fresh.size() && fresh[row]; }
 
   uint32_t intern(const kr_str &s) {
     if (!s.p) return KR_ID_ABSENT;
@@ -316,6 +325,7 @@ int kr_packer_cluster_upsert(kr_packer *p, const kr_cluster_obj *o) {
     p->clusters[row].ns_id = ns; p->clusters[row].name_id = nm; p->clusters[row].row = row;
     p->cluster_row.emplace(Key{ns, nm}, row);
     p->tables_dirty = true;
+    p->set_fresh(row, 1);
   } else row = it->second;
   ClusterRec &c = p->clusters[row];
   kr_snapshot_bufs &b = p->b;
@@ -349,7 +359,7 @@ int kr_packer_cluster_upsert(kr_packer *p, const kr_cluster_obj *o) {
     r.wtd.resize(g.n_workers_to_delete);
     for (uint32_t k = 0; k < g.n_workers_to_delete; k++) r.wtd[k] = p->intern(g.workers_to_delete[k]);
   }
-  if (shape && row < p->engine_sizes.n_clusters) p->reshaped = true;
+  if (shape && row < p->engine_sizes.n_clusters && !p->is_fresh(row)) p->reshaped = true;
   if (shape || p->tables_dirty) p->tables_dirty = true;
   else {  // same shape: the group rows are rewritten in place
     const uint32_t g0 = b.c_group_off[row];
@@ -389,6 +399,19 @@ int kr_packer_cluster_delete(kr_packer *p, kr_str ns, kr_str name) {
   p->json_dead += (p->clusters[row].json.size() + 15) & ~15ull;
   p->cluster_row.erase(it);
   p->clusters_moved = true;
+  // the placed-spec flag goes with the RayCluster: the deleted one's is dropped, the moved one's moves to its new row, which is fresh
+  auto unplace = [&](uint32_t r) {
+    if (r >= p->json_flag.size() || !p->json_flag[r]) return false;
+    p->json_flag[r] = 0;
+    p->json_rows.erase(std::find(p->json_rows.begin(), p->json_rows.end(), r));
+    return true;
+  };
+  unplace(row);
+  if (row != last) {
+    if (unplace(last)) { p->json_flag[row] = 1; p->json_rows.push_back(row); }
+    p->set_fresh(row, 1);
+  }
+  p->set_fresh(last, 0);
   if (row != last) {  // the last RayCluster moves into the hole: copy its scalar columns
     ClusterRec moved = std::move(p->clusters[last]);
     moved.row = row;
@@ -461,13 +484,20 @@ int kr_packer_flush(kr_packer *p, uint32_t *mode_out) {
   kr_engine_get_option(p->e, KR_OPT_CLUSTER_CREATES, &creates_opt);
   const uint32_t old_nc = p->engine_sizes.n_clusters;
   const bool appends = creates_opt && !p->first && !p->clusters_moved && !p->reshaped && !p->json_compacted && want.n_clusters > old_nc;
+  // KR_OPT_CLUSTER_DELETES: RayClusters deleted by swap-remove (none the engine holds reshaped, the arena not compacted) keep the
+  // incremental epoch as well: the kept RayClusters' edited specs as spec rows before the object part, the moved and created ones'
+  // after it
+  uint64_t deletes_opt = 0;
+  kr_engine_get_option(p->e, KR_OPT_CLUSTER_DELETES, &deletes_opt);
+  const bool renumbered = deletes_opt && !p->first && p->clusters_moved && !p->reshaped && !p->json_compacted;
   // Row-granular spec commit (KR_OPT_SPEC_ROWS): only the re-emitted blobs travel, while every other one stays where it was.
   uint64_t spec_opt = 0;
   kr_engine_get_option(p->e, KR_OPT_SPEC_ROWS, &spec_opt);
   const bool spec_ok = spec_opt && p->json_dirty && !p->first && !p->json_compacted && !p->clusters_moved && (want.n_clusters == old_nc || appends);
-  std::vector<uint32_t> new_rows, old_rows;  // blobs placed this flush: of appended RayClusters / of the others
-  for (uint32_t r : p->json_rows) (r >= old_nc ? new_rows : old_rows).push_back(r);
-  const bool json_rows_ok = spec_ok || (appends && old_rows.empty());  // every placed blob travels as a spec row
+  std::vector<uint32_t> new_rows, old_rows;  // blobs placed this flush: of appended, moved or created RayClusters / of the others
+  for (uint32_t r : p->json_rows) (r >= old_nc || p->is_fresh(r) ? new_rows : old_rows).push_back(r);
+  // every placed blob travels as a spec row
+  const bool json_rows_ok = spec_ok || ((appends || renumbered) && (old_rows.empty() || spec_opt));
   if (memcmp(&want, &p->engine_sizes, sizeof want) != 0 || p->first) {
     if (int rc = kr_snapshot_begin(p->e, &p->sizes, &same)) return rc;  // fixed layout: new live counts, same addresses, resident data kept
     p->engine_sizes = want;
@@ -488,7 +518,7 @@ int kr_packer_flush(kr_packer *p, uint32_t *mode_out) {
       if (int rc = kr_snapshot_commit_object_rows(p->e, p->dirty_cl.data(), (uint32_t)p->dirty_cl.size(), p->dirty_hd.data(), (uint32_t)p->dirty_hd.size())) return rc;
       mode |= KR_PACK_OBJECT_ROWS;
     }
-    if (json_rows_ok && !new_rows.empty()) {  // the appended RayClusters' specs, once the object part has recorded them as new rows
+    if (json_rows_ok && !new_rows.empty()) {  // the new RayClusters' specs, once the object part has recorded them as new rows
       if (int rc = kr_snapshot_commit_spec_rows(p->e, new_rows.data(), (uint32_t)new_rows.size())) return rc;
       mode |= KR_PACK_SPEC_ROWS;
     }
@@ -506,6 +536,7 @@ int kr_packer_flush(kr_packer *p, uint32_t *mode_out) {
   p->dirty_cl.clear(); p->dirty_hd.clear(); p->wtd_changed = false;
   for (uint32_t r : p->json_rows) p->json_flag[r] = 0;
   p->json_rows.clear(); p->json_compacted = p->clusters_moved = p->reshaped = false;
+  if (p->fresh_any) { std::fill(p->fresh.begin(), p->fresh.end(), 0); p->fresh_any = false; }
   p->first = p->objects_dirty = p->tables_dirty = p->heads_dirty = p->jobs_dirty = p->json_dirty = false;
   p->epoch++;
   p->last_mode = mode;

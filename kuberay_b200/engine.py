@@ -234,7 +234,8 @@ class Engine:
     @classmethod
     def for_snapshot(cls, snap: Snapshot, device: int = 0, max_creates: int | None = None, slack: float = 1.0,
                      large_clusters: bool = False, wide_clusters: bool = False, huge_clusters: bool = False,
-                     wtd_edits: bool = False, spec_rows: bool = False, cluster_creates: bool = False) -> "Engine":
+                     wtd_edits: bool = False, spec_rows: bool = False, cluster_creates: bool = False,
+                     cluster_deletes: bool = False) -> "Engine":
         d = snap.dims
         up = lambda x: int(x * slack) + 1  # noqa: E731
         if max_creates is None:
@@ -253,6 +254,8 @@ class Engine:
             eng.set_spec_rows(True)
         if cluster_creates:
             eng.set_cluster_creates(True)
+        if cluster_deletes:
+            eng.set_cluster_deletes(True)
         return eng
 
     def _check(self, rc: int):
@@ -310,6 +313,12 @@ class Engine:
         RayJobs are created or deleted (commit the object part, then the new RayClusters' specs with commit_spec_rows); read at each
         begin and object commit."""
         self._check(self._L.kr_engine_set_option(self._h, abi.OPT_CLUSTER_CREATES, 1 if on else 0))
+
+    def set_cluster_deletes(self, on: bool = True):
+        """KR_OPT_CLUSTER_DELETES: under the fixed layout, keep incremental epochs when RayClusters are deleted by swap-remove (begin
+        with the new counts, commit the object part; with cluster_creates the same epoch may create RayClusters in vacated rows); read
+        at each begin and object commit."""
+        self._check(self._L.kr_engine_set_option(self._h, abi.OPT_CLUSTER_DELETES, 1 if on else 0))
 
     def get_option(self, option: int) -> int:
         """kr_engine_get_option: an option's current value, or the read-only OPT_BUCKET_STRIDE (0: the sort pipeline)."""

@@ -483,6 +483,46 @@ def first_clusters(snap: Snapshot, k: int, free_from: int | None = None, jobs=No
     return out.validate()
 
 
+def swap_remove_order(n: int, rows) -> np.ndarray:
+    """The old row of each new row after deleting the RayClusters at (old) rows `rows` one by one by swap-remove, as the native
+    packer does: the last RayCluster moves into each hole."""
+    order = list(range(n))
+    where = {c: c for c in order}
+    for r in rows:
+        pos = where.pop(int(r))
+        last = order.pop()
+        if last != int(r):
+            order[pos] = last
+            where[last] = pos
+    return np.asarray(order, dtype=np.int64)
+
+
+def select_clusters(snap: Snapshot, order) -> Snapshot:
+    """The RayClusters at old rows `order`, in that row order, with their groups and workersToDelete names laid out again in row
+    order; every pod row, head-aux row, RayJob row and the JSON arena stay as they are."""
+    order = np.asarray(order, dtype=np.int64)
+    d = snap.dims
+    goff, gcnt = snap.c_group_off.astype(np.int64), snap.c_group_cnt.astype(np.int64)
+    groups = np.concatenate([np.arange(goff[c], goff[c] + gcnt[c]) for c in order] + [np.zeros(0, np.int64)])
+    names = np.concatenate([np.arange(int(snap.g_wtd_off[g]), int(snap.g_wtd_off[g] + snap.g_wtd_cnt[g])) for g in groups] + [np.zeros(0, np.int64)])
+    out = Snapshot(order.size, groups.size, names.size, d["pods"], d["heads"], d["jobs"], d["json"])
+    rows = {"clusters": order, "groups": groups, "wtd": names}
+    for name, _dt, mult, dim in abi.COLUMNS:
+        src = snap.cols[name]
+        out.cols[name][:] = (src.reshape(-1, mult)[rows[dim]].reshape(-1) if mult > 1 else src[rows[dim]]) if dim in rows else src
+    cnt = gcnt[order]
+    out.c_group_off[:] = np.concatenate([[0], np.cumsum(cnt)[:-1]]).astype(np.uint32) if order.size else 0
+    out.g_cluster_idx[:] = np.repeat(np.arange(order.size), cnt).astype(np.uint32)
+    out.g_wtd_off[:] = np.concatenate([[0], np.cumsum(out.g_wtd_cnt)[:-1]]).astype(np.uint32) if groups.size else 0
+    return out.validate()
+
+
+def delete_clusters(snap: Snapshot, rows) -> Snapshot:
+    """The snapshot after the RayClusters at rows `rows` were deleted by swap-remove (swap_remove_order), with groups and names laid
+    out again in row order.  Their Pods stay, as orphans (until garbage collection removes them)."""
+    return select_clusters(snap, swap_remove_order(snap.dims["clusters"], rows))
+
+
 def config(name: str, **overrides) -> SynthParams:
     d = dict(CONFIGS[name])
     d.update(overrides)

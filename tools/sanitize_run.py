@@ -114,6 +114,53 @@ def creations(snap, flags, label):
     print(label, "ok:", inc, "of 2 creation epochs incremental", flush=True)
 
 
+def deletions(snap, flags, label):
+    """KR_OPT_CLUSTER_DELETES (kr_incr.cuh): 12 RayClusters deleted by swap-remove under a fixed layout after a full pass — once with
+    no resident orphan before the epoch (k_inc_clusters_release, _translate, _rekey, k_inc_groups_gather, the name table rebuilt,
+    k_inc_clusters_insert for the moved ones), once with orphans resident and RayClusters created in the same epoch (with
+    KR_OPT_CLUSTER_CREATES: k_inc_orphan_adopt as well)."""
+    flags.fetch_pod_lists = 0
+    nc = snap.dims["clusters"]
+    inc = 0
+    for orphans in (False, True):
+        k = nc - 8 if orphans else nc
+        before = synthetic.select_clusters(snap, np.arange(k))
+        if not orphans:  # no Pod of the fleet is an orphan to begin with: the Pods no RayCluster owns become free rows
+            ckey = (snap.c_ns_id.astype(np.uint64) << np.uint64(32)) | snap.c_name_id.astype(np.uint64)
+            pkey = (snap.p_ns_id.astype(np.uint64) << np.uint64(32)) | snap.p_cluster_name_id.astype(np.uint64)
+            lost = np.flatnonzero(~np.isin(pkey, ckey))
+            for c, _d, _m, dim in abi.COLUMNS:
+                if dim == "pods":
+                    before.cols[c][lost] = 0
+            before.p_packed[lost] = np.uint32(abi.PP_TOMBSTONE)
+        order = synthetic.swap_remove_order(k, np.arange(3, 3 + 12 * 7, 7))
+        after = synthetic.select_clusters(before, order)
+        if orphans:  # ... and the 8 RayClusters past the first k created after the last row
+            after = synthetic.select_clusters(snap, np.concatenate([order, np.arange(k, nc)]))
+        eng = Engine.for_snapshot(snap, slack=1.2, cluster_deletes=True, cluster_creates=orphans)
+        eng.set_fixed_layout(True)
+        try:
+            views = eng.begin(before.sizes())
+            eng.fill(views, before)
+            eng.commit()
+            eng.reconcile(flags)
+            views = eng.begin(after.sizes())
+            for c, _d, _m, dim in abi.COLUMNS:
+                if dim not in ("pods", "json"):
+                    np.copyto(views[c], after.cols[c])
+            eng.commit(abi.PART_OBJECTS)
+            if orphans:
+                eng.commit_spec_rows(np.arange(order.size, after.dims["clusters"], dtype=np.uint32))
+            prof = eng.reconcile_profiled(flags)
+            names = [n for n, _ in prof["kernels"]]
+            assert "k_inc_clusters_release" in names and ("k_inc_orphan_adopt" in names) == orphans, names
+            got = eng.fetch()
+            inc += got.changed_clusters is not None or got.n_changed < after.dims["clusters"]
+        finally:
+            eng.close()
+    print(label, "ok:", inc, "of 2 deletion epochs incremental", flush=True)
+
+
 def wtd_edits(snap, flags, label):
     """KR_OPT_WTD_EDITS (kr_incr.cuh): workersToDelete renames, a list grown past the old n_wtd, then every list cleared — each epoch
     rebuilds the name table on the device (k_inc_wtd_release / _clear / _insert / _resolve)."""
@@ -184,6 +231,8 @@ def spec_rows(snap, flags, label):
 
 
 def main():
+    deletions(*synthetic.generate(synthetic.config("C2", n_clusters=300, pods_per_cluster=20, groups=2, wtd_group_frac=0.3, recreate_frac=0.3)),
+              "RayCluster deletions")
     creations(*synthetic.generate(synthetic.config("C2", n_clusters=300, pods_per_cluster=20, groups=2, wtd_group_frac=0.3, recreate_frac=0.3)),
               "RayCluster creations")
     spec_rows(*synthetic.generate(synthetic.config("C2", n_clusters=300, pods_per_cluster=20, groups=2, recreate_frac=0.3)), "spec rows")
