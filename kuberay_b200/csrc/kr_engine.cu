@@ -36,10 +36,11 @@ int kr_specjson_emit_string(const uint8_t *spec_json, uint64_t len, bool muted, 
 namespace {
 
 constexpr size_t kAlign = 256;
-// most RayClusters one incremental epoch appends while there are orphans (k_inc_orphan_adopt: 16 Bloom bits and two 4-byte table
+// most RayClusters one incremental epoch brings in while there are orphans (k_inc_orphan_adopt: 16 Bloom bits and two 4-byte table
 // slots per RayCluster in shared memory, 40 KB); more take the full pass
 constexpr uint32_t kAdoptMax = 4096;
-// most RayClusters one incremental epoch of KR_OPT_CLUSTER_DELETES deletes, moves and creates together; more take the full pass
+// most RayClusters one incremental epoch that renumbers them (KR_OPT_CLUSTER_DELETES) deletes, moves and creates together; more take
+// the full pass
 constexpr uint32_t kMapMax = 4096;
 enum MapList { MP_GONE, MP_INIT, MP_DIGESTS, MP_GSRC, MP_WSRC, MP_LISTS };  // the lists of a row map on the device, in this order
 inline size_t align_up(size_t x, size_t a = kAlign) { return (x + a - 1) / a * a; }
@@ -141,7 +142,8 @@ struct CommitRecord {
     uint32_t ns, name, wtd_off;    // key and first workersToDelete name: whole with the object part
   };
   std::vector<Row> rows;             // per RayCluster row (sized, zero-filled, by every whole commit)
-  // KR_OPT_CLUSTER_DELETES: how the last object commit renumbered the RayClusters (swap-remove), for the next pass
+  // KR_OPT_CLUSTER_CREATES / KR_OPT_CLUSTER_DELETES: the RayCluster rows that entered the fleet since the last pass and how the last
+  // object commit renumbered the others (swap-remove), for the next pass.  Without gone rows: RayClusters appended after the resident ones.
   struct RowMap {
     std::vector<uint32_t> gone;      // old rows no RayCluster keeps (deleted, or moved away), ascending
     std::vector<uint32_t> init;      // new rows of a moved or created RayCluster, ascending
@@ -151,7 +153,7 @@ struct CommitRecord {
     uint32_t gs0 = 0, ws0 = 0;       // groups / names from these on were shifted
     std::vector<uint32_t> gsrc, wsrc;  // ... and came from these old ones (KR_EMPTY32: of a moved or created RayCluster)
     uint32_t g_lo = 0, g_hi = 0;     // the old groups gsrc reads
-    bool names_moved = false;        // some workersToDelete name shifted, vanished or appeared
+    bool names_moved = false;        // a resident workersToDelete name shifted or vanished, or a map with gone rows brought new ones
   };
   RowMap map;
   uint32_t n_recreate = 0;           // RayClusters with KR_CF_UPGRADE_RECREATE (decide phase 1 needed): whole
@@ -194,27 +196,36 @@ struct CommitRecord {
     return std::includes(given.begin(), given.end(), json_cols_behind.begin(), json_cols_behind.end());
   }
 
-  // KR_OPT_CLUSTER_DELETES: the row map of an object part that renumbered the recorded RayClusters (into `map`).  Only the rows whose
-  // key changed and the old rows at or past the new count are looked at.  -> 0: nothing was renumbered (appended rows are the
-  // creation path's), 1: a swap-remove map, -1: a renumbering the resident state does not follow (the next pass is a full one).
-  // `resident`: the RayCluster rows the device tables hold; `wide_ok`: KR_OPT_WIDE_CLUSTERS.
-  int derive_map(const kr_snapshot_bufs &hb, const kr_sizes &n, bool creates, bool wide_ok, uint32_t resident, uint32_t res_groups_old,
+  // The row map of an object part that brought RayClusters into the recorded fleet or renumbered it (into `map`).  With `deletes`
+  // (KR_OPT_CLUSTER_DELETES) the rows whose key changed and the old rows at or past the new count are looked at; without it only the
+  // rows past the recorded ones are (a changed key is the device diff's to find).  -> 0: nothing entered, left or moved, 1: a map the
+  // resident state follows, -1: a renumbering it does not follow (the next pass is a full one).
+  // `creates`: KR_OPT_CLUSTER_CREATES; `resident`: the RayCluster rows the device tables hold.
+  int derive_map(const kr_snapshot_bufs &hb, const kr_sizes &n, bool creates, bool deletes, uint32_t resident, uint32_t res_groups_old,
                  uint32_t res_wtd_old) {
     const uint32_t had = (uint32_t)rows.size(), nn = n.n_clusters, lo = std::min(had, nn);
     auto key = [](uint32_t ns, uint32_t name) { return (uint64_t)ns << 32 | name; };
     std::vector<uint32_t> old_ch, new_ch;
-    for (uint32_t c = 0; c < lo; c++)
-      if (rows[c].ns != hb.c_ns_id[c] || rows[c].name != hb.c_name_id[c]) old_ch.push_back(c), new_ch.push_back(c);
-    for (uint32_t c = nn; c < had; c++) old_ch.push_back(c);
-    if (old_ch.empty()) return 0;
-    if (had != resident) return -1;  // (an earlier object commit of this epoch appended rows the device tables do not hold yet)
+    if (deletes) {
+      for (uint32_t c = 0; c < lo; c++)
+        if (rows[c].ns != hb.c_ns_id[c] || rows[c].name != hb.c_name_id[c]) old_ch.push_back(c), new_ch.push_back(c);
+      for (uint32_t c = nn; c < had; c++) old_ch.push_back(c);
+    }
+    if (old_ch.empty()) {
+      // No recorded row left or moved: the rows past the resident ones, if this part added any, are created RayClusters, any number of
+      // them, with their groups and names after the resident ones.  Counted from the resident rows (all of them recorded), not from
+      // the recorded ones: the map of a second such commit in one epoch stands for both.
+      if (!creates || nn <= had || had < resident) return 0;
+      RowMap m;
+      for (uint32_t c = resident; c < nn; c++) m.init.push_back(c);
+      m.created = m.init;
+      m.gs0 = n.n_groups; m.ws0 = n.n_wtd;
+      map = std::move(m);
+      return 1;
+    }
+    if (had != resident) return -1;  // (an earlier object commit of this epoch added rows the device tables do not hold yet)
     for (uint32_t c = had; c < nn; c++) new_ch.push_back(c);
     if (old_ch.size() > kMapMax || new_ch.size() > kMapMax) return -1;
-    // (a RayCluster of more than KR_SMEM_GROUPS worker groups is decided on the bucket pipeline only with KR_OPT_WIDE_CLUSTERS)
-    if (!wide_ok) {
-      for (uint32_t o : old_ch) if (rows[o].group_cnt > KR_SMEM_GROUPS) return -1;
-      for (uint32_t c : new_ch) if (hb.c_group_cnt[c] > KR_SMEM_GROUPS) return -1;
-    }
     std::unordered_map<uint64_t, uint32_t> old_key;  // key of a gone row -> that row
     for (uint32_t o : old_ch) if (!old_key.emplace(key(rows[o].ns, rows[o].name), o).second) return -1;
     for (uint32_t c = 0; c < lo; c++)  // a kept row holding a gone row's key: the table's lowest-row rule would move it
@@ -264,25 +275,23 @@ struct CommitRecord {
     return 1;
   }
 
-  // what a whole commit moved: the launch shape / pipeline, the wide set, the hash order; RayClusters from row `appended` on are new
-  // rows of KR_OPT_CLUSTER_CREATES (n_clusters: none), whose specs the caller commits as spec rows; `map`: derive_map's verdict
-  struct Moved { bool shape, wide, order; uint32_t appended; int map; };
-  // (`deletes`, `wide_ok`, `resident`: KR_OPT_CLUSTER_DELETES, KR_OPT_WIDE_CLUSTERS, the RayCluster rows the device tables hold)
-  Moved commit_whole(const kr_snapshot_bufs &hb, const kr_sizes &n, uint32_t parts, bool wtd_edits, bool creates, bool deletes, bool wide_ok,
-                     uint32_t resident) {
+  // what a whole commit moved: the launch shape / pipeline, the wide set, the hash order; `map`: derive_map's verdict (1: the created
+  // RayClusters of `map`, whose specs the caller commits as spec rows, are hashed by the next pass)
+  struct Moved { bool shape, wide, order; int map; };
+  // (`creates`, `deletes`, `resident`: KR_OPT_CLUSTER_CREATES, KR_OPT_CLUSTER_DELETES, the RayCluster rows the device tables hold)
+  Moved commit_whole(const kr_snapshot_bufs &hb, const kr_sizes &n, uint32_t parts, bool wtd_edits, bool creates, bool deletes, uint32_t resident) {
     const bool objects = parts & (KR_PART_COLUMNS | KR_PART_OBJECTS);
     const size_t had = rows.size();
-    const int mapped = deletes && objects && had ? derive_map(hb, n, creates, wide_ok, resident, res_groups, res_wtd) : 0;
-    const bool appends = creates && objects && n.n_clusters > had && mapped == 0;  // (not a moved range: only the new rows are hashed)
-    bool ranges_moved = had != n.n_clusters && !appends && mapped != 1;  // some RayCluster's JSON range differs from the one the digests / the hash order were computed from
+    const int mapped = (creates || deletes) && objects && had ? derive_map(hb, n, creates, deletes, resident, res_groups, res_wtd) : 0;
+    bool ranges_moved = had != n.n_clusters && mapped != 1;  // some RayCluster's JSON range differs from the one the digests / the hash order were computed from
     uint32_t n_rc = 0, n_mh_now = 0, max_groups = 0;
     std::vector<uint32_t> wide;
     rows.resize(n.n_clusters);
     uint32_t woff = 0;
     for (uint32_t c = 0; c < n.n_clusters; c++) {
       Row &r = rows[c];
-      const bool fresh = mapped == 1 && std::binary_search(map.init.begin(), map.init.end(), c);  // (derive_map compared its range)
-      const bool moved = fresh ? false : c >= had ? !appends : r.json_off != hb.c_json_off[c] || r.json_len != hb.c_json_len[c];
+      const bool fresh = mapped == 1 && std::binary_search(map.init.begin(), map.init.end(), c);  // (its digest moves with it or is computed anew)
+      const bool moved = !fresh && (c >= had || r.json_off != hb.c_json_off[c] || r.json_len != hb.c_json_len[c]);
       if (moved && !objects) json_cols_behind.push_back(c);  // (the device's range columns keep the old range)
       ranges_moved |= moved;
       r.json_off = hb.c_json_off[c]; r.json_len = hb.c_json_len[c];
@@ -308,7 +317,7 @@ struct CommitRecord {
     for (uint32_t c = 0; c < n.n_clusters; c++) if (hb.c_flags[c] & KR_CF_UPGRADE_RECREATE) rsig = (rsig ^ c) * 0x100000001B3ull;
     // (a spec-row commit updates the recorded ranges itself: its own flag says the order no longer follows them)
     bool order = ranges_moved || rsig != recreate_sig || spec_order_stale;
-    if ((appends || mapped == 1) && !ranges_moved) { spec_order_stale = true; order = false; }  // (the order lacks the new rows: the next pass that hashes every message rebuilds it)
+    if (mapped == 1 && !ranges_moved) { spec_order_stale = true; order = false; }  // (the order lacks the new rows: the next pass that hashes every message rebuilds it)
     if (order) spec_order_stale = false;  // (the new order travels with this commit)
     recreate_sig = rsig;
     if ((parts & KR_PART_JSON) || ranges_moved) hash_dirty = true;
@@ -327,7 +336,7 @@ struct CommitRecord {
         prev_wtd.insert(prev_wtd.end(), hb.w_name_id, hb.w_name_id + n.n_wtd);
       }
     }
-    return {shape, wide_moved, order, appends ? (uint32_t)had : n.n_clusters, mapped};
+    return {shape, wide_moved, order, mapped};
   }
   // -> the snapshot's first multi-host group came or its last went (a numOfHosts edit)
   bool commit_rows(const kr_snapshot_bufs &hb, const uint32_t *cl, uint32_t n_cl, const uint32_t *hd, uint32_t n_hd) {
@@ -345,7 +354,7 @@ struct CommitRecord {
   }
   // the m pulled rows' new ranges: a later object commit does not re-hash everything on their account; the full-pass hash order
   // does not follow them (spec_order_stale when a block count moved)
-  // (rows past the recorded ones: the next object commit records them as appended, or sees every range as moved)
+  // (rows past the recorded ones: the next object commit records them as created, or sees every range as moved)
   void commit_spec_rows(const uint32_t *cl, const uint64_t *off, const uint32_t *len, uint32_t m) {
     for (uint32_t i = 0; i < m; i++) {
       if (cl[i] >= rows.size()) continue;
@@ -532,7 +541,7 @@ struct kr_engine {
   Staging hb;                  // kr_hash_batch
   Staging pr;                  // incremental pod commits
   Staging orow;                // kr_snapshot_commit_object_rows
-  Staging mp;                  // KR_OPT_CLUSTER_DELETES: the row map of an object commit (rec.map), for its diff and the next pass
+  Staging mp;                  // the row map of an object commit (rec.map), for its diff and the next pass
   bool map_pending = false;    // ... uploaded and not yet applied by a pass
   kr_sizes map_sizes{};        // ... the live counts of that object commit
   size_t mp_at[5]{};           // offsets in mp of its lists (MapList)
@@ -596,7 +605,7 @@ struct kr_engine {
   bool wtd_edits = false;        // KR_OPT_WTD_EDITS
   bool cluster_creates = false;  // KR_OPT_CLUSTER_CREATES
   bool cluster_deletes = false;  // KR_OPT_CLUSTER_DELETES
-  uint32_t inc_n_clusters = 0;   // RayClusters in the resident tables (those past it were appended since the last pass)
+  uint32_t inc_n_clusters = 0;   // RayClusters in the resident tables
   uint32_t res_n_wtd = 0;        // names in the resident name table and its resolutions (wtd_pod_idx)
   bool ran_inc = false;          // the last pass was an incremental one
   bool host_results_stale = false;  // an incremental pass went unfetched: the host copy misses its records, the next fetch copies everything
@@ -1202,20 +1211,18 @@ void commits_read(kr_engine *e) {
 int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile, bool *done_inc) {
   *done_inc = false;
   const kr_sizes &n = e->sizes;
-  // RayClusters appended since the last pass (KR_OPT_CLUSTER_CREATES; the keep test of kr_snapshot_begin let nothing else move
-  // n_clusters): their rows must have been committed, the bucket arena must hold them at this stride, a wide one needs
-  // KR_OPT_WIDE_CLUSTERS, and the orphan scan's shared-memory table holds kAdoptMax of them
-  const uint32_t c0 = e->inc_n_clusters, c1 = n.n_clusters;
-  // KR_OPT_CLUSTER_DELETES: an object commit renumbered the RayClusters (rec.map, uploaded to mp): its RayCluster rows must be the
-  // committed ones, and the orphan scan's table holds kAdoptMax created RayClusters
-  const bool mapped = e->map_pending;
-  const CommitRecord::RowMap &m = e->rec.map;
-  const bool adopt = (mapped ? !m.created.empty() : c1 > c0) && e->h_totals[1] != 0;  // (the last pass counted orphans: some of them may be the new RayClusters' Pods)
-  if (mapped && (e->rec.res_clusters != c1 || e->rec.res_groups != n.n_groups || e->map_sizes.n_clusters != c1 || e->map_sizes.n_groups != n.n_groups ||
-                 (size_t)c1 * e->bstride > e->sl.bucket_entries || (adopt && m.init.size() > kAdoptMax)))
-    return KR_OK;
-  if (!mapped && c1 != c0 && (c1 < c0 || e->rec.res_clusters != c1 || e->rec.res_groups != n.n_groups || (size_t)c1 * e->bstride > e->sl.bucket_entries ||
-                              (e->rec.snap_max_groups > KR_SMEM_GROUPS && !e->wide_on) || (adopt && c1 - c0 > kAdoptMax)))
+  // An object commit created or renumbered RayClusters (rec.map, uploaded to mp; none: no list of it holds a row): its RayCluster and
+  // group rows must be the committed ones, the bucket arena must hold the RayClusters at this stride, a wide one needs
+  // KR_OPT_WIDE_CLUSTERS, and the orphan scan's shared-memory table holds kAdoptMax new RayClusters.  A RayCluster count that
+  // kr_snapshot_begin moved without an object commit behind it takes the full pass.
+  static const CommitRecord::RowMap no_map;
+  const CommitRecord::RowMap &m = e->map_pending ? e->rec.map : no_map;
+  const uint32_t n_gone = (uint32_t)m.gone.size(), n_init = (uint32_t)m.init.size();
+  const bool adopt = !m.created.empty() && e->h_totals[1] != 0;  // (the last pass counted orphans: some of them may be the new RayClusters' Pods)
+  if (e->map_pending ? e->rec.res_clusters != n.n_clusters || e->rec.res_groups != n.n_groups || e->map_sizes.n_clusters != n.n_clusters ||
+                           e->map_sizes.n_groups != n.n_groups || (size_t)n.n_clusters * e->bstride > e->sl.bucket_entries ||
+                           (e->rec.snap_max_groups > KR_SMEM_GROUPS && !e->wide_on) || (adopt && n_init > kAdoptMax)
+                     : n.n_clusters != e->inc_n_clusters)
     return KR_OK;
   PassCtx c(e, profile);
   const SnapDev &s = c.s; const ResDev &r = c.r; const ScratchDev &sc = c.sc; const Sizes &z = c.z;
@@ -1223,8 +1230,7 @@ int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile
   CK(cudaStreamWaitEvent(M, e->ev_cols, 0));
   const bool do_hash = e->rec.hash_dirty && !f.skip_hash && n.n_clusters > 0;
   auto map_dev = [&](MapList i) { return reinterpret_cast<const uint32_t *>(e->mp.d + e->mp_at[i]); };
-  const uint32_t n_gone = mapped ? (uint32_t)m.gone.size() : 0, n_init = mapped ? (uint32_t)m.init.size() : 0;
-  if (mapped && !do_hash && !m.digests.empty()) {  // (ahead of the hash stream's fork: a re-hashed row's digest lands after it)
+  if (!do_hash && !m.digests.empty()) {  // (ahead of the hash stream's fork: a re-hashed row's digest lands after it)
     const uint32_t nd = (uint32_t)m.digests.size() / 2;
     c.mark("k_inc_digest_move");
     k_inc_digest_move<<<(2 * nd + 255) / 256, 256, 0, M>>>(map_dev(MP_DIGESTS), nd, r.hash);
@@ -1246,7 +1252,8 @@ int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile
     if (e->rec.n_recreate && !do_hash) { c.mark("k_inc_mark_rows"); k_inc_mark_rows<<<(n_rows + 255) / 256, 256, 0, M>>>(s, sc, spec_rows, n_rows); }
   }
   const int grid = e->sm_count * 2;
-  if (mapped) {  // RayClusters renumbered (kr_incr.cuh): the gone rows' Pods touched while the table holds the old rows
+  // RayClusters created or renumbered (kr_incr.cuh), each step when its list of the map holds a row
+  if (n_gone) {  // the gone rows' Pods touched while the table holds the old rows
     c.mark("k_inc_clusters_release");
     k_inc_clusters_release<<<(32 * n_gone + 255) / 256, 256, 0, M>>>(s, sc, r, map_dev(MP_GONE), n_gone, e->inc_n_pods);
   }
@@ -1268,18 +1275,15 @@ int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile
     e->res_n_wtd = n.n_wtd;
     e->rec.wtd_rebuild = false;
   }
-  // RayClusters appended or created (kr_incr.cuh): their orphans touched while the table does not hold them
-  const uint32_t *adopt_rows = mapped ? map_dev(MP_INIT) : nullptr;
-  const uint32_t a0 = mapped ? 0 : c0, a1 = mapped ? n_init : c1;
-  if (adopt) {
+  if (adopt) {  // the created RayClusters' orphans touched while the table does not hold them
     uint32_t bloom_bits = 1024, slots = 64;
-    while (bloom_bits < 16 * (a1 - a0)) bloom_bits <<= 1;
-    while (slots < 2 * (a1 - a0)) slots <<= 1;
+    while (bloom_bits < 16 * n_init) bloom_bits <<= 1;
+    while (slots < 2 * n_init) slots <<= 1;
     c.mark("k_inc_orphan_adopt");
     k_inc_orphan_adopt<<<std::min<uint32_t>((uint32_t)e->sm_count * 4, (e->inc_n_pods + 255) / 256 + 1), 256, bloom_bits / 8 + 4 * (size_t)slots, M>>>(
-        s, sc, r, adopt_rows, a0, a1, bloom_bits - 1, slots - 1, e->inc_n_pods);
+        s, sc, r, map_dev(MP_INIT), n_init, bloom_bits - 1, slots - 1, e->inc_n_pods);
   }
-  if (mapped) {  // ... then the resident state in the new numbering, and the moved and created RayClusters enter it as new ones
+  if (n_gone) {  // ... then the resident state in the new numbering
     c.mark("k_inc_clusters_translate");
     k_inc_clusters_translate<<<1, 1024, 0, M>>>(sc, map_dev(MP_GONE), n_gone, n.n_clusters);
     c.mark("k_inc_clusters_rekey");
@@ -1294,16 +1298,13 @@ int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile
       c.mark("k_inc_groups_gather");
       k_inc_groups_gather<<<std::min<uint32_t>(grid, (n.n_groups - m.gs0 + 255) / 256 + 1), 256, 0, M>>>(r, sc, map_dev(MP_GSRC), m.gs0, n.n_groups - m.gs0, og, oc, m.g_lo);
     }
-    if (n_init) {  // (their names, if any, came with the rebuilt name table)
-      c.mark("k_inc_clusters_insert");
-      k_inc_clusters_insert<<<(n_init + 255) / 256, 256, 0, M>>>(s, sc, r, map_dev(MP_INIT), 0u, n_init, 0);
-    }
   }
-  if (!mapped && c1 > c0) {  // RayClusters appended: they enter the table
-    // their workersToDelete names: inserted here and resolved against every pod row (unless the whole table was rebuilt above)
+  if (n_init) {  // ... and the moved and created RayClusters enter the table as new ones
+    // their workersToDelete names after the resident ones: inserted here and resolved against every pod row (a map that moved a
+    // resident name had the whole table rebuilt above, the new names with it)
     const bool names = n.n_wtd > e->res_n_wtd;
     c.mark("k_inc_clusters_insert");
-    k_inc_clusters_insert<<<(c1 - c0 + 255) / 256, 256, 0, M>>>(s, sc, r, nullptr, c0, c1, names ? 1 : 0);
+    k_inc_clusters_insert<<<(n_init + 255) / 256, 256, 0, M>>>(s, sc, r, map_dev(MP_INIT), n_init, names ? 1 : 0);
     if (names) {
       c.mark("k_inc_wtd_resolve");
       k_inc_wtd_resolve<<<std::min<uint32_t>((uint32_t)e->sm_count * 4, (n.n_pods + 255) / 256 + 1), 256, e->sl.wt_bits_n / 8, M>>>(s, sc, r, z, e->inc_n_pods, e->res_n_wtd);
@@ -1359,17 +1360,16 @@ int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile
     e->spec_hashed.assign(h, h + n_rows);
   }
   if (do_hash || n_rows) clear_spec_rows(e);
-  if (mapped) {  // the host copy in the new numbering as well: moved digests, shifted group records (re-decided RayClusters come with the fetch)
-    ResDev hr = bind_out(e->ol, e->h_out);
-    if (!do_hash)
-      for (size_t i = 0; i < m.digests.size(); i += 2) memcpy(hr.hash + 32 * (size_t)m.digests[i + 1], hr.hash + 32 * (size_t)m.digests[i], 32);
-    if (m.gs0 < n.n_groups && m.g_hi > m.g_lo) {
-      const std::vector<kr_group_result> old(hr.groups + m.g_lo, hr.groups + m.g_hi);
-      for (uint32_t k = 0; k < n.n_groups - m.gs0; k++)
-        if (m.gsrc[k] != KR_EMPTY32) hr.groups[m.gs0 + k] = old[m.gsrc[k] - m.g_lo];
-    }
-    e->map_pending = false;
+  // the host copy in the new numbering as well: moved digests, shifted group records (re-decided RayClusters come with the fetch)
+  ResDev hr = bind_out(e->ol, e->h_out);
+  if (!do_hash)
+    for (size_t i = 0; i < m.digests.size(); i += 2) memcpy(hr.hash + 32 * (size_t)m.digests[i + 1], hr.hash + 32 * (size_t)m.digests[i], 32);
+  if (m.gs0 < n.n_groups && m.g_hi > m.g_lo) {
+    const std::vector<kr_group_result> old(hr.groups + m.g_lo, hr.groups + m.g_hi);
+    for (uint32_t k = 0; k < n.n_groups - m.gs0; k++)
+      if (m.gsrc[k] != KR_EMPTY32) hr.groups[m.gs0 + k] = old[m.gsrc[k] - m.g_lo];
   }
+  e->map_pending = false;
   e->ran_inc = true;
   *done_inc = true;
   return KR_OK;
@@ -1395,7 +1395,7 @@ int run_pass(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile) {
   e->last_flags = f;
   new_pull_epoch(e);
   // (the list moves with a group count, an option or a new layout, when a full pass follows, and with the RayClusters an incremental
-  // epoch of KR_OPT_CLUSTER_CREATES appended)
+  // epoch created)
   if (e->lg_stale) if (int rc = upload_lg(e)) return rc;
   if (e->inc_valid && !e->no_incr && memcmp(&e->inc_flags, &f, sizeof f) == 0) {
     if (profile) CK(cudaEventRecord(e->ev_a, e->sm));
@@ -1602,17 +1602,17 @@ ObjDiffArgs object_diff_args(const kr_engine *e, const uint8_t *stage, const siz
   return oa;
 }
 
-// KR_OPT_CLUSTER_DELETES, an object commit whose part renumbered the RayClusters, or moved a row count after such a commit in the same
-// epoch (on the copy stream, before its diff): a row map the resident state follows (`ok`, rec.map) is checked against what the pass
-// can move, renumbers the pending spec rows, travels to the device and sets up the diff (oa).  Otherwise `voided`: the resident state
-// does not follow this epoch, and the caller drops it once the diff has copied the object part into place (the next pass is a full
-// one, which re-hashes every spec).
+// An object commit whose part created or renumbered RayClusters, or moved a row count after a renumbering of the same epoch (on the
+// copy stream, before its diff): a row map the resident state follows (`ok`, rec.map) is checked against what the pass can move,
+// queues the created RayClusters' specs and renumbers the pending spec rows, travels to the device and, when rows were renumbered,
+// sets up the diff (oa).  Otherwise `voided`: the resident state does not follow this epoch, and the caller drops it once the diff
+// has copied the object part into place (the next pass is a full one, which re-hashes every spec).
 int commit_map(kr_engine *e, bool ok, ObjDiffArgs &oa, bool &voided) {
   const CommitRecord::RowMap &m = e->rec.map;
   const kr_sizes &n = e->sizes;
-  // (a large RayCluster's region and tiles do not move with it; a second renumbering in one epoch would need the two maps composed;
-  // the old groups the gather reads are staged in the incremental staging buffer, which the pass fills only later)
-  ok = ok && !e->map_pending && 36 * (size_t)(m.g_hi - m.g_lo) <= e->inc_stage.cap;
+  // (a large RayCluster's region and tiles do not move with it; the old groups the gather reads are staged in the incremental staging
+  // buffer, which the pass fills only later)
+  ok = ok && 36 * (size_t)(m.g_hi - m.g_lo) <= e->inc_stage.cap;
   for (uint32_t o : m.gone) ok = ok && !std::binary_search(e->large_rows.begin(), e->large_rows.end(), o);
   if (!ok) {  // (the record took the new rows' ranges as the digests' ones)
     e->rec.hash_dirty = true;
@@ -1642,17 +1642,19 @@ int commit_map(kr_engine *e, bool ok, ObjDiffArgs &oa, bool &voided) {
   CK(cudaEventRecord(e->mp.ev, e->scopy));
   e->mp.busy = true;
   e->h2d_accum += bytes;
-  auto dev = [&](MapList i) { return reinterpret_cast<const uint32_t *>(e->mp.d + e->mp_at[i]); };
-  oa.map_pass = 1;
-  oa.init = dev(MP_INIT); oa.n_init = (uint32_t)m.init.size();
-  oa.gsrc = dev(MP_GSRC); oa.wsrc = dev(MP_WSRC);
-  for (int k = 0, i = 0; i < kNumCols - 1; i++) {
-    const int d = kCols[i].dim;
-    if (d == D_PODS) continue;
-    oa.map_kind[k] = d == D_CLUSTERS ? KR_MAP_CLUSTER : d == D_GROUPS ? KR_MAP_GROUP : d == D_WTD ? KR_MAP_NAME : 0;
-    oa.shift_from[k] = d == D_GROUPS ? m.gs0 : d == D_WTD ? m.ws0 : 0u;
-    if (i == kGroupOffCol || i == kWtdOffCol) oa.cls[k] = KR_OC_COPY;  // (the offsets follow from the counts: groups and names stay in row order)
-    k++;
+  if (!m.gone.empty()) {  // (without gone rows no resident row shifted: the diff classes the rows past the resident ones as new by itself)
+    auto dev = [&](MapList i) { return reinterpret_cast<const uint32_t *>(e->mp.d + e->mp_at[i]); };
+    oa.map_pass = 1;
+    oa.init = dev(MP_INIT); oa.n_init = (uint32_t)m.init.size();
+    oa.gsrc = dev(MP_GSRC); oa.wsrc = dev(MP_WSRC);
+    for (int k = 0, i = 0; i < kNumCols - 1; i++) {
+      const int d = kCols[i].dim;
+      if (d == D_PODS) continue;
+      oa.map_kind[k] = d == D_CLUSTERS ? KR_MAP_CLUSTER : d == D_GROUPS ? KR_MAP_GROUP : d == D_WTD ? KR_MAP_NAME : 0;
+      oa.shift_from[k] = d == D_GROUPS ? m.gs0 : d == D_WTD ? m.ws0 : 0u;
+      if (i == kGroupOffCol || i == kWtdOffCol) oa.cls[k] = KR_OC_COPY;  // (the offsets follow from the counts: groups and names stay in row order)
+      k++;
+    }
   }
   if (m.names_moved) e->rec.wtd_rebuild = true;
   e->map_pending = true;
@@ -1877,8 +1879,8 @@ int kr_engine_create(const kr_config *cfg, kr_engine **out) {
     if (cudaMalloc((void **)&e->d_obj_stage, objs) != cudaSuccess) return bail(KR_E_CUDA);
     e->obj_stage_cap = objs;
     if (e->inc_stage.reserve(inc_stage_layout(cfg->max_clusters, cfg->max_groups).total, 0) != cudaSuccess) return bail(KR_E_CUDA);
-    // the largest row map of KR_OPT_CLUSTER_DELETES: gone / init / digests of kMapMax rows, every group and name shifted
-    if (e->mp.reserve(4 * (4 * (size_t)kMapMax + cfg->max_groups + cfg->max_wtd) + MP_LISTS * 16, 0) != cudaSuccess) return bail(KR_E_CUDA);
+    // the largest row map: gone / digests of kMapMax rows, every RayCluster created, every group and name shifted
+    if (e->mp.reserve(4 * (3 * (size_t)kMapMax + cfg->max_clusters + cfg->max_groups + cfg->max_wtd) + MP_LISTS * 16, 0) != cudaSuccess) return bail(KR_E_CUDA);
     const size_t chg = std::max<size_t>(1024, (size_t)cfg->max_clusters);
     if (cudaHostAlloc((void **)&e->h_changed, 4 * chg, cudaHostAllocDefault) != cudaSuccess) return bail(KR_E_CUDA);
     e->h_changed_cap = chg;
@@ -1936,19 +1938,15 @@ int kr_snapshot_begin(kr_engine *e, const kr_sizes *sizes, kr_snapshot_bufs *out
     e->gvalid = false;
     // The resident state of the incremental path survives new live counts under a fixed layout as long as the object tables keep
     // their shape: pod rows appended (they arrive as committed rows), head-aux rows come and go, the JSON arena grows; with
-    // KR_OPT_WTD_EDITS workersToDelete lists grow and shrink as well (the name table is sized for the capacity); with
-    // KR_OPT_CLUSTER_CREATES RayClusters are appended (with their groups and names: the object diff checks that every resident row
-    // stayed) while the bucket arena holds them at the current stride, and RayJobs come and go.
-    const bool grow = creates_on(e) && sizes->n_clusters >= e->sizes.n_clusters && sizes->n_groups >= e->sizes.n_groups && sizes->n_wtd >= e->sizes.n_wtd &&
-                      (size_t)sizes->n_clusters * e->bstride <= e->sl.bucket_entries;
-    // With KR_OPT_CLUSTER_DELETES the three counts may also shrink (RayClusters deleted by swap-remove: the object commit's row map
-    // checks the rest), and with both options each may move either way.
+    // KR_OPT_WTD_EDITS workersToDelete lists grow and shrink as well while the RayClusters and groups stay (the name table is sized
+    // for the capacity).  The RayCluster, group and name counts may each grow with KR_OPT_CLUSTER_CREATES (RayClusters created, with
+    // their groups and names) while the bucket arena holds the RayClusters at the current stride, with which RayJobs come and go as
+    // well, and shrink with KR_OPT_CLUSTER_DELETES (RayClusters deleted by swap-remove); the object commit's row map checks the rest.
     const bool fits = (size_t)sizes->n_clusters * e->bstride <= e->sl.bucket_entries;
     auto moves_ok = [&](uint32_t now, uint32_t was) { return now == was || (now < was ? deletes_on(e) : creates_on(e) && fits); };
-    const bool renumber = deletes_on(e) && moves_ok(sizes->n_clusters, e->sizes.n_clusters) && moves_ok(sizes->n_groups, e->sizes.n_groups) &&
-                          moves_ok(sizes->n_wtd, e->sizes.n_wtd);
-    const bool keep = e->inc_valid && e->fixed_layout && ((sizes->n_clusters == e->sizes.n_clusters && sizes->n_groups == e->sizes.n_groups) || grow || renumber) &&
-                      (sizes->n_wtd == e->sizes.n_wtd || e->wtd_edits || grow || renumber) && (sizes->n_jobs == e->sizes.n_jobs || creates_on(e)) &&
+    const bool same_groups = sizes->n_clusters == e->sizes.n_clusters && sizes->n_groups == e->sizes.n_groups;
+    const bool keep = e->inc_valid && e->fixed_layout && moves_ok(sizes->n_clusters, e->sizes.n_clusters) && moves_ok(sizes->n_groups, e->sizes.n_groups) &&
+                      (moves_ok(sizes->n_wtd, e->sizes.n_wtd) || (e->wtd_edits && same_groups)) && (sizes->n_jobs == e->sizes.n_jobs || creates_on(e)) &&
                       sizes->n_pods >= e->sizes.n_pods;
     if (!e->fixed_layout) { e->committed_full = false; e->inc_zero_needed = true; }
     // (the next pass is a full one, which hashes every message: listed rows may not exist any more)
@@ -2014,21 +2012,17 @@ int kr_snapshot_commit_parts(kr_engine *e, uint32_t parts) {
   ObjDiffArgs oa = object_diff_args(e, e->d_obj_stage, at, cnt, nullptr);  // (before the record moves on)
   if (e->order_pending) { CK(cudaEventSynchronize(e->ev_order)); e->order_pending = false; }  // a previous upload may still be reading h_order
   if (int rc = begin_commit(e)) return rc;
-  const bool had_map = e->map_pending;
-  const CommitRecord::Moved moved = e->rec.commit_whole(hb, n, parts, e->wtd_edits, creates_on(e), deletes_on(e), e->wide_on, e->inc_n_clusters);
+  const bool renumbered = e->map_pending && !e->rec.map.gone.empty();  // (by an earlier object commit of this epoch)
+  const CommitRecord::Moved moved = e->rec.commit_whole(hb, n, parts, e->wtd_edits, creates_on(e), deletes_on(e), e->inc_n_clusters);
   if (moved.shape) e->gvalid = false;  // launch shape / pipeline depend on it
-  // KR_OPT_CLUSTER_DELETES: the object part renumbered the RayClusters, or moved a row count after a renumbering of this epoch (the
-  // pending map would no longer describe the rows: not composed)
+  // The object part created or renumbered RayClusters, or moved a row count after a renumbering of this epoch.  A pending renumbering
+  // is not composed with either: its map would no longer describe the rows.  (Created RayClusters after created ones: the new map
+  // lists them all.)
   bool voided = false;
-  const bool recounted = had_map && (parts & KR_PART_OBJECTS) &&
+  const bool recounted = renumbered && (parts & KR_PART_OBJECTS) &&
                          (n.n_clusters != e->map_sizes.n_clusters || n.n_groups != e->map_sizes.n_groups || n.n_wtd != e->map_sizes.n_wtd);
   if (moved.map != 0 || recounted) {
-    if (int rc = commit_map(e, moved.map == 1 && stage_objects, oa, voided)) return rc;
-  }
-  if (moved.appended < n.n_clusters) {  // KR_OPT_CLUSTER_CREATES: the next pass hashes the new RayClusters' specs (committed as spec rows)
-    if (e->spec_stamp.size() < n.n_clusters) e->spec_stamp.resize(n.n_clusters, 0u);
-    for (uint32_t c = moved.appended; c < n.n_clusters; c++)
-      if (e->spec_stamp[c] != e->spec_epoch) { e->spec_stamp[c] = e->spec_epoch; e->spec_pending.push_back(c); }
+    if (int rc = commit_map(e, moved.map == 1 && stage_objects && !renumbered, oa, voided)) return rc;
   }
   if (moved.wide && e->wide_on) e->lg_stale = true;  // a different wide set is a different list, and grid, of the per-cluster kernels
   if (parts & KR_PART_COLUMNS) e->inc_valid = false;  // pod columns uploaded wholesale: the resident buckets no longer describe them

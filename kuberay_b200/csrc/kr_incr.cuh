@@ -385,28 +385,46 @@ __global__ void __launch_bounds__(256) k_inc_admit(SnapDev s, ScratchDev sc, Res
   }
 }
 
-// ------------------------------------------------------------------------------------------------ RayCluster creation
-// KR_OPT_CLUSTER_CREATES: an epoch whose object commit appended RayClusters [c0, c1) after the last resident row (every resident
-// RayCluster, group and workersToDelete name kept its row; k_inc_objects copied the new rows into place and marked the new RayClusters
-// dirty) brings them into the resident state in front of k_inc_admit:
-//   k_inc_orphan_adopt     touches every resident Pod row labelled for one of them — an orphan until now, or a Pod of an older
-//                          RayCluster of the same key (the lowest row keeps such a key) — while the cluster table does not hold them
-//                          yet: inc_touch takes an orphan out of the orphan count, and k_inc_admit appends it to its new bucket.  The
-//                          host launches it only when the last pass counted orphans;
-//   k_inc_clusters_insert  inserts them into the cluster table (k_build_tables' per-cluster part) and initialises every per-cluster
-//                          cell a decide warp or k_decide_large reads: rows past the previous count may hold values of an earlier,
-//                          larger fleet.  With `names`, it also inserts their groups' workersToDelete names into the name table and
-//                          its Bloom bitmap (k_build_tables' group part) and sets their resolutions to -1;
-//   k_inc_wtd_resolve      (first_name = the first new name; only when there are new names) then probes every pod row once: a new
-//                          name may name any resident Pod.  It resolves the new names and touches the rows that hit one.  A row of
-//                          a new RayCluster was an orphan and k_inc_orphan_adopt touched it already; any other resident row still
-//                          probes to the RayCluster that holds it (the lowest row keeps a duplicate key).
-// (An epoch whose object commit also changed an existing list, KR_OPT_WTD_EDITS, rebuilds the whole name table instead: `names` = 0.)
-// Both take the RayClusters as entries [c0, c1) of the ascending row list `rows` (nullptr: rows c0 .. c1 - 1).
-__global__ void __launch_bounds__(256) k_inc_clusters_insert(SnapDev s, ScratchDev sc, ResDev r, const uint32_t *rows, uint32_t c0, uint32_t c1, int names) {
-  const uint32_t i = c0 + blockIdx.x * blockDim.x + threadIdx.x;
-  if (i >= c1 || __ldcg(&sc.inc[KR_INC_STRUCTURAL])) return;
-  const uint32_t c = rows ? rows[i] : i;
+// ------------------------------------------------------------------------------------------------ RayCluster creation and deletion
+// KR_OPT_CLUSTER_CREATES / KR_OPT_CLUSTER_DELETES: an epoch whose object commit brought RayClusters into the fleet or renumbered
+// them by swap-remove carries the commit's row map: the old rows `gone` that no RayCluster keeps (deleted, or moved to a row a
+// deleted one vacated) and the new rows `init` that were created or moved (k_inc_objects copied them into place and marked them
+// dirty).  RayClusters appended after the last resident row are the map without gone rows: every resident RayCluster, group and
+// workersToDelete name kept its row, and only the steps that read `init` run.  In front of k_inc_admit, each step launched only
+// when its list is not empty:
+//   k_inc_digest_move          first, ahead of the hash stream: the digests of moved RayClusters whose spec range stayed;
+//   k_inc_clusters_release     one warp per gone row, while the cluster table still holds the old rows: touches every Pod in its
+//                              bucket (k_inc_admit re-matches it against the new table: a Pod of a deleted RayCluster becomes an
+//                              orphan, one of a moved RayCluster joins its new bucket) and takes the row's share out of the running
+//                              totals, the way the incremental decide counts it (its act_cnt, its groups' n_create);
+//   (the rebuild of the workersToDelete name table, when a resident name shifted, vanished or changed)
+//   k_inc_orphan_adopt         touches every resident Pod row labelled for an `init` RayCluster — an orphan until now, or a Pod of an
+//                              older RayCluster of the same key (the lowest row keeps such a key) — while the cluster table does not
+//                              hold them yet: inc_touch takes an orphan out of the orphan count, and k_inc_admit appends it to its new
+//                              bucket.  The host launches it only when RayClusters were created and the last pass counted orphans;
+//   k_inc_clusters_translate   one CTA: a touched row whose old RayCluster is gone had no RayCluster (its stale record went with the
+//                              bucket), and the dirty list drops the old rows at or past the new count (every entry below it names a
+//                              RayCluster of the new numbering: a kept one, or one that k_inc_clusters_insert marks anyway);
+//   k_inc_clusters_rekey       the cluster table cleared and rebuilt from every new row (cl_slots, cl_rec and cl_in: the offsets of
+//                              the shifted groups), the lowest row keeping a duplicate key;
+//   k_inc_groups_gather        the kept RayClusters' group records and create offsets from the first shifted group on, out of a
+//                              copy of the old ones (the ranges overlap);
+//   k_inc_clusters_insert      inserts the `init` RayClusters into the cluster table (k_build_tables' per-cluster part) and
+//                              initialises every per-cluster cell a decide warp or k_decide_large reads: a moved or created
+//                              RayCluster starts from an empty bucket, and rows past the previous count may hold values of an earlier,
+//                              larger fleet.  With `names` (new names after the resident ones, the name table not rebuilt), it also
+//                              inserts their groups' workersToDelete names into the name table and its Bloom bitmap (k_build_tables'
+//                              group part) and sets their resolutions to -1;
+//   k_inc_wtd_resolve          (first_name = the first new name; only with `names`) then probes every pod row once: a new name may
+//                              name any resident Pod.  It resolves the new names and touches the rows that hit one.  A row of a new
+//                              RayCluster was an orphan and k_inc_orphan_adopt touched it already; any other resident row still
+//                              probes to the RayCluster that holds it (the lowest row keeps a duplicate key).
+// Places in the action list and create arena that a gone RayCluster held are abandoned until the next full pass.
+// k_inc_clusters_insert and k_inc_orphan_adopt take the `init` RayClusters as the ascending row list `rows` of n entries.
+__global__ void __launch_bounds__(256) k_inc_clusters_insert(SnapDev s, ScratchDev sc, ResDev r, const uint32_t *rows, uint32_t n, int names) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n || __ldcg(&sc.inc[KR_INC_STRUCTURAL])) return;
+  const uint32_t c = rows[i];
   cl_insert_cluster(s, sc, c);
   sc.cl_dyn[c] = make_uint4(0u, 0u, 0u, 0u);  // no pod yet (k_inc_admit appends them), no first head, not "lost a row"
   sc.act_res[c] = 0u; sc.cre_res[c] = 0u;     // no reserved places: the decide takes new ones at the cursors
@@ -428,15 +446,15 @@ __global__ void __launch_bounds__(256) k_inc_clusters_insert(SnapDev s, ScratchD
 // Grid-stride over the resident pod rows, 8 bytes per row (namespace, ray.io/cluster), against a Bloom bitmap of the new RayClusters'
 // keys and, behind it, an open-addressed table of their rows (both built per CTA in shared memory: 4 * (slot_mask + 1) bytes of slots
 // after (bloom_mask + 1) / 8 bytes of bits).
-__global__ void __launch_bounds__(256) k_inc_orphan_adopt(SnapDev s, ScratchDev sc, ResDev r, const uint32_t *rows, uint32_t c0, uint32_t c1,
-                                                          uint32_t bloom_mask, uint32_t slot_mask, uint32_t n_resident) {
+__global__ void __launch_bounds__(256) k_inc_orphan_adopt(SnapDev s, ScratchDev sc, ResDev r, const uint32_t *rows, uint32_t n, uint32_t bloom_mask,
+                                                          uint32_t slot_mask, uint32_t n_resident) {
   extern __shared__ uint32_t sm_adopt[];
   uint32_t *bits = sm_adopt, *slots = sm_adopt + ((bloom_mask + 1) >> 5);
   for (uint32_t i = threadIdx.x; i < (bloom_mask + 1) >> 5; i += blockDim.x) bits[i] = 0u;
   for (uint32_t i = threadIdx.x; i <= slot_mask; i += blockDim.x) slots[i] = KR_EMPTY32;
   __syncthreads();
-  for (uint32_t i = c0 + threadIdx.x; i < c1; i += blockDim.x) {
-    const uint32_t c = rows ? rows[i] : i;
+  for (uint32_t i = threadIdx.x; i < n; i += blockDim.x) {
+    const uint32_t c = rows[i];
     const uint32_t ns = s.c_ns_id[c], nm = s.c_name_id[c];
     if (nm == 0) continue;  // (cl_probe matches no pod against an absent name)
     const uint32_t hk = hash_pair(ns, nm), h2 = bloom2(hk);
@@ -462,25 +480,6 @@ __global__ void __launch_bounds__(256) k_inc_orphan_adopt(SnapDev s, ScratchDev 
   }
 }
 
-// ------------------------------------------------------------------------------------------------ RayCluster deletion
-// KR_OPT_CLUSTER_DELETES: an epoch whose object commit renumbered the RayClusters by swap-remove (the commit's row map: the old
-// rows `gone` that no RayCluster keeps — deleted, or moved to a row a deleted one vacated — and the new rows `init` that were moved
-// or created) brings the resident state into the new numbering in front of k_inc_admit:
-//   k_inc_digest_move          first, ahead of the hash stream: the digests of moved RayClusters whose spec range stayed;
-//   k_inc_clusters_release     one warp per gone row, while the cluster table still holds the old rows: touches every Pod in its
-//                              bucket (k_inc_admit re-matches it against the new table: a Pod of a deleted RayCluster becomes an
-//                              orphan, one of a moved RayCluster joins its new bucket) and takes the row's share out of the running
-//                              totals, the way the incremental decide counts it (its act_cnt, its groups' n_create);
-//   (the rebuild of the workersToDelete name table, and k_inc_orphan_adopt for the created RayClusters, still against the old table)
-//   k_inc_clusters_translate   one CTA: a touched row whose old RayCluster is gone had no RayCluster (its stale record went with the
-//                              bucket), and the dirty list drops the old rows at or past the new count (every entry below it names a
-//                              RayCluster of the new numbering: a kept one, or one that k_inc_clusters_insert marks anyway);
-//   k_inc_clusters_rekey       the cluster table cleared and rebuilt from every new row (cl_slots, cl_rec and cl_in: the offsets of
-//                              the shifted groups), the lowest row keeping a duplicate key;
-//   k_inc_groups_gather        the kept RayClusters' group records and create offsets from the first shifted group on, out of a
-//                              copy of the old ones (the ranges overlap);
-//   k_inc_clusters_insert      (rows = init) a moved or created RayCluster starts from an empty bucket at its new row, as a created one.
-// Places in the action list and create arena that a gone RayCluster held are abandoned until the next full pass.
 __global__ void __launch_bounds__(256) k_inc_digest_move(const uint32_t *__restrict__ pairs, uint32_t n, char *hash) {
   const uint32_t t = blockIdx.x * blockDim.x + threadIdx.x;
   if (t >= 2 * n) return;

@@ -12,7 +12,7 @@ import copy
 import numpy as np
 import pytest
 
-from harness import PACKER_CAPS, POD_COLS, Driver, Mirror, device_incremental, events, flip_ready, members, objects, packer_check
+from harness import PACKER_CAPS, POD_COLS, Driver, Mirror, device_incremental, events, flip_ready, members, objects, packer_check, with_wtd_lists
 from kuberay_b200 import abi, synthetic
 from kuberay_b200.packer import GroupPacker, Packer
 from kuberay_b200.snapshot import Snapshot
@@ -202,13 +202,19 @@ def test_wide_with_option_large_and_overflow(oracle_mod):
             dr.close()
 
 
-@pytest.mark.parametrize("other", ["pod_events", "spec_rows", "wtd_edits", "job_created", "job_deleted"])
+@pytest.mark.parametrize("other", ["pod_events", "spec_rows", "wtd_edits", "job_created", "job_deleted", "two_commits", "new_names"])
 def test_creation_with_other_events(other, oracle_mod):
     full, flags = _fleet(205, seed=51, jobs=True, wtd_group_frac=0.3)
+    if other == "new_names":  # two created RayClusters name resident Pods of theirs (orphans until now) in workersToDelete
+        lists = [full.w_name_id[int(o):int(o + n)].tolist() for o, n in zip(full.g_wtd_off, full.g_wtd_cnt)]
+        for c in (201, 203):
+            lists[int(full.c_group_off[c])] += full.p_name_id[members(full, c)[1:3]].tolist()
+        full = with_wtd_lists(full, lists)
     nj = full.dims["jobs"]
     assert nj >= 2
     jobs_before = np.arange(nj - 1) if other == "job_created" else None
-    before = _prefix(full, 200, jobs=jobs_before)
+    before = _prefix(full, 200, jobs=jobs_before, free_pods=other != "new_names")
+    assert before.dims["wtd"] < full.dims["wtd"] or other != "new_names"
     dr = _driver(before, flags, full, wtd_edits=other == "wtd_edits")
     try:
         _check(dr, oracle_mod, expect_incremental=False)
@@ -227,8 +233,13 @@ def test_creation_with_other_events(other, oracle_mod):
             new.json[int(new.c_json_off[c]):int(new.c_json_off[c] + new.c_json_len[c])] = np.frombuffer(bytes(body), np.uint8)
             np.copyto(dr.views["json"][:new.dims["json"]], new.json)
             dr.eng.commit_spec_rows(np.array([c], dtype=np.uint32))
+        if other == "two_commits":  # two object commits of one epoch that both append RayClusters
+            _create(dr, _prefix(full, 202))
         _create(dr, new)
-        _check(dr, oracle_mod, expect_incremental=True)
+        _, names = _check(dr, oracle_mod, expect_incremental=True, profiled=True)
+        assert "k_inc_clusters_insert" in names, names
+        if other == "new_names":  # the new names are inserted and resolved; the name table is not rebuilt
+            assert "k_inc_wtd_resolve" in names and "k_inc_wtd_clear" not in names, names
     finally:
         dr.close()
 
