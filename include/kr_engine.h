@@ -540,9 +540,9 @@ int kr_last_profile(kr_engine *e, kr_profile *prof);
  *   same pointers, and what is resident in HBM stays valid across begins.  A head Pod appearing or going, or a Pod appended after
  *   the last row, is still an incremental epoch: kr_snapshot_begin(new counts) + KR_PART_OBJECTS + kr_snapshot_commit_pod_rows/
  *   _values.  So are workersToDelete lists that grow or shrink, with KR_OPT_WTD_EDITS, and RayClusters appended after the last row
- *   or RayJobs created or deleted, with KR_OPT_CLUSTER_CREATES, and RayClusters deleted by swap-remove, with KR_OPT_CLUSTER_DELETES.
- *   Any other change of a row count (a worker group added to a RayCluster, a deletion without that option) makes the next pass a
- *   full one. */
+ *   or RayJobs created or deleted, with KR_OPT_CLUSTER_CREATES, RayClusters deleted by swap-remove, with KR_OPT_CLUSTER_DELETES,
+ *   and worker groups added to or removed from a RayCluster, with KR_OPT_GROUP_EDITS.  Any other change of a row count (one of these
+ *   without its option) makes the next pass a full one. */
 enum {
   KR_OPT_FIXED_LAYOUT = 1,
   KR_OPT_INCREMENTAL = 2,  /* 1 (default): passes after a full bucket-pipeline pass are incremental on the device whenever the commits in
@@ -588,24 +588,25 @@ enum {
                               counts), the object part (KR_PART_OBJECTS), then the new RayClusters' specs with
                               kr_snapshot_commit_spec_rows.  The next pass hashes only those specs, inserts the new RayClusters into
                               the resident tables, moves the resident Pods labelled for them out of the orphans and into their buckets,
-                              and returns them among changed_clusters.  A RayCluster deleted, a worker group added to an existing one,
-                              fewer RayClusters than before, or a RayCluster the resident state cannot hold (more Pods than its bucket
+                              and returns them among changed_clusters.  A RayCluster deleted, a worker group added to an existing one
+                              (unless KR_OPT_GROUP_EDITS), fewer RayClusters than before, or a RayCluster the resident state cannot hold (more Pods than its bucket
                               without KR_OPT_LARGE_CLUSTERS, more than 32 worker groups without KR_OPT_WIDE_CLUSTERS) still takes the
                               full pass.  Results are the same as with 0 (the default: every such event makes the next pass a full
                               one).  May be set at any time; read at each kr_snapshot_begin and object commit.  No effect without
                               KR_OPT_FIXED_LAYOUT.  The native packer's flush takes this path by itself when the engine has the option
                               and a flush only appended RayClusters or created and deleted RayJobs.  Deleting a RayCluster is
                               KR_OPT_CLUSTER_DELETES. */
-  KR_OPT_CLUSTER_DELETES = 10 /* 1, together with KR_OPT_FIXED_LAYOUT: RayClusters deleted by swap-remove keep the incremental epoch:
+  KR_OPT_CLUSTER_DELETES = 10, /* 1, together with KR_OPT_FIXED_LAYOUT: RayClusters deleted by swap-remove keep the incremental epoch:
                               kr_snapshot_begin(new counts), then the object part (KR_PART_OBJECTS), where every surviving RayCluster
                               either keeps its row or moves from a row at or past the new n_clusters into a row a deleted RayCluster
-                              vacated, keeps its worker-group count, and groups and workersToDelete names stay in row order.  With
+                              vacated, keeps its worker-group count (unless KR_OPT_GROUP_EDITS), and groups and workersToDelete names
+                              stay in row order.  With
                               KR_OPT_CLUSTER_CREATES the same epoch may also create RayClusters, in vacated rows or after the last one
                               (their specs then follow with kr_snapshot_commit_spec_rows).  The next pass releases the deleted
                               RayClusters' Pods (orphans from then on), brings every moved RayCluster's Pods to its new row, moves its
                               digest when its spec range stayed, shifts the per-group results, and re-decides only the moved and created
                               RayClusters, which it returns among changed_clusters.  Still full passes: another renumbering, a surviving
-                              RayCluster whose group count changed, a deleted or moved key that another row also holds, more than 4 096
+                              RayCluster whose group count changed (without KR_OPT_GROUP_EDITS), a deleted or moved key that another row also holds, more than 4 096
                               RayClusters deleted, moved or created at once, a deleted or moved RayCluster that is large
                               (KR_OPT_LARGE_CLUSTERS: its region does not move), and, within one epoch, a renumbering after an object
                               commit that appended RayClusters, or any object commit after a renumbering that changes a row count or
@@ -614,6 +615,26 @@ enum {
                               at any time; read at each kr_snapshot_begin and object commit.  No effect without KR_OPT_FIXED_LAYOUT.
                               The native packer's flush takes this path by itself when the engine has the option (the specs it placed
                               travel as spec rows unless it compacted the JSON arena). */
+  KR_OPT_GROUP_EDITS = 11     /* 1, together with KR_OPT_FIXED_LAYOUT: a RayCluster whose list of worker groups changed (groups appended,
+                              as a RayService in-place update does, removed, renamed or reordered) keeps the incremental epoch:
+                              kr_snapshot_begin(new counts; n_groups and n_wtd may move either way), then the object part
+                              (KR_PART_OBJECTS), with the RayCluster's spec, when it was re-emitted, as a spec row before or after it.
+                              The RayCluster is released and initialised again in its own row: the next pass touches its Pods and matches
+                              them against its new groups (a Pod of a removed group stays among its Pods, in no group), shifts the
+                              per-group results of the RayClusters after it, keeps its digest unless its spec range moved, and
+                              re-decides it, returning it among changed_clusters with the RayClusters whose Pods a rebuilt
+                              workersToDelete name table touched.  With KR_OPT_CLUSTER_DELETES a RayCluster moved by swap-remove may
+                              change its group count in the same epoch, and with KR_OPT_CLUSTER_CREATES the epoch may create
+                              RayClusters as well.  Still full passes: a regrouped RayCluster that is large (KR_OPT_LARGE_CLUSTERS: its
+                              region would have to be initialised again in place; left open), one of more than 32 worker groups without
+                              KR_OPT_WIDE_CLUSTERS, more than 4 096 RayClusters deleted, moved, created or regrouped at once, the rules
+                              of KR_OPT_CLUSTER_DELETES for two object commits in one epoch, and group edits committed with
+                              kr_snapshot_commit_object_rows (a changed group count falls back to the whole object part; a renamed
+                              group there is structural).  Results are the same as with 0 (the default: every such edit makes the
+                              next pass a full one).  May be set at any time; read at each kr_snapshot_begin and object commit (the
+                              first object commit with it on records the group names, the next ones compare against them).  No effect
+                              without KR_OPT_FIXED_LAYOUT.  The native packer's flush takes this path by itself when the engine has the
+                              option: the regrouped RayClusters' specs travel as spec rows. */
 };
 enum { KR_LARGE_MAX_PODS = 8192 };  /* largest RayCluster KR_OPT_LARGE_CLUSTERS keeps on the bucket pipeline */
 int kr_engine_set_option(kr_engine *e, uint32_t option, uint64_t value);

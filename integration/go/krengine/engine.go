@@ -150,6 +150,10 @@ const (
 	// KR_OPT_FIXED_LAYOUT; recommended for fleets that delete RayClusters, such as RayJob fleets with shutdownAfterJobFinishes;
 	// read at each Begin and object commit).
 	OptClusterDeletes = uint32(C.KR_OPT_CLUSTER_DELETES)
+	// OptGroupEdits is KR_OPT_GROUP_EDITS (1: a RayCluster whose worker groups were appended, removed, renamed or reordered keeps
+	// incremental epochs; only under KR_OPT_FIXED_LAYOUT; recommended for RayService fleets, whose in-place updates append worker
+	// groups; read at each Begin and object commit).
+	OptGroupEdits = uint32(C.KR_OPT_GROUP_EDITS)
 )
 
 // SetOption: KR_OPT_FIXED_LAYOUT (before the first Begin), KR_OPT_INCREMENTAL, KR_OPT_LARGE_CLUSTERS (1: RayClusters of 257 to
@@ -161,7 +165,8 @@ const (
 // re-emitted specs with CommitSpecRows instead of the whole JSON arena and reports PackSpecRows), KR_OPT_CLUSTER_CREATES (1, with
 // KR_OPT_FIXED_LAYOUT: RayClusters appended after the last row and RayJobs created or deleted keep incremental epochs; read at each
 // Begin and object commit), KR_OPT_CLUSTER_DELETES (1, with KR_OPT_FIXED_LAYOUT: RayClusters deleted by swap-remove keep incremental
-// epochs; read at each Begin and object commit).  For a Packer, call it on Packer.Engine().
+// epochs; read at each Begin and object commit), KR_OPT_GROUP_EDITS (1, with KR_OPT_FIXED_LAYOUT: a RayCluster whose list of worker
+// groups changed keeps incremental epochs; read at each Begin and object commit).  For a Packer, call it on Packer.Engine().
 func (e *Engine) SetOption(option uint32, value uint64) error {
 	if rc := C.kr_engine_set_option(e.h, C.uint32_t(option), C.uint64_t(value)); rc != C.KR_OK {
 		return e.err(rc)

@@ -39,8 +39,8 @@ constexpr size_t kAlign = 256;
 // most RayClusters one incremental epoch brings in while there are orphans (k_inc_orphan_adopt: 16 Bloom bits and two 4-byte table
 // slots per RayCluster in shared memory, 40 KB); more take the full pass
 constexpr uint32_t kAdoptMax = 4096;
-// most RayClusters one incremental epoch that renumbers them (KR_OPT_CLUSTER_DELETES) deletes, moves and creates together; more take
-// the full pass
+// most RayClusters one incremental epoch that renumbers them (KR_OPT_CLUSTER_DELETES) or regroups them (KR_OPT_GROUP_EDITS) deletes,
+// moves, creates and regroups together; more take the full pass
 constexpr uint32_t kMapMax = 4096;
 enum MapList { MP_GONE, MP_INIT, MP_DIGESTS, MP_GSRC, MP_WSRC, MP_LISTS };  // the lists of a row map on the device, in this order
 inline size_t align_up(size_t x, size_t a = kAlign) { return (x + a - 1) / a * a; }
@@ -121,7 +121,8 @@ static_assert(kCols[kGroupOffCol].dim == D_CLUSTERS && kCols[kGroupOffCol + 1].d
 static_assert(kCols[kWtdCntCol].dim == D_GROUPS && kCols[kWtdNameCol].dim == D_WTD && kCols[kWtdNameCol + 1].dim == D_PODS, "workersToDelete column indices");
 // With KR_OPT_CLUSTER_CREATES a row past the resident rows of a RayCluster / group / workersToDelete column belongs to a RayCluster
 // the epoch appended (`appended`): it marks that RayCluster dirty and refreshes its input record (a group row: its RayCluster's) instead
-// of making the epoch structural.
+// of making the epoch structural.  A row map (KR_OPT_CLUSTER_DELETES, KR_OPT_GROUP_EDITS) classes the rows of its moved, created and
+// regrouped RayClusters the same way.
 uint8_t obj_class(int col, bool wtd_edits, bool appended = false) {
   if (appended && kObjClass[col] == KR_OC_STRUCT)
     return kCols[col].dim == D_CLUSTERS ? KR_OC_CLUSTER : kCols[col].dim == D_GROUPS ? KR_OC_GROUP : KR_OC_COPY;
@@ -142,14 +143,16 @@ struct CommitRecord {
     uint32_t ns, name, wtd_off;    // key and first workersToDelete name: whole with the object part
   };
   std::vector<Row> rows;             // per RayCluster row (sized, zero-filled, by every whole commit)
-  // KR_OPT_CLUSTER_CREATES / KR_OPT_CLUSTER_DELETES: the RayCluster rows that entered the fleet since the last pass and how the last
-  // object commit renumbered the others (swap-remove), for the next pass.  Without gone rows: RayClusters appended after the resident ones.
+  // KR_OPT_CLUSTER_CREATES / KR_OPT_CLUSTER_DELETES / KR_OPT_GROUP_EDITS: the RayCluster rows that entered the fleet since the last
+  // pass, how the last object commit renumbered the others (swap-remove) and which ones changed their list of worker groups, for the
+  // next pass.  Without gone rows: RayClusters appended after the resident ones.  A regrouped RayCluster (same key and row, another
+  // ordered list of group names) is gone and initialised again in its own row: listed in both `gone` and `init`.
   struct RowMap {
-    std::vector<uint32_t> gone;      // old rows no RayCluster keeps (deleted, or moved away), ascending
-    std::vector<uint32_t> init;      // new rows of a moved or created RayCluster, ascending
-    std::vector<uint32_t> created;   // ... those created (their specs are hashed)
+    std::vector<uint32_t> gone;      // old rows no RayCluster keeps (deleted, moved away, or regrouped), ascending
+    std::vector<uint32_t> init;      // new rows of a moved, created or regrouped RayCluster, ascending
+    std::vector<uint32_t> created;   // ... those whose specs are hashed (created, or moved / regrouped with a new spec range)
     std::vector<uint32_t> digests;   // (old row, new row) of the moved RayClusters whose spec range stayed: the digest moves
-    std::vector<uint32_t> moved_to;  // per gone row: its new row, or KR_EMPTY32 (deleted)
+    std::vector<uint32_t> moved_to;  // per gone row: its new row (itself when regrouped), or KR_EMPTY32 (deleted)
     uint32_t gs0 = 0, ws0 = 0;       // groups / names from these on were shifted
     std::vector<uint32_t> gsrc, wsrc;  // ... and came from these old ones (KR_EMPTY32: of a moved or created RayCluster)
     uint32_t g_lo = 0, g_hi = 0;     // the old groups gsrc reads
@@ -168,6 +171,7 @@ struct CommitRecord {
   uint32_t res_clusters = 0, res_groups = 0, res_wtd = 0;  // ... and RayCluster / group / workersToDelete rows: whole with the object part
   std::vector<uint32_t> prev_h_pod_idx;  // ... and their keys: whole with the object part, rows
   std::vector<uint32_t> prev_wtd;        // KR_OPT_WTD_EDITS: {n_groups, g_wtd_off, g_wtd_cnt, w_name_id} (empty while it is off): whole with the object part
+  std::vector<uint32_t> prev_gnames;     // KR_OPT_GROUP_EDITS: g_name_id of the resident groups (empty while it is off): whole with the object part, rows
   bool hash_dirty = false;        // spec JSON or a JSON range committed since the digests were computed: whole
   bool heads_rebuild = false;     // a head key changed: the pod -> head-aux row table is rebuilt: whole, rows
   bool wtd_rebuild = false;       // a workersToDelete list changed: the name table is rebuilt (kr_incr.cuh): whole
@@ -196,21 +200,28 @@ struct CommitRecord {
     return std::includes(given.begin(), given.end(), json_cols_behind.begin(), json_cols_behind.end());
   }
 
-  // The row map of an object part that brought RayClusters into the recorded fleet or renumbered it (into `map`).  With `deletes`
-  // (KR_OPT_CLUSTER_DELETES) the rows whose key changed and the old rows at or past the new count are looked at; without it only the
-  // rows past the recorded ones are (a changed key is the device diff's to find).  -> 0: nothing entered, left or moved, 1: a map the
-  // resident state follows, -1: a renumbering it does not follow (the next pass is a full one).
+  // The row map of an object part that brought RayClusters into the recorded fleet, renumbered it or regrouped some of it (into
+  // `map`).  With `deletes` (KR_OPT_CLUSTER_DELETES) the rows whose key changed and the old rows at or past the new count are looked
+  // at, with `regroups` (KR_OPT_GROUP_EDITS) the rows whose key stayed and whose ordered group names did not; otherwise only the rows
+  // past the recorded ones are (a changed key or group is the device diff's to find).  -> 0: nothing entered, left, moved or
+  // regrouped, 1: a map the resident state follows, -1: a renumbering it does not follow (the next pass is a full one).
   // `creates`: KR_OPT_CLUSTER_CREATES; `resident`: the RayCluster rows the device tables hold.
-  int derive_map(const kr_snapshot_bufs &hb, const kr_sizes &n, bool creates, bool deletes, uint32_t resident, uint32_t res_groups_old,
-                 uint32_t res_wtd_old) {
+  int derive_map(const kr_snapshot_bufs &hb, const kr_sizes &n, bool creates, bool deletes, bool regroups, uint32_t resident,
+                 uint32_t res_groups_old, uint32_t res_wtd_old) {
     const uint32_t had = (uint32_t)rows.size(), nn = n.n_clusters, lo = std::min(had, nn);
     auto key = [](uint32_t ns, uint32_t name) { return (uint64_t)ns << 32 | name; };
+    regroups = regroups && prev_gnames.size() == res_groups_old;  // (the names are recorded from the object commit after the option came on)
     std::vector<uint32_t> old_ch, new_ch;
-    if (deletes) {
-      for (uint32_t c = 0; c < lo; c++)
-        if (rows[c].ns != hb.c_ns_id[c] || rows[c].name != hb.c_name_id[c]) old_ch.push_back(c), new_ch.push_back(c);
-      for (uint32_t c = nn; c < had; c++) old_ch.push_back(c);
+    uint32_t n_regrouped = 0;
+    for (uint32_t c = 0; c < lo && (deletes || regroups); c++) {
+      const Row &r = rows[c];
+      const bool same_key = r.ns == hb.c_ns_id[c] && r.name == hb.c_name_id[c];
+      const bool regrouped = regroups && same_key &&
+                             (r.group_cnt != hb.c_group_cnt[c] || r.group_off + r.group_cnt > prev_gnames.size() || memcmp(prev_gnames.data() + r.group_off, hb.g_name_id + hb.c_group_off[c], 4 * (size_t)r.group_cnt) != 0);
+      if ((deletes && !same_key) || regrouped) old_ch.push_back(c), new_ch.push_back(c);
+      n_regrouped += regrouped;
     }
+    if (deletes) for (uint32_t c = nn; c < had; c++) old_ch.push_back(c);
     if (old_ch.empty()) {
       // No recorded row left or moved: the rows past the resident ones, if this part added any, are created RayClusters, any number of
       // them, with their groups and names after the resident ones.  Counted from the resident rows (all of them recorded), not from
@@ -229,7 +240,9 @@ struct CommitRecord {
     std::unordered_map<uint64_t, uint32_t> old_key;  // key of a gone row -> that row
     for (uint32_t o : old_ch) if (!old_key.emplace(key(rows[o].ns, rows[o].name), o).second) return -1;
     for (uint32_t c = 0; c < lo; c++)  // a kept row holding a gone row's key: the table's lowest-row rule would move it
-      if (rows[c].ns == hb.c_ns_id[c] && rows[c].name == hb.c_name_id[c] && old_key.count(key(rows[c].ns, rows[c].name))) return -1;
+      if (rows[c].ns == hb.c_ns_id[c] && rows[c].name == hb.c_name_id[c] && !std::binary_search(new_ch.begin(), new_ch.end(), c) &&
+          old_key.count(key(rows[c].ns, rows[c].name)))
+        return -1;
     RowMap m;
     m.gone = old_ch;
     m.moved_to.assign(old_ch.size(), KR_EMPTY32);
@@ -238,15 +251,18 @@ struct CommitRecord {
       const uint64_t k = key(hb.c_ns_id[c], hb.c_name_id[c]);
       if (!new_keys.insert(k).second) return -1;
       const auto it = old_key.find(k);
-      if (it != old_key.end() && it->second >= nn && rows[it->second].group_cnt == hb.c_group_cnt[c]) {  // moved by swap-remove
+      // regrouped in its own row, or moved by swap-remove (with KR_OPT_GROUP_EDITS its group count may have changed as well: it
+      // starts from an empty bucket either way); a digest stays or moves with an unchanged spec range, else it is hashed anew
+      const bool regrouped = it != old_key.end() && it->second == c;
+      if (regrouped || (it != old_key.end() && it->second >= nn && (regroups || rows[it->second].group_cnt == hb.c_group_cnt[c]))) {
         const uint32_t o = it->second;
         m.moved_to[std::lower_bound(m.gone.begin(), m.gone.end(), o) - m.gone.begin()] = c;
-        if (rows[o].json_off == hb.c_json_off[c] && rows[o].json_len == hb.c_json_len[c]) { m.digests.push_back(o); m.digests.push_back(c); }
-        else m.created.push_back(c);  // (a moved RayCluster whose range moved as well is hashed like a created one)
+        if (rows[o].json_off != hb.c_json_off[c] || rows[o].json_len != hb.c_json_len[c]) m.created.push_back(c);
+        else if (!regrouped) { m.digests.push_back(o); m.digests.push_back(c); }
       } else if (creates) m.created.push_back(c);
       else return -1;
     }
-    if (old_ch.size() - m.digests.size() / 2 + new_ch.size() > kMapMax) return -1;  // deleted + moved + created
+    if (old_ch.size() - m.digests.size() / 2 + new_ch.size() - n_regrouped > kMapMax) return -1;  // deleted + moved + created + regrouped
     m.init = new_ch;
     std::sort(m.created.begin(), m.created.end());
     // groups and names from the first renumbered row on: a kept RayCluster's come from its old ones, the others' are new
@@ -278,11 +294,13 @@ struct CommitRecord {
   // what a whole commit moved: the launch shape / pipeline, the wide set, the hash order; `map`: derive_map's verdict (1: the created
   // RayClusters of `map`, whose specs the caller commits as spec rows, are hashed by the next pass)
   struct Moved { bool shape, wide, order; int map; };
-  // (`creates`, `deletes`, `resident`: KR_OPT_CLUSTER_CREATES, KR_OPT_CLUSTER_DELETES, the RayCluster rows the device tables hold)
-  Moved commit_whole(const kr_snapshot_bufs &hb, const kr_sizes &n, uint32_t parts, bool wtd_edits, bool creates, bool deletes, uint32_t resident) {
+  // (`creates`, `deletes`, `regroups`, `resident`: KR_OPT_CLUSTER_CREATES, KR_OPT_CLUSTER_DELETES, KR_OPT_GROUP_EDITS, the RayCluster
+  // rows the device tables hold)
+  Moved commit_whole(const kr_snapshot_bufs &hb, const kr_sizes &n, uint32_t parts, bool wtd_edits, bool creates, bool deletes, bool regroups,
+                     uint32_t resident) {
     const bool objects = parts & (KR_PART_COLUMNS | KR_PART_OBJECTS);
     const size_t had = rows.size();
-    const int mapped = (creates || deletes) && objects && had ? derive_map(hb, n, creates, deletes, resident, res_groups, res_wtd) : 0;
+    const int mapped = (creates || deletes || regroups) && objects && had ? derive_map(hb, n, creates, deletes, regroups, resident, res_groups, res_wtd) : 0;
     bool ranges_moved = had != n.n_clusters && mapped != 1;  // some RayCluster's JSON range differs from the one the digests / the hash order were computed from
     uint32_t n_rc = 0, n_mh_now = 0, max_groups = 0;
     std::vector<uint32_t> wide;
@@ -335,6 +353,8 @@ struct CommitRecord {
         prev_wtd.insert(prev_wtd.end(), hb.g_wtd_cnt, hb.g_wtd_cnt + n.n_groups);
         prev_wtd.insert(prev_wtd.end(), hb.w_name_id, hb.w_name_id + n.n_wtd);
       }
+      if (regroups) prev_gnames.assign(hb.g_name_id, hb.g_name_id + n.n_groups);
+      else prev_gnames.clear();
     }
     return {shape, wide_moved, order, mapped};
   }
@@ -346,6 +366,8 @@ struct CommitRecord {
       uint8_t bit = 0;
       for (uint32_t g = r.group_off; g < r.group_off + r.group_cnt; g++) bit |= hb.g_num_hosts[g] > 1 ? 1 : 0;
       n_mh += bit - r.mh; r.mh = bit;
+      if (r.group_off + r.group_cnt <= prev_gnames.size())  // (a renamed group here is the diff's structural change: the full pass follows)
+        std::copy(hb.g_name_id + r.group_off, hb.g_name_id + r.group_off + r.group_cnt, prev_gnames.begin() + r.group_off);
     }
     for (uint32_t i = 0; i < n_hd; i++)  // the pod -> head-aux row table follows the keys
       if (prev_h_pod_idx[hd[i]] != hb.h_pod_idx[hd[i]]) { heads_rebuild = true; prev_h_pod_idx[hd[i]] = hb.h_pod_idx[hd[i]]; }
@@ -605,6 +627,7 @@ struct kr_engine {
   bool wtd_edits = false;        // KR_OPT_WTD_EDITS
   bool cluster_creates = false;  // KR_OPT_CLUSTER_CREATES
   bool cluster_deletes = false;  // KR_OPT_CLUSTER_DELETES
+  bool group_edits = false;      // KR_OPT_GROUP_EDITS
   uint32_t inc_n_clusters = 0;   // RayClusters in the resident tables
   uint32_t res_n_wtd = 0;        // names in the resident name table and its resolutions (wtd_pod_idx)
   bool ran_inc = false;          // the last pass was an incremental one
@@ -1574,6 +1597,8 @@ int begin_commit(kr_engine *e) {
 bool creates_on(const kr_engine *e) { return e->cluster_creates && e->fixed_layout; }
 // KR_OPT_CLUSTER_DELETES has an effect
 bool deletes_on(const kr_engine *e) { return e->cluster_deletes && e->fixed_layout; }
+// KR_OPT_GROUP_EDITS has an effect
+bool regroups_on(const kr_engine *e) { return e->group_edits && e->fixed_layout; }
 
 // The column table of an object commit's diff: every object column i, staged at stage + at[i] with cnt[d] rows of its dimension d,
 // against the resident one as the record last left it.  Without row lists, staged row k is resident row k; with them (the row path)
@@ -1593,7 +1618,7 @@ ObjDiffArgs object_diff_args(const kr_engine *e, const uint8_t *stage, const siz
     oa.rows_old[k] = d == D_HEADS ? e->rec.res_n_heads : d == D_CLUSTERS ? e->rec.res_clusters : d == D_GROUPS ? e->rec.res_groups : d == D_WTD ? e->rec.res_wtd : (uint32_t)dn[d];
     oa.row_bytes[k] = (uint16_t)(kCols[i].elem * kCols[i].mult);
     oa.cls[k] = obj_class(i, e->wtd_edits);
-    oa.cls_new[k] = obj_class(i, e->wtd_edits, creates_on(e) || deletes_on(e));
+    oa.cls_new[k] = obj_class(i, e->wtd_edits, creates_on(e) || deletes_on(e) || regroups_on(e));
     if (i == kGroupClusterCol) oa.g_cluster_idx_new = reinterpret_cast<const uint32_t *>(stage + at[i]);
     if (i == kHeadKeyCol) oa.h_pod_idx_new = reinterpret_cast<const uint32_t *>(stage + at[i]);
   }
@@ -1739,6 +1764,10 @@ int kr_engine_set_option(kr_engine *e, uint32_t option, uint64_t value) {
     e->cluster_deletes = value != 0;
     return KR_OK;
   }
+  if (option == KR_OPT_GROUP_EDITS) {  // (read at each kr_snapshot_begin and object commit, and by kr_packer_cluster_upsert)
+    e->group_edits = value != 0;
+    return KR_OK;
+  }
   if (option == KR_OPT_LARGE_CLUSTERS || option == KR_OPT_WIDE_CLUSTERS || option == KR_OPT_HUGE_CLUSTERS) {
     bool &on = option == KR_OPT_LARGE_CLUSTERS ? e->large_on : option == KR_OPT_WIDE_CLUSTERS ? e->wide_on : e->huge_on;
     if (on == (value != 0)) return KR_OK;
@@ -1788,6 +1817,7 @@ int kr_engine_get_option(kr_engine *e, uint32_t option, uint64_t *value) {
     case KR_OPT_SPEC_ROWS: *value = e->spec_rows_opt; return KR_OK;
     case KR_OPT_CLUSTER_CREATES: *value = e->cluster_creates; return KR_OK;
     case KR_OPT_CLUSTER_DELETES: *value = e->cluster_deletes; return KR_OK;
+    case KR_OPT_GROUP_EDITS: *value = e->group_edits; return KR_OK;
     case KR_OPT_BUCKET_STRIDE: *value = e->bstride; return KR_OK;
     default: return fail(e, KR_E_INVALID, "unknown option %u", option);
   }
@@ -1941,13 +1971,15 @@ int kr_snapshot_begin(kr_engine *e, const kr_sizes *sizes, kr_snapshot_bufs *out
     // KR_OPT_WTD_EDITS workersToDelete lists grow and shrink as well while the RayClusters and groups stay (the name table is sized
     // for the capacity).  The RayCluster, group and name counts may each grow with KR_OPT_CLUSTER_CREATES (RayClusters created, with
     // their groups and names) while the bucket arena holds the RayClusters at the current stride, with which RayJobs come and go as
-    // well, and shrink with KR_OPT_CLUSTER_DELETES (RayClusters deleted by swap-remove); the object commit's row map checks the rest.
+    // well, and shrink with KR_OPT_CLUSTER_DELETES (RayClusters deleted by swap-remove); with KR_OPT_GROUP_EDITS the group and name
+    // counts may move either way (RayClusters that gained or lost worker groups); the object commit's row map checks the rest.
     const bool fits = (size_t)sizes->n_clusters * e->bstride <= e->sl.bucket_entries;
     auto moves_ok = [&](uint32_t now, uint32_t was) { return now == was || (now < was ? deletes_on(e) : creates_on(e) && fits); };
     const bool same_groups = sizes->n_clusters == e->sizes.n_clusters && sizes->n_groups == e->sizes.n_groups;
-    const bool keep = e->inc_valid && e->fixed_layout && moves_ok(sizes->n_clusters, e->sizes.n_clusters) && moves_ok(sizes->n_groups, e->sizes.n_groups) &&
-                      (moves_ok(sizes->n_wtd, e->sizes.n_wtd) || (e->wtd_edits && same_groups)) && (sizes->n_jobs == e->sizes.n_jobs || creates_on(e)) &&
-                      sizes->n_pods >= e->sizes.n_pods;
+    const bool keep = e->inc_valid && e->fixed_layout && moves_ok(sizes->n_clusters, e->sizes.n_clusters) &&
+                      (moves_ok(sizes->n_groups, e->sizes.n_groups) || regroups_on(e)) &&
+                      (moves_ok(sizes->n_wtd, e->sizes.n_wtd) || (e->wtd_edits && same_groups) || regroups_on(e)) &&
+                      (sizes->n_jobs == e->sizes.n_jobs || creates_on(e)) && sizes->n_pods >= e->sizes.n_pods;
     if (!e->fixed_layout) { e->committed_full = false; e->inc_zero_needed = true; }
     // (the next pass is a full one, which hashes every message: listed rows may not exist any more)
     if (sizes->n_clusters != e->sizes.n_clusters && !keep) clear_spec_rows(e);
@@ -2013,7 +2045,7 @@ int kr_snapshot_commit_parts(kr_engine *e, uint32_t parts) {
   if (e->order_pending) { CK(cudaEventSynchronize(e->ev_order)); e->order_pending = false; }  // a previous upload may still be reading h_order
   if (int rc = begin_commit(e)) return rc;
   const bool renumbered = e->map_pending && !e->rec.map.gone.empty();  // (by an earlier object commit of this epoch)
-  const CommitRecord::Moved moved = e->rec.commit_whole(hb, n, parts, e->wtd_edits, creates_on(e), deletes_on(e), e->inc_n_clusters);
+  const CommitRecord::Moved moved = e->rec.commit_whole(hb, n, parts, e->wtd_edits, creates_on(e), deletes_on(e), regroups_on(e), e->inc_n_clusters);
   if (moved.shape) e->gvalid = false;  // launch shape / pipeline depend on it
   // The object part created or renumbered RayClusters, or moved a row count after a renumbering of this epoch.  A pending renumbering
   // is not composed with either: its map would no longer describe the rows.  (Created RayClusters after created ones: the new map

@@ -215,10 +215,10 @@ __global__ void __launch_bounds__(256) k_inc_objects(ObjDiffArgs a, SnapDev s, S
     const bool shifted = mk >= KR_MAP_GROUP && row >= a.shift_from[col];
     if (shifted && a.map_pass == 2) { for (uint32_t k = 0; k < rb; k++) dst[k] = src[k]; return; }  // (diffed by the first launch)
     if (!shifted && a.map_pass == 1) return;
-    if (shifted) {
+    if (shifted) {  // (a kept RayCluster's row may land past the old count when groups or names were added before it)
       const uint32_t o = (mk == KR_MAP_GROUP ? a.gsrc : a.wsrc)[row - a.shift_from[col]];
-      if (o == KR_EMPTY32) past = true;
-      else old = a.dst[col] + (size_t)o * rb;
+      past = o == KR_EMPTY32;
+      if (!past) old = a.dst[col] + (size_t)o * rb;
     } else if (mk == KR_MAP_CLUSTER && !past) past = sorted_has(a.init, a.n_init, row);
   }
   const uint8_t cls = past ? a.cls_new[col] : a.cls[col];
@@ -390,8 +390,11 @@ __global__ void __launch_bounds__(256) k_inc_admit(SnapDev s, ScratchDev sc, Res
 // them by swap-remove carries the commit's row map: the old rows `gone` that no RayCluster keeps (deleted, or moved to a row a
 // deleted one vacated) and the new rows `init` that were created or moved (k_inc_objects copied them into place and marked them
 // dirty).  RayClusters appended after the last resident row are the map without gone rows: every resident RayCluster, group and
-// workersToDelete name kept its row, and only the steps that read `init` run.  In front of k_inc_admit, each step launched only
-// when its list is not empty:
+// workersToDelete name kept its row, and only the steps that read `init` run.  KR_OPT_GROUP_EDITS adds regrouped RayClusters (same
+// key and row, another list of worker groups): such a row is listed in both `gone` and `init`, so it is released with the old group
+// table, stays on the dirty list at its index, is rekeyed with its new group 0 and offset, and starts again from an empty bucket;
+// k_inc_admit then matches its Pods against the new group names (a Pod of a removed group stays among its Pods, in no group).  In
+// front of k_inc_admit, each step launched only when its list is not empty:
 //   k_inc_digest_move          first, ahead of the hash stream: the digests of moved RayClusters whose spec range stayed;
 //   k_inc_clusters_release     one warp per gone row, while the cluster table still holds the old rows: touches every Pod in its
 //                              bucket (k_inc_admit re-matches it against the new table: a Pod of a deleted RayCluster becomes an

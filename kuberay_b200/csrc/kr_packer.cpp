@@ -108,9 +108,11 @@ struct kr_packer {
   std::vector<uint32_t> json_rows;
   std::vector<uint8_t> json_flag;
   bool json_compacted = false, clusters_moved = false;
-  bool reshaped = false;              // a RayCluster the engine holds changed its group count or a workersToDelete list length
-  // per row: a RayCluster created in, or moved into, this row since the last flush (its spec travels after the object part, whose
-  // row map tells the engine about it); `fresh_any`: some row is set
+  bool reshaped = false;              // a RayCluster the engine holds changed its group count or a workersToDelete list length (with
+                                      // KR_OPT_GROUP_EDITS: a list length, unless KR_OPT_WTD_EDITS as well)
+  bool regrouped = false;             // KR_OPT_GROUP_EDITS: a RayCluster the engine holds changed its list of worker groups
+  // per row: a RayCluster created in, moved into or (KR_OPT_GROUP_EDITS) regrouped in this row since the last flush (its spec travels
+  // after the object part, whose row map tells the engine about it); `fresh_any`: some row is set
   std::vector<uint8_t> fresh;
   bool fresh_any = false;
   void set_fresh(uint32_t row, uint8_t v) {
@@ -349,17 +351,29 @@ int kr_packer_cluster_upsert(kr_packer *p, const kr_cluster_obj *o) {
   if (row >= p->cl_flag.size()) p->cl_flag.resize((size_t)row + 256, 0);
   if (!p->cl_flag[row]) { p->cl_flag[row] = 1; p->dirty_cl.push_back(row); }
   // worker groups (replicas / expectations / workersToDelete move every few seconds under the autoscaler)
-  bool shape = c.groups.size() != o->n_groups;
+  bool shape = c.groups.size() != o->n_groups, wtd_len = false;
+  bool regroup = shape;  // the ordered list of group names changed
   c.groups.resize(o->n_groups);
   for (uint32_t gi = 0; gi < o->n_groups; gi++) {
     const kr_group_obj &g = o->groups[gi];
     GroupRec &r = c.groups[gi];
-    r.name_id = p->intern(g.name); r.replicas = g.replicas; r.mn = g.min_replicas; r.mx = g.max_replicas; r.hosts = g.num_hosts; r.flags = g.flags;
-    if (r.wtd.size() != g.n_workers_to_delete) shape = true;
+    const uint32_t name_id = p->intern(g.name);
+    regroup |= r.name_id != name_id;
+    r.name_id = name_id; r.replicas = g.replicas; r.mn = g.min_replicas; r.mx = g.max_replicas; r.hosts = g.num_hosts; r.flags = g.flags;
+    if (r.wtd.size() != g.n_workers_to_delete) wtd_len = true;
     r.wtd.resize(g.n_workers_to_delete);
     for (uint32_t k = 0; k < g.n_workers_to_delete; k++) r.wtd[k] = p->intern(g.workers_to_delete[k]);
   }
-  if (shape && row < p->engine_sizes.n_clusters && !p->is_fresh(row)) p->reshaped = true;
+  shape |= wtd_len;
+  // KR_OPT_GROUP_EDITS: the engine initialises a regrouped RayCluster again in its row (its spec travels after the object part, which
+  // always goes whole: the row path takes a renamed group as structural), and with KR_OPT_WTD_EDITS as well it follows list lengths
+  uint64_t group_edits = 0, wtd_edits = 0;
+  kr_engine_get_option(p->e, KR_OPT_GROUP_EDITS, &group_edits);
+  if (group_edits) kr_engine_get_option(p->e, KR_OPT_WTD_EDITS, &wtd_edits);
+  if (row < p->engine_sizes.n_clusters && !p->is_fresh(row)) {
+    if (group_edits && regroup) { p->set_fresh(row, 1); p->regrouped = true; p->tables_dirty = true; }
+    else if (shape && !(group_edits && wtd_edits && !regroup)) p->reshaped = true;
+  }
   if (shape || p->tables_dirty) p->tables_dirty = true;
   else {  // same shape: the group rows are rewritten in place
     const uint32_t g0 = b.c_group_off[row];
@@ -490,6 +504,10 @@ int kr_packer_flush(kr_packer *p, uint32_t *mode_out) {
   uint64_t deletes_opt = 0;
   kr_engine_get_option(p->e, KR_OPT_CLUSTER_DELETES, &deletes_opt);
   const bool renumbered = deletes_opt && !p->first && p->clusters_moved && !p->reshaped && !p->json_compacted;
+  // KR_OPT_GROUP_EDITS: RayClusters that changed their worker groups (none reshaped, the arena not compacted, any creation or deletion
+  // of the flush on the path above) keep the incremental epoch too: the object part, then their specs as spec rows
+  const bool regroups = p->regrouped && !p->first && !p->reshaped && !p->json_compacted &&
+                        ((want.n_clusters == old_nc && !p->clusters_moved) || appends || renumbered);
   // Row-granular spec commit (KR_OPT_SPEC_ROWS): only the re-emitted blobs travel, while every other one stays where it was.
   uint64_t spec_opt = 0;
   kr_engine_get_option(p->e, KR_OPT_SPEC_ROWS, &spec_opt);
@@ -497,7 +515,7 @@ int kr_packer_flush(kr_packer *p, uint32_t *mode_out) {
   std::vector<uint32_t> new_rows, old_rows;  // blobs placed this flush: of appended, moved or created RayClusters / of the others
   for (uint32_t r : p->json_rows) (r >= old_nc || p->is_fresh(r) ? new_rows : old_rows).push_back(r);
   // every placed blob travels as a spec row
-  const bool json_rows_ok = spec_ok || ((appends || renumbered) && (old_rows.empty() || spec_opt));
+  const bool json_rows_ok = spec_ok || ((appends || renumbered || regroups) && (old_rows.empty() || spec_opt));
   if (memcmp(&want, &p->engine_sizes, sizeof want) != 0 || p->first) {
     if (int rc = kr_snapshot_begin(p->e, &p->sizes, &same)) return rc;  // fixed layout: new live counts, same addresses, resident data kept
     p->engine_sizes = want;
@@ -535,7 +553,7 @@ int kr_packer_flush(kr_packer *p, uint32_t *mode_out) {
   for (uint32_t r : p->dirty_hd) if (r < p->hd_flag.size()) p->hd_flag[r] = 0;
   p->dirty_cl.clear(); p->dirty_hd.clear(); p->wtd_changed = false;
   for (uint32_t r : p->json_rows) p->json_flag[r] = 0;
-  p->json_rows.clear(); p->json_compacted = p->clusters_moved = p->reshaped = false;
+  p->json_rows.clear(); p->json_compacted = p->clusters_moved = p->reshaped = p->regrouped = false;
   if (p->fresh_any) { std::fill(p->fresh.begin(), p->fresh.end(), 0); p->fresh_any = false; }
   p->first = p->objects_dirty = p->tables_dirty = p->heads_dirty = p->jobs_dirty = p->json_dirty = false;
   p->epoch++;

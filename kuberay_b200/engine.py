@@ -235,7 +235,7 @@ class Engine:
     def for_snapshot(cls, snap: Snapshot, device: int = 0, max_creates: int | None = None, slack: float = 1.0,
                      large_clusters: bool = False, wide_clusters: bool = False, huge_clusters: bool = False,
                      wtd_edits: bool = False, spec_rows: bool = False, cluster_creates: bool = False,
-                     cluster_deletes: bool = False) -> "Engine":
+                     cluster_deletes: bool = False, group_edits: bool = False) -> "Engine":
         d = snap.dims
         up = lambda x: int(x * slack) + 1  # noqa: E731
         if max_creates is None:
@@ -256,6 +256,8 @@ class Engine:
             eng.set_cluster_creates(True)
         if cluster_deletes:
             eng.set_cluster_deletes(True)
+        if group_edits:
+            eng.set_group_edits(True)
         return eng
 
     def _check(self, rc: int):
@@ -319,6 +321,12 @@ class Engine:
         with the new counts, commit the object part; with cluster_creates the same epoch may create RayClusters in vacated rows); read
         at each begin and object commit."""
         self._check(self._L.kr_engine_set_option(self._h, abi.OPT_CLUSTER_DELETES, 1 if on else 0))
+
+    def set_group_edits(self, on: bool = True):
+        """KR_OPT_GROUP_EDITS: under the fixed layout, keep incremental epochs when a RayCluster's worker groups are appended, removed,
+        renamed or reordered (begin with the new counts, commit the object part, and a re-emitted spec as a spec row); read at each begin
+        and object commit."""
+        self._check(self._L.kr_engine_set_option(self._h, abi.OPT_GROUP_EDITS, 1 if on else 0))
 
     def get_option(self, option: int) -> int:
         """kr_engine_get_option: an option's current value, or the read-only OPT_BUCKET_STRIDE (0: the sort pipeline)."""

@@ -523,6 +523,32 @@ def delete_clusters(snap: Snapshot, rows) -> Snapshot:
     return select_clusters(snap, swap_remove_order(snap.dims["clusters"], rows))
 
 
+def regroup_clusters(snap: Snapshot, edits) -> Snapshot:
+    """A copy of `snap` in which each RayCluster c of `edits` has the worker groups edits[c]: a list of (source group row, name id)
+    pairs, each group a copy of its source row (its workersToDelete names included) under that name (None: the source's own).
+    Pod rows, head-aux rows, RayJob rows and the JSON arena stay; groups and names are laid out again in row order."""
+    d = snap.dims
+    goff, gcnt = snap.c_group_off.astype(np.int64), snap.c_group_cnt.astype(np.int64)
+    src, names, owner = [], [], []
+    for c in range(d["clusters"]):
+        pairs = edits.get(c, [(g, None) for g in range(goff[c], goff[c] + gcnt[c])])
+        for g, nm in pairs:
+            src.append(int(g)); names.append(int(snap.g_name_id[g]) if nm is None else int(nm)); owner.append(c)
+    src = np.asarray(src, dtype=np.int64)
+    wsrc = np.concatenate([np.arange(int(snap.g_wtd_off[g]), int(snap.g_wtd_off[g] + snap.g_wtd_cnt[g])) for g in src] + [np.zeros(0, np.int64)])
+    out = Snapshot(d["clusters"], src.size, wsrc.size, d["pods"], d["heads"], d["jobs"], d["json"])
+    rows = {"groups": src, "wtd": wsrc}
+    for name, _dt, _m, dim in abi.COLUMNS:
+        out.cols[name][:] = snap.cols[name][rows[dim]] if dim in rows else snap.cols[name]
+    out.g_name_id[:] = np.asarray(names, dtype=np.uint32)
+    out.g_cluster_idx[:] = np.asarray(owner, dtype=np.uint32)
+    cnt = np.bincount(np.asarray(owner, dtype=np.int64), minlength=d["clusters"])
+    out.c_group_cnt[:] = cnt.astype(np.uint32)
+    out.c_group_off[:] = np.concatenate([[0], np.cumsum(cnt)[:-1]]).astype(np.uint32) if d["clusters"] else 0
+    out.g_wtd_off[:] = np.concatenate([[0], np.cumsum(out.g_wtd_cnt)[:-1]]).astype(np.uint32) if src.size else 0
+    return out.validate()
+
+
 def config(name: str, **overrides) -> SynthParams:
     d = dict(CONFIGS[name])
     d.update(overrides)

@@ -161,6 +161,42 @@ def deletions(snap, flags, label):
     print(label, "ok:", inc, "of 2 deletion epochs incremental", flush=True)
 
 
+def group_edits(snap, flags, label):
+    """KR_OPT_GROUP_EDITS (kr_incr.cuh): a worker group appended to RayCluster 40 whose resident Pods are already labelled for it,
+    then its first group removed while its Pods live on — each epoch releases the RayCluster, rekeys the table, gathers the shifted
+    group records and initialises it again in its row."""
+    flags.fetch_pod_lists = 0
+    c = 40
+    w = np.flatnonzero((snap.p_ns_id == snap.c_ns_id[c]) & (snap.p_cluster_name_id == snap.c_name_id[c]) &
+                       (((snap.p_packed >> abi.PP_NODE_TYPE_SHIFT) & 3) == abi.NT_WORKER))[:4]
+    fresh = int(max(snap.g_name_id.max(), snap.p_group_name_id.max(), snap.p_name_id.max(), snap.c_name_id.max())) + 1
+    snap.p_group_name_id[w] = fresh
+    eng = Engine.for_snapshot(snap, slack=1.5, group_edits=True)
+    eng.set_fixed_layout(True)
+    inc = 0
+    try:
+        views = eng.load(snap)
+        eng.reconcile(flags)
+        g0, cur = int(snap.c_group_off[c]), snap
+        for pairs in ([(g, None) for g in range(g0, g0 + int(snap.c_group_cnt[c]))] + [(g0, fresh)], None):
+            if pairs is None:  # the first group removed
+                g0 = int(cur.c_group_off[c])
+                pairs = [(g, None) for g in range(g0 + 1, g0 + int(cur.c_group_cnt[c]))]
+            cur = synthetic.regroup_clusters(cur, {c: pairs})
+            views = eng.begin(cur.sizes())
+            for col, _d, _m, dim in abi.COLUMNS:
+                if dim not in ("pods", "json"):
+                    np.copyto(views[col], cur.cols[col])
+            eng.commit(abi.PART_OBJECTS)
+            names = [n for n, _ in eng.reconcile_profiled(flags)["kernels"]]
+            assert "k_inc_clusters_release" in names and "k_inc_clusters_insert" in names, names
+            got = eng.fetch()
+            inc += got.changed_clusters is not None
+    finally:
+        eng.close()
+    print(label, "ok:", inc, "of 2 group-edit epochs incremental", flush=True)
+
+
 def wtd_edits(snap, flags, label):
     """KR_OPT_WTD_EDITS (kr_incr.cuh): workersToDelete renames, a list grown past the old n_wtd, then every list cleared — each epoch
     rebuilds the name table on the device (k_inc_wtd_release / _clear / _insert / _resolve)."""
@@ -235,6 +271,8 @@ def main():
               "RayCluster deletions")
     creations(*synthetic.generate(synthetic.config("C2", n_clusters=300, pods_per_cluster=20, groups=2, wtd_group_frac=0.3, recreate_frac=0.3)),
               "RayCluster creations")
+    group_edits(*synthetic.generate(synthetic.config("C2", n_clusters=300, pods_per_cluster=20, groups=2, wtd_group_frac=0.3, recreate_frac=0.3)),
+                "worker-group edits")
     spec_rows(*synthetic.generate(synthetic.config("C2", n_clusters=300, pods_per_cluster=20, groups=2, recreate_frac=0.3)), "spec rows")
     wtd_edits(*synthetic.generate(synthetic.config("C2", n_clusters=300, pods_per_cluster=20, groups=2, autoscaling_frac=1.0, wtd_group_frac=0.3)),
               "workersToDelete edits")
