@@ -388,7 +388,8 @@ typedef struct kr_results_view {
    * complete and bit-identical to what a full pass would return.  n_changed / changed_clusters name the records that were
    * recomputed: n_changed == n_clusters and changed_clusters == NULL after a full pass.  Anything the resident state cannot
    * absorb (a changed table key or CSR offset, wholesale column commits, different flags, an overflowing bucket) silently
-   * takes the full pass.  Snapshots with multi-host worker groups (numOfHosts > 1) keep incremental epochs, and so does an edit of
+   * takes the full pass (with KR_OPT_LARGE_GROWTH, a RayCluster that outgrows its bucket or region gets a new region in the
+   * incremental pass instead).  Snapshots with multi-host worker groups (numOfHosts > 1) keep incremental epochs, and so does an edit of
    * numOfHosts; so does an edit of a workersToDelete list with KR_OPT_WTD_EDITS (a length change only under KR_OPT_FIXED_LAYOUT).  Every pass is a full one on the sort pipeline — no resident state — while the caller fetches the full pod lists
    * (fetch_pod_lists = 1), while some RayCluster lists more than 256 pods (more than KR_LARGE_MAX_PODS with KR_OPT_LARGE_CLUSTERS,
    * unless KR_OPT_HUGE_CLUSTERS) or has more than 32 worker groups (unless KR_OPT_WIDE_CLUSTERS is set), or when KR_NO_INCR=1 is set in the environment. */
@@ -553,7 +554,9 @@ enum {
                               of the whole fleet or leaving the pipeline, so such a fleet keeps its incremental epochs.  Results are the
                               same as with 0 (the default: one such RayCluster sends every pass to the sort pipeline).  May be set at any
                               time; takes effect at the next full pass.  A RayCluster of more than KR_LARGE_MAX_PODS pods still sends
-                              the pass to the sort / radix pipelines, unless KR_OPT_HUGE_CLUSTERS.  Turning it on allocates the region arena once, for the
+                              the pass to the sort / radix pipelines, unless KR_OPT_HUGE_CLUSTERS.  A RayCluster that outgrows its
+                              bucket or region in an incremental epoch makes that epoch a full pass, unless KR_OPT_LARGE_GROWTH.
+                              Turning it on allocates the region arena once, for the
                               capacities: about 22 B per max_pods + 20 B per max_clusters of device memory. */
   KR_OPT_BUCKET_STRIDE = 4,   /* read only (kr_engine_get_option): records per RayCluster bucket of the current layout (64 / 128 / 256);
                               0 = the passes take the sort pipeline */
@@ -615,7 +618,7 @@ enum {
                               at any time; read at each kr_snapshot_begin and object commit.  No effect without KR_OPT_FIXED_LAYOUT.
                               The native packer's flush takes this path by itself when the engine has the option (the specs it placed
                               travel as spec rows unless it compacted the JSON arena). */
-  KR_OPT_GROUP_EDITS = 11     /* 1, together with KR_OPT_FIXED_LAYOUT: a RayCluster whose list of worker groups changed (groups appended,
+  KR_OPT_GROUP_EDITS = 11,    /* 1, together with KR_OPT_FIXED_LAYOUT: a RayCluster whose list of worker groups changed (groups appended,
                               as a RayService in-place update does, removed, renamed or reordered) keeps the incremental epoch:
                               kr_snapshot_begin(new counts; n_groups and n_wtd may move either way), then the object part
                               (KR_PART_OBJECTS), with the RayCluster's spec, when it was re-emitted, as a spec row before or after it.
@@ -635,8 +638,29 @@ enum {
                               first object commit with it on records the group names, the next ones compare against them).  No effect
                               without KR_OPT_FIXED_LAYOUT.  The native packer's flush takes this path by itself when the engine has the
                               option: the regrouped RayClusters' specs travel as spec rows. */
+  KR_OPT_LARGE_GROWTH = 12    /* 1, together with KR_OPT_LARGE_CLUSTERS: a RayCluster that outgrows its room in an incremental epoch (an
+                              ordinary one its bucket, a large one its region, as Pods join it when it scales up) keeps the incremental
+                              epoch: the pass gives it a region of the size a full pass would (1.25x its Pods rounded up to 32, at
+                              most KR_LARGE_MAX_PODS, less the stride) past the regions in use, copies a large one's old region into it,
+                              places the records that did not fit and decides it with the per-cluster kernels in the same pass.  The
+                              stride does not move, and the grown RayClusters are among changed_clusters.  This also covers a
+                              RayCluster KR_OPT_CLUSTER_CREATES creates and that adopts more resident orphan Pods than its bucket holds.
+                              Still full passes: more than KR_GROW_MAX RayClusters outgrowing their room at once, promotions that
+                              would take the per-cluster list past max(KR_GROW_LIST_MIN, n_clusters / KR_GROW_LIST_DIV) RayClusters (a
+                              regrowth alone adds no one to the list and is never held back by it), a RayCluster of more than
+                              KR_LARGE_MAX_PODS Pods (a huge one, KR_OPT_HUGE_CLUSTERS, needs tiles), a full region arena (regions a
+                              regrowth abandons are reclaimed by the next full pass that reclassifies) and more than KR_GROW_SPILL Pods
+                              joining grown RayClusters in one epoch.  Results are the same as with 0 (the default: each such epoch is
+                              a full pass that widens the stride or reclassifies the fleet).  May be set at any time; read at each
+                              incremental pass.  No effect without KR_OPT_LARGE_CLUSTERS.  Turning it on allocates about 0.5 MB of
+                              device memory and 1 KB of pinned host memory once. */
 };
 enum { KR_LARGE_MAX_PODS = 8192 };  /* largest RayCluster KR_OPT_LARGE_CLUSTERS keeps on the bucket pipeline */
+/* KR_OPT_LARGE_GROWTH: at most KR_GROW_MAX RayClusters get a region in one incremental epoch, and an epoch that puts RayClusters on
+ * the per-cluster kernels' list may leave it at most max(KR_GROW_LIST_MIN, n_clusters / KR_GROW_LIST_DIV) long (BASELINE.md: k_decide_large over promoted
+ * RayClusters); beyond either, the epoch is a full pass, so a fleet that grows as a whole still widens its stride.  At most
+ * KR_GROW_SPILL records of grown RayClusters wait for their new regions in one epoch. */
+enum { KR_GROW_MAX = 64, KR_GROW_LIST_MIN = 64, KR_GROW_LIST_DIV = 64, KR_GROW_SPILL = 16384 };
 int kr_engine_set_option(kr_engine *e, uint32_t option, uint64_t value);
 /* Current value of an option (KR_OPT_*), and the read-only KR_OPT_BUCKET_STRIDE. */
 int kr_engine_get_option(kr_engine *e, uint32_t option, uint64_t *value);

@@ -154,6 +154,9 @@ const (
 	// incremental epochs; only under KR_OPT_FIXED_LAYOUT; recommended for RayService fleets, whose in-place updates append worker
 	// groups; read at each Begin and object commit).
 	OptGroupEdits = uint32(C.KR_OPT_GROUP_EDITS)
+	// OptLargeGrowth is KR_OPT_LARGE_GROWTH (1: a RayCluster that outgrows its bucket or region in an incremental epoch gets a new
+	// region in that epoch; only with KR_OPT_LARGE_CLUSTERS; recommended for autoscaled fleets; read at each incremental pass).
+	OptLargeGrowth = uint32(C.KR_OPT_LARGE_GROWTH)
 )
 
 // SetOption: KR_OPT_FIXED_LAYOUT (before the first Begin), KR_OPT_INCREMENTAL, KR_OPT_LARGE_CLUSTERS (1: RayClusters of 257 to
@@ -166,7 +169,9 @@ const (
 // KR_OPT_FIXED_LAYOUT: RayClusters appended after the last row and RayJobs created or deleted keep incremental epochs; read at each
 // Begin and object commit), KR_OPT_CLUSTER_DELETES (1, with KR_OPT_FIXED_LAYOUT: RayClusters deleted by swap-remove keep incremental
 // epochs; read at each Begin and object commit), KR_OPT_GROUP_EDITS (1, with KR_OPT_FIXED_LAYOUT: a RayCluster whose list of worker
-// groups changed keeps incremental epochs; read at each Begin and object commit).  For a Packer, call it on Packer.Engine().
+// groups changed keeps incremental epochs; read at each Begin and object commit), KR_OPT_LARGE_GROWTH (1, with KR_OPT_LARGE_CLUSTERS:
+// a RayCluster that outgrows its bucket or region keeps incremental epochs; read at each incremental pass).  For a Packer, call it on
+// Packer.Engine().
 func (e *Engine) SetOption(option uint32, value uint64) error {
 	if rc := C.kr_engine_set_option(e.h, C.uint32_t(option), C.uint64_t(value)); rc != C.KR_OK {
 		return e.err(rc)

@@ -50,6 +50,12 @@ __device__ __forceinline__ uint4 *large_slot(const ScratchDev &sc, uint32_t c, u
 __device__ __forceinline__ uint4 *rec_slot(const ScratchDev &sc, uint32_t c, uint32_t rank) {
   return rank < sc.bucket_stride ? sc.bucket + (size_t)c * sc.bucket_stride + rank : large_slot(sc, c, rank);
 }
+// Region capacity of a RayCluster of `count` pods at this stride: 1.25x its pods rounded up to 32, capped at KR_LARGE_MAX_PODS unless
+// the cluster is huge, less the stride (the full pass's reclassification and k_inc_grow both size regions by it)
+__host__ __device__ __forceinline__ uint32_t large_region_cap(uint32_t count, uint32_t stride) {
+  const uint32_t want = ((count + count / 4 + 31) / 32) * 32;
+  return (count > KR_LARGE_MAX_PODS ? want : (want < KR_LARGE_MAX_PODS ? want : (uint32_t)KR_LARGE_MAX_PODS)) - stride;
+}
 
 
 // ------------------------------------------------------------------------------------------------ k_match2

@@ -109,6 +109,9 @@ enum {
   KR_INC_VOID = 5,         // the incremental attempt is void (a bucket or an arena overflowed): take a full pass
   KR_INC_GROUPS = 6,       // gather: group records staged so far
   KR_INC_LSEG = 7,         // large RayClusters: scratch positions handed out so far (k_large_sort)
+  KR_INC_GROW = 8,         // KR_OPT_LARGE_GROWTH: RayClusters k_inc_admit put on the grow list (k_inc_grow, kr_incr.cuh)
+  KR_INC_SPILL = 9,        // ... records it spilled for them
+  KR_INC_GROWN = 10,       // ... entries of k_inc_grow's result (0: nothing grew, or the epoch is void)
 };
 // words of a cl_in record (built by k_build_tables; k_decide2 loads it with one coalesced 128-byte access, lane i = word i)
 enum {

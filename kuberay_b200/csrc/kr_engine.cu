@@ -610,6 +610,12 @@ struct kr_engine {
   uint8_t *d_huge = nullptr;
   size_t huge_tiles = 0;
   std::vector<uint4> h_tiles;
+  // KR_OPT_LARGE_GROWTH, allocated when first turned on: the grow buffer of the incremental pass (kGrowBytes: list, result, spill)
+  // and a pinned copy of its result; lg_cursor is the region arena's first entry past every region in use (after_bucket_void lays
+  // them out from 0, each growth allocates past it)
+  bool large_growth = false;
+  uint4 *d_grow = nullptr; uint4 *h_grow = nullptr;
+  size_t lg_cursor = 0;
   bool ran_bucket = false;
   uint64_t h2d_accum = 0;       // bytes uploaded by the commits since the last pass (kr_profile.h2d_bytes)
   // hash order: message ids by descending SHA-1 block count, rebuilt at every commit from c_json_len
@@ -755,9 +761,13 @@ cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t sme
   return cudaLaunchKernelEx(&cfg, kern, KArgs(args)...);
 }
 
-// Points the pass at the cluster table of the per-cluster kernels when their list is not empty; returns the device list.
-const uint32_t *bind_large(const kr_engine *e, ScratchDev &sc) {
-  if (!e->n_large) return nullptr;
+// An incremental pass may give RayClusters regions (KR_OPT_LARGE_GROWTH): the engine's bucket layout has a region arena and table.
+bool grows(const kr_engine *e) { return e->large_growth && e->large_on && e->d_grow && e->d_region && e->d_lg; }
+
+// Points the pass at the cluster table of the per-cluster kernels when their list is not empty, or the pass may grow regions
+// (`grow`); returns the device list.
+const uint32_t *bind_large(const kr_engine *e, ScratchDev &sc, bool grow) {
+  if (!e->n_large && !grow) return nullptr;
   sc.lg = reinterpret_cast<uint4 *>(e->d_lg);
   sc.region = e->d_region;  // (nullptr without KR_OPT_LARGE_CLUSTERS: every capacity is then 0)
   return reinterpret_cast<const uint32_t *>(e->d_lg + align_up(16 * (size_t)e->cfg.max_clusters));
@@ -804,14 +814,15 @@ int upload_lg(kr_engine *e) {
   if (tiles.size() > e->huge_tiles) return fail(e, KR_E_STATE, "internal: %zu huge-cluster tiles, room for %zu", tiles.size(), e->huge_tiles);
   if ((uint32_t)list.size() != e->n_large || n_lsort != e->n_lsort || (uint32_t)tiles.size() != e->n_tiles) e->gvalid = false;
   e->n_large = (uint32_t)list.size(); e->n_lsort = n_lsort; e->n_tiles = (uint32_t)tiles.size();
-  if (list.empty()) return KR_OK;
+  if (list.empty() && !grows(e)) return KR_OK;  // (an incremental pass that grows regions reads the table even then: all zero)
   const uint32_t Nc = e->sizes.n_clusters;
   std::vector<uint4> lg(Nc, make_uint4(0, 0, 0, 0));  // a wide cluster without a region: capacity 0
   for (size_t i = 0; i < e->large_rows.size(); i++) lg[e->large_rows[i]] = make_uint4(e->large_reg[i].x, e->large_reg[i].y, 0, 0);
   CK(cudaStreamSynchronize(e->sm));  // the previous upload has left the host copies
   e->h_lg.swap(lg); e->h_lg_list.swap(list); e->h_tiles.swap(tiles);
   CK(cudaMemcpyAsync(e->d_lg, e->h_lg.data(), 16 * (size_t)Nc, cudaMemcpyHostToDevice, e->sm));
-  CK(cudaMemcpyAsync(e->d_lg + align_up(16 * (size_t)e->cfg.max_clusters), e->h_lg_list.data(), 4 * e->h_lg_list.size(), cudaMemcpyHostToDevice, e->sm));
+  if (!e->h_lg_list.empty())
+    CK(cudaMemcpyAsync(e->d_lg + align_up(16 * (size_t)e->cfg.max_clusters), e->h_lg_list.data(), 4 * e->h_lg_list.size(), cudaMemcpyHostToDevice, e->sm));
   if (!e->h_tiles.empty()) CK(cudaMemcpyAsync(e->d_huge, e->h_tiles.data(), 16 * e->h_tiles.size(), cudaMemcpyHostToDevice, e->sm));
   return KR_OK;
 }
@@ -890,8 +901,8 @@ struct PassCtx {
   SnapDev s; ResDev r; ScratchDev sc; const uint32_t *lg_list; HugeDev hd; Sizes z;
   cudaStream_t M, H;
   int k = 0;
-  PassCtx(kr_engine *e_, bool profile_)
-      : e(e_), profile(profile_), r(bind_out(e->ol, e->d_out)), sc(bind_scratch(e->sl, e->d_scratch)), lg_list(bind_large(e, sc)),
+  PassCtx(kr_engine *e_, bool profile_, bool grow = false)
+      : e(e_), profile(profile_), r(bind_out(e->ol, e->d_out)), sc(bind_scratch(e->sl, e->d_scratch)), lg_list(bind_large(e, sc, grow)),
         hd(bind_huge(e)), z(sizes_of(e->sizes)), M(e->sm), H(profile ? e->sm : e->sh) {
     bind_in(e->il, e->d_in, &s);
     sc.bucket_stride = e->bstride;
@@ -933,12 +944,13 @@ cudaError_t launch_decide2(const PassCtx &c, const Decide2Args &da, dim3 grid, b
   return launch_pdl(kern[st][inc][mh], grid, dim3(kD2Warps * 32), 0, c.M, pdl, da);
 }
 
-// The sorts of the per-cluster kernels' RayClusters (kr_large.cuh): k_large_sort for the first n_lsort of the list, the huge ones
-// after them tile by tile, then merged (kr_huge.cuh).
+// The sorts of the per-cluster kernels' RayClusters (kr_large.cuh): k_large_sort for the first n_lsort of the list (and, with `grown`,
+// k_inc_grow's result, for the RayClusters it listed), the huge ones after them tile by tile, then merged (kr_huge.cuh).
 template <bool kInc>
-void launch_large_sort(PassCtx &c, const Decide2Args &da) {
+void launch_large_sort(PassCtx &c, const Decide2Args &da, const uint4 *grown = nullptr) {
   const kr_engine *e = c.e;
-  if (e->n_lsort) { c.mark("k_large_sort"); k_large_sort<kInc><<<e->n_lsort, kLargeSortThreads, 0, c.M>>>(da, c.lg_list); }
+  const uint32_t n = e->n_lsort + (grown ? KR_GROW_MAX : 0);
+  if (n) { c.mark("k_large_sort"); k_large_sort<kInc><<<n, kLargeSortThreads, 0, c.M>>>(da, c.lg_list, e->n_lsort, grown); }
   if (e->n_tiles) {
     c.mark("k_huge_tiles"); k_huge_tiles<kInc><<<e->n_tiles, kHugeThreads, 0, c.M>>>(da, c.hd);
     c.mark("k_huge_merge"); k_huge_merge<kInc><<<e->n_tiles, kHugeThreads, 0, c.M>>>(da, c.hd);
@@ -1022,7 +1034,7 @@ int launch_pass(kr_engine *e, const kr_flags &f, bool profile, bool capturing = 
     const bool large = e->n_large && sc.lg && n.n_clusters;  // large RayClusters (kr_large.cuh): sorted beside the hash, decided after it
     if (large) launch_large_sort<false>(c, da);
     if (int rc = join_hash()) return rc;
-    if (large) { c.mark("k_decide_large"); k_decide_large<false><<<e->n_large, kLargeDecideThreads, 0, M>>>(da, c.lg_list); }
+    if (large) { c.mark("k_decide_large"); k_decide_large<false><<<e->n_large, kLargeDecideThreads, 0, M>>>(da, c.lg_list, e->n_large, nullptr); }
     if (e->rec.n_recreate > 0 && do_hash && !spin) {  // clusters whose Recreate gate needs the digest: decided again, in the places phase 0 reserved
       da.phase = 1;
       c.mark("k_decide2_phase1");
@@ -1179,7 +1191,7 @@ int after_bucket_void(kr_engine *e) {
   std::vector<uint4> dyn(Nc);
   CK(cudaMemcpyAsync(dyn.data(), e->d_scratch + e->sl.cl_dyn, 16 * (size_t)Nc, cudaMemcpyDeviceToHost, e->sm));
   CK(cudaStreamSynchronize(e->sm));
-  e->large_rows.clear(); e->large_reg.clear();  // (rebuilt below from this attempt's counts)
+  e->large_rows.clear(); e->large_reg.clear(); e->lg_cursor = 0;  // (rebuilt below from this attempt's counts)
   e->lg_stale = true;  // (uploaded below; a layout that leaves the bucket pipeline uploads nothing it would read)
   uint32_t st = e->bstride, n_big = 0, most = 0;
   for (const uint4 &d : dyn) { if (d.x > 256) n_big++; if (d.x <= 256) most = std::max(most, d.x); }
@@ -1196,14 +1208,14 @@ int after_bucket_void(kr_engine *e) {
   size_t off = 0, tiles = 0;
   for (uint32_t c = 0; c < Nc; c++) {
     if (dyn[c].x <= 256) continue;
-    const uint32_t want = ((dyn[c].x + dyn[c].x / 4 + 31) / 32) * 32;
-    const uint32_t cap = (dyn[c].x > KR_LARGE_MAX_PODS ? want : std::min<uint32_t>(want, KR_LARGE_MAX_PODS)) - st;
+    const uint32_t cap = large_region_cap(dyn[c].x, st);
     e->large_rows.push_back(c); e->large_reg.push_back(make_uint2((uint32_t)off, cap));
     off += cap;
     if (is_huge(st, cap)) tiles += huge_tile_count(st, cap);
   }
   if (off > e->large_entries || tiles > e->huge_tiles) { e->large_rows.clear(); e->large_reg.clear(); e->bstride = 0; return KR_OK; }
   e->bstride = st;
+  e->lg_cursor = off;
   return upload_lg(e);  // (on the pass's stream: ordered before the rerun)
 }
 // a bucket-pipeline pass leaves everything an incremental epoch needs on the device
@@ -1247,7 +1259,8 @@ int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile
                            (e->rec.snap_max_groups > KR_SMEM_GROUPS && !e->wide_on) || (adopt && n_init > kAdoptMax)
                      : n.n_clusters != e->inc_n_clusters)
     return KR_OK;
-  PassCtx c(e, profile);
+  const bool grow = grows(e) && e->bstride;  // (KR_OPT_LARGE_GROWTH: a RayCluster that outgrows its room gets a region in this pass)
+  PassCtx c(e, profile, grow);
   const SnapDev &s = c.s; const ResDev &r = c.r; const ScratchDev &sc = c.sc; const Sizes &z = c.z;
   const cudaStream_t M = c.M, H = c.H;
   CK(cudaStreamWaitEvent(M, e->ev_cols, 0));
@@ -1336,7 +1349,12 @@ int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile
   }
   // (k_inc_refresh ran behind the object commits' diff kernels: the input records are current)
   c.mark("k_inc_admit");
-  k_inc_admit<<<grid, 256, 0, M>>>(s, sc, r, z, n.n_wtd ? 1 : 0);
+  k_inc_admit<<<grid, 256, 0, M>>>(s, sc, r, z, n.n_wtd ? 1 : 0, grow ? e->d_grow : nullptr);
+  if (grow) {  // regions for the RayClusters that outgrew their room (most launches find the grow list empty and leave at once)
+    c.mark("k_inc_grow");
+    const uint32_t list_cap = std::max<uint32_t>(KR_GROW_LIST_MIN, n.n_clusters / KR_GROW_LIST_DIV);
+    k_inc_grow<<<e->sm_count, 256, 0, M>>>(s, sc, e->d_grow, (uint32_t)e->lg_cursor, (uint32_t)e->large_entries, e->n_large, list_cap, e->wide_on ? 1 : 0);
+  }
   if ((do_hash || n_rows) && !profile) CK(cudaStreamWaitEvent(M, e->ev_hash, 0));
   const IncStageLayout sl = e->inc_layout = inc_stage_layout(n.n_clusters, n.n_groups);  // staging for the changed records
   if (sl.total > e->inc_stage.cap) return fail(e, KR_E_STATE, "internal: incremental staging of %zu bytes, room for %zu", sl.total, e->inc_stage.cap);
@@ -1352,11 +1370,12 @@ int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile
     c.mark("k_decide2_dirty");
     // (the multi-host rows as of the latest commit: an object commit may have brought the snapshot's first multi-host group or taken its last)
     CK(launch_decide2(c, da, dim3((n.n_clusters + kD2Warps - 1) / kD2Warps), true, false));
-    if (e->n_large) {  // the dirty large RayClusters (k_decide2 left every cluster past the stride alone)
+    if (e->n_large || grow) {  // the dirty large RayClusters (k_decide2 left every cluster past the stride alone), and those k_inc_grow listed
+      const uint4 *grown = grow ? e->d_grow + kGrowResult : nullptr;
       CK(cudaMemsetAsync(sc.inc + KR_INC_LSEG, 0, 4, M));
-      launch_large_sort<true>(c, da);
+      launch_large_sort<true>(c, da, grown);
       c.mark("k_decide_large");
-      k_decide_large<true><<<e->n_large, kLargeDecideThreads, 0, M>>>(da, c.lg_list);
+      k_decide_large<true><<<e->n_large + (grow ? KR_GROW_MAX : 0), kLargeDecideThreads, 0, M>>>(da, c.lg_list, e->n_large, grown);
     }
   }
   if (n.n_jobs) { c.mark("k_jobs"); k_jobs<<<(n.n_jobs + 255) / 256, 256, 0, M>>>(s, sc, r, z); }
@@ -1364,13 +1383,27 @@ int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile
   if (done) CK(cudaEventRecord(done, M));
   CK(cudaMemcpyAsync(e->h_totals, e->d_out + e->ol.totals, 48, cudaMemcpyDeviceToHost, M));
   CK(cudaMemcpyAsync(e->h_inc, sc.inc, 64, cudaMemcpyDeviceToHost, M));
+  if (grow) CK(cudaMemcpyAsync(e->h_grow, e->d_grow + kGrowResult, 16 * KR_GROW_MAX, cudaMemcpyDeviceToHost, M));
   CK(cudaEventRecord(e->ev_inc, M));
   k_inc_finish<<<1, 32, 0, M>>>(sc);  // (the host does not wait for it: whatever comes next is ordered behind it on this stream)
   CK(cudaGetLastError());
   CK(cudaEventSynchronize(e->ev_inc));
   commits_read(e);
   e->rec.heads_rebuild = false;  // (rebuilt here, or about to be rebuilt by the full pass)
-  if (e->h_inc[KR_INC_VOID] || e->h_inc[KR_INC_STRUCTURAL]) return KR_OK;  // the caller takes the full pass
+  if (e->h_inc[KR_INC_VOID] || e->h_inc[KR_INC_STRUCTURAL]) {  // the caller takes the full pass
+    if (grow) e->lg_stale = true;  // (k_inc_grow may have written regions of this attempt into the device table: the full pass reads the host's)
+    return KR_OK;
+  }
+  // the regions k_inc_grow gave, into the large half (rows ascending: commit_map and upload_lg search it); the next pass's upload
+  // lists the newly listed RayClusters
+  for (uint32_t i = 0; grow && i < e->h_inc[KR_INC_GROWN]; i++) {
+    const uint4 g = e->h_grow[i];
+    const size_t at = std::lower_bound(e->large_rows.begin(), e->large_rows.end(), g.x) - e->large_rows.begin();
+    if (at == e->large_rows.size() || e->large_rows[at] != g.x) { e->large_rows.insert(e->large_rows.begin() + at, g.x); e->large_reg.insert(e->large_reg.begin() + at, make_uint2(g.y, g.z)); }
+    else e->large_reg[at] = make_uint2(g.y, g.z);
+    e->lg_cursor = std::max<size_t>(e->lg_cursor, (size_t)g.y + g.z);
+    e->lg_stale = true;
+  }
   if (!e->fetched) e->host_results_stale = true;  // the previous pass's records never reached the host copy
   e->fetched = false;
   e->inc_n_dirty = e->h_inc[KR_INC_DIRTY];
@@ -1425,6 +1458,7 @@ int run_pass(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile) {
     bool ok = false;
     if (int rc = run_pass_inc(e, f, done, profile, &ok)) return rc;
     if (ok) { e->inc_n_pods = e->sizes.n_pods; e->inc_n_heads = e->sizes.n_heads; e->inc_n_clusters = e->sizes.n_clusters; return pass_done(e, done); }
+    if (e->lg_stale) if (int rc = upload_lg(e)) return rc;  // (a void attempt that grew regions left them in the device table)
   }
   e->inc_valid = false; e->ran_inc = false;
   if (e->inc_zero_needed) {  // first pass on this layout: stamps, dirty flags and epoch counters start from zero
@@ -1768,6 +1802,16 @@ int kr_engine_set_option(kr_engine *e, uint32_t option, uint64_t value) {
     e->group_edits = value != 0;
     return KR_OK;
   }
+  if (option == KR_OPT_LARGE_GROWTH) {  // (read at each incremental pass)
+    if (value && !e->d_grow) {
+      CK(cudaSetDevice(e->cfg.device));
+      CK(cudaMalloc((void **)&e->d_grow, kGrowBytes));
+      CK(cudaHostAlloc((void **)&e->h_grow, 16 * KR_GROW_MAX, cudaHostAllocDefault));
+    }
+    e->large_growth = value != 0;
+    e->lg_stale = true;  // (the next pass uploads the region table, all zero while no RayCluster has a region)
+    return KR_OK;
+  }
   if (option == KR_OPT_LARGE_CLUSTERS || option == KR_OPT_WIDE_CLUSTERS || option == KR_OPT_HUGE_CLUSTERS) {
     bool &on = option == KR_OPT_LARGE_CLUSTERS ? e->large_on : option == KR_OPT_WIDE_CLUSTERS ? e->wide_on : e->huge_on;
     if (on == (value != 0)) return KR_OK;
@@ -1796,7 +1840,7 @@ int kr_engine_set_option(kr_engine *e, uint32_t option, uint64_t value) {
     on = value != 0;
     // the next full pass starts again from the layout's first stride and the fast sort pipeline: a pass with the option off may
     // have left the bucket pipeline (and the fast pipeline, for a cluster above 1024 pods) for this layout
-    e->large_rows.clear(); e->large_reg.clear(); e->lg_stale = true; e->inc_valid = false; e->gvalid = false;
+    e->large_rows.clear(); e->large_reg.clear(); e->lg_cursor = 0; e->lg_stale = true; e->inc_valid = false; e->gvalid = false;
     e->force_radix = e->env_radix;
     if (e->begun) e->bstride = first_stride(e->sizes);
     return KR_OK;
@@ -1818,6 +1862,7 @@ int kr_engine_get_option(kr_engine *e, uint32_t option, uint64_t *value) {
     case KR_OPT_CLUSTER_CREATES: *value = e->cluster_creates; return KR_OK;
     case KR_OPT_CLUSTER_DELETES: *value = e->cluster_deletes; return KR_OK;
     case KR_OPT_GROUP_EDITS: *value = e->group_edits; return KR_OK;
+    case KR_OPT_LARGE_GROWTH: *value = e->large_growth; return KR_OK;
     case KR_OPT_BUCKET_STRIDE: *value = e->bstride; return KR_OK;
     default: return fail(e, KR_E_INVALID, "unknown option %u", option);
   }
@@ -1887,7 +1932,7 @@ int kr_engine_create(const kr_config *cfg, kr_engine **out) {
                         (const void *)k_inc_mark_recreate, (const void *)k_decide2<2, true>, (const void *)k_decide2<4, true>, (const void *)k_decide2<8, true>, (const void *)k_inc_refresh, (const void *)k_inc_admit,
                         (const void *)k_inc_finish, (const void *)k_decide2<2, false, true>, (const void *)k_decide2<4, false, true>, (const void *)k_decide2<8, false, true>,
                         (const void *)k_decide2<2, true, true>, (const void *)k_decide2<4, true, true>, (const void *)k_decide2<8, true, true>,
-                        (const void *)k_large_sort<false>, (const void *)k_large_sort<true>, (const void *)k_decide_large<false>, (const void *)k_decide_large<true>,
+                        (const void *)k_large_sort<false>, (const void *)k_large_sort<true>, (const void *)k_decide_large<false>, (const void *)k_decide_large<true>, (const void *)k_inc_grow,
                         (const void *)k_huge_tiles<false>, (const void *)k_huge_tiles<true>, (const void *)k_huge_merge<false>, (const void *)k_huge_merge<true>};
     for (const void *k : ks) cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, pct);
   }
@@ -1934,10 +1979,12 @@ void kr_engine_destroy(kr_engine *e) {
   if (e->h_totals) cudaFreeHost(e->h_totals);
   if (e->h_order) cudaFreeHost(e->h_order);
   if (e->h_inc) cudaFreeHost(e->h_inc);
+  if (e->h_grow) cudaFreeHost(e->h_grow);
   if (e->h_changed) cudaFreeHost(e->h_changed);
   if (e->d_obj_stage) cudaFree(e->d_obj_stage);
   if (e->d_lg) cudaFree(e->d_lg);
   if (e->d_region) cudaFree(e->d_region);
+  if (e->d_grow) cudaFree(e->d_grow);
   if (e->d_huge) cudaFree(e->d_huge);
   if (e->d_order) cudaFree(e->d_order);
   if (e->d_in) cudaFree(e->d_in);
@@ -1987,7 +2034,7 @@ int kr_snapshot_begin(kr_engine *e, const kr_sizes *sizes, kr_snapshot_bufs *out
       e->inc_valid = false;
       e->force_radix = e->env_radix;
       e->bstride = first_stride(*sizes);
-      e->large_rows.clear(); e->large_reg.clear(); e->lg_stale = true;
+      e->large_rows.clear(); e->large_reg.clear(); e->lg_cursor = 0; e->lg_stale = true;
     }
   }
   e->sizes = *sizes;

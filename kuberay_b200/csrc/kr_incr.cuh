@@ -317,8 +317,36 @@ __global__ void __launch_bounds__(256) k_inc_refresh(SnapDev s, ScratchDev sc) {
 }
 
 // ------------------------------------------------------------------------------------------------ k_inc_admit
-// The selector match of k_match2 for the touched rows' new values (grid-stride over the touched list).
-__global__ void __launch_bounds__(256) k_inc_admit(SnapDev s, ScratchDev sc, ResDev r, Sizes n, int has_wtd) {
+// KR_OPT_LARGE_GROWTH: the grow buffer (16-byte words) holds the grow list {cluster, old region offset, old capacity, -} at
+// [0, KR_GROW_MAX), k_inc_grow's result {cluster, offset, capacity, newly listed} at [KR_GROW_MAX, 2 KR_GROW_MAX), then the spill:
+// per record a pair {pod, rank, cluster, -}, record.
+static constexpr uint32_t kGrowResult = KR_GROW_MAX, kGrowSpill = 2 * KR_GROW_MAX;
+static constexpr size_t kGrowBytes = 16 * ((size_t)kGrowSpill + 2 * (size_t)KR_GROW_SPILL);
+
+// A record of arrival rank `rank` that has no slot in RayCluster c's bucket or region waits in the spill for the region k_inc_grow
+// gives c.  The thread that meets the first rank past the room (exactly one per cluster and epoch: every record before the epoch fit)
+// puts c on the grow list, with the region it has now.  false: the list or the spill is full (the attempt is void).
+// Out of line, and given the few scratch fields it uses by value: k_inc_admit's loop keeps its registers, and no kernel parameter
+// has its address taken (that would copy the whole parameter block to local memory in every thread of the launch).
+__device__ __noinline__ bool grow_spill(const uint4 *lg, uint32_t *inc, uint32_t *pos, uint32_t stride, uint4 *grow, uint32_t c,
+                                        uint32_t rank, uint4 rec) {
+  const uint4 l = __ldcg(&lg[c]);  // (bound whenever the pass grows: 0 for an ordinary cluster)
+  if (rank == stride + l.y) {
+    const uint32_t j = atomicAdd(&inc[KR_INC_GROW], 1u);
+    if (j >= KR_GROW_MAX) return false;
+    grow[j] = make_uint4(c, l.x, l.y, 0u);
+  }
+  const uint32_t k = atomicAdd(&inc[KR_INC_SPILL], 1u);
+  if (k >= KR_GROW_SPILL) return false;
+  grow[kGrowSpill + 2 * k] = make_uint4(rec.x, rank, c, 0u);
+  grow[kGrowSpill + 2 * k + 1] = rec;
+  pos[rec.x] = rank;
+  return true;
+}
+
+// The selector match of k_match2 for the touched rows' new values (grid-stride over the touched list).  grow: the grow buffer
+// (KR_OPT_LARGE_GROWTH), nullptr: a record without a slot voids the attempt.
+__global__ void __launch_bounds__(256) k_inc_admit(SnapDev s, ScratchDev sc, ResDev r, Sizes n, int has_wtd, uint4 *grow) {
   const uint32_t n_touched = __ldcg(&sc.inc[KR_INC_TOUCHED]);
   const uint32_t epoch = inc_epoch(sc);
   if (__ldcg(&sc.inc[KR_INC_STRUCTURAL])) return;
@@ -380,8 +408,10 @@ __global__ void __launch_bounds__(256) k_inc_admit(SnapDev s, ScratchDev sc, Res
     }
     mark_dirty(sc, c, epoch);  // the row joined this cluster: a fresh record at the end of its bucket
     const uint32_t rank = atomicAdd(&sc.cl_dyn[c].x, 1u);
-    if (uint4 *at = rec_slot(sc, c, rank)) { *at = make_uint4(p, (slot << 16) | flags | KR_ROW_FRESH, ri, nm); sc.pos[p] = rank; }
-    else sc.inc[KR_INC_VOID] = 1u;  // (an ordinary RayCluster outgrew its bucket, a large one its region: the full pass reclassifies)
+    const uint4 rec = make_uint4(p, (slot << 16) | flags | KR_ROW_FRESH, ri, nm);
+    if (uint4 *at = rec_slot(sc, c, rank)) { *at = rec; sc.pos[p] = rank; }
+    // (an ordinary RayCluster outgrew its bucket, a large one its region: k_inc_grow gives it a new one, or the full pass reclassifies)
+    else if (!grow || !grow_spill(sc.lg, sc.inc, sc.pos, sc.bucket_stride, grow, c, rank, rec)) sc.inc[KR_INC_VOID] = 1u;
   }
 }
 
@@ -558,6 +588,7 @@ __global__ void __launch_bounds__(256) k_inc_groups_gather(ResDev r, ScratchDev 
 __global__ void k_inc_finish(ScratchDev sc) {
   if (threadIdx.x == 0 && blockIdx.x == 0) {
     sc.inc[KR_INC_TOUCHED] = 0; sc.inc[KR_INC_DIRTY] = 0; sc.inc[KR_INC_STRUCTURAL] = 0; sc.inc[KR_INC_HEADS] = 0; sc.inc[KR_INC_VOID] = 0; sc.inc[KR_INC_GROUPS] = 0; sc.inc[KR_INC_LSEG] = 0;
+    sc.inc[KR_INC_GROW] = 0; sc.inc[KR_INC_SPILL] = 0; sc.inc[KR_INC_GROWN] = 0;
     sc.inc[KR_INC_EPOCH] += 1u;
   }
 }

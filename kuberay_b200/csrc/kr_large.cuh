@@ -47,14 +47,92 @@ __device__ __forceinline__ void block_sort_asc(uint32_t *s, uint32_t total, uint
   }
 }
 
-// One CTA per large RayCluster (lg_list).  kInc: only the ones the epoch marked dirty.
+// ------------------------------------------------------------------------------------------------ k_inc_grow
+// KR_OPT_LARGE_GROWTH: regions for the RayClusters k_inc_admit put on the grow list (kr_incr.cuh: grow_spill), in one launch.  Every
+// CTA reads the list and reaches the same allocation: the entries by row, each final count (cl_dyn.x) sized by large_region_cap, one
+// prefix from the region cursor past every region in use.  The epoch is void (every CTA decides so alike) when a count passes
+// KR_LARGE_MAX_PODS (a huge RayCluster needs tiles), the arena has no room, or newly listed RayClusters would take the per-cluster
+// list past list_cap (a regrowth adds no one: it is never held back by the cap).  Else the
+// CTAs copy each regrown RayCluster's old region into its new one and place the spilled records; CTA 0 writes the region table and
+// the result the host and the per-cluster kernels read (a RayCluster is newly listed when it had no region and is not wide: a wide
+// one is on the list already).  No other kernel reads the table between k_inc_admit and this one, and the list kept the old regions.
+__global__ void __launch_bounds__(256) k_inc_grow(SnapDev s, ScratchDev sc, uint4 *grow, uint32_t cursor, uint32_t arena, uint32_t n_list,
+                                                  uint32_t list_cap, int wide) {
+  __shared__ uint4 s_e[KR_GROW_MAX];  // {cluster, old offset, old capacity, count}, ascending rows
+  __shared__ uint32_t s_off[KR_GROW_MAX], s_cap[KR_GROW_MAX], s_new[KR_GROW_MAX];
+  __shared__ uint32_t s_ok;
+  const uint32_t tid = threadIdx.x;
+  const uint32_t n = __ldcg(&sc.inc[KR_INC_GROW]);
+  if (n == 0 || n > KR_GROW_MAX || __ldcg(&sc.inc[KR_INC_VOID]) || __ldcg(&sc.inc[KR_INC_STRUCTURAL])) return;  // (nothing grew, or void)
+  const uint32_t S = sc.bucket_stride;
+  uint4 mine = make_uint4(0u, 0u, 0u, 0u);
+  if (tid < n) { mine = __ldcg(&grow[tid]); mine.w = __ldcg(&sc.cl_dyn[mine.x].x); }
+  uint32_t rank = 0;  // (rows are distinct: one entry per cluster)
+  for (uint32_t k = 0; k < n; k++) rank += __ldcg(&grow[k].x) < mine.x ? 1u : 0u;
+  if (tid < n) s_e[rank] = mine;
+  __syncthreads();
+  if (tid == 0) {
+    uint64_t off = cursor;
+    uint32_t listed = 0;
+    bool ok = true;
+    for (uint32_t i = 0; i < n; i++) {
+      const uint4 e = s_e[i];
+      ok = ok && e.w <= KR_LARGE_MAX_PODS;
+      const uint32_t cap = ok ? large_region_cap(e.w, S) : 0u;
+      s_off[i] = (uint32_t)off; s_cap[i] = cap;
+      off += cap;
+      s_new[i] = e.z == 0 && !(wide && s.c_group_cnt[e.x] > KR_SMEM_GROUPS);
+      listed += s_new[i];
+    }
+    s_ok = ok && off <= arena && (listed == 0 || n_list + listed <= list_cap);  // (a pure regrowth lists no one)
+  }
+  __syncthreads();
+  if (!s_ok) {
+    if (blockIdx.x == 0 && tid == 0) sc.inc[KR_INC_VOID] = 1u;
+    return;
+  }
+  for (uint32_t i = blockIdx.x; i < n; i += gridDim.x)  // a regrown RayCluster's records of ranks [stride, stride + old capacity)
+    for (uint32_t j = tid; j < s_e[i].z; j += blockDim.x) sc.region[s_off[i] + j] = __ldcg(&sc.region[s_e[i].y + j]);
+  const uint32_t n_spill = __ldcg(&sc.inc[KR_INC_SPILL]);  // (at most KR_GROW_SPILL: k_inc_admit voided the attempt otherwise)
+  for (uint32_t k = blockIdx.x * blockDim.x + tid; k < n_spill && k < KR_GROW_SPILL; k += gridDim.x * blockDim.x) {
+    const uint4 at = __ldcg(&grow[kGrowSpill + 2 * k]);
+    uint32_t lo = 0, hi = n - 1;
+    while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (s_e[mid].x < at.z) lo = mid + 1; else hi = mid; }
+    // (a record whose RayCluster is not on the list, or whose rank the new region does not hold, cannot be placed: void rather than
+    // write into another region; the full pass that follows rebuilds every bucket and region)
+    if (s_e[lo].x != at.z || at.y < S + s_e[lo].z || at.y - S >= s_cap[lo]) { sc.inc[KR_INC_VOID] = 1u; continue; }
+    sc.region[s_off[lo] + at.y - S] = __ldcg(&grow[kGrowSpill + 2 * k + 1]);
+  }
+  if (blockIdx.x == 0) {
+    if (tid < n) {
+      sc.lg[s_e[tid].x] = make_uint4(s_off[tid], s_cap[tid], 0u, 0u);
+      grow[kGrowResult + tid] = make_uint4(s_e[tid].x, s_off[tid], s_cap[tid], s_new[tid]);
+    }
+    if (tid == 0) sc.inc[KR_INC_GROWN] = n;
+  }
+}
+
+// The k-th RayCluster of k_inc_grow's result that was newly listed (KR_EMPTY32: fewer were).  The per-cluster kernels give each such
+// RayCluster one of their KR_GROW_MAX CTAs past the list.
+__device__ __forceinline__ uint32_t grown_row(const ScratchDev &sc, const uint4 *grown, uint32_t k) {
+  const uint32_t n = __ldcg(&sc.inc[KR_INC_GROWN]);
+  for (uint32_t i = 0; i < n; i++) {
+    const uint4 g = __ldcg(&grown[i]);
+    if (g.w && k-- == 0) return g.x;
+  }
+  return KR_EMPTY32;
+}
+
+// One CTA per large RayCluster (lg_list, n_list entries).  kInc: only the ones the epoch marked dirty.  grown (KR_OPT_LARGE_GROWTH:
+// k_inc_grow's result): the CTAs past the list take the newly listed RayClusters.
 template <bool kInc>
-__global__ void __launch_bounds__(kLargeSortThreads) k_large_sort(Decide2Args a, const uint32_t *__restrict__ lg_list) {
+__global__ void __launch_bounds__(kLargeSortThreads) k_large_sort(Decide2Args a, const uint32_t *__restrict__ lg_list, uint32_t n_list, const uint4 *grown) {
   __shared__ uint32_t s_idx[KR_LARGE_MAX_PODS];
   __shared__ uint32_t s_warp[kLargeSortThreads / 32];
   __shared__ uint32_t s_seg;
   const ScratchDev &sc = a.sc;
-  const uint32_t c = lg_list[blockIdx.x];
+  const uint32_t c = !kInc || blockIdx.x < n_list ? lg_list[blockIdx.x] : grown_row(sc, grown, blockIdx.x - n_list);
+  if (kInc && c == KR_EMPTY32) return;
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const uint32_t S = sc.bucket_stride;
   const uint32_t epoch = kInc ? inc_epoch_of(sc) : 0u;
@@ -123,14 +201,15 @@ __global__ void __launch_bounds__(kLargeSortThreads) k_large_sort(Decide2Args a,
 
 // One CTA per large RayCluster that k_large_sort took: warp 0 decides, every warp fills replica indices.
 template <bool kInc>
-__global__ void __launch_bounds__(kLargeDecideThreads) k_decide_large(Decide2Args a, const uint32_t *__restrict__ lg_list) {
+__global__ void __launch_bounds__(kLargeDecideThreads) k_decide_large(Decide2Args a, const uint32_t *__restrict__ lg_list, uint32_t n_list, const uint4 *grown) {
   __shared__ int32_t s_acc[4][KR_SMEM_GROUPS];
   __shared__ int32_t s_mode[2][KR_SMEM_GROUPS];
   __shared__ uint32_t s_bits[kLargeDecideThreads / 32][32];
   __shared__ uint32_t s_place[4];  // act_off, n_act, stage index, go on
   const ScratchDev &sc = a.sc;
   const ResDev &r = a.r;
-  const uint32_t c = lg_list[blockIdx.x];
+  const uint32_t c = !kInc || blockIdx.x < n_list ? lg_list[blockIdx.x] : grown_row(sc, grown, blockIdx.x - n_list);
+  if (kInc && c == KR_EMPTY32) return;
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const uint4 l = __ldcg(&sc.lg[c]);  // (written by k_large_sort: an earlier grid)
   if (!(l.w & KR_LG_OWNED)) return;

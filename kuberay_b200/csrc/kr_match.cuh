@@ -107,6 +107,7 @@ __global__ void __launch_bounds__(256) k_build_tables(SnapDev s, ScratchDev sc, 
     // and the next epoch's stamps must differ from every stamp written so far.  (Every commit kernel of this epoch has finished:
     // the pass waits for the commit stream before this kernel.)
     sc.inc[KR_INC_TOUCHED] = 0; sc.inc[KR_INC_DIRTY] = 0; sc.inc[KR_INC_STRUCTURAL] = 0; sc.inc[KR_INC_HEADS] = 0; sc.inc[KR_INC_VOID] = 0; sc.inc[KR_INC_GROUPS] = 0; sc.inc[KR_INC_LSEG] = 0;
+    sc.inc[KR_INC_GROW] = 0; sc.inc[KR_INC_SPILL] = 0; sc.inc[KR_INC_GROWN] = 0;
     sc.inc[KR_INC_EPOCH] += 1u;
   }
   if (t < n.n_clusters) {

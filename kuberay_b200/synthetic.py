@@ -409,6 +409,15 @@ def grow_clusters(snap: Snapshot, clusters, size: int) -> None:
         snap.p_ns_id[move], snap.p_cluster_name_id[move], snap.p_group_name_id[move] = snap.c_ns_id[c], snap.c_name_id[c], snap.g_name_id[g0]
 
 
+def grow_epochs(snap: Snapshot, clusters, sizes):
+    """Scale `clusters` up over several epochs, as an autoscaler does: for each size in `sizes`, grow_clusters(snap, clusters, size)
+    and yield the pod rows that changed (the Pods that joined)."""
+    for size in sizes:
+        before = (snap.p_ns_id.copy(), snap.p_cluster_name_id.copy())
+        grow_clusters(snap, clusters, size)
+        yield np.flatnonzero((snap.p_ns_id != before[0]) | (snap.p_cluster_name_id != before[1]))
+
+
 _ID_COLUMNS = ("c_ns_id", "c_name_id", "c_ext_err_msg_id", "c_old_cond_reason_id", "c_old_cond_msg_id", "c_old_head_ids", "c_svc_ip_id",
                "c_svc_name_id", "c_summary_id", "g_name_id", "w_name_id", "p_ns_id", "p_cluster_name_id", "p_group_name_id", "p_name_id",
                "p_replica_name_id", "h_ready_reason_id", "h_ready_msg_id", "h_pod_ip_id", "j_ns_id", "j_cluster_name_id", "j_summary_id")

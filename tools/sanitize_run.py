@@ -197,6 +197,29 @@ def group_edits(snap, flags, label):
     print(label, "ok:", inc, "of 2 group-edit epochs incremental", flush=True)
 
 
+def large_growth(snap, flags, label):
+    """KR_OPT_LARGE_GROWTH (kr_incr.cuh, kr_large.cuh): RayCluster 40 outgrows its bucket (a promotion: k_inc_admit spills the
+    records past the stride, k_inc_grow gives it a region and places them, the per-cluster kernels take it past their list), then its
+    region (a regrowth: the old region copied into a new one)."""
+    flags.fetch_pod_lists = 0
+    eng = Engine.for_snapshot(snap, large_clusters=True, large_growth=True)
+    eng.set_fixed_layout(True)
+    inc = 0
+    try:
+        eng.load(snap)
+        eng.reconcile(flags)
+        for rows in synthetic.grow_epochs(snap, [40], [eng.get_option(abi.OPT_BUCKET_STRIDE) + 8, 300]):
+            rows = rows.astype(np.uint32)
+            cols = [c for c, _d, _m, dim in abi.COLUMNS if dim == "pods"]
+            eng.commit_pod_values(rows, np.stack([snap.cols[c][rows].view(np.uint32) for c in cols], axis=1))
+            names = [n for n, _ in eng.reconcile_profiled(flags)["kernels"]]
+            assert "k_inc_grow" in names and "k_decide_large" in names, names
+            inc += eng.fetch().changed_clusters is not None
+    finally:
+        eng.close()
+    print(label, "ok:", inc, "of 2 growth epochs incremental", flush=True)
+
+
 def wtd_edits(snap, flags, label):
     """KR_OPT_WTD_EDITS (kr_incr.cuh): workersToDelete renames, a list grown past the old n_wtd, then every list cleared — each epoch
     rebuilds the name table on the device (k_inc_wtd_release / _clear / _insert / _resolve)."""
@@ -273,6 +296,8 @@ def main():
               "RayCluster creations")
     group_edits(*synthetic.generate(synthetic.config("C2", n_clusters=300, pods_per_cluster=20, groups=2, wtd_group_frac=0.3, recreate_frac=0.3)),
                 "worker-group edits")
+    large_growth(*synthetic.generate(synthetic.config("C2", n_clusters=300, pods_per_cluster=20, groups=2, wtd_group_frac=0.3, recreate_frac=0.3)),
+                 "RayClusters outgrowing their bucket and region")
     spec_rows(*synthetic.generate(synthetic.config("C2", n_clusters=300, pods_per_cluster=20, groups=2, recreate_frac=0.3)), "spec rows")
     wtd_edits(*synthetic.generate(synthetic.config("C2", n_clusters=300, pods_per_cluster=20, groups=2, autoscaling_frac=1.0, wtd_group_frac=0.3)),
               "workersToDelete edits")
