@@ -793,6 +793,18 @@ uint32_t huge_tile_count(uint32_t stride, uint32_t cap) { return (stride + cap +
 // k_large_sort's shared memory could not hold it.
 bool is_huge(uint32_t stride, uint32_t cap) { return stride + cap > KR_LARGE_MAX_PODS; }
 
+// Drops the large half's entries from `from` on (its rows ascending), in the device table too, and marks the list for upload.  The
+// device table holds a region for the rows of the large half only (every other entry is zero): a RayCluster created later in a row the
+// half no longer lists starts without a region, whatever the row held before.  (One span: the rows between hold zero already.)
+int drop_regions(kr_engine *e, size_t from) {
+  if (from >= e->large_rows.size()) return KR_OK;
+  const size_t r0 = e->large_rows[from], r1 = e->large_rows.back();
+  CK(cudaMemsetAsync(e->d_lg + 16 * r0, 0, 16 * (r1 - r0 + 1), e->sm));
+  e->large_rows.resize(from); e->large_reg.resize(from);
+  e->lg_stale = true;
+  return KR_OK;
+}
+
 // Rebuilds the cluster table and the list of the per-cluster kernels from the large half and, with KR_OPT_WIDE_CLUSTERS, the wide
 // RayClusters, and uploads them on stream M, ahead of the next pass.  The huge RayClusters go last, after the ones k_large_sort
 // takes, and their tiles into the tile table.  A new list length, split or tile count is a new grid of the captured graph.
@@ -800,8 +812,10 @@ int upload_lg(kr_engine *e) {
   e->lg_stale = false;
   std::vector<uint32_t> list, huge;  // (both halves ascending: a wide cluster with a region is listed once)
   std::vector<uint4> tiles;
+  const uint32_t Nc = e->sizes.n_clusters;
   for (size_t i = 0; i < e->large_rows.size(); i++) {
     const uint32_t c = e->large_rows[i], cap = e->large_reg[i].y;
+    if (c >= Nc) return fail(e, KR_E_STATE, "internal: region of RayCluster row %u, past the %u live rows", c, Nc);
     if (!is_huge(e->bstride, cap)) { list.push_back(c); continue; }
     huge.push_back(c);
     const uint32_t nt = huge_tile_count(e->bstride, cap), first = (uint32_t)tiles.size();
@@ -815,7 +829,6 @@ int upload_lg(kr_engine *e) {
   if ((uint32_t)list.size() != e->n_large || n_lsort != e->n_lsort || (uint32_t)tiles.size() != e->n_tiles) e->gvalid = false;
   e->n_large = (uint32_t)list.size(); e->n_lsort = n_lsort; e->n_tiles = (uint32_t)tiles.size();
   if (list.empty() && !grows(e)) return KR_OK;  // (an incremental pass that grows regions reads the table even then: all zero)
-  const uint32_t Nc = e->sizes.n_clusters;
   std::vector<uint4> lg(Nc, make_uint4(0, 0, 0, 0));  // a wide cluster without a region: capacity 0
   for (size_t i = 0; i < e->large_rows.size(); i++) lg[e->large_rows[i]] = make_uint4(e->large_reg[i].x, e->large_reg[i].y, 0, 0);
   CK(cudaStreamSynchronize(e->sm));  // the previous upload has left the host copies
@@ -1191,8 +1204,8 @@ int after_bucket_void(kr_engine *e) {
   std::vector<uint4> dyn(Nc);
   CK(cudaMemcpyAsync(dyn.data(), e->d_scratch + e->sl.cl_dyn, 16 * (size_t)Nc, cudaMemcpyDeviceToHost, e->sm));
   CK(cudaStreamSynchronize(e->sm));
-  e->large_rows.clear(); e->large_reg.clear(); e->lg_cursor = 0;  // (rebuilt below from this attempt's counts)
-  e->lg_stale = true;  // (uploaded below; a layout that leaves the bucket pipeline uploads nothing it would read)
+  if (int rc = drop_regions(e, 0)) return rc;  // (rebuilt below from this attempt's counts; a layout that leaves the bucket pipeline
+  e->lg_cursor = 0;                             // uploads nothing it would read)
   uint32_t st = e->bstride, n_big = 0, most = 0;
   for (const uint4 &d : dyn) { if (d.x > 256) n_big++; if (d.x <= 256) most = std::max(most, d.x); }
   if (!e->huge_on)
@@ -1213,7 +1226,7 @@ int after_bucket_void(kr_engine *e) {
     off += cap;
     if (is_huge(st, cap)) tiles += huge_tile_count(st, cap);
   }
-  if (off > e->large_entries || tiles > e->huge_tiles) { e->large_rows.clear(); e->large_reg.clear(); e->bstride = 0; return KR_OK; }
+  if (off > e->large_entries || tiles > e->huge_tiles) { e->bstride = 0; return drop_regions(e, 0); }
   e->bstride = st;
   e->lg_cursor = off;
   return upload_lg(e);  // (on the pass's stream: ordered before the rerun)
@@ -1450,6 +1463,11 @@ int run_pass(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile) {
   if (!profile) CK(cudaEventRecord(e->ev_a, e->sm));
   e->last_flags = f;
   new_pull_epoch(e);
+  // Regions of rows past the live count (a deleted large RayCluster in the last rows, whose row map voided the epoch) go: the full
+  // pass that follows would list a row it does not hold.  (Large rows at or past the count are gone rows of the map, and a map with a
+  // large gone row is never followed incrementally.)  A deleted large RayCluster's row below the count keeps its region for the
+  // RayCluster that took the row.
+  if (int rc = drop_regions(e, std::lower_bound(e->large_rows.begin(), e->large_rows.end(), e->sizes.n_clusters) - e->large_rows.begin())) return rc;
   // (the list moves with a group count, an option or a new layout, when a full pass follows, and with the RayClusters an incremental
   // epoch created)
   if (e->lg_stale) if (int rc = upload_lg(e)) return rc;
@@ -1819,6 +1837,7 @@ int kr_engine_set_option(kr_engine *e, uint32_t option, uint64_t value) {
     if (value && option != KR_OPT_HUGE_CLUSTERS && !e->d_lg) {  // the cluster table and list of the per-cluster kernels
       const size_t Nc = e->cfg.max_clusters;
       CK(cudaMalloc((void **)&e->d_lg, align_up(16 * Nc) + 4 * Nc));
+      CK(cudaMemset(e->d_lg, 0, align_up(16 * Nc)));  // (no region anywhere: see drop_regions)
     }
     if (value && option == KR_OPT_LARGE_CLUSTERS && !e->d_region) {
       // every region holds about 1.25x its cluster's pods rounded up to 32 records, and a large cluster lists more than 256 pods:
@@ -1840,7 +1859,8 @@ int kr_engine_set_option(kr_engine *e, uint32_t option, uint64_t value) {
     on = value != 0;
     // the next full pass starts again from the layout's first stride and the fast sort pipeline: a pass with the option off may
     // have left the bucket pipeline (and the fast pipeline, for a cluster above 1024 pods) for this layout
-    e->large_rows.clear(); e->large_reg.clear(); e->lg_cursor = 0; e->lg_stale = true; e->inc_valid = false; e->gvalid = false;
+    if (int rc = drop_regions(e, 0)) return rc;
+    e->lg_cursor = 0; e->lg_stale = true; e->inc_valid = false; e->gvalid = false;
     e->force_radix = e->env_radix;
     if (e->begun) e->bstride = first_stride(e->sizes);
     return KR_OK;
@@ -2034,7 +2054,8 @@ int kr_snapshot_begin(kr_engine *e, const kr_sizes *sizes, kr_snapshot_bufs *out
       e->inc_valid = false;
       e->force_radix = e->env_radix;
       e->bstride = first_stride(*sizes);
-      e->large_rows.clear(); e->large_reg.clear(); e->lg_cursor = 0; e->lg_stale = true;
+      if (int rc = drop_regions(e, 0)) return rc;
+      e->lg_cursor = 0; e->lg_stale = true;
     }
   }
   e->sizes = *sizes;

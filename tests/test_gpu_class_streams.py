@@ -16,89 +16,13 @@ import json
 import numpy as np
 import pytest
 
+from class_model import Model
+from class_model import counts as _counts
+from class_model import owners as _owners
 from harness import OBJ_COLS, SORT_KERNELS, Driver, b32, head_row, incremental, scale_to, set_phase, spec_bytes, workers
 from kuberay_b200 import abi, synthetic
 
 pytestmark = pytest.mark.gpu
-
-SMEM_GROUPS = 32
-
-
-def _owners(snap):
-    """The RayCluster every pod row belongs to (-1: none), matched on (namespace, ray.io/cluster) as k_match2 does."""
-    ckey = (snap.c_ns_id.astype(np.uint64) << np.uint64(32)) | snap.c_name_id.astype(np.uint64)
-    order = np.argsort(ckey)
-    pkey = (snap.p_ns_id.astype(np.uint64) << np.uint64(32)) | snap.p_cluster_name_id.astype(np.uint64)
-    pos = np.minimum(np.searchsorted(ckey[order], pkey), order.size - 1)
-    return np.where((ckey[order][pos] == pkey) & (snap.p_cluster_name_id != 0), order[pos], -1)
-
-
-def _counts(snap, own):
-    return np.bincount(own[own >= 0], minlength=snap.dims["clusters"])
-
-
-class Model:
-    """The engine's host-side classification (kr_engine.cu: first_stride, run_pass's ladder through after_bucket_void, upload_lg,
-    kr_engine_set_option) and the capacities an incremental epoch is checked against on the device."""
-
-    def __init__(self, n_clusters, n_pods, large, wide):
-        self.nc, self.n_pods, self.large, self.wide = n_clusters, n_pods, large, wide
-        self.reset()
-
-    def first_stride(self):
-        st, want = 64, (self.n_pods * 5 // 4 + self.nc - 1) // self.nc
-        while st < want and st < 512:
-            st <<= 1
-        return st if st <= 256 else 0
-
-    def reset(self):
-        """An option changed: the next full pass starts from the layout's first stride, without regions."""
-        self.stride, self.caps, self.valid = self.first_stride(), {}, False
-
-    def limits(self):
-        lim = np.full(self.nc, self.stride, dtype=np.int64)
-        for c, cap in self.caps.items():
-            lim[c] += cap
-        return lim
-
-    def bucket(self, groups):
-        return self.stride != 0 and (groups.max() <= SMEM_GROUPS or self.wide)
-
-    def full_pass(self, counts, groups):
-        """A full pass over `counts`: the ladder of voided bucket attempts.  -> whether it ended on the bucket pipeline."""
-        for _ in range(5):
-            if not self.bucket(groups) or not (counts > self.limits()).any():
-                break
-            self._after_void(counts)
-        self.valid = self.bucket(groups)
-        return self.valid
-
-    def _after_void(self, counts):
-        if not self.large:
-            self.stride = self.stride * 2 if self.stride * 2 <= 256 else 0
-            return
-        self.caps = {}
-        if counts.max() > abi.LARGE_MAX_PODS:
-            self.stride = 0
-            return
-        big = np.flatnonzero(counts > 256)
-        if not big.size:
-            self.stride = self.stride * 2 if self.stride * 2 <= 256 else 0
-            return
-        most, st = int(counts[counts <= 256].max(initial=0)), self.stride
-        while st < most and st * 2 <= 256:
-            st <<= 1
-        if st < most:
-            self.stride = 0
-            return
-        for c in big.tolist():
-            n = int(counts[c])
-            self.caps[c] = min((n + n // 4 + 31) // 32 * 32, abi.LARGE_MAX_PODS) - st
-        self.stride = st
-
-    def per_cluster_list(self, groups):
-        wide = set(np.flatnonzero(groups > SMEM_GROUPS).tolist()) if self.wide else set()
-        return set(self.caps) | wide
 
 
 class Stream(Driver):

@@ -1,5 +1,6 @@
-"""The native packer in the configuration production would run with every opt-in option on (KR_OPT_LARGE_CLUSTERS, _WIDE_CLUSTERS,
-_HUGE_CLUSTERS, _WTD_EDITS, _SPEC_ROWS), against a twin packer with all of them off, on the same informer event stream.
+"""The native packer with five opt-in options on (KR_OPT_LARGE_CLUSTERS, _WIDE_CLUSTERS, _HUGE_CLUSTERS, _WTD_EDITS, _SPEC_ROWS),
+against a twin packer with all of them off, on the same informer event stream.  (The structural options, KR_OPT_CLUSTER_CREATES,
+_CLUSTER_DELETES, _GROUP_EDITS and _LARGE_GROWTH, run with these in tests/test_gpu_structural_streams.py.)
 
 The fleet: about 150 RayClusters cloned from fuzz objects (multi-host groups, Recreate gates, RayJobs, every adversarial field),
 plus healthy RayClusters of about 1 500 and 8 190 Pods, one of 9 000 Pods, three of 33-40 worker groups, one of 250 Pods and one of

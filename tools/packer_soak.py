@@ -4,8 +4,9 @@ fuzz-generated object set, then epochs of mixed Pod / RayCluster / RayJob events
 epoch compared with the oracle on an independently re-packed snapshot (tests/harness.py's Mirror / packer_check).  usage (GPU box):
 python tools/packer_soak.py [first_seed] [seeds] [epochs] [--all-options] [--json-bytes N]
 
---all-options turns on every opt-in engine option (large / wide / huge RayClusters, workersToDelete edits, spec rows) and adds spec edits
-with a bumped generation to every epoch (tests/test_gpu_packer_streams.py runs the same configuration at suite length); --json-bytes sets
+--all-options turns on all nine opt-in engine options (large / wide / huge RayClusters, workersToDelete edits, spec rows, RayCluster
+creates and deletes, group edits, large growth) and adds spec edits with a bumped generation to every epoch
+(tests/test_gpu_packer_streams.py and tests/test_gpu_structural_streams.py run these options at suite length); --json-bytes sets
 kr_config.max_json_bytes, small enough (a few KiB above the fleet's muted specs) that the stream compacts the JSON arena as it goes."""
 import argparse
 import copy
@@ -29,7 +30,8 @@ ap.add_argument("epochs", nargs="?", type=int, default=30)
 ap.add_argument("--all-options", action="store_true")
 ap.add_argument("--json-bytes", type=int, default=4 << 20)
 a = ap.parse_args()
-opts = dict(large_clusters=True, wide_clusters=True, huge_clusters=True, wtd_edits=True, spec_rows=True) if a.all_options else {}
+opts = dict(large_clusters=True, wide_clusters=True, huge_clusters=True, wtd_edits=True, spec_rows=True, cluster_creates=True,
+            cluster_deletes=True, group_edits=True, large_growth=True) if a.all_options else {}
 oracle.lib()
 total = inc = 0
 for seed in range(a.first, a.first + a.seeds):
