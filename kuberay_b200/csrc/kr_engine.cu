@@ -994,9 +994,13 @@ int launch_pass(kr_engine *e, const kr_flags &f, bool profile, bool capturing = 
     else if (n.n_clusters) CK(cudaMemsetAsync(r.hash, 0, 32 * (size_t)n.n_clusters, H));
     return KR_OK;
   };
-  // where stream M needs the digests: it joins the hash stream (profiled, it runs the hash itself there)
+  // where stream M needs the digests: it joins the hash stream (profiled, it runs the hash itself there, once the JSON arena and
+  // the hash order have landed: the commit sends both after ev_cols, the only upload stream M waited for so far)
   auto join_hash = [&]() -> int {
-    if (profile) return hash_or_zero();
+    if (profile) {
+      CK(cudaStreamWaitEvent(M, e->ev_json, 0));
+      return hash_or_zero();
+    }
     CK(cudaStreamWaitEvent(M, e->ev_hash, 0));
     return KR_OK;
   };
