@@ -611,7 +611,7 @@ enum {
                               RayClusters, which it returns among changed_clusters.  Still full passes: another renumbering, a surviving
                               RayCluster whose group count changed (without KR_OPT_GROUP_EDITS), a deleted or moved key that another row also holds, more than 4 096
                               RayClusters deleted, moved or created at once, a deleted or moved RayCluster that is large
-                              (KR_OPT_LARGE_CLUSTERS: its region does not move), and, within one epoch, a renumbering after an object
+                              (KR_OPT_LARGE_CLUSTERS: one with a region) unless KR_OPT_LARGE_MOVES, and, within one epoch, a renumbering after an object
                               commit that appended RayClusters, or any object commit after a renumbering that changes a row count or
                               renumbers again.  With KR_OPT_WIDE_CLUSTERS, RayClusters of more than 32 worker groups are followed too.
                               Results are the same as with 0 (the default: every deletion makes the next pass a full one).  May be set
@@ -628,8 +628,8 @@ enum {
                               re-decides it, returning it among changed_clusters with the RayClusters whose Pods a rebuilt
                               workersToDelete name table touched.  With KR_OPT_CLUSTER_DELETES a RayCluster moved by swap-remove may
                               change its group count in the same epoch, and with KR_OPT_CLUSTER_CREATES the epoch may create
-                              RayClusters as well.  Still full passes: a regrouped RayCluster that is large (KR_OPT_LARGE_CLUSTERS: its
-                              region would have to be initialised again in place; left open), one of more than 32 worker groups without
+                              RayClusters as well.  Still full passes: a regrouped RayCluster that is large (KR_OPT_LARGE_CLUSTERS: one
+                              with a region) unless KR_OPT_LARGE_MOVES, one of more than 32 worker groups without
                               KR_OPT_WIDE_CLUSTERS, more than 4 096 RayClusters deleted, moved, created or regrouped at once, the rules
                               of KR_OPT_CLUSTER_DELETES for two object commits in one epoch, and group edits committed with
                               kr_snapshot_commit_object_rows (a changed group count falls back to the whole object part; a renamed
@@ -638,7 +638,7 @@ enum {
                               first object commit with it on records the group names, the next ones compare against them).  No effect
                               without KR_OPT_FIXED_LAYOUT.  The native packer's flush takes this path by itself when the engine has the
                               option: the regrouped RayClusters' specs travel as spec rows. */
-  KR_OPT_LARGE_GROWTH = 12    /* 1, together with KR_OPT_LARGE_CLUSTERS: a RayCluster that outgrows its room in an incremental epoch (an
+  KR_OPT_LARGE_GROWTH = 12,   /* 1, together with KR_OPT_LARGE_CLUSTERS: a RayCluster that outgrows its room in an incremental epoch (an
                               ordinary one its bucket, a large one its region, as Pods join it when it scales up) keeps the incremental
                               epoch: the pass gives it a region of the size a full pass would (1.25x its Pods rounded up to 32, at
                               most KR_LARGE_MAX_PODS, less the stride) past the regions in use, copies a large one's old region into it,
@@ -654,6 +654,20 @@ enum {
                               a full pass that widens the stride or reclassifies the fleet).  May be set at any time; read at each
                               incremental pass.  No effect without KR_OPT_LARGE_CLUSTERS.  Turning it on allocates about 0.5 MB of
                               device memory and 1 KB of pinned host memory once. */
+  KR_OPT_LARGE_MOVES = 13     /* 1, together with KR_OPT_LARGE_CLUSTERS and KR_OPT_FIXED_LAYOUT: KR_OPT_CLUSTER_DELETES and
+                              KR_OPT_GROUP_EDITS also follow large RayClusters (those with a region, huge ones included) incrementally.
+                              A deleted large RayCluster's Pods are released, bucket and region, and become orphans; its region is
+                              abandoned until the next full pass that reclassifies the fleet.  A large RayCluster moved by swap-remove
+                              carries its region (offset and capacity) and, a huge one, its tiles to its new row, and its Pods are
+                              admitted there again.  A regrouped large RayCluster keeps its region and is initialised again in place.
+                              Either one is re-decided by the per-cluster kernels in the same pass and returned among changed_clusters.
+                              Still full passes with it: the other rules of KR_OPT_CLUSTER_DELETES and KR_OPT_GROUP_EDITS (more than
+                              4 096 RayClusters in one map, two object commits in one epoch), and a moved or regrouped large RayCluster
+                              that joins more Pods than its carried region holds, unless KR_OPT_LARGE_GROWTH gives it a new region in
+                              the same pass (a huge one, of more than KR_LARGE_MAX_PODS Pods, cannot grow in an incremental epoch).
+                              Results are the same as with 0 (the default: every such epoch is a full pass).  May be set at any time;
+                              read at each object commit.  No effect without KR_OPT_LARGE_CLUSTERS and
+                              KR_OPT_FIXED_LAYOUT. */
 };
 enum { KR_LARGE_MAX_PODS = 8192 };  /* largest RayCluster KR_OPT_LARGE_CLUSTERS keeps on the bucket pipeline */
 /* KR_OPT_LARGE_GROWTH: at most KR_GROW_MAX RayClusters get a region in one incremental epoch, and an epoch that puts RayClusters on

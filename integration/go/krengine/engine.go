@@ -157,6 +157,10 @@ const (
 	// OptLargeGrowth is KR_OPT_LARGE_GROWTH (1: a RayCluster that outgrows its bucket or region in an incremental epoch gets a new
 	// region in that epoch; only with KR_OPT_LARGE_CLUSTERS; recommended for autoscaled fleets; read at each incremental pass).
 	OptLargeGrowth = uint32(C.KR_OPT_LARGE_GROWTH)
+	// OptLargeMoves is KR_OPT_LARGE_MOVES (1: KR_OPT_CLUSTER_DELETES and KR_OPT_GROUP_EDITS also keep incremental epochs when a large
+	// RayCluster is deleted, moved by swap-remove or regrouped; only with KR_OPT_LARGE_CLUSTERS and KR_OPT_FIXED_LAYOUT; recommended
+	// for RayJob fleets whose RayClusters grow large and RayService fleets; read at each object commit).
+	OptLargeMoves = uint32(C.KR_OPT_LARGE_MOVES)
 )
 
 // SetOption: KR_OPT_FIXED_LAYOUT (before the first Begin), KR_OPT_INCREMENTAL, KR_OPT_LARGE_CLUSTERS (1: RayClusters of 257 to
@@ -170,8 +174,9 @@ const (
 // Begin and object commit), KR_OPT_CLUSTER_DELETES (1, with KR_OPT_FIXED_LAYOUT: RayClusters deleted by swap-remove keep incremental
 // epochs; read at each Begin and object commit), KR_OPT_GROUP_EDITS (1, with KR_OPT_FIXED_LAYOUT: a RayCluster whose list of worker
 // groups changed keeps incremental epochs; read at each Begin and object commit), KR_OPT_LARGE_GROWTH (1, with KR_OPT_LARGE_CLUSTERS:
-// a RayCluster that outgrows its bucket or region keeps incremental epochs; read at each incremental pass).  For a Packer, call it on
-// Packer.Engine().
+// a RayCluster that outgrows its bucket or region keeps incremental epochs; read at each incremental pass), KR_OPT_LARGE_MOVES (1, with
+// KR_OPT_LARGE_CLUSTERS and KR_OPT_FIXED_LAYOUT: a large RayCluster deleted, moved or regrouped keeps incremental epochs; read at
+// each object commit).  For a Packer, call it on Packer.Engine().
 func (e *Engine) SetOption(option uint32, value uint64) error {
 	if rc := C.kr_engine_set_option(e.h, C.uint32_t(option), C.uint64_t(value)); rc != C.KR_OK {
 		return e.err(rc)

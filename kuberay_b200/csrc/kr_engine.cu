@@ -42,7 +42,7 @@ constexpr uint32_t kAdoptMax = 4096;
 // most RayClusters one incremental epoch that renumbers them (KR_OPT_CLUSTER_DELETES) or regroups them (KR_OPT_GROUP_EDITS) deletes,
 // moves, creates and regroups together; more take the full pass
 constexpr uint32_t kMapMax = 4096;
-enum MapList { MP_GONE, MP_INIT, MP_DIGESTS, MP_GSRC, MP_WSRC, MP_LISTS };  // the lists of a row map on the device, in this order
+enum MapList { MP_GONE, MP_INIT, MP_DIGESTS, MP_GSRC, MP_WSRC, MP_SGONE, MP_LARGE, MP_LISTS };  // the lists of a row map on the device, in this order
 inline size_t align_up(size_t x, size_t a = kAlign) { return (x + a - 1) / a * a; }
 inline uint32_t pow2_at_least(uint64_t x) { uint32_t p = 16; while (p < x) p <<= 1; return p; }
 // staging of an incremental pass's changed records, for up to a quarter of the RayClusters (beyond that the whole record arrays are
@@ -157,6 +157,9 @@ struct CommitRecord {
     std::vector<uint32_t> gsrc, wsrc;  // ... and came from these old ones (KR_EMPTY32: of a moved or created RayCluster)
     uint32_t g_lo = 0, g_hi = 0;     // the old groups gsrc reads
     bool names_moved = false;        // a resident workersToDelete name shifted or vanished, or a map with gone rows brought new ones
+    // KR_OPT_LARGE_MOVES, filled by commit_map when some gone row has a region: the gone rows without one, and per gone row with one
+    // {old row, region offset, region capacity, new row or KR_EMPTY32} (kr_incr.cuh: k_inc_large_release, k_inc_large_carry)
+    std::vector<uint32_t> small_gone, large;
   };
   RowMap map;
   uint32_t n_recreate = 0;           // RayClusters with KR_CF_UPGRADE_RECREATE (decide phase 1 needed): whole
@@ -566,7 +569,7 @@ struct kr_engine {
   Staging mp;                  // the row map of an object commit (rec.map), for its diff and the next pass
   bool map_pending = false;    // ... uploaded and not yet applied by a pass
   kr_sizes map_sizes{};        // ... the live counts of that object commit
-  size_t mp_at[5]{};           // offsets in mp of its lists (MapList)
+  size_t mp_at[MP_LISTS]{};     // offsets in mp of its lists (MapList)
   uint8_t *h_in_dev = nullptr;  // device-side address of h_in
   int sm_count = 148;
   // the whole pass (both streams) captured once per (layout, flags, n_recreate) and replayed
@@ -596,6 +599,7 @@ struct kr_engine {
   // from the last bucket attempt that voided, sticky like bstride) and, with KR_OPT_WIDE_CLUSTERS, the wide ones of the last commit.
   std::vector<uint32_t> large_rows; std::vector<uint2> large_reg;
   bool lg_stale = false;        // the device table / list do not reflect the two halves yet (upload_lg at the next pass)
+  bool lg_moved = false;        // KR_OPT_LARGE_MOVES: an object commit renumbered the large half: the next upload writes the table
   uint32_t n_large = 0;         // RayClusters in the device list
   uint32_t n_lsort = 0;         // ... of which the first n_lsort are k_large_sort's; the huge ones after them go to k_huge_tiles / k_huge_merge
   uint32_t n_tiles = 0;         // tiles of the huge RayClusters in the device tile table
@@ -634,6 +638,7 @@ struct kr_engine {
   bool cluster_creates = false;  // KR_OPT_CLUSTER_CREATES
   bool cluster_deletes = false;  // KR_OPT_CLUSTER_DELETES
   bool group_edits = false;      // KR_OPT_GROUP_EDITS
+  bool large_moves = false;      // KR_OPT_LARGE_MOVES
   uint32_t inc_n_clusters = 0;   // RayClusters in the resident tables
   uint32_t res_n_wtd = 0;        // names in the resident name table and its resolutions (wtd_pod_idx)
   bool ran_inc = false;          // the last pass was an incremental one
@@ -828,7 +833,10 @@ int upload_lg(kr_engine *e) {
   if (tiles.size() > e->huge_tiles) return fail(e, KR_E_STATE, "internal: %zu huge-cluster tiles, room for %zu", tiles.size(), e->huge_tiles);
   if ((uint32_t)list.size() != e->n_large || n_lsort != e->n_lsort || (uint32_t)tiles.size() != e->n_tiles) e->gvalid = false;
   e->n_large = (uint32_t)list.size(); e->n_lsort = n_lsort; e->n_tiles = (uint32_t)tiles.size();
-  if (list.empty() && !grows(e)) return KR_OK;  // (an incremental pass that grows regions reads the table even then: all zero)
+  // (an incremental pass that grows regions reads the table even then: all zero; and so does one that follows a renumbered large
+  // half, KR_OPT_LARGE_MOVES, whose vacated rows must read zero)
+  if (list.empty() && !grows(e) && !e->lg_moved) return KR_OK;
+  e->lg_moved = false;
   std::vector<uint4> lg(Nc, make_uint4(0, 0, 0, 0));  // a wide cluster without a region: capacity 0
   for (size_t i = 0; i < e->large_rows.size(); i++) lg[e->large_rows[i]] = make_uint4(e->large_reg[i].x, e->large_reg[i].y, 0, 0);
   CK(cudaStreamSynchronize(e->sm));  // the previous upload has left the host copies
@@ -1277,7 +1285,8 @@ int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile
                      : n.n_clusters != e->inc_n_clusters)
     return KR_OK;
   const bool grow = grows(e) && e->bstride;  // (KR_OPT_LARGE_GROWTH: a RayCluster that outgrows its room gets a region in this pass)
-  PassCtx c(e, profile, grow);
+  const uint32_t n_large_gone = (uint32_t)m.large.size() / 4;  // (KR_OPT_LARGE_MOVES: gone rows with a region)
+  PassCtx c(e, profile, grow || n_large_gone);
   const SnapDev &s = c.s; const ResDev &r = c.r; const ScratchDev &sc = c.sc; const Sizes &z = c.z;
   const cudaStream_t M = c.M, H = c.H;
   CK(cudaStreamWaitEvent(M, e->ev_cols, 0));
@@ -1306,9 +1315,14 @@ int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile
   }
   const int grid = e->sm_count * 2;
   // RayClusters created or renumbered (kr_incr.cuh), each step when its list of the map holds a row
-  if (n_gone) {  // the gone rows' Pods touched while the table holds the old rows
+  const uint32_t n_small_gone = n_large_gone ? (uint32_t)m.small_gone.size() : n_gone;
+  if (n_small_gone) {  // the gone rows' Pods touched while the table holds the old rows
     c.mark("k_inc_clusters_release");
-    k_inc_clusters_release<<<(32 * n_gone + 255) / 256, 256, 0, M>>>(s, sc, r, map_dev(MP_GONE), n_gone, e->inc_n_pods);
+    k_inc_clusters_release<<<(32 * n_small_gone + 255) / 256, 256, 0, M>>>(s, sc, r, map_dev(n_large_gone ? MP_SGONE : MP_GONE), n_small_gone, e->inc_n_pods);
+  }
+  if (n_large_gone) {  // ... those with a region a CTA each, their old regions from the map (the table is in the new numbering)
+    c.mark("k_inc_large_release");
+    k_inc_large_release<<<n_large_gone, 256, 0, M>>>(s, sc, r, reinterpret_cast<const uint4 *>(map_dev(MP_LARGE)), e->inc_n_pods);
   }
   if (e->rec.heads_rebuild) {  // a head Pod came or went since the table was built (the commit compared the keys on the host)
     c.mark("k_inc_aux_rebuild");
@@ -1358,6 +1372,10 @@ int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile
     const bool names = n.n_wtd > e->res_n_wtd;
     c.mark("k_inc_clusters_insert");
     k_inc_clusters_insert<<<(n_init + 255) / 256, 256, 0, M>>>(s, sc, r, map_dev(MP_INIT), n_init, names ? 1 : 0);
+    if (n_large_gone) {  // (the insert cleared their entries)
+      c.mark("k_inc_large_carry");
+      k_inc_large_carry<<<(n_large_gone + 255) / 256, 256, 0, M>>>(sc, reinterpret_cast<const uint4 *>(map_dev(MP_LARGE)), n_large_gone);
+    }
     if (names) {
       c.mark("k_inc_wtd_resolve");
       k_inc_wtd_resolve<<<std::min<uint32_t>((uint32_t)e->sm_count * 4, (n.n_pods + 255) / 256 + 1), 256, e->sl.wt_bits_n / 8, M>>>(s, sc, r, z, e->inc_n_pods, e->res_n_wtd);
@@ -1469,8 +1487,9 @@ int run_pass(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile) {
   new_pull_epoch(e);
   // Regions of rows past the live count (a deleted large RayCluster in the last rows, whose row map voided the epoch) go: the full
   // pass that follows would list a row it does not hold.  (Large rows at or past the count are gone rows of the map, and a map with a
-  // large gone row is never followed incrementally.)  A deleted large RayCluster's row below the count keeps its region for the
-  // RayCluster that took the row.
+  // large gone row is followed incrementally only with KR_OPT_LARGE_MOVES, whose commit renumbered the large half: nothing is left
+  // past the count then.)  A deleted large RayCluster's row below the count keeps its region for the RayCluster that took the row
+  // when the map was not followed.
   if (int rc = drop_regions(e, std::lower_bound(e->large_rows.begin(), e->large_rows.end(), e->sizes.n_clusters) - e->large_rows.begin())) return rc;
   // (the list moves with a group count, an option or a new layout, when a full pass follows, and with the RayClusters an incremental
   // epoch created)
@@ -1656,6 +1675,36 @@ bool deletes_on(const kr_engine *e) { return e->cluster_deletes && e->fixed_layo
 // KR_OPT_GROUP_EDITS has an effect
 bool regroups_on(const kr_engine *e) { return e->group_edits && e->fixed_layout; }
 
+// KR_OPT_LARGE_MOVES has an effect
+bool large_moves_on(const kr_engine *e) { return e->large_moves && e->large_on && e->fixed_layout && e->d_lg && e->d_region; }
+
+// KR_OPT_LARGE_MOVES: a row map the pass follows takes the large half into the new numbering (rows ascending: upload_lg, drop_regions
+// and commit_map search it).  A deleted RayCluster's region is abandoned until the next full pass that reclassifies; a moved or
+// regrouped one's goes with it to its new row.  The map lists the gone rows with a region apart (RowMap::large), since the release
+// reads their old regions after the pass's upload wrote the table in the new numbering, which leaves zero in the rows a deleted one
+// vacated.  Rows left past the count are cleared here, on stream M ahead of the pass: nothing uploads them.
+int renumber_large(kr_engine *e, CommitRecord::RowMap &m) {
+  m.small_gone.clear(); m.large.clear();
+  std::vector<std::pair<uint32_t, uint2>> half;
+  for (size_t i = 0; i < e->large_rows.size(); i++) {
+    const uint32_t o = e->large_rows[i];
+    const uint2 reg = e->large_reg[i];
+    const auto it = std::lower_bound(m.gone.begin(), m.gone.end(), o);
+    if (it == m.gone.end() || *it != o) { half.push_back({o, reg}); continue; }
+    const uint32_t to = m.moved_to[it - m.gone.begin()];
+    m.large.insert(m.large.end(), {o, reg.x, reg.y, to});
+    if (to != KR_EMPTY32) half.push_back({to, reg});
+    if (o >= e->sizes.n_clusters) CK(cudaMemsetAsync(e->d_lg + 16 * (size_t)o, 0, 16, e->sm));
+  }
+  if (m.large.empty()) return KR_OK;
+  for (uint32_t o : m.gone) if (!std::binary_search(e->large_rows.begin(), e->large_rows.end(), o)) m.small_gone.push_back(o);
+  std::sort(half.begin(), half.end(), [](const std::pair<uint32_t, uint2> &a, const std::pair<uint32_t, uint2> &b) { return a.first < b.first; });
+  e->large_rows.clear(); e->large_reg.clear();
+  for (const auto &h : half) { e->large_rows.push_back(h.first); e->large_reg.push_back(h.second); }
+  e->lg_stale = true; e->lg_moved = true;
+  return KR_OK;
+}
+
 // The column table of an object commit's diff: every object column i, staged at stage + at[i] with cnt[d] rows of its dimension d,
 // against the resident one as the record last left it.  Without row lists, staged row k is resident row k; with them (the row path)
 // it is the k-th row of the list of dimension d at stage + list_at[d], and a dimension without staged rows is left out.
@@ -1689,18 +1738,19 @@ ObjDiffArgs object_diff_args(const kr_engine *e, const uint8_t *stage, const siz
 // sets up the diff (oa).  Otherwise `voided`: the resident state does not follow this epoch, and the caller drops it once the diff
 // has copied the object part into place (the next pass is a full one, which re-hashes every spec).
 int commit_map(kr_engine *e, bool ok, ObjDiffArgs &oa, bool &voided) {
-  const CommitRecord::RowMap &m = e->rec.map;
+  CommitRecord::RowMap &m = e->rec.map;
   const kr_sizes &n = e->sizes;
-  // (a large RayCluster's region and tiles do not move with it; the old groups the gather reads are staged in the incremental staging
-  // buffer, which the pass fills only later)
+  // (a large RayCluster's region and tiles move with it only with KR_OPT_LARGE_MOVES; the old groups the gather reads are staged in
+  // the incremental staging buffer, which the pass fills only later)
   ok = ok && 36 * (size_t)(m.g_hi - m.g_lo) <= e->inc_stage.cap;
-  for (uint32_t o : m.gone) ok = ok && !std::binary_search(e->large_rows.begin(), e->large_rows.end(), o);
+  if (!large_moves_on(e)) for (uint32_t o : m.gone) ok = ok && !std::binary_search(e->large_rows.begin(), e->large_rows.end(), o);
   if (!ok) {  // (the record took the new rows' ranges as the digests' ones)
     e->rec.hash_dirty = true;
     e->map_pending = false;
     voided = true;
     return KR_OK;
   }
+  if (int rc = renumber_large(e, m)) return rc;
   // the digests the next pass computes: the created RayClusters', and the pending spec rows in the new numbering
   std::vector<uint32_t> pending;
   for (uint32_t r : e->spec_pending) {
@@ -1713,7 +1763,7 @@ int commit_map(kr_engine *e, bool ok, ObjDiffArgs &oa, bool &voided) {
   if (e->spec_stamp.size() < n.n_clusters) e->spec_stamp.resize(n.n_clusters, 0u);
   for (uint32_t c : pending)
     if (e->spec_stamp[c] != e->spec_epoch) { e->spec_stamp[c] = e->spec_epoch; e->spec_pending.push_back(c); }
-  const std::vector<uint32_t> *lists[MP_LISTS] = {&m.gone, &m.init, &m.digests, &m.gsrc, &m.wsrc};
+  const std::vector<uint32_t> *lists[MP_LISTS] = {&m.gone, &m.init, &m.digests, &m.gsrc, &m.wsrc, &m.small_gone, &m.large};
   size_t bytes = 0;
   for (int i = 0; i < MP_LISTS; i++) { e->mp_at[i] = bytes; bytes += align_up(4 * lists[i]->size(), 16); }
   CK(e->mp.wait());
@@ -1824,6 +1874,10 @@ int kr_engine_set_option(kr_engine *e, uint32_t option, uint64_t value) {
     e->group_edits = value != 0;
     return KR_OK;
   }
+  if (option == KR_OPT_LARGE_MOVES) {  // (read at each object commit)
+    e->large_moves = value != 0;
+    return KR_OK;
+  }
   if (option == KR_OPT_LARGE_GROWTH) {  // (read at each incremental pass)
     if (value && !e->d_grow) {
       CK(cudaSetDevice(e->cfg.device));
@@ -1887,6 +1941,7 @@ int kr_engine_get_option(kr_engine *e, uint32_t option, uint64_t *value) {
     case KR_OPT_CLUSTER_DELETES: *value = e->cluster_deletes; return KR_OK;
     case KR_OPT_GROUP_EDITS: *value = e->group_edits; return KR_OK;
     case KR_OPT_LARGE_GROWTH: *value = e->large_growth; return KR_OK;
+    case KR_OPT_LARGE_MOVES: *value = e->large_moves; return KR_OK;
     case KR_OPT_BUCKET_STRIDE: *value = e->bstride; return KR_OK;
     default: return fail(e, KR_E_INVALID, "unknown option %u", option);
   }
@@ -1978,8 +2033,9 @@ int kr_engine_create(const kr_config *cfg, kr_engine **out) {
     if (cudaMalloc((void **)&e->d_obj_stage, objs) != cudaSuccess) return bail(KR_E_CUDA);
     e->obj_stage_cap = objs;
     if (e->inc_stage.reserve(inc_stage_layout(cfg->max_clusters, cfg->max_groups).total, 0) != cudaSuccess) return bail(KR_E_CUDA);
-    // the largest row map: gone / digests of kMapMax rows, every RayCluster created, every group and name shifted
-    if (e->mp.reserve(4 * (3 * (size_t)kMapMax + cfg->max_clusters + cfg->max_groups + cfg->max_wtd) + MP_LISTS * 16, 0) != cudaSuccess) return bail(KR_E_CUDA);
+    // the largest row map: gone / digests of kMapMax rows, every RayCluster created, every group and name shifted, and with
+    // KR_OPT_LARGE_MOVES the gone rows once more and four words per gone row
+    if (e->mp.reserve(4 * (8 * (size_t)kMapMax + cfg->max_clusters + cfg->max_groups + cfg->max_wtd) + MP_LISTS * 16, 0) != cudaSuccess) return bail(KR_E_CUDA);
     const size_t chg = std::max<size_t>(1024, (size_t)cfg->max_clusters);
     if (cudaHostAlloc((void **)&e->h_changed, 4 * chg, cudaHostAllocDefault) != cudaSuccess) return bail(KR_E_CUDA);
     e->h_changed_cap = chg;

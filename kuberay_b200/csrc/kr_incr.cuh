@@ -452,6 +452,8 @@ __global__ void __launch_bounds__(256) k_inc_admit(SnapDev s, ScratchDev sc, Res
 //                              name any resident Pod.  It resolves the new names and touches the rows that hit one.  A row of a new
 //                              RayCluster was an orphan and k_inc_orphan_adopt touched it already; any other resident row still
 //                              probes to the RayCluster that holds it (the lowest row keeps a duplicate key).
+// (KR_OPT_LARGE_MOVES adds two steps for gone rows that have a region: k_inc_large_release beside k_inc_clusters_release, and
+// k_inc_large_carry right behind k_inc_clusters_insert; see there.)
 // Places in the action list and create arena that a gone RayCluster held are abandoned until the next full pass.
 // k_inc_clusters_insert and k_inc_orphan_adopt take the `init` RayClusters as the ascending row list `rows` of n entries.
 __global__ void __launch_bounds__(256) k_inc_clusters_insert(SnapDev s, ScratchDev sc, ResDev r, const uint32_t *rows, uint32_t n, int names) {
@@ -538,6 +540,46 @@ __global__ void __launch_bounds__(256) k_inc_clusters_release(SnapDev s, Scratch
     if (r.act_cnt[o]) atomicSub(&r.totals[2], r.act_cnt[o]);
     if (cre) atomicSub(&r.totals[6], cre);
   }
+}
+
+// KR_OPT_LARGE_MOVES: the gone rows that have a region (large RayClusters deleted, moved or regrouped) are listed apart, as
+// {old row, region offset, region capacity, new row or KR_EMPTY32}, and k_inc_clusters_release takes only the others.  The host
+// uploaded the region table in the new numbering at the start of the pass, so the old regions come from the list:
+//   k_inc_large_release  one CTA per listed row (a 2 000-Pod row is 8 iterations per thread, not 63 per lane of one warp): the work of
+//                        k_inc_clusters_release for ranks [0, stride) in the bucket and [stride, stride + capacity) in the region;
+//   k_inc_large_carry    behind k_inc_clusters_insert, which cleared the entry of every init row: a moved or regrouped RayCluster's
+//                        region back into the table at its new row ({offset, capacity}, no sorted segment yet), so k_inc_admit
+//                        brings its Pods into the bucket and then the carried region.  Every record before the epoch fits it, so
+//                        with KR_OPT_LARGE_GROWTH exactly one record meets the first rank past it (grow_spill).
+__global__ void __launch_bounds__(256) k_inc_large_release(SnapDev s, ScratchDev sc, ResDev r, const uint4 *gone, uint32_t n_resident) {
+  __shared__ uint32_t s_cre[8];
+  const uint4 g = gone[blockIdx.x];
+  const uint32_t o = g.x, S = sc.bucket_stride, epoch = inc_epoch(sc), tid = threadIdx.x;
+  const uint32_t P = min(__ldcg(&sc.cl_dyn[o].x), S + g.z);
+  for (uint32_t k = tid; k < P; k += blockDim.x) {
+    const uint4 *at = k < S ? sc.bucket + (size_t)o * S + k : sc.region + g.y + (k - S);
+    uint32_t ns, nm;
+    inc_touch(s, sc, r, at->x, epoch, n_resident, ns, nm);
+  }
+  const uint4 rec = sc.cl_rec[o];  // {group_off, group_cnt} of the old row
+  uint32_t cre = 0;
+  for (uint32_t gi = rec.x + tid; gi < rec.x + rec.y; gi += blockDim.x) cre += r.groups[gi].n_create;
+  cre = __reduce_add_sync(0xFFFFFFFFu, cre);
+  if ((tid & 31) == 0) s_cre[tid >> 5] = cre;
+  __syncthreads();
+  if (tid == 0) {
+    cre = 0;
+    for (uint32_t w = 0; w < blockDim.x / 32; w++) cre += s_cre[w];
+    if (r.act_cnt[o]) atomicSub(&r.totals[2], r.act_cnt[o]);
+    if (cre) atomicSub(&r.totals[6], cre);
+  }
+}
+
+__global__ void __launch_bounds__(256) k_inc_large_carry(ScratchDev sc, const uint4 *gone, uint32_t n) {
+  const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;
+  if (i >= n) return;
+  const uint4 g = gone[i];
+  if (g.w != KR_EMPTY32) sc.lg[g.w] = make_uint4(g.y, g.z, 0u, 0u);
 }
 
 __global__ void __launch_bounds__(1024) k_inc_clusters_translate(ScratchDev sc, const uint32_t *gone, uint32_t n_gone, uint32_t n_clusters) {

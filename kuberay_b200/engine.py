@@ -235,7 +235,8 @@ class Engine:
     def for_snapshot(cls, snap: Snapshot, device: int = 0, max_creates: int | None = None, slack: float = 1.0,
                      large_clusters: bool = False, wide_clusters: bool = False, huge_clusters: bool = False,
                      wtd_edits: bool = False, spec_rows: bool = False, cluster_creates: bool = False,
-                     cluster_deletes: bool = False, group_edits: bool = False, large_growth: bool = False) -> "Engine":
+                     cluster_deletes: bool = False, group_edits: bool = False, large_growth: bool = False,
+                     large_moves: bool = False) -> "Engine":
         d = snap.dims
         up = lambda x: int(x * slack) + 1  # noqa: E731
         if max_creates is None:
@@ -260,6 +261,8 @@ class Engine:
             eng.set_group_edits(True)
         if large_growth:
             eng.set_large_growth(True)
+        if large_moves:
+            eng.set_large_moves(True)
         return eng
 
     def _check(self, rc: int):
@@ -334,6 +337,12 @@ class Engine:
         """KR_OPT_LARGE_GROWTH: with set_large_clusters, a RayCluster that outgrows its bucket or region in an incremental epoch (it
         scaled up) gets a new region in that epoch instead of making the pass a full one; read at each incremental pass."""
         self._check(self._L.kr_engine_set_option(self._h, abi.OPT_LARGE_GROWTH, 1 if on else 0))
+
+    def set_large_moves(self, on: bool = True):
+        """KR_OPT_LARGE_MOVES: with set_large_clusters under the fixed layout, set_cluster_deletes and set_group_edits also keep
+        incremental epochs when a large RayCluster (one with a region) is deleted, moved by swap-remove or regrouped: a moved or
+        regrouped one carries its region; read at each object commit."""
+        self._check(self._L.kr_engine_set_option(self._h, abi.OPT_LARGE_MOVES, 1 if on else 0))
 
     def get_option(self, option: int) -> int:
         """kr_engine_get_option: an option's current value, or the read-only OPT_BUCKET_STRIDE (0: the sort pipeline)."""

@@ -220,6 +220,42 @@ def large_growth(snap, flags, label):
     print(label, "ok:", inc, "of 2 growth epochs incremental", flush=True)
 
 
+def large_moves(snap, flags, label, grown, edits, huge=False):
+    """KR_OPT_LARGE_MOVES (kr_incr.cuh): the RayClusters `grown` made large, then each edit of `edits` in an epoch of its own: ("delete",
+    rows) by swap-remove, or ("regroup", row) a worker group appended.  A large gone row is released by k_inc_large_release from its
+    old region while the table is in the new numbering, and a moved or regrouped one's region goes back into the table behind
+    k_inc_clusters_insert (k_inc_large_carry)."""
+    flags.fetch_pod_lists = 0
+    synthetic.grow_clusters(snap, grown, 9000 if huge else 600)
+    eng = Engine.for_snapshot(snap, slack=1.25, large_clusters=True, huge_clusters=huge, cluster_deletes=True, group_edits=True, large_moves=True)
+    eng.set_fixed_layout(True)
+    inc = 0
+    try:
+        views = eng.load(snap)
+        eng.reconcile(flags)
+        eng.reconcile(flags)
+        eng.commit(abi.PART_OBJECTS)  # (records the group names for the regroup)
+        eng.reconcile(flags)
+        for kind, arg in edits:
+            if kind == "delete":
+                snap = synthetic.delete_clusters(snap, arg)
+            else:
+                g0 = int(snap.c_group_off[arg])
+                groups = [(g, None) for g in range(g0, g0 + int(snap.c_group_cnt[arg]))]
+                snap = synthetic.regroup_clusters(snap, {arg: groups + [(g0, int(snap.g_name_id.max()) + 1)]})
+            views = eng.begin(snap.sizes())
+            for c, _dt, _m, dim in abi.COLUMNS:
+                if dim not in ("pods", "json"):
+                    np.copyto(views[c], snap.cols[c])
+            eng.commit(abi.PART_OBJECTS)
+            names = [n for n, _ in eng.reconcile_profiled(flags)["kernels"]]
+            assert "k_inc_large_release" in names, names
+            inc += eng.fetch().changed_clusters is not None
+    finally:
+        eng.close()
+    print(label, "ok:", inc, f"of {len(edits)} epochs incremental", flush=True)
+
+
 def wtd_edits(snap, flags, label):
     """KR_OPT_WTD_EDITS (kr_incr.cuh): workersToDelete renames, a list grown past the old n_wtd, then every list cleared — each epoch
     rebuilds the name table on the device (k_inc_wtd_release / _clear / _insert / _resolve)."""
@@ -298,6 +334,12 @@ def main():
                 "worker-group edits")
     large_growth(*synthetic.generate(synthetic.config("C2", n_clusters=300, pods_per_cluster=20, groups=2, wtd_group_frac=0.3, recreate_frac=0.3)),
                  "RayClusters outgrowing their bucket and region")
+    large_moves(*synthetic.generate(synthetic.config("C2", n_clusters=300, pods_per_cluster=20, groups=2, wtd_group_frac=0.3, recreate_frac=0.3)),
+                "large RayCluster deleted in a middle row, a large one moving into it", [120, 299], [("delete", [120])])
+    large_moves(*synthetic.generate(synthetic.config("C2", n_clusters=300, pods_per_cluster=20, groups=2, wtd_group_frac=0.3, recreate_frac=0.3)),
+                "large RayCluster regrouped", [150], [("regroup", 150)])
+    large_moves(*synthetic.generate(synthetic.config("C2", n_clusters=800, pods_per_cluster=20, groups=2)),
+                "huge RayCluster moved, then deleted", [799], [("delete", [10]), ("delete", [10])], huge=True)
     spec_rows(*synthetic.generate(synthetic.config("C2", n_clusters=300, pods_per_cluster=20, groups=2, recreate_frac=0.3)), "spec rows")
     wtd_edits(*synthetic.generate(synthetic.config("C2", n_clusters=300, pods_per_cluster=20, groups=2, autoscaling_frac=1.0, wtd_group_frac=0.3)),
               "workersToDelete edits")
