@@ -648,13 +648,13 @@ enum {
                               Still full passes: more than KR_GROW_MAX RayClusters outgrowing their room at once, promotions that
                               would take the per-cluster list past max(KR_GROW_LIST_MIN, n_clusters / KR_GROW_LIST_DIV) RayClusters (a
                               regrowth alone adds no one to the list and is never held back by it), a RayCluster of more than
-                              KR_LARGE_MAX_PODS Pods (a huge one, KR_OPT_HUGE_CLUSTERS, needs tiles), a full region arena (regions a
+                              KR_LARGE_MAX_PODS Pods (a huge one needs tiles) unless KR_OPT_HUGE_GROWTH, a full region arena (regions a
                               regrowth abandons are reclaimed by the next full pass that reclassifies) and more than KR_GROW_SPILL Pods
                               joining grown RayClusters in one epoch.  Results are the same as with 0 (the default: each such epoch is
                               a full pass that widens the stride or reclassifies the fleet).  May be set at any time; read at each
                               incremental pass.  No effect without KR_OPT_LARGE_CLUSTERS.  Turning it on allocates about 0.5 MB of
                               device memory and 1 KB of pinned host memory once. */
-  KR_OPT_LARGE_MOVES = 13     /* 1, together with KR_OPT_LARGE_CLUSTERS and KR_OPT_FIXED_LAYOUT: KR_OPT_CLUSTER_DELETES and
+  KR_OPT_LARGE_MOVES = 13,    /* 1, together with KR_OPT_LARGE_CLUSTERS and KR_OPT_FIXED_LAYOUT: KR_OPT_CLUSTER_DELETES and
                               KR_OPT_GROUP_EDITS also follow large RayClusters (those with a region, huge ones included) incrementally.
                               A deleted large RayCluster's Pods are released, bucket and region, and become orphans; its region is
                               abandoned until the next full pass that reclassifies the fleet.  A large RayCluster moved by swap-remove
@@ -664,10 +664,25 @@ enum {
                               Still full passes with it: the other rules of KR_OPT_CLUSTER_DELETES and KR_OPT_GROUP_EDITS (more than
                               4 096 RayClusters in one map, two object commits in one epoch), and a moved or regrouped large RayCluster
                               that joins more Pods than its carried region holds, unless KR_OPT_LARGE_GROWTH gives it a new region in
-                              the same pass (a huge one, of more than KR_LARGE_MAX_PODS Pods, cannot grow in an incremental epoch).
-                              Results are the same as with 0 (the default: every such epoch is a full pass).  May be set at any time;
-                              read at each object commit.  No effect without KR_OPT_LARGE_CLUSTERS and
-                              KR_OPT_FIXED_LAYOUT. */
+                              the same pass (one that grows past KR_LARGE_MAX_PODS Pods also needs KR_OPT_HUGE_GROWTH: its carried
+                              tiles are retired and new ones appended).  Results are the same as with 0 (the default: every such
+                              epoch is a full pass).  May be set at any time; read at each object commit.  No effect without
+                              KR_OPT_LARGE_CLUSTERS and KR_OPT_FIXED_LAYOUT. */
+  KR_OPT_HUGE_GROWTH = 14     /* 1, together with KR_OPT_LARGE_CLUSTERS, KR_OPT_HUGE_CLUSTERS and KR_OPT_LARGE_GROWTH: a RayCluster that
+                              grows past KR_LARGE_MAX_PODS Pods in an incremental epoch (a large one that scales past it, an ordinary
+                              one that jumps past it, or a huge one that outgrows its region) keeps the incremental epoch: the pass
+                              gives it a region of the size a full pass would (1.25x its Pods rounded up to 32, less the stride),
+                              appends its tiles to the KR_HUGE_GROW_TILES reserve entries of the tile table (retiring a huge one's
+                              old tiles), and sorts and decides it with the tile kernels in the same pass.  The stride does not move,
+                              and the grown RayClusters are among changed_clusters.  Still full passes: more tiles than
+                              KR_HUGE_GROW_TILES appended in one epoch (a RayCluster regrown to about 200 000 Pods or more), more
+                              resident tiles than the engine's capacities hold, and the limits of KR_OPT_LARGE_GROWTH: more than
+                              KR_GROW_SPILL Pods waiting for new regions, a full region arena, the per-cluster list cap and more than
+                              KR_GROW_MAX RayClusters growing at once.  Results are the same as with 0 (the default: each such epoch
+                              is a full pass that lays every region out again).  May be set at any time; read at each incremental
+                              pass.  No effect without the three other options.  Turning it on allocates the tile scratch with
+                              KR_HUGE_GROW_TILES more tiles (64 KB of device memory each); an engine whose KR_OPT_HUGE_CLUSTERS had
+                              allocated it reallocates it. */
 };
 enum { KR_LARGE_MAX_PODS = 8192 };  /* largest RayCluster KR_OPT_LARGE_CLUSTERS keeps on the bucket pipeline */
 /* KR_OPT_LARGE_GROWTH: at most KR_GROW_MAX RayClusters get a region in one incremental epoch, and an epoch that puts RayClusters on
@@ -675,6 +690,9 @@ enum { KR_LARGE_MAX_PODS = 8192 };  /* largest RayCluster KR_OPT_LARGE_CLUSTERS 
  * RayClusters); beyond either, the epoch is a full pass, so a fleet that grows as a whole still widens its stride.  At most
  * KR_GROW_SPILL records of grown RayClusters wait for their new regions in one epoch. */
 enum { KR_GROW_MAX = 64, KR_GROW_LIST_MIN = 64, KR_GROW_LIST_DIV = 64, KR_GROW_SPILL = 16384 };
+/* KR_OPT_HUGE_GROWTH: tile-table entries kept free past the resident tiles for the RayClusters an incremental epoch makes huge or
+ * regrows (KR_LARGE_MAX_PODS arrival ranks each: 262 144 in all). */
+enum { KR_HUGE_GROW_TILES = 32 };
 int kr_engine_set_option(kr_engine *e, uint32_t option, uint64_t value);
 /* Current value of an option (KR_OPT_*), and the read-only KR_OPT_BUCKET_STRIDE. */
 int kr_engine_get_option(kr_engine *e, uint32_t option, uint64_t *value);

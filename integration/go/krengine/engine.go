@@ -161,6 +161,10 @@ const (
 	// RayCluster is deleted, moved by swap-remove or regrouped; only with KR_OPT_LARGE_CLUSTERS and KR_OPT_FIXED_LAYOUT; recommended
 	// for RayJob fleets whose RayClusters grow large and RayService fleets; read at each object commit).
 	OptLargeMoves = uint32(C.KR_OPT_LARGE_MOVES)
+	// OptHugeGrowth is KR_OPT_HUGE_GROWTH (1: a RayCluster that grows past KR_LARGE_MAX_PODS Pods, or a huge one that outgrows its
+	// region, in an incremental epoch gets a new region and tiles in that epoch; only with KR_OPT_LARGE_CLUSTERS, KR_OPT_HUGE_CLUSTERS
+	// and KR_OPT_LARGE_GROWTH; recommended for fleets of very large autoscaled RayClusters; read at each incremental pass).
+	OptHugeGrowth = uint32(C.KR_OPT_HUGE_GROWTH)
 )
 
 // SetOption: KR_OPT_FIXED_LAYOUT (before the first Begin), KR_OPT_INCREMENTAL, KR_OPT_LARGE_CLUSTERS (1: RayClusters of 257 to
@@ -176,7 +180,9 @@ const (
 // groups changed keeps incremental epochs; read at each Begin and object commit), KR_OPT_LARGE_GROWTH (1, with KR_OPT_LARGE_CLUSTERS:
 // a RayCluster that outgrows its bucket or region keeps incremental epochs; read at each incremental pass), KR_OPT_LARGE_MOVES (1, with
 // KR_OPT_LARGE_CLUSTERS and KR_OPT_FIXED_LAYOUT: a large RayCluster deleted, moved or regrouped keeps incremental epochs; read at
-// each object commit).  For a Packer, call it on Packer.Engine().
+// each object commit), KR_OPT_HUGE_GROWTH (1, with KR_OPT_LARGE_CLUSTERS, KR_OPT_HUGE_CLUSTERS and KR_OPT_LARGE_GROWTH: a RayCluster
+// that grows past KR_LARGE_MAX_PODS Pods keeps incremental epochs; read at each incremental pass).  For a Packer, call it on
+// Packer.Engine().
 func (e *Engine) SetOption(option uint32, value uint64) error {
 	if rc := C.kr_engine_set_option(e.h, C.uint32_t(option), C.uint64_t(value)); rc != C.KR_OK {
 		return e.err(rc)

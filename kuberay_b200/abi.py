@@ -93,6 +93,8 @@ OPT_CLUSTER_DELETES = 10
 OPT_GROUP_EDITS = 11
 OPT_LARGE_GROWTH = 12
 OPT_LARGE_MOVES = 13
+OPT_HUGE_GROWTH = 14
+HUGE_GROW_TILES = 32
 LARGE_MAX_PODS = 8192
 SPEC_JSON_UNMUTED = 1
 KR_OK, KR_E_INVALID, KR_E_CAPACITY, KR_E_CUDA, KR_E_STATE, KR_E_NO_DEVICE = 0, -1, -2, -3, -4, -5

@@ -614,6 +614,10 @@ struct kr_engine {
   uint8_t *d_huge = nullptr;
   size_t huge_tiles = 0;
   std::vector<uint4> h_tiles;
+  // KR_OPT_HUGE_GROWTH: the tile scratch holds huge_reserve (KR_HUGE_GROW_TILES once the option was first turned on) more tiles
+  // past the huge_tiles resident ones, where k_inc_grow appends the tiles of the RayClusters it makes huge or regrows
+  bool huge_growth = false;
+  size_t huge_reserve = 0;
   // KR_OPT_LARGE_GROWTH, allocated when first turned on: the grow buffer of the incremental pass (kGrowBytes: list, result, spill)
   // and a pinned copy of its result; lg_cursor is the region arena's first entry past every region in use (after_bucket_void lays
   // them out from 0, each growth allocates past it)
@@ -768,6 +772,8 @@ cudaError_t launch_pdl(void (*kern)(KArgs...), dim3 grid, dim3 block, size_t sme
 
 // An incremental pass may give RayClusters regions (KR_OPT_LARGE_GROWTH): the engine's bucket layout has a region arena and table.
 bool grows(const kr_engine *e) { return e->large_growth && e->large_on && e->d_grow && e->d_region && e->d_lg; }
+// ... and make RayClusters huge, with tiles in the reserve entries of the tile table (KR_OPT_HUGE_GROWTH).
+bool huge_grows(const kr_engine *e) { return e->huge_growth && e->huge_on && e->huge_reserve && grows(e); }
 
 // Points the pass at the cluster table of the per-cluster kernels when their list is not empty, or the pass may grow regions
 // (`grow`); returns the device list.
@@ -782,7 +788,7 @@ const uint32_t *bind_large(const kr_engine *e, ScratchDev &sc, bool grow) {
 HugeDev bind_huge(const kr_engine *e) {
   HugeDev h{};
   if (!e->d_huge) return h;
-  const size_t T = e->huge_tiles;
+  const size_t T = e->huge_tiles + e->huge_reserve;
   uint8_t *b = e->d_huge;
   h.tiles = reinterpret_cast<const uint4 *>(b); b += align_up(16 * T);
   h.cnt = reinterpret_cast<uint32_t *>(b); b += align_up(4 * T);
@@ -794,6 +800,29 @@ HugeDev bind_huge(const kr_engine *e) {
 size_t huge_bytes(size_t T) { return align_up(16 * T) + 2 * align_up(4 * T) + 2 * align_up(4 * (size_t)kHugeTile * T); }
 // Tiles a huge RayCluster's bucket and region take: its arrival ranks [0, stride + region capacity) in kHugeTile-rank tiles.
 uint32_t huge_tile_count(uint32_t stride, uint32_t cap) { return (stride + cap + kHugeTile - 1) / kHugeTile; }
+// Resident tiles of the tile scratch: a huge cluster's tiles cover about 1.25x its pods rounded up to 32, plus at most one partial
+// tile, and it lists more than KR_LARGE_MAX_PODS pods: this many tiles hold those of any snapshot within the capacities.
+size_t resident_tiles(const kr_config &cfg) {
+  const size_t Np = cfg.max_pods, n_huge = Np / (KR_LARGE_MAX_PODS + 1);
+  return (Np * 5 / 4 + 32 * (n_huge + 1)) / kHugeTile + n_huge + 2;
+}
+// Allocates the tile scratch for huge_tiles resident tiles and `reserve` more, zeroed (the per-cluster tile counters start at 0;
+// every pass leaves them there).  A scratch allocated before goes once the new one is in place (between passes: the captured graph
+// and the table go with it); when the allocation fails, the engine keeps the old scratch and its reserve.
+int alloc_huge(kr_engine *e, size_t reserve) {
+  const size_t T = e->huge_tiles + reserve;
+  uint8_t *d = nullptr;
+  CK(cudaMalloc((void **)&d, huge_bytes(T)));
+  if (cudaMemset(d, 0, huge_bytes(T)) != cudaSuccess) { cudaFree(d); return fail(e, KR_E_CUDA, "tile scratch of %zu tiles", T); }
+  if (e->d_huge) {
+    CK(cudaStreamSynchronize(e->sm));
+    CK(cudaFree(e->d_huge));
+  }
+  e->d_huge = d;
+  e->huge_reserve = reserve;
+  e->lg_stale = true; e->gvalid = false;
+  return KR_OK;
+}
 // A RayCluster of the large half is huge when its region reaches past KR_LARGE_MAX_PODS ranks (it listed more than that many pods):
 // k_large_sort's shared memory could not hold it.
 bool is_huge(uint32_t stride, uint32_t cap) { return stride + cap > KR_LARGE_MAX_PODS; }
@@ -833,6 +862,8 @@ int upload_lg(kr_engine *e) {
   if (tiles.size() > e->huge_tiles) return fail(e, KR_E_STATE, "internal: %zu huge-cluster tiles, room for %zu", tiles.size(), e->huge_tiles);
   if ((uint32_t)list.size() != e->n_large || n_lsort != e->n_lsort || (uint32_t)tiles.size() != e->n_tiles) e->gvalid = false;
   e->n_large = (uint32_t)list.size(); e->n_lsort = n_lsort; e->n_tiles = (uint32_t)tiles.size();
+  // (KR_OPT_HUGE_GROWTH: the reserve entries past the resident tiles free again, whatever the last incremental pass appended)
+  if (huge_grows(e)) tiles.resize(tiles.size() + e->huge_reserve, make_uint4(KR_EMPTY32, 0, 0, 0));
   // (an incremental pass that grows regions reads the table even then: all zero; and so does one that follows a renumbered large
   // half, KR_OPT_LARGE_MOVES, whose vacated rows must read zero)
   if (list.empty() && !grows(e) && !e->lg_moved) return KR_OK;
@@ -966,15 +997,16 @@ cudaError_t launch_decide2(const PassCtx &c, const Decide2Args &da, dim3 grid, b
 }
 
 // The sorts of the per-cluster kernels' RayClusters (kr_large.cuh): k_large_sort for the first n_lsort of the list (and, with `grown`,
-// k_inc_grow's result, for the RayClusters it listed), the huge ones after them tile by tile, then merged (kr_huge.cuh).
+// k_inc_grow's result, for the RayClusters it listed), the huge ones after them tile by tile, then merged (kr_huge.cuh).  reserve:
+// the tile table's reserve entries too (KR_OPT_HUGE_GROWTH, incremental: k_inc_grow may have appended tiles there).
 template <bool kInc>
-void launch_large_sort(PassCtx &c, const Decide2Args &da, const uint4 *grown = nullptr) {
+void launch_large_sort(PassCtx &c, const Decide2Args &da, const uint4 *grown = nullptr, uint32_t reserve = 0) {
   const kr_engine *e = c.e;
-  const uint32_t n = e->n_lsort + (grown ? KR_GROW_MAX : 0);
+  const uint32_t n = e->n_lsort + (grown ? KR_GROW_MAX : 0), nt = e->n_tiles + reserve;
   if (n) { c.mark("k_large_sort"); k_large_sort<kInc><<<n, kLargeSortThreads, 0, c.M>>>(da, c.lg_list, e->n_lsort, grown); }
-  if (e->n_tiles) {
-    c.mark("k_huge_tiles"); k_huge_tiles<kInc><<<e->n_tiles, kHugeThreads, 0, c.M>>>(da, c.hd);
-    c.mark("k_huge_merge"); k_huge_merge<kInc><<<e->n_tiles, kHugeThreads, 0, c.M>>>(da, c.hd);
+  if (nt) {
+    c.mark("k_huge_tiles"); k_huge_tiles<kInc><<<nt, kHugeThreads, 0, c.M>>>(da, c.hd);
+    c.mark("k_huge_merge"); k_huge_merge<kInc><<<nt, kHugeThreads, 0, c.M>>>(da, c.hd);
   }
 }
 
@@ -1285,6 +1317,7 @@ int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile
                      : n.n_clusters != e->inc_n_clusters)
     return KR_OK;
   const bool grow = grows(e) && e->bstride;  // (KR_OPT_LARGE_GROWTH: a RayCluster that outgrows its room gets a region in this pass)
+  const bool huge_grow = grow && huge_grows(e);  // (KR_OPT_HUGE_GROWTH: ... past KR_LARGE_MAX_PODS Pods too, with tiles)
   const uint32_t n_large_gone = (uint32_t)m.large.size() / 4;  // (KR_OPT_LARGE_MOVES: gone rows with a region)
   PassCtx c(e, profile, grow || n_large_gone);
   const SnapDev &s = c.s; const ResDev &r = c.r; const ScratchDev &sc = c.sc; const Sizes &z = c.z;
@@ -1388,7 +1421,12 @@ int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile
   if (grow) {  // regions for the RayClusters that outgrew their room (most launches find the grow list empty and leave at once)
     c.mark("k_inc_grow");
     const uint32_t list_cap = std::max<uint32_t>(KR_GROW_LIST_MIN, n.n_clusters / KR_GROW_LIST_DIV);
-    k_inc_grow<<<e->sm_count, 256, 0, M>>>(s, sc, e->d_grow, (uint32_t)e->lg_cursor, (uint32_t)e->large_entries, e->n_large, list_cap, e->wide_on ? 1 : 0);
+    if (huge_grow)
+      k_inc_grow<true><<<e->sm_count, 256, 0, M>>>(s, sc, e->d_grow, (uint32_t)e->lg_cursor, (uint32_t)e->large_entries, e->n_large, list_cap,
+                                                    e->wide_on ? 1 : 0, const_cast<uint4 *>(c.hd.tiles), e->n_tiles, (uint32_t)e->huge_tiles);
+    else
+      k_inc_grow<false><<<e->sm_count, 256, 0, M>>>(s, sc, e->d_grow, (uint32_t)e->lg_cursor, (uint32_t)e->large_entries, e->n_large, list_cap,
+                                                     e->wide_on ? 1 : 0, nullptr, 0u, 0u);
   }
   if ((do_hash || n_rows) && !profile) CK(cudaStreamWaitEvent(M, e->ev_hash, 0));
   const IncStageLayout sl = e->inc_layout = inc_stage_layout(n.n_clusters, n.n_groups);  // staging for the changed records
@@ -1408,7 +1446,7 @@ int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile
     if (e->n_large || grow) {  // the dirty large RayClusters (k_decide2 left every cluster past the stride alone), and those k_inc_grow listed
       const uint4 *grown = grow ? e->d_grow + kGrowResult : nullptr;
       CK(cudaMemsetAsync(sc.inc + KR_INC_LSEG, 0, 4, M));
-      launch_large_sort<true>(c, da, grown);
+      launch_large_sort<true>(c, da, grown, huge_grow ? (uint32_t)e->huge_reserve : 0u);
       c.mark("k_decide_large");
       k_decide_large<true><<<e->n_large + (grow ? KR_GROW_MAX : 0), kLargeDecideThreads, 0, M>>>(da, c.lg_list, e->n_large, grown);
     }
@@ -1878,6 +1916,16 @@ int kr_engine_set_option(kr_engine *e, uint32_t option, uint64_t value) {
     e->large_moves = value != 0;
     return KR_OK;
   }
+  if (option == KR_OPT_HUGE_GROWTH) {  // (read at each incremental pass)
+    if (value && e->huge_reserve < KR_HUGE_GROW_TILES) {
+      CK(cudaSetDevice(e->cfg.device));
+      if (!e->d_huge) e->huge_tiles = resident_tiles(e->cfg);  // (KR_OPT_HUGE_CLUSTERS then finds the scratch allocated)
+      if (int rc = alloc_huge(e, KR_HUGE_GROW_TILES)) return rc;
+    }
+    e->huge_growth = value != 0;
+    e->lg_stale = true;  // (the next pass uploads the reserve entries free)
+    return KR_OK;
+  }
   if (option == KR_OPT_LARGE_GROWTH) {  // (read at each incremental pass)
     if (value && !e->d_grow) {
       CK(cudaSetDevice(e->cfg.device));
@@ -1906,13 +1954,8 @@ int kr_engine_set_option(kr_engine *e, uint32_t option, uint64_t value) {
       e->large_entries = entries;
     }
     if (value && option == KR_OPT_HUGE_CLUSTERS && !e->d_huge) {
-      // a huge cluster's tiles cover about 1.25x its pods rounded up to 32, plus at most one partial tile, and it lists more than
-      // KR_LARGE_MAX_PODS pods: this many tiles hold those of any snapshot within the capacities
-      const size_t Np = e->cfg.max_pods, n_huge = Np / (KR_LARGE_MAX_PODS + 1);
-      const size_t T = (Np * 5 / 4 + 32 * (n_huge + 1)) / kHugeTile + n_huge + 2;
-      CK(cudaMalloc((void **)&e->d_huge, huge_bytes(T)));
-      CK(cudaMemset(e->d_huge, 0, huge_bytes(T)));  // (the per-cluster tile counters start at 0; every pass leaves them there)
-      e->huge_tiles = T;
+      e->huge_tiles = resident_tiles(e->cfg);
+      if (int rc = alloc_huge(e, 0)) return rc;
     }
     on = value != 0;
     // the next full pass starts again from the layout's first stride and the fast sort pipeline: a pass with the option off may
@@ -1942,6 +1985,7 @@ int kr_engine_get_option(kr_engine *e, uint32_t option, uint64_t *value) {
     case KR_OPT_GROUP_EDITS: *value = e->group_edits; return KR_OK;
     case KR_OPT_LARGE_GROWTH: *value = e->large_growth; return KR_OK;
     case KR_OPT_LARGE_MOVES: *value = e->large_moves; return KR_OK;
+    case KR_OPT_HUGE_GROWTH: *value = e->huge_growth; return KR_OK;
     case KR_OPT_BUCKET_STRIDE: *value = e->bstride; return KR_OK;
     default: return fail(e, KR_E_INVALID, "unknown option %u", option);
   }
@@ -2011,7 +2055,7 @@ int kr_engine_create(const kr_config *cfg, kr_engine **out) {
                         (const void *)k_inc_mark_recreate, (const void *)k_decide2<2, true>, (const void *)k_decide2<4, true>, (const void *)k_decide2<8, true>, (const void *)k_inc_refresh, (const void *)k_inc_admit,
                         (const void *)k_inc_finish, (const void *)k_decide2<2, false, true>, (const void *)k_decide2<4, false, true>, (const void *)k_decide2<8, false, true>,
                         (const void *)k_decide2<2, true, true>, (const void *)k_decide2<4, true, true>, (const void *)k_decide2<8, true, true>,
-                        (const void *)k_large_sort<false>, (const void *)k_large_sort<true>, (const void *)k_decide_large<false>, (const void *)k_decide_large<true>, (const void *)k_inc_grow,
+                        (const void *)k_large_sort<false>, (const void *)k_large_sort<true>, (const void *)k_decide_large<false>, (const void *)k_decide_large<true>, (const void *)k_inc_grow<false>, (const void *)k_inc_grow<true>,
                         (const void *)k_huge_tiles<false>, (const void *)k_huge_tiles<true>, (const void *)k_huge_merge<false>, (const void *)k_huge_merge<true>};
     for (const void *k : ks) cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, pct);
   }

@@ -16,14 +16,15 @@
 //                  previous one.  In an incremental epoch it also rewrites the bucket and region compacted in arrival order from
 //                  the stash (pos[] follows, cl_dyn[c].x takes the kept count): a tile's compacted ranks overlap its predecessors'
 //                  records, so this waits for the grid after the one that read them.
-// Both run on stream M between k_large_sort and the join with the hash stream; their grids are the tile count.
+// Both run on stream M between k_large_sort and the join with the hash stream; their grids are the tile count (in an incremental
+// pass with KR_OPT_HUGE_GROWTH, also the KR_HUGE_GROW_TILES reserve entries past it, where k_inc_grow appends the tiles of the
+// RayClusters it makes huge or regrows; a free entry, and a resident tile it retired, has the cluster word KR_EMPTY32).
 #pragma once
 
 #include "kr_large.cuh"
 
 namespace kr {
 
-static constexpr int kHugeTile = KR_LARGE_MAX_PODS;   // arrival ranks per tile
 static constexpr int kHugeThreads = 1024;
 static constexpr int kHugePer = kHugeTile / kHugeThreads;  // keys per thread in k_huge_merge
 
@@ -52,6 +53,7 @@ __global__ void __launch_bounds__(kHugeThreads) k_huge_tiles(Decide2Args a, Huge
   __shared__ uint32_t s_go;
   const ScratchDev &sc = a.sc;
   const uint4 t = h.tiles[blockIdx.x];
+  if (t.x == KR_EMPTY32) return;  // a free reserve entry, or a tile k_inc_grow retired (KR_OPT_HUGE_GROWTH)
   const uint32_t c = t.x, r0 = t.y;
   const uint32_t tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const uint32_t S = sc.bucket_stride;
@@ -119,6 +121,7 @@ __global__ void __launch_bounds__(kHugeThreads) k_huge_merge(Decide2Args a, Huge
   __shared__ uint32_t s_run[kHugeTile];  // another tile's run
   const ScratchDev &sc = a.sc;
   const uint4 t = h.tiles[blockIdx.x];
+  if (t.x == KR_EMPTY32) return;  // (as in k_huge_tiles)
   const uint32_t c = t.x, me = blockIdx.x, tid = threadIdx.x;
   const uint4 l = __ldcg(&sc.lg[c]);  // (written by k_huge_tiles: an earlier grid)
   if (!(l.w & KR_LG_OWNED)) return;

@@ -25,6 +25,7 @@ namespace kr {
 
 static constexpr int kLargeSortThreads = 512;
 static constexpr int kLargeDecideThreads = 128;
+static constexpr int kHugeTile = KR_LARGE_MAX_PODS;  // arrival ranks per tile of a huge RayCluster (kr_huge.cuh)
 
 // Ascending bitonic sort of s[0, total) in shared memory, padded to the next power of two (at least 2) with 0xFFFFFFFF: s must
 // hold that many words.  Every thread of the CTA calls it; the stores of s[0, total) are ordered before by its first barrier.
@@ -51,13 +52,19 @@ __device__ __forceinline__ void block_sort_asc(uint32_t *s, uint32_t total, uint
 // KR_OPT_LARGE_GROWTH: regions for the RayClusters k_inc_admit put on the grow list (kr_incr.cuh: grow_spill), in one launch.  Every
 // CTA reads the list and reaches the same allocation: the entries by row, each final count (cl_dyn.x) sized by large_region_cap, one
 // prefix from the region cursor past every region in use.  The epoch is void (every CTA decides so alike) when a count passes
-// KR_LARGE_MAX_PODS (a huge RayCluster needs tiles), the arena has no room, or newly listed RayClusters would take the per-cluster
-// list past list_cap (a regrowth adds no one: it is never held back by the cap).  Else the
+// KR_LARGE_MAX_PODS (a huge RayCluster needs tiles) without kHuge, the arena has no room, or newly listed RayClusters would take the
+// per-cluster list past list_cap (a regrowth adds no one: it is never held back by the cap).  Else the
 // CTAs copy each regrown RayCluster's old region into its new one and place the spilled records; CTA 0 writes the region table and
 // the result the host and the per-cluster kernels read (a RayCluster is newly listed when it had no region and is not wide: a wide
 // one is on the list already).  No other kernel reads the table between k_inc_admit and this one, and the list kept the old regions.
+// kHuge (KR_OPT_HUGE_GROWTH): a RayCluster whose new region reaches past KR_LARGE_MAX_PODS ranks is huge.  CTA 0 appends its tiles
+// (kr_huge.cuh) to the KR_HUGE_GROW_TILES reserve entries at tiles[n_tiles, ...) and retires a huge one's old tiles among the
+// n_tiles resident ones (cluster word KR_EMPTY32: k_huge_tiles and k_huge_merge pass over them); the epoch is also void when the
+// appended tiles pass the reserve or the resident tiles would pass tile_cap.  A huge old region (up to about 25 000 records) is
+// copied by every CTA of the launch.
+template <bool kHuge>
 __global__ void __launch_bounds__(256) k_inc_grow(SnapDev s, ScratchDev sc, uint4 *grow, uint32_t cursor, uint32_t arena, uint32_t n_list,
-                                                  uint32_t list_cap, int wide) {
+                                                  uint32_t list_cap, int wide, uint4 *tiles, uint32_t n_tiles, uint32_t tile_cap) {
   __shared__ uint4 s_e[KR_GROW_MAX];  // {cluster, old offset, old capacity, count}, ascending rows
   __shared__ uint32_t s_off[KR_GROW_MAX], s_cap[KR_GROW_MAX], s_new[KR_GROW_MAX];
   __shared__ uint32_t s_ok;
@@ -73,17 +80,20 @@ __global__ void __launch_bounds__(256) k_inc_grow(SnapDev s, ScratchDev sc, uint
   __syncthreads();
   if (tid == 0) {
     uint64_t off = cursor;
-    uint32_t listed = 0;
+    uint32_t listed = 0, added = 0, retired = 0;
     bool ok = true;
     for (uint32_t i = 0; i < n; i++) {
       const uint4 e = s_e[i];
-      ok = ok && e.w <= KR_LARGE_MAX_PODS;
+      ok = ok && (kHuge || e.w <= KR_LARGE_MAX_PODS);
       const uint32_t cap = ok ? large_region_cap(e.w, S) : 0u;
       s_off[i] = (uint32_t)off; s_cap[i] = cap;
       off += cap;
       s_new[i] = e.z == 0 && !(wide && s.c_group_cnt[e.x] > KR_SMEM_GROUPS);
       listed += s_new[i];
+      if (kHuge && S + cap > KR_LARGE_MAX_PODS) added += (S + cap + kHugeTile - 1) / kHugeTile;
+      if (kHuge && S + e.z > KR_LARGE_MAX_PODS) retired += (S + e.z + kHugeTile - 1) / kHugeTile;  // (upload_lg cut them alike)
     }
+    ok = ok && (!kHuge || (added <= KR_HUGE_GROW_TILES && n_tiles + added <= tile_cap + retired));
     s_ok = ok && off <= arena && (listed == 0 || n_list + listed <= list_cap);  // (a pure regrowth lists no one)
   }
   __syncthreads();
@@ -92,7 +102,12 @@ __global__ void __launch_bounds__(256) k_inc_grow(SnapDev s, ScratchDev sc, uint
     return;
   }
   for (uint32_t i = blockIdx.x; i < n; i += gridDim.x)  // a regrown RayCluster's records of ranks [stride, stride + old capacity)
-    for (uint32_t j = tid; j < s_e[i].z; j += blockDim.x) sc.region[s_off[i] + j] = __ldcg(&sc.region[s_e[i].y + j]);
+    if (!kHuge || s_e[i].z <= KR_LARGE_MAX_PODS)
+      for (uint32_t j = tid; j < s_e[i].z; j += blockDim.x) sc.region[s_off[i] + j] = __ldcg(&sc.region[s_e[i].y + j]);
+  if (kHuge)  // ... a huge old region over the whole launch
+    for (uint32_t i = 0; i < n; i++)
+      if (s_e[i].z > KR_LARGE_MAX_PODS)
+        for (uint32_t j = blockIdx.x * blockDim.x + tid; j < s_e[i].z; j += gridDim.x * blockDim.x) sc.region[s_off[i] + j] = __ldcg(&sc.region[s_e[i].y + j]);
   const uint32_t n_spill = __ldcg(&sc.inc[KR_INC_SPILL]);  // (at most KR_GROW_SPILL: k_inc_admit voided the attempt otherwise)
   for (uint32_t k = blockIdx.x * blockDim.x + tid; k < n_spill && k < KR_GROW_SPILL; k += gridDim.x * blockDim.x) {
     const uint4 at = __ldcg(&grow[kGrowSpill + 2 * k]);
@@ -109,6 +124,23 @@ __global__ void __launch_bounds__(256) k_inc_grow(SnapDev s, ScratchDev sc, uint
       grow[kGrowResult + tid] = make_uint4(s_e[tid].x, s_off[tid], s_cap[tid], s_new[tid]);
     }
     if (tid == 0) sc.inc[KR_INC_GROWN] = n;
+    if (kHuge) {
+      for (uint32_t t = tid; t < n_tiles; t += blockDim.x) {  // the regrown huge RayClusters' resident tiles
+        const uint32_t c = tiles[t].x;
+        uint32_t lo = 0, hi = n - 1;
+        while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (s_e[mid].x < c) lo = mid + 1; else hi = mid; }
+        if (s_e[lo].x == c) tiles[t].x = KR_EMPTY32;
+      }
+      if (tid == 0) {
+        uint32_t k = n_tiles;
+        for (uint32_t i = 0; i < n; i++) {
+          const uint32_t span = S + s_cap[i];
+          if (span <= KR_LARGE_MAX_PODS) continue;
+          const uint32_t nt = (span + kHugeTile - 1) / kHugeTile, first = k;
+          for (uint32_t t = 0; t < nt; t++) tiles[k++] = make_uint4(s_e[i].x, t * kHugeTile, first, nt);
+        }
+      }
+    }
   }
 }
 
@@ -146,7 +178,8 @@ __global__ void __launch_bounds__(kLargeSortThreads) k_large_sort(Decide2Args a,
     // a large cluster past the stride, within its region; a wide one (k_decide2 leaves it alone) also with every pod in its bucket.
     // Else k_decide2 decides it, or the attempt is void (k_match2 / k_inc_admit flagged it: a wide cluster without a region has cap 0)
     const bool wide = a.s.c_group_cnt[c] > KR_SMEM_GROUPS;
-    s_seg = go && (P > S ? P - S <= cap : wide);
+    // (and never one that k_inc_grow made huge this pass, KR_OPT_HUGE_GROWTH: s_idx holds KR_LARGE_MAX_PODS ranks, its tiles sort it)
+    s_seg = go && (P > S ? P - S <= cap : wide) && S + cap <= KR_LARGE_MAX_PODS;
   }
   __syncthreads();
   if (!s_seg) return;

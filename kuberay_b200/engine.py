@@ -236,7 +236,7 @@ class Engine:
                      large_clusters: bool = False, wide_clusters: bool = False, huge_clusters: bool = False,
                      wtd_edits: bool = False, spec_rows: bool = False, cluster_creates: bool = False,
                      cluster_deletes: bool = False, group_edits: bool = False, large_growth: bool = False,
-                     large_moves: bool = False) -> "Engine":
+                     large_moves: bool = False, huge_growth: bool = False) -> "Engine":
         d = snap.dims
         up = lambda x: int(x * slack) + 1  # noqa: E731
         if max_creates is None:
@@ -263,6 +263,8 @@ class Engine:
             eng.set_large_growth(True)
         if large_moves:
             eng.set_large_moves(True)
+        if huge_growth:
+            eng.set_huge_growth(True)
         return eng
 
     def _check(self, rc: int):
@@ -343,6 +345,12 @@ class Engine:
         incremental epochs when a large RayCluster (one with a region) is deleted, moved by swap-remove or regrouped: a moved or
         regrouped one carries its region; read at each object commit."""
         self._check(self._L.kr_engine_set_option(self._h, abi.OPT_LARGE_MOVES, 1 if on else 0))
+
+    def set_huge_growth(self, on: bool = True):
+        """KR_OPT_HUGE_GROWTH: with set_large_clusters, set_huge_clusters and set_large_growth, a RayCluster that grows past
+        LARGE_MAX_PODS Pods in an incremental epoch (or a huge one that outgrows its region) gets a region and tiles in that epoch
+        instead of making the pass a full one; read at each incremental pass."""
+        self._check(self._L.kr_engine_set_option(self._h, abi.OPT_HUGE_GROWTH, 1 if on else 0))
 
     def get_option(self, option: int) -> int:
         """kr_engine_get_option: an option's current value, or the read-only OPT_BUCKET_STRIDE (0: the sort pipeline)."""

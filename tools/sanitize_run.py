@@ -256,6 +256,41 @@ def large_moves(snap, flags, label, grown, edits, huge=False):
     print(label, "ok:", inc, f"of {len(edits)} epochs incremental", flush=True)
 
 
+def huge_growth(snap, flags, label, grown, size, steps, move=False):
+    """KR_OPT_HUGE_GROWTH (kr_large.cuh, kr_huge.cuh): RayCluster `grown` (made `size` Pods) scales to each of `steps` in an epoch of
+    its own: past KR_LARGE_MAX_PODS (k_inc_grow<true> appends its tiles to the reserve entries, k_large_sort passes it over), or past
+    a huge one's region (its resident tiles retired, its old region copied by the whole launch).  move: first an ordinary RayCluster
+    deleted by swap-remove, so that the huge last row moves into its hole, carrying its tiles, and grows in the same epoch."""
+    flags.fetch_pod_lists = 0
+    synthetic.grow_clusters(snap, [grown], size)
+    eng = Engine.for_snapshot(snap, slack=1.25, max_creates=1 << 18, large_clusters=True, huge_clusters=True, large_growth=True,
+                              huge_growth=True, cluster_deletes=move, large_moves=move)
+    eng.set_fixed_layout(True)
+    cols = [c for c, _d, _m, dim in abi.COLUMNS if dim == "pods"]
+    inc = 0
+    try:
+        views = eng.load(snap)
+        eng.reconcile(flags)
+        eng.reconcile(flags)
+        if move:
+            snap = synthetic.delete_clusters(snap, [12])
+            views = eng.begin(snap.sizes())
+            for c, _dt, _m, dim in abi.COLUMNS:
+                if dim not in ("pods", "json"):
+                    np.copyto(views[c], snap.cols[c])
+            eng.commit(abi.PART_OBJECTS)
+            grown = 12
+        for rows in synthetic.grow_epochs(snap, [grown], steps):
+            rows = rows.astype(np.uint32)
+            eng.commit_pod_values(rows, np.stack([snap.cols[c][rows].view(np.uint32) for c in cols], axis=1))
+            names = [n for n, _ in eng.reconcile_profiled(flags)["kernels"]]
+            assert "k_inc_grow" in names and "k_huge_tiles" in names, names
+            inc += eng.fetch().changed_clusters is not None
+    finally:
+        eng.close()
+    print(label, "ok:", inc, f"of {len(steps)} growth epochs incremental", flush=True)
+
+
 def wtd_edits(snap, flags, label):
     """KR_OPT_WTD_EDITS (kr_incr.cuh): workersToDelete renames, a list grown past the old n_wtd, then every list cleared — each epoch
     rebuilds the name table on the device (k_inc_wtd_release / _clear / _insert / _resolve)."""
@@ -340,6 +375,12 @@ def main():
                 "large RayCluster regrouped", [150], [("regroup", 150)])
     large_moves(*synthetic.generate(synthetic.config("C2", n_clusters=800, pods_per_cluster=20, groups=2)),
                 "huge RayCluster moved, then deleted", [799], [("delete", [10]), ("delete", [10])], huge=True)
+    huge_growth(*synthetic.generate(synthetic.config("C2", n_clusters=1300, pods_per_cluster=20, groups=2)),
+                "large RayCluster crossing 8 192 Pods", 600, 8000, [8300])
+    huge_growth(*synthetic.generate(synthetic.config("C2", n_clusters=1300, pods_per_cluster=20, groups=2)),
+                "huge RayCluster outgrowing its region", 600, 9000, [11400])
+    huge_growth(*synthetic.generate(synthetic.config("C2", n_clusters=1400, pods_per_cluster=16, groups=2)),
+                "huge RayCluster moved by swap-remove and grown", 1399, 9000, [11400], move=True)
     spec_rows(*synthetic.generate(synthetic.config("C2", n_clusters=300, pods_per_cluster=20, groups=2, recreate_frac=0.3)), "spec rows")
     wtd_edits(*synthetic.generate(synthetic.config("C2", n_clusters=300, pods_per_cluster=20, groups=2, autoscaling_frac=1.0, wtd_group_frac=0.3)),
               "workersToDelete edits")
