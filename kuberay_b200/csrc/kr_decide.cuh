@@ -392,90 +392,32 @@ __device__ __forceinline__ void warp_bitonic_sort_striped(uint32_t (&v)[K], uint
   }
 }
 
-// reconcilePods (raycluster_controller.go:619-935) + calculateStatus for one RayCluster, by one warp.
-// K > 0: the cluster's bucket (<= 32*K pods) is sorted and kept in registers — pod index pidx[k] and row word pw[k] of list
-// position k*32+lane — so the two scans below touch no memory.  K == 0: positions are read from sorted_pod_idx / rows
-// (radix pipeline, buckets larger than 256 pods, and phase 1).
-template <int K, bool kMH>
-__device__ __forceinline__ void decide_cluster(const DecideArgs &a, const uint32_t c, const uint32_t seg0, const uint32_t seg1,
-                                               uint32_t (&pidx)[K ? K : 1], uint32_t (&pw)[K ? K : 1],
-                                               int32_t (&s_acc)[4][KR_SMEM_GROUPS], int32_t (&s_mode)[2][KR_SMEM_GROUPS], const uint32_t lane) {
+// The scalar middle of reconcilePods for one RayCluster, by one warp (uniformly; lane 0 stores), from the scan-1 counters
+// (acc_list / acc_unh / acc_wtd per worker group): the path, the head decision and every worker group's record, n_create and mode
+// and delete-prefix length (g_mode / g_prefix, or gacc when those are null).  all_action: the action of every pod (delete-all
+// paths).  Shared by the warp decide (decide_cluster) and the block decide (decide_cluster_block).  -> false when phase 0 defers
+// the cluster to phase 1 (its Recreate gate needs the digest).
+template <bool kMH>
+__device__ __forceinline__ bool decide_cluster_scalar(const DecideArgs &a, const uint32_t c, const uint32_t seg0, const uint32_t seg1, const uint32_t cf,
+                                                      const uint32_t G, const uint32_t g0, const uint8_t suspend_status, const uint8_t ext_err,
+                                                      const uint8_t old_prov, const int32_t n_heads, const int32_t head_pod, const int32_t *acc_list,
+                                                      const int32_t *acc_unh, const int32_t *acc_wtd, int32_t *g_mode, int32_t *g_prefix,
+                                                      kr_cluster_result &cr, uint32_t &head_name, uint8_t &all_action, bool &head_delete,
+                                                      bool &run_groups, const uint32_t lane) {
   const SnapDev &s = a.s;
-  const uint32_t lt = lanemask_lt();
-  const uint32_t P = seg1 - seg0;
-  const uint32_t nchunks = (P + 31) / 32;
-  // cluster scalars: independent read-only loads, issued together
-  const uint32_t cf = LDG(s.c_flags[c]);
-  const uint32_t G = LDG(s.c_group_cnt[c]), g0 = LDG(s.c_group_off[c]);
-  const uint8_t suspend_status = LDG(s.c_suspend_status[c]);
-  const uint8_t ext_err = LDG(s.c_ext_err_kind[c]);
-  const uint8_t old_prov = LDG(s.c_old_cond_status[5 * (size_t)c + KR_COND_PROVISIONED]);
   const bool gate = a.f.gate_status_conditions != 0;
-
-  // accumulators: shared memory for the common case, global scratch for clusters with many groups
-  int32_t *acc_list, *acc_unh, *acc_wtd, *acc_rank, *g_mode, *g_prefix;
-  if (G <= KR_SMEM_GROUPS) {
-    acc_list = s_acc[0]; acc_unh = s_acc[1]; acc_wtd = s_acc[2]; acc_rank = s_acc[3];
-    g_mode = s_mode[0]; g_prefix = s_mode[1];
-    if (lane < KR_SMEM_GROUPS) { acc_list[lane] = 0; acc_unh[lane] = 0; acc_wtd[lane] = 0; acc_rank[lane] = 0; g_mode[lane] = GM_UNPROCESSED; g_prefix[lane] = 0; }
-  } else {
-    const uint32_t Ng = a.n.n_groups;
-    acc_list = a.sc.gacc + g0; acc_unh = a.sc.gacc + Ng + g0; acc_wtd = a.sc.gacc + 2 * (size_t)Ng + g0; acc_rank = a.sc.gacc + 3 * (size_t)Ng + g0;
-    g_mode = nullptr; g_prefix = nullptr;  // modes recycle the n_list / n_unhealthy cells once they are consumed
-    for (uint32_t gi = lane; gi < G; gi += 32) { acc_list[gi] = 0; acc_unh[gi] = 0; acc_wtd[gi] = 0; acc_rank[gi] = 0; }
-  }
-  __syncwarp();
-
-  // ---------------- scan 1: counts over the cluster's pods (list order)
-  int32_t ready = 0, available = 0, n_heads = 0;
-  bool all_running = P > 0;  // CheckAllPodsRunning (utils/util.go:584-603)
-  int32_t head_pod = -1;     // first head in list order
-#pragma unroll
-  for (int k = 0; k < (K ? K : 1 << 30); k++) {
-    if ((uint32_t)k >= nchunks) break;
-    const uint32_t i = seg0 + k * 32 + lane;
-    const bool valid = i < seg1;
-    uint32_t pod, w;
-    if (K) { pod = pidx[K ? k : 0]; w = pw[K ? k : 0]; }
-    else { pod = valid ? LDG(a.r.sorted_pod_idx[i]) : 0u; w = valid ? reinterpret_cast<const uint32_t *>(a.sc.rows)[4 * (size_t)pod + 3] : 0u; }
-    const uint32_t fl = w & 0xFFFFu, slot = valid ? (w >> 16) : KR_ROW_NO_GROUP;
-    const uint32_t nt = pp_node_type(fl), ph = pp_phase(fl), rd = pp_ready(fl);
-    const bool w_run = valid && nt == KR_NT_WORKER && ph == KR_PHASE_RUNNING;
-    available += __popc(__ballot_sync(0xFFFFFFFFu, w_run));
-    ready += __popc(__ballot_sync(0xFFFFFFFFu, w_run && rd == KR_COND_TRUE));
-    const bool not_ok = valid && (ph != KR_PHASE_RUNNING || rd == KR_COND_FALSE || rd == KR_COND_UNKNOWN);
-    if (__any_sync(0xFFFFFFFFu, not_ok)) all_running = false;
-    const uint32_t hb = __ballot_sync(0xFFFFFFFFu, valid && nt == KR_NT_HEAD);
-    if (hb) { if (n_heads == 0) head_pod = (int32_t)__shfl_sync(0xFFFFFFFFu, pod, __ffs(hb) - 1); n_heads += __popc(hb); }
-    // warp-ballot group-by on the group slot
-    const uint32_t gkey = (slot < G) ? slot : KR_ROW_NO_GROUP;
-    const uint32_t peers = __match_any_sync(0xFFFFFFFFu, gkey);
-    if (gkey != KR_ROW_NO_GROUP) {
-      const uint32_t ub = __ballot_sync(peers, should_delete(fl));
-      const uint32_t wb = __ballot_sync(peers, (fl & KR_ROW_WTD_OWN) != 0);
-      if ((peers & lt) == 0) {  // leader of its group in this chunk
-        acc_list[gkey] += __popc(peers);
-        acc_unh[gkey] += __popc(ub & peers);
-        acc_wtd[gkey] += __popc(wb & peers);
-      }
-    }
-    __syncwarp();
-  }
-
-  uint32_t head_flags = 0, head_name = 0;
+  uint32_t head_flags = 0; head_name = 0;
   if (n_heads > 0) { uint4 hrow = __ldg(&a.sc.rows[head_pod]); head_flags = hrow.w & 0xFFFFu; head_name = hrow.x; }
 
-  // ---------------- scalar decisions (uniform across the warp)
-  kr_cluster_result cr;
   {
     uint32_t *z = reinterpret_cast<uint32_t *>(&cr);
 #pragma unroll
     for (int k = 0; k < (int)(sizeof(cr) / 4); k++) z[k] = 0;
   }
   cr.head_pod_idx = -1; cr.stop_after_group = -1; cr.pod_start = seg0;
-  uint8_t all_action = KR_ACT_KEEP;  // action applied to every pod of the cluster (delete-all paths)
-  bool head_delete = false;
-  bool run_groups = false;
+  all_action = KR_ACT_KEEP;
+  head_delete = false;
+  run_groups = false;
 
   if (cf & KR_CF_SKIP) {
     cr.path = KR_PATH_SKIPPED;
@@ -497,7 +439,7 @@ __device__ __forceinline__ void decide_cluster(const DecideArgs &a, const uint32
       else if (ast == KR_ANNOT_HASH32 && !a.f.skip_hash) {
         if (a.phase == 0) {  // the hash kernel runs concurrently on another stream: decide this cluster in phase 1
           if (lane == 0) a.sc.deferred_list[atomicAdd(&a.r.totals[4], 1u)] = c;
-          return;
+          return false;
         }
         const uint8_t *ah = s.h_annot_hash + 32 * (size_t)aux;
         const char *hh = a.r.hash + 32 * (size_t)c;
@@ -589,6 +531,97 @@ __device__ __forceinline__ void decide_cluster(const DecideArgs &a, const uint32
     }
   }
   __syncwarp();
+  return true;
+}
+
+// The RayCluster's record (calculateStatus on top of the decisions, except for a skipped cluster) and its action count.  Lane 0.
+__device__ __forceinline__ void decide_cluster_record(const DecideArgs &a, const uint32_t c, const uint32_t cf, kr_cluster_result &cr, const uint32_t P,
+                                                      const int32_t n_heads, const int32_t head_pod, const uint32_t head_name, const int32_t ready,
+                                                      const int32_t available, const bool all_running, const uint32_t n_act) {
+  if (!(cf & KR_CF_SKIP))
+    status_rollup(a.s, a.f, ColumnsCI{a.s, c}, cr, P, (uint32_t)n_heads, head_pod, n_heads == 1 ? aux_lookup(a.sc, (uint32_t)head_pod) : -1, head_name, ready, available, all_running);
+  a.r.clusters[c] = cr;
+  a.sc.cact[c] = n_act;
+  if (n_act) atomicAdd(&a.r.totals[2], n_act);
+}
+
+// reconcilePods (raycluster_controller.go:619-935) + calculateStatus for one RayCluster, by one warp.
+// K > 0: the cluster's bucket (<= 32*K pods) is sorted and kept in registers — pod index pidx[k] and row word pw[k] of list
+// position k*32+lane — so the two scans below touch no memory.  K == 0: positions are read from sorted_pod_idx / rows
+// (radix pipeline, buckets larger than 256 pods, and phase 1).
+template <int K, bool kMH>
+__device__ __forceinline__ void decide_cluster(const DecideArgs &a, const uint32_t c, const uint32_t seg0, const uint32_t seg1,
+                                               uint32_t (&pidx)[K ? K : 1], uint32_t (&pw)[K ? K : 1],
+                                               int32_t (&s_acc)[4][KR_SMEM_GROUPS], int32_t (&s_mode)[2][KR_SMEM_GROUPS], const uint32_t lane) {
+  const SnapDev &s = a.s;
+  const uint32_t lt = lanemask_lt();
+  const uint32_t P = seg1 - seg0;
+  const uint32_t nchunks = (P + 31) / 32;
+  // cluster scalars: independent read-only loads, issued together
+  const uint32_t cf = LDG(s.c_flags[c]);
+  const uint32_t G = LDG(s.c_group_cnt[c]), g0 = LDG(s.c_group_off[c]);
+  const uint8_t suspend_status = LDG(s.c_suspend_status[c]);
+  const uint8_t ext_err = LDG(s.c_ext_err_kind[c]);
+  const uint8_t old_prov = LDG(s.c_old_cond_status[5 * (size_t)c + KR_COND_PROVISIONED]);
+
+  // accumulators: shared memory for the common case, global scratch for clusters with many groups
+  int32_t *acc_list, *acc_unh, *acc_wtd, *acc_rank, *g_mode, *g_prefix;
+  if (G <= KR_SMEM_GROUPS) {
+    acc_list = s_acc[0]; acc_unh = s_acc[1]; acc_wtd = s_acc[2]; acc_rank = s_acc[3];
+    g_mode = s_mode[0]; g_prefix = s_mode[1];
+    if (lane < KR_SMEM_GROUPS) { acc_list[lane] = 0; acc_unh[lane] = 0; acc_wtd[lane] = 0; acc_rank[lane] = 0; g_mode[lane] = GM_UNPROCESSED; g_prefix[lane] = 0; }
+  } else {
+    const uint32_t Ng = a.n.n_groups;
+    acc_list = a.sc.gacc + g0; acc_unh = a.sc.gacc + Ng + g0; acc_wtd = a.sc.gacc + 2 * (size_t)Ng + g0; acc_rank = a.sc.gacc + 3 * (size_t)Ng + g0;
+    g_mode = nullptr; g_prefix = nullptr;  // modes recycle the n_list / n_unhealthy cells once they are consumed
+    for (uint32_t gi = lane; gi < G; gi += 32) { acc_list[gi] = 0; acc_unh[gi] = 0; acc_wtd[gi] = 0; acc_rank[gi] = 0; }
+  }
+  __syncwarp();
+
+  // ---------------- scan 1: counts over the cluster's pods (list order)
+  int32_t ready = 0, available = 0, n_heads = 0;
+  bool all_running = P > 0;  // CheckAllPodsRunning (utils/util.go:584-603)
+  int32_t head_pod = -1;     // first head in list order
+#pragma unroll
+  for (int k = 0; k < (K ? K : 1 << 30); k++) {
+    if ((uint32_t)k >= nchunks) break;
+    const uint32_t i = seg0 + k * 32 + lane;
+    const bool valid = i < seg1;
+    uint32_t pod, w;
+    if (K) { pod = pidx[K ? k : 0]; w = pw[K ? k : 0]; }
+    else { pod = valid ? LDG(a.r.sorted_pod_idx[i]) : 0u; w = valid ? reinterpret_cast<const uint32_t *>(a.sc.rows)[4 * (size_t)pod + 3] : 0u; }
+    const uint32_t fl = w & 0xFFFFu, slot = valid ? (w >> 16) : KR_ROW_NO_GROUP;
+    const uint32_t nt = pp_node_type(fl), ph = pp_phase(fl), rd = pp_ready(fl);
+    const bool w_run = valid && nt == KR_NT_WORKER && ph == KR_PHASE_RUNNING;
+    available += __popc(__ballot_sync(0xFFFFFFFFu, w_run));
+    ready += __popc(__ballot_sync(0xFFFFFFFFu, w_run && rd == KR_COND_TRUE));
+    const bool not_ok = valid && (ph != KR_PHASE_RUNNING || rd == KR_COND_FALSE || rd == KR_COND_UNKNOWN);
+    if (__any_sync(0xFFFFFFFFu, not_ok)) all_running = false;
+    const uint32_t hb = __ballot_sync(0xFFFFFFFFu, valid && nt == KR_NT_HEAD);
+    if (hb) { if (n_heads == 0) head_pod = (int32_t)__shfl_sync(0xFFFFFFFFu, pod, __ffs(hb) - 1); n_heads += __popc(hb); }
+    // warp-ballot group-by on the group slot
+    const uint32_t gkey = (slot < G) ? slot : KR_ROW_NO_GROUP;
+    const uint32_t peers = __match_any_sync(0xFFFFFFFFu, gkey);
+    if (gkey != KR_ROW_NO_GROUP) {
+      const uint32_t ub = __ballot_sync(peers, should_delete(fl));
+      const uint32_t wb = __ballot_sync(peers, (fl & KR_ROW_WTD_OWN) != 0);
+      if ((peers & lt) == 0) {  // leader of its group in this chunk
+        acc_list[gkey] += __popc(peers);
+        acc_unh[gkey] += __popc(ub & peers);
+        acc_wtd[gkey] += __popc(wb & peers);
+      }
+    }
+    __syncwarp();
+  }
+
+  // ---------------- scalar decisions (uniform across the warp)
+  kr_cluster_result cr;
+  uint32_t head_name;
+  uint8_t all_action;  // action applied to every pod of the cluster (delete-all paths)
+  bool head_delete, run_groups;
+  if (!decide_cluster_scalar<kMH>(a, c, seg0, seg1, cf, G, g0, suspend_status, ext_err, old_prov, n_heads, head_pod, acc_list, acc_unh, acc_wtd,
+                                  g_mode, g_prefix, cr, head_name, all_action, head_delete, run_groups, lane))
+    return;
   const int32_t *mode_arr = g_mode ? g_mode : a.sc.gacc + g0;
   const int32_t *prefix_arr = g_prefix ? g_prefix : a.sc.gacc + a.n.n_groups + g0;
 
@@ -642,12 +675,183 @@ __device__ __forceinline__ void decide_cluster(const DecideArgs &a, const uint32
   }
 
   // ---------------- status roll-up + record
-  if (lane == 0) {
-    if (!(cf & KR_CF_SKIP))
-      status_rollup(a.s, a.f, ColumnsCI{a.s, c}, cr, P, (uint32_t)n_heads, head_pod, n_heads == 1 ? aux_lookup(a.sc, (uint32_t)head_pod) : -1, head_name, ready, available, all_running);
-    a.r.clusters[c] = cr;
-    a.sc.cact[c] = n_act;
-    if (n_act) atomicAdd(&a.r.totals[2], n_act);
+  if (lane == 0) decide_cluster_record(a, c, cf, cr, P, n_heads, head_pod, head_name, ready, available, all_running, n_act);
+}
+
+// Shared memory of decide_cluster_block.
+template <int kWarps>
+struct BlockDecideSmem {
+  int32_t w_cnt[3][kWarps][KR_SMEM_GROUPS];  // per warp and worker group (scan 1): pods, unhealthy pods, workersToDelete-owned pods
+  int32_t acc[3][KR_SMEM_GROUPS];            // ... summed over the warps
+  int32_t mode[2][KR_SMEM_GROUPS];           // per worker group: mode, delete-prefix length
+  int32_t rank[kWarps][KR_SMEM_GROUPS];      // per warp and worker group: running-rank cursor of scan 2
+  uint32_t w_red[kWarps][5];                 // per warp (scan 1): ready, available, heads, position of its first head, not all running
+  uint32_t w_act[kWarps];                    // per warp (scan 2): pods with an action
+  uint32_t plan[2];                          // all_action | head_delete << 8 | run_groups << 9; the first head's pod index
+};
+
+// reconcilePods + calculateStatus for one RayCluster of at most KR_SMEM_GROUPS worker groups whose List-ordered pods are
+// sorted_pod_idx[seg0, seg1), by all kWarps warps of the CTA (every thread calls it), with the results of decide_cluster<0, true>.
+// Warp w owns the positions [seg0 + w * per, seg0 + (w + 1) * per) (per: P / kWarps rounded up to whole chunks of 32), so List
+// order inside a warp's range is kept:
+//   scan 1  each warp counts its range: ready, available, heads and its first one, all running, and per worker group its pods,
+//           unhealthy pods and workersToDelete-owned pods.  A group's pods that are not workersToDelete-owned are exactly its
+//           candidates for the ordered delete prefix of normal mode, so their exclusive prefix over the warps is each warp's rank
+//           base in scan 2;
+//   scalar  warp 0 sums the counters (the first head is the first warp's that has one) and runs decide_cluster_scalar; a
+//           multi-host group's decide_multihost sweeps the whole cluster on warp 0 while the other warps wait at the barrier;
+//   scan 2  each warp decides its pods (stable rank: its base + the rank inside the warp) and counts its actions; after the block
+//           prefix of those counts, a warp with actions compacts them at seg0 + its base, so the run stays in List order.
+// sorted_pod_idx and the rows come through the read-only cache (an earlier grid wrote them); what this call writes and reads
+// back (mh_act, sorted_action) takes plain loads after a barrier.  Phase 1 only (a.phase: nothing is deferred).
+template <int kWarps>
+__device__ __forceinline__ void decide_cluster_block(const DecideArgs &a, const uint32_t c, const uint32_t seg0, const uint32_t seg1,
+                                                     BlockDecideSmem<kWarps> &sm, const uint32_t warp, const uint32_t lane) {
+  static_assert(kWarps <= 32 && KR_SMEM_GROUPS == 32, "one lane per warp and per worker group");
+  const SnapDev &s = a.s;
+  const uint32_t lt = lanemask_lt();
+  const uint32_t P = seg1 - seg0;
+  const uint32_t G = LDG(s.c_group_cnt[c]);
+  const uint32_t per = ((P + kWarps - 1) / kWarps + 31) & ~31u;
+  const uint32_t r0 = seg0 + min(warp * per, P), r1 = seg0 + min(warp * per + per, P);
+  int32_t *w_list = sm.w_cnt[0][warp], *w_unh = sm.w_cnt[1][warp], *w_wtd = sm.w_cnt[2][warp];
+  w_list[lane] = 0; w_unh[lane] = 0; w_wtd[lane] = 0;
+  __syncwarp();
+
+  // ---------------- scan 1: this warp's counts
+  int32_t ready = 0, available = 0, n_heads = 0;
+  uint32_t first_head = KR_EMPTY32;
+  bool not_ok_any = false;
+  for (uint32_t b = r0; b < r1; b += 32) {
+    const uint32_t i = b + lane;
+    const bool valid = i < r1;
+    const uint32_t pod = valid ? LDG(a.r.sorted_pod_idx[i]) : 0u;
+    const uint32_t w = valid ? reinterpret_cast<const uint32_t *>(a.sc.rows)[4 * (size_t)pod + 3] : 0u;
+    const uint32_t fl = w & 0xFFFFu, slot = valid ? (w >> 16) : KR_ROW_NO_GROUP;
+    const uint32_t nt = pp_node_type(fl), ph = pp_phase(fl), rd = pp_ready(fl);
+    const bool w_run = valid && nt == KR_NT_WORKER && ph == KR_PHASE_RUNNING;
+    available += __popc(__ballot_sync(0xFFFFFFFFu, w_run));
+    ready += __popc(__ballot_sync(0xFFFFFFFFu, w_run && rd == KR_COND_TRUE));
+    const bool not_ok = valid && (ph != KR_PHASE_RUNNING || rd == KR_COND_FALSE || rd == KR_COND_UNKNOWN);
+    if (__any_sync(0xFFFFFFFFu, not_ok)) not_ok_any = true;
+    const uint32_t hb = __ballot_sync(0xFFFFFFFFu, valid && nt == KR_NT_HEAD);
+    if (hb) { if (n_heads == 0) first_head = b + __ffs(hb) - 1; n_heads += __popc(hb); }
+    const uint32_t gkey = (slot < G) ? slot : KR_ROW_NO_GROUP;
+    const uint32_t peers = __match_any_sync(0xFFFFFFFFu, gkey);
+    if (gkey != KR_ROW_NO_GROUP) {
+      const uint32_t ub = __ballot_sync(peers, should_delete(fl));
+      const uint32_t wb = __ballot_sync(peers, (fl & KR_ROW_WTD_OWN) != 0);
+      if ((peers & lt) == 0) {  // leader of its group in this chunk
+        w_list[gkey] += __popc(peers);
+        w_unh[gkey] += __popc(ub & peers);
+        w_wtd[gkey] += __popc(wb & peers);
+      }
+    }
+    __syncwarp();
+  }
+  if (lane == 0) { sm.w_red[warp][0] = ready; sm.w_red[warp][1] = available; sm.w_red[warp][2] = n_heads; sm.w_red[warp][3] = first_head; sm.w_red[warp][4] = not_ok_any; }
+  __syncthreads();
+
+  // ---------------- scalar decisions (warp 0), while the other warps find their rank bases
+  kr_cluster_result cr;
+  uint32_t cf = 0, head_name = 0;
+  int32_t head_pod = -1;
+  bool all_running = false;
+  if (warp == 0) {
+    cf = LDG(s.c_flags[c]);
+    const uint32_t g0 = LDG(s.c_group_off[c]);
+    const uint8_t suspend_status = LDG(s.c_suspend_status[c]);
+    const uint8_t ext_err = LDG(s.c_ext_err_kind[c]);
+    const uint8_t old_prov = LDG(s.c_old_cond_status[5 * (size_t)c + KR_COND_PROVISIONED]);
+    const bool mine = lane < (uint32_t)kWarps;
+    ready = (int32_t)__reduce_add_sync(0xFFFFFFFFu, mine ? sm.w_red[lane][0] : 0u);
+    available = (int32_t)__reduce_add_sync(0xFFFFFFFFu, mine ? sm.w_red[lane][1] : 0u);
+    n_heads = (int32_t)__reduce_add_sync(0xFFFFFFFFu, mine ? sm.w_red[lane][2] : 0u);
+    all_running = P > 0 && !__any_sync(0xFFFFFFFFu, mine && sm.w_red[lane][4]);
+    const uint32_t hw = __ballot_sync(0xFFFFFFFFu, mine && sm.w_red[lane][2] != 0);
+    if (hw) head_pod = (int32_t)LDG(a.r.sorted_pod_idx[sm.w_red[__ffs(hw) - 1][3]]);
+    int32_t l = 0, u = 0, t = 0;
+    for (int w = 0; w < kWarps; w++) { l += sm.w_cnt[0][w][lane]; u += sm.w_cnt[1][w][lane]; t += sm.w_cnt[2][w][lane]; }
+    sm.acc[0][lane] = l; sm.acc[1][lane] = u; sm.acc[2][lane] = t;
+    sm.mode[0][lane] = GM_UNPROCESSED; sm.mode[1][lane] = 0;
+    sm.rank[0][lane] = 0;
+    __syncwarp();
+    uint8_t all_action;
+    bool head_delete, run_groups;
+    decide_cluster_scalar<true>(a, c, seg0, seg1, cf, G, g0, suspend_status, ext_err, old_prov, n_heads, head_pod, sm.acc[0], sm.acc[1], sm.acc[2],
+                                sm.mode[0], sm.mode[1], cr, head_name, all_action, head_delete, run_groups, lane);
+    if (lane == 0) { sm.plan[0] = all_action | (head_delete ? 0x100u : 0u) | (run_groups ? 0x200u : 0u); sm.plan[1] = (uint32_t)head_pod; }
+  } else {
+    int32_t base = 0;
+    for (uint32_t w = 0; w < warp; w++) base += sm.w_cnt[0][w][lane] - sm.w_cnt[2][w][lane];
+    sm.rank[warp][lane] = base;
+  }
+  __syncthreads();
+
+  // ---------------- scan 2: this warp's per-pod actions
+  const uint32_t plan = sm.plan[0];
+  const uint8_t all_action = (uint8_t)(plan & 0xFFu);
+  const bool head_delete = (plan & 0x100u) != 0, run_groups = (plan & 0x200u) != 0;
+  const int32_t head = (int32_t)sm.plan[1];
+  int32_t *acc_rank = sm.rank[warp];
+  const int32_t *mode_arr = sm.mode[0], *prefix_arr = sm.mode[1];
+  uint32_t n_act = 0;
+  for (uint32_t b = r0; b < r1; b += 32) {
+    const uint32_t i = b + lane;
+    const bool valid = i < r1;
+    const uint32_t pod = valid ? LDG(a.r.sorted_pod_idx[i]) : 0u;
+    uint32_t w = 0;
+    if (valid && run_groups) w = reinterpret_cast<const uint32_t *>(a.sc.rows)[4 * (size_t)pod + 3];
+    uint8_t act = KR_ACT_KEEP;
+    uint32_t gkey = KR_ROW_NO_GROUP;
+    const uint32_t fl = w & 0xFFFFu;
+    if (valid && run_groups && (w >> 16) < G) gkey = w >> 16;
+    const int32_t mode = (gkey != KR_ROW_NO_GROUP) ? mode_arr[gkey] : GM_UNPROCESSED;
+    bool candidate = false;
+    if (all_action != KR_ACT_KEEP) act = valid ? all_action : (uint8_t)KR_ACT_KEEP;
+    else if (head_delete) { if (valid && (int32_t)pod == head) act = KR_ACT_DELETE_HEAD; }
+    else if (mode == GM_SUSPENDED) act = KR_ACT_DELETE_GROUP_SUSPEND;
+    else if (mode == GM_MULTIHOST) act = a.sc.mh_act[i];
+    else if (mode == GM_UNHEALTHY) { if (should_delete(fl)) act = KR_ACT_DELETE_UNHEALTHY; }
+    else if (mode == GM_NORMAL) {
+      if (fl & KR_ROW_WTD_OWN) act = KR_ACT_DELETE_WTD;
+      else candidate = true;
+    }
+    const uint32_t ckey = candidate ? gkey : KR_ROW_NO_GROUP;
+    const uint32_t peers = __match_any_sync(0xFFFFFFFFu, ckey);
+    if (candidate) {
+      const int32_t cur = acc_rank[ckey];
+      __syncwarp(peers);
+      const int32_t rank = cur + __popc(peers & lt);
+      if ((peers & lt) == 0) acc_rank[ckey] = cur + __popc(peers);
+      if (rank < prefix_arr[ckey]) act = KR_ACT_DELETE_RANDOM;  // runningPods.Items[0 .. -diff) (:916-919)
+    }
+    __syncwarp();
+    if (valid) a.r.sorted_action[i] = act;
+    n_act += __popc(__ballot_sync(0xFFFFFFFFu, valid && act != KR_ACT_KEEP));
+  }
+  if (lane == 0) sm.w_act[warp] = n_act;
+  __syncthreads();
+
+  // ---------------- the cluster's action list, in List order
+  const uint32_t v = lane < (uint32_t)kWarps ? sm.w_act[lane] : 0u;
+  const uint32_t before = __reduce_add_sync(0xFFFFFFFFu, lane < warp ? v : 0u);
+  if (n_act) {
+    uint32_t o = seg0 + before;
+    for (uint32_t b = r0; b < r1; b += 32) {
+      const uint32_t i = b + lane;
+      const uint8_t act = i < r1 ? a.r.sorted_action[i] : (uint8_t)KR_ACT_KEEP;
+      const uint32_t abal = __ballot_sync(0xFFFFFFFFu, act != KR_ACT_KEEP);
+      if (act != KR_ACT_KEEP) {
+        const size_t p = (size_t)o + __popc(abal & lt);
+        a.sc.act_tmp_idx[p] = LDG(a.r.sorted_pod_idx[i]); a.sc.act_tmp_code[p] = act;
+      }
+      o += __popc(abal);
+    }
+  }
+  if (warp == 0) {
+    const uint32_t total = __reduce_add_sync(0xFFFFFFFFu, v);
+    if (lane == 0) decide_cluster_record(a, c, cf, cr, P, n_heads, head_pod, head_name, ready, available, all_running, total);
   }
 }
 

@@ -1010,6 +1010,19 @@ void launch_large_sort(PassCtx &c, const Decide2Args &da, const uint4 *grown = n
   }
 }
 
+// The decides of the per-cluster kernels' RayClusters (kr_large.cuh): k_decide_large over the list (and, with `grown`, one CTA per
+// RayCluster k_inc_grow listed), then k_decide_huge over its huge part, but for the wide RayClusters there, which k_decide_large keeps.
+template <bool kInc>
+void launch_large_decide(PassCtx &c, const Decide2Args &da, const uint4 *grown = nullptr) {
+  const kr_engine *e = c.e;
+  c.mark("k_decide_large");
+  k_decide_large<kInc, kLargeDecideThreads><<<e->n_large + (grown ? KR_GROW_MAX : 0), kLargeDecideThreads, 0, c.M>>>(da, c.lg_list, e->n_large, e->n_lsort, grown);
+  if (const uint32_t n_huge = e->n_large - e->n_lsort) {
+    c.mark("k_decide_huge");
+    k_decide_large<kInc, kHugeDecideThreads><<<n_huge, kHugeDecideThreads, 0, c.M>>>(da, c.lg_list + e->n_lsort, n_huge, 0u, nullptr);
+  }
+}
+
 // Launches the whole pass.  profile: serialise everything on stream M and bracket each kernel with events.
 int launch_pass(kr_engine *e, const kr_flags &f, bool profile, bool capturing = false) {
   PassCtx c(e, profile);
@@ -1091,7 +1104,7 @@ int launch_pass(kr_engine *e, const kr_flags &f, bool profile, bool capturing = 
     const bool large = e->n_large && sc.lg && n.n_clusters;  // large RayClusters (kr_large.cuh): sorted beside the hash, decided after it
     if (large) launch_large_sort<false>(c, da);
     if (int rc = join_hash()) return rc;
-    if (large) { c.mark("k_decide_large"); k_decide_large<false><<<e->n_large, kLargeDecideThreads, 0, M>>>(da, c.lg_list, e->n_large, nullptr); }
+    if (large) launch_large_decide<false>(c, da);
     if (e->rec.n_recreate > 0 && do_hash && !spin) {  // clusters whose Recreate gate needs the digest: decided again, in the places phase 0 reserved
       da.phase = 1;
       c.mark("k_decide2_phase1");
@@ -1447,8 +1460,7 @@ int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile
       const uint4 *grown = grow ? e->d_grow + kGrowResult : nullptr;
       CK(cudaMemsetAsync(sc.inc + KR_INC_LSEG, 0, 4, M));
       launch_large_sort<true>(c, da, grown, huge_grow ? (uint32_t)e->huge_reserve : 0u);
-      c.mark("k_decide_large");
-      k_decide_large<true><<<e->n_large + (grow ? KR_GROW_MAX : 0), kLargeDecideThreads, 0, M>>>(da, c.lg_list, e->n_large, grown);
+      launch_large_decide<true>(c, da, grown);
     }
   }
   if (n.n_jobs) { c.mark("k_jobs"); k_jobs<<<(n.n_jobs + 255) / 256, 256, 0, M>>>(s, sc, r, z); }
@@ -2055,7 +2067,8 @@ int kr_engine_create(const kr_config *cfg, kr_engine **out) {
                         (const void *)k_inc_mark_recreate, (const void *)k_decide2<2, true>, (const void *)k_decide2<4, true>, (const void *)k_decide2<8, true>, (const void *)k_inc_refresh, (const void *)k_inc_admit,
                         (const void *)k_inc_finish, (const void *)k_decide2<2, false, true>, (const void *)k_decide2<4, false, true>, (const void *)k_decide2<8, false, true>,
                         (const void *)k_decide2<2, true, true>, (const void *)k_decide2<4, true, true>, (const void *)k_decide2<8, true, true>,
-                        (const void *)k_large_sort<false>, (const void *)k_large_sort<true>, (const void *)k_decide_large<false>, (const void *)k_decide_large<true>, (const void *)k_inc_grow<false>, (const void *)k_inc_grow<true>,
+                        (const void *)k_large_sort<false>, (const void *)k_large_sort<true>, (const void *)k_decide_large<false, kLargeDecideThreads>, (const void *)k_decide_large<true, kLargeDecideThreads>,
+                        (const void *)k_decide_large<false, kHugeDecideThreads>, (const void *)k_decide_large<true, kHugeDecideThreads>, (const void *)k_inc_grow<false>, (const void *)k_inc_grow<true>,
                         (const void *)k_huge_tiles<false>, (const void *)k_huge_tiles<true>, (const void *)k_huge_merge<false>, (const void *)k_huge_merge<true>};
     for (const void *k : ks) cudaFuncSetAttribute(k, cudaFuncAttributePreferredSharedMemoryCarveout, pct);
   }

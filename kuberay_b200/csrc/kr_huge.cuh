@@ -2,14 +2,14 @@
 // KR_OPT_LARGE_CLUSTERS).  Part of the sm_90a kernel set of the batched reconcile engine; see kr_kernels.cuh for the overview.
 //
 // Such a "huge" RayCluster gets a region of the large-cluster arena like a large one (kr_large.cuh) and is decided by the same
-// k_decide_large; only its List-order sort differs, because k_large_sort sorts a whole cluster in one CTA's shared memory.  The
+// block decide, in k_decide_large's 512-thread instantiation (k_decide_huge); only its List-order sort differs, because k_large_sort sorts a whole cluster in one CTA's shared memory.  The
 // engine cuts the arrival ranks a huge cluster's bucket and region can hold, [0, stride + region capacity), into tiles of
 // kHugeTile ranks (a table {cluster, first rank, the cluster's first tile, its tile count}, uploaded with the cluster list):
 //   k_huge_tiles   one CTA per tile: drops the stale records of an incremental epoch (k_large_sort's rule), writes each kept pod's
 //                  16-byte row, sorts the kept pod indices in shared memory and stores the sorted run and the same indices in
 //                  arrival order (the stash) in the tile's scratch slots.  The last CTA of a cluster (fenced tile counts, one
 //                  counting atomic) reserves the cluster's sorted_pod_idx segment at KR_INC_LSEG and publishes it in lg[c].z / .w
-//                  as k_large_sort does, so k_decide_large decides the cluster unchanged;
+//                  as k_large_sort does, so k_decide_huge (k_decide_large's 512-thread instantiation) decides the cluster;
 //   k_huge_merge   one CTA per tile: a pod's place in List order is its rank in its own run plus, for every other tile of the
 //                  cluster, how many of that tile's pods precede it (the keys are distinct pod indices).  Each other run is staged
 //                  in shared memory in turn; a thread owns kHugePer consecutive keys and finds their places by galloping from the
@@ -68,7 +68,7 @@ __global__ void __launch_bounds__(kHugeThreads) k_huge_tiles(Decide2Args a, Huge
     if (kInc) go = go && !__ldcg(&sc.inc[KR_INC_VOID]) && !__ldcg(&sc.inc[KR_INC_STRUCTURAL]) && __ldcg(&sc.dirty_flag[c]) == epoch;
     const bool wide = a.s.c_group_cnt[c] > KR_SMEM_GROUPS;
     s_go = go && (P > S ? P - S <= cap : wide);
-    if (!s_go && r0 == 0) sc.lg[c].w = 0;  // not taken this pass: k_huge_merge and k_decide_large leave it alone
+    if (!s_go && r0 == 0) sc.lg[c].w = 0;  // not taken this pass: k_huge_merge and the decide leave it alone
   }
   __syncthreads();
   if (!s_go) return;

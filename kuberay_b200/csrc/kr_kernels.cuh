@@ -20,10 +20,11 @@
 //   k_jobs           RayJob -> RayCluster status roll-up join
 //   k_large_sort / k_decide_large   KR_OPT_LARGE_CLUSTERS / KR_OPT_WIDE_CLUSTERS only (kr_large.cuh): the RayClusters of
 //                    257..KR_LARGE_MAX_PODS pods and those of more than KR_SMEM_GROUPS worker groups, one CTA each — List order by a
-//                    shared-memory sort beside the hash, then the sort pipeline's memory-resident decide
+//                    shared-memory sort beside the hash, then a decide by every warp of the CTA (a wide one: the sort pipeline's
+//                    memory-resident warp decide)
 //   k_huge_tiles / k_huge_merge     KR_OPT_HUGE_CLUSTERS only (kr_huge.cuh): the RayClusters of more than KR_LARGE_MAX_PODS pods —
 //                    List order by a shared-memory sort per 8 192-rank tile and a rank merge of the tiles, one CTA per tile,
-//                    beside the hash; then k_decide_large decides them
+//                    beside the hash; then k_decide_huge (k_decide_large with 512 threads) decides them
 // When the caller asks for the full per-cluster pod lists (fetch_pod_lists == 1) or the snapshot does not qualify — the SORT pipeline:
 //   k_match -> k_place_fused -> k_decide_small (+ k_decide on a side stream) -> [phase 1] -> k_creates_fused
 //   (buckets restored to List order by an in-register bitonic sort), and for RayClusters with > 1024 pods the RADIX pipeline

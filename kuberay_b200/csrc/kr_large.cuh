@@ -8,14 +8,16 @@
 // at the region table.  Wide clusters are known at commit (their group counts); one without a region keeps its pods in its bucket,
 // and an overflow past the stride voids the attempt as for any cluster.  Both kinds share one cluster table and one list (lg,
 // lg_list).  k_decide2 leaves every cluster whose count exceeds the stride, and every wide one, alone; these two kernels, one CTA per
-// listed RayCluster, decide them instead (decide_cluster spills the accumulators of a wide one to gacc, as the sort pipeline does):
+// listed RayCluster, decide them instead:
 //   k_large_sort    (beside the hash) loads the cluster's records, drops the stale ones of an incremental epoch and stores the rest
 //                   back compacted, writes each pod's 16-byte row (what the memory-resident decide reads), sorts the pod indices
 //                   into List order in shared memory and publishes them at a scratch segment (sorted_pod_idx);
-//   k_decide_large  (after the join with the hash stream: a Recreate gate reads a finished digest) decides the cluster with the
-//                   memory-resident warp decide of the sort pipeline (decide_cluster<0, true>), reserves its action run and create
-//                   run at the bucket pipeline's cursors, moves the actions into place and fills the replica indices.
-// Two kernels, because decide_cluster reads sorted_pod_idx and the rows through the read-only cache, which is only coherent with
+//   k_decide_large  (after the join with the hash stream: a Recreate gate reads a finished digest) decides the cluster with every
+//                   warp of the CTA (decide_cluster_block, kr_decide.cuh; a wide one with warp 0 alone: decide_cluster<0, true>, which
+//                   spills the accumulators to gacc, as the sort pipeline does), reserves its action run and create run at the bucket
+//                   pipeline's cursors, moves the actions into place and fills the replica indices.  Its 512-thread instantiation,
+//                   k_decide_huge, decides the huge RayClusters (kr_huge.cuh).
+// Two kernels, because the decide reads sorted_pod_idx and the rows through the read-only cache, which is only coherent with
 // stores of an earlier grid.
 #pragma once
 
@@ -25,6 +27,7 @@ namespace kr {
 
 static constexpr int kLargeSortThreads = 512;
 static constexpr int kLargeDecideThreads = 128;
+static constexpr int kHugeDecideThreads = 512;  // (k_decide_huge: the most threads that keep its registers free of spills)
 static constexpr int kHugeTile = KR_LARGE_MAX_PODS;  // arrival ranks per tile of a huge RayCluster (kr_huge.cuh)
 
 // Ascending bitonic sort of s[0, total) in shared memory, padded to the next power of two (at least 2) with 0xFFFFFFFF: s must
@@ -232,12 +235,20 @@ __global__ void __launch_bounds__(kLargeSortThreads) k_large_sort(Decide2Args a,
   if (tid == 0) { sc.lg[c].z = seg; sc.lg[c].w = total | KR_LG_OWNED; }
 }
 
-// One CTA per large RayCluster that k_large_sort took: warp 0 decides, every warp fills replica indices.
-template <bool kInc>
-__global__ void __launch_bounds__(kLargeDecideThreads) k_decide_large(Decide2Args a, const uint32_t *__restrict__ lg_list, uint32_t n_list, const uint4 *grown) {
-  __shared__ int32_t s_acc[4][KR_SMEM_GROUPS];
+// One CTA per RayCluster of the list that k_large_sort or k_huge_tiles took: every warp decides it (decide_cluster_block) but for a
+// wide one, whose accumulators live in gacc (warp 0 alone: decide_cluster<0, true>); warp 0 reserves its action and create runs;
+// every warp fills replica indices.  Two instantiations split the list (in profiles, k_decide_large and k_decide_huge):
+//   kThreads = kLargeDecideThreads  the list, the grown CTAs past it, and the wide RayClusters of its huge part [n_lsort, n_list);
+//   kThreads = kHugeDecideThreads   the rest of the huge part (launched on lg_list + n_lsort, with n_lsort = 0 and no grown CTAs).
+template <bool kInc, int kThreads>
+__global__ void __launch_bounds__(kThreads, 1) k_decide_large(Decide2Args a, const uint32_t *__restrict__ lg_list, uint32_t n_list, uint32_t n_lsort,
+                                                           const uint4 *grown) {
+  constexpr int kWarps = kThreads / 32;
+  constexpr bool kHugePart = kThreads != kLargeDecideThreads;
+  __shared__ int32_t s_acc[4][KR_SMEM_GROUPS];  // (a wide RayCluster's warp decide)
   __shared__ int32_t s_mode[2][KR_SMEM_GROUPS];
-  __shared__ uint32_t s_bits[kLargeDecideThreads / 32][32];
+  __shared__ BlockDecideSmem<kWarps> s_dec;
+  __shared__ uint32_t s_bits[kWarps][32];
   __shared__ uint32_t s_place[4];  // act_off, n_act, stage index, go on
   const ScratchDev &sc = a.sc;
   const ResDev &r = a.r;
@@ -248,27 +259,34 @@ __global__ void __launch_bounds__(kLargeDecideThreads) k_decide_large(Decide2Arg
   if (!(l.w & KR_LG_OWNED)) return;
   const uint32_t seg = l.z, P = l.w & ~KR_LG_OWNED;
   const uint32_t G = a.s.c_group_cnt[c], g0 = a.s.c_group_off[c];
+  const bool wide = G > KR_SMEM_GROUPS;
+  if (kHugePart ? wide : (blockIdx.x >= n_lsort && blockIdx.x < n_list && !wide)) return;  // the other instantiation's
   if (kInc) {  // this cluster's place in the dirty list (= its entry of the staging buffer)
     if (tid == 0) s_place[2] = 0xFFFFFFFFu;
     __syncthreads();
     const uint32_t n_dirty = __ldcg(&sc.inc[KR_INC_DIRTY]);
-    for (uint32_t i = tid; i < n_dirty; i += kLargeDecideThreads) if (__ldcg(&sc.dirty_list[i]) == c) s_place[2] = i;
+    for (uint32_t i = tid; i < n_dirty; i += kThreads) if (__ldcg(&sc.dirty_list[i]) == c) s_place[2] = i;
   }
-  if (warp == 0) {
-    // what the cluster holds in the resident results (an incremental epoch keeps its places while they suffice)
-    uint32_t old_create = 0, old_act = 0, old_create_off = 0;
-    if (kInc) {
-      for (uint32_t gi = lane; gi < G; gi += 32) old_create += r.groups[g0 + gi].n_create;
-      old_create = __reduce_add_sync(0xFFFFFFFFu, old_create);
-      old_act = r.act_cnt[c];
-      old_create_off = G ? sc.gcreate[g0] : 0u;
+  // what the cluster holds in the resident results (an incremental epoch keeps its places while they suffice), read before the
+  // decide rewrites them
+  uint32_t old_create = 0, old_act = 0, old_create_off = 0;
+  if (kInc && warp == 0) {
+    for (uint32_t gi = lane; gi < G; gi += 32) old_create += r.groups[g0 + gi].n_create;
+    old_create = __reduce_add_sync(0xFFFFFFFFu, old_create);
+    old_act = r.act_cnt[c];
+    old_create_off = G ? sc.gcreate[g0] : 0u;
+  }
+  __syncwarp();
+  DecideArgs da{a.s, a.sc, a.r, a.n, a.f, nullptr, nullptr, 0, 1};  // phase 1: the digests are final
+  if (!kHugePart && wide) {
+    if (warp == 0) {
+      uint32_t d0[1] = {0}, d1[1] = {0};
+      decide_cluster<0, true>(da, c, seg, seg + P, d0, d1, s_acc, s_mode, lane);
     }
+  } else decide_cluster_block<kWarps>(da, c, seg, seg + P, s_dec, warp, lane);
+  if (warp == 0) {
     __syncwarp();
-    DecideArgs da{a.s, a.sc, a.r, a.n, a.f, nullptr, nullptr, 0, 1};  // phase 1: the digests are final
-    uint32_t d0[1] = {0}, d1[1] = {0};
-    decide_cluster<0, true>(da, c, seg, seg + P, d0, d1, s_acc, s_mode, lane);
-    __syncwarp();
-    // decide_cluster left n_create per group in gcreate[] and the action count in cact[]
+    // the decide left n_create per group in gcreate[] and the action count in cact[]
     uint32_t n_create = 0;
     for (uint32_t gi = lane; gi < G; gi += 32) n_create += sc.gcreate[g0 + gi];
     n_create = __reduce_add_sync(0xFFFFFFFFu, n_create);
@@ -289,7 +307,7 @@ __global__ void __launch_bounds__(kLargeDecideThreads) k_decide_large(Decide2Arg
         if ((need & 2u) && (uint64_t)create_off + n_create > a.create_cap) sc.inc[KR_INC_VOID] = 1u;  // a full pass packs it again
         if (need & 1u) sc.act_res[c] = n_act;
         if (need & 2u) sc.cre_res[c] = n_create;
-        if (old_act) atomicSub(&r.totals[2], old_act);  // (decide_cluster added this pass's n_act)
+        if (old_act) atomicSub(&r.totals[2], old_act);  // (the decide added this pass's n_act)
         if (n_create != old_create) atomicAdd(&r.totals[6], n_create - old_create);
       }
       if (!kInc) { sc.act_res[c] = n_act; sc.cre_res[c] = n_create; }
@@ -307,7 +325,7 @@ __global__ void __launch_bounds__(kLargeDecideThreads) k_decide_large(Decide2Arg
   }
   __syncthreads();
   if (!s_place[3]) return;
-  for (uint32_t gi = warp; gi < G; gi += kLargeDecideThreads / 32)
+  for (uint32_t gi = warp; gi < G; gi += kWarps)
     create_fill_group(a.s, sc, r, a.f, g0 + gi, r.groups[g0 + gi].create_off, a.create_cap, s_bits[warp], lane);
   if (warp == 0) compact_cluster_actions(r, sc, c, s_place[0], s_place[1], lane);
   __syncthreads();  // both read the cluster's pod_start

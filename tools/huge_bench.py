@@ -3,7 +3,8 @@ JSON line per measurement).
 
   C3H  the pipeline and stride, full-pass ms (incremental epochs off; host clock around kr_reconcile_batch, so the results copy is
        included), then 20 epochs of 1 % pod churn (PodReady flips) with incremental epochs on: how many ran incrementally on the
-       device and their median kernel ms; k_huge_tiles, k_huge_merge and k_decide_large alone in a profiled pass;
+       device and their median kernel ms; k_huge_tiles, k_huge_merge, k_decide_large and k_decide_huge alone in a
+       profiled pass;
   C3   the same full pass with the option off and on (no huge RayCluster): the kernels launched, which must be the same.
 Usage: python tools/huge_bench.py [--steps 30] [--out DIR]"""
 import argparse
@@ -85,7 +86,7 @@ def main():
                 rec = {"workload": name, "run": run, "huge_clusters": huge, "pipeline": "bucket" if "k_match2" in names else "sort",
                        "stride": stride, "full_pass_ms": round(ms, 4)}
                 if name == "C3H":
-                    rec.update({k + "_ms": kd.get(k) for k in ("k_huge_tiles", "k_huge_merge", "k_decide_large")})
+                    rec.update({k + "_ms": kd.get(k) for k in ("k_huge_tiles", "k_huge_merge", "k_decide_large", "k_decide_huge")})
                     s2, _ = synthetic.generate(synthetic.config(name))
                     rec["incremental_epochs_of_20"], rec["epoch_kernel_ms_median"] = churn(s2, flags, huge)
                 else:

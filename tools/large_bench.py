@@ -32,7 +32,7 @@ def full_pass_ms(snap, flags, large, steps):
             eng.reconcile(flags)
         ms = (time.perf_counter() - t) * 1e3 / steps
         kern = {k: v for k, v in eng.reconcile_profiled(flags)["kernels"]}
-        return ms, kern.get("k_decide_large"), kern.get("k_large_sort"), eng.get_option(abi.OPT_BUCKET_STRIDE)
+        return ms, kern.get("k_decide_large"), kern.get("k_decide_huge"), kern.get("k_large_sort"), eng.get_option(abi.OPT_BUCKET_STRIDE)
     finally:
         eng.close()
 
@@ -75,9 +75,9 @@ def main():
         flags.fetch_pod_lists = 0
         for run in range(a.runs):
             for large in (False, True):
-                ms, dl, ls, stride = full_pass_ms(snap, flags, large, a.steps)
+                ms, dl, dh, ls, stride = full_pass_ms(snap, flags, large, a.steps)
                 rec = {"workload": name, "run": run, "large_clusters": large, "full_pass_ms": round(ms, 4), "stride": stride,
-                       "k_large_sort_ms": ls, "k_decide_large_ms": dl}
+                       "k_large_sort_ms": ls, "k_decide_large_ms": dl, "k_decide_huge_ms": dh}
                 if name == "C3L":
                     s2, _ = synthetic.generate(synthetic.config(name))
                     rec["incremental_epochs_of_20"], rec["epoch_kernel_ms_median"] = churn(s2, flags, large)

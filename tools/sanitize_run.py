@@ -220,6 +220,32 @@ def large_growth(snap, flags, label):
     print(label, "ok:", inc, "of 2 growth epochs incremental", flush=True)
 
 
+def block_decides(snap, flags, label):
+    """The block decide (kr_decide.cuh: decide_cluster_block) in both of its launches: k_decide_large for a large RayCluster and
+    k_decide_huge for a huge one, in a full pass, then in an incremental epoch that flips Pods of both."""
+    flags.fetch_pod_lists = 0
+    synthetic.grow_clusters(snap, [0], 9000)
+    synthetic.grow_clusters(snap, [400], 1500)
+    eng = Engine.for_snapshot(snap, slack=1.2, max_creates=1 << 18, large_clusters=True, huge_clusters=True)
+    eng.set_fixed_layout(True)
+    inc = 0
+    try:
+        eng.load(snap)
+        for epoch in range(2):
+            if epoch:
+                key = lambda c: (snap.p_ns_id == snap.c_ns_id[c]) & (snap.p_cluster_name_id == snap.c_name_id[c])  # noqa: E731
+                rows = np.concatenate([np.flatnonzero(key(0))[::53], np.flatnonzero(key(400))[::29]]).astype(np.uint32)
+                snap.p_packed[rows] ^= np.uint32(1 << abi.PP_READY_SHIFT)
+                cols = [c for c, _d, _m, dim in abi.COLUMNS if dim == "pods"]
+                eng.commit_pod_values(rows, np.stack([snap.cols[c][rows].view(np.uint32) for c in cols], axis=1))
+            names = [n for n, _ in eng.reconcile_profiled(flags)["kernels"]]
+            assert "k_decide_large" in names and "k_decide_huge" in names, names
+            inc += eng.fetch().changed_clusters is not None
+    finally:
+        eng.close()
+    print(label, "ok:", inc, "of 1 epoch incremental", flush=True)
+
+
 def large_moves(snap, flags, label, grown, edits, huge=False):
     """KR_OPT_LARGE_MOVES (kr_incr.cuh): the RayClusters `grown` made large, then each edit of `edits` in an epoch of its own: ("delete",
     rows) by swap-remove, or ("regroup", row) a worker group appended.  A large gone row is released by k_inc_large_release from its
@@ -397,6 +423,8 @@ def main():
     # incremental epochs (the deletions compact its bucket and region across tiles)
     incremental(*synthetic.generate(synthetic.config("C3H", n_clusters=700, pods_per_cluster=20, large_pods=9000, n_large=1)),
                 "incremental epochs, huge RayCluster", large=True, huge=True)
+    # a large and a huge RayCluster decided by every warp of their CTA (kr_decide.cuh: decide_cluster_block), full pass and epoch
+    block_decides(*synthetic.generate(synthetic.config("C2", n_clusters=1200, pods_per_cluster=20, groups=2)), "block decides, large and huge")
     # keys built to collide (tests/table_keys.py): probe chains that start in the last slot of the cluster, workersToDelete and
     # head-aux tables and wrap, in a full pass and in incremental epochs
     from table_keys import k1, k2, k3
