@@ -557,7 +557,7 @@ enum {
                               the pass to the sort / radix pipelines, unless KR_OPT_HUGE_CLUSTERS.  A RayCluster that outgrows its
                               bucket or region in an incremental epoch makes that epoch a full pass, unless KR_OPT_LARGE_GROWTH.
                               Turning it on allocates the region arena once, for the
-                              capacities: about 22 B per max_pods + 20 B per max_clusters of device memory. */
+                              capacities: about 11 B per max_pods + 20 B per max_clusters of device memory. */
   KR_OPT_BUCKET_STRIDE = 4,   /* read only (kr_engine_get_option): records per RayCluster bucket of the current layout (64 / 128 / 256);
                               0 = the passes take the sort pipeline */
   KR_OPT_WIDE_CLUSTERS = 5,   /* 1: RayClusters with more than 32 worker groups stay on the bucket pipeline (DESIGN §4.1): one CTA per

@@ -8,7 +8,7 @@
 // (common/association.go:184-196), a scale-down deletes the first -diff running pods (raycluster_controller.go:916-919), and
 // the Delete calls are issued in List order.  Everything else (selectors, counts, the unhealthy / workersToDelete sets, the
 // lowest free replica indices, the status roll-up) is a set computation.  So here
-//   k_match2   drops each pod's 16-byte record {pod idx, group slot | flags, replica index, name id} straight into its
+//   k_match2   drops each pod's 8-byte record {pod idx, group slot | flags} straight into its
 //              cluster's fixed-stride bucket at the arrival rank a returning atomic hands out: no scan, no placement pass, no
 //              row array — three scattered accesses per pod (table probe, atomic, record store) instead of four plus a gather;
 //   k_decide2  (one warp per RayCluster, bucket in registers, ARRIVAL order) takes the first head as a warp minimum over pod
@@ -41,13 +41,13 @@ static constexpr int kD2Warps = KR_D2WARPS;  // RayClusters per k_decide2 CTA
 // (KR_OPT_LARGE_CLUSTERS, kr_large.cuh), which holds ranks [stride, stride + capacity).  nullptr: no room (an ordinary RayCluster,
 // or a large one that outgrew its region): the attempt is void.  Ranks below the stride stay in the cluster's bucket, so an
 // ordinary pod never reaches this lookup.
-__device__ __forceinline__ uint4 *large_slot(const ScratchDev &sc, uint32_t c, uint32_t rank) {
+__device__ __forceinline__ uint2 *large_slot(const ScratchDev &sc, uint32_t c, uint32_t rank) {
   if (!sc.lg) return nullptr;
   const uint4 l = __ldcg(&sc.lg[c]);
   const uint32_t j = rank - sc.bucket_stride;
   return j < l.y ? sc.region + l.x + j : nullptr;
 }
-__device__ __forceinline__ uint4 *rec_slot(const ScratchDev &sc, uint32_t c, uint32_t rank) {
+__device__ __forceinline__ uint2 *rec_slot(const ScratchDev &sc, uint32_t c, uint32_t rank) {
   return rank < sc.bucket_stride ? sc.bucket + (size_t)c * sc.bucket_stride + rank : large_slot(sc, c, rank);
 }
 // Region capacity of a RayCluster of `count` pods at this stride: 1.25x its pods rounded up to 32, capped at KR_LARGE_MAX_PODS unless
@@ -59,10 +59,12 @@ __host__ __device__ __forceinline__ uint32_t large_region_cap(uint32_t count, ui
 
 
 // ------------------------------------------------------------------------------------------------ k_match2
-// The selector match (common/association.go:83-130) + bucketing.  7 coalesced column loads per pod (issued before the
+// The selector match (common/association.go:83-130) + bucketing.  5 coalesced column loads per pod (issued before the
 // programmatic-launch wait: they do not depend on the table build), one 16-byte probe of the cluster table (which also
 // carries the name of worker group 0, so a single-group RayCluster needs no second lookup), a shared-memory Bloom test
-// for the workersToDelete names, one returning atomic and one 16-byte record store.
+// for the workersToDelete names, one returning atomic and one 8-byte record store.  The record leaves out the replica index and the
+// name: k_decide2 reads them from the Pod columns for the few pods that need them (the head's name, the replica indices in use of a
+// RayCluster that creates), and the bucket arena is half the size (C3: 8 MB written and read back instead of 16 MB).
 template <int kItems>
 __global__ void __launch_bounds__(kSortThreads) k_match2(SnapDev s, ScratchDev sc, ResDev r, Sizes n, int has_wtd) {
   KR_TL(1);
@@ -71,14 +73,14 @@ __global__ void __launch_bounds__(kSortThreads) k_match2(SnapDev s, ScratchDev s
   const uint32_t tile = blockIdx.x;
   const uint32_t warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
   const uint32_t base = tile * (kSortThreads * kItems) + warp * (32 * kItems) + lane;
-  uint32_t ns[kItems], cn[kItems], gn[kItems], nm[kItems], pk[kItems], ri[kItems];
+  uint32_t ns[kItems], cn[kItems], gn[kItems], nm[kItems], pk[kItems];
 #pragma unroll
   for (int it = 0; it < kItems; it++) {
     const uint32_t p = base + it * 32;
     const bool v = p < n.n_pods;
     ns[it] = v ? __ldg(&s.p_ns_id[p]) : 0u; cn[it] = v ? __ldg(&s.p_cluster_name_id[p]) : 0u;
     gn[it] = v ? __ldg(&s.p_group_name_id[p]) : 0u; nm[it] = v ? __ldg(&s.p_name_id[p]) : 0u;
-    pk[it] = v ? __ldg(&s.p_packed[p]) : 0u; ri[it] = v ? (uint32_t)__ldg(&s.p_replica_index[p]) : 0u;
+    pk[it] = v ? __ldg(&s.p_packed[p]) : 0u;
   }
   pdl_wait(); pdl_trigger();
   // (Keep this wait unconditional and in straight-line code: the table probes below use __ldg, i.e. loads the compiler treats as
@@ -172,10 +174,10 @@ __global__ void __launch_bounds__(kSortThreads) k_match2(SnapDev s, ScratchDev s
   for (int it = 0; it < kItems; it++) {
     if (cidx[it] >= n.n_clusters) continue;
     if (rank[it] < sc.bucket_stride) {
-      sc.bucket[(size_t)cidx[it] * sc.bucket_stride + rank[it]] = make_uint4(base + it * 32, roww[it], ri[it], nm[it]);
+      sc.bucket[(size_t)cidx[it] * sc.bucket_stride + rank[it]] = make_uint2(base + it * 32, roww[it]);
       sc.pos[base + it * 32] = rank[it];  // (coalesced; incremental epochs rewrite a row's record in place)
-    } else if (uint4 *slot = large_slot(sc, cidx[it], rank[it])) {
-      *slot = make_uint4(base + it * 32, roww[it], ri[it], nm[it]);
+    } else if (uint2 *slot = large_slot(sc, cidx[it], rank[it])) {
+      *slot = make_uint2(base + it * 32, roww[it]);
       sc.pos[base + it * 32] = rank[it];
     } else KR_MARK_ATTEMPT_VOID(r.totals);  // the engine reruns the pass with a wider stride / large regions / on the sort pipeline
   }
@@ -235,7 +237,7 @@ __device__ __forceinline__ void stage_cluster(const Decide2Args &a, uint32_t i, 
 // A replica is the set of the group's pods sharing a ray.io/worker-group-replica-name; it is identified by its smallest pod index,
 // so ascending identity is "first appearance in List order" (the stand-in for the reference's Go-map iteration) although the
 // bucket is in arrival order.  Replicas are peeled off in that order (a warp minimum over the unassigned members, then a compare
-// of its name against the K registers): O(replicas x K) warp steps.  The replica-name id is not in the 16-byte bucket record; it
+// of its name against the K registers): O(replicas x K) warp steps.  The replica-name id is not in the 8-byte bucket record; it
 // is read from the pod column here, for the group's members only (an incremental epoch patches that column before this kernel).
 // The group's per-pod actions go straight into act[]; mh_head gets bit k for every pod that is the first pod of a healthy
 // replica (its replica index is "in use" for the creates); s_rep (>= 32*K words of the warp's shared memory) holds the
@@ -365,7 +367,7 @@ __global__ void __launch_bounds__(kD2Warps * 32, (K <= 4 && !kMH ? 32 : 16) / kD
   __shared__ uint32_t s_bits[kD2Warps][32];                // 1024-bit window of replica indices in use
   // Per-cluster state that is uniform across the warp sits in the warp's shared memory, not in every lane's registers: the input
   // record (each field one broadcast load), the result record, and two scalars the placement needs.  With that, and with the
-  // replica indices and the head's name read again from the bucket where they are used and the roll-up ahead of the action list,
+  // replica indices and the head's name read from the Pod columns where they are used and the roll-up ahead of the action list,
   // the K <= 4 instantiations fit their 64-register cap (32 warps per SM) without spilling.
   __shared__ uint32_t s_in[kD2Warps][32];                  // the cluster's cl_in record (RecordCI)
   __shared__ kr_cluster_result s_cr[kD2Warps];             // the cluster's kr_cluster_result, built in place
@@ -403,9 +405,9 @@ __global__ void __launch_bounds__(kD2Warps * 32, (K <= 4 && !kMH ? 32 : 16) / kD
   // that walk was 4 M of the 13.8 M warp instructions of a 63 %-dirty epoch and nearly all of a 1 %-dirty one.
   if (kInc && !mine) return;
   // pod count + first head, and the whole bucket beside them (stale records past the count are masked once it is here)
-  uint4 *bucket = a.sc.bucket + (size_t)(mine ? c : 0) * S;
+  uint2 *bucket = a.sc.bucket + (size_t)(mine ? c : 0) * S;
   uint4 dyn = make_uint4(0, 0, 0, 0);
-  uint4 recs[K] = {};
+  uint2 recs[K] = {};
   if (mine) {
     dyn = __ldcg(&a.sc.cl_dyn[c]);
 #pragma unroll
@@ -429,7 +431,7 @@ __global__ void __launch_bounds__(kD2Warps * 32, (K <= 4 && !kMH ? 32 : 16) / kD
       if (keep && lost && !fresh) keep = __ldcg(&a.sc.stamp[recs[k].x]) != epoch;
       const uint32_t bal = __ballot_sync(0xFFFFFFFFu, keep);
       if (keep) {
-        uint4 rec = recs[k];
+        uint2 rec = recs[k];
         rec.y &= ~KR_ROW_FRESH;
         const uint32_t to = kept + __popc(bal & lt);
         if (fresh || to != j) { bucket[to] = rec; if (to != j) a.sc.pos[rec.x] = to; }
@@ -449,7 +451,7 @@ __global__ void __launch_bounds__(kD2Warps * 32, (K <= 4 && !kMH ? 32 : 16) / kD
     }
     // the compacted bucket (every register rewritten, so none of the records read before the compaction stays live past it)
 #pragma unroll
-    for (int k = 0; k < K; k++) recs[k] = mine && (uint32_t)(k * 32) + lane < kept ? __ldcg(&bucket[k * 32 + lane]) : make_uint4(0, 0, 0, 0);
+    for (int k = 0; k < K; k++) recs[k] = mine && (uint32_t)(k * 32) + lane < kept ? __ldcg(&bucket[k * 32 + lane]) : make_uint2(0, 0);
   }
   const uint32_t cf = ci.flags(), G = ci.group_cnt(), g0 = ci.group_off();
   const uint8_t suspend_status = ci.suspend_status(), ext_err = ci.ext_err_kind(), old_prov = ci.cond_status(KR_COND_PROVISIONED);
@@ -739,7 +741,7 @@ __global__ void __launch_bounds__(kD2Warps * 32, (K <= 4 && !kMH ? 32 : 16) / kD
   // ---------------- status roll-up + record (needs nothing from the action list and the placement below: it comes first, so no
   // register of theirs is live through it)
   if (!(cf & KR_CF_SKIP)) {  // (every lane runs it, uniformly: the inputs are one broadcast load away in the record)
-    const uint32_t head_name = (n_heads == 1 && head_pos != 0xFFFFFFFFu) ? __ldcg(&a.sc.bucket[(size_t)c * S + head_pos].w) : 0u;
+    const uint32_t head_name = (n_heads == 1 && head_pos != 0xFFFFFFFFu) ? __ldg(&s.p_name_id[head_pod]) : 0u;
     status_rollup(a.s, a.f, ci, cr, P, (uint32_t)n_heads, n_heads > 0 ? (int32_t)head_pod : -1, head_aux, head_name, ready, available, all_running);
   }
   __syncwarp();
@@ -858,8 +860,8 @@ __global__ void __launch_bounds__(kD2Warps * 32, (K <= 4 && !kMH ? 32 : 16) / kD
           for (int k = 0; k < K; k++) {
             // runningPods of this group: listed, not deleted by name, label present and numeric
             if ((pw[k] >> 16) == gi && (pw[k] & KR_PP_HAS_REPLICA_IDX) && (mh ? ((mh_head >> k) & 1u) != 0 : (act[k] == KR_ACT_KEEP && pidx[k] != 0xFFFFFFFFu))) {
-              // (read again here from the bucket: no register holds it, or the bucket's address, through the decisions)
-              const int32_t idx = (int32_t)__ldcg(&a.sc.bucket[(size_t)c * S + k * 32 + lane].z);
+              // (read from the Pod column: the bucket record does not carry it, and no register holds it through the decisions)
+              const int32_t idx = __ldg(&s.p_replica_index[pidx[k]]);
               if (idx >= 0 && (uint64_t)idx >= w0 && (uint64_t)idx < w0 + 1024 && (uint64_t)idx < bound)
                 atomicOr(&s_bits[warp][(idx - w0) >> 5], 1u << ((idx - w0) & 31));
             }

@@ -82,7 +82,8 @@ struct ScratchDev {
   uint32_t *deferred_list;                                     // clusters left for decide phase 1 (count in totals[4])
   int32_t *gacc;                                               // [4 * n_groups] spill accumulators (clusters with > KR_SMEM_GROUPS groups)
   // bucket pipeline (kr_bucket2.cuh)
-  uint4 *bucket; uint32_t bucket_stride;                       // [n_clusters * stride] {pod idx, slot << 16 | flags, replica index, name id}, arrival order
+  uint2 *bucket; uint32_t bucket_stride;                       // [n_clusters * stride] {pod idx, slot << 16 | flags}, arrival order (the replica index and
+                                                               // the name are read from the Pod columns where they are used)
   uint32_t *wt_bits; uint32_t wt_bits_mask;                    // Bloom bitmap over the workersToDelete (ns, name) keys (power-of-two bit count)
   uint32_t *cl_in;                                             // [32 * n_clusters] every per-cluster input of the decide kernel as ONE 128-byte record (KR_CI_*)
   uint4 *cl_dyn;                                               // [n_clusters] {pods bucketed so far, incremental epoch in which the cluster LOST a row (its bucket must be
@@ -99,7 +100,7 @@ struct ScratchDev {
   uint32_t *inc;                                               // [16] counters / flags of the running epoch (KR_INC_*)
   // large RayClusters (KR_OPT_LARGE_CLUSTERS, kr_large.cuh): records of arrival rank >= bucket_stride go to the cluster's region
   uint4 *lg;                                                   // [n_clusters] {region offset, region capacity (0: not large), scratch segment, kept pods | KR_LG_OWNED}; nullptr: none
-  uint4 *region;                                               // large-cluster record arena (16-byte bucket records)
+  uint2 *region;                                               // large-cluster record arena (8-byte bucket records)
 };
 enum {
   KR_INC_TOUCHED = 0, KR_INC_DIRTY = 1,

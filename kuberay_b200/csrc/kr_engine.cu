@@ -493,13 +493,13 @@ ScratchLayout scratch_layout(const kr_sizes &n) {
   L.mh_head = o; o = align_up(o + (size_t)n.n_pods);
   L.act_tmp_idx = o; o = align_up(o + 4 * (size_t)n.n_pods);
   L.act_tmp_code = o; o = align_up(o + (size_t)n.n_pods);
-  // bucket pipeline: fixed-stride buckets of 16-byte records.  Room for a stride of >= 4x the mean cluster size, at least 64
+  // bucket pipeline: fixed-stride buckets of 8-byte records.  Room for a stride of >= 4x the mean cluster size, at least 64
   // records per cluster; snapshots of very many tiny clusters (64 records per cluster would dwarf the pods) do without.
   L.bucket_entries = std::max<size_t>(4 * (size_t)n.n_pods, 64 * (size_t)n.n_clusters);
   L.bucket_entries = std::max<size_t>(L.bucket_entries, std::min<size_t>(256 * (size_t)n.n_clusters, (size_t)4 << 20));  // small snapshots: room for the widest stride
   if (64 * (size_t)n.n_clusters > 8 * (size_t)n.n_pods + (4u << 20)) L.bucket_entries = 0;
   L.cl_in = o; o = align_up(o + 128 * (size_t)n.n_clusters);
-  L.bucket = o; o = align_up(o + 16 * L.bucket_entries);
+  L.bucket = o; o = align_up(o + sizeof(uint2) * L.bucket_entries);
   // incremental epochs (kr_incr.cuh): [stamps | dirty flags | counters] start out zero (one memset when the layout moves)
   L.inc_zero = o;
   L.stamp = o; o = align_up(o + 4 * (size_t)n.n_pods);
@@ -604,9 +604,9 @@ struct kr_engine {
   uint32_t n_lsort = 0;         // ... of which the first n_lsort are k_large_sort's; the huge ones after them go to k_huge_tiles / k_huge_merge
   uint32_t n_tiles = 0;         // tiles of the huge RayClusters in the device tile table
   // Sized for the capacities so that they never grow, allocated when an option first needs them (an engine without either pays
-  // nothing): [lg: 16 B x max_clusters | lg_list: 4 B x max_clusters] for both options, regions (16 B x large_entries) for large ones
+  // nothing): [lg: 16 B x max_clusters | lg_list: 4 B x max_clusters] for both options, regions (8 B x large_entries) for large ones
   uint8_t *d_lg = nullptr;
-  uint4 *d_region = nullptr;
+  uint2 *d_region = nullptr;
   size_t large_entries = 0;
   std::vector<uint4> h_lg; std::vector<uint32_t> h_lg_list;  // host side of the last upload (kept alive while it is in flight)
   // KR_OPT_HUGE_CLUSTERS, allocated when first turned on, for the capacities: the tile table {cluster, first rank, first tile, tiles}
@@ -744,7 +744,7 @@ ScratchDev bind_scratch(const ScratchLayout &L, uint8_t *b) {
   s.mh_meta = reinterpret_cast<uint32_t *>(b + L.mh_meta); s.mh_cnt = reinterpret_cast<uint32_t *>(b + L.mh_cnt);
   s.mh_flg = reinterpret_cast<uint32_t *>(b + L.mh_flg); s.mh_act = b + L.mh_act; s.mh_head = b + L.mh_head;
   s.act_tmp_idx = reinterpret_cast<uint32_t *>(b + L.act_tmp_idx); s.act_tmp_code = b + L.act_tmp_code;
-  s.bucket = reinterpret_cast<uint4 *>(b + L.bucket); s.bucket_stride = 0;
+  s.bucket = reinterpret_cast<uint2 *>(b + L.bucket); s.bucket_stride = 0;
   s.wt_bits = reinterpret_cast<uint32_t *>(b + L.wt_bits); s.wt_bits_mask = L.wt_bits_n - 1;
   s.cl_in = reinterpret_cast<uint32_t *>(b + L.cl_in);
   s.cl_dyn = reinterpret_cast<uint4 *>(b + L.cl_dyn);
@@ -1962,7 +1962,7 @@ int kr_engine_set_option(kr_engine *e, uint32_t option, uint64_t value) {
       // this many records hold the regions of any snapshot within the capacities
       const size_t Np = e->cfg.max_pods;
       const size_t entries = Np * 5 / 4 + 32 * (Np / 257 + 1);
-      CK(cudaMalloc((void **)&e->d_region, 16 * entries));
+      CK(cudaMalloc((void **)&e->d_region, sizeof(uint2) * entries));
       e->large_entries = entries;
     }
     if (value && option == KR_OPT_HUGE_CLUSTERS && !e->d_huge) {

@@ -79,9 +79,12 @@ __global__ void __launch_bounds__(kHugeThreads) k_huge_tiles(Decide2Args a, Huge
   const uint32_t j0 = r0 + min(tid * per, n), j1 = min(j0 + per, r1);
   uint32_t kept = 0;
   for (uint32_t j = j0; j < j1; j++) {
-    const uint4 rec = __ldcg(rec_slot(sc, c, j));
+    const uint2 rec = __ldcg(rec_slot(sc, c, j));
     const bool keep = !lost || (rec.y & KR_ROW_FRESH) || __ldcg(&sc.stamp[rec.x]) != epoch;
-    if (keep) { sc.rows[rec.x] = make_uint4(rec.w, a.s.p_replica_name_id[rec.x], rec.z, rec.y & ~KR_ROW_FRESH); kept++; }
+    if (keep) {  // (the name and the replica index come from the Pod columns, as in k_large_sort)
+      sc.rows[rec.x] = make_uint4(a.s.p_name_id[rec.x], a.s.p_replica_name_id[rec.x], (uint32_t)a.s.p_replica_index[rec.x], rec.y & ~KR_ROW_FRESH);
+      kept++;
+    }
   }
   // exclusive prefix of the kept counts over the CTA
   uint32_t x = kept;
@@ -94,7 +97,7 @@ __global__ void __launch_bounds__(kHugeThreads) k_huge_tiles(Decide2Args a, Huge
   uint32_t o = before + x - kept;
   uint32_t *stash = h.stash + (size_t)blockIdx.x * kHugeTile;
   for (uint32_t j = j0; j < j1; j++) {
-    const uint4 rec = __ldcg(rec_slot(sc, c, j));
+    const uint2 rec = __ldcg(rec_slot(sc, c, j));
     const bool keep = !lost || (rec.y & KR_ROW_FRESH) || __ldcg(&sc.stamp[rec.x]) != epoch;
     if (keep) { s_idx[o] = rec.x; stash[o] = rec.x; o++; }
   }
@@ -161,7 +164,7 @@ __global__ void __launch_bounds__(kHugeThreads) k_huge_merge(Decide2Args a, Huge
     for (uint32_t k = tid; k < n_me; k += kHugeThreads) {
       const uint32_t p = __ldcg(stash + k);
       const uint4 row = __ldcg(&sc.rows[p]);
-      *rec_slot(sc, c, base + k) = make_uint4(p, row.w, row.z, row.x);
+      *rec_slot(sc, c, base + k) = make_uint2(p, row.w);
       sc.pos[p] = base + k;
     }
     if (me == t.z && tid == 0) { sc.cl_dyn[c].x = total; sc.cl_dyn[c].y = 0u; }

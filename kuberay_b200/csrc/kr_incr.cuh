@@ -319,7 +319,7 @@ __global__ void __launch_bounds__(256) k_inc_refresh(SnapDev s, ScratchDev sc) {
 // ------------------------------------------------------------------------------------------------ k_inc_admit
 // KR_OPT_LARGE_GROWTH: the grow buffer (16-byte words) holds the grow list {cluster, old region offset, old capacity, -} at
 // [0, KR_GROW_MAX), k_inc_grow's result {cluster, offset, capacity, newly listed} at [KR_GROW_MAX, 2 KR_GROW_MAX), then the spill:
-// per record a pair {pod, rank, cluster, -}, record.
+// per record a pair {pod, rank, cluster, -}, {pod, slot << 16 | flags, -, -} (the 8-byte record).
 static constexpr uint32_t kGrowResult = KR_GROW_MAX, kGrowSpill = 2 * KR_GROW_MAX;
 static constexpr size_t kGrowBytes = 16 * ((size_t)kGrowSpill + 2 * (size_t)KR_GROW_SPILL);
 
@@ -329,7 +329,7 @@ static constexpr size_t kGrowBytes = 16 * ((size_t)kGrowSpill + 2 * (size_t)KR_G
 // Out of line, and given the few scratch fields it uses by value: k_inc_admit's loop keeps its registers, and no kernel parameter
 // has its address taken (that would copy the whole parameter block to local memory in every thread of the launch).
 __device__ __noinline__ bool grow_spill(const uint4 *lg, uint32_t *inc, uint32_t *pos, uint32_t stride, uint4 *grow, uint32_t c,
-                                        uint32_t rank, uint4 rec) {
+                                        uint32_t rank, uint2 rec) {
   const uint4 l = __ldcg(&lg[c]);  // (bound whenever the pass grows: 0 for an ordinary cluster)
   if (rank == stride + l.y) {
     const uint32_t j = atomicAdd(&inc[KR_INC_GROW], 1u);
@@ -339,7 +339,7 @@ __device__ __noinline__ bool grow_spill(const uint4 *lg, uint32_t *inc, uint32_t
   const uint32_t k = atomicAdd(&inc[KR_INC_SPILL], 1u);
   if (k >= KR_GROW_SPILL) return false;
   grow[kGrowSpill + 2 * k] = make_uint4(rec.x, rank, c, 0u);
-  grow[kGrowSpill + 2 * k + 1] = rec;
+  grow[kGrowSpill + 2 * k + 1] = make_uint4(rec.x, rec.y, 0u, 0u);
   pos[rec.x] = rank;
   return true;
 }
@@ -354,7 +354,6 @@ __global__ void __launch_bounds__(256) k_inc_admit(SnapDev s, ScratchDev sc, Res
     const uint32_t p = sc.touched[i], c_old = sc.touched_old[i];
     if (p >= n.n_pods) continue;
     const uint32_t ns = s.p_ns_id[p], cn = s.p_cluster_name_id[p], gn = s.p_group_name_id[p], nm = s.p_name_id[p], pk = s.p_packed[p];
-    const uint32_t ri = (uint32_t)s.p_replica_index[p];
     uint32_t c = n.n_clusters, cflags = 0, gname0 = 0;
     const bool matched = cl_probe(sc, ns, cn, c, cflags, gname0);
     uint32_t slot = KR_ROW_NO_GROUP, g0 = 0xFFFFFFFFu;
@@ -395,9 +394,9 @@ __global__ void __launch_bounds__(256) k_inc_admit(SnapDev s, ScratchDev sc, Res
     if (matched && c == c_old) {
       // the usual event — a status update: the row stays in its RayCluster, its record is rewritten where it sits and the row's
       // stamp is lifted (nothing of this cluster has to be dropped on its account)
-      uint4 *at = rec_slot(sc, c, sc.pos[p]);  // (a record of a large RayCluster may sit in its region)
+      uint2 *at = rec_slot(sc, c, sc.pos[p]);  // (a record of a large RayCluster may sit in its region)
       if (!at) { sc.inc[KR_INC_VOID] = 1u; continue; }
-      *at = make_uint4(p, (slot << 16) | flags, ri, nm);
+      *at = make_uint2(p, (slot << 16) | flags);
       sc.stamp[p] = 0u;
       continue;  // (k_inc_retire marked the cluster dirty)
     }
@@ -408,8 +407,8 @@ __global__ void __launch_bounds__(256) k_inc_admit(SnapDev s, ScratchDev sc, Res
     }
     mark_dirty(sc, c, epoch);  // the row joined this cluster: a fresh record at the end of its bucket
     const uint32_t rank = atomicAdd(&sc.cl_dyn[c].x, 1u);
-    const uint4 rec = make_uint4(p, (slot << 16) | flags | KR_ROW_FRESH, ri, nm);
-    if (uint4 *at = rec_slot(sc, c, rank)) { *at = rec; sc.pos[p] = rank; }
+    const uint2 rec = make_uint2(p, (slot << 16) | flags | KR_ROW_FRESH);
+    if (uint2 *at = rec_slot(sc, c, rank)) { *at = rec; sc.pos[p] = rank; }
     // (an ordinary RayCluster outgrew its bucket, a large one its region: k_inc_grow gives it a new one, or the full pass reclassifies)
     else if (!grow || !grow_spill(sc.lg, sc.inc, sc.pos, sc.bucket_stride, grow, c, rank, rec)) sc.inc[KR_INC_VOID] = 1u;
   }
@@ -529,7 +528,7 @@ __global__ void __launch_bounds__(256) k_inc_clusters_release(SnapDev s, Scratch
   const uint4 rec = sc.cl_rec[o];  // {group_off, group_cnt} of the old row
   const uint32_t P = sc.cl_dyn[o].x;
   for (uint32_t k = lane; k < P; k += 32) {
-    const uint4 *at = rec_slot(sc, o, k);
+    const uint2 *at = rec_slot(sc, o, k);
     uint32_t ns, nm;
     if (at) inc_touch(s, sc, r, at->x, epoch, n_resident, ns, nm);
   }
@@ -557,7 +556,7 @@ __global__ void __launch_bounds__(256) k_inc_large_release(SnapDev s, ScratchDev
   const uint32_t o = g.x, S = sc.bucket_stride, epoch = inc_epoch(sc), tid = threadIdx.x;
   const uint32_t P = min(__ldcg(&sc.cl_dyn[o].x), S + g.z);
   for (uint32_t k = tid; k < P; k += blockDim.x) {
-    const uint4 *at = k < S ? sc.bucket + (size_t)o * S + k : sc.region + g.y + (k - S);
+    const uint2 *at = k < S ? sc.bucket + (size_t)o * S + k : sc.region + g.y + (k - S);
     uint32_t ns, nm;
     inc_touch(s, sc, r, at->x, epoch, n_resident, ns, nm);
   }

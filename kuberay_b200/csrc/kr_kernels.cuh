@@ -11,7 +11,7 @@
 //   k_build_tables   cluster table (ns,name)->{idx, flags, name of worker group 0}, the 128-byte per-cluster input record (cl_in),
 //                    workersToDelete-name table + Bloom bitmap, head-aux table; closes the running incremental epoch
 //   k_match2         per pod: selector match -> its cluster's fixed-stride bucket at an arrival rank (one returning atomic):
-//                    16-byte record {pod idx, group slot | flags, replica index, name id}; first head per cluster by a 64-bit atomicMax
+//                    8-byte record {pod idx, group slot | flags}; first head per cluster by a 64-bit atomicMax
 //   k_decide2        one warp per RayCluster, bucket in registers, ARRIVAL order: order-free counts, the ordered delete prefix by
 //                    min-extraction / counting rank, status roll-up, action list + replica indices placed with one atomic per cluster
 //   k_hash3          (stream H, concurrent) SHA-1 + base32hex of every muted-spec JSON: producer warp (staging, padding, W expansion)

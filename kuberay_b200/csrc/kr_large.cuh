@@ -119,7 +119,8 @@ __global__ void __launch_bounds__(256) k_inc_grow(SnapDev s, ScratchDev sc, uint
     // (a record whose RayCluster is not on the list, or whose rank the new region does not hold, cannot be placed: void rather than
     // write into another region; the full pass that follows rebuilds every bucket and region)
     if (s_e[lo].x != at.z || at.y < S + s_e[lo].z || at.y - S >= s_cap[lo]) { sc.inc[KR_INC_VOID] = 1u; continue; }
-    sc.region[s_off[lo] + at.y - S] = __ldcg(&grow[kGrowSpill + 2 * k + 1]);
+    const uint4 rec = __ldcg(&grow[kGrowSpill + 2 * k + 1]);
+    sc.region[s_off[lo] + at.y - S] = make_uint2(rec.x, rec.y);
   }
   if (blockIdx.x == 0) {
     if (tid < n) {
@@ -192,9 +193,12 @@ __global__ void __launch_bounds__(kLargeSortThreads) k_large_sort(Decide2Args a,
   const uint32_t j0 = min(tid * per, P), j1 = min(j0 + per, P);
   uint32_t kept = 0;
   for (uint32_t j = j0; j < j1; j++) {
-    const uint4 rec = __ldcg(rec_slot(sc, c, j));
+    const uint2 rec = __ldcg(rec_slot(sc, c, j));
     const bool keep = !lost || (rec.y & KR_ROW_FRESH) || __ldcg(&sc.stamp[rec.x]) != epoch;
-    if (keep) { sc.rows[rec.x] = make_uint4(rec.w, a.s.p_replica_name_id[rec.x], rec.z, rec.y & ~KR_ROW_FRESH); kept++; }
+    if (keep) {  // (the name and the replica index come from the Pod columns: the 8-byte record does not carry them)
+      sc.rows[rec.x] = make_uint4(a.s.p_name_id[rec.x], a.s.p_replica_name_id[rec.x], (uint32_t)a.s.p_replica_index[rec.x], rec.y & ~KR_ROW_FRESH);
+      kept++;
+    }
   }
   // exclusive prefix of the kept counts over the CTA
   uint32_t x = kept;
@@ -206,7 +210,7 @@ __global__ void __launch_bounds__(kLargeSortThreads) k_large_sort(Decide2Args a,
   for (uint32_t w = 0; w < kLargeSortThreads / 32; w++) { const uint32_t v = s_warp[w]; before += w < warp ? v : 0u; total += v; }
   uint32_t o = before + x - kept;
   for (uint32_t j = j0; j < j1; j++) {
-    const uint4 rec = __ldcg(rec_slot(sc, c, j));
+    const uint2 rec = __ldcg(rec_slot(sc, c, j));
     const bool keep = !lost || (rec.y & KR_ROW_FRESH) || __ldcg(&sc.stamp[rec.x]) != epoch;
     if (keep) s_idx[o++] = rec.x;
   }
@@ -224,7 +228,7 @@ __global__ void __launch_bounds__(kLargeSortThreads) k_large_sort(Decide2Args a,
     for (uint32_t k = tid; k < total; k += kLargeSortThreads) {
       const uint32_t p = s_idx[k];
       const uint4 row = sc.rows[p];
-      *rec_slot(sc, c, k) = make_uint4(p, row.w, row.z, row.x);
+      *rec_slot(sc, c, k) = make_uint2(p, row.w);
       sc.pos[p] = k;
     }
     if (tid == 0) { sc.cl_dyn[c].x = total; sc.cl_dyn[c].y = 0u; }
