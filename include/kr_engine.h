@@ -340,7 +340,7 @@ typedef struct kr_group_result {        /* 32 bytes */
   int32_t  n_list;               /* len(workerPods.Items) (:761) */
   int32_t  n_unhealthy;          /* :794 */
   int32_t  n_running;            /* len(runningPods.Items) (:837-842); multi-host: valid replica groups (:1055) */
-  int32_t  diff;                 /* :849; multi-host: replicasToCreate (:1064) */
+  int32_t  diff;                 /* :849 (Go int, saturated at INT32_MIN); multi-host: replicasToCreate (:1064) */
   uint32_t n_create;             /* entries of create_idx this group owns: pods to create; for a KR_GR_MULTIHOST group REPLICA GROUPS to create
                                     (each one is NumOfHosts pods with one generated replica name, raycluster_controller.go:1081-1094) */
   uint32_t create_off;           /* first replica index of this group in create_idx[] (one entry per pod; multi-host: per replica) */

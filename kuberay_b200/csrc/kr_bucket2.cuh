@@ -641,12 +641,12 @@ __global__ void __launch_bounds__(kD2Warps * 32, (K <= 4 && !kMH ? 32 : 16) / kD
           } else {
             gr.flags |= KR_GR_WTD_EXECUTED; mode = GM_NORMAL;  // :814-849
             const int32_t running = n_list - n_wtd;
-            const int32_t diff = expected - running;
-            gr.n_running = running; gr.diff = diff;
+            const long long diff = (long long)expected - running;  // Go int (:757, :849): no int32 wrap below -2^31
+            gr.n_running = running; gr.diff = diff < INT32_MIN ? INT32_MIN : (int32_t)diff;  // (saturated in the record)
             if (diff > 0) gr.n_create = (uint32_t)diff;
             else if (diff < 0) {
               if (!autoscaling || a.f.env_random_pod_delete) {  // :898-928
-                const long long remove = -(long long)diff;
+                const long long remove = -diff;
                 if (remove > running) {  // expected < 0: the Go loop would index past runningPods (:917)
                   prefix = running; gr.flags |= KR_GR_ABORTED;
                   cr.err_kind = KR_ERR_NEGATIVE_EXPECTED; cr.err_arg = expected; abort_here = true;

@@ -40,6 +40,30 @@ class Env:
     enable_random_pod_delete: bool = False   # ENABLE_RANDOM_POD_DELETE == "true"
 
 
+def _terminated_text(pod: dict) -> str:
+    """fmt's %v of getRayContainerStateTerminated(pod) (raycluster_controller.go:1237-1248), a *ContainerStateTerminated:
+    <nil>, or &{ExitCode Signal Reason Message StartedAt FinishedAt ContainerID} with zero times."""
+    if not snapmod.ray_container_terminated(pod):
+        return "<nil>"
+    t = {}
+    if "rayContainerTerminated" not in pod:
+        ray_name = (pod.get("containers") or [{}])[0].get("name")
+        t = next(((st.get("state") or {}).get("terminated") for st in pod.get("containerStatuses") or [] if st.get("name") == ray_name), {})
+    zero = "{0001-01-01 00:00:00 +0000 UTC}"
+    return f"&{{{t.get('exitCode', 0)} {t.get('signal', 0)} {t.get('reason', '')} {t.get('message', '')} {zero} {zero} {t.get('containerID', '')}}}"
+
+
+def _should_delete(pod: dict) -> bool:
+    """shouldDeletePod's verdict (raycluster_controller.go:1181-1231)."""
+    ph = pod.get("phase", "")
+    return ph in ("Failed", "Succeeded") or (ph == "Running" and snapmod.ray_container_terminated(pod) and pod.get("restartPolicy") == "Never")
+
+
+def _pod_status_text(pod: dict) -> str:
+    """The Pod part of the delete events (:703-710, 798-805, 947-948)."""
+    return f"Pod status: {pod.get('phase', '')}; Pod restart policy: {pod.get('restartPolicy', '')}; Ray container terminated status: {_terminated_text(pod)}"
+
+
 class ApiError(Exception):
     """A Create/Delete call that failed at the API server (anything but NotFound)."""
 
@@ -145,13 +169,27 @@ class RayClusterReconciler:
 
     def _apply_decisions(self, pr: PassResult, ci: int):
         """-> None, the plain error string reconcilePods returns, or ("Failed<Verb><Kind>Pod", message) when an API call
-        failed: the reference joins one of the five ErrFailed* markers (utils/constant.go:322-334) onto that error, and only
-        those set the ReplicaFailure condition (raycluster_controller.go:1563-1571)."""
+        failed: the reference records a Warning event, joins one of the five ErrFailed* markers (utils/constant.go:322-334)
+        onto that error, and only those set the ReplicaFailure condition (raycluster_controller.go:1563-1571)."""
         self._stage = "FailedDeleteAllPods"
+        self._warning = None   # (reason, message before the error) of the call in flight
         try:
             return self._apply_decisions_inner(pr, ci)
         except ApiError as ex:
+            if self._warning:
+                self.client.events.append(("Warning", self._warning[0], f"{self._warning[1]}, {ex}"))
             return (self._stage, str(ex))
+
+    def _delete_listed(self, ns: str, name: str):
+        """Delete of a Pod the List returned (:701, :796): NotFound is an error there, unlike at :823 and :920."""
+        if not self.client.delete_pod(ns, name):
+            raise ApiError(f'pods "{name}" not found')
+
+    def _delete_collection(self, pods: list[tuple[str, str]], terminating: list[bool]):
+        """deleteAllPods (:130-146): one DeleteAllOf, issued only when a listed Pod is not terminating yet."""
+        if not all(terminating):
+            for ns, name in pods:
+                self.client.delete_pod(ns, name)
 
     def _apply_decisions_inner(self, pr: PassResult, ci: int) -> str | None:
         cl = self.client
@@ -164,20 +202,20 @@ class RayClusterReconciler:
         listed = [(int(res.act_pod_idx[i]), int(res.act_code[i])) for i in range(int(res.act_start[ci]), int(res.act_start[ci]) + int(res.act_cnt[ci]))]
         ev = cl.events.append
         path = int(cr["path"])
-        if path == abi.PATH_SKIPPED:
-            return "external error" if cr["err_kind"] == abi.ERR_EXTERNAL else None
+        if path == abi.PATH_SKIPPED:                # an earlier sub-reconciler's error is what Reconcile returns (:308-314)
+            return (cluster.get("extErr") or {}).get("message", "") if cr["err_kind"] == abi.ERR_EXTERNAL else None
         if path == abi.PATH_SUSPENDING_DELETE_ALL:  # :633-643
-            for pi, act in listed:
-                if act == abi.ACT_DELETE_ALL_SUSPEND:
-                    cl.delete_pod(*meta.pod_keys[pi])
+            rows = [pi for pi, act in listed if act == abi.ACT_DELETE_ALL_SUSPEND]
+            self._warning = ("FailedToDeletePodCollection", f"Failed deleting Pods due to suspension for RayCluster {ns}/{cname}")
+            self._delete_collection([meta.pod_keys[pi] for pi in rows], [bool(pr.pods[pi].get("deletionTimestamp")) for pi in rows])
             ev(("Normal", EV_DELETED_POD, f"Deleted Pods for RayCluster {ns}/{cname} due to suspension"))
             return None
         if path == abi.PATH_SUSPENDED_NOOP:
             return None
         if path == abi.PATH_RECREATE_DELETE_ALL:    # :659-669
-            for pi, act in listed:
-                if act == abi.ACT_DELETE_ALL_RECREATE:
-                    cl.delete_pod(*meta.pod_keys[pi])
+            rows = [pi for pi, act in listed if act == abi.ACT_DELETE_ALL_RECREATE]
+            self._warning = ("FailedToDeletePodCollection", f"Failed deleting Pods due to spec change with Recreate upgradeStrategy for RayCluster {ns}/{cname}")
+            self._delete_collection([meta.pod_keys[pi] for pi in rows], [bool(pr.pods[pi].get("deletionTimestamp")) for pi in rows])
             ev(("Normal", EV_DELETED_POD, f"Deleted all Pods for RayCluster {ns}/{cname} due to spec change with Recreate upgradeStrategy"))
             return None
         if cr["head_update_annotations"]:           # :1155-1162
@@ -190,18 +228,20 @@ class RayClusterReconciler:
         if ha == abi.HEAD_DELETE:                   # :700-711
             pi = next(pi for pi, act in listed if act == abi.ACT_DELETE_HEAD)
             pod = pr.pods[pi]
-            cl.delete_pod(*meta.pod_keys[pi])
-            ev(("Normal", EV_DELETED_HEAD_POD, f"Deleted head Pod {ns}/{pod['name']}; Pod status: {pod.get('phase', '')}; Pod restart policy: {pod.get('restartPolicy', '')}; "
-                f"Ray container terminated status: {snapmod.ray_container_terminated(pod)}"))
+            self._warning = ("FailedToDeleteHeadPod", f"Failed deleting head Pod {ns}/{pod['name']}; {_pod_status_text(pod)}")
+            self._delete_listed(*meta.pod_keys[pi])
+            ev(("Normal", EV_DELETED_HEAD_POD, f"Deleted head Pod {ns}/{pod['name']}; {_pod_status_text(pod)}"))
             return self._should_delete_reason(pod, "head")
         if ha == abi.HEAD_SKIP_RESTART:
             return None
         if ha == abi.HEAD_MULTIPLE:                 # :738-747
-            names = [p["name"] for p in cl.pods_of(ns, cname, **{snapmod.RAY_NODE_TYPE_LABEL: "head"})]  # the head List of :674
-            return f"{int(cr['err_arg'])} head pods found {names}. Please delete extra head pods"
+            names = [p["name"] for p in pr.pods if p.get("namespace", "default") == ns and (p.get("labels") or {}).get(snapmod.RAY_CLUSTER_LABEL) == cname
+                     and p["labels"].get(snapmod.RAY_NODE_TYPE_LABEL) == "head"]  # the head List of :674, from the pass's cache
+            return f"{int(cr['err_arg'])} head pods found [{' '.join(names)}]. Please delete extra head pods"   # %v of a []string
         self._stage = "FailedCreateHeadPod"         # :736
         if ha == abi.HEAD_CREATE:                   # :735, createHeadPod :1307-1337
             pod = self._build_pod(cluster, (-1, 0, 0, ""), cluster_hash=bytes(res.hash[ci]).decode())
+            self._warning = ("FailedToCreateHeadPod", f"Failed to create head Pod {ns}/")   # :1330: the Pod has only a generateName
             cl.create_pod(pod)
             ev(("Normal", EV_CREATED_HEAD_POD, f"Created head Pod {ns}/{pod['name']}"))
         # worker groups in spec order (:751-933)
@@ -218,9 +258,9 @@ class RayClusterReconciler:
             if fl & abi.GR_EXPECT_PENDING:
                 continue
             if fl & abi.GR_SUSPENDED:               # :766-775
-                for pi, act in in_group:
-                    if act == abi.ACT_DELETE_GROUP_SUSPEND:
-                        cl.delete_pod(*meta.pod_keys[pi])
+                rows = [pi for pi, act in in_group if act == abi.ACT_DELETE_GROUP_SUSPEND]
+                self._warning = ("FailedToDeleteWorkerPodCollection", f"Failed deleting worker Pods for suspended group {gname} in RayCluster {ns}/{cname}")
+                self._delete_collection([meta.pod_keys[pi] for pi in rows], [bool(pr.pods[pi].get("deletionTimestamp")) for pi in rows])
                 ev(("Normal", EV_DELETED_WORKER_POD, f"Deleted all pods for suspended worker group {gname} in RayCluster {ns}/{cname}"))
                 continue
             if fl & abi.GR_MULTIHOST:
@@ -231,9 +271,9 @@ class RayClusterReconciler:
             unhealthy = [pi for pi, act in in_group if act == abi.ACT_DELETE_UNHEALTHY]
             for pi in unhealthy:                    # :790-806
                 pod = pr.pods[pi]
-                cl.delete_pod(*meta.pod_keys[pi])
-                ev(("Normal", EV_DELETED_WORKER_POD, f"Deleted worker Pod {ns}/{pod['name']}; Pod status: {pod.get('phase', '')}; Pod restart policy: {pod.get('restartPolicy', '')}; "
-                    f"Ray container terminated status: {snapmod.ray_container_terminated(pod)}"))
+                self._warning = ("FailedToDeleteWorkerPod", f"Failed deleting worker Pod {ns}/{pod['name']}; {_pod_status_text(pod)}")
+                self._delete_listed(*meta.pod_keys[pi])
+                ev(("Normal", EV_DELETED_WORKER_POD, f"Deleted worker Pod {ns}/{pod['name']}; {_pod_status_text(pod)}"))
             if unhealthy:
                 return f"delete {len(unhealthy)} unhealthy worker Pods"  # :811
             if fl & abi.GR_WTD_EXECUTED:            # :817-835: one Delete per name, NotFound tolerated
@@ -244,6 +284,7 @@ class RayClusterReconciler:
                     # hold yet (wtd_pod_idx == -1: not in the cache, or owned by another shard) is still deleted there;
                     # wtd_pod_idx only told the engine which listed pods leave runningPods (:837-842)
                     assert int(res.wtd_pod_idx[w0 + k]) < 0 or meta.pod_keys[int(res.wtd_pod_idx[w0 + k])] == (ns, nm)
+                    self._warning = ("FailedToDeleteWorkerPod", f"Failed deleting pod {ns}/{nm}")
                     if cl.delete_pod(ns, nm):
                         ev(("Normal", EV_DELETED_WORKER_POD, f"Deleted pod {ns}/{nm}"))
                 # (:835 clears worker.ScaleStrategy.WorkersToDelete on the loop's COPY of the group spec only — the CR keeps
@@ -252,11 +293,13 @@ class RayClusterReconciler:
             for k in range(int(gr["n_create"])):    # :865-890
                 idx = int(res.create_idx[int(gr["create_off"]) + k])
                 pod = self._build_pod(cluster, (gi, idx if self.env.multihost_indexing_gate else 0, 0, ""))   # :878 / :887
+                self._warning = ("FailedToCreateWorkerPod", f"Failed to create worker Pod for the cluster {ns}/{cname}")
                 cl.create_pod(pod)
                 ev(("Normal", EV_CREATED_WORKER_POD, f"Created worker Pod {ns}/{pod['name']}"))
             self._stage = "FailedDeleteWorkerPod"   # :922
             for pi, act in in_group:                # :916-928
                 if act == abi.ACT_DELETE_RANDOM:
+                    self._warning = ("FailedToDeleteWorkerPod", f"Failed deleting Pod {ns}/{pr.pods[pi]['name']}")
                     cl.delete_pod(*meta.pod_keys[pi])
                     ev(("Normal", EV_DELETED_WORKER_POD, f"Deleted Pod {ns}/{pr.pods[pi]['name']}"))
             if fl & abi.GR_ABORTED:
@@ -273,16 +316,30 @@ class RayClusterReconciler:
         gname = grp["groupName"]
         reasons = {abi.ACT_DELETE_MH_INCOMPLETE: "cleanup of incomplete multi-host group", abi.ACT_DELETE_MH_WTD: "autoscaler scale-down request",
                    abi.ACT_DELETE_MH_SCALE_DOWN: "scaling down"}
-        for pi, act in in_group:
+        # an unhealthy replica group is deleted with the reason of its first Pod (List order) that shouldDeletePod names (:992-999)
+        trigger, rank = {}, {}
+        for k, (pi, act) in enumerate(in_group):
+            pod = pr.pods[pi]
+            rname = (pod.get("labels") or {}).get(snapmod.REPLICA_NAME_LABEL)
+            rank.setdefault(rname, k)
+            if act == abi.ACT_DELETE_MH_UNHEALTHY and _should_delete(pod) and rname not in trigger:
+                trigger[rname], rank[rname] = pod, k
+        # deletePods runs one replica group at a time: unhealthy groups in the order of their trigger, then the others in the order
+        # of their first Pod (:986-1007, 1108-1118)
+        order = sorted(in_group, key=lambda e: (e[1] != abi.ACT_DELETE_MH_UNHEALTHY, rank[(pr.pods[e[0]].get("labels") or {}).get(snapmod.REPLICA_NAME_LABEL)]))
+        for pi, act in order:
             if act in (abi.ACT_DELETE_MH_INCOMPLETE, abi.ACT_DELETE_MH_UNHEALTHY, abi.ACT_DELETE_MH_WTD, abi.ACT_DELETE_MH_SCALE_DOWN):
                 pod = pr.pods[pi]
+                self._warning = ("FailedToDeleteWorkerPod", f"Failed deleting worker Pod {ns}/{pod['name']} for group {gname}; {_pod_status_text(pod)}")
                 if cl.delete_pod(*meta.pod_keys[pi]):
-                    why = reasons.get(act) or self._should_delete_reason(pod, "worker")
+                    # (no trigger: the engine named a replica group shouldDeletePod does not; the event then shows it)
+                    why = reasons.get(act) or self._should_delete_reason(trigger.get((pod.get("labels") or {}).get(snapmod.REPLICA_NAME_LABEL), pod), "worker")
                     cl.events.append(("Normal", EV_DELETED_WORKER_POD, f"Deleted worker Pod {ns}/{pod['name']} for group {gname}: {why}"))
         ek = int(cr["err_kind"])
         if int(gr["flags"]) & abi.GR_ABORTED:
-            if ek == abi.ERR_MH_INCOMPLETE:
-                return "cleaned up incomplete replica group, requeueing"
+            if ek == abi.ERR_MH_INCOMPLETE:         # :982 names the replica group whose Pods were deleted
+                rname = next((pr.pods[pi].get("labels") or {}).get(snapmod.REPLICA_NAME_LABEL) for pi, act in in_group if act == abi.ACT_DELETE_MH_INCOMPLETE)
+                return f"cleaned up incomplete replica group {rname}, requeueing"
             if ek == abi.ERR_MH_WTD:
                 return f"deleted {int(cr['err_arg'])} worker Pods based on ScaleStrategy, requeueing"
             if ek == abi.ERR_MH_NOT_MULTIPLE:
@@ -294,6 +351,7 @@ class RayClusterReconciler:
             rname = f"{gname}-{cl.gen_suffix()}"
             for j in range(hosts):
                 pod = self._build_pod(cluster, (gi, idx, j, rname))   # :1090
+                self._warning = ("FailedToCreateWorkerPod", f"Failed to create worker Pod for the cluster {ns}/{cname}")
                 cl.create_pod(pod)
                 cl.events.append(("Normal", EV_CREATED_WORKER_POD, f"Created worker Pod {ns}/{pod['name']}"))
         return None
@@ -327,7 +385,7 @@ class RayClusterReconciler:
             return (f"The {node_type} Pod {pod['name']} status is {ph} which is a terminal state. "
                     "KubeRay will delete the Pod and create new Pods in the next reconciliation if necessary.")
         return (f"The Pod status of the {node_type} Pod {pod['name']} is {ph}, and the Ray container terminated status is "
-                f"{snapmod.ray_container_terminated(pod)}. The container is unable to restart due to its restart policy {pod.get('restartPolicy', '')}, so KubeRay will delete it.")
+                f"{_terminated_text(pod)}. The container is unable to restart due to its restart policy {pod.get('restartPolicy', '')}, so KubeRay will delete it.")
 
     # ------------------------------------------------------------------ calculateStatus
     def calculate_status(self, ns: str, name: str, reconcile_err=None) -> tuple[dict | None, str | None]:
@@ -364,7 +422,10 @@ class RayClusterReconciler:
         conds_old = {c["type"]: c for c in old.get("conditions") or []}
         conds = []
         order = [c["type"] for c in old.get("conditions") or []]
-        for slot in range(abi.NUM_CONDS):
+        # a condition calculateStatus adds goes last, in the order of its SetStatusCondition calls (:1566, 1614-1622, 1630-1693)
+        suspending = int(pr.snap.c_suspend_status[ci]) == abi.SUSPEND_SUSPENDING
+        for slot in (abi.COND_REPLICA_FAILURE, abi.COND_HEAD_POD_READY, abi.COND_PROVISIONED,
+                     *((abi.COND_SUSPENDING, abi.COND_SUSPENDED) if suspending else (abi.COND_SUSPENDED, abi.COND_SUSPENDING))):
             t = snapmod.COND_NAMES[slot]
             if t not in order and cr["cond_status"][slot] != abi.COND_ABSENT:
                 order.append(t)
@@ -391,7 +452,8 @@ class RayClusterReconciler:
                 if int(pr.snap.c_ext_err_kind[ci]) == var:
                     cond["message"] = it.str(mid) or ""
             conds.append(cond)
-        new["conditions"] = conds
+        if conds or "conditions" in old:
+            new["conditions"] = conds
         hid = [int(x) for x in cr["head_ids"]]
         new["head"] = {"podIP": it.str(hid[0]) or "", "serviceIP": it.str(hid[1]) or "", "podName": it.str(hid[2]) or "", "serviceName": it.str(hid[3]) or ""}
         cluster = self.client.clusters[(ns, cname)]
@@ -414,16 +476,22 @@ class RayClusterReconciler:
 
     # ------------------------------------------------------------------ the full Reconcile body for one key (:296-355)
     def reconcile(self, ns: str, name: str, now: str = "now") -> tuple[float, str | None]:
-        """-> (requeue seconds, error).  One pass feeds both the decisions and the status, as the engine produces them —
+        """-> (requeue seconds, error; 0 = no requeue).  One pass feeds both the decisions and the status, as the engine produces them —
         unless a side-effect call failed at the API server: the record's status was computed for reconcileErr == nil, so it
         is discarded and the status is re-evaluated (status-only pass, c_ext_err_kind = the ErrFailed* kind), which is what
         calculateStatus(ctx, instance, reconcileErr) sees in the reference (:308-316, 1563-1577, 1599)."""
         pr = self._pass()
-        ci = self._cluster_index(pr, ns, name)
+        return self.reconcile_record(pr, self._cluster_index(pr, ns, name), now)
+
+    def reconcile_record(self, pr: PassResult, ci: int, now: str = "now") -> tuple[float, str | None]:
+        """The Reconcile body of RayCluster ci once the pass `pr` decided it."""
+        ns, name = pr.meta.cluster_keys[ci]
+        if int(pr.snap.c_flags[ci]) & abi.CF_SKIP:   # being deleted: no status, no requeue (:291-294)
+            return 0.0, None
         err = self._apply_decisions(pr, ci)
         if isinstance(err, tuple):
-            new, cerr = self.calculate_status(ns, name, err)
-            err = f"{err[0]}: {err[1]}"
+            err = f"{err[0]}\n{err[1]}"   # errors.Join(ErrFailed..., err).Error(): also the ReplicaFailure message (:1570)
+            new, cerr = self.calculate_status(ns, name, (err.split("\n", 1)[0], err))
         else:
             new, cerr = self.status_from_record(pr, ci)
         inconsistent = False

@@ -148,7 +148,8 @@ def find_suspend_status(conditions) -> int:
 
 
 def ray_container_terminated(pod: dict) -> bool:
-    """getRayContainerStateTerminated(pod) != nil (raycluster_controller.go:1237-1248)."""
+    """getRayContainerStateTerminated(pod) != nil (raycluster_controller.go:1237-1248): a present `terminated` state counts even
+    when it is empty."""
     if "rayContainerTerminated" in pod:
         return bool(pod["rayContainerTerminated"])
     containers = pod.get("containers") or []
@@ -157,7 +158,7 @@ def ray_container_terminated(pod: dict) -> bool:
     ray_name = containers[0].get("name")
     for st in pod.get("containerStatuses") or []:
         if st.get("name") == ray_name:
-            return bool((st.get("state") or {}).get("terminated"))
+            return (st.get("state") or {}).get("terminated") is not None
     return False
 
 

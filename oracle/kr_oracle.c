@@ -559,11 +559,10 @@ static void reconcile_pods(const octx *x, oscratch *t, uint32_t c, const char *h
     int32_t running = 0;
     for (uint32_t i = 0; i < L->n; i++) if (!t->deleted[i]) running++;
     gr->n_running = running;
-    /* Go's int32 arithmetic wraps (:836): an expected count near -2^31 turns into billions of pods to create.  The subtraction is done
-     * in uint32_t so that the wrap is defined here too; such a stream is a capacity error, and ivec_reserve stops the process if it
-     * cannot even be counted (tests/fuzz_objects.py keeps |expected| <= 300 for that reason). */
-    int32_t diff = (int32_t)((uint32_t)expected - (uint32_t)running);
-    gr->diff = diff;
+    /* Go takes diff in int (:757, :849): it does not wrap.  An expected count near -2^31 (an int32 product that wrapped in
+     * GetWorkerGroupDesiredReplicas) less the running pods lies below INT32_MIN; it is a scale-down, and the record keeps it saturated. */
+    const int64_t diff = (int64_t)expected - (int64_t)running;
+    gr->diff = diff < INT32_MIN ? INT32_MIN : (int32_t)diff;
     if (diff > 0) { /* :865-890 */
       uint32_t want = (uint32_t)diff;
       gr->n_create = want;
@@ -587,7 +586,7 @@ static void reconcile_pods(const octx *x, oscratch *t, uint32_t c, const char *h
     } else if (diff < 0) { /* :894-932 */
       int autoscaling = (cf & KR_CF_AUTOSCALING) != 0;
       if (!autoscaling || f->env_random_pod_delete) {
-        int64_t remove = -(int64_t)diff;
+        int64_t remove = -diff;
         int64_t done = 0;
         for (uint32_t i = 0; i < L->n && done < remove; i++) {
           if (t->deleted[i]) continue;

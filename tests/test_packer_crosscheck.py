@@ -33,7 +33,7 @@ def go_ray_container_terminated(pod):
     want = containers[0].get("name")
     for cs in pod.get("containerStatuses") or []:
         if cs.get("name") == want:
-            return (cs.get("state") or {}).get("terminated") is not None and bool((cs.get("state") or {}).get("terminated"))
+            return (cs.get("state") or {}).get("terminated") is not None  # a non-nil pointer, even to an empty state
     return False
 
 
@@ -157,6 +157,7 @@ def test_container_status_forms_the_fuzzer_does_not_generate():
         ("t-ray-second", [{"name": "sidecar", "state": {"running": {}}}, {"name": "ray-head", "state": {"terminated": {"reason": "OOMKilled", "message": "oom"}}}]),
         ("t-no-status", []),
         ("t-other-name", [{"name": "not-ray", "state": {"terminated": {"reason": "Completed"}}}]),
+        ("t-empty-terminated", [{"name": "ray-head", "state": {"terminated": {}}}]),
     ]
     extra = []
     for name, statuses in variants:
@@ -173,6 +174,7 @@ def test_container_status_forms_the_fuzzer_does_not_generate():
     _check_snapshot(clusters, allpods, jobs)
     got = {p["name"]: (go_should_delete_pod(p), go_find_head_pod_ready_condition(p)) for p in extra}
     assert got["t-sidecar-first"][0] is False and got["t-ray-second"][0] is True and got["t-no-status"][0] is False and got["t-other-name"][0] is False
+    assert got["t-empty-terminated"][0] is True
     assert got["t-sidecar-first"][1] == ("False", "Error", "containers with unready status: [ray-head]; sidecar: boom")
     assert got["t-waiting"][1] == ("False", "ImagePullBackOff", "ray-head: Back-off pulling image")
 
