@@ -535,6 +535,53 @@ int kr_hash_compare_batch(kr_engine *e, const kr_hash_compare_row *rows, uint32_
 /* Timings of the last batch. */
 int kr_last_profile(kr_engine *e, kr_profile *prof);
 
+/* What the last pass was, and why it was not an incremental epoch (DESIGN §4.3 names each rule).  An operator exports these as
+ * counters to see which option, cap or commit keeps a fleet on full passes; tests hold every fallback rule to its cause. */
+enum { KR_PASSK_INCREMENTAL = 1, KR_PASSK_FULL = 2 };
+enum { KR_PIPE_BUCKET = 1, KR_PIPE_SORT = 2, KR_PIPE_RADIX = 3 };
+/* kr_pass_report.why_full bits.  A bit is recorded where the resident state is dropped or an incremental attempt voids: by a commit
+ * while the state is resident (and by every later commit of the same epoch), by the pass that finds it cannot follow the epoch, by
+ * the device in the attempt, or by a full pass that leaves nothing resident (those bits describe the NEXT pass).  They accumulate
+ * until a pass reports them, and are cleared then. */
+enum {
+  KR_FULL_FIRST      = 1u << 0,   /* nothing resident yet: the engine's first pass */
+  KR_FULL_CAPACITY   = 1u << 1,   /* the previous full pass overran kr_config.max_creates (KR_E_CAPACITY) */
+  KR_FULL_DISABLED   = 1u << 2,   /* KR_OPT_INCREMENTAL = 0, or KR_NO_INCR=1 / KR_NO_BUCKET=1 / KR_FORCE_RADIX=1 in the environment */
+  KR_FULL_FLAGS      = 1u << 3,   /* kr_flags differ from the resident pass's */
+  KR_FULL_POD_LISTS  = 1u << 4,   /* the previous pass fetched the full pod lists (fetch_pod_lists = 1: sort pipeline, nothing resident) */
+  KR_FULL_LARGE      = 1u << 5,   /* the previous pass left the bucket pipeline: a RayCluster had more Pods than the stride and the
+                                     options in force hold (more than 256 without KR_OPT_LARGE_CLUSTERS, more than KR_LARGE_MAX_PODS
+                                     without KR_OPT_HUGE_CLUSTERS, or regions past their arena) */
+  KR_FULL_WIDE       = 1u << 6,   /* the previous pass left the bucket pipeline: a RayCluster had more than 32 worker groups without
+                                     KR_OPT_WIDE_CLUSTERS */
+  KR_FULL_OPTION     = 1u << 7,   /* KR_OPT_LARGE_CLUSTERS / _WIDE_CLUSTERS / _HUGE_CLUSTERS toggled: takes effect at this full pass */
+  KR_FULL_COLUMNS    = 1u << 8,   /* a wholesale commit of the pod columns (kr_snapshot_commit, KR_PART_COLUMNS) */
+  KR_FULL_SIZES      = 1u << 9,   /* kr_snapshot_begin moved a row count the options in force do not follow, or laid the arenas out
+                                     again (no KR_OPT_FIXED_LAYOUT), or a RayCluster count moved without an object commit behind it */
+  KR_FULL_STRUCTURAL = 1u << 10,  /* an object commit changed a table key or a CSR offset (device diff, k_inc_objects) */
+  KR_FULL_ROW_MAP    = 1u << 11,  /* RayClusters created, deleted, moved or regrouped in a way the pass cannot follow (KR_OPT_CLUSTER_
+                                     CREATES / _DELETES / _GROUP_EDITS / _LARGE_MOVES rules: more than 4 096 rows, a renumbering that is
+                                     not swap-remove, a duplicated key, a large row without KR_OPT_LARGE_MOVES, a wide row without
+                                     KR_OPT_WIDE_CLUSTERS, a second object commit that does not compose, too many adopting RayClusters,
+                                     a bucket arena too small for the new count) */
+  KR_FULL_OVERFLOW   = 1u << 12,  /* a RayCluster outgrew its bucket or region and no growth option gave it room (device) */
+  KR_FULL_GROW_LIMIT = 1u << 13,  /* KR_OPT_LARGE_GROWTH / _HUGE_GROWTH refused a growth: grow list, spill, list cap, region arena,
+                                     tile reserve or capacity, or past KR_LARGE_MAX_PODS without KR_OPT_HUGE_GROWTH (device) */
+  KR_FULL_ARENA      = 1u << 14   /* a cursor of the pass's arenas (action list, create arena, per-cluster sort scratch) ran past its
+                                     end (device) */
+};
+typedef struct kr_pass_report {       /* 16 bytes */
+  uint8_t  kind;        /* KR_PASSK_INCREMENTAL or KR_PASSK_FULL */
+  uint8_t  pipeline;    /* KR_PIPE_BUCKET / KR_PIPE_SORT / KR_PIPE_RADIX: the pipeline whose results stood */
+  uint8_t  attempts;    /* full-pass attempts that voided before the one that stood (stride widened, regions laid out, next pipeline) */
+  uint8_t  hash_wait;   /* a decide warp gave up waiting for its digest: the pass was rerun on the two-phase schedule */
+  uint32_t stride;      /* bucket stride of the pass; 0 off the bucket pipeline */
+  uint32_t why_full;    /* KR_FULL_* bits: every cause recorded since the previous pass; 0 for an incremental pass */
+  uint32_t reserved_;
+} kr_pass_report;
+/* The last pass that returned KR_OK (kr_reconcile_batch, _device_only, _batch_profiled); KR_E_STATE before any.  A struct copy. */
+int kr_last_pass(kr_engine *e, kr_pass_report *out);
+
 /* Engine options (call before the first kr_snapshot_begin).
  * KR_OPT_FIXED_LAYOUT = 1: lay the arenas out once, for the capacities given to kr_engine_create, instead of per snapshot.
  *   Column addresses then never move: kr_snapshot_begin(sizes) only sets the live row counts (<= capacities) and returns the

@@ -7,6 +7,7 @@ import "C"
 
 import (
 	"context"
+	"sync"
 	"time"
 )
 
@@ -45,6 +46,16 @@ type Batcher struct {
 	lookups chan lookup
 	res     *Results
 	podset  uint64
+	mu      sync.Mutex // guards stats: a metrics scraper reads them from its own goroutine
+	stats   Stats
+}
+
+// Stats counts the passes of the batcher's epochs by kind, and the full passes by cause (KR_FULL_* bit -> passes that reported
+// it; one pass may report several).  What an operator's metrics code exports: a fleet whose epochs keep falling back to full passes
+// shows which rule sends them there (DESIGN §4.3), and so which option or cap would keep them incremental.
+type Stats struct {
+	Incremental, Full uint64
+	Causes            map[uint32]uint64
 }
 
 func NewBatcher(p *Packer, flags Flags, period time.Duration) *Batcher {
@@ -116,7 +127,39 @@ func (b *Batcher) epoch() bool {
 	}
 	b.res = res
 	_, b.podset = b.p.Epoch()
+	if rep, err := b.p.Engine().LastPass(); err == nil {
+		b.count(rep)
+	}
 	return true
+}
+
+func (b *Batcher) count(rep PassReport) {
+	b.mu.Lock()
+	defer b.mu.Unlock()
+	if rep.Incremental {
+		b.stats.Incremental++
+		return
+	}
+	b.stats.Full++
+	if b.stats.Causes == nil {
+		b.stats.Causes = map[uint32]uint64{}
+	}
+	for _, c := range FullCauses {
+		if rep.WhyFull&c.Bit != 0 {
+			b.stats.Causes[c.Bit]++
+		}
+	}
+}
+
+// Stats returns a copy of the pass counters; safe from any goroutine.
+func (b *Batcher) Stats() Stats {
+	b.mu.Lock()
+	defer b.mu.Unlock()
+	s := Stats{Incremental: b.stats.Incremental, Full: b.stats.Full, Causes: map[uint32]uint64{}}
+	for k, v := range b.stats.Causes {
+		s.Causes[k] = v
+	}
+	return s
 }
 
 func (b *Batcher) record(ns, name string) *Record {

@@ -282,6 +282,37 @@ func (e *Engine) Reconcile(f Flags) (*Results, error) {
 	return wrapResults(&view, e.sizes), nil
 }
 
+// PassReport is kr_pass_report: what the last pass was and why it was not an incremental epoch.
+type PassReport struct {
+	Incremental bool   // KR_PASSK_INCREMENTAL; false: a full pass
+	Pipeline    uint8  // KR_PIPE_BUCKET / KR_PIPE_SORT / KR_PIPE_RADIX
+	Attempts    uint8  // full-pass attempts that voided before the one that stood
+	HashWait    bool   // a decide warp gave up waiting for its digest: the pass was rerun on the two-phase schedule
+	Stride      uint32 // bucket stride; 0 off the bucket pipeline
+	WhyFull     uint32 // KR_FULL_* bits; 0 for an incremental pass
+}
+
+// FullCauses names the KR_FULL_* bits, in bit order: the label values of an operator's per-cause counter.
+var FullCauses = []struct {
+	Bit  uint32
+	Name string
+}{
+	{C.KR_FULL_FIRST, "first"}, {C.KR_FULL_CAPACITY, "capacity"}, {C.KR_FULL_DISABLED, "disabled"}, {C.KR_FULL_FLAGS, "flags"},
+	{C.KR_FULL_POD_LISTS, "pod_lists"}, {C.KR_FULL_LARGE, "large"}, {C.KR_FULL_WIDE, "wide"}, {C.KR_FULL_OPTION, "option"},
+	{C.KR_FULL_COLUMNS, "columns"}, {C.KR_FULL_SIZES, "sizes"}, {C.KR_FULL_STRUCTURAL, "structural"}, {C.KR_FULL_ROW_MAP, "row_map"},
+	{C.KR_FULL_OVERFLOW, "overflow"}, {C.KR_FULL_GROW_LIMIT, "grow_limit"}, {C.KR_FULL_ARENA, "arena"},
+}
+
+// LastPass reports the last pass that returned KR_OK (one struct copy, no device work).
+func (e *Engine) LastPass() (PassReport, error) {
+	var r C.kr_pass_report
+	if rc := C.kr_last_pass(e.h, &r); rc != C.KR_OK {
+		return PassReport{}, e.err(rc)
+	}
+	return PassReport{Incremental: r.kind == C.KR_PASSK_INCREMENTAL, Pipeline: uint8(r.pipeline), Attempts: uint8(r.attempts),
+		HashWait: r.hash_wait != 0, Stride: uint32(r.stride), WhyFull: uint32(r.why_full)}, nil
+}
+
 // HashBatch: utils.GenerateJsonHash's digest half for n messages (msgs[offsets[i]:offsets[i+1]]); out receives 32 characters each.
 func (e *Engine) HashBatch(msgs []byte, offsets []uint64, out []byte) error {
 	n := len(offsets) - 1

@@ -304,6 +304,33 @@ class kr_profile(C.Structure):
                 ("h2d_bytes", C.c_uint64), ("d2h_bytes", C.c_uint64)]
 
 
+# kr_last_pass (kr_pass_report): what the last pass was and which KR_FULL_* rules kept it from being an incremental epoch
+PASSK_INCREMENTAL, PASSK_FULL = 1, 2
+PIPE_BUCKET, PIPE_SORT, PIPE_RADIX = 1, 2, 3
+FULL_BITS = {  # name -> KR_FULL_* bit, in bit order
+    "FIRST": 1 << 0, "CAPACITY": 1 << 1, "DISABLED": 1 << 2, "FLAGS": 1 << 3, "POD_LISTS": 1 << 4, "LARGE": 1 << 5, "WIDE": 1 << 6,
+    "OPTION": 1 << 7, "COLUMNS": 1 << 8, "SIZES": 1 << 9, "STRUCTURAL": 1 << 10, "ROW_MAP": 1 << 11, "OVERFLOW": 1 << 12,
+    "GROW_LIMIT": 1 << 13, "ARENA": 1 << 14,
+}
+globals().update({"FULL_" + k: v for k, v in FULL_BITS.items()})
+
+
+def full_names(why: int) -> list[str]:
+    """The KR_FULL_* names of a why_full bit set, in bit order (an unknown bit reads as BIT<n>)."""
+    names = [k for k, v in FULL_BITS.items() if why & v]
+    known = sum(FULL_BITS.values())
+    names += [f"BIT{i}" for i in range(32) if (why & ~known) >> i & 1]
+    return names
+
+
+class kr_pass_report(C.Structure):
+    _fields_ = [("kind", C.c_uint8), ("pipeline", C.c_uint8), ("attempts", C.c_uint8), ("hash_wait", C.c_uint8),
+                ("stride", C.c_uint32), ("why_full", C.c_uint32), ("reserved_", C.c_uint32)]
+
+
+assert C.sizeof(kr_pass_report) == 16
+
+
 class kr_oracle_out(C.Structure):  # oracle/kr_oracle.h (test infrastructure; declared here only for layout sharing)
     _fields_ = [("clusters", C.c_void_p), ("hash", C.c_void_p), ("groups", C.c_void_p), ("wtd_pod_idx", C.c_void_p),
                 ("sorted_pod_idx", C.c_void_p), ("sorted_action", C.c_void_p), ("create_idx", C.c_void_p), ("jobs", C.c_void_p),
@@ -315,7 +342,7 @@ class kr_oracle_out(C.Structure):  # oracle/kr_oracle.h (test infrastructure; de
 ENGINE_SYMBOLS = [
     "kr_device_count", "kr_engine_create", "kr_engine_destroy", "kr_snapshot_begin", "kr_snapshot_commit", "kr_snapshot_commit_parts", "kr_snapshot_commit_pod_rows", "kr_snapshot_commit_pod_values", "kr_snapshot_commit_object_rows", "kr_snapshot_commit_spec_rows", "kr_engine_set_option", "kr_engine_get_option",
     "kr_reconcile_batch", "kr_reconcile_device_only", "kr_reconcile_batch_profiled", "kr_results_fetch",
-    "kr_hash_batch", "kr_last_profile", "kr_group_results_device", "kr_group_results_copy", "kr_last_error", "kr_algorithmic_bytes",
+    "kr_hash_batch", "kr_last_profile", "kr_last_pass", "kr_group_results_device", "kr_group_results_copy", "kr_last_error", "kr_algorithmic_bytes",
     "kr_spec_json_emit", "kr_spec_json_emit_arena", "kr_quantity_canonical", "kr_spec_json_last_error", "kr_hash_compare_batch",
     "kr_group_create", "kr_group_destroy", "kr_group_size", "kr_group_engine", "kr_group_device", "kr_group_shard_of_uid", "kr_group_route",
     "kr_group_commit", "kr_group_reconcile", "kr_group_allgather_group_results", "kr_group_last_error",

@@ -801,8 +801,8 @@ __global__ void __launch_bounds__(kD2Warps * 32, (K <= 4 && !kMH ? 32 : 16) / kD
       const uint32_t old_act = a.r.act_cnt[c], old_create = s_old_create[warp];
       need = (n_act > a.sc.act_res[c] ? 1u : 0u) | (n_create_cluster > a.sc.cre_res[c] ? 2u : 0u);
       if (need) base = atomicAdd(reinterpret_cast<unsigned long long *>(&a.r.totals[8]), ((unsigned long long)((need & 2u) ? n_create_cluster : 0u) << 32) | ((need & 1u) ? n_act : 0u));
-      if ((need & 1u) && (uint64_t)(uint32_t)base + n_act > a.n.n_pods) a.sc.inc[KR_INC_VOID] = 1u;          // the action list is full of abandoned runs:
-      if ((need & 2u) && (uint64_t)(uint32_t)(base >> 32) + n_create_cluster > a.create_cap) a.sc.inc[KR_INC_VOID] = 1u;  // a full pass packs it again
+      if ((need & 1u) && (uint64_t)(uint32_t)base + n_act > a.n.n_pods) atomicOr(&a.sc.inc[KR_INC_VOID], KR_FULL_ARENA);         // the action list is full of abandoned runs:
+      if ((need & 2u) && (uint64_t)(uint32_t)(base >> 32) + n_create_cluster > a.create_cap) atomicOr(&a.sc.inc[KR_INC_VOID], KR_FULL_ARENA);  // a full pass packs it again
       if (n_act != old_act) atomicAdd(&a.r.totals[2], n_act - old_act);
       if (n_create_cluster != old_create) atomicAdd(&a.r.totals[6], n_create_cluster - old_create);
     }

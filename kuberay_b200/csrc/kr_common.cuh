@@ -104,10 +104,11 @@ struct ScratchDev {
 };
 enum {
   KR_INC_TOUCHED = 0, KR_INC_DIRTY = 1,
-  KR_INC_STRUCTURAL = 2,   // an object commit changed a table key / CSR offset: the resident tables are stale, take a full pass
+  KR_INC_STRUCTURAL = 2,   // an object commit changed a table key / CSR offset: the resident tables are stale, take a full pass (KR_FULL_STRUCTURAL)
   KR_INC_EPOCH = 3,        // epochs completed; stamps / dirty flags of the running epoch carry this + 1
   KR_INC_HEADS = 4,        // the pod idx -> head-aux row table must be rebuilt
-  KR_INC_VOID = 5,         // the incremental attempt is void (a bucket or an arena overflowed): take a full pass
+  KR_INC_VOID = 5,         // the incremental attempt is void (a bucket or an arena overflowed): take a full pass.  Both words hold the
+                           // KR_FULL_* bits of their causes (atomicOr; readers test them for non-zero) for kr_last_pass
   KR_INC_GROUPS = 6,       // gather: group records staged so far
   KR_INC_LSEG = 7,         // large RayClusters: scratch positions handed out so far (k_large_sort)
   KR_INC_GROW = 8,         // KR_OPT_LARGE_GROWTH: RayClusters k_inc_admit put on the grow list (k_inc_grow, kr_incr.cuh)

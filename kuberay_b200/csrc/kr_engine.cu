@@ -670,6 +670,13 @@ struct kr_engine {
   IncStageLayout inc_layout{};   // ... as the last incremental pass laid them out
   uint32_t *h_inc = nullptr;     // pinned copy of the epoch counters (16 words) + the changed-cluster list
   uint32_t *h_changed = nullptr; size_t h_changed_cap = 0;
+  // kr_last_pass: the KR_FULL_* causes recorded since the last pass (a full pass that leaves nothing resident starts the next
+  // pass's with its own), whether a commit of this epoch dropped the resident state (the later ones then record theirs too), the
+  // report run_pass made of its pass and the one the last call that returned KR_OK published
+  uint32_t why_full = KR_FULL_FIRST;
+  bool epoch_dropped = false;
+  kr_pass_report pass_made{}, pass_last{};
+  bool has_pass = false;
 };
 
 namespace {
@@ -1288,6 +1295,37 @@ int after_bucket_void(kr_engine *e) {
   e->lg_cursor = off;
   return upload_lg(e);  // (on the pass's stream: ordered before the rerun)
 }
+// A commit drops the resident state: its cause goes to the next pass's report (and so do the causes of the epoch's later commits).
+void drop_state(kr_engine *e, uint32_t why) {
+  if (e->inc_valid || e->epoch_dropped) { e->why_full |= why; e->epoch_dropped = true; }
+  e->inc_valid = false;
+}
+// Why a full pass left nothing resident (KR_FULL_*; 0: it did): every term of run_pass_once's bucket-pipeline test, and of
+// after_full_pass's, that failed.
+uint32_t why_not_resident(const kr_engine *e, const kr_flags &f) {
+  if (e->inc_valid) return 0;
+  uint32_t why = 0;
+  if (e->no_incr || e->no_bucket || e->env_radix) why |= KR_FULL_DISABLED;
+  if (e->ran_bucket) return e->h_totals[9] > e->cfg.max_creates ? why | KR_FULL_CAPACITY : why;  // (totals[9]: the bucket pipeline's create extent)
+  if (f.fetch_pod_lists) why |= KR_FULL_POD_LISTS;
+  if (e->bstride == 0 || (e->force_radix && !e->env_radix) || (size_t)e->sizes.n_clusters * e->bstride > e->sl.bucket_entries) why |= KR_FULL_LARGE;
+  if (e->rec.snap_max_groups > KR_SMEM_GROUPS && !e->wide_on) why |= KR_FULL_WIDE;
+  return why;
+}
+// The pass's results stand: run_pass makes its report (the call publishes it when it returns KR_OK), and the causes recorded for
+// it make way for those the pass leaves for the next one.
+void make_report(kr_engine *e, bool inc, uint32_t attempts, bool hash_wait, uint32_t why_next) {
+  kr_pass_report &p = e->pass_made;
+  p = kr_pass_report{};
+  p.kind = inc ? KR_PASSK_INCREMENTAL : KR_PASSK_FULL;
+  p.pipeline = e->ran_bucket ? KR_PIPE_BUCKET : e->ran_fast ? KR_PIPE_SORT : KR_PIPE_RADIX;
+  p.attempts = (uint8_t)attempts;
+  p.hash_wait = hash_wait ? 1 : 0;
+  p.stride = e->ran_bucket ? e->bstride : 0;
+  p.why_full = e->why_full;
+  e->why_full = why_next;
+  e->epoch_dropped = false;
+}
 // a bucket-pipeline pass leaves everything an incremental epoch needs on the device
 void after_full_pass(kr_engine *e, const kr_flags &f) {
   // (a pass whose create runs overran kr_config.max_creates is reported as KR_E_CAPACITY and left groups' runs unwritten: an
@@ -1327,8 +1365,10 @@ int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile
   if (e->map_pending ? e->rec.res_clusters != n.n_clusters || e->rec.res_groups != n.n_groups || e->map_sizes.n_clusters != n.n_clusters ||
                            e->map_sizes.n_groups != n.n_groups || (size_t)n.n_clusters * e->bstride > e->sl.bucket_entries ||
                            (e->rec.snap_max_groups > KR_SMEM_GROUPS && !e->wide_on) || (adopt && n_init > kAdoptMax)
-                     : n.n_clusters != e->inc_n_clusters)
+                     : n.n_clusters != e->inc_n_clusters) {
+    e->why_full |= e->map_pending ? KR_FULL_ROW_MAP : KR_FULL_SIZES;
     return KR_OK;
+  }
   const bool grow = grows(e) && e->bstride;  // (KR_OPT_LARGE_GROWTH: a RayCluster that outgrows its room gets a region in this pass)
   const bool huge_grow = grow && huge_grows(e);  // (KR_OPT_HUGE_GROWTH: ... past KR_LARGE_MAX_PODS Pods too, with tiles)
   const uint32_t n_large_gone = (uint32_t)m.large.size() / 4;  // (KR_OPT_LARGE_MOVES: gone rows with a region)
@@ -1476,6 +1516,9 @@ int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile
   commits_read(e);
   e->rec.heads_rebuild = false;  // (rebuilt here, or about to be rebuilt by the full pass)
   if (e->h_inc[KR_INC_VOID] || e->h_inc[KR_INC_STRUCTURAL]) {  // the caller takes the full pass
+    // (the device's KR_FULL_* bits; k_inc_admit reports every record without room as an overflow, which growth refused when it could grow)
+    const uint32_t why = e->h_inc[KR_INC_VOID] | e->h_inc[KR_INC_STRUCTURAL];
+    e->why_full |= grow && (why & KR_FULL_OVERFLOW) ? (why & ~KR_FULL_OVERFLOW) | KR_FULL_GROW_LIMIT : why;
     if (grow) e->lg_stale = true;  // (k_inc_grow may have written regions of this attempt into the device table: the full pass reads the host's)
     return KR_OK;
   }
@@ -1548,15 +1591,21 @@ int run_pass(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile) {
     if (profile) CK(cudaEventRecord(e->ev_a, e->sm));
     bool ok = false;
     if (int rc = run_pass_inc(e, f, done, profile, &ok)) return rc;
-    if (ok) { e->inc_n_pods = e->sizes.n_pods; e->inc_n_heads = e->sizes.n_heads; e->inc_n_clusters = e->sizes.n_clusters; return pass_done(e, done); }
+    if (ok) {
+      e->inc_n_pods = e->sizes.n_pods; e->inc_n_heads = e->sizes.n_heads; e->inc_n_clusters = e->sizes.n_clusters;
+      make_report(e, true, 0, false, 0);
+      return pass_done(e, done);
+    }
     if (e->lg_stale) if (int rc = upload_lg(e)) return rc;  // (a void attempt that grew regions left them in the device table)
-  }
+  } else if (e->inc_valid && !e->no_incr) e->why_full |= KR_FULL_FLAGS;
   e->inc_valid = false; e->ran_inc = false;
   if (e->inc_zero_needed) {  // first pass on this layout: stamps, dirty flags and epoch counters start from zero
     CK(cudaMemsetAsync(e->d_scratch + e->sl.inc_zero, 0, e->sl.inc_zero_end - e->sl.inc_zero, e->sm));
     e->inc_zero_needed = false;
   }
   if (e->rec.spec_order_stale && !f.skip_hash) if (int rc = refresh_order(e)) return rc;
+  uint32_t voided = 0;
+  bool hash_wait = false;
   for (int attempt = 0; attempt < 5; attempt++) {
     if (profile) CK(cudaEventRecord(e->ev_a, e->sm));
     if (int rc = profile ? launch_pass(e, f, true) : run_pass_once(e, f)) return rc;
@@ -1569,9 +1618,15 @@ int run_pass(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile) {
     else e->order_pending = false;
     if (e->h_totals[3] & KR_TOTALS_HASH_WAIT) {  // a decide warp gave up waiting for its digest (a profiled pass never waits): rerun on the two-phase schedule
       e->hash_spin = false; e->gvalid = false;
+      hash_wait = true;
       continue;
     }
-    if (!(e->h_totals[3] & KR_TOTALS_BIG_BUCKET)) { after_full_pass(e, f); return pass_done(e, done); }
+    if (!(e->h_totals[3] & KR_TOTALS_BIG_BUCKET)) {
+      after_full_pass(e, f);
+      make_report(e, false, voided, hash_wait, why_not_resident(e, f));
+      return pass_done(e, done);
+    }
+    voided++;
     // some RayCluster outgrew what this pipeline holds per bucket: bucket pipeline -> wider stride -> sort pipeline -> radix pipeline
     if (e->ran_bucket) {
       if (int rc = after_bucket_void(e)) return rc;
@@ -1901,7 +1956,7 @@ int kr_engine_set_option(kr_engine *e, uint32_t option, uint64_t value) {
   }
   if (option == KR_OPT_INCREMENTAL) {
     e->no_incr = value == 0;
-    if (e->no_incr) e->inc_valid = false;
+    if (e->no_incr) drop_state(e, KR_FULL_DISABLED);
     return KR_OK;
   }
   if (option == KR_OPT_WTD_EDITS) {  // (read at each object commit: nothing resident depends on it)
@@ -1973,7 +2028,8 @@ int kr_engine_set_option(kr_engine *e, uint32_t option, uint64_t value) {
     // the next full pass starts again from the layout's first stride and the fast sort pipeline: a pass with the option off may
     // have left the bucket pipeline (and the fast pipeline, for a cluster above 1024 pods) for this layout
     if (int rc = drop_regions(e, 0)) return rc;
-    e->lg_cursor = 0; e->lg_stale = true; e->inc_valid = false; e->gvalid = false;
+    e->lg_cursor = 0; e->lg_stale = true; e->gvalid = false;
+    drop_state(e, KR_FULL_OPTION);
     e->force_radix = e->env_radix;
     if (e->begun) e->bstride = first_stride(e->sizes);
     return KR_OK;
@@ -2158,17 +2214,21 @@ int kr_snapshot_begin(kr_engine *e, const kr_sizes *sizes, kr_snapshot_bufs *out
     // well, and shrink with KR_OPT_CLUSTER_DELETES (RayClusters deleted by swap-remove); with KR_OPT_GROUP_EDITS the group and name
     // counts may move either way (RayClusters that gained or lost worker groups); the object commit's row map checks the rest.
     const bool fits = (size_t)sizes->n_clusters * e->bstride <= e->sl.bucket_entries;
-    auto moves_ok = [&](uint32_t now, uint32_t was) { return now == was || (now < was ? deletes_on(e) : creates_on(e) && fits); };
     const bool same_groups = sizes->n_clusters == e->sizes.n_clusters && sizes->n_groups == e->sizes.n_groups;
-    const bool keep = e->inc_valid && e->fixed_layout && moves_ok(sizes->n_clusters, e->sizes.n_clusters) &&
-                      (moves_ok(sizes->n_groups, e->sizes.n_groups) || regroups_on(e)) &&
-                      (moves_ok(sizes->n_wtd, e->sizes.n_wtd) || (e->wtd_edits && same_groups) || regroups_on(e)) &&
-                      (sizes->n_jobs == e->sizes.n_jobs || creates_on(e)) && sizes->n_pods >= e->sizes.n_pods;
+    auto keeps = [&](bool room) {
+      auto moves_ok = [&](uint32_t now, uint32_t was) { return now == was || (now < was ? deletes_on(e) : creates_on(e) && room); };
+      return e->inc_valid && e->fixed_layout && moves_ok(sizes->n_clusters, e->sizes.n_clusters) &&
+             (moves_ok(sizes->n_groups, e->sizes.n_groups) || regroups_on(e)) &&
+             (moves_ok(sizes->n_wtd, e->sizes.n_wtd) || (e->wtd_edits && same_groups) || regroups_on(e)) &&
+             (sizes->n_jobs == e->sizes.n_jobs || creates_on(e)) && sizes->n_pods >= e->sizes.n_pods;
+    };
+    const bool keep = keeps(fits);
     if (!e->fixed_layout) { e->committed_full = false; e->inc_zero_needed = true; }
     // (the next pass is a full one, which hashes every message: listed rows may not exist any more)
     if (sizes->n_clusters != e->sizes.n_clusters && !keep) clear_spec_rows(e);
     if (!keep) {
-      e->inc_valid = false;
+      // (KR_OPT_CLUSTER_CREATES follows these counts, but the bucket arena does not hold the new RayClusters at this stride)
+      drop_state(e, keeps(true) ? KR_FULL_ROW_MAP : KR_FULL_SIZES);
       e->force_radix = e->env_radix;
       e->bstride = first_stride(*sizes);
       if (int rc = drop_regions(e, 0)) return rc;
@@ -2242,7 +2302,7 @@ int kr_snapshot_commit_parts(kr_engine *e, uint32_t parts) {
     if (int rc = commit_map(e, moved.map == 1 && stage_objects && !renumbered, oa, voided)) return rc;
   }
   if (moved.wide && e->wide_on) e->lg_stale = true;  // a different wide set is a different list, and grid, of the per-cluster kernels
-  if (parts & KR_PART_COLUMNS) e->inc_valid = false;  // pod columns uploaded wholesale: the resident buckets no longer describe them
+  if (parts & KR_PART_COLUMNS) drop_state(e, KR_FULL_COLUMNS);  // pod columns uploaded wholesale: the resident buckets no longer describe them
   if (moved.order) build_order(e, hb);  // (unchanged lengths and gates: the resident order stands — an object / pod epoch does not pay for it)
   // Asynchronous, in two parts on the copy stream: every column first, the spec-JSON arena (the larger half) second.
   // The pass waits on the two events, so match/place/decide run while the JSON is still crossing PCIe and only the hash
@@ -2266,7 +2326,7 @@ int kr_snapshot_commit_parts(kr_engine *e, uint32_t parts) {
         if (int rc = up(e->il.off[kFirstPodCol + k], 4 * (size_t)n.n_pods)) return rc;
   }
   if (stage_objects) { if (int rc = launch_object_diff(e, oa, n.n_heads, nullptr, n.n_clusters != 0)) return rc; }
-  if (voided) e->inc_valid = false;  // (the diff above copied the object part into place: the full pass reads it)
+  if (voided) drop_state(e, KR_FULL_ROW_MAP);  // (the diff above copied the object part into place: the full pass reads it)
   CK(cudaEventRecord(e->ev_cols, e->scopy));
   if (moved.order && n.n_clusters) {  // the new order travels with this commit
     CK(cudaMemcpyAsync(e->d_order, e->h_order, 4 * (size_t)n.n_clusters, cudaMemcpyHostToDevice, e->scopy)); bytes += 4 * (size_t)n.n_clusters;
@@ -2447,9 +2507,15 @@ int kr_snapshot_commit_pod_values(kr_engine *e, const uint32_t *rows, const uint
   return commit_pod_patch(e, rows, values, n);
 }
 
+// the report of the pass a call that returns KR_OK made (kr_last_pass)
+static int published(kr_engine *e, int rc) {
+  if (rc == KR_OK) { e->pass_last = e->pass_made; e->has_pass = true; }
+  return rc;
+}
+
 int kr_reconcile_device_only(kr_engine *e, const kr_flags *flags) {
   if (!e || !flags) return KR_E_INVALID;
-  return run_pass(e, *flags, e->ev_b, false);
+  return published(e, run_pass(e, *flags, e->ev_b, false));
 }
 
 int kr_reconcile_batch(kr_engine *e, const kr_flags *flags, kr_results_view *out) {
@@ -2465,7 +2531,7 @@ int kr_reconcile_batch(kr_engine *e, const kr_flags *flags, kr_results_view *out
     fprintf(stderr, "kr_reconcile_batch: pass %.0f us (device %.0f us), fetch %.0f us (device copy %.0f us, %llu bytes)%s\n", us(t0, t1), e->prof.kernels_ms * 1e3, us(t1, t2),
             e->prof.d2h_ms * 1e3, (unsigned long long)e->prof.d2h_bytes, e->ran_inc ? " [incremental]" : "");
   }
-  return rc;
+  return published(e, rc);
 }
 
 int kr_reconcile_batch_profiled(kr_engine *e, const kr_flags *flags, kr_profile *prof) {
@@ -2478,7 +2544,7 @@ int kr_reconcile_batch_profiled(kr_engine *e, const kr_flags *flags, kr_profile 
     e->prof.kernel_ms[i] = t;
   }
   if (prof) *prof = e->prof;
-  return KR_OK;
+  return published(e, KR_OK);
 }
 
 int kr_results_fetch(kr_engine *e, kr_results_view *out) {
@@ -2630,6 +2696,13 @@ int kr_hash_compare_batch(kr_engine *e, const kr_hash_compare_row *rows, uint32_
 int kr_last_profile(kr_engine *e, kr_profile *prof) {
   if (!e || !prof) return KR_E_INVALID;
   *prof = e->prof;
+  return KR_OK;
+}
+
+int kr_last_pass(kr_engine *e, kr_pass_report *out) {
+  if (!e || !out) return KR_E_INVALID;
+  if (!e->has_pass) return fail(e, KR_E_STATE, "no pass has returned KR_OK on this engine");
+  *out = e->pass_last;
   return KR_OK;
 }
 

@@ -132,7 +132,7 @@ __global__ void __launch_bounds__(kHugeThreads) k_huge_merge(Decide2Args a, Huge
   if ((uint64_t)seg + total > a.n.n_pods) {  // cannot happen while the regions hold distinct live rows; void rather than overrun
     if (me == t.z && tid == 0) {
       sc.lg[c].w = 0;  // (the cluster's other CTAs return here too, whichever value they read)
-      if (kInc) sc.inc[KR_INC_VOID] = 1u; else KR_MARK_ATTEMPT_VOID(a.r.totals);
+      if (kInc) atomicOr(&sc.inc[KR_INC_VOID], KR_FULL_ARENA); else KR_MARK_ATTEMPT_VOID(a.r.totals);
     }
     return;
   }

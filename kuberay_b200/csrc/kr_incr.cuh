@@ -230,7 +230,7 @@ __global__ void __launch_bounds__(256) k_inc_objects(ObjDiffArgs a, SnapDev s, S
   if (!differ) return;
   const uint32_t epoch = inc_epoch(sc);
   switch (cls) {
-    case KR_OC_STRUCT: sc.inc[KR_INC_STRUCTURAL] = 1u; break;
+    case KR_OC_STRUCT: atomicOr(&sc.inc[KR_INC_STRUCTURAL], KR_FULL_STRUCTURAL); break;
     case KR_OC_CLUSTER: if (row < n.n_clusters) { sc.obj_flag[row] = epoch; mark_dirty(sc, row, epoch); } break;
     case KR_OC_GROUP: { const uint32_t c = a.g_cluster_idx_new[k_st]; if (c < n.n_clusters) { sc.obj_flag[c] = epoch; mark_dirty(sc, c, epoch); } break; }
     case KR_OC_HEADKEY:  // (the host compared the keys as well and rebuilds the pod -> row table); both pods' clusters see a different head-aux row now
@@ -395,7 +395,7 @@ __global__ void __launch_bounds__(256) k_inc_admit(SnapDev s, ScratchDev sc, Res
       // the usual event — a status update: the row stays in its RayCluster, its record is rewritten where it sits and the row's
       // stamp is lifted (nothing of this cluster has to be dropped on its account)
       uint2 *at = rec_slot(sc, c, sc.pos[p]);  // (a record of a large RayCluster may sit in its region)
-      if (!at) { sc.inc[KR_INC_VOID] = 1u; continue; }
+      if (!at) { sc.inc[KR_INC_VOID] = KR_FULL_OVERFLOW; continue; }
       *at = make_uint2(p, (slot << 16) | flags);
       sc.stamp[p] = 0u;
       continue;  // (k_inc_retire marked the cluster dirty)
@@ -409,8 +409,13 @@ __global__ void __launch_bounds__(256) k_inc_admit(SnapDev s, ScratchDev sc, Res
     const uint32_t rank = atomicAdd(&sc.cl_dyn[c].x, 1u);
     const uint2 rec = make_uint2(p, (slot << 16) | flags | KR_ROW_FRESH);
     if (uint2 *at = rec_slot(sc, c, rank)) { *at = rec; sc.pos[p] = rank; }
-    // (an ordinary RayCluster outgrew its bucket, a large one its region: k_inc_grow gives it a new one, or the full pass reclassifies)
-    else if (!grow || !grow_spill(sc.lg, sc.inc, sc.pos, sc.bucket_stride, grow, c, rank, rec)) sc.inc[KR_INC_VOID] = 1u;
+    // (an ordinary RayCluster outgrew its bucket, a large one its region: k_inc_grow gives it a new one, or the full pass reclassifies.
+    // Here and for a rewritten record without a slot above, a plain store of one constant keeps this kernel's registers (an atomicOr
+    // of a selected bit cost three).  It is right only because k_inc_admit is the first kernel of an attempt that writes
+    // KR_INC_VOID: a void site launched before it must not be added without making these stores atomicOr.  The host reads the
+    // constant as KR_FULL_GROW_LIMIT when the pass could grow, the rewritten-record case included, which cannot happen while every
+    // resident record has its slot.)
+    else if (!grow || !grow_spill(sc.lg, sc.inc, sc.pos, sc.bucket_stride, grow, c, rank, rec)) sc.inc[KR_INC_VOID] = KR_FULL_OVERFLOW;
   }
 }
 

@@ -101,7 +101,7 @@ __global__ void __launch_bounds__(256) k_inc_grow(SnapDev s, ScratchDev sc, uint
   }
   __syncthreads();
   if (!s_ok) {
-    if (blockIdx.x == 0 && tid == 0) sc.inc[KR_INC_VOID] = 1u;
+    if (blockIdx.x == 0 && tid == 0) atomicOr(&sc.inc[KR_INC_VOID], KR_FULL_GROW_LIMIT);
     return;
   }
   for (uint32_t i = blockIdx.x; i < n; i += gridDim.x)  // a regrown RayCluster's records of ranks [stride, stride + old capacity)
@@ -118,7 +118,7 @@ __global__ void __launch_bounds__(256) k_inc_grow(SnapDev s, ScratchDev sc, uint
     while (lo < hi) { const uint32_t mid = (lo + hi) >> 1; if (s_e[mid].x < at.z) lo = mid + 1; else hi = mid; }
     // (a record whose RayCluster is not on the list, or whose rank the new region does not hold, cannot be placed: void rather than
     // write into another region; the full pass that follows rebuilds every bucket and region)
-    if (s_e[lo].x != at.z || at.y < S + s_e[lo].z || at.y - S >= s_cap[lo]) { sc.inc[KR_INC_VOID] = 1u; continue; }
+    if (s_e[lo].x != at.z || at.y < S + s_e[lo].z || at.y - S >= s_cap[lo]) { atomicOr(&sc.inc[KR_INC_VOID], KR_FULL_GROW_LIMIT); continue; }
     const uint4 rec = __ldcg(&grow[kGrowSpill + 2 * k + 1]);
     sc.region[s_off[lo] + at.y - S] = make_uint2(rec.x, rec.y);
   }
@@ -217,7 +217,7 @@ __global__ void __launch_bounds__(kLargeSortThreads) k_large_sort(Decide2Args a,
   if (tid == 0) {
     s_seg = atomicAdd(&sc.inc[KR_INC_LSEG], total);
     if ((uint64_t)s_seg + total > a.n.n_pods) {  // cannot happen while the regions hold distinct live rows; void rather than overrun
-      if (kInc) sc.inc[KR_INC_VOID] = 1u; else KR_MARK_ATTEMPT_VOID(a.r.totals);
+      if (kInc) atomicOr(&sc.inc[KR_INC_VOID], KR_FULL_ARENA); else KR_MARK_ATTEMPT_VOID(a.r.totals);
     }
   }
   __syncthreads();  // (also orders every rows[] store of the CTA before the record rewrite below)
@@ -307,8 +307,8 @@ __global__ void __launch_bounds__(kThreads, 1) k_decide_large(Decide2Args a, con
         if (need) base = atomicAdd(reinterpret_cast<unsigned long long *>(&r.totals[8]), ((unsigned long long)((need & 2u) ? n_create : 0u) << 32) | ((need & 1u) ? n_act : 0u));
         act_off = (need & 1u) ? (uint32_t)base : r.act_start[c];
         create_off = (need & 2u) ? (uint32_t)(base >> 32) : old_create_off;
-        if ((need & 1u) && (uint64_t)act_off + n_act > a.n.n_pods) sc.inc[KR_INC_VOID] = 1u;             // the action list is full of abandoned runs:
-        if ((need & 2u) && (uint64_t)create_off + n_create > a.create_cap) sc.inc[KR_INC_VOID] = 1u;  // a full pass packs it again
+        if ((need & 1u) && (uint64_t)act_off + n_act > a.n.n_pods) atomicOr(&sc.inc[KR_INC_VOID], KR_FULL_ARENA);            // the action list is full of abandoned runs:
+        if ((need & 2u) && (uint64_t)create_off + n_create > a.create_cap) atomicOr(&sc.inc[KR_INC_VOID], KR_FULL_ARENA);  // a full pass packs it again
         if (need & 1u) sc.act_res[c] = n_act;
         if (need & 2u) sc.cre_res[c] = n_create;
         if (old_act) atomicSub(&r.totals[2], old_act);  // (the decide added this pass's n_act)

@@ -69,6 +69,7 @@ def lib() -> C.CDLL:
         L.kr_results_fetch.argtypes = [C.c_void_p, P(abi.kr_results_view)]
         L.kr_hash_batch.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p]
         L.kr_last_profile.argtypes = [C.c_void_p, P(abi.kr_profile)]
+        L.kr_last_pass.argtypes = [C.c_void_p, P(abi.kr_pass_report)]
         L.kr_group_results_device.argtypes = [C.c_void_p, P(C.c_void_p), P(C.c_uint64)]
         L.kr_group_results_copy.argtypes = [C.c_void_p, C.c_void_p, C.c_uint64]
         L.kr_last_error.argtypes = [C.c_void_p]
@@ -433,6 +434,16 @@ class Engine:
         prof = abi.kr_profile()
         self._check(self._L.kr_last_profile(self._h, C.byref(prof)))
         return self._profile_dict(prof, kernels=False)
+
+    def last_pass(self) -> dict:
+        """kr_last_pass: what the last pass that returned KR_OK was — kind ("incremental" / "full"), pipeline ("bucket" / "sort" /
+        "radix"), attempts, hash_wait, stride — and why it was not incremental: why_full (the KR_FULL_* bits) and why (their names)."""
+        rep = abi.kr_pass_report()
+        self._check(self._L.kr_last_pass(self._h, C.byref(rep)))
+        return {"kind": {abi.PASSK_INCREMENTAL: "incremental", abi.PASSK_FULL: "full"}.get(rep.kind, rep.kind),
+                "pipeline": {abi.PIPE_BUCKET: "bucket", abi.PIPE_SORT: "sort", abi.PIPE_RADIX: "radix"}.get(rep.pipeline, rep.pipeline),
+                "attempts": rep.attempts, "hash_wait": bool(rep.hash_wait), "stride": rep.stride,
+                "why_full": rep.why_full, "why": abi.full_names(rep.why_full)}
 
     @staticmethod
     def _profile_dict(prof: abi.kr_profile, kernels: bool) -> dict:

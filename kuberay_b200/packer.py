@@ -267,6 +267,10 @@ class Packer:
         self._check(self._L.kr_packer_sizes(self._h, C.byref(self.engine.sizes)))
         return mode.value
 
+    def last_pass(self) -> dict:
+        """Engine.last_pass of the packer's engine: the kind of the last pass and why it was not incremental."""
+        return self.engine.last_pass()
+
     def flags(self, **kw) -> abi.kr_flags:
         return abi.default_flags(id_head_not_found_reason=self._L.kr_packer_intern(self._h, _s(snp.HEAD_NOT_FOUND_REASON)),
                                  id_head_not_found_msg=self._L.kr_packer_intern(self._h, _s(snp.HEAD_NOT_FOUND_MSG)), **kw)
@@ -396,3 +400,7 @@ class GroupPacker:
         views = (abi.kr_results_view * self.n)()
         self._check(self._L.kr_group_packer_reconcile(self._h, fl, views))
         return [sh.engine._results(views[i], copy) for i, sh in enumerate(self.shards)]
+
+    def last_passes(self) -> list[dict]:
+        """Every shard's Engine.last_pass: each shard's engine reports its own pass."""
+        return [sh.last_pass() for sh in self.shards]

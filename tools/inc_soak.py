@@ -2,7 +2,9 @@
 """Randomised soak of the device-side incremental epochs (development aid; run on the GPU box): many epochs of mixed informer traffic —
 status flips, deletions, additions into free rows and past the end of the arena, pods moving between RayClusters and namespaces, head
 pods coming and going, RayCluster / group / head-aux row edits through BOTH object-commit entry points, JSON re-commits — each epoch
-compared with a from-scratch oracle run.  usage: python tools/inc_soak.py [seeds] [epochs]"""
+compared with a from-scratch oracle run; at the end, how many passes were incremental and full and how often each KR_FULL_* cause
+sent a pass to the full pass (kr_last_pass).  usage: python tools/inc_soak.py [seeds] [epochs]"""
+import collections
 import os
 import sys
 
@@ -41,6 +43,9 @@ def grow(snap, extra_pods, drop_head=None, add_head_for=None):
             a = a.reshape(-1)
         out.cols[name][:] = a
     return out
+
+
+KINDS, CAUSES = collections.Counter(), collections.Counter()
 
 
 def run(seed, epochs):
@@ -162,6 +167,10 @@ def run(seed, epochs):
             got = eng.fetch()
         else:
             got = eng.reconcile(flags)
+        rep = eng.last_pass()
+        KINDS[rep["kind"]] += 1
+        CAUSES.update(rep["why"])
+        assert (rep["kind"] == "incremental") == (got.changed_clusters is not None or got.n_changed < snap.dims["clusters"]), (seed, epoch, rep)
         want = oracle.run(snap, flags, threads=8)
         d = want.diff(got)
         assert not d, (seed, epoch, d[:5], got.n_changed)
@@ -182,3 +191,4 @@ if __name__ == "__main__":
         tot[0] += a; tot[1] += b
         print(f"seed {s}: {a} incremental + {b} full epochs, all equal to the oracle", flush=True)
     print(f"soak ok: {tot[0]} incremental epochs, {tot[1]} full passes", flush=True)
+    print(f"passes: {dict(KINDS)}; full-pass causes (KR_FULL_*, a pass may have several): {dict(CAUSES.most_common())}", flush=True)
