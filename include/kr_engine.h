@@ -567,8 +567,10 @@ enum {
   KR_FULL_OVERFLOW   = 1u << 12,  /* a RayCluster outgrew its bucket or region and no growth option gave it room (device) */
   KR_FULL_GROW_LIMIT = 1u << 13,  /* KR_OPT_LARGE_GROWTH / _HUGE_GROWTH refused a growth: grow list, spill, list cap, region arena,
                                      tile reserve or capacity, or past KR_LARGE_MAX_PODS without KR_OPT_HUGE_GROWTH (device) */
-  KR_FULL_ARENA      = 1u << 14   /* a cursor of the pass's arenas (action list, create arena, per-cluster sort scratch) ran past its
+  KR_FULL_ARENA      = 1u << 14,  /* a cursor of the pass's arenas (action list, create arena, per-cluster sort scratch) ran past its
                                      end (device) */
+  KR_FULL_EPOCH_WRAP = 1u << 15   /* the device's 32-bit epoch counter neared its wrap: stamps, dirty flags and counters were zeroed
+                                     again (once per 2^32 - 8 epochs) */
 };
 typedef struct kr_pass_report {       /* 16 bytes */
   uint8_t  kind;        /* KR_PASSK_INCREMENTAL or KR_PASSK_FULL */

@@ -301,6 +301,7 @@ var FullCauses = []struct {
 	{C.KR_FULL_POD_LISTS, "pod_lists"}, {C.KR_FULL_LARGE, "large"}, {C.KR_FULL_WIDE, "wide"}, {C.KR_FULL_OPTION, "option"},
 	{C.KR_FULL_COLUMNS, "columns"}, {C.KR_FULL_SIZES, "sizes"}, {C.KR_FULL_STRUCTURAL, "structural"}, {C.KR_FULL_ROW_MAP, "row_map"},
 	{C.KR_FULL_OVERFLOW, "overflow"}, {C.KR_FULL_GROW_LIMIT, "grow_limit"}, {C.KR_FULL_ARENA, "arena"},
+	{C.KR_FULL_EPOCH_WRAP, "epoch_wrap"},
 }
 
 // LastPass reports the last pass that returned KR_OK (one struct copy, no device work).

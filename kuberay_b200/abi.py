@@ -310,7 +310,7 @@ PIPE_BUCKET, PIPE_SORT, PIPE_RADIX = 1, 2, 3
 FULL_BITS = {  # name -> KR_FULL_* bit, in bit order
     "FIRST": 1 << 0, "CAPACITY": 1 << 1, "DISABLED": 1 << 2, "FLAGS": 1 << 3, "POD_LISTS": 1 << 4, "LARGE": 1 << 5, "WIDE": 1 << 6,
     "OPTION": 1 << 7, "COLUMNS": 1 << 8, "SIZES": 1 << 9, "STRUCTURAL": 1 << 10, "ROW_MAP": 1 << 11, "OVERFLOW": 1 << 12,
-    "GROW_LIMIT": 1 << 13, "ARENA": 1 << 14,
+    "GROW_LIMIT": 1 << 13, "ARENA": 1 << 14, "EPOCH_WRAP": 1 << 15,
 }
 globals().update({"FULL_" + k: v for k, v in FULL_BITS.items()})
 

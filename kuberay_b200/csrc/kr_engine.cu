@@ -42,6 +42,15 @@ constexpr uint32_t kAdoptMax = 4096;
 // most RayClusters one incremental epoch that renumbers them (KR_OPT_CLUSTER_DELETES) or regroups them (KR_OPT_GROUP_EDITS) deletes,
 // moves, creates and regroups together; more take the full pass
 constexpr uint32_t kMapMax = 4096;
+
+// Attempts of one full pass: bucket pipeline -> wider stride -> sort pipeline -> radix pipeline, or a rerun on the two-phase hash
+// schedule.  Each closes an epoch of the device counter (k_build_tables), and a void incremental attempt before them one more
+// (k_inc_finish).  A counter past 2^32 - 1 - kEpochMargin before a pass is zeroed again, so none reaches 2^32 - 1: no epoch stamps
+// with 0, the value of the zeroed stamps and of "not this epoch", and no stamp written since the zeroing comes round again.
+constexpr int kFullAttempts = 5;
+constexpr uint32_t kEpochMargin = 8;
+static_assert(kEpochMargin > kFullAttempts + 1, "one pass may close kFullAttempts + 1 epochs");
+
 enum MapList { MP_GONE, MP_INIT, MP_DIGESTS, MP_GSRC, MP_WSRC, MP_SGONE, MP_LARGE, MP_LISTS };  // the lists of a row map on the device, in this order
 inline size_t align_up(size_t x, size_t a = kAlign) { return (x + a - 1) / a * a; }
 inline uint32_t pow2_at_least(uint64_t x) { uint32_t p = 16; while (p < x) p <<= 1; return p; }
@@ -636,6 +645,8 @@ struct kr_engine {
   bool no_incr = false;          // KR_NO_INCR=1: every pass is a full pass (tests)
   bool inc_valid = false;        // the resident buckets / tables / results describe the committed snapshot up to the commits since the last pass
   bool inc_zero_needed = true;   // the stamp / dirty-flag / counter region of this layout has not been zeroed yet
+  uint32_t dev_epoch = 0;        // the device's epoch counter (sc.inc[KR_INC_EPOCH]) as of the last pass
+  uint32_t epoch_seed = 0;       // KR_EPOCH_BASE: the counter's value after the engine's first zeroing (later zeroings start from 0)
   kr_flags inc_flags{};          // flags of the pass that left the resident state
   uint32_t inc_n_pods = 0, inc_n_heads = 0;  // rows resident at the last pass
   bool wtd_edits = false;        // KR_OPT_WTD_EDITS
@@ -1513,6 +1524,7 @@ int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile
   k_inc_finish<<<1, 32, 0, M>>>(sc);  // (the host does not wait for it: whatever comes next is ordered behind it on this stream)
   CK(cudaGetLastError());
   CK(cudaEventSynchronize(e->ev_inc));
+  e->dev_epoch = e->h_inc[KR_INC_EPOCH] + 1u;  // (k_inc_finish closes the epoch, void or not)
   commits_read(e);
   e->rec.heads_rebuild = false;  // (rebuilt here, or about to be rebuilt by the full pass)
   if (e->h_inc[KR_INC_VOID] || e->h_inc[KR_INC_STRUCTURAL]) {  // the caller takes the full pass
@@ -1587,7 +1599,12 @@ int run_pass(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile) {
   // (the list moves with a group count, an option or a new layout, when a full pass follows, and with the RayClusters an incremental
   // epoch created)
   if (e->lg_stale) if (int rc = upload_lg(e)) return rc;
-  if (e->inc_valid && !e->no_incr && memcmp(&e->inc_flags, &f, sizeof f) == 0) {
+  // The running epoch stamps with the counter + 1, and 0 means "not this epoch": before the counter can reach 2^32 - 1 the region is
+  // zeroed again and a full pass runs (kEpochMargin).
+  const bool wrap = e->dev_epoch > 0xFFFFFFFFu - kEpochMargin;
+  if (wrap) { e->why_full |= KR_FULL_EPOCH_WRAP; e->inc_zero_needed = true; e->epoch_seed = 0; }
+  const bool same_flags = memcmp(&e->inc_flags, &f, sizeof f) == 0;
+  if (e->inc_valid && !e->no_incr && same_flags && !wrap) {
     if (profile) CK(cudaEventRecord(e->ev_a, e->sm));
     bool ok = false;
     if (int rc = run_pass_inc(e, f, done, profile, &ok)) return rc;
@@ -1597,18 +1614,22 @@ int run_pass(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile) {
       return pass_done(e, done);
     }
     if (e->lg_stale) if (int rc = upload_lg(e)) return rc;  // (a void attempt that grew regions left them in the device table)
-  } else if (e->inc_valid && !e->no_incr) e->why_full |= KR_FULL_FLAGS;
+  } else if (e->inc_valid && !e->no_incr && !same_flags) e->why_full |= KR_FULL_FLAGS;
   e->inc_valid = false; e->ran_inc = false;
-  if (e->inc_zero_needed) {  // first pass on this layout: stamps, dirty flags and epoch counters start from zero
+  if (e->inc_zero_needed) {  // first pass on this layout, or the counter's wrap: stamps, dirty flags and epoch counters start from zero
     CK(cudaMemsetAsync(e->d_scratch + e->sl.inc_zero, 0, e->sl.inc_zero_end - e->sl.inc_zero, e->sm));
+    if (e->epoch_seed) CK(cudaMemcpyAsync(e->d_scratch + e->sl.inc + 4 * KR_INC_EPOCH, &e->epoch_seed, 4, cudaMemcpyHostToDevice, e->sm));
+    e->dev_epoch = e->epoch_seed;
+    e->epoch_seed = 0;
     e->inc_zero_needed = false;
   }
   if (e->rec.spec_order_stale && !f.skip_hash) if (int rc = refresh_order(e)) return rc;
   uint32_t voided = 0;
   bool hash_wait = false;
-  for (int attempt = 0; attempt < 5; attempt++) {
+  for (int attempt = 0; attempt < kFullAttempts; attempt++) {
     if (profile) CK(cudaEventRecord(e->ev_a, e->sm));
     if (int rc = profile ? launch_pass(e, f, true) : run_pass_once(e, f)) return rc;
+    if (e->sizes.n_clusters + e->sizes.n_groups + e->sizes.n_heads) e->dev_epoch++;  // (k_build_tables closed an epoch)
     if (done) CK(cudaEventRecord(done, e->sm));
     CK(cudaMemcpyAsync(e->h_totals, e->d_out + e->ol.totals, 48, cudaMemcpyDeviceToHost, e->sm));
     CK(cudaStreamSynchronize(e->sm));
@@ -2139,6 +2160,10 @@ int kr_engine_create(const kr_config *cfg, kr_engine **out) {
   if (const char *g = getenv("KR_NO_BUCKET")) e->no_bucket = (g[0] == '1');
   if (const char *g = getenv("KR_NO_INCR")) e->no_incr = (g[0] == '1');
   if (const char *g = getenv("KR_NO_HASH_SPIN")) e->hash_spin = !(g[0] == '1');
+  if (const char *g = getenv("KR_EPOCH_BASE")) {  // (tests: the device's and the host's stamp counters start near their wrap)
+    const uint32_t base = (uint32_t)strtoul(g, nullptr, 0);
+    if (base) e->epoch_seed = e->dev_epoch = e->row_epoch = e->spec_epoch = e->pull_epoch = base;
+  }
   if (cudaHostAlloc((void **)&e->h_inc, 64, cudaHostAllocDefault) != cudaSuccess) return bail(KR_E_CUDA);
   {  // buffers of the incremental path, sized for the capacities up front (a pinned allocation inside an epoch costs milliseconds)
     const InLayout capl = in_layout(cap);
