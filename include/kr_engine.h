@@ -717,7 +717,7 @@ enum {
                               tiles are retired and new ones appended).  Results are the same as with 0 (the default: every such
                               epoch is a full pass).  May be set at any time; read at each object commit.  No effect without
                               KR_OPT_LARGE_CLUSTERS and KR_OPT_FIXED_LAYOUT. */
-  KR_OPT_HUGE_GROWTH = 14     /* 1, together with KR_OPT_LARGE_CLUSTERS, KR_OPT_HUGE_CLUSTERS and KR_OPT_LARGE_GROWTH: a RayCluster that
+  KR_OPT_HUGE_GROWTH = 14,    /* 1, together with KR_OPT_LARGE_CLUSTERS, KR_OPT_HUGE_CLUSTERS and KR_OPT_LARGE_GROWTH: a RayCluster that
                               grows past KR_LARGE_MAX_PODS Pods in an incremental epoch (a large one that scales past it, an ordinary
                               one that jumps past it, or a huge one that outgrows its region) keeps the incremental epoch: the pass
                               gives it a region of the size a full pass would (1.25x its Pods rounded up to 32, less the stride),
@@ -732,6 +732,9 @@ enum {
                               pass.  No effect without the three other options.  Turning it on allocates the tile scratch with
                               KR_HUGE_GROW_TILES more tiles (64 KB of device memory each); an engine whose KR_OPT_HUGE_CLUSTERS had
                               allocated it reallocates it. */
+  KR_OPT_SM_COUNT = 15        /* read only (kr_engine_get_option): the SM count the engine sizes its SM-sized grids by: the device's
+                              multiprocessor count, or the lower KR_SM_COUNT=<n> of the environment at kr_engine_create (at most the
+                              device's count; a value that is not a positive number is ignored; a development switch, DESIGN §4.5) */
 };
 enum { KR_LARGE_MAX_PODS = 8192 };  /* largest RayCluster KR_OPT_LARGE_CLUSTERS keeps on the bucket pipeline */
 /* KR_OPT_LARGE_GROWTH: at most KR_GROW_MAX RayClusters get a region in one incremental epoch, and an epoch that puts RayClusters on
@@ -743,7 +746,7 @@ enum { KR_GROW_MAX = 64, KR_GROW_LIST_MIN = 64, KR_GROW_LIST_DIV = 64, KR_GROW_S
  * regrows (KR_LARGE_MAX_PODS arrival ranks each: 262 144 in all). */
 enum { KR_HUGE_GROW_TILES = 32 };
 int kr_engine_set_option(kr_engine *e, uint32_t option, uint64_t value);
-/* Current value of an option (KR_OPT_*), and the read-only KR_OPT_BUCKET_STRIDE. */
+/* Current value of an option (KR_OPT_*), and the read-only KR_OPT_BUCKET_STRIDE and KR_OPT_SM_COUNT. */
 int kr_engine_get_option(kr_engine *e, uint32_t option, uint64_t *value);
 
 /* Device pointer + byte size of the per-group delta records (kr_group_result[n_groups]) of the last pass:

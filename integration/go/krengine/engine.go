@@ -165,6 +165,9 @@ const (
 	// region, in an incremental epoch gets a new region and tiles in that epoch; only with KR_OPT_LARGE_CLUSTERS, KR_OPT_HUGE_CLUSTERS
 	// and KR_OPT_LARGE_GROWTH; recommended for fleets of very large autoscaled RayClusters; read at each incremental pass).
 	OptHugeGrowth = uint32(C.KR_OPT_HUGE_GROWTH)
+	// OptSMCount is KR_OPT_SM_COUNT (read only, with GetOption: the SM count the engine sizes its SM-sized grids by, the device's
+	// multiprocessor count or the lower KR_SM_COUNT of the environment at New).
+	OptSMCount = uint32(C.KR_OPT_SM_COUNT)
 )
 
 // SetOption: KR_OPT_FIXED_LAYOUT (before the first Begin), KR_OPT_INCREMENTAL, KR_OPT_LARGE_CLUSTERS (1: RayClusters of 257 to
@@ -188,6 +191,15 @@ func (e *Engine) SetOption(option uint32, value uint64) error {
 		return e.err(rc)
 	}
 	return nil
+}
+
+// GetOption reads an option's current value, or the read-only KR_OPT_SM_COUNT (kr_engine_get_option).
+func (e *Engine) GetOption(option uint32) (uint64, error) {
+	var v C.uint64_t
+	if rc := C.kr_engine_get_option(e.h, C.uint32_t(option), &v); rc != C.KR_OK {
+		return 0, e.err(rc)
+	}
+	return uint64(v), nil
 }
 
 // Begin hands out the pinned arenas for a snapshot of the given sizes.

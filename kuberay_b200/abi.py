@@ -94,6 +94,7 @@ OPT_GROUP_EDITS = 11
 OPT_LARGE_GROWTH = 12
 OPT_LARGE_MOVES = 13
 OPT_HUGE_GROWTH = 14
+OPT_SM_COUNT = 15
 HUGE_GROW_TILES = 32
 LARGE_MAX_PODS = 8192
 SPEC_JSON_UNMUTED = 1

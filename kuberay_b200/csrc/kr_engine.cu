@@ -580,7 +580,7 @@ struct kr_engine {
   kr_sizes map_sizes{};        // ... the live counts of that object commit
   size_t mp_at[MP_LISTS]{};     // offsets in mp of its lists (MapList)
   uint8_t *h_in_dev = nullptr;  // device-side address of h_in
-  int sm_count = 148;
+  int sm_count = 148;         // SMs the SM-sized grids are laid out for: the device's count, or fewer with KR_SM_COUNT
   // the whole pass (both streams) captured once per (layout, flags, n_recreate) and replayed
   cudaGraphExec_t gexec = nullptr;
   kr_flags gflags{};
@@ -2056,6 +2056,7 @@ int kr_engine_set_option(kr_engine *e, uint32_t option, uint64_t value) {
     return KR_OK;
   }
   if (option == KR_OPT_BUCKET_STRIDE) return fail(e, KR_E_INVALID, "KR_OPT_BUCKET_STRIDE can only be read");
+  if (option == KR_OPT_SM_COUNT) return fail(e, KR_E_INVALID, "KR_OPT_SM_COUNT can only be read");
   return fail(e, KR_E_INVALID, "unknown option %u", option);
 }
 
@@ -2076,6 +2077,7 @@ int kr_engine_get_option(kr_engine *e, uint32_t option, uint64_t *value) {
     case KR_OPT_LARGE_MOVES: *value = e->large_moves; return KR_OK;
     case KR_OPT_HUGE_GROWTH: *value = e->huge_growth; return KR_OK;
     case KR_OPT_BUCKET_STRIDE: *value = e->bstride; return KR_OK;
+    case KR_OPT_SM_COUNT: *value = (uint64_t)e->sm_count; return KR_OK;
     default: return fail(e, KR_E_INVALID, "unknown option %u", option);
   }
 }
@@ -2155,6 +2157,9 @@ int kr_engine_create(const kr_config *cfg, kr_engine **out) {
   if (const char *g = getenv("KR_NO_PDL")) e->use_pdl = !(g[0] == '1');
   if (const char *g = getenv("KR_HASH_CTAS")) e->hash_ctas_per_sm = atoi(g) > 0 ? atoi(g) : 2;
   if (const char *g = getenv("KR_PLACE_CTAS")) e->place_ctas = atoi(g) > 0 ? atoi(g) : 1;
+  // (tests: the grids of a part with fewer SMs; never more than the device has, so no persistent or spinning CTA waits for a slot;
+  // a value that is not a positive number is ignored, like the two knobs above)
+  if (const char *g = getenv("KR_SM_COUNT")) if (atoi(g) > 0) e->sm_count = std::min(e->sm_count, atoi(g));
   e->force_radix = e->env_radix;
   if (cudaHostAlloc((void **)&e->h_totals, 64, cudaHostAllocDefault) != cudaSuccess) return bail(KR_E_CUDA);
   if (const char *g = getenv("KR_NO_BUCKET")) e->no_bucket = (g[0] == '1');

@@ -354,7 +354,8 @@ class Engine:
         self._check(self._L.kr_engine_set_option(self._h, abi.OPT_HUGE_GROWTH, 1 if on else 0))
 
     def get_option(self, option: int) -> int:
-        """kr_engine_get_option: an option's current value, or the read-only OPT_BUCKET_STRIDE (0: the sort pipeline)."""
+        """kr_engine_get_option: an option's current value, or the read-only OPT_BUCKET_STRIDE (0: the sort pipeline) or OPT_SM_COUNT
+        (the SM count the SM-sized grids are laid out for: the device's, or a lower KR_SM_COUNT)."""
         v = C.c_uint64()
         self._check(self._L.kr_engine_get_option(self._h, option, C.byref(v)))
         return v.value
