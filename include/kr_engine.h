@@ -238,7 +238,10 @@ typedef struct kr_flags {
                                         sorted_action: 5 B/pod; cluster_result.pod_start) and kr_reconcile_batch / kr_results_fetch copy
                                         it back — verification and debugging; 0 => only the compact action list (act_*) is produced,
                                         which is all the shim consumes, and the pass takes the bucket pipeline (no per-cluster sort;
-                                        pod_start is then 0) */
+                                        pod_start is then 0).  Without KR_OPT_BUCKET_POD_LISTS, 1 also sends the pass to the sort
+                                        pipeline, a full pass that leaves nothing resident; with it, 1 only asks for the lists: the pass
+                                        takes the pipeline it takes with 0 and stays incremental, and the bucket pipeline builds the same
+                                        lists and pod_start from its resident state */
   uint8_t  reserved_[3];
   uint32_t id_head_not_found_reason; /* interned id of "HeadPodNotFound" */
   uint32_t id_head_not_found_msg;    /* interned id of "Head Pod not found" */
@@ -361,16 +364,19 @@ typedef struct kr_results_view {
   const char              *hash;       /* [32*n_clusters] base32hex(sha1(json)) (utils/util.go:628-640) */
   const kr_group_result   *groups;     /* [n_groups] */
   const int32_t           *wtd_pod_idx;/* [n_wtd]: pod (same namespace, same name) the Delete call resolves to, -1 = NotFound */
-  const uint32_t          *sorted_pod_idx; /* [n_pods]: pods bucketed by cluster, list order kept; orphans last.  NULL unless kr_flags.fetch_pod_lists */
+  const uint32_t          *sorted_pod_idx; /* [n_pods]: pods bucketed by cluster in row order, list order kept; orphans and free rows last (in row
+                                            order).  NULL unless kr_flags.fetch_pod_lists.  The same bytes on every pipeline */
   const uint8_t           *sorted_action;  /* [n_pods]: KR_ACT_* aligned with sorted_pod_idx.  NULL unless kr_flags.fetch_pod_lists */
   const int32_t           *create_idx; /* [n_create_total] replica indices (:869-881,1081-1094) */
   const kr_job_result     *jobs;       /* [n_jobs] */
   /* compact action list: every pod whose action != KEEP (orphans excluded), one contiguous run per cluster, List order inside
    * a run; cluster c owns entries [act_start[c], act_start[c] + act_cnt[c]).  This is all the Go shim needs to issue the Delete
-   * calls.  The ORDER of the runs inside the list is unspecified when kr_flags.fetch_pod_lists == 0 (each RayCluster reserves
-   * its run with one atomic; a RayCluster whose Recreate gate was still waiting for the digest reserves its whole bucket and
-   * may use less), and is cluster order with act_start[c + 1] == act_start[c] + act_cnt[c] when it is 1.  The same holds for
-   * create_idx: group g owns [create_off, create_off + n_create).  act_start[n_clusters] is only meaningful in the second case. */
+   * calls.  The ORDER of the runs inside the list is unspecified on the bucket pipeline (each RayCluster reserves its run with one
+   * atomic; a RayCluster whose Recreate gate was still waiting for the digest reserves its whole bucket and may use less), which
+   * every pass with kr_flags.fetch_pod_lists == 0 may take, and so may one with 1 under KR_OPT_BUCKET_POD_LISTS; it is cluster
+   * order with act_start[c + 1] == act_start[c] + act_cnt[c] on the sort and radix pipelines (kr_last_pass tells which one the pass
+   * took), where fetch_pod_lists == 1 without that option always sends the pass.  The same holds for create_idx: group g owns
+   * [create_off, create_off + n_create).  act_start[n_clusters] is only meaningful in the second case. */
   const uint32_t          *act_start;  /* [n_clusters + 1] */
   const uint32_t          *act_cnt;    /* [n_clusters] */
   const uint32_t          *act_pod_idx;/* [act_extent] */
@@ -391,7 +397,7 @@ typedef struct kr_results_view {
    * takes the full pass (with KR_OPT_LARGE_GROWTH, a RayCluster that outgrows its bucket or region gets a new region in the
    * incremental pass instead).  Snapshots with multi-host worker groups (numOfHosts > 1) keep incremental epochs, and so does an edit of
    * numOfHosts; so does an edit of a workersToDelete list with KR_OPT_WTD_EDITS (a length change only under KR_OPT_FIXED_LAYOUT).  Every pass is a full one on the sort pipeline — no resident state — while the caller fetches the full pod lists
-   * (fetch_pod_lists = 1), while some RayCluster lists more than 256 pods (more than KR_LARGE_MAX_PODS with KR_OPT_LARGE_CLUSTERS,
+   * (fetch_pod_lists = 1) without KR_OPT_BUCKET_POD_LISTS, while some RayCluster lists more than 256 pods (more than KR_LARGE_MAX_PODS with KR_OPT_LARGE_CLUSTERS,
    * unless KR_OPT_HUGE_CLUSTERS) or has more than 32 worker groups (unless KR_OPT_WIDE_CLUSTERS is set), or when KR_NO_INCR=1 is set in the environment. */
   uint32_t n_changed;
   const uint32_t          *changed_clusters; /* [n_changed] cluster rows, unordered */
@@ -548,7 +554,8 @@ enum {
   KR_FULL_CAPACITY   = 1u << 1,   /* the previous full pass overran kr_config.max_creates (KR_E_CAPACITY) */
   KR_FULL_DISABLED   = 1u << 2,   /* KR_OPT_INCREMENTAL = 0, or KR_NO_INCR=1 / KR_NO_BUCKET=1 / KR_FORCE_RADIX=1 in the environment */
   KR_FULL_FLAGS      = 1u << 3,   /* kr_flags differ from the resident pass's */
-  KR_FULL_POD_LISTS  = 1u << 4,   /* the previous pass fetched the full pod lists (fetch_pod_lists = 1: sort pipeline, nothing resident) */
+  KR_FULL_POD_LISTS  = 1u << 4,   /* the previous pass fetched the full pod lists (fetch_pod_lists = 1 without KR_OPT_BUCKET_POD_LISTS:
+                                     sort pipeline, nothing resident) */
   KR_FULL_LARGE      = 1u << 5,   /* the previous pass left the bucket pipeline: a RayCluster had more Pods than the stride and the
                                      options in force hold (more than 256 without KR_OPT_LARGE_CLUSTERS, more than KR_LARGE_MAX_PODS
                                      without KR_OPT_HUGE_CLUSTERS, or regions past their arena) */
@@ -732,9 +739,21 @@ enum {
                               pass.  No effect without the three other options.  Turning it on allocates the tile scratch with
                               KR_HUGE_GROW_TILES more tiles (64 KB of device memory each); an engine whose KR_OPT_HUGE_CLUSTERS had
                               allocated it reallocates it. */
-  KR_OPT_SM_COUNT = 15        /* read only (kr_engine_get_option): the SM count the engine sizes its SM-sized grids by: the device's
+  KR_OPT_SM_COUNT = 15,       /* read only (kr_engine_get_option): the SM count the engine sizes its SM-sized grids by: the device's
                               multiprocessor count, or the lower KR_SM_COUNT=<n> of the environment at kr_engine_create (at most the
                               device's count; a value that is not a positive number is ignored; a development switch, DESIGN §4.5) */
+  KR_OPT_BUCKET_POD_LISTS = 16 /* 1: kr_flags.fetch_pod_lists = 1 is a request for output only.  The pass takes the pipeline the same
+                              snapshot takes with 0 (a snapshot that leaves the bucket pipeline for its own reasons still gets its lists
+                              from the sort or radix pipeline), and turning the flag on or off between epochs keeps them incremental.
+                              On the bucket pipeline, after a full pass and after an incremental one, sorted_pod_idx, sorted_action and
+                              every cluster_result.pod_start are byte for byte the sort pipeline's: RayClusters in row order, Pods in List
+                              order inside each, then the orphans and free rows.  They are built from the resident buckets behind the
+                              pass's last decide kernel, and the fetch copies them plus 4 B per
+                              RayCluster for the starts, which it writes into every host cluster record (changed_clusters still names
+                              only the re-decided ones).  The action-list runs keep the bucket pipeline's contract: their order is
+                              unspecified (kr_results_view).  Off (the default): a pass with fetch_pod_lists = 1 is a full pass on the
+                              sort pipeline and the next pass is full too (KR_FULL_POD_LISTS).  May be set at any time; read at each
+                              pass.  Needs no other option and no fixed layout. */
 };
 enum { KR_LARGE_MAX_PODS = 8192 };  /* largest RayCluster KR_OPT_LARGE_CLUSTERS keeps on the bucket pipeline */
 /* KR_OPT_LARGE_GROWTH: at most KR_GROW_MAX RayClusters get a region in one incremental epoch, and an epoch that puts RayClusters on

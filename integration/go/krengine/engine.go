@@ -165,6 +165,10 @@ const (
 	// region, in an incremental epoch gets a new region and tiles in that epoch; only with KR_OPT_LARGE_CLUSTERS, KR_OPT_HUGE_CLUSTERS
 	// and KR_OPT_LARGE_GROWTH; recommended for fleets of very large autoscaled RayClusters; read at each incremental pass).
 	OptHugeGrowth = uint32(C.KR_OPT_HUGE_GROWTH)
+	// OptBucketPodLists is KR_OPT_BUCKET_POD_LISTS (1: FetchPodLists only asks for the full pod lists; the pass keeps its pipeline
+	// and its incremental epoch, and the bucket pipeline builds the same lists and pod_start as the sort pipeline; for debug
+	// endpoints and per-Pod logs on production fleets; read at each pass).
+	OptBucketPodLists = uint32(C.KR_OPT_BUCKET_POD_LISTS)
 	// OptSMCount is KR_OPT_SM_COUNT (read only, with GetOption: the SM count the engine sizes its SM-sized grids by, the device's
 	// multiprocessor count or the lower KR_SM_COUNT of the environment at New).
 	OptSMCount = uint32(C.KR_OPT_SM_COUNT)
@@ -184,7 +188,8 @@ const (
 // a RayCluster that outgrows its bucket or region keeps incremental epochs; read at each incremental pass), KR_OPT_LARGE_MOVES (1, with
 // KR_OPT_LARGE_CLUSTERS and KR_OPT_FIXED_LAYOUT: a large RayCluster deleted, moved or regrouped keeps incremental epochs; read at
 // each object commit), KR_OPT_HUGE_GROWTH (1, with KR_OPT_LARGE_CLUSTERS, KR_OPT_HUGE_CLUSTERS and KR_OPT_LARGE_GROWTH: a RayCluster
-// that grows past KR_LARGE_MAX_PODS Pods keeps incremental epochs; read at each incremental pass).  For a Packer, call it on
+// that grows past KR_LARGE_MAX_PODS Pods keeps incremental epochs; read at each incremental pass), KR_OPT_BUCKET_POD_LISTS (1:
+// fetching the full pod lists keeps the pass's pipeline and its incremental epoch; read at each pass).  For a Packer, call it on
 // Packer.Engine().
 func (e *Engine) SetOption(option uint32, value uint64) error {
 	if rc := C.kr_engine_set_option(e.h, C.uint32_t(option), C.uint64_t(value)); rc != C.KR_OK {

@@ -95,6 +95,7 @@ OPT_LARGE_GROWTH = 12
 OPT_LARGE_MOVES = 13
 OPT_HUGE_GROWTH = 14
 OPT_SM_COUNT = 15
+OPT_BUCKET_POD_LISTS = 16
 HUGE_GROW_TILES = 32
 LARGE_MAX_PODS = 8192
 SPEC_JSON_UNMUTED = 1

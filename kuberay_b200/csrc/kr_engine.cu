@@ -27,6 +27,7 @@
 #include "kr_incr.cuh"
 #include "kr_large.cuh"
 #include "kr_huge.cuh"
+#include "kr_lists.cuh"
 
 using namespace kr;
 
@@ -420,7 +421,7 @@ InLayout in_layout(const kr_sizes &n) {
 }
 
 struct OutLayout {  // results arena: [small fixed part | full pod lists | variable-length lists]
-  size_t totals, clusters, hash, groups, wtd, jobs, act_start, act_cnt, small_total, sorted_idx, sorted_act, act_idx, act_code, create, total;
+  size_t totals, clusters, hash, groups, wtd, jobs, act_start, act_cnt, small_total, sorted_idx, sorted_act, act_idx, act_code, create, pod_start, total;
 };
 OutLayout out_layout(const kr_sizes &n, uint32_t create_cap) {
   OutLayout L;
@@ -439,6 +440,7 @@ OutLayout out_layout(const kr_sizes &n, uint32_t create_cap) {
   L.act_idx = o; o = align_up(o + 4 * (size_t)n.n_pods);
   L.act_code = o; o = align_up(o + (size_t)n.n_pods);
   L.create = o; o = align_up(o + 4 * (size_t)create_cap);
+  L.pod_start = o; o = align_up(o + 4 * ((size_t)n.n_clusters + 1));  // the bucket pipeline's list starts (kr_lists.cuh)
   L.total = o;
   return L;
 }
@@ -634,6 +636,8 @@ struct kr_engine {
   uint4 *d_grow = nullptr; uint4 *h_grow = nullptr;
   size_t lg_cursor = 0;
   bool ran_bucket = false;
+  bool bucket_lists = false;    // KR_OPT_BUCKET_POD_LISTS: fetch_pod_lists asks the bucket pipeline for the lists (kr_lists.cuh)
+  bool host_starts = false;     // ... and the host's cluster records hold the list starts the last fetch patched in
   uint64_t h2d_accum = 0;       // bytes uploaded by the commits since the last pass (kr_profile.h2d_bytes)
   // hash order: message ids by descending SHA-1 block count, rebuilt at every commit from c_json_len
   uint32_t *h_order = nullptr, *d_order = nullptr;
@@ -1041,6 +1045,34 @@ void launch_large_decide(PassCtx &c, const Decide2Args &da, const uint4 *grown =
   }
 }
 
+// Every RayCluster's full pod list from the bucket pipeline's resident state (kr_lists.cuh), behind the pass's last decide kernel on
+// stream M: owners, the radix pipeline's stable sort by owner, then the actions along the list and the starts.
+void launch_lists(PassCtx &c, bool inc) {
+  const kr_engine *e = c.e;
+  const ScratchDev &sc = c.sc;
+  const uint32_t Np = c.z.n_pods, Nc = c.z.n_clusters;
+  const ListsArgs la{c.s, sc, c.r, c.z, sc.keys[0], sc.act_tmp_code, reinterpret_cast<uint32_t *>(e->d_out + e->ol.pod_start), inc ? 1 : 0};
+  int cur = 0;
+  if (Np) {
+    c.mark("k_lists_init");
+    k_lists_init<<<(Np + 255) / 256, 256, 0, c.M>>>(la);
+    if (Nc) { c.mark("k_lists_owner"); k_lists_owner<<<(Nc + 7) / 8, 256, 0, c.M>>>(la); }  // (a warp per RayCluster)
+    uint32_t bits = 1;
+    while ((1ull << bits) <= Nc) bits++;  // keys are in [0, n_clusters]
+    const uint32_t nt = (Np + kSortTile - 1) / kSortTile;  // (the live rows: at most the layout's tiles)
+    for (uint32_t shift = 0; shift < bits; shift += kRadixBits) {
+      c.mark("k_hist"); k_hist<<<nt, kSortThreads, 0, c.M>>>(sc.keys[cur], sc.hist, Np, (int)shift);
+      c.mark("k_scan_rows"); k_scan_rows<<<kRadix, kRowScanThreads, 0, c.M>>>(sc.hist, sc.row_total, nt);
+      c.mark("k_scatter");
+      uint32_t *vout = shift + kRadixBits >= bits ? c.r.sorted_pod_idx : sc.vals[cur ^ 1];
+      k_scatter<<<nt, kSortThreads, 0, c.M>>>(sc.keys[cur], sc.vals[cur], sc.keys[cur ^ 1], vout, sc.hist, sc.row_total, Np, (int)shift, shift == 0);
+      cur ^= 1;
+    }
+  }
+  c.mark("k_lists_gather");
+  k_lists_gather<<<Np / 256 + 1, 256, 0, c.M>>>(la, sc.keys[cur]);  // (a thread per list position and one past the end)
+}
+
 // Launches the whole pass.  profile: serialise everything on stream M and bracket each kernel with events.
 int launch_pass(kr_engine *e, const kr_flags &f, bool profile, bool capturing = false) {
   PassCtx c(e, profile);
@@ -1053,9 +1085,10 @@ int launch_pass(kr_engine *e, const kr_flags &f, bool profile, bool capturing = 
   // the committed snapshot: columns gate stream M, the JSON arena gates the hash
   const unsigned wflag = capturing ? cudaEventWaitExternal : cudaEventWaitDefault;
   // (the fork comes first so the hash can start while the columns are still landing — an incremental pod-row epoch leaves the JSON untouched)
-  // bucket pipeline (kr_bucket2.cuh): the caller does not fetch the full pod lists, every RayCluster has few worker groups (or
-  // KR_OPT_WIDE_CLUSTERS lists the others for the per-cluster kernels) and (checked on the device) at most `bstride` pods
-  const bool bucket = !e->no_bucket && !f.fetch_pod_lists && e->bstride != 0 && !e->force_radix && (e->rec.snap_max_groups <= KR_SMEM_GROUPS || e->wide_on) &&
+  // bucket pipeline (kr_bucket2.cuh): the caller does not fetch the full pod lists (or KR_OPT_BUCKET_POD_LISTS builds them there),
+  // every RayCluster has few worker groups (or KR_OPT_WIDE_CLUSTERS lists the others for the per-cluster kernels) and (checked on the
+  // device) at most `bstride` pods
+  const bool bucket = !e->no_bucket && (!f.fetch_pod_lists || e->bucket_lists) && e->bstride != 0 && !e->force_radix && (e->rec.snap_max_groups <= KR_SMEM_GROUPS || e->wide_on) &&
                       (size_t)n.n_clusters * e->bstride <= e->sl.bucket_entries;
   // ... and there the clusters whose Recreate gate reads a digest wait for it inside the decide kernel (the hash runs beside it)
   const bool spin = bucket && !profile && do_hash && e->hash_spin && e->rec.n_recreate > 0;
@@ -1128,6 +1161,7 @@ int launch_pass(kr_engine *e, const kr_flags &f, bool profile, bool capturing = 
       c.mark("k_decide2_phase1");
       CK(launch_decide2(c, da, dim3((e->rec.n_recreate + kD2Warps - 1) / kD2Warps), false, false));
     }
+    if (f.fetch_pod_lists) launch_lists(c, false);  // (KR_OPT_BUCKET_POD_LISTS: behind the last decide)
   } else {
   const uint32_t ntiles = e->sl.ntiles;
   const bool fast = !e->force_radix;
@@ -1232,7 +1266,7 @@ int launch_pass(kr_engine *e, const kr_flags &f, bool profile, bool capturing = 
 // Replays the captured CUDA graph of the pass (captures it first when the layout / flags changed).
 int run_pass_once(kr_engine *e, const kr_flags &f) {
   if (!e->use_graph) return launch_pass(e, f, false);
-  kr_flags fk = f;  // (fetch_pod_lists selects the pipeline: part of the key)
+  kr_flags fk = f;  // (fetch_pod_lists selects the pipeline, or the list builder on the bucket pipeline: part of the key)
   if (!e->gvalid || memcmp(&e->gflags, &fk, sizeof fk) != 0) {
     e->gvalid = false;
     CK(cudaStreamBeginCapture(e->sm, cudaStreamCaptureModeThreadLocal));
@@ -1318,7 +1352,7 @@ uint32_t why_not_resident(const kr_engine *e, const kr_flags &f) {
   uint32_t why = 0;
   if (e->no_incr || e->no_bucket || e->env_radix) why |= KR_FULL_DISABLED;
   if (e->ran_bucket) return e->h_totals[9] > e->cfg.max_creates ? why | KR_FULL_CAPACITY : why;  // (totals[9]: the bucket pipeline's create extent)
-  if (f.fetch_pod_lists) why |= KR_FULL_POD_LISTS;
+  if (f.fetch_pod_lists && !e->bucket_lists) why |= KR_FULL_POD_LISTS;
   if (e->bstride == 0 || (e->force_radix && !e->env_radix) || (size_t)e->sizes.n_clusters * e->bstride > e->sl.bucket_entries) why |= KR_FULL_LARGE;
   if (e->rec.snap_max_groups > KR_SMEM_GROUPS && !e->wide_on) why |= KR_FULL_WIDE;
   return why;
@@ -1342,7 +1376,9 @@ void after_full_pass(kr_engine *e, const kr_flags &f) {
   // (a pass whose create runs overran kr_config.max_creates is reported as KR_E_CAPACITY and left groups' runs unwritten: an
   // incremental epoch would inherit that cursor and fail the same way, so the next pass starts over)
   e->inc_valid = e->ran_bucket && !e->no_incr && e->h_totals[9] <= e->cfg.max_creates;
-  e->inc_flags = f; e->inc_n_pods = e->sizes.n_pods; e->inc_n_heads = e->sizes.n_heads; e->inc_n_clusters = e->sizes.n_clusters;
+  // (without fetch_pod_lists: a pass that left the state resident took the bucket pipeline, so it did not fetch them or
+  // KR_OPT_BUCKET_POD_LISTS made them output only)
+  e->inc_flags = f; e->inc_flags.fetch_pod_lists = 0; e->inc_n_pods = e->sizes.n_pods; e->inc_n_heads = e->sizes.n_heads; e->inc_n_clusters = e->sizes.n_clusters;
   e->host_results_stale = false; e->inc_n_dirty = 0; e->fetched = false; e->ran_inc = false; e->rec.heads_rebuild = false;
   e->rec.wtd_rebuild = false; e->res_n_wtd = e->sizes.n_wtd; e->map_pending = false;
   if (!f.skip_hash) { e->rec.hash_dirty = false; clear_spec_rows(e); }
@@ -1515,6 +1551,7 @@ int run_pass_inc(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile
     }
   }
   if (n.n_jobs) { c.mark("k_jobs"); k_jobs<<<(n.n_jobs + 255) / 256, 256, 0, M>>>(s, sc, r, z); }
+  if (f.fetch_pod_lists) launch_lists(c, true);  // (only with KR_OPT_BUCKET_POD_LISTS: the flags of the resident pass leave it out)
   c.close();
   if (done) CK(cudaEventRecord(done, M));
   CK(cudaMemcpyAsync(e->h_totals, e->d_out + e->ol.totals, 48, cudaMemcpyDeviceToHost, M));
@@ -1603,7 +1640,9 @@ int run_pass(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile) {
   // zeroed again and a full pass runs (kEpochMargin).
   const bool wrap = e->dev_epoch > 0xFFFFFFFFu - kEpochMargin;
   if (wrap) { e->why_full |= KR_FULL_EPOCH_WRAP; e->inc_zero_needed = true; e->epoch_seed = 0; }
-  const bool same_flags = memcmp(&e->inc_flags, &f, sizeof f) == 0;
+  kr_flags fk = f;  // (KR_OPT_BUCKET_POD_LISTS: fetching the lists keeps the epoch incremental)
+  if (e->bucket_lists) fk.fetch_pod_lists = 0;
+  const bool same_flags = memcmp(&e->inc_flags, &fk, sizeof fk) == 0;
   if (e->inc_valid && !e->no_incr && same_flags && !wrap) {
     if (profile) CK(cudaEventRecord(e->ev_a, e->sm));
     bool ok = false;
@@ -1667,6 +1706,7 @@ int fetch_results(kr_engine *e, kr_results_view *out) {
   // bucket pipeline: the two arenas can hold reserved-but-unused places (totals[9] / totals[8] are their extents, [6] / [2] the counts)
   const uint32_t n_create = e->ran_bucket ? tot[9] : tot[0], n_actions = e->ran_bucket ? tot[8] : tot[2];
   const bool full = e->last_flags.fetch_pod_lists != 0;
+  const bool starts = full && e->ran_bucket;  // (KR_OPT_BUCKET_POD_LISTS: the lists' starts travel apart from the cluster records)
   CK(cudaEventRecord(e->ev_b, e->sm));
   if (n_create > e->cfg.max_creates) {
     CK(cudaEventRecord(e->ev_c, e->sm));
@@ -1716,6 +1756,10 @@ int fetch_results(kr_engine *e, kr_results_view *out) {
       bytes += 5 * (size_t)n.n_pods;
     }
   }
+  if (starts && n.n_clusters) {
+    CK(cudaMemcpyAsync(e->h_out + e->ol.pod_start, e->d_out + e->ol.pod_start, 4 * (size_t)n.n_clusters, cudaMemcpyDeviceToHost, e->sm));
+    bytes += 4ull * n.n_clusters;
+  }
   if (n_actions) {
     CK(cudaMemcpyAsync(e->h_out + e->ol.act_idx, e->d_out + e->ol.act_idx, 4 * (size_t)n_actions, cudaMemcpyDeviceToHost, e->sm));
     CK(cudaMemcpyAsync(e->h_out + e->ol.act_code, e->d_out + e->ol.act_code, (size_t)n_actions, cudaMemcpyDeviceToHost, e->sm));
@@ -1743,6 +1787,14 @@ int fetch_results(kr_engine *e, kr_results_view *out) {
     char *hh = reinterpret_cast<char *>(e->h_out + e->ol.hash);
     for (uint32_t i = 0; i < e->inc_spec_n; i++) memcpy(hh + 32 * (size_t)e->spec_hashed[i], e->inc_stage.h + st_dig + 32 * (size_t)i, 32);
   }
+  // The list starts into the host's cluster records, and out again on a fetch without the lists: the records a packed incremental
+  // fetch leaves alone still hold the starts of an earlier one (on the device they are 0, as the bucket pipeline leaves them).
+  if (starts || (packed && e->host_starts)) {
+    kr_cluster_result *hc = bind_out(e->ol, e->h_out).clusters;
+    const uint32_t *st = reinterpret_cast<const uint32_t *>(e->h_out + e->ol.pod_start);
+    for (uint32_t c = 0; c < n.n_clusters; c++) hc[c].pod_start = starts ? st[c] : 0u;
+  }
+  e->host_starts = starts;
   e->fetched = true; e->host_results_stale = false;
   if (out) {
     ResDev hr = bind_out(e->ol, e->h_out);
@@ -2000,6 +2052,11 @@ int kr_engine_set_option(kr_engine *e, uint32_t option, uint64_t value) {
     e->group_edits = value != 0;
     return KR_OK;
   }
+  if (option == KR_OPT_BUCKET_POD_LISTS) {  // (read at each pass; a fetching pass's captured graph follows it)
+    if (e->bucket_lists != (value != 0)) e->gvalid = false;
+    e->bucket_lists = value != 0;
+    return KR_OK;
+  }
   if (option == KR_OPT_LARGE_MOVES) {  // (read at each object commit)
     e->large_moves = value != 0;
     return KR_OK;
@@ -2076,6 +2133,7 @@ int kr_engine_get_option(kr_engine *e, uint32_t option, uint64_t *value) {
     case KR_OPT_LARGE_GROWTH: *value = e->large_growth; return KR_OK;
     case KR_OPT_LARGE_MOVES: *value = e->large_moves; return KR_OK;
     case KR_OPT_HUGE_GROWTH: *value = e->huge_growth; return KR_OK;
+    case KR_OPT_BUCKET_POD_LISTS: *value = e->bucket_lists; return KR_OK;
     case KR_OPT_BUCKET_STRIDE: *value = e->bstride; return KR_OK;
     case KR_OPT_SM_COUNT: *value = (uint64_t)e->sm_count; return KR_OK;
     default: return fail(e, KR_E_INVALID, "unknown option %u", option);

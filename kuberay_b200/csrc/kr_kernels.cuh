@@ -25,7 +25,10 @@
 //   k_huge_tiles / k_huge_merge     KR_OPT_HUGE_CLUSTERS only (kr_huge.cuh): the RayClusters of more than KR_LARGE_MAX_PODS pods —
 //                    List order by a shared-memory sort per 8 192-rank tile and a rank merge of the tiles, one CTA per tile,
 //                    beside the hash; then k_decide_huge (k_decide_large with 512 threads) decides them
-// When the caller asks for the full per-cluster pod lists (fetch_pod_lists == 1) or the snapshot does not qualify — the SORT pipeline:
+//   k_lists_init / k_lists_owner / (radix sort) / k_lists_gather   KR_OPT_BUCKET_POD_LISTS with fetch_pod_lists == 1 only
+//                    (kr_lists.cuh): every RayCluster's full pod list in List order from the resident buckets, behind the last decide
+// When the caller asks for the full per-cluster pod lists (fetch_pod_lists == 1, without KR_OPT_BUCKET_POD_LISTS) or the snapshot does
+// not qualify — the SORT pipeline:
 //   k_match -> k_place_fused -> k_decide_small (+ k_decide on a side stream) -> [phase 1] -> k_creates_fused
 //   (buckets restored to List order by an in-register bitonic sort), and for RayClusters with > 1024 pods the RADIX pipeline
 //   (k_match<radix>, k_hist, k_scan_rows, k_scatter: stable LSD sort) with the unfused scan kernels.

@@ -237,7 +237,7 @@ class Engine:
                      large_clusters: bool = False, wide_clusters: bool = False, huge_clusters: bool = False,
                      wtd_edits: bool = False, spec_rows: bool = False, cluster_creates: bool = False,
                      cluster_deletes: bool = False, group_edits: bool = False, large_growth: bool = False,
-                     large_moves: bool = False, huge_growth: bool = False) -> "Engine":
+                     large_moves: bool = False, bucket_pod_lists: bool = False, huge_growth: bool = False) -> "Engine":
         d = snap.dims
         up = lambda x: int(x * slack) + 1  # noqa: E731
         if max_creates is None:
@@ -264,6 +264,8 @@ class Engine:
             eng.set_large_growth(True)
         if large_moves:
             eng.set_large_moves(True)
+        if bucket_pod_lists:
+            eng.set_bucket_pod_lists(True)
         if huge_growth:
             eng.set_huge_growth(True)
         return eng
@@ -352,6 +354,11 @@ class Engine:
         LARGE_MAX_PODS Pods in an incremental epoch (or a huge one that outgrows its region) gets a region and tiles in that epoch
         instead of making the pass a full one; read at each incremental pass."""
         self._check(self._L.kr_engine_set_option(self._h, abi.OPT_HUGE_GROWTH, 1 if on else 0))
+
+    def set_bucket_pod_lists(self, on: bool = True):
+        """KR_OPT_BUCKET_POD_LISTS: fetch_pod_lists only asks for the lists; the pass keeps its pipeline and its incremental epoch, and
+        the bucket pipeline builds the same sorted_pod_idx, sorted_action and pod_start as the sort pipeline; read at each pass."""
+        self._check(self._L.kr_engine_set_option(self._h, abi.OPT_BUCKET_POD_LISTS, 1 if on else 0))
 
     def get_option(self, option: int) -> int:
         """kr_engine_get_option: an option's current value, or the read-only OPT_BUCKET_STRIDE (0: the sort pipeline) or OPT_SM_COUNT

@@ -3,7 +3,8 @@
 status flips, deletions, additions into free rows and past the end of the arena, pods moving between RayClusters and namespaces, head
 pods coming and going, RayCluster / group / head-aux row edits through BOTH object-commit entry points, JSON re-commits — each epoch
 compared with a from-scratch oracle run; at the end, how many passes were incremental and full and how often each KR_FULL_* cause
-sent a pass to the full pass (kr_last_pass).  usage: python tools/inc_soak.py [seeds] [epochs]"""
+sent a pass to the full pass (kr_last_pass).  usage: python tools/inc_soak.py [seeds] [epochs] [--bucket-pod-lists]
+--bucket-pod-lists turns on KR_OPT_BUCKET_POD_LISTS and fetches the full pod lists every third epoch, compared with the oracle too."""
 import collections
 import os
 import sys
@@ -48,13 +49,13 @@ def grow(snap, extra_pods, drop_head=None, add_head_for=None):
 KINDS, CAUSES = collections.Counter(), collections.Counter()
 
 
-def run(seed, epochs):
+def run(seed, epochs, lists=False):
     rng = np.random.default_rng(seed)
     groups = int(rng.integers(1, 4))
     snap, flags = synthetic.generate(synthetic.config("C2", n_clusters=int(rng.integers(150, 500)), pods_per_cluster=int(rng.integers(8, 40)), groups=groups,
                                                       jobs=bool(rng.integers(2)), recreate_frac=0.08, wtd_group_frac=0.3, seed=1000 + seed))
     flags.fetch_pod_lists = 0
-    eng = Engine.for_snapshot(snap, slack=1.6, max_creates=snap.dims["groups"] * 64 + 4096)
+    eng = Engine.for_snapshot(snap, slack=1.6, max_creates=snap.dims["groups"] * 64 + 4096, bucket_pod_lists=lists)
     eng.set_fixed_layout(True)
     views = eng.begin(snap.sizes())
     eng.fill(views, snap)
@@ -162,6 +163,7 @@ def run(seed, epochs):
                 half = rows.size // 2
                 eng.commit_pod_rows(rows[:half]) if half else None
                 eng.commit_pod_rows(rows[half:])
+        flags.fetch_pod_lists = int(lists and epoch % 3 == 0)
         if rng.random() < 0.15:
             eng.reconcile_device_only(flags)
             got = eng.fetch()
@@ -183,11 +185,13 @@ def run(seed, epochs):
 
 
 if __name__ == "__main__":
-    seeds = int(sys.argv[1]) if len(sys.argv) > 1 else 6
-    epochs = int(sys.argv[2]) if len(sys.argv) > 2 else 60
+    lists = "--bucket-pod-lists" in sys.argv
+    args = [x for x in sys.argv[1:] if x != "--bucket-pod-lists"]
+    seeds = int(args[0]) if len(args) > 0 else 6
+    epochs = int(args[1]) if len(args) > 1 else 60
     tot = [0, 0]
     for s in range(seeds):
-        a, b = run(s, epochs)
+        a, b = run(s, epochs, lists)
         tot[0] += a; tot[1] += b
         print(f"seed {s}: {a} incremental + {b} full epochs, all equal to the oracle", flush=True)
     print(f"soak ok: {tot[0]} incremental epochs, {tot[1]} full passes", flush=True)

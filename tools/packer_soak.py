@@ -2,7 +2,7 @@
 """A longer run of the native packer's random informer-event streams than tests/test_packer.py affords (4 seeds x 10 epochs there): per seed a
 fuzz-generated object set, then epochs of mixed Pod / RayCluster / RayJob events — structural ones included — through kr_packer_*, every
 epoch compared with the oracle on an independently re-packed snapshot (tests/harness.py's Mirror / packer_check).  usage (GPU box):
-python tools/packer_soak.py [first_seed] [seeds] [epochs] [--all-options] [--json-bytes N] [--lean]
+python tools/packer_soak.py [first_seed] [seeds] [epochs] [--all-options] [--bucket-pod-lists] [--json-bytes N] [--lean]
 
 At the end it prints how many passes were incremental and full, and how often each KR_FULL_* cause sent a pass to the full pass
 (kr_last_pass) — counts over synthetic streams, the input for choosing the options' defaults.
@@ -11,7 +11,8 @@ creates and deletes, group edits, large growth) and adds spec edits with a bumpe
 (tests/test_gpu_packer_streams.py and tests/test_gpu_structural_streams.py run these options at suite length); --json-bytes sets
 kr_config.max_json_bytes, small enough (a few KiB above the fleet's muted specs) that the stream compacts the JSON arena as it goes;
 --lean keeps fetch_pod_lists at 0 (by default every third epoch fetches the full pod lists, which takes the full pass twice), so the
-histogram counts only what the events and options cause."""
+histogram counts only what the events and options cause; --bucket-pod-lists turns on KR_OPT_BUCKET_POD_LISTS instead, with which the
+fetching epochs keep the bucket pipeline and their incremental epochs."""
 import argparse
 import collections
 import copy
@@ -35,9 +36,12 @@ ap.add_argument("epochs", nargs="?", type=int, default=30)
 ap.add_argument("--all-options", action="store_true")
 ap.add_argument("--json-bytes", type=int, default=4 << 20)
 ap.add_argument("--lean", action="store_true")
+ap.add_argument("--bucket-pod-lists", action="store_true")
 a = ap.parse_args()
 opts = dict(large_clusters=True, wide_clusters=True, huge_clusters=True, wtd_edits=True, spec_rows=True, cluster_creates=True,
             cluster_deletes=True, group_edits=True, large_growth=True) if a.all_options else {}
+if a.bucket_pod_lists:
+    opts["bucket_pod_lists"] = True
 oracle.lib()
 total = inc = 0
 kinds, causes = collections.Counter(), collections.Counter()

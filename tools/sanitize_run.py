@@ -31,6 +31,23 @@ def one(snap, flags, label):
         eng.close()
 
 
+def pod_lists(snap, flags, label):
+    """KR_OPT_BUCKET_POD_LISTS (kr_lists.cuh): one fetching full pass and one fetching incremental pass on the bucket pipeline."""
+    flags.fetch_pod_lists = 1
+    eng = Engine.for_snapshot(snap, slack=1.2, bucket_pod_lists=True)
+    eng.set_fixed_layout(True)
+    try:
+        views = eng.load(snap)
+        eng.reconcile(flags)
+        rows = np.arange(0, snap.dims["pods"], 7, dtype=np.uint32)
+        views["p_packed"][rows] ^= np.uint32(1 << 5)
+        eng.commit_pod_values(rows, np.stack([views[c][rows].view(np.uint32) for c, _d, _m, dim in abi.COLUMNS if dim == "pods"], axis=1))
+        res = eng.reconcile(flags)
+        print(label, "ok:", eng.last_pass()["kind"], "pass,", res.sorted_pod_idx.size, "Pods listed", flush=True)
+    finally:
+        eng.close()
+
+
 def incremental(snap, flags, label, large=False, wide=False, huge=False):
     """Bucket pipeline + device-side incremental epochs (kr_incr.cuh): pod rows, object rows, a structural change, unfetched passes."""
     flags.fetch_pod_lists = 0
@@ -411,6 +428,8 @@ def main():
     wtd_edits(*synthetic.generate(synthetic.config("C2", n_clusters=300, pods_per_cluster=20, groups=2, autoscaling_frac=1.0, wtd_group_frac=0.3)),
               "workersToDelete edits")
     incremental(*synthetic.generate(synthetic.config("C2", n_clusters=300, pods_per_cluster=20, groups=2, jobs=True, wtd_group_frac=0.3)), "incremental epochs")
+    pod_lists(*synthetic.generate(synthetic.config("C2", n_clusters=300, pods_per_cluster=20, groups=2, wtd_group_frac=0.3, orphan_frac=0.02)),
+              "pod lists on the bucket pipeline")
     incremental(*synthetic.generate(synthetic.config("C2", n_clusters=300, pods_per_cluster=41, groups=2, wtd_group_frac=0.3, multihost_frac=0.5)),
                 "incremental epochs, multi-host groups")
     # large RayClusters in their own regions (KR_OPT_LARGE_CLUSTERS, kr_large.cuh): a full pass, then incremental epochs
