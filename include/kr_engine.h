@@ -496,6 +496,22 @@ int kr_snapshot_commit_object_rows(kr_engine *e, const uint32_t *cluster_rows, u
  * range past json_bytes (nothing is committed then). */
 int kr_snapshot_commit_spec_rows(kr_engine *e, const uint32_t *cluster_rows, uint32_t n);
 
+/* The muted-spec JSON of the RayClusters `cluster_rows` is unchanged, byte for byte, and now sits in the pinned arena at the range
+ * the host c_json_off gives (same c_json_len), as after a compaction of the arena.  The engine moves those bytes inside the device
+ * arena, from the range it last committed for each row to the new one, and sets the device c_json_off.  No spec byte crosses PCIe
+ * and no digest is recomputed: the next pass is incremental as if the ranges had not moved, and a later object commit
+ * (KR_PART_OBJECTS or kr_snapshot_commit_object_rows) sees no moved range on their account.  Call it BEFORE the epoch's spec-row and
+ * object commits.  Sources and destinations may overlap in any direction (the copy goes through a device scratch as large as
+ * max_json_bytes, allocated at the first call).  Only the listed destination ranges (padded to 16 bytes) and the listed rows'
+ * c_json_off / c_json_len change on the device.  A recorded RayCluster that is not listed but whose committed range a destination
+ * overlaps loses its device bytes: until a spec-row commit of it, a whole KR_PART_JSON, or an object commit after which the row is
+ * gone (a RayCluster moved by swap-remove keeps the mark while its range stays), every pass returns KR_E_STATE naming the first such
+ * row.  kr_profile.h2d_bytes counts 24 B per listed row (row, length, destination, source).  KR_E_STATE before a full commit of the
+ * layout; KR_E_INVALID for a row at or past the committed rows or n_clusters, a repeated row, a c_json_len that differs from the
+ * committed one, an offset that is not 16-byte aligned, a range past json_bytes, or two listed destinations whose padded ranges
+ * overlap (nothing is committed then); KR_E_CUDA when the scratch cannot be allocated. */
+int kr_snapshot_commit_json_moves(kr_engine *e, const uint32_t *cluster_rows, uint32_t n);
+
 /* Run the whole decision + status pass over the committed snapshot and copy the results back.
  * Replaces the decision halves of reconcilePods (raycluster_controller.go:619-935), reconcileMultiHostWorkerGroup
  * (:963-1125), shouldRecreatePodsForUpgrade (:1132-1171), shouldDeletePod (:1181-1231), calculateStatus (:1552-1719),
@@ -640,7 +656,7 @@ enum {
                               are committed as the whole object part. */
   KR_OPT_SPEC_ROWS = 8,       /* 1: the native packer (kr_packer_flush) commits re-emitted specs with kr_snapshot_commit_spec_rows and
                               reports KR_PACK_SPEC_ROWS instead of KR_PART_JSON (a flush that compacts the JSON arena still sends
-                              KR_PART_JSON).  The engine call itself needs no option.  Results are the same as with 0 (the default). */
+                              KR_PART_JSON, unless KR_OPT_JSON_MOVES).  The engine call itself needs no option.  Results are the same as with 0 (the default). */
   KR_OPT_CLUSTER_CREATES = 9, /* 1, together with KR_OPT_FIXED_LAYOUT: RayClusters appended after the last row (every existing
                               RayCluster keeps its row, its groups and its workersToDelete names, and the new groups and names come after
                               all the old ones), and RayJobs created or deleted, keep the incremental epoch: kr_snapshot_begin(new
@@ -673,7 +689,7 @@ enum {
                               Results are the same as with 0 (the default: every deletion makes the next pass a full one).  May be set
                               at any time; read at each kr_snapshot_begin and object commit.  No effect without KR_OPT_FIXED_LAYOUT.
                               The native packer's flush takes this path by itself when the engine has the option (the specs it placed
-                              travel as spec rows unless it compacted the JSON arena). */
+                              travel as spec rows unless it compacted the JSON arena without KR_OPT_JSON_MOVES). */
   KR_OPT_GROUP_EDITS = 11,    /* 1, together with KR_OPT_FIXED_LAYOUT: a RayCluster whose list of worker groups changed (groups appended,
                               as a RayService in-place update does, removed, renamed or reordered) keeps the incremental epoch:
                               kr_snapshot_begin(new counts; n_groups and n_wtd may move either way), then the object part
@@ -742,7 +758,7 @@ enum {
   KR_OPT_SM_COUNT = 15,       /* read only (kr_engine_get_option): the SM count the engine sizes its SM-sized grids by: the device's
                               multiprocessor count, or the lower KR_SM_COUNT=<n> of the environment at kr_engine_create (at most the
                               device's count; a value that is not a positive number is ignored; a development switch, DESIGN §4.5) */
-  KR_OPT_BUCKET_POD_LISTS = 16 /* 1: kr_flags.fetch_pod_lists = 1 is a request for output only.  The pass takes the pipeline the same
+  KR_OPT_BUCKET_POD_LISTS = 16, /* 1: kr_flags.fetch_pod_lists = 1 is a request for output only.  The pass takes the pipeline the same
                               snapshot takes with 0 (a snapshot that leaves the bucket pipeline for its own reasons still gets its lists
                               from the sort or radix pipeline), and turning the flag on or off between epochs keeps them incremental.
                               On the bucket pipeline, after a full pass and after an incremental one, sorted_pod_idx, sorted_action and
@@ -754,6 +770,14 @@ enum {
                               unspecified (kr_results_view).  Off (the default): a pass with fetch_pod_lists = 1 is a full pass on the
                               sort pipeline and the next pass is full too (KR_FULL_POD_LISTS).  May be set at any time; read at each
                               pass.  Needs no other option and no fixed layout. */
+  KR_OPT_JSON_MOVES = 17      /* 1, together with KR_OPT_SPEC_ROWS: a native-packer flush that compacted the JSON arena (dead bytes past
+                              half the cursor and 1 MiB at flush, or a full arena while placing a spec) commits the compaction with
+                              kr_snapshot_commit_json_moves instead of KR_PART_JSON: first the moves of every RayCluster the engine
+                              holds in the same row whose spec was not re-emitted and whose range changed, then the re-emitted and
+                              the created, moved or regrouped RayClusters' specs as spec rows, as a flush without compaction sends
+                              them.  It reports KR_PACK_JSON_MOVES, and the flush keeps every row path a flush without compaction
+                              takes.  Results are the same as with 0 (the default).  Read by kr_packer_flush only; no effect without
+                              KR_OPT_SPEC_ROWS or on the first flush.  The engine call itself needs no option. */
 };
 enum { KR_LARGE_MAX_PODS = 8192 };  /* largest RayCluster KR_OPT_LARGE_CLUSTERS keeps on the bucket pipeline */
 /* KR_OPT_LARGE_GROWTH: at most KR_GROW_MAX RayClusters get a region in one incremental epoch, and an epoch that puts RayClusters on
@@ -869,7 +893,7 @@ typedef struct kr_cluster_obj {
 } kr_cluster_obj;
 typedef struct kr_job_obj { kr_str ns, name, cluster_name, status_summary; } kr_job_obj;
 typedef struct kr_packer kr_packer;
-enum { KR_PACK_POD_ROWS = 8, KR_PACK_FULL = 16, KR_PACK_OBJECT_ROWS = 32, KR_PACK_SPEC_ROWS = 64 };  /* kr_packer_flush mode bits, beside KR_PART_OBJECTS / KR_PART_JSON (OBJECT_ROWS: kr_snapshot_commit_object_rows instead of the whole object part; SPEC_ROWS: kr_snapshot_commit_spec_rows instead of KR_PART_JSON, with KR_OPT_SPEC_ROWS) */
+enum { KR_PACK_POD_ROWS = 8, KR_PACK_FULL = 16, KR_PACK_OBJECT_ROWS = 32, KR_PACK_SPEC_ROWS = 64, KR_PACK_JSON_MOVES = 128 };  /* kr_packer_flush mode bits, beside KR_PART_OBJECTS / KR_PART_JSON (OBJECT_ROWS: kr_snapshot_commit_object_rows instead of the whole object part; SPEC_ROWS: kr_snapshot_commit_spec_rows instead of KR_PART_JSON, with KR_OPT_SPEC_ROWS; JSON_MOVES: kr_snapshot_commit_json_moves instead of KR_PART_JSON after a compaction, with KR_OPT_JSON_MOVES) */
 int        kr_packer_create(const kr_config *capacities, kr_packer **out);
 void       kr_packer_destroy(kr_packer *p);
 kr_engine *kr_packer_engine(kr_packer *p);

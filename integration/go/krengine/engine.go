@@ -169,6 +169,10 @@ const (
 	// and its incremental epoch, and the bucket pipeline builds the same lists and pod_start as the sort pipeline; for debug
 	// endpoints and per-Pod logs on production fleets; read at each pass).
 	OptBucketPodLists = uint32(C.KR_OPT_BUCKET_POD_LISTS)
+	// OptJsonMoves is KR_OPT_JSON_MOVES (1, with KR_OPT_SPEC_ROWS: Packer.Flush commits a compaction of its JSON arena with
+	// CommitJsonMoves instead of the whole arena and reports PackJsonMoves; recommended for RayJob fleets and spec rollouts, whose
+	// dead spec bytes make the packer compact often; read by Packer.Flush).
+	OptJsonMoves = uint32(C.KR_OPT_JSON_MOVES)
 	// OptSMCount is KR_OPT_SM_COUNT (read only, with GetOption: the SM count the engine sizes its SM-sized grids by, the device's
 	// multiprocessor count or the lower KR_SM_COUNT of the environment at New).
 	OptSMCount = uint32(C.KR_OPT_SM_COUNT)
@@ -189,8 +193,9 @@ const (
 // KR_OPT_LARGE_CLUSTERS and KR_OPT_FIXED_LAYOUT: a large RayCluster deleted, moved or regrouped keeps incremental epochs; read at
 // each object commit), KR_OPT_HUGE_GROWTH (1, with KR_OPT_LARGE_CLUSTERS, KR_OPT_HUGE_CLUSTERS and KR_OPT_LARGE_GROWTH: a RayCluster
 // that grows past KR_LARGE_MAX_PODS Pods keeps incremental epochs; read at each incremental pass), KR_OPT_BUCKET_POD_LISTS (1:
-// fetching the full pod lists keeps the pass's pipeline and its incremental epoch; read at each pass).  For a Packer, call it on
-// Packer.Engine().
+// fetching the full pod lists keeps the pass's pipeline and its incremental epoch; read at each pass), KR_OPT_JSON_MOVES (1, with
+// KR_OPT_SPEC_ROWS: Packer.Flush commits a compaction of its JSON arena with CommitJsonMoves and reports PackJsonMoves; read by
+// Packer.Flush).  For a Packer, call it on Packer.Engine().
 func (e *Engine) SetOption(option uint32, value uint64) error {
 	if rc := C.kr_engine_set_option(e.h, C.uint32_t(option), C.uint64_t(value)); rc != C.KR_OK {
 		return e.err(rc)
@@ -284,6 +289,20 @@ func (e *Engine) CommitSpecRows(clusterRows []uint32) error {
 		return nil
 	}
 	if rc := C.kr_snapshot_commit_spec_rows(e.h, (*C.uint32_t)(unsafe.Pointer(&clusterRows[0])), C.uint32_t(len(clusterRows))); rc != C.KR_OK {
+		return e.err(rc)
+	}
+	return nil
+}
+
+// CommitJsonMoves tells the engine that the unchanged muted-spec JSON of these RayClusters now sits at the ranges c_json_off gives
+// (same c_json_len), as after a compaction of the arena; the device moves its copies there, so no spec byte crosses PCIe and no
+// digest is recomputed.  Call it before CommitSpecRows and the object commit of the epoch.  clusterRows is ordinary Go memory
+// without pointers: C copies it before returning.
+func (e *Engine) CommitJsonMoves(clusterRows []uint32) error {
+	if len(clusterRows) == 0 {
+		return nil
+	}
+	if rc := C.kr_snapshot_commit_json_moves(e.h, (*C.uint32_t)(unsafe.Pointer(&clusterRows[0])), C.uint32_t(len(clusterRows))); rc != C.KR_OK {
 		return e.err(rc)
 	}
 	return nil

@@ -197,8 +197,12 @@ func (p *Packer) DeleteJob(ns, name string) error {
 // PackSpecRows is the Flush mode bit of a flush that committed re-emitted specs row by row (OptSpecRows) instead of KR_PART_JSON.
 const PackSpecRows = uint32(C.KR_PACK_SPEC_ROWS)
 
+// PackJsonMoves is the Flush mode bit of a flush that committed a compaction of its JSON arena as moves inside the device arena
+// (OptJsonMoves) instead of KR_PART_JSON.
+const PackJsonMoves = uint32(C.KR_PACK_JSON_MOVES)
+
 // Flush uploads what moved since the last flush; mode reports how (KR_PACK_FULL | KR_PACK_POD_ROWS | KR_PACK_OBJECT_ROWS |
-// KR_PACK_SPEC_ROWS | KR_PART_*).
+// KR_PACK_SPEC_ROWS | KR_PACK_JSON_MOVES | KR_PART_*).
 func (p *Packer) Flush() (mode uint32, err error) {
 	var m C.uint32_t
 	if rc := C.kr_packer_flush(p.h, &m); rc != C.KR_OK {

@@ -96,6 +96,7 @@ OPT_LARGE_MOVES = 13
 OPT_HUGE_GROWTH = 14
 OPT_SM_COUNT = 15
 OPT_BUCKET_POD_LISTS = 16
+OPT_JSON_MOVES = 17
 HUGE_GROW_TILES = 32
 LARGE_MAX_PODS = 8192
 SPEC_JSON_UNMUTED = 1
@@ -209,7 +210,7 @@ class kr_job_obj(C.Structure):
     _fields_ = [("ns", kr_str), ("name", kr_str), ("cluster_name", kr_str), ("status_summary", kr_str)]
 
 
-PACK_POD_ROWS, PACK_FULL, PACK_OBJECT_ROWS, PACK_SPEC_ROWS = 8, 16, 32, 64
+PACK_POD_ROWS, PACK_FULL, PACK_OBJECT_ROWS, PACK_SPEC_ROWS, PACK_JSON_MOVES = 8, 16, 32, 64, 128
 
 
 class kr_kv(C.Structure):
@@ -342,7 +343,7 @@ class kr_oracle_out(C.Structure):  # oracle/kr_oracle.h (test infrastructure; de
 
 # every symbol include/kr_engine.h declares
 ENGINE_SYMBOLS = [
-    "kr_device_count", "kr_engine_create", "kr_engine_destroy", "kr_snapshot_begin", "kr_snapshot_commit", "kr_snapshot_commit_parts", "kr_snapshot_commit_pod_rows", "kr_snapshot_commit_pod_values", "kr_snapshot_commit_object_rows", "kr_snapshot_commit_spec_rows", "kr_engine_set_option", "kr_engine_get_option",
+    "kr_device_count", "kr_engine_create", "kr_engine_destroy", "kr_snapshot_begin", "kr_snapshot_commit", "kr_snapshot_commit_parts", "kr_snapshot_commit_pod_rows", "kr_snapshot_commit_pod_values", "kr_snapshot_commit_object_rows", "kr_snapshot_commit_spec_rows", "kr_snapshot_commit_json_moves", "kr_engine_set_option", "kr_engine_get_option",
     "kr_reconcile_batch", "kr_reconcile_device_only", "kr_reconcile_batch_profiled", "kr_results_fetch",
     "kr_hash_batch", "kr_last_profile", "kr_last_pass", "kr_group_results_device", "kr_group_results_copy", "kr_last_error", "kr_algorithmic_bytes",
     "kr_spec_json_emit", "kr_spec_json_emit_arena", "kr_quantity_canonical", "kr_spec_json_last_error", "kr_hash_compare_batch",

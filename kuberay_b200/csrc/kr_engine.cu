@@ -142,9 +142,10 @@ uint8_t obj_class(int col, bool wtd_edits, bool appended = false) {
 }
 
 // The host's record of what the device's object columns, JSON ranges and hash order were last committed from, and of what the next
-// pass owes them.  Only its three update functions change it, each after its commit has checked the whole input and before the
+// pass owes them.  Only its four update functions change it, each after its commit has checked the whole input and before the
 // commit uploads anything: commit_whole (kr_snapshot_commit_parts, any parts), commit_rows (the row path of
-// kr_snapshot_commit_object_rows) and commit_spec_rows (kr_snapshot_commit_spec_rows).  The passes clear the four flags at the end.
+// kr_snapshot_commit_object_rows), commit_spec_rows (kr_snapshot_commit_spec_rows) and commit_json_moves
+// (kr_snapshot_commit_json_moves).  The passes clear the four flags at the end.
 struct CommitRecord {
   struct Row {
     uint64_t json_off;             // the JSON range the digests and the hash order were computed from: whole, spec rows
@@ -180,6 +181,9 @@ struct CommitRecord {
   // rows whose range a JSON-only whole commit recorded while the device's c_json_off / c_json_len kept the old one (sorted,
   // distinct): the row path takes them only all together; any object commit clears the list
   std::vector<uint32_t> json_cols_behind;
+  // rows whose device JSON bytes a move overwrote (sorted, distinct): no pass runs until each is re-committed (a spec row of it, or the
+  // whole JSON part) or an object commit leaves it gone.  Through a row map the mark goes with its RayCluster while the range stays.
+  std::vector<uint32_t> overwritten;
   uint32_t res_n_heads = 0;              // head-aux rows the resident device columns hold: whole with the object part
   uint32_t res_clusters = 0, res_groups = 0, res_wtd = 0;  // ... and RayCluster / group / workersToDelete rows: whole with the object part
   std::vector<uint32_t> prev_h_pod_idx;  // ... and their keys: whole with the object part, rows
@@ -315,6 +319,19 @@ struct CommitRecord {
     const size_t had = rows.size();
     const int mapped = (creates || deletes || regroups) && objects && had ? derive_map(hb, n, creates, deletes, regroups, resident, res_groups, res_wtd) : 0;
     bool ranges_moved = had != n.n_clusters && mapped != 1;  // some RayCluster's JSON range differs from the one the digests / the hash order were computed from
+    if (parts & KR_PART_JSON) overwritten.clear();
+    else if (objects && !overwritten.empty()) {
+      std::vector<uint32_t> kept;
+      for (uint32_t o : overwritten) {
+        const auto it = mapped == 1 ? std::lower_bound(map.gone.begin(), map.gone.end(), o) : map.gone.end();
+        if (it == map.gone.end() || *it != o) { if (o < n.n_clusters) kept.push_back(o); continue; }
+        const uint32_t c = map.moved_to[it - map.gone.begin()];
+        if (c != KR_EMPTY32 && rows[o].json_off == hb.c_json_off[c] && rows[o].json_len == hb.c_json_len[c]) kept.push_back(c);
+      }
+      std::sort(kept.begin(), kept.end());
+      kept.erase(std::unique(kept.begin(), kept.end()), kept.end());
+      overwritten.swap(kept);
+    }
     uint32_t n_rc = 0, n_mh_now = 0, max_groups = 0;
     std::vector<uint32_t> wide;
     rows.resize(n.n_clusters);
@@ -397,6 +414,37 @@ struct CommitRecord {
       if ((r.json_len + 8) / 64 != (len[i] + 8) / 64) spec_order_stale = true;
       r.json_off = off[i]; r.json_len = len[i];
     }
+    if (overwritten.empty()) return;
+    std::vector<uint32_t> pulled(cl, cl + m);
+    std::sort(pulled.begin(), pulled.end());
+    overwritten.erase(std::remove_if(overwritten.begin(), overwritten.end(), [&](uint32_t c) { return std::binary_search(pulled.begin(), pulled.end(), c); }),
+                      overwritten.end());
+  }
+  // the moved rows' new ranges (`to`: {destination, row} by destination, distinct recorded rows of unchanged lengths whose padded
+  // destinations are disjoint; `listed`: per recorded row, whether it is among them): their bytes moved on the device, so the digests
+  // and the hash order still hold and the device's range columns follow; every other recorded row whose range a destination
+  // overlaps has lost its bytes (`overwritten`).  -> the rows it newly marked.
+  std::vector<uint32_t> commit_json_moves(const std::vector<std::pair<uint64_t, uint32_t>> &to, const std::vector<uint8_t> &listed) {
+    std::vector<uint64_t> lo, hi;  // the padded destination ranges that hold bytes, ascending
+    for (const auto &t : to) {
+      Row &r = rows[t.second];
+      r.json_off = t.first;
+      if (r.json_len) { lo.push_back(t.first); hi.push_back(t.first + ((r.json_len + 15ull) & ~15ull)); }
+    }
+    json_cols_behind.erase(std::remove_if(json_cols_behind.begin(), json_cols_behind.end(), [&](uint32_t c) { return listed[c] != 0; }), json_cols_behind.end());
+    std::vector<uint32_t> hit;
+    for (uint32_t c = 0; c < rows.size() && !lo.empty(); c++) {
+      const Row &r = rows[c];
+      if (!r.json_len || listed[c]) continue;
+      const size_t k = std::lower_bound(lo.begin(), lo.end(), r.json_off + r.json_len) - lo.begin();  // (destinations starting before its end)
+      if (k && hi[k - 1] > r.json_off) hit.push_back(c);
+    }
+    if (!hit.empty()) {
+      std::vector<uint32_t> all;
+      std::set_union(overwritten.begin(), overwritten.end(), hit.begin(), hit.end(), std::back_inserter(all));
+      overwritten.swap(all);
+    }
+    return hit;
   }
 };
 
@@ -677,6 +725,11 @@ struct kr_engine {
   std::vector<uint32_t> pull_stamp;    // cluster row -> pull_epoch that pulled it: a pass in between lets the caller rewrite the arena,
   uint32_t pull_epoch = 1;             // so a row listed again after a pass (skip_hash leaves it pending) is pulled again
   bool spec_rows_opt = false;          // KR_OPT_SPEC_ROWS (read by kr_packer_flush)
+  bool json_moves_opt = false;         // KR_OPT_JSON_MOVES (read by kr_packer_flush)
+  // kr_snapshot_commit_json_moves, allocated at the first move commit: pinned mirror and device copy of {rows u32 | lens u32 | dst u64 |
+  // src u64}[max_clusters], and the out-of-place copy's scratch, as large as the JSON arena's capacity
+  Staging mv;
+  uint8_t *d_json_scratch = nullptr;
   uint32_t inc_spec_n = 0;             // rows the last incremental pass re-hashed ...
   bool inc_spec_gathered = false;      // ... and their digests sit packed in the staging buffer
   std::vector<uint32_t> spec_hashed;   // ... which rows (the fetch scatters the digests)
@@ -1623,6 +1676,8 @@ int pass_done(kr_engine *e, cudaEvent_t done) {
 // and ev_a recorded again before each attempt, so that kernels_ms covers the last one.
 int run_pass(kr_engine *e, const kr_flags &f, cudaEvent_t done, bool profile) {
   if (!e->committed) return fail(e, KR_E_STATE, "no committed snapshot");
+  if (!e->rec.overwritten.empty())  // (a pass would hash bytes a move overwrote)
+    return fail(e, KR_E_STATE, "cluster %u: a JSON move overwrote its spec bytes on the device; commit its spec row or the JSON part first", e->rec.overwritten.front());
   CK(cudaSetDevice(e->cfg.device));
   if (!profile) CK(cudaEventRecord(e->ev_a, e->sm));
   e->last_flags = f;
@@ -2040,6 +2095,10 @@ int kr_engine_set_option(kr_engine *e, uint32_t option, uint64_t value) {
     e->spec_rows_opt = value != 0;
     return KR_OK;
   }
+  if (option == KR_OPT_JSON_MOVES) {  // (read by kr_packer_flush only)
+    e->json_moves_opt = value != 0;
+    return KR_OK;
+  }
   if (option == KR_OPT_CLUSTER_CREATES) {  // (read at each kr_snapshot_begin and object commit)
     e->cluster_creates = value != 0;
     return KR_OK;
@@ -2134,6 +2193,7 @@ int kr_engine_get_option(kr_engine *e, uint32_t option, uint64_t *value) {
     case KR_OPT_LARGE_MOVES: *value = e->large_moves; return KR_OK;
     case KR_OPT_HUGE_GROWTH: *value = e->huge_growth; return KR_OK;
     case KR_OPT_BUCKET_POD_LISTS: *value = e->bucket_lists; return KR_OK;
+    case KR_OPT_JSON_MOVES: *value = e->json_moves_opt; return KR_OK;
     case KR_OPT_BUCKET_STRIDE: *value = e->bstride; return KR_OK;
     case KR_OPT_SM_COUNT: *value = (uint64_t)e->sm_count; return KR_OK;
     default: return fail(e, KR_E_INVALID, "unknown option %u", option);
@@ -2171,7 +2231,7 @@ int kr_engine_create(const kr_config *cfg, kr_engine **out) {
   if (cudaStreamCreateWithPriority(&e->sg, cudaStreamNonBlocking, prio_greatest) != cudaSuccess) return bail(KR_E_CUDA);
   if (cudaStreamCreateWithFlags(&e->scopy, cudaStreamNonBlocking) != cudaSuccess) return bail(KR_E_CUDA);
   cudaEventCreate(&e->ev_h2d0); cudaEventCreate(&e->ev_h2d1); cudaEventCreate(&e->ev_cols); cudaEventCreate(&e->ev_json);
-  for (cudaEvent_t *ev : {&e->pr.ev, &e->orow.ev, &e->mp.ev, &e->ev_inc, &e->ev_order, &e->ev_fork2, &e->ev_join2, &e->ev_fork3, &e->ev_join3, &e->ev_fork, &e->ev_hash})
+  for (cudaEvent_t *ev : {&e->pr.ev, &e->orow.ev, &e->mp.ev, &e->mv.ev, &e->ev_inc, &e->ev_order, &e->ev_fork2, &e->ev_join2, &e->ev_fork3, &e->ev_join3, &e->ev_fork, &e->ev_hash})
     cudaEventCreateWithFlags(ev, cudaEventDisableTiming);
   cudaEventCreate(&e->ev_a); cudaEventCreate(&e->ev_b); cudaEventCreate(&e->ev_c);
   for (auto &ev : e->ev_k) cudaEventCreate(&ev);
@@ -2256,7 +2316,8 @@ void kr_engine_destroy(kr_engine *e) {
   if (e->sh) cudaStreamSynchronize(e->sh);
   if (e->h_in) cudaFreeHost(e->h_in);
   if (e->h_out) cudaFreeHost(e->h_out);
-  e->hb.release(); e->pr.release(); e->orow.release(); e->mp.release(); e->inc_stage.release(); e->spec.release();
+  e->hb.release(); e->pr.release(); e->orow.release(); e->mp.release(); e->inc_stage.release(); e->spec.release(); e->mv.release();
+  if (e->d_json_scratch) cudaFree(e->d_json_scratch);
   if (e->h_totals) cudaFreeHost(e->h_totals);
   if (e->h_order) cudaFreeHost(e->h_order);
   if (e->h_inc) cudaFreeHost(e->h_inc);
@@ -2580,6 +2641,68 @@ int kr_snapshot_commit_spec_rows(kr_engine *e, const uint32_t *rows, uint32_t n)
   CK(cudaGetLastError());
   e->n_pull += m;
   return finish_commit(e, bytes, true, true);  // (k_spec_pull wrote the columns' ranges as well as the JSON)
+}
+
+int kr_snapshot_commit_json_moves(kr_engine *e, const uint32_t *rows, uint32_t n) {
+  if (!e || (!rows && n)) return KR_E_INVALID;
+  if (!e->begun || !e->committed_full) return fail(e, KR_E_STATE, "a JSON move commit needs a full commit of this layout first");
+  if (n == 0) return KR_OK;
+  const kr_sizes &z = e->sizes;
+  kr_snapshot_bufs hb;
+  bind_in(e->il, e->h_in, &hb);
+  const std::vector<CommitRecord::Row> &rec = e->rec.rows;
+  std::vector<uint8_t> seen(rec.size(), 0);
+  std::vector<std::pair<uint64_t, uint32_t>> to(n);  // (destination, row) for the overlap check
+  for (uint32_t i = 0; i < n; i++) {
+    const uint32_t c = rows[i];
+    if (c >= rec.size() || c >= z.n_clusters) return fail(e, KR_E_INVALID, "cluster row %u: not a recorded row", c);
+    if (seen[c]) return fail(e, KR_E_INVALID, "cluster row %u appears twice", c);
+    seen[c] = 1;
+    if (hb.c_json_len[c] != rec[c].json_len) return fail(e, KR_E_INVALID, "cluster %u: json length %u, recorded %u (a move keeps the bytes)", c, hb.c_json_len[c], rec[c].json_len);
+    if (int rc = check_cluster_row(e, hb, z, c, true)) return rc;
+    to[i] = {hb.c_json_off[c], c};
+  }
+  if (!std::is_sorted(to.begin(), to.end())) std::sort(to.begin(), to.end());  // (a compaction in row order lists them sorted)
+  uint64_t end = 0;
+  uint32_t last = KR_EMPTY32;  // (the listed row with a non-empty destination that ends last so far)
+  for (const auto &t : to) {
+    if (!hb.c_json_len[t.second]) continue;
+    if (last != KR_EMPTY32 && t.first < end) return fail(e, KR_E_INVALID, "clusters %u and %u: json destinations overlap", last, t.second);
+    end = t.first + ((hb.c_json_len[t.second] + 15ull) & ~15ull); last = t.second;
+  }
+  CK(cudaSetDevice(e->cfg.device));
+  const size_t cap = (size_t)e->cfg.max_clusters + 1;
+  if (!e->d_json_scratch) {  // (an engine that never moves pays nothing)
+    if (e->mv.reserve(24 * cap, 0) != cudaSuccess) return fail(e, KR_E_CUDA, "allocation of the JSON move list failed");
+    if (cudaMalloc((void **)&e->d_json_scratch, align_up((size_t)e->cfg.max_json_bytes + 16)) != cudaSuccess) {
+      e->d_json_scratch = nullptr;
+      return fail(e, KR_E_CUDA, "allocation of the JSON move scratch failed");
+    }
+  }
+  CK(e->mv.wait());  // a previous move list may still be crossing
+  uint32_t *lr = reinterpret_cast<uint32_t *>(e->mv.h), *ll = reinterpret_cast<uint32_t *>(e->mv.h + 4 * cap);
+  uint64_t *ld = reinterpret_cast<uint64_t *>(e->mv.h + 8 * cap), *ls = reinterpret_cast<uint64_t *>(e->mv.h + 16 * cap);
+  for (uint32_t i = 0; i < n; i++) {
+    const uint32_t c = rows[i];
+    lr[i] = c; ll[i] = rec[c].json_len; ld[i] = hb.c_json_off[c]; ls[i] = rec[c].json_off;
+  }
+  if (int rc = begin_commit(e)) return rc;
+  // a row whose bytes went is pulled again by its next spec-row commit, even within this epoch
+  for (uint32_t c : e->rec.commit_json_moves(to, seen)) if (c < e->pull_stamp.size()) e->pull_stamp[c] = 0;
+  uint32_t *dr = reinterpret_cast<uint32_t *>(e->mv.d), *dl = reinterpret_cast<uint32_t *>(e->mv.d + 4 * cap);
+  uint64_t *dd = reinterpret_cast<uint64_t *>(e->mv.d + 8 * cap), *ds = reinterpret_cast<uint64_t *>(e->mv.d + 16 * cap);
+  CK(cudaMemcpyAsync(dr, lr, 4 * (size_t)n, cudaMemcpyHostToDevice, e->scopy));
+  CK(cudaMemcpyAsync(dl, ll, 4 * (size_t)n, cudaMemcpyHostToDevice, e->scopy));
+  CK(cudaMemcpyAsync(dd, ld, 8 * (size_t)n, cudaMemcpyHostToDevice, e->scopy));
+  CK(cudaMemcpyAsync(ds, ls, 8 * (size_t)n, cudaMemcpyHostToDevice, e->scopy));
+  CK(cudaEventRecord(e->mv.ev, e->scopy));
+  e->mv.busy = true;
+  uint8_t *d_json = e->d_in + e->il.off[kNumCols - 1];
+  k_json_move_gather<<<n, 128, 0, e->scopy>>>(ds, dd, dl, d_json, e->d_json_scratch);
+  k_json_move_scatter<<<n, 128, 0, e->scopy>>>(dr, dd, dl, e->d_json_scratch, d_json, reinterpret_cast<uint64_t *>(e->d_in + e->il.off[kJsonOffCol]),
+                                               reinterpret_cast<uint32_t *>(e->d_in + e->il.off[kJsonOffCol + 1]));
+  CK(cudaGetLastError());
+  return finish_commit(e, 24 * (uint64_t)n, true, true);  // (the move list only: no spec byte crosses PCIe)
 }
 
 int kr_snapshot_commit_pod_rows(kr_engine *e, const uint32_t *rows, uint32_t n) { return commit_pod_patch(e, rows, nullptr, n); }

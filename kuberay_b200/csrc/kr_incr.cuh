@@ -290,6 +290,29 @@ __global__ void __launch_bounds__(128) k_spec_pull(const uint32_t *__restrict__ 
   if (threadIdx.x == 0) { c_json_off[rows[i]] = off; c_json_len[rows[i]] = len; }
 }
 
+// kr_snapshot_commit_json_moves: the listed RayClusters' unchanged muted-spec JSON moves inside the device arena, from the range the
+// record holds (src) to the host's new one (dst).  Sources and destinations may overlap in any direction (a compaction re-places the
+// blobs in row order), so the copy goes out of place: k_json_move_gather copies every listed range into the scratch at its
+// destination offset, then k_json_move_scatter copies the destination ranges back and sets the rows' c_json_off / c_json_len.  One
+// CTA per row, 16-byte loads; the padded destinations are disjoint, so no two CTAs write the same bytes.
+__global__ void __launch_bounds__(128) k_json_move_gather(const uint64_t *__restrict__ src, const uint64_t *__restrict__ dst, const uint32_t *__restrict__ lens,
+                                                          const uint8_t *__restrict__ d_json, uint8_t *__restrict__ scratch) {
+  const uint32_t i = blockIdx.x;
+  const uint4 *from = reinterpret_cast<const uint4 *>(d_json + src[i]);
+  uint4 *to = reinterpret_cast<uint4 *>(scratch + dst[i]);
+  for (uint32_t k = threadIdx.x; k < (lens[i] + 15) / 16; k += blockDim.x) to[k] = from[k];
+}
+__global__ void __launch_bounds__(128) k_json_move_scatter(const uint32_t *__restrict__ rows, const uint64_t *__restrict__ dst, const uint32_t *__restrict__ lens,
+                                                           const uint8_t *__restrict__ scratch, uint8_t *__restrict__ d_json, uint64_t *c_json_off, uint32_t *c_json_len) {
+  const uint32_t i = blockIdx.x;
+  const uint64_t off = dst[i];
+  const uint32_t len = lens[i];
+  const uint4 *from = reinterpret_cast<const uint4 *>(scratch + off);
+  uint4 *to = reinterpret_cast<uint4 *>(d_json + off);
+  for (uint32_t k = threadIdx.x; k < (len + 15) / 16; k += blockDim.x) to[k] = from[k];
+  if (threadIdx.x == 0) { c_json_off[rows[i]] = off; c_json_len[rows[i]] = len; }
+}
+
 // the listed RayClusters whose Recreate gate reads the digest (k_inc_mark_recreate's test, for the listed rows only)
 __global__ void __launch_bounds__(256) k_inc_mark_rows(SnapDev s, ScratchDev sc, const uint32_t *__restrict__ rows, uint32_t n) {
   const uint32_t i = blockIdx.x * blockDim.x + threadIdx.x;

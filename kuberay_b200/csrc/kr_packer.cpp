@@ -103,11 +103,15 @@ struct kr_packer {
   std::vector<uint32_t> dirty_cl, dirty_hd;
   std::vector<uint8_t> cl_flag, hd_flag;
   bool wtd_changed = false;           // a workersToDelete name was rewritten in place (same count): the whole object part travels
-  // RayClusters whose muted-spec JSON was placed since the last flush (kr_snapshot_commit_spec_rows with KR_OPT_SPEC_ROWS, unless the
-  // arena was compacted or, without KR_OPT_CLUSTER_DELETES, a RayCluster row moved); a deletion moves a row's flag with the row
+  // RayClusters whose muted-spec JSON was re-emitted since the last flush (kr_snapshot_commit_spec_rows with KR_OPT_SPEC_ROWS, unless
+  // the arena was compacted without KR_OPT_JSON_MOVES or, without KR_OPT_CLUSTER_DELETES, a RayCluster row moved); a deletion moves a
+  // row's flag with the row.  A compaction re-places every blob without flagging it.
   std::vector<uint32_t> json_rows;
   std::vector<uint8_t> json_flag;
   bool json_compacted = false, clusters_moved = false;
+  // per row, the blob's offset before the first compaction since the last flush (valid while json_compacted): for a RayCluster that
+  // kept its row and was not re-emitted, the range the engine holds (KR_OPT_JSON_MOVES moves it from there)
+  std::vector<uint64_t> pre_compact_off;
   bool reshaped = false;              // a RayCluster the engine holds changed its group count or a workersToDelete list length (with
                                       // KR_OPT_GROUP_EDITS: a list length, unless KR_OPT_WTD_EDITS as well)
   bool regrouped = false;             // KR_OPT_GROUP_EDITS: a RayCluster the engine holds changed its list of worker groups
@@ -200,7 +204,13 @@ int rebuild_tables(kr_packer *p) {
   return KR_OK;
 }
 
-int place_json(kr_packer *p, ClusterRec &c) {  // put the cluster's blob at the arena's cursor (16-byte aligned, zero padded)
+void mark_emitted(kr_packer *p, uint32_t row) {
+  if (row >= p->json_flag.size()) p->json_flag.resize((size_t)row + 256, 0);
+  if (!p->json_flag[row]) { p->json_flag[row] = 1; p->json_rows.push_back(row); }
+}
+
+// put the cluster's blob at the arena's cursor (16-byte aligned, zero padded); `emitted`: a new blob, not a compaction's
+int place_json(kr_packer *p, ClusterRec &c, bool emitted = true) {
   const uint64_t padded = (c.json.size() + 15) & ~15ull;
   if (p->json_cursor + padded > p->cap.max_json_bytes) return KR_E_CAPACITY;
   memcpy(p->b.json + p->json_cursor, c.json.data(), c.json.size());
@@ -208,14 +218,17 @@ int place_json(kr_packer *p, ClusterRec &c) {  // put the cluster's blob at the 
   c.json_off = p->json_cursor; c.json_placed = true;
   p->b.c_json_off[c.row] = c.json_off; p->b.c_json_len[c.row] = (uint32_t)c.json.size();
   p->json_cursor += padded;
-  if (c.row >= p->json_flag.size()) p->json_flag.resize((size_t)c.row + 256, 0);
-  if (!p->json_flag[c.row]) { p->json_flag[c.row] = 1; p->json_rows.push_back(c.row); }
+  if (emitted) mark_emitted(p, c.row);
   return KR_OK;
 }
 
 int compact_json(kr_packer *p) {
+  if (!p->json_compacted) {
+    p->pre_compact_off.resize(p->clusters.size());
+    for (size_t r = 0; r < p->clusters.size(); r++) p->pre_compact_off[r] = p->clusters[r].json_off;
+  }
   p->json_cursor = 0; p->json_dead = 0; p->json_compacted = true;
-  for (auto &c : p->clusters) if (int rc = place_json(p, c)) return pfail(p, rc, "kr_packer: muted-spec JSON exceeds kr_config.max_json_bytes");
+  for (auto &c : p->clusters) if (int rc = place_json(p, c, false)) return pfail(p, rc, "kr_packer: muted-spec JSON exceeds kr_config.max_json_bytes");
   return KR_OK;
 }
 
@@ -397,6 +410,7 @@ int kr_packer_cluster_upsert(kr_packer *p, const kr_cluster_obj *o) {
       if (place_json(p, c) != KR_OK) {  // arena full: compact once, then give up
         p->json_dead = 0;
         if (int rc2 = compact_json(p)) return rc2;
+        mark_emitted(p, row);  // (the compaction placed the new blob)
       }
       p->json_dirty = true;
     }
@@ -497,25 +511,40 @@ int kr_packer_flush(kr_packer *p, uint32_t *mode_out) {
   uint64_t creates_opt = 0;
   kr_engine_get_option(p->e, KR_OPT_CLUSTER_CREATES, &creates_opt);
   const uint32_t old_nc = p->engine_sizes.n_clusters;
-  const bool appends = creates_opt && !p->first && !p->clusters_moved && !p->reshaped && !p->json_compacted && want.n_clusters > old_nc;
+  // KR_OPT_JSON_MOVES (with KR_OPT_SPEC_ROWS): a compaction travels as moves inside the device arena and keeps every row path below;
+  // without it, a compacted arena goes whole
+  uint64_t spec_opt = 0, moves_opt = 0;
+  kr_engine_get_option(p->e, KR_OPT_SPEC_ROWS, &spec_opt);
+  kr_engine_get_option(p->e, KR_OPT_JSON_MOVES, &moves_opt);
+  const bool compacted = p->json_compacted && !(moves_opt && spec_opt && !p->first);
+  const bool appends = creates_opt && !p->first && !p->clusters_moved && !p->reshaped && !compacted && want.n_clusters > old_nc;
   // KR_OPT_CLUSTER_DELETES: RayClusters deleted by swap-remove (none the engine holds reshaped, the arena not compacted) keep the
   // incremental epoch as well: the kept RayClusters' edited specs as spec rows before the object part, the moved and created ones'
   // after it
   uint64_t deletes_opt = 0;
   kr_engine_get_option(p->e, KR_OPT_CLUSTER_DELETES, &deletes_opt);
-  const bool renumbered = deletes_opt && !p->first && p->clusters_moved && !p->reshaped && !p->json_compacted;
+  const bool renumbered = deletes_opt && !p->first && p->clusters_moved && !p->reshaped && !compacted;
   // KR_OPT_GROUP_EDITS: RayClusters that changed their worker groups (none reshaped, the arena not compacted, any creation or deletion
   // of the flush on the path above) keep the incremental epoch too: the object part, then their specs as spec rows
-  const bool regroups = p->regrouped && !p->first && !p->reshaped && !p->json_compacted &&
+  const bool regroups = p->regrouped && !p->first && !p->reshaped && !compacted &&
                         ((want.n_clusters == old_nc && !p->clusters_moved) || appends || renumbered);
   // Row-granular spec commit (KR_OPT_SPEC_ROWS): only the re-emitted blobs travel, while every other one stays where it was.
-  uint64_t spec_opt = 0;
-  kr_engine_get_option(p->e, KR_OPT_SPEC_ROWS, &spec_opt);
-  const bool spec_ok = spec_opt && p->json_dirty && !p->first && !p->json_compacted && !p->clusters_moved && (want.n_clusters == old_nc || appends);
+  const bool spec_ok = spec_opt && p->json_dirty && !p->first && !compacted && !p->clusters_moved && (want.n_clusters == old_nc || appends);
   std::vector<uint32_t> new_rows, old_rows;  // blobs placed this flush: of appended, moved or created RayClusters / of the others
   for (uint32_t r : p->json_rows) (r >= old_nc || p->is_fresh(r) ? new_rows : old_rows).push_back(r);
   // every placed blob travels as a spec row
   const bool json_rows_ok = spec_ok || ((appends || renumbered || regroups) && (old_rows.empty() || spec_opt));
+  // A compaction under KR_OPT_JSON_MOVES: the RayClusters the engine holds in the same row, not re-emitted, move where the compaction
+  // put them; every created, moved or regrouped RayCluster's spec follows the object part as a spec row (its range changed too)
+  const bool moves = p->json_compacted && !compacted && json_rows_ok;
+  std::vector<uint32_t> move_rows;
+  if (moves) {
+    const uint32_t kept = std::min<uint32_t>(old_nc, want.n_clusters);
+    for (uint32_t r = 0; r < kept && r < p->pre_compact_off.size(); r++)
+      if (!p->is_fresh(r) && !(r < p->json_flag.size() && p->json_flag[r]) && p->pre_compact_off[r] != p->clusters[r].json_off) move_rows.push_back(r);
+    new_rows.clear();
+    for (uint32_t r = 0; r < want.n_clusters; r++) if (r >= old_nc || p->is_fresh(r)) new_rows.push_back(r);
+  }
   if (memcmp(&want, &p->engine_sizes, sizeof want) != 0 || p->first) {
     if (int rc = kr_snapshot_begin(p->e, &p->sizes, &same)) return rc;  // fixed layout: new live counts, same addresses, resident data kept
     p->engine_sizes = want;
@@ -526,6 +555,10 @@ int kr_packer_flush(kr_packer *p, uint32_t *mode_out) {
     mode = KR_PACK_FULL;
   } else {
     if (trace) t2 = now();
+    if (moves) {  // (first: the spec-row and object commits below then find the ranges where the host has them)
+      if (int rc = kr_snapshot_commit_json_moves(p->e, move_rows.data(), (uint32_t)move_rows.size())) return rc;
+      mode |= KR_PACK_JSON_MOVES;
+    }
     if (json_rows_ok && !old_rows.empty()) {  // (before the object commit, which would otherwise see the moved ranges and re-hash every RayCluster)
       if (int rc = kr_snapshot_commit_spec_rows(p->e, old_rows.data(), (uint32_t)old_rows.size())) return rc;
       mode |= KR_PACK_SPEC_ROWS;

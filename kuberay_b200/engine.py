@@ -61,6 +61,7 @@ def lib() -> C.CDLL:
         L.kr_snapshot_commit_pod_values.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_uint32]
         L.kr_snapshot_commit_object_rows.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32, C.c_void_p, C.c_uint32]
         L.kr_snapshot_commit_spec_rows.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
+        L.kr_snapshot_commit_json_moves.argtypes = [C.c_void_p, C.c_void_p, C.c_uint32]
         L.kr_engine_set_option.argtypes = [C.c_void_p, C.c_uint32, C.c_uint64]
         L.kr_engine_get_option.argtypes = [C.c_void_p, C.c_uint32, P(C.c_uint64)]
         L.kr_reconcile_batch.argtypes = [C.c_void_p, P(abi.kr_flags), P(abi.kr_results_view)]
@@ -237,7 +238,8 @@ class Engine:
                      large_clusters: bool = False, wide_clusters: bool = False, huge_clusters: bool = False,
                      wtd_edits: bool = False, spec_rows: bool = False, cluster_creates: bool = False,
                      cluster_deletes: bool = False, group_edits: bool = False, large_growth: bool = False,
-                     large_moves: bool = False, bucket_pod_lists: bool = False, huge_growth: bool = False) -> "Engine":
+                     large_moves: bool = False, bucket_pod_lists: bool = False, json_moves: bool = False,
+                     huge_growth: bool = False) -> "Engine":
         d = snap.dims
         up = lambda x: int(x * slack) + 1  # noqa: E731
         if max_creates is None:
@@ -266,6 +268,8 @@ class Engine:
             eng.set_large_moves(True)
         if bucket_pod_lists:
             eng.set_bucket_pod_lists(True)
+        if json_moves:
+            eng.set_json_moves(True)
         if huge_growth:
             eng.set_huge_growth(True)
         return eng
@@ -360,6 +364,11 @@ class Engine:
         the bucket pipeline builds the same sorted_pod_idx, sorted_action and pod_start as the sort pipeline; read at each pass."""
         self._check(self._L.kr_engine_set_option(self._h, abi.OPT_BUCKET_POD_LISTS, 1 if on else 0))
 
+    def set_json_moves(self, on: bool = True):
+        """KR_OPT_JSON_MOVES: with KR_OPT_SPEC_ROWS, the native packer commits a compaction of its JSON arena as moves inside the device
+        arena (commit_json_moves) instead of re-sending the arena; commit_json_moves itself works either way."""
+        self._check(self._L.kr_engine_set_option(self._h, abi.OPT_JSON_MOVES, 1 if on else 0))
+
     def get_option(self, option: int) -> int:
         """kr_engine_get_option: an option's current value, or the read-only OPT_BUCKET_STRIDE (0: the sort pipeline) or OPT_SM_COUNT
         (the SM count the SM-sized grids are laid out for: the device's, or a lower KR_SM_COUNT)."""
@@ -412,6 +421,12 @@ class Engine:
         travel; the next pass re-hashes only them.  Call before the epoch's object commit."""
         r = np.ascontiguousarray(rows, dtype=np.uint32)
         self._check(self._L.kr_snapshot_commit_spec_rows(self._h, r.ctypes.data if r.size else None, r.size))
+
+    def commit_json_moves(self, rows):
+        """kr_snapshot_commit_json_moves: these RayClusters' unchanged specs now sit at the ranges c_json_off gives; the device moves
+        its copies there (no spec byte crosses PCIe, no digest is recomputed).  Call before the epoch's spec-row and object commits."""
+        r = np.ascontiguousarray(rows, dtype=np.uint32)
+        self._check(self._L.kr_snapshot_commit_json_moves(self._h, r.ctypes.data if r.size else None, r.size))
 
     def load(self, snap: Snapshot):
         views = self.begin(snap.sizes())

@@ -173,7 +173,8 @@ class Packer:
     def __init__(self, device=0, max_clusters=1024, max_groups=4096, max_wtd=4096, max_pods=65536, max_heads=2048, max_jobs=1024,
                  max_creates=65536, max_json_bytes=64 << 20, large_clusters=False, wide_clusters=False,
                  huge_clusters=False, wtd_edits=False, spec_rows=False, cluster_creates=False,
-                 cluster_deletes=False, group_edits=False, large_growth=False, large_moves=False, bucket_pod_lists=False, huge_growth=False):
+                 cluster_deletes=False, group_edits=False, large_growth=False, large_moves=False, bucket_pod_lists=False, json_moves=False,
+                 huge_growth=False):
         L = self._L = lib()
         _bind(L)
         if L.kr_device_count() <= 0:
@@ -186,7 +187,7 @@ class Packer:
         self._owned = True
         self._attach_engine(cfg)
         self.set_options(large_clusters, wide_clusters, huge_clusters, wtd_edits, spec_rows, cluster_creates, cluster_deletes, group_edits,
-                         large_growth, large_moves, bucket_pod_lists, huge_growth)
+                         large_growth, large_moves, bucket_pod_lists, json_moves, huge_growth)
 
     @classmethod
     def view(cls, handle: int, cfg: abi.kr_config) -> "Packer":
@@ -204,7 +205,8 @@ class Packer:
         self.engine._L, self.engine._h, self.engine.sizes, self.engine.cfg = self._L, C.c_void_p(self._L.kr_packer_engine(self._h)), abi.kr_sizes(), cfg
 
     def set_options(self, large_clusters=False, wide_clusters=False, huge_clusters=False, wtd_edits=False, spec_rows=False, cluster_creates=False,
-                    cluster_deletes=False, group_edits=False, large_growth=False, large_moves=False, bucket_pod_lists=False, huge_growth=False):
+                    cluster_deletes=False, group_edits=False, large_growth=False, large_moves=False, bucket_pod_lists=False, json_moves=False,
+                    huge_growth=False):
         """Switch on the opt-in engine options of this packer's engine (kr_packer_engine)."""
         if large_clusters:  # KR_OPT_LARGE_CLUSTERS, set through kr_packer_engine()
             self.engine.set_large_clusters(True)
@@ -228,6 +230,8 @@ class Packer:
             self.engine.set_large_moves(True)
         if bucket_pod_lists:  # KR_OPT_BUCKET_POD_LISTS, likewise: fetching the pod lists keeps the pipeline and the incremental epoch
             self.engine.set_bucket_pod_lists(True)
+        if json_moves:  # KR_OPT_JSON_MOVES, likewise: with spec_rows, a compaction of the JSON arena moves the specs on the device (PACK_JSON_MOVES)
+            self.engine.set_json_moves(True)
         if huge_growth:  # KR_OPT_HUGE_GROWTH, likewise: a RayCluster that scales past LARGE_MAX_PODS Pods stays incremental
             self.engine.set_huge_growth(True)
 
@@ -330,7 +334,7 @@ class GroupPacker:
     def __init__(self, devices: list[int], max_clusters=1024, max_groups=4096, max_wtd=4096, max_pods=65536, max_heads=2048, max_jobs=1024,
                  max_creates=65536, max_json_bytes=64 << 20, large_clusters=False, wide_clusters=False, huge_clusters=False,
                  wtd_edits=False, spec_rows=False, cluster_creates=False, cluster_deletes=False, group_edits=False, large_growth=False,
-                 large_moves=False, bucket_pod_lists=False, huge_growth=False):
+                 large_moves=False, bucket_pod_lists=False, json_moves=False, huge_growth=False):
         L = self._L = lib()
         _bind(L)
         if L.kr_device_count() <= 0:
@@ -345,7 +349,7 @@ class GroupPacker:
         self.shards = [Packer.view(L.kr_group_packer_shard(self._h, i), cfg) for i in range(self.n)]
         for sh in self.shards:  # options are per shard (the native group packer does not forward them)
             sh.set_options(large_clusters, wide_clusters, huge_clusters, wtd_edits, spec_rows, cluster_creates, cluster_deletes, group_edits,
-                           large_growth, large_moves, bucket_pod_lists, huge_growth)
+                           large_growth, large_moves, bucket_pod_lists, json_moves, huge_growth)
         self.group = Group.__new__(Group)  # a view over the group packer's kr_group (not owned: close() is the group packer's)
         self.group._L, self.group._h, self.group.n, self.group.engines = L, C.c_void_p(L.kr_group_packer_group(self._h)), self.n, [sh.engine for sh in self.shards]
 
