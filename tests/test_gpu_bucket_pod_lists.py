@@ -86,6 +86,12 @@ def open_driver(snap, flags, **options):
 
 @pytest.mark.parametrize("seed", [1, 2])
 def test_every_fleet_class_full_and_incremental(seed, oracle_mod):
+    fleet_stream(seed, oracle_mod, lambda epoch: epoch % 3 == 2)
+
+
+def fleet_stream(seed, oracle_mod, big):
+    """The fleet, a full pass and six incremental epochs of Pod churn, a moved and a deleted Pod; the large, huge and wide
+    RayClusters also churn in the epochs where big(epoch), and stay untouched in the others."""
     dr = open_driver(*fleet(seed), **CLASSES)
     rng = np.random.default_rng(seed)
     try:
@@ -94,7 +100,7 @@ def test_every_fleet_class_full_and_incremental(seed, oracle_mod):
         ordinary = np.array([c for c in range(dr.snap.dims["clusters"]) if c not in (HUGE, LARGE, WIDE)])
         for epoch in range(6):
             rows = [workers(dr.snap, int(c))[:2] for c in rng.choice(ordinary, 30, replace=False)]
-            if epoch % 3 == 2:  # every third epoch also the large, huge and wide ones; the others leave them untouched
+            if big(epoch):
                 rows += [workers(dr.snap, c)[::97] for c in (HUGE, LARGE, WIDE)]
             rows = np.concatenate(rows)
             flip_ready(dr.snap, rows)
@@ -199,3 +205,124 @@ def test_launch_shapes_at_eight_sms():
     env = dict(os.environ, KR_SM_COUNT="8")
     out = subprocess.run([sys.executable, "-c", code], env=env, capture_output=True, text=True, timeout=900)
     assert out.returncode == 0, out.stdout[-2000:] + out.stderr[-4000:]
+
+
+# ------------------------------------------------------------------------------------------------ list edges
+
+def keep_pods(snap, rows):
+    """A copy of `snap` with only the pod rows `rows` (in that order) and the head-aux rows of the heads among them; every
+    RayCluster, group, name and the JSON arena stay."""
+    d = snap.dims
+    rows = np.asarray(rows, dtype=np.int64)
+    new_p = np.full(d["pods"], -1, dtype=np.int64)
+    new_p[rows] = np.arange(rows.size)
+    heads = np.flatnonzero(new_p[snap.h_pod_idx] >= 0) if d["heads"] else np.zeros(0, np.int64)
+    out = snap_like(snap, pods=rows.size, heads=heads.size)
+    for name, _dt, mult, dim in abi.COLUMNS:
+        src = snap.cols[name]
+        if dim == "pods":
+            out.cols[name][:] = src[rows]
+        elif dim == "heads":
+            out.cols[name][:] = src.reshape(-1, mult)[heads].reshape(-1)
+        else:
+            out.cols[name][:] = src
+    out.h_pod_idx[:] = new_p[snap.h_pod_idx[heads]]
+    return out.validate()
+
+
+def snap_like(snap, **dims):
+    d = dict(snap.dims, **dims)
+    return snp.Snapshot(d["clusters"], d["groups"], d["wtd"], d["pods"], d["heads"], d["jobs"], d["json"])
+
+
+def orphan(snap, rows):
+    """Pods whose RayCluster is not in the snapshot."""
+    snap.p_cluster_name_id[rows] = np.uint32(0x7E000000)
+
+
+def tile_fleet(n_pods, tail):
+    """RayClusters of 8 Pods in row order (no shuffle), cut to exactly `n_pods` rows, the first RayCluster's rows first.  tail:
+    "orphans" — the last three rows are orphans; "flush" — the last RayCluster's Pods are the last rows; "empty" — so are those of
+    the RayCluster before it, and the last two RayClusters have no Pods (their starts are n_pods)."""
+    nc = n_pods // 8 + 4
+    snap, flags = synthetic.generate(synthetic.SynthParams(n_clusters=nc, pods_per_cluster=8, groups=1, orphan_frac=0.0, shuffle=False, seed=n_pods))
+    total = snap.dims["pods"]
+    end = total - (16 if tail == "empty" else 0)
+    snap = keep_pods(snap, np.arange(end - n_pods, end))
+    if tail == "orphans":
+        orphan(snap, np.arange(max(0, n_pods - 3), n_pods))
+    flags.fetch_pod_lists = 1
+    return snap, flags
+
+
+@pytest.mark.parametrize("tail", ["orphans", "flush", "empty"])
+@pytest.mark.parametrize("n_pods", [1, 255, 256, 257, 2047, 2048, 2049])
+def test_pod_counts_around_the_tiles(n_pods, tail, oracle_mod):
+    """Pod counts at the edges of k_lists_gather's 256-thread blocks (its thread one past the end writes the starts of the
+    trailing RayClusters without Pods) and of the sort's tiles; a full pass, then an incremental epoch that flips one Pod."""
+    snap, flags = tile_fleet(n_pods, tail)
+    assert snap.dims["pods"] == n_pods
+    dr = open_driver(snap, flags)
+    try:
+        got = check(dr, oracle_mod, "full")
+        if tail == "orphans":
+            assert got.n_orphans == min(3, n_pods)
+        else:
+            assert got.n_orphans == 0 and got.clusters["n_pods"][-1 - 2 * (tail == "empty")] > 0
+        if tail == "empty":
+            assert (got.clusters["n_pods"][-2:] == 0).all() and (got.clusters["pod_start"][-2:] == n_pods).all()
+        rows = np.array([n_pods // 2])
+        flip_ready(dr.snap, rows)
+        dr.commit_rows(rows)
+        check(dr, oracle_mod, "incremental")
+    finally:
+        dr.close()
+
+
+@pytest.mark.parametrize("shape", ["all_orphans", "no_clusters", "no_pods"])
+def test_fleets_without_lists_to_build(shape, oracle_mod):
+    """Every Pod an orphan (every RayCluster's list empty, each starting at 0), no RayClusters at all (kr_snapshot_begin takes
+    the layout: every Pod in the orphans' segment), and no Pods."""
+    snap, flags = tile_fleet(300, "flush")
+    if shape == "all_orphans":
+        orphan(snap, np.arange(snap.dims["pods"]))
+    elif shape == "no_clusters":
+        snap = synthetic.first_clusters(snap, 0, free_pods=False)
+    else:
+        snap = keep_pods(snap, [])
+    dr = open_driver(snap, flags)
+    try:
+        got = check(dr, oracle_mod, "full")
+        assert not got.clusters["pod_start"].any()
+        if shape != "no_pods":
+            assert got.n_orphans == snap.dims["pods"]
+    finally:
+        dr.close()
+
+
+def test_structural_void_then_full_then_incremental(oracle_mod):
+    """A renamed worker group is a table key: the incremental attempt flags KR_INC_STRUCTURAL (k_lists_owner then leaves every
+    owner unset) and the full pass that follows builds the lists; Pod churn after that is incremental again."""
+    dr = open_driver(*small_fleet(8))
+    try:
+        check(dr, oracle_mod, "full")
+        rows = np.arange(5, dr.snap.dims["pods"], 331)
+        flip_ready(dr.snap, rows)
+        dr.snap.g_name_id[7] += np.uint32(100000)
+        dr.commit_objects()
+        dr.commit_rows(rows)
+        check(dr, oracle_mod, "full")
+        assert dr.eng.last_pass()["why"] == ["STRUCTURAL"], dr.eng.last_pass()
+        donor = workers(dr.snap, 250)[:2]
+        move(dr.snap, donor, 1)
+        dr.commit_rows(donor)
+        check(dr, oracle_mod, "incremental")
+    finally:
+        dr.close()
+
+
+@pytest.mark.parametrize("seed", [5])
+def test_large_and_huge_redecided_in_consecutive_epochs(seed, oracle_mod):
+    """The large, huge and wide RayClusters re-decided in every epoch: each pass's per-cluster kernels find their sort segments in
+    sorted_pod_idx overwritten by the lists of the pass before, and must sort them again before the builder overwrites them."""
+    fleet_stream(seed, oracle_mod, lambda epoch: True)

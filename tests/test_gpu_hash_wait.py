@@ -288,23 +288,33 @@ ENVS = {"default": {}, "no_spin": {"KR_NO_HASH_SPIN": "1"}, "no_pdl": {"KR_NO_PD
         "no_fuse": {"KR_NO_FUSE": "1"}, "radix": {"KR_FORCE_RADIX": "1"}}
 
 
-@pytest.mark.parametrize("fetch", [0, 1])
+@pytest.mark.parametrize("fetch", [0, 1, 2])
 @pytest.mark.parametrize("env", list(ENVS))
 def test_every_schedule_and_pipeline(env, fetch, fleet, oracle_mod, monkeypatch):
     """Compact results take the bucket pipeline (the radix one under KR_FORCE_RADIX) and the full pod lists the sort pipeline;
-    only the bucket pipeline's spin schedule waits, and falls back.  A second pass follows on the same engine."""
+    only the bucket pipeline's spin schedule waits, and falls back.  fetch = 2: the full pod lists on an engine with
+    KR_OPT_BUCKET_POD_LISTS, which keeps the bucket pipeline and its spin schedule, so the fallback reruns the list builder behind
+    k_decide2_phase1.  A second pass follows on the same engine."""
     for k, v in ENVS[env].items():
         monkeypatch.setenv(k, v)                                       # (kr_engine_create reads them)
     snap, flags, _, _ = fleet
     flags = abi.kr_flags.from_buffer_copy(flags)
-    flags.fetch_pod_lists = fetch
-    eng = Engine.for_snapshot(snap, max_creates=1 << 16)
+    flags.fetch_pod_lists = min(fetch, 1)
+    opts = dict(bucket_pod_lists=True) if fetch == 2 else {}
+    bucket = fetch != 1 and env != "radix"
+    eng = Engine.for_snapshot(snap, max_creates=1 << 16, **opts)
     try:
         eng.load(snap)
-        check(snap, flags, eng.reconcile(flags), oracle_mod)
-        spin = fetch == 0 and env not in ("no_spin", "radix")
-        assert phase1_extra(eng, snap, flags) == (1 if spin else 0)
-        check(snap, flags, eng.reconcile(flags), oracle_mod)
+        for first in (True, False):
+            got = eng.reconcile(flags)
+            check(snap, flags, got, oracle_mod)
+            rep = eng.last_pass()
+            assert (rep["pipeline"] == "bucket") == bucket, rep
+            assert got.sorted_pod_idx.size == (snap.dims["pods"] if fetch else 0)
+            if first:
+                spin = bucket and env != "no_spin"
+                assert rep["kind"] == "full" and rep["hash_wait"] == spin, rep
+                assert phase1_extra(eng, snap, flags, **opts) == (1 if spin else 0)
     finally:
         eng.close()
 

@@ -419,18 +419,67 @@ def test_one_cluster_at_each_bucket_stride_edge(multihost, regimes, oracle_mod):
         assert _bucket_taken(snap, flags) == (size <= regimes.max_stride), size
 
 
+@pytest.mark.parametrize("multihost", [False, True])
+def test_one_cluster_at_each_bucket_stride_edge_with_lists(multihost, regimes, oracle_mod):
+    """KR_OPT_BUCKET_POD_LISTS fetching the lists: one Pod past a stride voids the attempt (k_lists_owner then leaves every owner
+    unset) and the stride widens, and past 256 Pods the pass leaves the bucket pipeline; the lists fetched are those of the attempt
+    that stood.  Then a second pass on the same engine, incremental wherever the first stayed on the bucket pipeline."""
+    strides = (64, 128, 256)
+    assert strides[-1] == regimes.max_stride
+    for size in (64, 65, 128, 129, 256, 257):
+        snap, flags = _one_cluster_of(size, multihost)
+        flags.fetch_pod_lists = 1
+        want = oracle_mod.run(snap, flags)
+        eng = Engine.for_snapshot(snap, bucket_pod_lists=True)
+        try:
+            eng.load(snap)
+            for kind in ("full", "incremental"):
+                got = eng.reconcile(flags)
+                rep = eng.last_pass()
+                d = want.diff(got)
+                assert not d, (size, kind, d[:6])
+                assert got.sorted_pod_idx.size == snap.dims["pods"] and got.clusters["n_pods"][0] == size
+                if size > regimes.max_stride:
+                    assert rep["pipeline"] != "bucket" and rep["kind"] == "full", (size, rep)
+                    continue
+                stride = next(s for s in strides if size <= s)
+                assert rep["pipeline"] == "bucket" and rep["kind"] == kind and rep["stride"] == stride, (size, rep)
+                assert kind != "full" or rep["attempts"] == strides.index(stride), (size, rep)
+        finally:
+            eng.close()
+
+
 # ------------------------------------------------------------------------------------------------ incremental arena exhaustion
 
 def test_incremental_epochs_that_run_out_of_arena(oracle_mod):
     """A tight max_creates: re-decided RayClusters that outgrow their create runs take new ones at the cursor, and unhealthy
     pods grow action runs; once a cursor passes its end the epoch is void and a full pass packs the arenas again."""
+    _arena_epochs(oracle_mod, lists=False)
+
+
+def test_incremental_epochs_that_run_out_of_arena_with_lists(oracle_mod):
+    """The same with KR_OPT_BUCKET_POD_LISTS fetching the lists every epoch: the void incremental attempt builds no lists, and
+    the full pass after it does."""
+    _arena_epochs(oracle_mod, lists=True)
+
+
+def _arena_epochs(oracle_mod, lists):
     snap, flags = synthetic.generate(synthetic.SynthParams(n_clusters=400, pods_per_cluster=12, groups=1, healthy=True, seed=14))
     nc = snap.dims["clusters"]
     members = _group_members(snap)
     cap = 600
-    dr = Driver(snap, flags, max_creates=cap)
+    dr = Driver(snap, flags, max_creates=cap, bucket_pod_lists=lists)
+    dr.flags.fetch_pod_lists = int(lists)
+
+    def check(expect_incremental=None):
+        got, _ = dr.check(oracle_mod, expect_incremental)
+        rep = dr.eng.last_pass()
+        assert rep["pipeline"] == "bucket" and rep["kind"] == ("incremental" if incremental(got, nc) else "full"), rep
+        assert got.sorted_pod_idx.size == (snap.dims["pods"] if lists else 0) and "POD_LISTS" not in rep["why"], rep
+        return got, _
+
     try:
-        got, _ = dr.check(oracle_mod, expect_incremental=False)
+        got, _ = check(expect_incremental=False)
         assert got.n_create_total == 0
         base = snap.g_replicas.copy()
         kinds, prev_up, prev_bad = [], np.zeros(0, np.int64), []
@@ -443,7 +492,7 @@ def test_incremental_epochs_that_run_out_of_arena(oracle_mod):
             set_phase(snap, bad, abi.PHASE_FAILED)
             dr.commit_objects()
             dr.commit_rows(list(bad) + list(prev_bad))
-            got, _ = dr.check(oracle_mod)
+            got, _ = check()
             inc = incremental(got, nc)
             full = got.changed_clusters is None and got.n_changed == nc
             assert inc != full
@@ -463,9 +512,9 @@ def test_incremental_epochs_that_run_out_of_arena(oracle_mod):
         dr.commit_objects()
         dr.commit_rows(prev_bad)
         dr.prev = None
-        dr.check(oracle_mod, expect_incremental=False)   # (the overrun left runs unwritten: this pass starts over)
+        check(expect_incremental=False)   # (the overrun left runs unwritten: this pass starts over)
         flip_ready(snap, bad)
         dr.commit_rows(bad)
-        dr.check(oracle_mod, expect_incremental=True)
+        check(expect_incremental=True)
     finally:
         dr.close()
