@@ -10,20 +10,16 @@ ms through the C ABI (host clock around the commits and kr_reconcile_batch, resu
 kernels alone in one profiled epoch.
 Usage: python tools/creates_bench.py [--epochs 10] [--runs 3] [--new 4] [--out DIR]"""
 import argparse
-import json
 import os
-import subprocess
 import sys
 import time
 
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from benchlib import OBJ_COLS, POD_COLS, Recorder, alternate, pod_values  # noqa: E402
 from kuberay_b200 import abi, synthetic  # noqa: E402
 from kuberay_b200.engine import Engine  # noqa: E402
-
-POD_COLS = [name for name, _dt, _m, dim in abi.COLUMNS if dim == "pods"]
-OBJ_COLS = [name for name, _dt, _m, dim in abi.COLUMNS if dim not in ("pods", "json")]
 KERNELS = ("k_inc_orphan_adopt", "k_inc_clusters_insert", "k_hash_rows", "k_inc_admit", "k_decide2_dirty")
 
 
@@ -34,16 +30,14 @@ def run(full, flags, base, on, pods, epochs, new):
         eng.set_cluster_creates(on)
         eng.set_fixed_layout(True)
         cur = synthetic.first_clusters(full, base, free_pods=pods == "with")
-        views = eng.begin(cur.sizes())
-        eng.fill(views, cur)
-        eng.commit()
+        eng.load(cur)
         eng.reconcile(flags)
         n_inc, kms, wall, prof = 0, [], [], None
         for i in range(epochs):
             k = base + (i + 1) * new
             s = synthetic.first_clusters(full, k, free_pods=pods == "with")   # (prepared outside the timed window)
             rows = np.flatnonzero(np.any([cur.cols[c] != s.cols[c] for c in POD_COLS], axis=0)).astype(np.uint32)
-            vals = np.stack([s.cols[c][rows].view(np.uint32) for c in POD_COLS], axis=1) if rows.size else None
+            vals = pod_values(s, rows) if rows.size else None
             t = time.perf_counter()
             views = eng.begin(s.sizes())
             for c in OBJ_COLS:
@@ -80,27 +74,13 @@ def main():
     ap.add_argument("--new", type=int, default=4)
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
-    q = "name,power.limit,clocks.sm,clocks.max.sm"
-    gpu = subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
-    lines = [{"gpu": gpu, "fields": q}]
-    print(json.dumps(lines[0]), flush=True)
+    out = Recorder("creates_bench", a.out)
     base = synthetic.config("C3").n_clusters
     full, flags = synthetic.generate(synthetic.config("C3", n_clusters=base + a.epochs * a.new))
     flags.fetch_pod_lists = 0
     for pods in ("with", "orphans"):
-        for r in range(a.runs):
-            for on in (False, True):
-                rec = run(full, flags, base, on, pods, a.epochs, a.new)
-                rec["run"] = r
-                lines.append(rec)
-                print(json.dumps(rec), flush=True)
-    gpu = subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
-    lines.append({"gpu_after": gpu})
-    print(json.dumps(lines[-1]), flush=True)
-    if a.out:
-        os.makedirs(a.out, exist_ok=True)
-        with open(os.path.join(a.out, "creates_bench.jsonl"), "w") as f:
-            f.write("\n".join(json.dumps(x) for x in lines) + "\n")
+        alternate(a.runs, lambda r, on: out.record(dict(run(full, flags, base, on, pods, a.epochs, a.new), run=r)))
+    out.finish()
 
 
 if __name__ == "__main__":

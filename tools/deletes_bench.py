@@ -12,19 +12,16 @@ around the commits and kr_reconcile_batch, results copy included), and, option o
 The card's name and power limit are read in the same run.
 Usage: python tools/deletes_bench.py [--epochs 10] [--runs 3] [--k 4] [--out DIR]"""
 import argparse
-import json
 import os
-import subprocess
 import sys
 import time
 
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from benchlib import OBJ_COLS, Recorder, alternate  # noqa: E402
 from kuberay_b200 import abi, synthetic  # noqa: E402
 from kuberay_b200.engine import Engine  # noqa: E402
-
-OBJ_COLS = [name for name, _dt, _m, dim in abi.COLUMNS if dim not in ("pods", "json")]
 KERNELS = ("k_inc_digest_move", "k_inc_clusters_release", "k_inc_orphan_adopt", "k_inc_clusters_translate", "k_inc_clusters_rekey",
            "k_inc_groups_gather", "k_inc_clusters_insert", "k_hash_rows", "k_inc_admit", "k_decide2_dirty")
 
@@ -56,9 +53,7 @@ def run(full, flags, base, on, create, steps):
         eng.set_cluster_creates(on)
         eng.set_fixed_layout(True)
         cur = synthetic.select_clusters(full, np.arange(base))
-        views = eng.begin(cur.sizes())
-        eng.fill(views, cur)
-        eng.commit()
+        eng.load(cur)
         eng.reconcile(flags)
         n_inc, kms, wall, prof = 0, [], [], None
         for i, (order, created) in enumerate(steps):
@@ -98,28 +93,14 @@ def main():
     ap.add_argument("--k", type=int, default=4)
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
-    q = "name,power.limit,clocks.sm,clocks.max.sm"
-    gpu = subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
-    lines = [{"gpu": gpu, "fields": q}]
-    print(json.dumps(lines[0]), flush=True)
+    out = Recorder("deletes_bench", a.out)
     base = synthetic.config("C3").n_clusters
     full, flags = synthetic.generate(synthetic.config("C3", n_clusters=base + a.epochs * a.k))
     flags.fetch_pod_lists = 0
     for create in (False, True):
         steps = plan(full, base, a.epochs, a.k, create, seed=7)
-        for r in range(a.runs):
-            for on in (False, True):
-                rec = run(full, flags, base, on, create, steps)
-                rec["k_per_epoch"], rec["run"] = a.k, r
-                lines.append(rec)
-                print(json.dumps(rec), flush=True)
-    gpu = subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
-    lines.append({"gpu_after": gpu})
-    print(json.dumps(lines[-1]), flush=True)
-    if a.out:
-        os.makedirs(a.out, exist_ok=True)
-        with open(os.path.join(a.out, "deletes_bench.jsonl"), "w") as f:
-            f.write("\n".join(json.dumps(x) for x in lines) + "\n")
+        alternate(a.runs, lambda r, on: out.record(dict(run(full, flags, base, on, create, steps), k_per_epoch=a.k, run=r)))
+    out.finish()
 
 
 if __name__ == "__main__":

@@ -11,20 +11,17 @@ around the commits and kr_reconcile_batch, results copy included), median H2D an
 list of the last epoch, profiled.  The card's name and power limit are read in the same run.
 Usage: python tools/group_edits_bench.py [--epochs 10] [--runs 3] [--k 4] [--out DIR]"""
 import argparse
-import json
 import os
-import subprocess
 import sys
 import time
 
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from benchlib import OBJ_COLS, Recorder, alternate  # noqa: E402
 from kuberay_b200 import abi, synthetic  # noqa: E402
 from kuberay_b200.engine import Engine  # noqa: E402
 from kuberay_b200.snapshot import Snapshot  # noqa: E402
-
-OBJ_COLS = [name for name, _dt, _m, dim in abi.COLUMNS if dim not in ("pods", "json")]
 
 
 def respec(snap, rows):
@@ -76,9 +73,7 @@ def run(base, flags, room, on, steps):
     try:
         eng.set_group_edits(on)
         eng.set_fixed_layout(True)
-        views = eng.begin(base.sizes())
-        eng.fill(views, base)
-        eng.commit()
+        eng.load(base)
         eng.reconcile(flags)
         n_inc, kms, wall, h2d, d2h, prof = 0, [], [], [], [], None
         for i, (s, specs) in enumerate(steps):
@@ -120,10 +115,7 @@ def main():
     ap.add_argument("--k", type=int, default=4)
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
-    q = "name,power.limit,clocks.sm,clocks.max.sm"
-    gpu = subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
-    lines = [{"gpu": gpu, "fields": q}]
-    print(json.dumps(lines[0]), flush=True)
+    out = Recorder("group_edits_bench", a.out)
     base, flags = synthetic.generate(synthetic.config("C3"))
     flags.fetch_pod_lists = 0
     extra = a.epochs * a.k
@@ -131,19 +123,8 @@ def main():
             "json": base.dims["json"] + 16 * extra + int(base.c_json_len.max()) * extra + 4096}
     for variant in ("append", "remove"):
         steps = plan(base, a.epochs, a.k, variant, seed=7)
-        for r in range(a.runs):
-            for on in (False, True):
-                rec = run(base, flags, room, on, steps)
-                rec.update({"variant": variant, "k_per_epoch": a.k, "run": r})
-                lines.append(rec)
-                print(json.dumps(rec), flush=True)
-    gpu = subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
-    lines.append({"gpu_after": gpu})
-    print(json.dumps(lines[-1]), flush=True)
-    if a.out:
-        os.makedirs(a.out, exist_ok=True)
-        with open(os.path.join(a.out, "group_edits_bench.jsonl"), "w") as f:
-            f.write("\n".join(json.dumps(x) for x in lines) + "\n")
+        alternate(a.runs, lambda r, on: out.record(dict(run(base, flags, room, on, steps), variant=variant, k_per_epoch=a.k, run=r)))
+    out.finish()
 
 
 if __name__ == "__main__":

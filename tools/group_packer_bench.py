@@ -11,15 +11,14 @@ kr_group_commit + kr_group_reconcile over a global snapshot of the same objects.
 same run.
 Usage: python tools/group_packer_bench.py [--fleets C5,C3] [--shards 1,2,4] [--epochs 10] [--out DIR]"""
 import argparse
-import json
 import os
-import subprocess
 import sys
 import time
 
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from benchlib import Recorder  # noqa: E402
 from kuberay_b200 import abi, snapshot as snp  # noqa: E402
 from kuberay_b200.engine import Group, lib  # noqa: E402
 from kuberay_b200.packer import GroupPacker  # noqa: E402
@@ -128,22 +127,13 @@ def main():
     ap.add_argument("--epochs", type=int, default=10)
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
-    q = "name,power.limit,clocks.sm,clocks.max.sm"
-    smi = lambda: subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()  # noqa: E731
     ndev = lib().kr_device_count()
-    lines = [{"gpu": smi(), "fields": q, "visible_devices": ndev}]
-    print(json.dumps(lines[0]), flush=True)
+    out = Recorder("group_packer_bench", a.out, visible_devices=ndev)
     rng = np.random.default_rng(1)
     for name in a.fleets.split(","):
         for n in [int(x) for x in a.shards.split(",")]:
-            lines.append(run(name, FLEETS[name], n, [i % ndev for i in range(n)], a.epochs, rng))
-            print(json.dumps(lines[-1]), flush=True)
-    lines.append({"gpu_after": smi()})
-    print(json.dumps(lines[-1]), flush=True)
-    if a.out:
-        os.makedirs(a.out, exist_ok=True)
-        with open(os.path.join(a.out, "group_packer_bench.jsonl"), "w") as f:
-            f.write("\n".join(json.dumps(x) for x in lines) + "\n")
+            out.record(run(name, FLEETS[name], n, [i % ndev for i in range(n)], a.epochs, rng))
+    out.finish()
 
 
 if __name__ == "__main__":

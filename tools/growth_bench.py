@@ -16,29 +16,15 @@ limit are read in the same run.
 Usage: python tools/growth_bench.py [--runs 3] [--out DIR]"""
 import argparse
 import copy
-import json
 import os
-import subprocess
 import sys
-import time
 
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from benchlib import Recorder, alternate, churn_rows, owners, timed_epoch  # noqa: E402
 from kuberay_b200 import abi, synthetic  # noqa: E402
 from kuberay_b200.engine import Engine  # noqa: E402
-
-POD_COLS = [name for name, _dt, _m, dim in abi.COLUMNS if dim == "pods"]
-
-
-def owners(snap):
-    """Pod row -> RayCluster row (-1: none), and each RayCluster's Pod count."""
-    ckey = (snap.c_ns_id.astype(np.uint64) << np.uint64(32)) | snap.c_name_id.astype(np.uint64)
-    order = np.argsort(ckey)
-    pkey = (snap.p_ns_id.astype(np.uint64) << np.uint64(32)) | snap.p_cluster_name_id.astype(np.uint64)
-    pos = np.minimum(np.searchsorted(ckey[order], pkey), order.size - 1)
-    own = np.where(ckey[order][pos] == pkey, order[pos], -1)
-    return own, np.bincount(own[own >= 0], minlength=snap.dims["clusters"])
 
 
 class Fleet:
@@ -48,9 +34,7 @@ class Fleet:
         self.snap, self.flags = snap, flags
         self.eng = Engine.for_snapshot(snap, max_creates=4 * snap.dims["pods"], large_clusters=True, large_growth=on)
         self.eng.set_fixed_layout(True)
-        views = self.eng.begin(snap.sizes())
-        self.eng.fill(views, snap)
-        self.eng.commit()
+        self.eng.load(snap)
         self.eng.reconcile(flags)
         self.stride = self.eng.get_option(abi.OPT_BUCKET_STRIDE)
         own, self.count = owners(snap)
@@ -69,24 +53,10 @@ class Fleet:
         return rows
 
     def churn(self):
-        rows = self.rng.choice(self.snap.dims["pods"], self.snap.dims["pods"] // 100, replace=False)
-        self.snap.p_packed[rows] ^= np.uint32(1 << abi.PP_READY_SHIFT)
-        return rows
+        return churn_rows(self.snap, self.rng)
 
     def epoch(self, rows, profiled=False):
-        rows = np.unique(rows).astype(np.uint32)
-        t = time.perf_counter()
-        self.eng.commit_pod_values(rows, np.stack([self.snap.cols[c][rows].view(np.uint32) for c in POD_COLS], axis=1))
-        if profiled:
-            kern = self.eng.reconcile_profiled(self.flags)["kernels"]
-            got = self.eng.fetch()
-        else:
-            got = self.eng.reconcile(self.flags)
-        wall = (time.perf_counter() - t) * 1e3
-        inc = got.changed_clusters is not None
-        if profiled:
-            return inc, kern
-        return {"incremental": inc, "wall_ms": round(wall, 4), "kernel_ms": round(self.eng.last_profile()["kernels_ms"], 4)}
+        return timed_epoch(self.eng, self.snap, rows, self.flags, profiled)
 
 
 def run(base, flags, workload, on, r):
@@ -121,25 +91,12 @@ def main():
     ap.add_argument("--runs", type=int, default=3)
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
-    q = "name,power.limit,clocks.sm,clocks.max.sm"
-    gpu = subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
-    lines = [{"gpu": gpu, "fields": q}]
-    print(json.dumps(lines[0]), flush=True)
+    out = Recorder("growth_bench", a.out)
     for workload in ("C3", "C3L"):
         base, flags = synthetic.generate(synthetic.config(workload))
         flags.fetch_pod_lists = 0
-        for r in range(a.runs):
-            for on in (False, True):
-                rec = run(base, flags, workload, on, r)
-                lines.append(rec)
-                print(json.dumps(rec), flush=True)
-    gpu = subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
-    lines.append({"gpu_after": gpu})
-    print(json.dumps(lines[-1]), flush=True)
-    if a.out:
-        os.makedirs(a.out, exist_ok=True)
-        with open(os.path.join(a.out, "growth_bench.jsonl"), "w") as f:
-            f.write("\n".join(json.dumps(x) for x in lines) + "\n")
+        alternate(a.runs, lambda r, on: out.record(run(base, flags, workload, on, r)))
+    out.finish()
 
 
 if __name__ == "__main__":

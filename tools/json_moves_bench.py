@@ -14,7 +14,6 @@ Usage: python tools/json_moves_bench.py [--clusters 10000] [--pods 100] [--epoch
 import argparse
 import json
 import os
-import subprocess
 import sys
 import time
 
@@ -22,6 +21,7 @@ import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
 sys.path.insert(0, os.path.dirname(os.path.abspath(__file__)))
+from benchlib import Recorder  # noqa: E402
 from kuberay_b200 import abi  # noqa: E402
 from kuberay_b200.packer import Packer  # noqa: E402
 from spec_rows_bench import cluster, pod  # noqa: E402
@@ -43,10 +43,7 @@ def main():
     ap.add_argument("--events", type=int, default=10_000)
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
-    q = "name,power.limit,clocks.sm,clocks.max.sm"
-    smi = lambda: subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()  # noqa: E731
-    lines = [{"gpu": smi(), "fields": q, "workload": f"{a.clusters} RayClusters x {a.pods} pods through the native packer, compaction epochs"}]
-    print(json.dumps(lines[0]), flush=True)
+    out = Recorder("json_moves_bench", a.out, workload=f"{a.clusters} RayClusters x {a.pods} pods through the native packer, compaction epochs")
     Nc, P = a.clusters, a.pods
     pk = Packer(max_clusters=Nc + 16, max_groups=Nc + 16, max_wtd=64, max_pods=Nc * P + 1024, max_heads=Nc + 16, max_jobs=16,
                 max_creates=max(1 << 16, Nc * P // 4), max_json_bytes=Nc * 4096 * 4 + 2 * HOT * HOT_NOTE, spec_rows=True)
@@ -66,8 +63,7 @@ def main():
         lens = pk.column("c_json_len")
         live = lambda: int(((lens[:Nc].astype(np.int64) + 15) // 16 * 16).sum())  # noqa: E731
         cursor = [live()]  # the packer's arena cursor: every blob it places goes there
-        lines.append({"load_s": round(time.perf_counter() - t, 1), "arena_bytes": cursor[0]})
-        print(json.dumps(lines[-1]), flush=True)
+        out.record({"load_s": round(time.perf_counter() - t, 1), "arena_bytes": cursor[0]})
 
         def edit(c, extra):
             gen[c] += 1
@@ -152,24 +148,17 @@ def main():
         for on in (False, True):
             mode, moves, kern = epoch(on, profile=True)
             r = np.array([x[:6] for x in rec[on]], dtype=np.float64)
-            out = {"json_moves": on, "epochs": a.epochs, "pod_events": a.events, "spec_edits": a.k + 1,
-                   "epoch_ms_median": round(float(np.median(r[:, 0])), 4), "epoch_ms_min": round(float(r[:, 0].min()), 4),
-                   "epoch_ms_max": round(float(r[:, 0].max()), 4), "flush_ms_median": round(float(np.median(r[:, 1])), 4),
-                   "reconcile_ms_median": round(float(np.median(r[:, 2])), 4), "pass_kernels_ms_median": round(float(np.median(r[:, 3])), 4),
-                   "h2d_bytes_median": int(np.median(r[:, 4])), "d2h_bytes_median": int(np.median(r[:, 5])),
-                   "incremental": int(sum(x[7] for x in rec[on])), "n_changed_median": int(np.median([x[6] for x in rec[on]])),
-                   "flush_mode": modes[on], "profiled_flush_mode": mode, "move_kernels_ms": [(n, round(ms, 4)) for n, ms in moves],
-                   "profiled_kernels_ms": [(n, round(ms, 4)) for n, ms in kern]}
-            lines.append(out)
-            print(json.dumps(out), flush=True)
+            out.record({"json_moves": on, "epochs": a.epochs, "pod_events": a.events, "spec_edits": a.k + 1,
+                        "epoch_ms_median": round(float(np.median(r[:, 0])), 4), "epoch_ms_min": round(float(r[:, 0].min()), 4),
+                        "epoch_ms_max": round(float(r[:, 0].max()), 4), "flush_ms_median": round(float(np.median(r[:, 1])), 4),
+                        "reconcile_ms_median": round(float(np.median(r[:, 2])), 4), "pass_kernels_ms_median": round(float(np.median(r[:, 3])), 4),
+                        "h2d_bytes_median": int(np.median(r[:, 4])), "d2h_bytes_median": int(np.median(r[:, 5])),
+                        "incremental": int(sum(x[7] for x in rec[on])), "n_changed_median": int(np.median([x[6] for x in rec[on]])),
+                        "flush_mode": modes[on], "profiled_flush_mode": mode, "move_kernels_ms": [(n, round(ms, 4)) for n, ms in moves],
+                        "profiled_kernels_ms": [(n, round(ms, 4)) for n, ms in kern]})
     finally:
         pk.close()
-    lines.append({"gpu_after": smi()})
-    print(json.dumps(lines[-1]), flush=True)
-    if a.out:
-        os.makedirs(a.out, exist_ok=True)
-        with open(os.path.join(a.out, "json_moves_bench.jsonl"), "w") as f:
-            f.write("\n".join(json.dumps(x) for x in lines) + "\n")
+    out.finish()
 
 
 if __name__ == "__main__":

@@ -14,30 +14,21 @@ around the commits and kr_reconcile_batch, results copy included), median H2D an
 list of the last epoch, profiled.  The card's name, power limit and clocks are read in the same run.
 Usage: python tools/large_moves_bench.py [--epochs 10] [--runs 3] [--out DIR]"""
 import argparse
-import json
 import os
-import subprocess
 import sys
 import time
 
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from benchlib import OBJ_COLS, Recorder, alternate, owners  # noqa: E402
 from kuberay_b200 import abi, synthetic  # noqa: E402
 from kuberay_b200.engine import Engine  # noqa: E402
-
-OBJ_COLS = [name for name, _dt, _m, dim in abi.COLUMNS if dim not in ("pods", "json")]
 
 
 def large_rows(snap):
     """Rows of the RayClusters that list more than 256 Pods."""
-    ckey = (snap.c_ns_id.astype(np.uint64) << np.uint64(32)) | snap.c_name_id.astype(np.uint64)
-    pkey = (snap.p_ns_id.astype(np.uint64) << np.uint64(32)) | snap.p_cluster_name_id.astype(np.uint64)
-    order = np.argsort(ckey)
-    pos = np.minimum(np.searchsorted(ckey[order], pkey), order.size - 1)
-    own = np.where(ckey[order][pos] == pkey, order[pos], -1)
-    cnt = np.bincount(own[own >= 0], minlength=snap.dims["clusters"])
-    return [int(c) for c in np.flatnonzero(cnt > 256)]
+    return [int(c) for c in np.flatnonzero(owners(snap)[1] > 256)]
 
 
 def plan(base, variant, epochs, seed):
@@ -81,9 +72,7 @@ def run(base, flags, steps, on, huge):
             getattr(eng, f"set_{opt}")(True)
         eng.set_large_moves(on)
         eng.set_fixed_layout(True)
-        views = eng.begin(base.sizes())
-        eng.fill(views, base)
-        eng.commit()
+        eng.load(base)
         eng.reconcile(flags)
         eng.reconcile(flags)
         n_inc, kms, wall, h2d, d2h, prof = 0, [], [], [], [], None
@@ -118,28 +107,15 @@ def main():
     ap.add_argument("--runs", type=int, default=3)
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
-    q = "name,power.limit,clocks.sm,clocks.max.sm"
-    gpu = subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
-    lines = [{"gpu": gpu, "fields": q}]
-    print(json.dumps(lines[0]), flush=True)
+    out = Recorder("large_moves_bench", a.out)
     for workload, variants in (("C3L", ("delete large", "move large", "append group")), ("C3H", ("huge",))):
         snap, flags = synthetic.generate(synthetic.config(workload))
         flags.fetch_pod_lists = 0
         for variant in variants:
             base, steps = plan(snap, variant, a.epochs, seed=7)
-            for r in range(a.runs):
-                for on in (False, True):
-                    rec = run(base, flags, steps, on, workload == "C3H")
-                    rec.update({"workload": workload, "variant": variant, "run": r})
-                    lines.append(rec)
-                    print(json.dumps(rec), flush=True)
-    gpu = subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
-    lines.append({"gpu_after": gpu})
-    print(json.dumps(lines[-1]), flush=True)
-    if a.out:
-        os.makedirs(a.out, exist_ok=True)
-        with open(os.path.join(a.out, "large_moves_bench.jsonl"), "w") as f:
-            f.write("\n".join(json.dumps(x) for x in lines) + "\n")
+            alternate(a.runs, lambda r, on: out.record(dict(run(base, flags, steps, on, workload == "C3H"), workload=workload, variant=variant,
+                                                            run=r)))
+    out.finish()
 
 
 if __name__ == "__main__":

@@ -8,19 +8,16 @@ epoch is profiled for the builder's kernels (k_lists_init .. k_lists_gather, dev
 in the same run.
 Usage: python tools/pod_lists_bench.py [--runs 2] [--epochs 30] [--out DIR]"""
 import argparse
-import json
 import os
-import subprocess
 import sys
 import time
 
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from benchlib import Recorder, churn_rows, pod_values  # noqa: E402
 from kuberay_b200 import abi, synthetic  # noqa: E402
 from kuberay_b200.engine import Engine  # noqa: E402
-
-POD_COLS = [name for name, _dt, _m, dim in abi.COLUMNS if dim == "pods"]
 
 
 def run(snap, flags, on, every, epochs, seed):
@@ -34,9 +31,8 @@ def run(snap, flags, on, every, epochs, seed):
         n = snap.dims["pods"]
         ms, d2h, inc = [], [], 0
         for e in range(epochs + 1):
-            rows = np.unique(rng.choice(n, n // 100, replace=False)).astype(np.uint32)
-            snap.cols["p_packed"][rows] ^= np.uint32(1 << abi.PP_READY_SHIFT)
-            vals = np.stack([snap.cols[c][rows].view(np.uint32) for c in POD_COLS], axis=1)
+            rows = churn_rows(snap, rng)
+            vals = pod_values(snap, rows)
             flags.fetch_pod_lists = 1 if e % every == 0 else 0
             t0 = time.perf_counter()
             eng.commit_pod_values(rows, vals)
@@ -52,7 +48,7 @@ def run(snap, flags, on, every, epochs, seed):
         if on:
             rows = np.arange(0, n, 100, dtype=np.uint32)
             snap.cols["p_packed"][rows] ^= np.uint32(1 << abi.PP_READY_SHIFT)
-            eng.commit_pod_values(rows, np.stack([snap.cols[c][rows].view(np.uint32) for c in POD_COLS], axis=1))
+            eng.commit_pod_values(rows, pod_values(snap, rows))
             flags.fetch_pod_lists = 1
             prof = eng.reconcile_profiled(flags)
             names = [k for k, _ in prof["kernels"]]
@@ -70,20 +66,13 @@ def main():
     ap.add_argument("--epochs", type=int, default=30)
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
-    gpu = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit,clocks.max.sm", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
-    lines = [{"gpu": gpu}]
-    print(json.dumps(lines[0]), flush=True)
+    out = Recorder("pod_lists_bench", a.out)
     for r in range(a.runs):
         for every in (1, 3):
             for on in (False, True):
                 snap, flags = synthetic.generate(synthetic.config("C3"))
-                res = dict(run(snap, flags, on, every, a.epochs, 100 + r), run=r)
-                lines.append(res)
-                print(json.dumps(res), flush=True)
-    if a.out:
-        os.makedirs(a.out, exist_ok=True)
-        with open(os.path.join(a.out, "pod_lists_bench.jsonl"), "w") as f:
-            f.writelines(json.dumps(x) + "\n" for x in lines)
+                out.record(dict(run(snap, flags, on, every, a.epochs, 100 + r), run=r))
+    out.finish()
 
 
 if __name__ == "__main__":

@@ -9,16 +9,15 @@ engine's counted H2D / D2H bytes of the epoch, the flush mode, and the kernel li
 card name and power limit are read in the same run.
 Usage: python tools/spec_rows_bench.py [--clusters 10000] [--pods 100] [--epochs 10] [--ks 0,1,10,100,1000] [--out DIR]"""
 import argparse
-import json
 import os
-import subprocess
 import sys
 import time
 
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
-from kuberay_b200 import abi, snapshot as snp  # noqa: E402
+from benchlib import Recorder  # noqa: E402
+from kuberay_b200 import snapshot as snp  # noqa: E402
 from kuberay_b200.packer import Packer  # noqa: E402
 
 
@@ -56,10 +55,7 @@ def main():
     ap.add_argument("--events", type=int, default=10_000)
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
-    q = "name,power.limit,clocks.sm,clocks.max.sm"
-    smi = lambda: subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()  # noqa: E731
-    lines = [{"gpu": smi(), "fields": q, "workload": f"{a.clusters} RayClusters x {a.pods} pods through the native packer"}]
-    print(json.dumps(lines[0]), flush=True)
+    out = Recorder("spec_rows_bench", a.out, workload=f"{a.clusters} RayClusters x {a.pods} pods through the native packer")
     Nc, P = a.clusters, a.pods
     pk = Packer(max_clusters=Nc + 16, max_groups=Nc + 16, max_wtd=64, max_pods=Nc * P + 1024, max_heads=Nc + 16, max_jobs=16,
                 max_creates=max(1 << 16, Nc * P // 4), max_json_bytes=Nc * 4096 * 3)
@@ -76,8 +72,7 @@ def main():
         pk.flush()
         flags = pk.flags(fetch_pod_lists=0)
         pk.engine.reconcile(flags)
-        lines.append({"load_s": round(time.perf_counter() - t, 1)})
-        print(json.dumps(lines[-1]), flush=True)
+        out.record({"load_s": round(time.perf_counter() - t, 1)})
 
         def prepare(k):
             """The epoch's events, handled before the timed window (as the shim's informer handlers do)."""
@@ -117,22 +112,15 @@ def main():
             for on in (False, True):
                 _, kern = epoch(on, k, profiled=True)
                 r = np.array([x[:5] for x in rec[on]], dtype=np.float64)
-                out = {"k": k, "spec_rows": on, "epochs": a.epochs, "pod_events": a.events,
-                       "epoch_ms_median": round(float(np.median(r[:, 0])), 4), "epoch_ms_min": round(float(r[:, 0].min()), 4),
-                       "epoch_ms_max": round(float(r[:, 0].max()), 4), "flush_ms_median": round(float(np.median(r[:, 1])), 4),
-                       "reconcile_ms_median": round(float(np.median(r[:, 2])), 4), "h2d_bytes_median": int(np.median(r[:, 3])),
-                       "d2h_bytes_median": int(np.median(r[:, 4])), "incremental": int(sum(x[5] for x in rec[on])),
-                       "flush_mode": modes[on], "profiled_kernels_ms": [(n, round(ms, 4)) for n, ms in kern]}
-                lines.append(out)
-                print(json.dumps(out), flush=True)
+                out.record({"k": k, "spec_rows": on, "epochs": a.epochs, "pod_events": a.events,
+                            "epoch_ms_median": round(float(np.median(r[:, 0])), 4), "epoch_ms_min": round(float(r[:, 0].min()), 4),
+                            "epoch_ms_max": round(float(r[:, 0].max()), 4), "flush_ms_median": round(float(np.median(r[:, 1])), 4),
+                            "reconcile_ms_median": round(float(np.median(r[:, 2])), 4), "h2d_bytes_median": int(np.median(r[:, 3])),
+                            "d2h_bytes_median": int(np.median(r[:, 4])), "incremental": int(sum(x[5] for x in rec[on])),
+                            "flush_mode": modes[on], "profiled_kernels_ms": [(n, round(ms, 4)) for n, ms in kern]})
     finally:
         pk.close()
-    lines.append({"gpu_after": smi()})
-    print(json.dumps(lines[-1]), flush=True)
-    if a.out:
-        os.makedirs(a.out, exist_ok=True)
-        with open(os.path.join(a.out, "spec_rows_bench.jsonl"), "w") as f:
-            f.write("\n".join(json.dumps(x) for x in lines) + "\n")
+    out.finish()
 
 
 if __name__ == "__main__":

@@ -8,21 +8,18 @@ commit, the pod commit and kr_reconcile_batch, results copy included), and, opti
 edit epoch.
 Usage: python tools/wtd_bench.py [--epochs 20] [--runs 3] [--out DIR]"""
 import argparse
-import json
 import os
-import subprocess
 import sys
 import time
 
 import numpy as np
 
 sys.path.insert(0, os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
+from benchlib import OBJ_COLS, POD_COLS, Recorder, alternate, pod_values  # noqa: E402
 from kuberay_b200 import abi, synthetic  # noqa: E402
 from kuberay_b200.engine import Engine  # noqa: E402
 from kuberay_b200.snapshot import Snapshot  # noqa: E402
 
-POD_COLS = [name for name, _dt, _m, dim in abi.COLUMNS if dim == "pods"]
-OBJ_COLS = [name for name, _dt, _m, dim in abi.COLUMNS if dim not in ("pods", "json")]
 NEW_KERNELS = ("k_inc_wtd_release", "k_inc_wtd_clear", "k_inc_wtd_insert", "k_inc_wtd_resolve")
 
 
@@ -98,9 +95,7 @@ def run(name, wtd, epochs, seed):
     try:
         eng.set_wtd_edits(wtd)
         eng.set_fixed_layout(True)
-        views = eng.begin(snap.sizes())
-        eng.fill(views, snap)
-        eng.commit()
+        views = eng.load(snap)
         eng.reconcile(flags)
         n_inc, kms, wall, prof, n_wtd = 0, [], [], None, []
         cur = snap
@@ -113,7 +108,7 @@ def run(name, wtd, epochs, seed):
             for c in OBJ_COLS:
                 np.copyto(views[c], s.cols[c])
             eng.commit(abi.PART_OBJECTS)
-            eng.commit_pod_values(rows, np.stack([s.cols[c][rows].view(np.uint32) for c in POD_COLS], axis=1))
+            eng.commit_pod_values(rows, pod_values(s, rows))
             if wtd and i == epochs - 1:   # the last epoch profiled: the new kernels alone
                 prof = dict(eng.reconcile_profiled(flags)["kernels"])
                 got = eng.fetch()
@@ -140,24 +135,10 @@ def main():
     ap.add_argument("--workloads", default="C5,C3")
     ap.add_argument("--out", default=None)
     a = ap.parse_args()
-    q = "name,power.limit,clocks.sm,clocks.max.sm"
-    gpu = subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
-    lines = [{"gpu": gpu, "fields": q}]
-    print(json.dumps(lines[0]), flush=True)
+    out = Recorder("wtd_bench", a.out)
     for name in a.workloads.split(","):
-        for r in range(a.runs):
-            for wtd in (False, True):
-                rec = run(name, wtd, a.epochs, seed=r + 1)
-                rec["run"] = r
-                lines.append(rec)
-                print(json.dumps(rec), flush=True)
-    gpu = subprocess.run(["nvidia-smi", f"--query-gpu={q}", "--format=csv,noheader"], capture_output=True, text=True).stdout.strip()
-    lines.append({"gpu_after": gpu})
-    print(json.dumps(lines[-1]), flush=True)
-    if a.out:
-        os.makedirs(a.out, exist_ok=True)
-        with open(os.path.join(a.out, "wtd_bench.jsonl"), "w") as f:
-            f.write("\n".join(json.dumps(x) for x in lines) + "\n")
+        alternate(a.runs, lambda r, wtd: out.record(dict(run(name, wtd, a.epochs, seed=r + 1), run=r)))
+    out.finish()
 
 
 if __name__ == "__main__":
